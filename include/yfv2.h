@@ -56,7 +56,8 @@ YFV2_API const char* yfv2_last_error(void);
 /* ---- plan -----------------------------------------------------------------------------------------
  * One plan per (device, N, H, W, A, C, training).  H and W must be multiples of 32
  * (model/backbone/shufflenetv2.py strides; utils/loss.py:78).  Replaces Detector.__init__'s shape
- * bookkeeping (model/detector.py:8-19). */
+ * bookkeeping (model/detector.py:8-19).  A <= 8, C <= 256 (else YFV2_EINVAL); A + C <= 192, i.e. up to 189 classes at 3
+ * anchors (the heads' output convolution runs as one or two 96-column tiles; larger: YFV2_EUNSUPPORTED). */
 YFV2_API int yfv2_plan_create(yfv2_plan** plan, int device, int N, int H, int W, int A, int C, int training);
 YFV2_API int yfv2_plan_destroy(yfv2_plan* plan);
 YFV2_API int yfv2_plan_workspace_bytes(const yfv2_plan* plan, size_t* bytes);

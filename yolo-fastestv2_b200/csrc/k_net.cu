@@ -348,31 +348,38 @@ fpn_kernel(const __grid_constant__ FpnArgs p) {
 struct HeadArgs {
     Planes in[2], out[2];          // branch 0 = cls head, 1 = reg head (flat planes, zero frame of 2)
     const float* dw[2];            // DW5 packs
-    const float* pw[2];            // half 0: PW pack 72 -> 72; half 1: folded [96][72] matrix | bias[96]
+    const float* pw[2];            // half 0: PW pack 72 -> 72; half 1: folded [NPt][72] matrix | bias[NPt], NPt = 96 or 192
     float* dst[2][2];              // half 1: branch 0 -> obj rows [0, A), cls rows [A, A + C); branch 1 -> reg rows [0, 4A)
     int split[2], rowsA[2], rowsB[2];
     int N, H, W, chunks;
 };
 
+constexpr int kHeadTile = 96;      // output columns of one contraction of the second head half (12 n-tiles of 8)
+
 // half 0: dw5x5 + BN + ReLU -> pw + BN -> flat planes.  half 1: dw5x5 + BN + ReLU -> folded matrix + bias -> head tensors.
+// HALF 2 (head2_kernel) is half 1 for A + C > 96: the cls branch contracts the same A fragments, kept in registers, against two
+// 96-column tiles of a [192][72] folded matrix; the reg branch (4A <= 32 columns) keeps one tile.  It contracts 48 columns at a
+// time, so that the A fragments (36 registers) and one pass of accumulators (24) leave room for two CTAs per SM.
 template <int HALF>
-__global__ void __launch_bounds__(kThreads)
-head_kernel(const __grid_constant__ HeadArgs p) {
+__device__ __forceinline__ void head_body(const HeadArgs& p) {
     pdl_trigger();
-    constexpr int NP = HALF ? 96 : 72, NT = NP / 8, S = w_stride(NP);
+    constexpr int NP = HALF == 0 ? 72 : HALF == 1 ? kHeadTile : 2 * kHeadTile;   // weight columns in shared memory
+    constexpr int NT = HALF == 0 ? 9 : HALF == 1 ? kHeadTile / 8 : kHeadTile / 16, S = w_stride(NP);   // n-tiles of one pass
     extern __shared__ __align__(16) float smem[];
     float* sW = smem;
     float* sD = sW + pw_smem_floats(72, NP);      // [72][28]: w[25] | scale | shift | 0
     const int br = blockIdx.y;
+    const int tiles = HALF == 2 && br == 0 ? 2 : 1;
     if (HALF == 0) {
         load_pw(sW, p.pw[br], 72, 72, 72);
     } else {
         const float* F = p.pw[br];
-        for (int i = threadIdx.x; i < 72 * NP; i += kThreads) {
-            const int k = i / NP, nn = i - k * NP;
+        const int NF = HALF == 2 ? kHeadTile * tiles : NP;   // rows of this branch's folded matrix; columns past NF stay unread
+        for (int i = threadIdx.x; i < 72 * NF; i += kThreads) {
+            const int k = i / NF, nn = i - k * NF;
             sW[k * S + nn] = __ldg(F + nn * 72 + k);
         }
-        for (int nn = threadIdx.x; nn < NP; nn += kThreads) { sW[72 * S + nn] = 1.f; sW[72 * S + NP + nn] = __ldg(F + NP * 72 + nn); }
+        for (int nn = threadIdx.x; nn < NF; nn += kThreads) { sW[72 * S + nn] = 1.f; sW[72 * S + NP + nn] = __ldg(F + NF * 72 + nn); }
     }
     load_floats(sD, p.dw[br], 72 * 28);
     pdl_wait();
@@ -391,8 +398,7 @@ head_kernel(const __grid_constant__ HeadArgs p) {
             off[h] = ok[h] ? in.org + (y - 2) * in.Ws + x - 2 : in.org;
         }
         const float* ib = in.base + (long long)n * in.sN;
-        float acc[NT][4];
-        warp_gemm<9, NT>(acc, sW, S, [&](int ks, float (&a)[4]) {
+        auto load_a = [&](int ks, float (&a)[4]) {
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
                 const int k = 8 * ks + t + 4 * q;
@@ -409,31 +415,59 @@ head_kernel(const __grid_constant__ HeadArgs p) {
                     a[2 * q + h] = ok[h] ? fmaxf(fmaf(v, w[25], w[26]), 0.f) : 0.f;
                 }
             }
-        });
-        const float* sc = sW + 72 * S;
+        };
+        // columns [c0, c0 + 8 NT) of the scaled result -> flat planes (half 0) or head tensors (half 1)
+        auto store = [&](const float (&acc)[NT][4], int c0) {
+            const float* sc = sW + 72 * S;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            if (!ok[h]) continue;
-            const int m = m0 + g + 8 * h;
+            for (int h = 0; h < 2; ++h) {
+                if (!ok[h]) continue;
+                const int m = m0 + g + 8 * h;
 #pragma unroll
-            for (int nt = 0; nt < NT; ++nt)
+                for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int col = 8 * nt + 2 * t + e;
-                    const float v = fmaf(acc[nt][2 * h + e], sc[col], sc[NP + col]);
-                    if (HALF == 0) {
-                        const Planes& o = p.out[br];
-                        const int y = m / p.W, x = m - y * p.W;
-                        o.base[(long long)n * o.sN + (long long)col * o.sC + o.org + y * o.Ws + x] = v;
-                    } else if (col < p.split[br]) {
-                        p.dst[br][0][((long long)n * p.rowsA[br] + col) * HW + m] = v;
-                    } else if (col < p.split[br] + p.rowsB[br]) {
-                        p.dst[br][1][((long long)n * p.rowsB[br] + col - p.split[br]) * HW + m] = v;
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = c0 + 8 * nt + 2 * t + e;
+                        const float v = fmaf(acc[nt][2 * h + e], sc[col], sc[NP + col]);
+                        if (HALF == 0) {
+                            const Planes& o = p.out[br];
+                            const int y = m / p.W, x = m - y * p.W;
+                            o.base[(long long)n * o.sN + (long long)col * o.sC + o.org + y * o.Ws + x] = v;
+                        } else if (col < p.split[br]) {
+                            p.dst[br][0][((long long)n * p.rowsA[br] + col) * HW + m] = v;
+                        } else if (col < p.split[br] + p.rowsB[br]) {
+                            p.dst[br][1][((long long)n * p.rowsB[br] + col - p.split[br]) * HW + m] = v;
+                        }
                     }
-                }
+            }
+        };
+        if constexpr (HALF < 2) {
+            float acc[NT][4];
+            warp_gemm<9, NT>(acc, sW, S, load_a);
+            store(acc, 0);
+        } else {
+            // The dw5x5 stencil (1800 FMAs per pixel) is computed once; each 96-column tile costs 324 MMAs per warp on it.
+            float af[9][4];
+#pragma unroll
+            for (int ks = 0; ks < 9; ++ks) load_a(ks, af[ks]);
+#pragma unroll 1
+            for (int c0 = 0; c0 < kHeadTile * tiles; c0 += 8 * NT) {
+                float acc[NT][4];
+                warp_gemm_regs<9, NT>(acc, sW + c0, S, af);
+                store(acc, c0);
+            }
         }
     }
 }
+
+template <int HALF>
+__global__ void __launch_bounds__(kThreads)
+head_kernel(const __grid_constant__ HeadArgs p) { head_body<HALF>(p); }
+
+// Two CTAs per SM, as half 1 gets on its own: 128 registers with 180 bytes of spill.  Left unbounded, ptxas gives it 144 registers
+// and one CTA per SM, which measured slower on an H100 (150 classes, batch 256 @352x352: heads2.b 430 us against 363-379 us).
+__global__ void __launch_bounds__(kThreads, 2)
+head2_kernel(const __grid_constant__ HeadArgs p) { head_body<2>(p); }
 
 // ---- test hook: out[n][p] = sum_k w[n][k] x[k][p] -------------------------------------------------------------------------
 template <int K, int NP>
@@ -572,8 +606,13 @@ int heads_launch(int half, const Planes& sIn, const Planes& tcls, const Planes& 
         YFV2_LAUNCH_CHECK();
         return YFV2_OK;
     };
-    return half == 0 ? run(head_kernel<0>, 72) : run(head_kernel<1>, 96);
+    if (half == 0) return run(head_kernel<0>, 72);
+    if (A + C <= kHeadTile) return run(head_kernel<1>, kHeadTile);
+    if (A + C <= 2 * kHeadTile && 4 * A <= kHeadTile) return run(head2_kernel, 2 * kHeadTile);
+    set_error("heads: anchors+classes = %d exceeds two %d-column output tiles", A + C, kHeadTile);
+    return YFV2_EUNSUPPORTED;
 }
+static_assert((pw_smem_floats(72, 2 * kHeadTile) + 72 * 28) * sizeof(float) <= kSmemCap, "two head tiles must fit in shared memory");
 
 }  // namespace yfv2
 

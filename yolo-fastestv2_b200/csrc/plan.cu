@@ -58,6 +58,7 @@ constexpr int kStageRepeats[3] = {4, 8, 4};          // shufflenetv2.py:69
 constexpr int kStageWidth[3] = {24, 48, 96};         // branch width = out_channels / 2 (detector.py:11)
 constexpr int kNumBlocks = 16;
 constexpr int kFpnDepth = 72;                        // detector.py:10
+constexpr int kHeadTile = 96;                        // output columns per tile of the heads' second half (k_net.cu)
 
 // ---- pack kernels ---------------------------------------------------------------------------------------
 // w: [Nout][K] row-major conv weight.  Writes Wt[k][n_off+n], scale/shift[n_off+n] with row length Np.
@@ -103,7 +104,7 @@ __global__ void pack_dw_kernel(const float* __restrict__ w, int Cn, int KK, int 
 // Heads, second half (reference fpn.py DWConvblock tail + detector.py:17-19,35-41): pw(72->72), its BN and the shared output
 // conv are consecutive affine maps with no activation between them, so they are ONE matrix at inference time:
 //   F = Wout . diag(sc) . Wpw,   f = Wout . sh + bias          (products accumulated in fp64, rounded once to fp32)
-// rows [n_off, n_off+Mo) of the folded [96 x K] matrix Fw and of the bias Fb.
+// rows [n_off, n_off+Mo) of the folded [NPt x K] matrix Fw (NPt = 96 or 192) and of the bias Fb.
 __global__ void fold_head_kernel(const float* __restrict__ wout, const float* __restrict__ bout, int Mo, const float* __restrict__ wpw,
                                  const float* gamma, const float* beta, const float* mean, const float* var, int K, int n_off,
                                  float* __restrict__ Fw, float* __restrict__ Fb) {
@@ -169,7 +170,8 @@ struct yfv2_plan {
     ChanTab c2, c3;
     ChanTab logical[kNumBlocks];       // logical channel order of each block's output (debug gather)
     int launches;
-    size_t pk_foldw[4];                // heads' second pointwise + BN + output conv folded into one matrix [96][72] | bias[96]
+    size_t pk_foldw[4];                // heads' second pointwise + BN + output conv folded into one matrix [NPt][72] | bias[NPt]
+    int fold_rows[4];                  // NPt: 96 or 192 output columns (one or two tiles of the head kernel)
     int n_stages;
     struct Stage { int kind, a, b; char name[24]; int group; } stages[64];   // group: first stage of the launch this stage shares
 };
@@ -282,14 +284,18 @@ extern "C" int yfv2_plan_create(yfv2_plan** out, int device, int N, int H, int W
     for (int i = 0; i < 4; ++i) { p->pk_head[i] = pk; pk += align_up(head_pack_floats(), 4); }
     p->pk_out_reg = pk; pk += pw_pack_floats(kFpnDepth, 4 * A);
     p->pk_out_oc = pk; pk += pw_pack_floats(kFpnDepth, A + C);
-    for (int i = 0; i < 4; ++i) { p->pk_foldw[i] = pk; pk += align_up(96 * 72 + 96, 4); }
-    p->pk_floats = pk;
-
-    if (A + C > 96 || 4 * A > 96) {
-        set_error("plan_create: anchors+classes = %d exceeds the 96-wide output-conv tile of this build", A + C);
+    if (A + C > 2 * kHeadTile || 4 * A > kHeadTile) {
+        set_error("plan_create: anchors+classes = %d exceeds the two 96-wide output-conv tiles of this build (at most 192)", A + C);
         delete p;
         return YFV2_EUNSUPPORTED;
     }
+    for (int i = 0; i < 4; ++i) {      // i: 0 cls2, 1 reg2, 2 cls3, 3 reg3
+        const int cols = i & 1 ? 4 * A : A + C;
+        p->fold_rows[i] = cols <= kHeadTile ? kHeadTile : 2 * kHeadTile;
+        p->pk_foldw[i] = pk; pk += align_up((size_t)p->fold_rows[i] * kFpnDepth + p->fold_rows[i], 4);
+    }
+    p->pk_floats = pk;
+
     auto add = [&](int kind, int a, int b, const char* fmt, int x, int y) {
         yfv2_plan::Stage& st = p->stages[p->n_stages++];
         st.kind = kind; st.a = a; st.b = b;
@@ -438,7 +444,7 @@ extern "C" int yfv2_pack_weights(yfv2_plan* p, const float* const* params, const
     for (int h = 0; h < 4; ++h) {
         const Pw2& q = pw2[h];
         float* Fw = pk + p->pk_foldw[h];
-        float* Fb = Fw + 96 * kFpnDepth;
+        float* Fb = Fw + (size_t)p->fold_rows[h] * kFpnDepth;
         const int K = kFpnDepth;
         auto fold = [&](int which, int Mo, int n_off) -> int {
             if (!wo[which] || !bo[which]) { set_error("pack_weights: null output-layer tensor"); return YFV2_EINVAL; }

@@ -93,5 +93,32 @@ __device__ __forceinline__ void warp_gemm(float (&acc)[NT][4], const float* __re
     }
 }
 
+// The same contraction with the KS A fragments already in registers (a[ks] as load_a would fill it), so that one A operand can
+// be contracted against several column tiles of W.  Fully unrolled: a[] must stay in registers.  Per accumulator the MMAs run in
+// the order warp_gemm issues them, so the result is bit-identical to warp_gemm on the same operands.
+template <int KS, int NT>
+__device__ __forceinline__ void warp_gemm_regs(float (&acc)[NT][4], const float* __restrict__ sW, int S, const float (&a)[KS][4]) {
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks) {
+        uint32_t ah[4], al[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) split_tf32(a[ks][i], ah[i], al[i]);
+        const float* w0 = sW + (8 * ks + t) * S + g;
+        const float* w1 = w0 + 4 * S;
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) {
+            uint32_t bh0, bl0, bh1, bl1;
+            split_tf32(w0[8 * nt], bh0, bl0);
+            split_tf32(w1[8 * nt], bh1, bl1);
+            mma_tf32(acc[nt], al, bh0, bh1);
+            mma_tf32(acc[nt], ah, bl0, bl1);
+            mma_tf32(acc[nt], ah, bh0, bh1);
+        }
+    }
+}
+
 }  // namespace tc
 }  // namespace yfv2
