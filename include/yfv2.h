@@ -147,6 +147,21 @@ YFV2_API int yfv2_batch_statistics(const float* dets, const int* counts, int N, 
 YFV2_API int yfv2_aug_contrast_brightness(const uint8_t* img, uint8_t* out, const float* alpha, const float* beta, int N,
                                           long long bytes_per_image, void* stream);
 
+/* ---- raw frames -> network input: cv2.resize(img, (W, H), interpolation=cv2.INTER_LINEAR) on the device ----------------
+ * The resize the reference runs on the host before every forward (test.py:35; utils/datasets.py:107 for training and
+ * validation), fused with the HWC -> CHW transpose of test.py:36-37.  frames: N HOST descriptors of packed HWC BGR uint8 frames
+ * in device memory (what cv2.imread and video decoders produce); each frame has its own size, so one batch may mix sizes, and
+ * `pitch` (bytes between rows, >= 3*w) lets a crop of a larger frame be passed in place.  dst: device uint8 [N,3,H,W], the input
+ * of yfv2_forward_u8 / yfv2_detect_u8_host.  H, W: any size in 1..32768 (not only multiples of 32).  Bit-identical to OpenCV's
+ * x86 8-bit INTER_LINEAR path (11-bit fixed-point weights; DESIGN.md §7).  The coefficients are computed in the kernel, so there
+ * is no workspace; descriptors are checked before anything is launched. */
+typedef struct yfv2_frame {
+    const uint8_t* data;   /* device pointer to pixel (0,0): B, G, R bytes */
+    int w, h;              /* size in pixels */
+    long long pitch;       /* bytes from one row to the next */
+} yfv2_frame;
+YFV2_API int yfv2_resize_bgr_u8(const yfv2_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
+
 /* ---- whole inference step with HOST buffers (the evaluation() inner loop, utils/utils.py:367-383) ----
  * x_host: pinned uint8 [N,3,H,W]; out_host: pinned [N,max_det,6]; counts_host: pinned [N].
  * Copies in, runs forward_u8 + decode_nms, copies out, all on `stream`; returns without synchronising. */

@@ -1,0 +1,167 @@
+#!/usr/bin/env python
+"""Raw-frame inference: device resize (yfv2_resize_bgr_u8) + forward + fused decode/NMS from 1920x1080 BGR frames resident in HBM.
+
+  python tools/bench_frames.py [--steps K --warmup W --batch 256 --frame 1920x1080 --runs 2]
+
+Same network, weights (Detector default init under seed 1), target size and NMS thresholds as bench.py.  Two frame batches
+(2 x 1.6 GB at batch 256) are alternated so that no step reads its frames from the 50 MB L2.  Prints one JSON line with, per run:
+  step_ms         resize + forward + decode/NMS per batch, CUDA events over K steps;
+  step_ms_noresize the same steps from an already resized uint8 batch (bench.py's timed step), so the resize's share is visible;
+  resize_us       the resize launch alone, L2 flushed before each launch, CUDA events;
+  resize_GBps / resize_frac: the bytes the resize touches over resize_us, against the HBM peak.
+Touched bytes are counted from the coefficients: 32-byte sectors of every source row the kernel reads (the two rows and the two
+columns of each output pixel) plus the planar output written.  `h2d_ms_per_batch` is one pinned host->device copy of a frame
+batch: frames that start on the host are bound by that copy (about 6.2 MB per frame), not by the kernel."""
+import argparse
+import ctypes
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for p in (ROOT, os.path.join(ROOT, "tests")):
+    if p not in sys.path:
+        sys.path.insert(0, p)
+import bench  # noqa: E402
+import torch  # noqa: E402
+
+
+def touched_bytes(h, w, H, W, pitch):
+    """Bytes of DRAM sectors one frame's resize reads (each 32-byte sector once) plus the bytes it writes."""
+    from oracle import resize as ore
+    sx, _, _ = ore.coeffs(w, W, True)
+    sy, _, _ = ore.coeffs(h, H, False)
+    cols = np.unique(np.concatenate([sx, np.minimum(sx + 1, w - 1)]))
+    rows = np.unique(np.clip(np.concatenate([sy, sy + 1]), 0, h - 1))
+    byte = (3 * cols[:, None] + np.arange(3)[None, :]).reshape(-1)
+    sectors = len(np.unique((rows[:, None] * pitch + byte[None, :]) // 32))
+    return 32 * sectors + 3 * H * W
+
+
+def events_ms(fn, n, stream):
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(stream)
+    for _ in range(n):
+        fn()
+    e1.record(stream)
+    e1.synchronize()
+    return e0.elapsed_time(e1)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--frame", default="1920x1080", help="source frame WxH")
+    ap.add_argument("--runs", type=int, default=2, help="measurement runs, alternated within one process")
+    args = ap.parse_args()
+    import yfv2  # noqa: F401
+    import yfv2_engine as eng
+    from oracle import resize as ore
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_frames.py: no CUDA device (the product path has no CPU fallback)")
+    fw, fh = (int(v) for v in args.frame.lower().split("x"))
+    N, S = args.batch, bench.SIDE
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    model, _ = bench.random_state_dict()
+    model = model.to(dev).eval()
+    c = bench.cfg()
+    L = eng.lib()
+    stream = torch.cuda.current_stream(dev)
+    sp = ctypes.c_void_p(stream.cuda_stream)
+
+    g = torch.Generator(device=dev).manual_seed(3)
+    frames = [torch.randint(0, 256, (N, fh, fw, 3), generator=g, dtype=torch.uint8, device=dev) for _ in range(2)]
+    descs = []
+    for fb in frames:
+        d = (eng.Frame * N)()
+        for i in range(N):
+            d[i].data, d[i].w, d[i].h, d[i].pitch = fb[i].data_ptr(), fw, fh, fb[i].stride(0)
+        descs.append(d)
+    x = torch.empty((N, 3, S, S), dtype=torch.uint8, device=dev)
+    plan = model._plan_for(x)
+    preds = plan.alloc_preds()
+    anchors = eng.anchors_array(c)
+    out = torch.empty((N, eng.MAX_DET, 6), dtype=torch.float32, device=dev)
+    counts = torch.empty((N,), dtype=torch.int32, device=dev)
+    it = [0]
+
+    def resize():
+        rc = L.yfv2_resize_bgr_u8(descs[it[0] % 2], N, S, S, ctypes.c_void_p(x.data_ptr()), sp)
+        if rc:
+            raise RuntimeError(L.yfv2_last_error())
+
+    def detect():
+        plan.forward(x, preds)
+        rc = L.yfv2_decode_nms(eng._ptr_array(preds), N, S, S, bench.ANCHORS, bench.CLASSES, anchors, ctypes.c_float(bench.CONF),
+                               ctypes.c_double(bench.IOU), None, 0, eng.MAX_DET, ctypes.c_float(eng.MAX_WH),
+                               ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(counts.data_ptr()), None, None, sp)
+        if rc:
+            raise RuntimeError(L.yfv2_last_error())
+
+    def step():
+        resize()
+        detect()
+        it[0] += 1
+
+    for _ in range(max(args.warmup, 3)):
+        step()
+    torch.cuda.synchronize(dev)
+    # parity of the timed path's resize: first and last frame of the batch the last warm-up step resized, against the oracle
+    last = frames[(it[0] - 1) % 2]
+    for i in (0, N - 1):
+        if not np.array_equal(x[i].cpu().numpy(), ore.resize_bgr_planar(last[i].cpu().numpy(), S, S)):
+            raise AssertionError("bench_frames parity: resized frame %d differs from the oracle" % i)
+
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)     # 256 MB > L2
+    per_frame = touched_bytes(fh, fw, S, S, frames[0][0].stride(0))
+    peak, peak_src = bench.measured_peak()
+    sampler = bench.ClockSampler(0)
+    sampler.start()
+    runs = []
+    for _ in range(args.runs):
+        ms_step = events_ms(step, args.steps, stream)
+        ms_det = events_ms(detect, args.steps, stream)
+        tot, reps = 0.0, max(5, min(args.steps, 20))
+        for _ in range(reps):
+            flush.zero_()
+            it[0] += 1
+            tot += events_ms(resize, 1, stream)
+        us = 1e3 * tot / reps
+        gbs = N * per_frame / (us * 1e-6) / 1e9
+        runs.append({"step_ms": round(ms_step / args.steps, 4), "step_ms_noresize": round(ms_det / args.steps, 4),
+                     "images_per_s": round(N * args.steps / (ms_step * 1e-3), 1), "resize_us": round(us, 2),
+                     "resize_share_of_step": round(us * 1e-3 / (ms_step / args.steps), 4),
+                     "resize_GBps": round(gbs, 1), "resize_frac": round(gbs / peak, 4)})
+    clocks = sampler.stop()
+    del flush
+
+    host = torch.empty((N, fh, fw, 3), dtype=torch.uint8, pin_memory=True)
+    h2d = [events_ms(lambda: frames[0].copy_(host, non_blocking=True), 1, stream) for _ in range(3)]
+    power = None
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        power = pynvml.nvmlDeviceGetPowerManagementLimit(pynvml.nvmlDeviceGetHandleByIndex(0)) / 1000.0
+    except Exception:
+        pass
+    line = {"metric": "images/sec %dx%d frames -> resize + fwd + decode + NMS at %dx%d" % (fw, fh, S, S),
+            "value": runs[-1]["images_per_s"], "unit": "images/s", "steps": args.steps, "batch": N, "runs": runs,
+            "device": torch.cuda.get_device_name(dev), "power_limit_w": power, "clocks": clocks,
+            "resize_touched_bytes_per_frame": per_frame, "resize_touched_bytes_per_batch": N * per_frame,
+            "frame_bytes": fh * fw * 3, "peak_GBps": peak, "peak_source": peak_src,
+            "timing": "CUDA events; frames resident in HBM, two batches alternated; resize_us with L2 flushed before each launch",
+            "h2d_ms_per_batch": round(min(h2d), 3),
+            "h2d_note": "one pinned host->device copy of %d frames (%.1f MB): the bound for frames that start on the host"
+                        % (N, N * fh * fw * 3 / 1e6),
+            "parity": "resized frames 0 and %d equal the oracle (oracle/resize.py) byte for byte" % (N - 1),
+            "kept_boxes_per_step": int(counts.sum().item())}
+    print(json.dumps(line), flush=True)
+
+
+if __name__ == "__main__":
+    main()

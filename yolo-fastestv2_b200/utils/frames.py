@@ -1,0 +1,38 @@
+"""Detection on raw frames: what test.py:34-68 does around the network, for a batch of BGR frames of any sizes.
+
+The reference resizes each frame on the host with cv2.resize (test.py:35), runs the network on the resized batch and scales the
+boxes back to the frame with scale_w = w / cfg["width"], scale_h = h / cfg["height"] (test.py:57-68).  Here the resize runs on
+the device (resize_bgr: yfv2_resize_bgr_u8, bit-identical to cv2's INTER_LINEAR bytes), followed by the uint8 forward and the
+fused decode + NMS; only the scale-back of at most 300 rows per frame stays on the host, in float64 like test.py's Python floats."""
+import torch
+
+from yfv2_engine import resize_bgr  # noqa: F401  (frames -> [N, 3, H, W] uint8 network input)
+from utils.utils import detect
+
+
+def to_source_pixels(rows, size, cfg):
+    """[n, 6] (x1, y1, x2, y2, conf, cls) in network-input pixels -> float64 [n, 6] with the corners in pixels of a frame of size
+    (h, w): x * (w / cfg["width"]), y * (h / cfg["height"]) (test.py:57-68); conf and cls are unchanged."""
+    h, w = size
+    scale_h, scale_w = h / cfg["height"], w / cfg["width"]
+    out = rows.detach().cpu().double().clone()
+    out[:, [0, 2]] *= scale_w
+    out[:, [1, 3]] *= scale_h
+    return out
+
+
+def int_corners(rows):
+    """The integer corners test.py draws, int(x1), int(y1), int(x2), int(y2) (truncation toward zero), of source-pixel rows."""
+    return rows[:, :4].trunc().long()
+
+
+def detect_frames(model, frames, cfg, conf_thres=0.3, iou_thres=0.4):
+    """Raw BGR frames -> detections in each frame's own pixels: a list of float64 CPU [n_i, 6] tensors (x1, y1, x2, y2, conf, cls),
+    descending conf.  model: an eval-mode Detector on a CUDA device; frames: HWC uint8 numpy arrays or CUDA tensors of any sizes;
+    cfg: the load_datafile dict (width, height, anchors)."""
+    frames = list(frames)
+    x = resize_bgr(frames, cfg["width"], cfg["height"], next(model.parameters()).device)
+    with torch.no_grad():
+        preds = model(x)
+    rows = detect(preds, cfg, conf_thres, iou_thres)
+    return [to_source_pixels(r, (f.shape[0], f.shape[1]), cfg) for r, f in zip(rows, frames)]

@@ -22,6 +22,12 @@ MAX_WH = 4096.0        # reference utils/utils.py:241
 _c_float_p = ctypes.POINTER(ctypes.c_float)
 _c_void_pp = ctypes.POINTER(ctypes.c_void_p)
 
+
+class Frame(ctypes.Structure):
+    """yfv2_frame: one packed HWC BGR uint8 source frame in device memory."""
+    _fields_ = [("data", ctypes.c_void_p), ("w", ctypes.c_int), ("h", ctypes.c_int), ("pitch", ctypes.c_longlong)]
+
+
 # name -> (restype, argtypes); must list every prototype of include/yfv2.h (tests check this)
 PROTOTYPES = {
     "yfv2_abi_version": (ctypes.c_int, []),
@@ -53,6 +59,8 @@ PROTOTYPES = {
     "yfv2_batch_statistics": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                              ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]),
     "yfv2_aug_contrast_brightness": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_longlong, ctypes.c_void_p]),
+    "yfv2_resize_bgr_u8": (ctypes.c_int, [ctypes.POINTER(Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                          ctypes.c_void_p]),
     "yfv2_detect_u8_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                            ctypes.POINTER(ctypes.c_double), ctypes.c_float, ctypes.c_double, ctypes.c_int,
                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
@@ -437,6 +445,47 @@ def contrast_and_brightness(imgs, alpha, beta, out=None):
         _check(lib().yfv2_aug_contrast_brightness(ctypes.c_void_p(imgs.data_ptr()), ctypes.c_void_p(out.data_ptr()),
                                                   ctypes.c_void_p(alpha.data_ptr()), ctypes.c_void_p(beta.data_ptr()), N,
                                                   imgs.numel() // N, _stream(imgs.device)), "aug_contrast_brightness")
+    return out
+
+
+def _frame_on_device(f, device):
+    """A packed HWC BGR uint8 frame as a CUDA tensor on `device` whose pixels are 3 bytes apart (rows may be further apart)."""
+    if not isinstance(f, torch.Tensor):
+        import numpy as np
+        f = torch.from_numpy(np.ascontiguousarray(f))
+    if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
+        raise Yfv2Error("resize_bgr: frames must be uint8 [h, w, 3] (BGR, as cv2.imread returns), got %s %s"
+                        % (f.dtype, tuple(f.shape)))
+    f = f.to(device)
+    if f.stride(2) != 1 or f.stride(1) != 3:
+        f = f.contiguous()
+    return f
+
+
+def resize_bgr(frames, W, H, device=None, out=None):
+    """cv2.resize(frame, (W, H), interpolation=cv2.INTER_LINEAR) of every frame, transposed to the [N, 3, H, W] uint8 batch the
+    network takes (test.py:34-37), bit for bit, in one kernel.  frames: HWC uint8 BGR numpy arrays or CUDA tensors, any sizes
+    (host arrays are copied to `device` first; a CUDA tensor that is a row crop of a larger frame is read in place)."""
+    frames = list(frames)
+    if not frames:
+        raise Yfv2Error("resize_bgr: no frames")
+    if device is None:
+        cuda = [f.device for f in frames if isinstance(f, torch.Tensor) and f.is_cuda]
+        device = cuda[0] if cuda else torch.device("cuda", torch.cuda.current_device())
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise Yfv2Error("resize_bgr: runs on CUDA devices only (no CPU fallback)")
+    dev_frames = [_frame_on_device(f, device) for f in frames]
+    descs = (Frame * len(dev_frames))()
+    for d, f in zip(descs, dev_frames):
+        d.data, d.w, d.h, d.pitch = f.data_ptr(), f.shape[1], f.shape[0], f.stride(0)
+    N = len(dev_frames)
+    if out is None:
+        out = torch.empty((N, 3, H, W), dtype=torch.uint8, device=device)
+    elif tuple(out.shape) != (N, 3, H, W) or out.dtype != torch.uint8 or not out.is_contiguous() or out.device != device:
+        raise Yfv2Error("resize_bgr: out must be a contiguous uint8 tensor of shape %s on %s" % ((N, 3, H, W), device))
+    with torch.cuda.device(device):
+        _check(lib().yfv2_resize_bgr_u8(descs, N, H, W, ctypes.c_void_p(out.data_ptr()), _stream(device)), "resize_bgr_u8")
     return out
 
 
