@@ -21,11 +21,11 @@ static int cmp_desc_stable(const void *a, const void *b) {
     return (x->idx > y->idx) - (x->idx < y->idx);   /* ties: lower original index first */
 }
 
-/* x: [M, 5+C] row-major fp32.  out: [max_det,6], src_idx: [max_det].  Returns kept count. */
+/* x: [M, 5+C] row-major fp32.  out: [max_det,6], src_idx: [max_det].  max_wh: the class offset of utils.py:283 (the
+ * reference's value is 4096).  Returns kept count. */
 int oracle_nms_image(const float *x, int M, int C, float conf_thres, double iou_thres,
-                     const int *classes, int n_classes, int max_det, float *out, int *src_idx) {
+                     const int *classes, int n_classes, int max_det, float max_wh, float *out, int *src_idx) {
     const int D = 5 + C;
-    const float max_wh = 4096.0f;
     float *box = (float *)malloc(sizeof(float) * 4 * (size_t)(M > 0 ? M : 1));
     float *obox = (float *)malloc(sizeof(float) * 4 * (size_t)(M > 0 ? M : 1));
     float *area = (float *)malloc(sizeof(float) * (size_t)(M > 0 ? M : 1));
@@ -65,7 +65,7 @@ int oracle_nms_image(const float *x, int M, int C, float conf_thres, double iou_
         ord[i].score = conf[i]; ord[i].idx = i;
     }
     qsort(ord, (size_t)n, sizeof(sitem), cmp_desc_stable);
-    for (int a = 0; a < n && kept < max_det; ++a) {           /* cap: i[:300], utils.py:287-288 */
+    for (int a = 0; a < n && kept < max_det; ++a) {           /* cap: i[:max_det], utils.py:287-288 */
         const int i = ord[a].idx;
         if (dead[i]) continue;
         memcpy(out + 6 * kept, box + 4 * i, 4 * sizeof(float));

@@ -96,12 +96,12 @@ def _load_c():
         lib.oracle_nms_image.restype = ctypes.c_int
         lib.oracle_nms_image.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float,
                                          ctypes.c_double, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
-                                         ctypes.c_void_p, ctypes.c_void_p]
+                                         ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]
         _clib = lib
     return _clib
 
 
-def nms_image_c(x, conf_thres, iou_thres, classes=None, max_det=MAX_DET):
+def nms_image_c(x, conf_thres, iou_thres, classes=None, max_det=MAX_DET, max_wh=MAX_WH):
     """One image through oracle/nms_ref.c.  x: [M,5+C] fp32 numpy.  Returns (rows[n,6], idx[n])."""
     lib = _load_c()
     x = np.ascontiguousarray(x, dtype=np.float32)
@@ -113,16 +113,18 @@ def nms_image_c(x, conf_thres, iou_thres, classes=None, max_det=MAX_DET):
     else:
         cls_arr = np.ascontiguousarray(classes, dtype=np.int32)
         ncls, cls_ptr = cls_arr.size, cls_arr.ctypes.data
-    n = lib.oracle_nms_image(x.ctypes.data, M, D - 5, conf_thres, iou_thres, cls_ptr, ncls, max_det,
+    n = lib.oracle_nms_image(x.ctypes.data, M, D - 5, conf_thres, iou_thres, cls_ptr, ncls, max_det, max_wh,
                              out.ctypes.data, idx.ctypes.data)
     if n < 0:
         raise RuntimeError("oracle_nms_image failed (%d)" % n)
     return out[:n].copy(), idx[:n].copy()
 
 
-def nms(prediction, conf_thres=0.3, iou_thres=0.45, classes=None, return_indices=False, impl="c"):
+def nms(prediction, conf_thres=0.3, iou_thres=0.45, classes=None, return_indices=False, impl="c", max_det=MAX_DET,
+        max_wh=MAX_WH):
     """non_max_suppression (utils/utils.py:232-296): list of [n_i,6] fp32 CPU tensors
-    (x1,y1,x2,y2,conf,cls) sorted by descending conf, at most 300 per image.
+    (x1,y1,x2,y2,conf,cls) sorted by descending conf, at most max_det (the reference: 300) per image.
+    max_wh is the per-class box offset of utils/utils.py:283 (the reference: 4096).
 
     impl="c" uses oracle/nms_ref.c, impl="numpy" the numpy restatement (slow, tests only).
     With return_indices also returns, per image, the row indices into prediction[i]."""
@@ -130,15 +132,15 @@ def nms(prediction, conf_thres=0.3, iou_thres=0.45, classes=None, return_indices
     outs, idxs = [], []
     for x in pred:
         if impl == "c":
-            rows, idx = nms_image_c(x, conf_thres, iou_thres, classes)
+            rows, idx = nms_image_c(x, conf_thres, iou_thres, classes, max_det, max_wh)
         else:
-            rows, idx = _nms_image_numpy(x, conf_thres, iou_thres, classes)
+            rows, idx = _nms_image_numpy(x, conf_thres, iou_thres, classes, max_det, max_wh)
         outs.append(torch.from_numpy(rows).reshape(-1, 6))
         idxs.append(idx.astype(np.int64))
     return (outs, idxs) if return_indices else outs
 
 
-def _nms_image_numpy(x, conf_thres, iou_thres, classes=None):
+def _nms_image_numpy(x, conf_thres, iou_thres, classes=None, max_det=MAX_DET, max_wh=MAX_WH):
     x = np.asarray(x, dtype=np.float32)
     ct = np.float32(conf_thres)                            # torch compares the fp32 tensor with float32(thres)
     src = np.nonzero(x[:, 4] > ct)[0]                      # utils/utils.py:254
@@ -159,7 +161,7 @@ def _nms_image_numpy(x, conf_thres, iou_thres, classes=None):
     if box.shape[0] > MAX_NMS:                             # :278-280
         top = np.argsort(-conf, kind="stable")[:MAX_NMS]
         box, conf, j, src = box[top], conf[top], j[top], src[top]
-    off = (j.astype(np.float32) * np.float32(MAX_WH))[:, None]                # :283
-    keep = greedy_nms_numpy(box + off, conf, iou_thres)[:MAX_DET]             # :285-288
+    off = (j.astype(np.float32) * np.float32(max_wh))[:, None]                # :283
+    keep = greedy_nms_numpy(box + off, conf, iou_thres)[:max_det]             # :285-288
     rows = np.concatenate((box[keep], conf[keep, None], j[keep, None].astype(np.float32)), 1)
     return rows.astype(np.float32), src[keep]

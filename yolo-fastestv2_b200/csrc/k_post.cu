@@ -10,6 +10,7 @@
 // strict '>' filters, box = xy -/+ wh/2, class offset cls*4096 added in fp32, IoU = inter/(a+b-inter)
 // in fp32 compared as double against the threshold, stable descending order (ties by original row),
 // and no FMA contraction anywhere in that arithmetic — every step uses the __f*_rn intrinsics.
+#include <float.h>
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -782,7 +783,9 @@ nms_kernel(const float* __restrict__ dets, int C, NmsParams p) {
 // (32 partial sums of classes l, l+32, l+64, then the xor-butterfly levels 16,8,4,2,1), so the probabilities equal those
 // decode_kernel writes.  Per (cell, anchor) only the winning class needs the division and the product: conf_c =
 // fl(fl(e_c/sum)*obj) is monotone in e_c, so the maximum is attained at the first arg-max of e; classes whose e is within
-// 1e-5 of the maximum are re-checked exactly so the reference's "first index of the maximal product" rule still holds.
+// 1e-5 of the maximum are re-checked exactly so the reference's "first index of the maximal product" rule still holds.  That
+// window assumes a normal product (24 bits): a subnormal conf (tiny objectness, conf_thres = 0) has fewer bits, classes further
+// below the maximum can round to the same product, and then every earlier class is re-checked.
 // ~10x fewer warp instructions than warp-per-cell (the loads are coalesced across the 32 cells of a warp).
 constexpr int kCT = 80;
 
@@ -826,7 +829,8 @@ __device__ __forceinline__ void thread_cell_candidates(const PostGeom& g, const 
             if (obj > p.conf_thres) {
                 conf = __fmul_rn(__fdiv_rn(emax, sum), obj);
                 cls = cstar;
-                const float near = emax * 0.99999f;
+                const bool sub = conf < FLT_MIN;                      // subnormal product: any earlier class may round to it
+                const float near = sub ? 0.f : emax * 0.99999f;
                 int nnear = 0;
 #pragma unroll
                 for (int c = 0; c < kCT; ++c) nnear += (e[c] >= near) ? 1 : 0;
@@ -911,8 +915,9 @@ __device__ __forceinline__ void thread_cell_candidates_80x3(const PostGeom& g, c
             const float obj = sigmoid_rn(ol[a]);
             if (obj > p.conf_thres) {
                 conf[a] = __fmul_rn(__fdiv_rn(emax, sum), obj);
-                if (nnear > 1) {                                      // rare: an earlier class may round to the same product
-                    const float near = emax * 0.99999f;
+                const bool sub = conf[a] < FLT_MIN;                   // subnormal product: any earlier class may round to it
+                if (nnear > 1 || sub) {                               // rare: an earlier class may round to the same product
+                    const float near = sub ? 0.f : emax * 0.99999f;
                     bool found = false;
 #pragma unroll
                     for (int c = 0; c < C; ++c)

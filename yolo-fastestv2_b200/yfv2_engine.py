@@ -375,8 +375,9 @@ def _filter_tensor(classes, device):
     return t, t.numel()
 
 
-def nms(dets, conf_thres=0.3, iou_thres=0.45, classes=None, max_det=MAX_DET, want_idx=True):
-    """Device NMS.  Returns (out [N,max_det,6], counts [N] int32, kept_idx [N,max_det] int32 or None)."""
+def nms(dets, conf_thres=0.3, iou_thres=0.45, classes=None, max_det=MAX_DET, want_idx=True, max_wh=MAX_WH):
+    """Device NMS.  Returns (out [N,max_det,6], counts [N] int32, kept_idx [N,max_det] int32 or None).
+    max_wh: the per-class box offset of utils/utils.py:283."""
     _require_cuda(dets, "dets")
     dets = dets.detach().contiguous().float()
     N, M, D = dets.shape
@@ -386,13 +387,13 @@ def nms(dets, conf_thres=0.3, iou_thres=0.45, classes=None, max_det=MAX_DET, wan
     filt, nf = _filter_tensor(classes, dets.device)
     with torch.cuda.device(dets.device):
         _check(lib().yfv2_nms(ctypes.c_void_p(dets.data_ptr()), N, M, D - 5, ctypes.c_float(conf_thres), ctypes.c_double(iou_thres),
-                              ctypes.c_void_p(filt.data_ptr()) if nf else None, nf, max_det, ctypes.c_float(MAX_WH),
+                              ctypes.c_void_p(filt.data_ptr()) if nf else None, nf, max_det, ctypes.c_float(max_wh),
                               ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(counts.data_ptr()),
                               ctypes.c_void_p(idx.data_ptr()) if want_idx else None, None, _stream(dets.device)), "nms")
     return out, counts, idx
 
 
-def decode_nms(preds, cfg, conf_thres=0.3, iou_thres=0.45, classes=None, max_det=MAX_DET, want_idx=False):
+def decode_nms(preds, cfg, conf_thres=0.3, iou_thres=0.45, classes=None, max_det=MAX_DET, want_idx=False, max_wh=MAX_WH):
     """Fused handel_preds + non_max_suppression on the device (no [N,M,5+C] tensor)."""
     for p in preds:
         _require_cuda(p, "preds")
@@ -408,7 +409,7 @@ def decode_nms(preds, cfg, conf_thres=0.3, iou_thres=0.45, classes=None, max_det
     with torch.cuda.device(dev):
         _check(lib().yfv2_decode_nms(_ptr_array(preds), N, H, W, A, C, anchors_array(cfg), ctypes.c_float(conf_thres),
                                      ctypes.c_double(iou_thres), ctypes.c_void_p(filt.data_ptr()) if nf else None, nf, max_det,
-                                     ctypes.c_float(MAX_WH), ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(counts.data_ptr()),
+                                     ctypes.c_float(max_wh), ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(counts.data_ptr()),
                                      ctypes.c_void_p(idx.data_ptr()) if want_idx else None, None, _stream(dev)), "decode_nms")
     return out, counts, idx
 
