@@ -131,7 +131,7 @@ def test_two_half_mask_resolve_equals_the_sequential_greedy_scan():
 
 
 def test_rolled_sort_direction_depends_on_the_thread_only():
-    """bitonic_sort_desc_reg_rolled takes keep_max from i0 = E*t for every element m of the thread in the stages with j >= E."""
+    """bitonic_sort_desc_reg takes keep_max from i0 = E*t for every element m of the thread in the stages with j >= E."""
     NT = 256
     for E in (1, 2, 4, 8):
         n2 = NT * E

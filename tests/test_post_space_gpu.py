@@ -366,9 +366,6 @@ def test_fused_subnormal_confidences():
 SWITCH_RUNS = {
     "YFV2_NMS_WARP_PER_CELL": "T.run_fused_shapes([(3, 80), (2, 80), (8, 20)]); T.run_fused_ties(); T.run_fused_subnormal(); "
                               "T.run_fused_sort_sizes(T.FUSED_CNTS[6:], warp_cells=True)",
-    "YFV2_NMS_GENERIC_CELLS": "T.run_fused_shapes([(3, 80)]); T.run_fused_ties([(3, 80)]); T.run_fused_subnormal([(3, 80)]); "
-                              "T.run_fused_sort_sizes(T.FUSED_CNTS[:8])",
-    "YFV2_NMS_SORT_UNROLLED": "T.run_nms_sort_sizes([1025, 1500, 2048]); T.run_fused_sort_sizes([T.FUSED_CNTS[5], T.FUSED_CNTS[8]])",
     "YFV2_NMS_LISTS": "assert T.run_caps_and_policy(True, ['m1815', 'm2048', 'm6000_640'], [64, 65, 300, 338]) >= 4; "
                       "T.run_near_midpoint_pairs(caps=(64, 300)); T.run_zone_pairs(); T.run_fused_subnormal([(3, 80), (8, 20)])",
 }

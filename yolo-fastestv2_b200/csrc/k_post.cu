@@ -77,47 +77,72 @@ __device__ __forceinline__ void stage_cells(float* __restrict__ S, const PostGeo
     }
 }
 
-// One warp decodes one staged cell.  Lane l keeps softmax probabilities of classes l, l+32, ...;
-// lanes a < A additionally keep (cx, cy, w, h, obj) of anchor a.  utils/utils.py:331-343.
-struct CellRegs {
-    float p[kCPL];
-    float bx, by, bw, bh, ob;
+// Chunk blockIdx.x of image blockIdx.y, for grids of (chunks of level 0, then chunks of level 1; N): its cells staged into S.
+struct Chunk {
+    int n, lv, cell0, ncell;
 };
-__device__ __forceinline__ void decode_cell(const float* __restrict__ S, const PostGeom& g, int lv, int cell, int cl,
-                                            int lane, CellRegs& r) {
-    const int A = g.A, C = g.C;
-    float l[kCPL];
+__device__ __forceinline__ Chunk stage_chunk(float* __restrict__ S, const PostGeom& g, int chunks0) {
+    Chunk k;
+    k.n = blockIdx.y;
+    k.lv = blockIdx.x < chunks0 ? 0 : 1;
+    k.cell0 = (k.lv ? blockIdx.x - chunks0 : blockIdx.x) * kChunkCells;
+    k.ncell = min(kChunkCells, g.hw[k.lv] - k.cell0);
+    stage_cells(S, g, k.n, k.lv, k.cell0, k.ncell);
+    __syncthreads();
+    return k;
+}
+
+// Box of one (cell, anchor) from its four box logits, utils/utils.py:331-343: xy = (sigmoid*2 - 0.5 + grid) * stride, and
+// (sigmoid*2)**2 in fp32, which the float64 anchor then promotes (utils/utils.py:305-306,337).  Returns (cx, cy, w, h).
+__device__ __forceinline__ float4 decode_box(float lx, float ly, float lw, float lh, int x, int y, float st, double aw, double ah) {
+    const float sx = sigmoid_rn(lx), sy = sigmoid_rn(ly), sw = sigmoid_rn(lw), sh = sigmoid_rn(lh);
+    const float tw = __fmul_rn(sw, 2.0f), th = __fmul_rn(sh, 2.0f);
+    return make_float4(__fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(sx, 2.0f), 0.5f), (float)x), st),
+                       __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(sy, 2.0f), 0.5f), (float)y), st),
+                       (float)__dmul_rn((double)__fmul_rn(tw, tw), aw), (float)__dmul_rn((double)__fmul_rn(th, th), ah));
+}
+
+// Softmax over the C class logits of staged cell cl (utils/utils.py:326, model/detector.py:40); lane l gets classes l, l+32, ...
+// (0 past C).
+__device__ __forceinline__ void warp_softmax(const float* __restrict__ S, int A, int C, int cl, int lane, float (&pr)[kCPL]) {
     float m = -INFINITY;
 #pragma unroll
     for (int j = 0; j < kCPL; ++j) {
         const int c = lane + 32 * j;
-        l[j] = (c < C) ? S[(5 * A + c) * kSStride + cl] : -INFINITY;
-        m = fmaxf(m, l[j]);
+        pr[j] = (c < C) ? S[(5 * A + c) * kSStride + cl] : -INFINITY;
+        m = fmaxf(m, pr[j]);
     }
     m = warp_max(m);
     float sum = 0.f;
 #pragma unroll
     for (int j = 0; j < kCPL; ++j) {
         const int c = lane + 32 * j;
-        l[j] = (c < C) ? expf(__fsub_rn(l[j], m)) : 0.f;
-        sum = __fadd_rn(sum, l[j]);
+        pr[j] = (c < C) ? expf(__fsub_rn(pr[j], m)) : 0.f;
+        sum = __fadd_rn(sum, pr[j]);
     }
     sum = warp_sum(sum);
 #pragma unroll
-    for (int j = 0; j < kCPL; ++j) r.p[j] = __fdiv_rn(l[j], sum);
-    r.bx = r.by = r.bw = r.bh = r.ob = 0.f;
+    for (int j = 0; j < kCPL; ++j) pr[j] = __fdiv_rn(pr[j], sum);
+}
+
+// One warp decodes one staged cell.  Lane l keeps softmax probabilities of classes l, l+32, ...;
+// lanes a < A additionally keep the box (cx, cy, w, h) and objectness of anchor a.
+struct CellRegs {
+    float p[kCPL];
+    float4 box;
+    float ob;
+};
+__device__ __forceinline__ void decode_cell(const float* __restrict__ S, const PostGeom& g, int lv, int cell, int cl,
+                                            int lane, CellRegs& r) {
+    const int A = g.A;
+    warp_softmax(S, A, g.C, cl, lane, r.p);
+    r.box = make_float4(0.f, 0.f, 0.f, 0.f);
+    r.ob = 0.f;
     if (lane < A) {
         const int y = cell / g.w[lv], x = cell - y * g.w[lv];
         const float* s = S + (4 * lane) * kSStride + cl;
-        const float sx = sigmoid_rn(s[0]), sy = sigmoid_rn(s[kSStride]);
-        const float sw = sigmoid_rn(s[2 * kSStride]), sh = sigmoid_rn(s[3 * kSStride]);
-        const float st = g.stride[lv];
-        r.bx = __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(sx, 2.0f), 0.5f), (float)x), st);
-        r.by = __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(sy, 2.0f), 0.5f), (float)y), st);
-        const float tw = __fmul_rn(sw, 2.0f), th = __fmul_rn(sh, 2.0f);
-        // (s*2)**2 in fp32, then the float64 anchor promotes the product (utils/utils.py:305-306,337)
-        r.bw = (float)__dmul_rn((double)__fmul_rn(tw, tw), g.anc[lv][lane][0]);
-        r.bh = (float)__dmul_rn((double)__fmul_rn(th, th), g.anc[lv][lane][1]);
+        r.box = decode_box(s[0], s[kSStride], s[2 * kSStride], s[3 * kSStride], x, y, g.stride[lv], g.anc[lv][lane][0],
+                           g.anc[lv][lane][1]);
         r.ob = sigmoid_rn(S[(4 * A + lane) * kSStride + cl]);
     }
 }
@@ -127,22 +152,17 @@ __device__ __forceinline__ void decode_cell(const float* __restrict__ S, const P
 __global__ void __launch_bounds__(NT)
 decode_kernel(PostGeom g, float* __restrict__ out, int chunks0) {
     __shared__ float S[(5 * kMaxA + 32 * kCPL) * kSStride];
-    const int n = blockIdx.y;
-    const int lv = blockIdx.x < chunks0 ? 0 : 1;
-    const int cell0 = (lv ? blockIdx.x - chunks0 : blockIdx.x) * kChunkCells;
-    const int ncell = min(kChunkCells, g.hw[lv] - cell0);
-    stage_cells(S, g, n, lv, cell0, ncell);
-    __syncthreads();
+    const Chunk k = stage_chunk(S, g, chunks0);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int A = g.A, C = g.C, D = g.D;
-    const long long row_base = (long long)n * g.M + (lv ? (long long)g.hw[0] * A : 0);
-    for (int cl = warp; cl < ncell; cl += NT / 32) {
+    const long long row_base = (long long)k.n * g.M + (k.lv ? (long long)g.hw[0] * A : 0);
+    for (int cl = warp; cl < k.ncell; cl += NT / 32) {
         CellRegs r;
-        decode_cell(S, g, lv, cell0 + cl, cl, lane, r);
-        float* o = out + (row_base + (long long)(cell0 + cl) * A) * D;
+        decode_cell(S, g, k.lv, k.cell0 + cl, cl, lane, r);
+        float* o = out + (row_base + (long long)(k.cell0 + cl) * A) * D;
         if (lane < A) {
             float* b = o + (long long)lane * D;
-            b[0] = r.bx; b[1] = r.by; b[2] = r.bw; b[3] = r.bh; b[4] = r.ob;
+            b[0] = r.box.x; b[1] = r.box.y; b[2] = r.box.z; b[3] = r.box.w; b[4] = r.ob;
         }
         for (int a = 0; a < A; ++a)
 #pragma unroll
@@ -159,39 +179,19 @@ decode_kernel(PostGeom g, float* __restrict__ out, int chunks0) {
 __global__ void __launch_bounds__(NT)
 export_head_kernel(PostGeom g, float* __restrict__ out2, float* __restrict__ out3, int chunks0) {
     __shared__ float S[(5 * kMaxA + 32 * kCPL) * kSStride];
-    const int n = blockIdx.y;
-    const int lv = blockIdx.x < chunks0 ? 0 : 1;
-    const int cell0 = (lv ? blockIdx.x - chunks0 : blockIdx.x) * kChunkCells;
-    const int ncell = min(kChunkCells, g.hw[lv] - cell0);
-    stage_cells(S, g, n, lv, cell0, ncell);
-    __syncthreads();
+    const Chunk k = stage_chunk(S, g, chunks0);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int A = g.A, C = g.C, D = 5 * A + C;
-    float* out = lv ? out3 : out2;
-    for (int cl = warp; cl < ncell; cl += NT / 32) {
-        float* o = out + ((long long)n * g.hw[lv] + cell0 + cl) * D;
+    float* out = k.lv ? out3 : out2;
+    for (int cl = warp; cl < k.ncell; cl += NT / 32) {
+        float* o = out + ((long long)k.n * g.hw[k.lv] + k.cell0 + cl) * D;
         for (int ch = lane; ch < 5 * A; ch += 32) o[ch] = sigmoid_rn(S[ch * kSStride + cl]);
-        float l[kCPL];
-        float m = -INFINITY;
+        float pr[kCPL];
+        warp_softmax(S, A, C, cl, lane, pr);
 #pragma unroll
         for (int j = 0; j < kCPL; ++j) {
             const int c = lane + 32 * j;
-            l[j] = (c < C) ? S[(5 * A + c) * kSStride + cl] : -INFINITY;
-            m = fmaxf(m, l[j]);
-        }
-        m = warp_max(m);
-        float sum = 0.f;
-#pragma unroll
-        for (int j = 0; j < kCPL; ++j) {
-            const int c = lane + 32 * j;
-            l[j] = (c < C) ? expf(__fsub_rn(l[j], m)) : 0.f;
-            sum = __fadd_rn(sum, l[j]);
-        }
-        sum = warp_sum(sum);
-#pragma unroll
-        for (int j = 0; j < kCPL; ++j) {
-            const int c = lane + 32 * j;
-            if (c < C) o[5 * A + c] = __fdiv_rn(l[j], sum);
+            if (c < C) o[5 * A + c] = pr[j];
         }
     }
 }
@@ -203,7 +203,6 @@ struct NmsParams {
     double iou_thres;
     double iou_mid;    // fl32(q) > iou_thres  <=>  q > iou_mid (or >= when iou_tie_up), see iou_gt()
     float iou_mid_f;   // (float)iou_mid: a 1e-6-wide fp32 pre-test decides almost every pair without the fp64 product
-    int sort_rolled;     // 2048-key register sort with rolled stage loops (default; YFV2_NMS_SORT_UNROLLED=1: the unrolled network)
     int list_min_det;    // per-class kept lists only for max_det >= this (YFV2_NMS_LISTS=1: always, for the tests of that path)
     float iou_fast_mid;  // iou_fast(): iou_mid_f, or NaN when iou_mid <= 0 (every pair then takes the exact path)
     float iou_zero;      // iou_fast(): 0 (an empty intersection is below a positive threshold), or NaN when iou_mid <= 0
@@ -238,35 +237,48 @@ struct NmsSmem {
     unsigned short* chcls;      // [2][64] classes of the staged chunks (own storage: the padding tail of `keys` only has room for the lists)
     unsigned int* chist;        // [kNmsListClasses] candidates per class (aliases kbox; only used before the suppression loop)
     bool lists_fit;
-    unsigned int* misc;         // [0]=count, [1..2]=suppressed bits, [3..4]=kept bits, [5]=some box outside (-max_wh/2, max_wh/2), [6] scratch
+    struct Misc {
+        unsigned int count;         // candidates pushed
+        unsigned int dead[2];       // chunk candidates suppressed by a kept box, phase (a)
+        unsigned int kept[2];       // chunk candidates kept, phase (c)
+        unsigned int outside;       // some box outside (-max_wh/2, max_wh/2)
+        unsigned int majority;      // some class holds more than half of the candidates
+        unsigned int unused;
+    }* misc;
 };
 
-__host__ __device__ inline size_t nms_smem_bytes(int M, int MCp, int max_det) {
-    size_t b = (size_t)MCp * 8 + (size_t)M * 16 + (((size_t)M * 2 + 15) & ~(size_t)15);
-    b += (size_t)max_det * 16 + (((size_t)max_det * 4 + 15) & ~(size_t)15);
-    b += 2 * kNmsChunk * 16 + 2 * kNmsChunk * 4 + kNmsChunk * 8 + kNmsChunk + 2 * kNmsChunk * 2 + 32;
-    return b;
+// n elements of T at `at`; the next buffer starts 16-byte aligned
+template <class T>
+__host__ __device__ __forceinline__ T* take(unsigned char*& at, size_t n) {
+    T* r = reinterpret_cast<T*>(at);
+    at += (n * sizeof(T) + 15) & ~(size_t)15;
+    return r;
 }
 
-__device__ __forceinline__ NmsSmem carve(unsigned char* base, int M, int MCp, int max_det) {
-    NmsSmem s;
-    s.keys = reinterpret_cast<unsigned long long*>(base); base += (size_t)MCp * 8;
-    s.cbox = reinterpret_cast<float4*>(base); base += (size_t)M * 16;
-    s.ccls = reinterpret_cast<unsigned short*>(base); base += (((size_t)M * 2 + 15) & ~(size_t)15);
-    s.kbox = reinterpret_cast<float4*>(base); base += (size_t)max_det * 16;
-    s.karea = reinterpret_cast<float*>(base); base += (((size_t)max_det * 4 + 15) & ~(size_t)15);
-    s.chbox = reinterpret_cast<float4*>(base); base += 2 * kNmsChunk * 16;
-    s.charea = reinterpret_cast<float*>(base); base += 2 * kNmsChunk * 4;
-    s.cmask = reinterpret_cast<unsigned int*>(base); base += kNmsChunk * 8;
-    s.alist = reinterpret_cast<unsigned char*>(base); base += kNmsChunk;
-    s.chcls = reinterpret_cast<unsigned short*>(base); base += 2 * kNmsChunk * 2;
-    s.misc = reinterpret_cast<unsigned int*>(base);
+// The shared memory of one NMS CTA, laid out from `base` (16-byte aligned).  Returns the end of the layout.
+__host__ __device__ __forceinline__ unsigned char* nms_layout(NmsSmem& s, unsigned char* base, int M, int MCp, int max_det) {
+    s.keys = take<unsigned long long>(base, MCp);
+    s.cbox = take<float4>(base, M);
+    s.ccls = take<unsigned short>(base, M);
+    s.kbox = take<float4>(base, max_det);
+    s.karea = take<float>(base, max_det);
+    s.chbox = take<float4>(base, 2 * kNmsChunk);
+    s.charea = take<float>(base, 2 * kNmsChunk);
+    s.cmask = take<unsigned int>(base, 2 * kNmsChunk);
+    s.alist = take<unsigned char>(base, kNmsChunk);
+    s.chcls = take<unsigned short>(base, 2 * kNmsChunk);
+    s.misc = take<NmsSmem::Misc>(base, 1);
     unsigned char* tail = reinterpret_cast<unsigned char*>(s.keys + M);
     s.kcn = reinterpret_cast<unsigned int*>(tail); tail += (size_t)max_det * 4;
     s.khead = reinterpret_cast<unsigned short*>(tail); tail += kNmsListClasses * 2;
     s.lists_fit = tail <= reinterpret_cast<unsigned char*>(s.keys + MCp) && (size_t)max_det * 16 >= kNmsListClasses * 4;
     s.chist = reinterpret_cast<unsigned int*>(s.kbox);
-    return s;
+    return base;
+}
+
+inline size_t nms_smem_bytes(int M, int MCp, int max_det) {
+    NmsSmem s;
+    return reinterpret_cast<size_t>(nms_layout(s, nullptr, M, MCp, max_det));
 }
 
 __device__ __forceinline__ unsigned int f2sortable(float f) {
@@ -293,7 +305,7 @@ __device__ __forceinline__ void write_candidate(const NmsSmem& s, unsigned int s
     const float hw = __fmul_rn(w, 0.5f), hh = __fmul_rn(h, 0.5f);
     const float4 bb = make_float4(__fsub_rn(cx, hw), __fsub_rn(cy, hh), __fadd_rn(cx, hw), __fadd_rn(cy, hh));
     const float lim = 0.5f * max_wh;
-    if (!(fabsf(bb.x) < lim && fabsf(bb.y) < lim && fabsf(bb.z) < lim && fabsf(bb.w) < lim)) s.misc[5] = 1u;    // (NaN lands here too)
+    if (!(fabsf(bb.x) < lim && fabsf(bb.y) < lim && fabsf(bb.z) < lim && fabsf(bb.w) < lim)) s.misc->outside = 1u;    // (NaN lands here too)
     s.cbox[slot] = bb;
     s.ccls[slot] = (unsigned short)cls;
     s.keys[slot] = ((unsigned long long)f2sortable(conf) << 32) |
@@ -303,7 +315,7 @@ __device__ __forceinline__ void write_candidate(const NmsSmem& s, unsigned int s
 __device__ __forceinline__ unsigned int alloc_slots(const NmsSmem& s, bool want) {
     const unsigned int bal = __ballot_sync(0xffffffffu, want);
     unsigned int base = 0;
-    if ((threadIdx.x & 31) == 0 && bal) base = atomicAdd(&s.misc[0], (unsigned int)__popc(bal));
+    if ((threadIdx.x & 31) == 0 && bal) base = atomicAdd(&s.misc->count, (unsigned int)__popc(bal));
     base = __shfl_sync(0xffffffffu, base, 0);
     return base + __popc(bal & ((1u << (threadIdx.x & 31)) - 1u));
 }
@@ -372,61 +384,10 @@ __device__ void bitonic_sort_desc(unsigned long long* keys, int n2) {
 // are compare-exchanges inside the thread, strides below 32 E are 64-bit warp shuffles, and only the log2(NT/32) largest
 // strides of the last merges (6 of the 66 steps for 2048 keys) go through shared memory and barriers.  The keys are
 // unique (or equal padding zeros), so every correct sorting network yields the same order as bitonic_sort_desc.
-template <int E>
-__device__ void bitonic_sort_desc_reg(unsigned long long* keys) {
-    constexpr int n2 = NT * E;
-    const int t = threadIdx.x;
-    unsigned long long v[E];
-#pragma unroll
-    for (int m = 0; m < E; ++m) v[m] = keys[E * t + m];
-#pragma unroll
-    for (int k = 2; k <= n2; k <<= 1) {
-#pragma unroll
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            if (j >= E) {
-                unsigned long long o[E];
-                if (j >= 32 * E) {                       // partner thread t ^ (j / E) sits in another warp
-                    __syncthreads();                     // every earlier read of `keys` is done
-#pragma unroll
-                    for (int m = 0; m < E; ++m) keys[m * NT + t] = v[m];          // transposed: conflict-free both ways
-                    __syncthreads();
-#pragma unroll
-                    for (int m = 0; m < E; ++m) o[m] = keys[m * NT + (t ^ (j / E))];
-                } else {
-#pragma unroll
-                    for (int m = 0; m < E; ++m) o[m] = __shfl_xor_sync(0xffffffffu, v[m], j / E);
-                }
-#pragma unroll
-                for (int m = 0; m < E; ++m) {
-                    const int i = E * t + m;
-                    const bool keep_max = ((i & k) == 0) == ((i & j) == 0);      // descending block: the lower index keeps the larger key
-                    const unsigned long long a = v[m], b = o[m];
-                    v[m] = keep_max ? (a > b ? a : b) : (a < b ? a : b);
-                }
-            } else {
-#pragma unroll
-                for (int m = 0; m < E; ++m) {
-                    if ((m & j) == 0) {
-                        const int i = E * t + m;
-                        const unsigned long long a = v[m], b = v[m | j];
-                        const bool desc = (i & k) == 0;
-                        if (desc ? (a < b) : (a > b)) { v[m] = b; v[m | j] = a; }
-                    }
-                }
-            }
-        }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int m = 0; m < E; ++m) keys[E * t + m] = v[m];
-    __syncthreads();
-}
-
-// The same network with the stage loops ROLLED: the fully unrolled version above is ~4000 SASS instructions that every warp runs
-// exactly once -- ncu (profiles/r2s3_kernels_ncu.txt, source page): 58 % of the stall samples inside the sort are instruction fetch.
-// Here k and j are run-time values: strides of 32 E and more go through shared memory, strides of E and more are shuffles with a
-// run-time lane mask, strides below E are compare-exchanges inside the thread (three instantiated bodies for E = 8).  Same
-// comparisons on the same pairs in the same order: identical result.
+// The stage loops are unrolled for E <= 4 and rolled for E = 8: unrolled, the 2048-key network is ~4000 SASS instructions that
+// every warp runs exactly once, and ncu found 58 % of the stall samples inside it on instruction fetch (decode + NMS 178.8 us
+// per launch unrolled, 161.1 rolled, on the bench workload).  Rolled, k and j are run-time values and the strides below E
+// dispatch to three instantiated bodies of sort_intra.
 template <int E, int J>
 __device__ __forceinline__ void sort_intra(unsigned long long (&v)[E], int k, int t) {
 #pragma unroll
@@ -440,15 +401,15 @@ __device__ __forceinline__ void sort_intra(unsigned long long (&v)[E], int k, in
     }
 }
 template <int E>
-__device__ void bitonic_sort_desc_reg_rolled(unsigned long long* keys) {
+__device__ void bitonic_sort_desc_reg(unsigned long long* keys) {
     constexpr int n2 = NT * E;
     const int t = threadIdx.x;
     unsigned long long v[E];
 #pragma unroll
     for (int m = 0; m < E; ++m) v[m] = keys[E * t + m];
-#pragma unroll 1
+#pragma unroll (E == 8 ? 1 : 16)
     for (int k = 2; k <= n2; k <<= 1) {
-#pragma unroll 1
+#pragma unroll (E == 8 ? 1 : 16)
         for (int j = k >> 1; j > 0; j >>= 1) {
             if (j >= E) {
                 unsigned long long o[E];
@@ -500,7 +461,7 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
     };
     __syncthreads();
     tick(0);
-    const int cnt = (int)s.misc[0];
+    const int cnt = (int)s.misc->count;
     // classes on disjoint intervals (see write_candidate) and a threshold whose rounding boundary is positive: pairs of different
     // classes have IoU exactly 0 and are skipped on their class ids
     // ... worth it only when the candidates are spread over classes: every kept box then sits in a per-class list (newest first)
@@ -508,23 +469,23 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
     // heads: every candidate has the same arg-max) keeps the dense 4-way unrolled scan.
     // (since the dense scan went branch-free it is the faster one while the kept list is short -- configs[4] sets, cap 300: 2.9 / 2.5 ms
     // per 10 000 images against 3.4 / 2.9 with the lists -- so the lists are only used for caps above kNmsListMinDet)
-    bool by_class = s.lists_fit && s.misc[5] == 0u && p.iou_mid > 0.0 && p.max_wh > 0.f && p.C <= kNmsListClasses && p.max_det >= p.list_min_det;
+    bool by_class = s.lists_fit && s.misc->outside == 0u && p.iou_mid > 0.0 && p.max_wh > 0.f && p.C <= kNmsListClasses &&
+                    p.max_det >= p.list_min_det;
     if (by_class) {
         for (int i = threadIdx.x; i < kNmsListClasses; i += NT) s.chist[i] = 0u;
-        if (threadIdx.x == 0) s.misc[6] = 0u;
+        if (threadIdx.x == 0) s.misc->majority = 0u;
         __syncthreads();
         for (int i = threadIdx.x; i < cnt; i += NT) atomicAdd(&s.chist[s.ccls[i]], 1u);
         __syncthreads();
-        for (int i = threadIdx.x; i < kNmsListClasses; i += NT) if (2u * s.chist[i] > (unsigned)cnt) s.misc[6] = 1u;
+        for (int i = threadIdx.x; i < kNmsListClasses; i += NT) if (2u * s.chist[i] > (unsigned)cnt) s.misc->majority = 1u;
         __syncthreads();
-        by_class = s.misc[6] == 0u;
+        by_class = s.misc->majority == 0u;
     }
     int n2 = 64;
     while (n2 < cnt) n2 <<= 1;
     for (int i = cnt + threadIdx.x; i < n2; i += NT) s.keys[i] = 0ull;
     __syncthreads();
-    if (p.sort_rolled && n2 == 8 * NT) bitonic_sort_desc_reg_rolled<8>(s.keys);
-    else if (n2 == NT) bitonic_sort_desc_reg<1>(s.keys);
+    if (n2 == NT) bitonic_sort_desc_reg<1>(s.keys);
     else if (n2 == 2 * NT) bitonic_sort_desc_reg<2>(s.keys);
     else if (n2 == 4 * NT) bitonic_sort_desc_reg<4>(s.keys);
     else if (n2 == 8 * NT) bitonic_sort_desc_reg<8>(s.keys);
@@ -558,7 +519,7 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
         }
     };
     if (t < kNmsChunk) stage(0, 0, t);
-    if (t == 0) { s.misc[1] = 0u; s.misc[2] = 0u; }
+    if (t == 0) { s.misc->dead[0] = 0u; s.misc->dead[1] = 0u; }
     __syncthreads();
     tick(2);
     for (int c0 = 0, it = 0; c0 < cnt && nk < p.max_det; c0 += kNmsChunk, ++it) {
@@ -577,30 +538,27 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
                 int k = 0;
                 for (unsigned i = s.khead[chcls[j]]; i != 0xFFFFu && !dead; i = s.kcn[i] >> 16, ++k)
                     if ((k & (NT / kNmsChunk - 1)) == q) dead = iou_gt(s.kbox[i], s.karea[i], bj, aj, p);
-                if (dead) atomicOr(&s.misc[1 + (j >> 5)], 1u << (j & 31));
+                if (dead) atomicOr(&s.misc->dead[j >> 5], 1u << (j & 31));
             } else if (j < cn) {
                 const float4 bj = chbox[j];
                 const float aj = charea[j];
-                // four kept boxes per trip: the loads and IoU tests are independent, only the exit test is shared
+                // four kept boxes per trip: the loads and IoU fronts are independent, only the exit test is shared
                 bool dead = false;
                 constexpr int STEP = NT / kNmsChunk;
                 int i = q;
                 for (; i + 3 * STEP < nk && !dead; i += 4 * STEP) {
-                    bool d0, d1, d2, d3, m0, m1, m2, m3;
-                    iou_fast(s.kbox[i], s.karea[i], bj, aj, p, d0, m0);
-                    iou_fast(s.kbox[i + STEP], s.karea[i + STEP], bj, aj, p, d1, m1);
-                    iou_fast(s.kbox[i + 2 * STEP], s.karea[i + 2 * STEP], bj, aj, p, d2, m2);
-                    iou_fast(s.kbox[i + 3 * STEP], s.karea[i + 3 * STEP], bj, aj, p, d3, m3);
-                    if (m0 | m1 | m2 | m3) {                                   // rare: some pair sits in the 1e-6 band / is degenerate
-                        d0 = iou_gt(s.kbox[i], s.karea[i], bj, aj, p);
-                        d1 = iou_gt(s.kbox[i + STEP], s.karea[i + STEP], bj, aj, p);
-                        d2 = iou_gt(s.kbox[i + 2 * STEP], s.karea[i + 2 * STEP], bj, aj, p);
-                        d3 = iou_gt(s.kbox[i + 3 * STEP], s.karea[i + 3 * STEP], bj, aj, p);
+                    bool d[4], m[4];
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) iou_fast(s.kbox[i + u * STEP], s.karea[i + u * STEP], bj, aj, p, d[u], m[u]);
+                    if (m[0] | m[1] | m[2] | m[3]) {                           // rare: some pair sits in the 1e-6 band / is degenerate
+#pragma unroll
+                        for (int u = 0; u < 4; ++u)
+                            d[u] = iou_gt(s.kbox[i + u * STEP], s.karea[i + u * STEP], bj, aj, p);
                     }
-                    dead = d0 | d1 | d2 | d3;
+                    dead = d[0] | d[1] | d[2] | d[3];
                 }
                 for (; i < nk && !dead; i += STEP) dead = iou_gt(s.kbox[i], s.karea[i], bj, aj, p);
-                if (dead) atomicOr(&s.misc[1 + (j >> 5)], 1u << (j & 31));
+                if (dead) atomicOr(&s.misc->dead[j >> 5], 1u << (j & 31));
             }
         }
         __syncthreads();
@@ -608,7 +566,7 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
         // (b) pairs INSIDE the chunk, only among the candidates (a) left alive (typically ~20 of 64 in a crowded class): the live
         // candidates are ranked (alist), thread <-> ordered pair of ranks, one IoU test per thread and round, hits OR-ed into the
         // 64-bit kill row of the earlier candidate.  Threads 64..127 meanwhile stage the next chunk into the other buffer.
-        unsigned long long alive = ~(((unsigned long long)s.misc[2] << 32) | s.misc[1]);
+        unsigned long long alive = ~(((unsigned long long)s.misc->dead[1] << 32) | s.misc->dead[0]);
         if (cn < 64) alive &= (1ull << cn) - 1ull;
         const int na = __popcll(alive);
         if (t < kNmsChunk) {
@@ -618,7 +576,7 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
             stage(c0 + kNmsChunk, (it + 1) & 1, t - kNmsChunk);       // (nothing to do past the end)
         }
         __syncthreads();
-        if (t == 0) { s.misc[1] = 0u; s.misc[2] = 0u; }              // every thread has read the dead bits
+        if (t == 0) { s.misc->dead[0] = 0u; s.misc->dead[1] = 0u; }  // every thread has read the dead bits
         if (na * na <= 4 * NT) {
             for (int pi = t; pi < na * na; pi += NT) {
                 const int rx = pi / na, ry = pi - rx * na;
@@ -675,10 +633,10 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
                 --room;
                 hi &= ~(1u << i) & ~s.cmask[2 * (i + 32) + 1];
             }
-            if (t == 0) { s.misc[3] = klo; s.misc[4] = khi; }
+            if (t == 0) { s.misc->kept[0] = klo; s.misc->kept[1] = khi; }
         }
         __syncthreads();
-        const unsigned long long kept = ((unsigned long long)s.misc[4] << 32) | (unsigned long long)s.misc[3];
+        const unsigned long long kept = ((unsigned long long)s.misc->kept[1] << 32) | (unsigned long long)s.misc->kept[0];
         if (by_class && t == 0) {                                     // per-class lists of kept boxes, in kept order
             int pos = nk;
             for (unsigned long long r = kept; r; r &= r - 1ull, ++pos) {
@@ -718,13 +676,15 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
     }
 }
 
-// NMS from an [N,M,5+C] tensor: one CTA per image, warp per row for the scoring pass.
-__global__ void __launch_bounds__(NT)
+// NMS from an [N,M,5+C] tensor: one CTA per image, warp per row for the scoring pass.  Three CTAs per SM: the scoring pass is
+// bound by the latency of its row loads (see below), and at two (above 85 registers) it is a third slower on the bench_nms sets.
+__global__ void __launch_bounds__(NT, 3)
 nms_kernel(const float* __restrict__ dets, int C, NmsParams p) {
     extern __shared__ __align__(16) unsigned char smraw[];
-    const NmsSmem s = carve(smraw, p.M, p.MCp, p.max_det);
+    NmsSmem s;
+    nms_layout(s, smraw, p.M, p.MCp, p.max_det);
     const int n = blockIdx.x;
-    if (threadIdx.x == 0) { s.misc[0] = 0u; s.misc[5] = 0u; }
+    if (threadIdx.x == 0) { s.misc->count = 0u; s.misc->outside = 0u; }
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int D = 5 + C;
@@ -768,7 +728,7 @@ nms_kernel(const float* __restrict__ dets, int C, NmsParams p) {
             if (!pass[u]) continue;
             warp_argmax(best[u], bi[u]);                               // :267 first max
             if (lane == 0 && best[u] > p.conf_thres && class_ok(p, bi[u])) {    // :268, :271-272
-                const unsigned int slot = atomicAdd(&s.misc[0], 1u);
+                const unsigned int slot = atomicAdd(&s.misc->count, 1u);
                 write_candidate(s, slot, box[u][0], box[u][1], box[u][2], box[u][3], best[u], bi[u], r0 + u * NW, p.max_wh);
             }
         }
@@ -776,19 +736,73 @@ nms_kernel(const float* __restrict__ dets, int C, NmsParams p) {
     sort_and_suppress<false>(s, p, n);
 }
 
-// Fused: candidates come straight from the head logits.
-//
-// Fast path (C <= 80): ONE THREAD PER CELL instead of one warp per cell.  A thread keeps the C exponentials of its cell in
-// registers and reproduces the warp version's arithmetic bit for bit: the same expf arguments and the same summation tree
-// (32 partial sums of classes l, l+32, l+64, then the xor-butterfly levels 16,8,4,2,1), so the probabilities equal those
-// decode_kernel writes.  Per (cell, anchor) only the winning class needs the division and the product: conf_c =
-// fl(fl(e_c/sum)*obj) is monotone in e_c, so the maximum is attained at the first arg-max of e; classes whose e is within
-// 1e-5 of the maximum are re-checked exactly so the reference's "first index of the maximal product" rule still holds.  That
-// window assumes a normal product (24 bits): a subnormal conf (tiny objectness, conf_thres = 0) has fewer bits, classes further
-// below the maximum can round to the same product, and then every earlier class is re-checked.
-// ~10x fewer warp instructions than warp-per-cell (the loads are coalesced across the 32 cells of a warp).
 constexpr int kCT = 80;
 
+// Softmax of one cell, one thread (thread_cell_candidates_80x3): e[kCT] holds the class logits on entry and the exponentials on
+// return.  The expf arguments and the summation tree (32 partial sums of classes l, l+32, l+64, then the
+// xor-butterfly levels 16, 8, 4, 2, 1) are warp_softmax's, so the sum is bit for bit the one decode_kernel divides by.
+struct CellSoftmax {
+    float sum, emax;
+    int cstar;   // first arg-max of e
+    int nnear;   // classes with e >= 0.99999 emax (cstar among them)
+};
+__device__ __forceinline__ CellSoftmax thread_softmax(float (&e)[kCT]) {
+    CellSoftmax r;
+    float m = -INFINITY;
+#pragma unroll
+    for (int c = 0; c < kCT; ++c) m = fmaxf(m, e[c]);
+    r.emax = 0.f;
+    r.cstar = 0;
+#pragma unroll
+    for (int c = 0; c < kCT; ++c) {
+        e[c] = expf(__fsub_rn(e[c], m));
+        if (e[c] > r.emax) { r.emax = e[c]; r.cstar = c; }
+    }
+    float ps[32];
+#pragma unroll
+    for (int l = 0; l < 32; ++l) {
+        float t = e[l];                                           // (0 + e_l) is exact
+        if (l + 32 < kCT) t = __fadd_rn(t, e[l + 32]);
+        if (l + 64 < kCT) t = __fadd_rn(t, e[l + 64]);
+        ps[l] = t;
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1)
+#pragma unroll
+        for (int i = 0; i < o; ++i) ps[i] = __fadd_rn(ps[i], ps[i + o]);
+    r.sum = ps[0];
+    const float near = r.emax * 0.99999f;
+    r.nnear = 0;
+#pragma unroll
+    for (int c = 0; c < kCT; ++c) r.nnear += (e[c] >= near) ? 1 : 0;
+    return r;
+}
+
+// The reference's class for conf = fl(fl(emax/sum)*obj): the first class with the largest product.  conf_c = fl(fl(e_c/sum)*obj)
+// is monotone in e_c, so that is the first arg-max of e unless an earlier class rounds to the same product, which needs e_c
+// within 1e-5 of emax while the product is normal (24 bits).  A subnormal conf (tiny objectness, conf_thres = 0) has fewer
+// bits, classes further below can round to it, and then every earlier class is re-checked.
+__device__ __forceinline__ int first_max_class(const float (&e)[kCT], const CellSoftmax& sm, float obj, float conf) {
+    const bool sub = conf < FLT_MIN;
+    int cls = sm.cstar;
+    if (sm.nnear > 1 || sub) {                                    // rare
+        const float near = sub ? 0.f : sm.emax * 0.99999f;
+        bool found = false;
+#pragma unroll
+        for (int c = 0; c < kCT; ++c)
+            if (!found && c < sm.cstar && e[c] >= near && __fmul_rn(__fdiv_rn(e[c], sm.sum), obj) == conf) { cls = c; found = true; }
+    }
+    return cls;
+}
+
+// Fused: candidates come straight from the head logits.
+//
+// C <= 80: ONE THREAD PER CELL instead of one warp per cell.  A thread keeps the C exponentials of its cell in registers and
+// computes the warp version's probabilities bit for bit (thread_softmax).  Per (cell, anchor) only the winning class needs the
+// division and the product (first_max_class).  ~10x fewer warp instructions than warp-per-cell (the loads are coalesced
+// across the 32 cells of a warp).
+// This generic version writes the same softmax and re-check out inline (with the near-tie count per anchor): built from the two
+// helpers, ptxas spills more of e[] in it (304 instead of 160 bytes of stack on sm_90a, nvcc 12.9).
 __device__ __forceinline__ void thread_cell_candidates(const PostGeom& g, const NmsParams& p, const NmsSmem& s, int n, int lv, int cell,
                                                        bool in_range, int row0) {
     const int A = g.A, C = g.C, hw = g.hw[lv];
@@ -822,7 +836,8 @@ __device__ __forceinline__ void thread_cell_candidates(const PostGeom& g, const 
     const int y = cell / g.w[lv], x = cell - y * g.w[lv];
     for (int a = 0; a < A; ++a) {
         bool want = false;
-        float conf = 0.f, bx = 0.f, by = 0.f, bw = 0.f, bh = 0.f;
+        float conf = 0.f;
+        float4 box = make_float4(0.f, 0.f, 0.f, 0.f);
         int cls = 0;
         if (in_range) {
             const float obj = sigmoid_rn(__ldg(g.obj[lv] + ((long long)n * A + a) * hw + cell));
@@ -843,19 +858,13 @@ __device__ __forceinline__ void thread_cell_candidates(const PostGeom& g, const 
                 if (conf > p.conf_thres && class_ok(p, cls)) {
                     want = true;
                     const float* rp = g.reg[lv] + ((long long)n * 4 * A + 4 * a) * hw + cell;
-                    const float sx = sigmoid_rn(__ldg(rp)), sy = sigmoid_rn(__ldg(rp + hw));
-                    const float sw = sigmoid_rn(__ldg(rp + 2 * (long long)hw)), sh = sigmoid_rn(__ldg(rp + 3 * (long long)hw));
-                    const float st = g.stride[lv];
-                    bx = __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(sx, 2.0f), 0.5f), (float)x), st);
-                    by = __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(sy, 2.0f), 0.5f), (float)y), st);
-                    const float tw = __fmul_rn(sw, 2.0f), th = __fmul_rn(sh, 2.0f);
-                    bw = (float)__dmul_rn((double)__fmul_rn(tw, tw), g.anc[lv][a][0]);
-                    bh = (float)__dmul_rn((double)__fmul_rn(th, th), g.anc[lv][a][1]);
+                    box = decode_box(__ldg(rp), __ldg(rp + hw), __ldg(rp + 2 * (long long)hw), __ldg(rp + 3 * (long long)hw), x, y,
+                                     g.stride[lv], g.anc[lv][a][0], g.anc[lv][a][1]);
                 }
             }
         }
         const unsigned int slot = alloc_slots(s, want);
-        if (want) write_candidate(s, slot, bx, by, bw, bh, conf, cls, row0 + cell * A + a, p.max_wh);
+        if (want) write_candidate(s, slot, box.x, box.y, box.z, box.w, conf, cls, row0 + cell * A + a, p.max_wh);
     }
 }
 
@@ -863,15 +872,14 @@ __device__ __forceinline__ void thread_cell_candidates(const PostGeom& g, const 
 // candidate phase was 26 % of the kernel (59 us of 227 per image) and 5500 issued instructions per thread and pass, 70 % of them
 // predicated 64-bit address arithmetic for `(c < C) ? __ldg(cp + (long long)c * hw)`, with seven dependent global round trips per
 // pass (classes, then objectness and box logits anchor by anchor).  Here the class count is a constant, offsets are 32-bit, the
-// three objectness logits travel with the class logits and the box logits of all wanted anchors in one more batch, and the
-// near-tie count (which only depends on the cell) is taken once.  Same arithmetic, same results bit for bit.
+// three objectness logits travel with the class logits and the box logits of all wanted anchors in one more batch.  Same
+// arithmetic, same results bit for bit.
 __device__ __forceinline__ void thread_cell_candidates_80x3(const PostGeom& g, const NmsParams& p, const NmsSmem& s, int n, int lv, int cell,
                                                             bool in_range, int row0) {
     constexpr int A = 3, C = kCT;
     const int hw = g.hw[lv];
     float e[C];
-    float sum = 1.f, emax = 0.f;
-    int cstar = 0, nnear = 0;
+    CellSoftmax sm = {1.f, 0.f, 0, 0};
     float ol[A] = {0.f, 0.f, 0.f};
     if (in_range) {
         const float* cp = g.cls[lv] + (long long)n * C * hw + cell;
@@ -880,49 +888,19 @@ __device__ __forceinline__ void thread_cell_candidates_80x3(const PostGeom& g, c
         for (int c = 0; c < C; ++c) e[c] = __ldg(cp + c * hw);
 #pragma unroll
         for (int a = 0; a < A; ++a) ol[a] = __ldg(op + a * hw);
-        float m = -INFINITY;
-#pragma unroll
-        for (int c = 0; c < C; ++c) m = fmaxf(m, e[c]);
-#pragma unroll
-        for (int c = 0; c < C; ++c) {
-            e[c] = expf(__fsub_rn(e[c], m));
-            if (e[c] > emax) { emax = e[c]; cstar = c; }             // first arg-max
-        }
-        float ps[32];
-#pragma unroll
-        for (int l = 0; l < 32; ++l) {
-            float t = e[l];                                           // (0 + e_l) is exact
-            if (l + 32 < C) t = __fadd_rn(t, e[l + 32]);
-            if (l + 64 < C) t = __fadd_rn(t, e[l + 64]);
-            ps[l] = t;
-        }
-#pragma unroll
-        for (int o = 16; o; o >>= 1)
-#pragma unroll
-            for (int i = 0; i < o; ++i) ps[i] = __fadd_rn(ps[i], ps[i + o]);
-        sum = ps[0];
-        const float near = emax * 0.99999f;
-#pragma unroll
-        for (int c = 0; c < C; ++c) nnear += (e[c] >= near) ? 1 : 0;
+        sm = thread_softmax(e);
     }
     bool want[A];
     float conf[A];
     int cls[A];
 #pragma unroll
     for (int a = 0; a < A; ++a) {
-        want[a] = false; conf[a] = 0.f; cls[a] = cstar;
+        want[a] = false; conf[a] = 0.f; cls[a] = sm.cstar;
         if (in_range) {
             const float obj = sigmoid_rn(ol[a]);
             if (obj > p.conf_thres) {
-                conf[a] = __fmul_rn(__fdiv_rn(emax, sum), obj);
-                const bool sub = conf[a] < FLT_MIN;                   // subnormal product: any earlier class may round to it
-                if (nnear > 1 || sub) {                               // rare: an earlier class may round to the same product
-                    const float near = sub ? 0.f : emax * 0.99999f;
-                    bool found = false;
-#pragma unroll
-                    for (int c = 0; c < C; ++c)
-                        if (!found && c < cstar && e[c] >= near && __fmul_rn(__fdiv_rn(e[c], sum), obj) == conf[a]) { cls[a] = c; found = true; }
-                }
+                conf[a] = __fmul_rn(__fdiv_rn(sm.emax, sm.sum), obj);
+                cls[a] = first_max_class(e, sm, obj, conf[a]);
                 want[a] = conf[a] > p.conf_thres && class_ok(p, cls[a]);
             }
         }
@@ -936,35 +914,28 @@ __device__ __forceinline__ void thread_cell_candidates_80x3(const PostGeom& g, c
 #pragma unroll
             for (int k = 0; k < 4; ++k) r[a][k] = want[a] ? __ldg(rp + (4 * a + k) * hw) : 0.f;
     }
-    const float st = g.stride[lv];
 #pragma unroll
     for (int a = 0; a < A; ++a) {
-        float bx = 0.f, by = 0.f, bw = 0.f, bh = 0.f;
-        if (want[a]) {
-            const float sx = sigmoid_rn(r[a][0]), sy = sigmoid_rn(r[a][1]), sw = sigmoid_rn(r[a][2]), sh = sigmoid_rn(r[a][3]);
-            bx = __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(sx, 2.0f), 0.5f), (float)x), st);
-            by = __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(sy, 2.0f), 0.5f), (float)y), st);
-            const float tw = __fmul_rn(sw, 2.0f), th = __fmul_rn(sh, 2.0f);
-            bw = (float)__dmul_rn((double)__fmul_rn(tw, tw), g.anc[lv][a][0]);
-            bh = (float)__dmul_rn((double)__fmul_rn(th, th), g.anc[lv][a][1]);
-        }
+        float4 box = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (want[a]) box = decode_box(r[a][0], r[a][1], r[a][2], r[a][3], x, y, g.stride[lv], g.anc[lv][a][0], g.anc[lv][a][1]);
         const unsigned int slot = alloc_slots(s, want[a]);
-        if (want[a]) write_candidate(s, slot, bx, by, bw, bh, conf[a], cls[a], row0 + cell * A + a, p.max_wh);
+        if (want[a]) write_candidate(s, slot, box.x, box.y, box.z, box.w, conf[a], cls[a], row0 + cell * A + a, p.max_wh);
     }
 }
 
 // FAST selects the candidate generation at compile time (one path per kernel: the register allocation and the instruction footprint
-// of one path no longer pay for the others): 2 = thread per cell with 80 classes x 3 anchors static, 1 = thread per cell, generic
-// (C <= 80), 0 = warp per cell (any C).
+// of one path no longer pay for the others): 2 = thread per cell with 80 classes x 3 anchors static, 1 = thread per cell, any
+// other C <= 80, 0 = warp per cell (any C; the path above 80 classes).
 template <bool PROF, int FAST>
 __global__ void __launch_bounds__(NT, 2)
 decode_nms_kernel(PostGeom g, NmsParams p) {
     pdl_wait();
     const long long tstart = PROF ? clock64() : 0ll;
     extern __shared__ __align__(16) unsigned char smraw[];
-    const NmsSmem s = carve(smraw, p.M, p.MCp, p.max_det);
+    NmsSmem s;
+    float* const S = reinterpret_cast<float*>(nms_layout(s, smraw, p.M, p.MCp, p.max_det));   // warp per cell: its staged cells
     const int n = blockIdx.x;
-    if (threadIdx.x == 0) { s.misc[0] = 0u; s.misc[5] = 0u; }
+    if (threadIdx.x == 0) { s.misc->count = 0u; s.misc->outside = 0u; }
     const int A = g.A, C = g.C;
     if (FAST) {
         __syncthreads();
@@ -980,7 +951,6 @@ decode_nms_kernel(PostGeom g, NmsParams p) {
             }
         }
     } else {
-        float* S = reinterpret_cast<float*>(smraw + nms_smem_bytes(p.M, p.MCp, p.max_det));
         const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
         for (int lv = 0; lv < 2; ++lv) {
             const int row0 = lv ? g.hw[0] * A : 0;
@@ -1012,7 +982,8 @@ decode_nms_kernel(PostGeom g, NmsParams p) {
                         if (lane == a && best > p.conf_thres && class_ok(p, bi)) { my_want = true; my_conf = best; my_cls = bi; }
                     }
                     const unsigned int slot = alloc_slots(s, my_want);
-                    if (my_want) write_candidate(s, slot, r.bx, r.by, r.bw, r.bh, my_conf, my_cls, row0 + (cell0 + cl) * A + lane, p.max_wh);
+                    if (my_want)
+                        write_candidate(s, slot, r.box.x, r.box.y, r.box.z, r.box.w, my_conf, my_cls, row0 + (cell0 + cl) * A + lane, p.max_wh);
                 }
             }
         }
@@ -1068,9 +1039,6 @@ int fill_nms(NmsParams& p, int M, float conf_thres, double iou_thres, const int*
     p.prof = nullptr;
     static const bool lists_always = getenv("YFV2_NMS_LISTS") != nullptr;
     p.list_min_det = lists_always ? 0 : kNmsListMinDet;
-    // default since the A/B on the bench workload (profiles/r2s3_ab_nms_sort_*.json): decode+NMS 178.8 -> 161.1 us per launch
-    static const bool sort_unrolled = getenv("YFV2_NMS_SORT_UNROLLED") != nullptr;
-    p.sort_rolled = sort_unrolled ? 0 : 1;
     return YFV2_OK;
 }
 }  // namespace
@@ -1138,12 +1106,12 @@ extern "C" int yfv2_decode_nms(const float* const preds[6], int N, int H, int W,
     if (rc) return rc;
     p.C = C;
     p.prof = g_nms_prof;
-    // 2: thread per cell, 80 classes x 3 anchors all static; 1: thread per cell, generic (C <= 80); 0: warp per cell
-    static const bool warp_cells = getenv("YFV2_NMS_WARP_PER_CELL") != nullptr, generic_cells = getenv("YFV2_NMS_GENERIC_CELLS") != nullptr;
-    const int fast = (C > kCT || warp_cells) ? 0 : (C == kCT && A == 3 && !generic_cells) ? 2 : 1;
-    void (*kern)(PostGeom, NmsParams) =
-        p.prof ? (fast == 2 ? decode_nms_kernel<true, 2> : fast == 1 ? decode_nms_kernel<true, 1> : decode_nms_kernel<true, 0>)
-               : (fast == 2 ? decode_nms_kernel<false, 2> : fast == 1 ? decode_nms_kernel<false, 1> : decode_nms_kernel<false, 0>);
+    static const bool warp_cells = getenv("YFV2_NMS_WARP_PER_CELL") != nullptr;
+    const int fast = (C > kCT || warp_cells) ? 0 : (C == kCT && A == 3) ? 2 : 1;
+    static void (*const kernels[2][3])(PostGeom, NmsParams) = {
+        {decode_nms_kernel<false, 0>, decode_nms_kernel<false, 1>, decode_nms_kernel<false, 2>},
+        {decode_nms_kernel<true, 0>, decode_nms_kernel<true, 1>, decode_nms_kernel<true, 2>}};
+    void (*const kern)(PostGeom, NmsParams) = kernels[p.prof != nullptr][fast];
     // the warp-per-cell path stages 5A+C logits of 32 cells behind the NMS state
     const size_t bytes = nms_smem_bytes(p.M, p.MCp, p.max_det) + (fast ? 0 : (size_t)(5 * A + C) * kSStride * sizeof(float));
     if (bytes > kSmemCap) { set_error("decode_nms: %zu bytes of shared memory needed", bytes); return YFV2_EUNSUPPORTED; }
