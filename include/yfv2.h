@@ -162,6 +162,30 @@ typedef struct yfv2_frame {
 } yfv2_frame;
 YFV2_API int yfv2_resize_bgr_u8(const yfv2_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
 
+/* ---- YUV 4:2:0 frames -> network input: cv2.cvtColor(COLOR_YUV2BGR_*) + cv2.resize INTER_LINEAR on the device ---------------
+ * What a caller with decoded video or camera frames runs on the host before test.py:35-37: cv2.cvtColor(frame,
+ * cv2.COLOR_YUV2BGR_NV12 / _NV21 / _I420 / _YV12) (BT.601 limited range, the only YUV 4:2:0 conversion cv2 has), then the resize
+ * and transpose of yfv2_resize_bgr_u8.  Each source pixel is converted in the kernel, so it reads 1.5 bytes per pixel instead of
+ * 3.  frames: N HOST descriptors of frames in device memory; one batch may mix sizes, pitches and layouts.  Every layout is one
+ * luma plane (w x h bytes, rows y_pitch apart) and chroma of (w/2) x (h/2) samples, sample (i, j) of U at u + i*uv_pitch +
+ * j*uv_step, of V likewise from v:
+ *   NV12: u = the interleaved UV plane, v = u + 1, uv_step 2;   NV21: v = the VU plane, u = v + 1, uv_step 2;
+ *   I420: u, v = the U and V planes, uv_step 1;                 YV12: the same with V stored before U.
+ * Planes need not be adjacent (a decoder surface with padded rows and height is passed as it is).  w and h must be even (cv2
+ * refuses odd sizes too); y_pitch >= w, uv_pitch >= w for uv_step 2 and >= w/2 for uv_step 1.  dst, H, W: as yfv2_resize_bgr_u8.
+ * Bit-identical to cv2.resize(cv2.cvtColor(...)) of OpenCV 4.x on x86 (DESIGN.md §7); descriptors are checked before anything
+ * is launched. */
+typedef struct yfv2_yuv420_frame {
+    const uint8_t* y;      /* device pointer to luma pixel (0,0) */
+    long long y_pitch;     /* bytes from one luma row to the next */
+    const uint8_t* u;      /* device pointer to the U sample of pixel (0,0) */
+    const uint8_t* v;      /* device pointer to the V sample of pixel (0,0) */
+    long long uv_pitch;    /* bytes from one chroma row (two pixel rows) to the next, for U and V alike */
+    int uv_step;           /* bytes from one chroma sample to the next along a row: 2 interleaved (NV12 / NV21), 1 planar */
+    int w, h;              /* size in pixels, both even */
+} yfv2_yuv420_frame;
+YFV2_API int yfv2_resize_yuv420_u8(const yfv2_yuv420_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
+
 /* ---- whole inference step with HOST buffers (the evaluation() inner loop, utils/utils.py:367-383) ----
  * x_host: pinned uint8 [N,3,H,W]; out_host: pinned [N,max_det,6]; counts_host: pinned [N].
  * Copies in, runs forward_u8 + decode_nms, copies out, all on `stream`; returns without synchronising. */

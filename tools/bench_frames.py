@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Raw-frame inference: device resize (yfv2_resize_bgr_u8) + forward + fused decode/NMS from 1920x1080 BGR frames resident in HBM.
 
-  python tools/bench_frames.py [--steps K --warmup W --batch 256 --frame 1920x1080 --runs 2]
+  python tools/bench_frames.py [--steps K --warmup W --batch 256 --frame 1920x1080 --runs 2 --layout bgr|nv12|i420]
 
 Same network, weights (Detector default init under seed 1), target size and NMS thresholds as bench.py.  Two frame batches
 (2 x 1.6 GB at batch 256) are alternated so that no step reads its frames from the 50 MB L2.  Prints one JSON line with, per run:
@@ -11,7 +11,13 @@ Same network, weights (Detector default init under seed 1), target size and NMS 
   resize_GBps / resize_frac: the bytes the resize touches over resize_us, against the HBM peak.
 Touched bytes are counted from the coefficients: 32-byte sectors of every source row the kernel reads (the two rows and the two
 columns of each output pixel) plus the planar output written.  `h2d_ms_per_batch` is one pinned host->device copy of a frame
-batch: frames that start on the host are bound by that copy (about 6.2 MB per frame), not by the kernel."""
+batch: frames that start on the host are bound by that copy (about 6.2 MB per frame), not by the kernel.
+
+--layout nv12 | i420 feeds the steps YUV 4:2:0 frames of the same size (cv2's single [h*3/2, w] buffer) through
+yfv2_resize_yuv420_u8 instead.  Each run then also times the BGR resize of the same frame size (bgr_resize_us), alternated launch
+by launch with the YUV resize, each after an L2 flush; the touched bytes count the sectors of the luma and chroma rows the YUV
+resize reads; `h2d_ms_per_batch` is the pinned copy of a YUV batch (1.5 bytes per pixel) next to `h2d_bgr_ms_per_batch`; and the
+parity check runs tests/yuv_oracle.py on frames 0 and N-1."""
 import argparse
 import ctypes
 import json
@@ -40,6 +46,40 @@ def touched_bytes(h, w, H, W, pitch):
     return 32 * sectors + 3 * H * W
 
 
+def touched_bytes_yuv420(h, w, H, W, layout):
+    """The same count for one YUV 4:2:0 single-buffer frame (rows w bytes apart): the sectors of the luma rows and chroma rows the
+    kernel reads (two rows, two columns and their chroma per output pixel) plus the bytes it writes."""
+    from oracle import resize as ore
+    sx, _, _ = ore.coeffs(w, W, True)
+    sy, _, _ = ore.coeffs(h, H, False)
+    cols = np.unique(np.concatenate([sx, np.minimum(sx + 1, w - 1)]))
+    rows = np.unique(np.clip(np.concatenate([sy, sy + 1]), 0, h - 1))
+    crows, ccols = np.unique(rows >> 1), np.unique(cols >> 1)
+    addr = [(rows[:, None] * w + cols[None, :]).reshape(-1)]
+    if layout == "nv12":
+        addr.append((h * w + crows[:, None] * w + (2 * ccols[:, None] + np.arange(2)[None, :]).reshape(-1)[None, :]).reshape(-1))
+    else:
+        for plane in (h * w, h * w + (h // 2) * (w // 2)):
+            addr.append((plane + crows[:, None] * (w // 2) + ccols[None, :]).reshape(-1))
+    return 32 * len(np.unique(np.concatenate(addr) // 32)) + 3 * H * W
+
+
+def yuv420_descs(fb, layout):
+    """Descriptors of a [N, h*3/2, w] batch of single-buffer NV12 or I420 frames."""
+    import yfv2_engine as eng
+    N, rows, w = fb.shape
+    h = rows // 3 * 2
+    d = (eng.Yuv420Frame * N)()
+    for i in range(N):
+        base = fb[i].data_ptr()
+        d[i].y, d[i].y_pitch, d[i].w, d[i].h = base, w, w, h
+        if layout == "nv12":
+            d[i].u, d[i].v, d[i].uv_pitch, d[i].uv_step = base + h * w, base + h * w + 1, w, 2
+        else:
+            d[i].u, d[i].v, d[i].uv_pitch, d[i].uv_step = base + h * w, base + h * w + (h // 2) * (w // 2), w // 2, 1
+    return d
+
+
 def events_ms(fn, n, stream):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record(stream)
@@ -57,6 +97,7 @@ def main():
     ap.add_argument("--batch", type=int, default=256)
     ap.add_argument("--frame", default="1920x1080", help="source frame WxH")
     ap.add_argument("--runs", type=int, default=2, help="measurement runs, alternated within one process")
+    ap.add_argument("--layout", default="bgr", choices=("bgr", "nv12", "i420"), help="source frame format")
     args = ap.parse_args()
     import yfv2  # noqa: F401
     import yfv2_engine as eng
@@ -82,6 +123,11 @@ def main():
         for i in range(N):
             d[i].data, d[i].w, d[i].h, d[i].pitch = fb[i].data_ptr(), fw, fh, fb[i].stride(0)
         descs.append(d)
+    yuv = args.layout != "bgr"
+    if yuv:
+        import yuv_oracle as yo
+        yframes = [torch.randint(0, 256, (N, fh * 3 // 2, fw), generator=g, dtype=torch.uint8, device=dev) for _ in range(2)]
+        ydescs = [yuv420_descs(fb, args.layout) for fb in yframes]
     x = torch.empty((N, 3, S, S), dtype=torch.uint8, device=dev)
     plan = model._plan_for(x)
     preds = plan.alloc_preds()
@@ -90,10 +136,17 @@ def main():
     counts = torch.empty((N,), dtype=torch.int32, device=dev)
     it = [0]
 
-    def resize():
+    def resize_bgr():
         rc = L.yfv2_resize_bgr_u8(descs[it[0] % 2], N, S, S, ctypes.c_void_p(x.data_ptr()), sp)
         if rc:
             raise RuntimeError(L.yfv2_last_error())
+
+    def resize_yuv():
+        rc = L.yfv2_resize_yuv420_u8(ydescs[it[0] % 2], N, S, S, ctypes.c_void_p(x.data_ptr()), sp)
+        if rc:
+            raise RuntimeError(L.yfv2_last_error())
+
+    resize = resize_yuv if yuv else resize_bgr
 
     def detect():
         plan.forward(x, preds)
@@ -112,13 +165,17 @@ def main():
         step()
     torch.cuda.synchronize(dev)
     # parity of the timed path's resize: first and last frame of the batch the last warm-up step resized, against the oracle
-    last = frames[(it[0] - 1) % 2]
+    last = (yframes if yuv else frames)[(it[0] - 1) % 2]
     for i in (0, N - 1):
-        if not np.array_equal(x[i].cpu().numpy(), ore.resize_bgr_planar(last[i].cpu().numpy(), S, S)):
+        src = last[i].cpu().numpy()
+        want = yo.resize_frame_planar(src, args.layout, S, S) if yuv else ore.resize_bgr_planar(src, S, S)
+        if not np.array_equal(x[i].cpu().numpy(), want):
             raise AssertionError("bench_frames parity: resized frame %d differs from the oracle" % i)
 
     flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)     # 256 MB > L2
     per_frame = touched_bytes(fh, fw, S, S, frames[0][0].stride(0))
+    if yuv:
+        per_frame_bgr, per_frame = per_frame, touched_bytes_yuv420(fh, fw, S, S, args.layout)
     peak, peak_src = bench.measured_peak()
     sampler = bench.ClockSampler(0)
     sampler.start()
@@ -126,22 +183,33 @@ def main():
     for _ in range(args.runs):
         ms_step = events_ms(step, args.steps, stream)
         ms_det = events_ms(detect, args.steps, stream)
-        tot, reps = 0.0, max(5, min(args.steps, 20))
+        tot, tot_bgr, reps = 0.0, 0.0, max(5, min(args.steps, 20))
         for _ in range(reps):
             flush.zero_()
             it[0] += 1
             tot += events_ms(resize, 1, stream)
+            if yuv:                      # the BGR resize of the same frame size, alternated launch by launch
+                flush.zero_()
+                tot_bgr += events_ms(resize_bgr, 1, stream)
         us = 1e3 * tot / reps
         gbs = N * per_frame / (us * 1e-6) / 1e9
         runs.append({"step_ms": round(ms_step / args.steps, 4), "step_ms_noresize": round(ms_det / args.steps, 4),
                      "images_per_s": round(N * args.steps / (ms_step * 1e-3), 1), "resize_us": round(us, 2),
                      "resize_share_of_step": round(us * 1e-3 / (ms_step / args.steps), 4),
                      "resize_GBps": round(gbs, 1), "resize_frac": round(gbs / peak, 4)})
+        if yuv:
+            us_bgr = 1e3 * tot_bgr / reps
+            runs[-1].update({"bgr_resize_us": round(us_bgr, 2),
+                             "bgr_resize_GBps": round(N * per_frame_bgr / (us_bgr * 1e-6) / 1e9, 1)})
     clocks = sampler.stop()
     del flush
 
     host = torch.empty((N, fh, fw, 3), dtype=torch.uint8, pin_memory=True)
     h2d = [events_ms(lambda: frames[0].copy_(host, non_blocking=True), 1, stream) for _ in range(3)]
+    if yuv:
+        del host
+        yhost = torch.empty((N, fh * 3 // 2, fw), dtype=torch.uint8, pin_memory=True)
+        h2d_bgr, h2d = h2d, [events_ms(lambda: yframes[0].copy_(yhost, non_blocking=True), 1, stream) for _ in range(3)]
     power = None
     try:
         import pynvml
@@ -160,6 +228,14 @@ def main():
                         % (N, N * fh * fw * 3 / 1e6),
             "parity": "resized frames 0 and %d equal the oracle (oracle/resize.py) byte for byte" % (N - 1),
             "kept_boxes_per_step": int(counts.sum().item())}
+    if yuv:
+        line["metric"] = "images/sec %dx%d %s frames -> resize + fwd + decode + NMS at %dx%d" % (fw, fh, args.layout.upper(), S, S)
+        line.update({"layout": args.layout, "frame_bytes": fh * fw * 3 // 2, "bgr_frame_bytes": fh * fw * 3,
+                     "bgr_resize_touched_bytes_per_frame": per_frame_bgr, "h2d_bgr_ms_per_batch": round(min(h2d_bgr), 3),
+                     "timing": line["timing"] + "; bgr_resize_us: the BGR resize of the same frame size, alternated with it",
+                     "h2d_note": "one pinned host->device copy of %d %s frames (%.1f MB); h2d_bgr_ms_per_batch: the same frames as BGR "
+                                 "(%.1f MB)" % (N, args.layout.upper(), N * fh * fw * 1.5 / 1e6, N * fh * fw * 3 / 1e6),
+                     "parity": "resized frames 0 and %d equal the oracle (tests/yuv_oracle.py) byte for byte" % (N - 1)})
     print(json.dumps(line), flush=True)
 
 

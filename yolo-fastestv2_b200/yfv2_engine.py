@@ -28,6 +28,12 @@ class Frame(ctypes.Structure):
     _fields_ = [("data", ctypes.c_void_p), ("w", ctypes.c_int), ("h", ctypes.c_int), ("pitch", ctypes.c_longlong)]
 
 
+class Yuv420Frame(ctypes.Structure):
+    """yfv2_yuv420_frame: one YUV 4:2:0 source frame (NV12 / NV21 / I420 / YV12) in device memory."""
+    _fields_ = [("y", ctypes.c_void_p), ("y_pitch", ctypes.c_longlong), ("u", ctypes.c_void_p), ("v", ctypes.c_void_p),
+                ("uv_pitch", ctypes.c_longlong), ("uv_step", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int)]
+
+
 # name -> (restype, argtypes); must list every prototype of include/yfv2.h (tests check this)
 PROTOTYPES = {
     "yfv2_abi_version": (ctypes.c_int, []),
@@ -61,6 +67,8 @@ PROTOTYPES = {
     "yfv2_aug_contrast_brightness": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_longlong, ctypes.c_void_p]),
     "yfv2_resize_bgr_u8": (ctypes.c_int, [ctypes.POINTER(Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                           ctypes.c_void_p]),
+    "yfv2_resize_yuv420_u8": (ctypes.c_int, [ctypes.POINTER(Yuv420Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                             ctypes.c_void_p]),
     "yfv2_detect_u8_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                            ctypes.POINTER(ctypes.c_double), ctypes.c_float, ctypes.c_double, ctypes.c_int,
                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
@@ -487,6 +495,109 @@ def resize_bgr(frames, W, H, device=None, out=None):
         raise Yfv2Error("resize_bgr: out must be a contiguous uint8 tensor of shape %s on %s" % ((N, 3, H, W), device))
     with torch.cuda.device(device):
         _check(lib().yfv2_resize_bgr_u8(descs, N, H, W, ctypes.c_void_p(out.data_ptr()), _stream(device)), "resize_bgr_u8")
+    return out
+
+
+YUV420_LAYOUTS = ("nv12", "nv21", "i420", "yv12")
+
+
+def _uint8_plane(p, what):
+    """p as a uint8 2-D torch tensor; a host numpy array is wrapped, not copied."""
+    if not isinstance(p, torch.Tensor):
+        import numpy as np
+        p = np.asarray(p)
+        if p.dtype != np.uint8 or p.ndim != 2:
+            raise Yfv2Error("resize_yuv420: %s must be a uint8 2-D array, got %s %s" % (what, p.dtype, p.shape))
+        p = torch.from_numpy(p if min(p.strides, default=0) >= 0 else np.ascontiguousarray(p))
+    elif p.dtype != torch.uint8 or p.dim() != 2:
+        raise Yfv2Error("resize_yuv420: %s must be a uint8 2-D tensor, got %s %s" % (what, p.dtype, tuple(p.shape)))
+    return p
+
+
+def _yuv420_planes(f, layout, i):
+    """Frame i as (y, u, v) uint8 2-D planes (u and v are the same [h/2, w] UV or VU plane for NV12 / NV21), checked, not
+    copied.  A single buffer is cv2's [h*3/2, w] layout: the luma rows, then the chroma (interleaved rows for NV12 / NV21; for
+    I420 / YV12 the two w/2-wide planes back to back, read from a contiguous buffer)."""
+    interleaved = layout in ("nv12", "nv21")
+    if isinstance(f, (tuple, list)):
+        planes = [_uint8_plane(p, "frame %d plane %d" % (i, k)) for k, p in enumerate(f)]
+        if len(planes) != (2 if interleaved else 3):
+            raise Yfv2Error("resize_yuv420: frame %d: %s takes %s, got %d planes"
+                            % (i, layout, "(y, uv)" if interleaved else "(y, u, v)", len(planes)))
+        y = planes[0]
+        h, w = y.shape
+        chroma = [(h // 2, w)] if interleaved else [(h // 2, w // 2)] * 2
+        for k, (p, want) in enumerate(zip(planes[1:], chroma)):
+            if tuple(p.shape) != want or h % 2 or w % 2:
+                raise Yfv2Error("resize_yuv420: frame %d: y %s needs even sizes and chroma planes of %s, plane %d is %s"
+                                % (i, tuple(y.shape), want, k + 1, tuple(p.shape)))
+        u, v = (planes[1], planes[1]) if interleaved else (planes[1], planes[2])
+        return y, u, v
+    buf = _uint8_plane(f, "frame %d" % i)
+    rows, w = buf.shape
+    h = rows // 3 * 2
+    if rows % 3 or h <= 0 or w <= 0 or w % 2:
+        raise Yfv2Error("resize_yuv420: frame %d: a single buffer is [h*3/2, w] with h, w even and > 0, got %s"
+                        % (i, tuple(buf.shape)))
+    if interleaved:
+        return buf[:h], buf[h:], buf[h:]
+    buf = buf.contiguous()
+    flat, q = buf.reshape(-1), (h // 2) * (w // 2)
+    first, second = (flat[h * w:h * w + q].view(h // 2, w // 2), flat[h * w + q:h * w + 2 * q].view(h // 2, w // 2))
+    return (buf[:h],) + ((first, second) if layout == "i420" else (second, first))
+
+
+def resize_yuv420(frames, W, H, layout, device=None, out=None):
+    """cv2.resize(cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_<LAYOUT>), (W, H), interpolation=cv2.INTER_LINEAR) of every frame,
+    transposed to the [N, 3, H, W] uint8 batch the network takes, bit for bit, in one kernel (yfv2_resize_yuv420_u8).
+    layout: "nv12" | "nv21" | "i420" | "yv12", or a list of one per frame (one launch may mix layouts).  Each frame is cv2's
+    single uint8 buffer [h*3/2, w], or its planes: (y [h, w], uv [h/2, w]) for NV12 / NV21, (y, u [h/2, w/2], v [h/2, w/2]) for
+    I420 / YV12; numpy arrays or CUDA tensors, any even sizes.  Planes may be views into larger surfaces (rows further apart than
+    w): CUDA views are read in place, host arrays are copied to `device` (1.5 bytes per pixel)."""
+    frames = list(frames)
+    layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
+    for lay in layouts if layouts else [layout]:
+        if lay not in YUV420_LAYOUTS:
+            raise Yfv2Error("resize_yuv420: layout must be one of %s, got %r" % (", ".join(YUV420_LAYOUTS), lay))
+    if not frames:
+        raise Yfv2Error("resize_yuv420: no frames")
+    if len(layouts) != len(frames):
+        raise Yfv2Error("resize_yuv420: %d layouts for %d frames" % (len(layouts), len(frames)))
+    planes = [_yuv420_planes(f, lay, i) for i, (f, lay) in enumerate(zip(frames, layouts))]
+    if device is None:
+        cuda = [p.device for ps in planes for p in ps if p.is_cuda]
+        device = cuda[0] if cuda else torch.device("cuda", torch.cuda.current_device())
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise Yfv2Error("resize_yuv420: runs on CUDA devices only (no CPU fallback)")
+    N = len(frames)
+    if out is None:
+        out = torch.empty((N, 3, H, W), dtype=torch.uint8, device=device)
+    elif tuple(out.shape) != (N, 3, H, W) or out.dtype != torch.uint8 or not out.is_contiguous() or out.device != device:
+        raise Yfv2Error("resize_yuv420: out must be a contiguous uint8 tensor of shape %s on %s" % ((N, 3, H, W), device))
+
+    def on_device(p):
+        p = p.to(device)
+        return p if p.stride(1) == 1 else p.contiguous()
+
+    descs = (Yuv420Frame * N)()
+    keep = []          # device copies stay referenced until the launch is queued: a freed block could take the next frame's copy
+    for d, (y, u, v), lay in zip(descs, planes, layouts):
+        if lay in ("nv12", "nv21"):
+            y, uv = on_device(y), on_device(u)
+            keep += [y, uv]
+            d.u = uv.data_ptr() + (lay == "nv21")
+            d.v = uv.data_ptr() + (lay == "nv12")
+            d.uv_pitch, d.uv_step = uv.stride(0), 2
+        else:
+            y, u, v = on_device(y), on_device(u), on_device(v)
+            if u.stride(0) != v.stride(0):                 # one chroma pitch per descriptor
+                u, v = u.contiguous(), v.contiguous()
+            keep += [y, u, v]
+            d.u, d.v, d.uv_pitch, d.uv_step = u.data_ptr(), v.data_ptr(), u.stride(0), 1
+        d.y, d.y_pitch, d.h, d.w = y.data_ptr(), y.stride(0), y.shape[0], y.shape[1]
+    with torch.cuda.device(device):
+        _check(lib().yfv2_resize_yuv420_u8(descs, N, H, W, ctypes.c_void_p(out.data_ptr()), _stream(device)), "resize_yuv420_u8")
     return out
 
 
