@@ -12,7 +12,8 @@
 //   3. loss_rows_kernel      per matched row: CIoU term and softmax-CE term (+ their gradients, atomics into dpreds)
 //   4. obj_loss_kernel       dense BCE-with-logits over every obj logit (+ gradient), per-block partial sums in fp64
 //   5. finalize_kernel       fixed-order fp64 reductions -> (lbox, lobj, lcls, loss)
-// dtype flow follows the reference: grid coordinates / tbox in fp32, anchor ratio test and the whole CIoU in fp64.
+// dtype flow follows the reference: grid coordinates / tbox in fp32, anchor ratio test and the CIoU in fp64, except the terms of
+// the fp32 target box alone (its corners, area, centre and atan(w/h)), which are fp32 there too.
 #include "common.cuh"
 
 namespace yfv2 {
@@ -125,6 +126,11 @@ __global__ void mark_obj_kernel(LossGeom g, LossWs ws) {
 // ---- 3. matched rows: CIoU + CE ---------------------------------------------------------------------------------------
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// acc += t * d min(a, b)/da  and  acc += t * d max(a, b)/da, with torch.min / torch.max's derivative: a tie gives each argument
+// half (loss.py:23,33).  Off ties the arithmetic is that of a plain `if (a < b) acc += t`.
+__device__ __forceinline__ void add_dmin(double& acc, double a, double b, double t) { if (a < b) acc += t; else if (a == b) acc += 0.5 * t; }
+__device__ __forceinline__ void add_dmax(double& acc, double a, double b, double t) { if (a > b) acc += t; else if (a == b) acc += 0.5 * t; }
+
 __global__ void __launch_bounds__(kLossThreads)
 loss_rows_kernel(LossGeom g, LossWs ws) {
     const int lv = blockIdx.y;
@@ -143,20 +149,26 @@ loss_rows_kernel(LossGeom g, LossWs ws) {
         const double aw = R.anch[2 * r], ah = R.anch[2 * r + 1];
         const float tw2 = sw * 2.0f, th2 = sh * 2.0f;
         const double pw = (double)(tw2 * tw2) * aw, ph = (double)(th2 * th2) * ah;                // loss.py:160
-        const double tx = R.tbox[4 * r], ty = R.tbox[4 * r + 1], tw = R.tbox[4 * r + 2], th = R.tbox[4 * r + 3];
         const double b1x1 = px - pw / 2, b1x2 = px + pw / 2, b1y1 = py - ph / 2, b1y2 = py + ph / 2;
-        const double b2x1 = tx - tw / 2, b2x2 = tx + tw / 2, b2y1 = ty - th / 2, b2y2 = ty + th / 2;
+        // tbox is fp32 in the reference, so what it computes from the target box alone is fp32 and promoted where it meets the
+        // fp64 predicted box: the corners, w2 * h2, the centre sums and atan(w2 / h2) (loss.py:19-20,28-29,42,46).  An fp64 atan
+        // would make D exactly 0 for a prediction with the target's aspect, and 0/0 in alpha where the prediction IS the target.
+        const float tx = R.tbox[4 * r], ty = R.tbox[4 * r + 1], tw = R.tbox[4 * r + 2], th = R.tbox[4 * r + 3];
+        const float b2x1f = __fsub_rn(tx, __fmul_rn(tw, 0.5f)), b2x2f = __fadd_rn(tx, __fmul_rn(tw, 0.5f));
+        const float b2y1f = __fsub_rn(ty, __fmul_rn(th, 0.5f)), b2y2f = __fadd_rn(ty, __fmul_rn(th, 0.5f));
+        const float w2f = __fsub_rn(b2x2f, b2x1f), h2f = __fsub_rn(b2y2f, b2y1f);
+        const double b2x1 = b2x1f, b2x2 = b2x2f, b2y1 = b2y1f, b2y2 = b2y2f;
         const double iw_raw = fmin(b1x2, b2x2) - fmax(b1x1, b2x1), ih_raw = fmin(b1y2, b2y2) - fmax(b1y1, b2y1);
         const double iw = fmax(iw_raw, 0.0), ih = fmax(ih_raw, 0.0);
         const double inter = iw * ih;
-        const double w1 = b1x2 - b1x1, h1 = b1y2 - b1y1, w2 = b2x2 - b2x1, h2 = b2y2 - b2y1;
-        const double uni = (w1 * h1 + 1e-16) + w2 * h2 - inter;
+        const double w1 = b1x2 - b1x1, h1 = b1y2 - b1y1;
+        const double uni = (w1 * h1 + 1e-16) + (double)__fmul_rn(w2f, h2f) - inter;
         const double iou = inter / uni;
         const double cw = fmax(b1x2, b2x2) - fmin(b1x1, b2x1), chh = fmax(b1y2, b2y2) - fmin(b1y1, b2y1);
         const double c2 = cw * cw + chh * chh + 1e-16;
-        const double Sx = (b2x1 + b2x2) - (b1x1 + b1x2), Sy = (b2y1 + b2y2) - (b1y1 + b1y2);
+        const double Sx = (double)__fadd_rn(b2x1f, b2x2f) - (b1x1 + b1x2), Sy = (double)__fadd_rn(b2y1f, b2y2f) - (b1y1 + b1y2);
         const double rho2 = Sx * Sx / 4 + Sy * Sy / 4;
-        const double D = atan(w2 / h2) - atan(w1 / h1);
+        const double D = (double)atanf(__fdiv_rn(w2f, h2f)) - atan(w1 / h1);
         const double v = (4.0 / (kPi * kPi)) * D * D;
         const double alpha = v / (1.0 - iou + v);                     // no_grad (loss.py:47-48)
         const double ciou = iou - (rho2 / c2 + v * alpha);
@@ -170,19 +182,23 @@ loss_rows_kernel(LossGeom g, LossWs ws) {
             const double Gv = -alpha;
             double gx1 = 0, gx2 = 0, gy1 = 0, gy2 = 0;                // d(ciou)/d(b1 corners)
             // intersection
-            if (iw_raw >= 0.0) { const double t = Ginter * ih; if (b1x2 < b2x2) gx2 += t; if (b1x1 > b2x1) gx1 -= t; }
-            if (ih_raw >= 0.0) { const double t = Ginter * iw; if (b1y2 < b2y2) gy2 += t; if (b1y1 > b2y1) gy1 -= t; }
+            // (the clamp's derivative at iw_raw == 0 is 1, as torch's clamp(0) has it)
+            if (iw_raw >= 0.0) { const double t = Ginter * ih; add_dmin(gx2, b1x2, b2x2, t); add_dmax(gx1, b1x1, b2x1, -t); }
+            if (ih_raw >= 0.0) { const double t = Ginter * iw; add_dmin(gy2, b1y2, b2y2, t); add_dmax(gy1, b1y1, b2y1, -t); }
             // U0 = w1*h1 + ...
             gx2 += GU0 * h1; gx1 -= GU0 * h1; gy2 += GU0 * w1; gy1 -= GU0 * w1;
             // enclosing box
-            { const double t = Gc2 * 2 * cw; if (b1x2 > b2x2) gx2 += t; if (b1x1 < b2x1) gx1 -= t; }
-            { const double t = Gc2 * 2 * chh; if (b1y2 > b2y2) gy2 += t; if (b1y1 < b2y1) gy1 -= t; }
+            { const double t = Gc2 * 2 * cw; add_dmax(gx2, b1x2, b2x2, t); add_dmin(gx1, b1x1, b2x1, -t); }
+            { const double t = Gc2 * 2 * chh; add_dmax(gy2, b1y2, b2y2, t); add_dmin(gy1, b1y1, b2y1, -t); }
             // centre distance
             gx1 += Grho * (-Sx / 2); gx2 += Grho * (-Sx / 2); gy1 += Grho * (-Sy / 2); gy2 += Grho * (-Sy / 2);
-            // aspect term v(w1, h1)
-            const double dv_dw1 = -(8.0 / (kPi * kPi)) * D * h1 / (w1 * w1 + h1 * h1);
-            const double dv_dh1 = (8.0 / (kPi * kPi)) * D * w1 / (w1 * w1 + h1 * h1);
-            gx2 += Gv * dv_dw1; gx1 -= Gv * dv_dw1; gy2 += Gv * dv_dh1; gy1 -= Gv * dv_dh1;
+            // aspect term v = c * (atan(w2/h2) - atan(w1/h1))^2, through atan' = 1 / (1 + x*x) and d(w1/h1) = (1/h1, -(w1/h1)/h1)
+            // as autograd takes it.  Where h1 is 0 in fp64 (a predicted height below the rounding of py) that is 0 * inf = NaN in the
+            // reference, and so here; the closed form D*w1 / (w1^2 + h1^2) would be finite.
+            const double x1 = w1 / h1;
+            const double Gat = -Gv * (8.0 / (kPi * kPi)) * D / (1.0 + x1 * x1);    // d(ciou)/d(w1/h1)
+            const double Gw1 = Gat / h1, Gh1 = -Gat * (x1 / h1);
+            gx2 += Gw1; gx1 -= Gw1; gy2 += Gh1; gy1 -= Gh1;
             // corners -> (px, py, pw, ph)
             const double gpx = gx1 + gx2, gpy = gy1 + gy2, gpw = (gx2 - gx1) / 2, gph = (gy2 - gy1) / 2;
             // -> logits; the xy branch is fp32 in the reference graph, the wh branch fp64 until the sigmoid

@@ -614,14 +614,41 @@ def debug_pw_tc(x, w):
     return out
 
 
+def loss_geometry(preds, cfg):
+    """(N, H, W, A, C) of the six head tensors, checked against each other and against cfg.  The kernel takes A, C and the
+    input size from the tensors while the reference takes anchor_num, classes and width / height from cfg (utils/loss.py:56,81,
+    148,198), so a cfg that disagrees with the tensors would silently select other anchors or another CE divisor: ValueError."""
+    if len(preds) != 6:
+        raise ValueError("compute_loss: expected the six head tensors, got %d" % len(preds))
+    N, _, h, w = preds[0].shape
+    A, C = preds[1].shape[1], preds[2].shape[1]
+    H, W = h * 16, w * 16
+    want = [(N, 4 * A, h, w), (N, A, h, w), (N, C, h, w), (N, 4 * A, h // 2, w // 2), (N, A, h // 2, w // 2),
+            (N, C, h // 2, w // 2)]
+    got = [tuple(p.shape) for p in preds]
+    if got != want or h % 2 or w % 2:
+        raise ValueError("compute_loss: head tensor shapes %s are not those of one %dx%d input with %d anchors and %d classes"
+                         % (got, H, W, A, C))
+    bad = []
+    if int(cfg["anchor_num"]) != A:
+        bad.append("anchor_num %s (the heads have %d anchors)" % (cfg["anchor_num"], A))
+    if int(cfg["classes"]) != C:
+        bad.append("classes %s (the heads have %d)" % (cfg["classes"], C))
+    if float(cfg["width"]) != W or float(cfg["height"]) != H:
+        bad.append("width x height %s x %s (the heads are those of a %d x %d input)" % (cfg["width"], cfg["height"], W, H))
+    if len(cfg["anchors"]) != 4 * A:
+        bad.append("%d anchor values (two levels of %d anchors need %d)" % (len(cfg["anchors"]), A, 4 * A))
+    if bad:
+        raise ValueError("compute_loss: cfg disagrees with the head tensors: " + "; ".join(bad))
+    return N, H, W, A, C
+
+
 def compute_loss(preds, targets, cfg, want_grads=True, return_workspace=False):
     """utils.loss.compute_loss on the device.  Returns (losses[4] CUDA tensor, dpreds 6-tuple or None[, workspace])."""
     for p in preds:
         _require_cuda(p, "preds")
+    N, H, W, A, C = loss_geometry(preds, cfg)
     preds = [p.detach().contiguous().float() for p in preds]
-    N, A4, h, w = preds[0].shape
-    A, C = preds[1].shape[1], preds[2].shape[1]
-    H, W = h * 16, w * 16
     dev = preds[0].device
     targets = targets.detach().to(dev).float().contiguous().reshape(-1, 6)
     nt = targets.shape[0]
