@@ -46,6 +46,40 @@ __device__ void load_floats(float* dst, const float* __restrict__ src, int count
     for (int i = threadIdx.x; i < count; i += blockDim.x) dst[i] = __ldg(src + i);
 }
 
+// The same for a square K x K layer (K % 4 == 0: the pack rows are K contiguous floats) and count % 4 == 0, by 16-byte cp.async
+// when the pack is 16-byte aligned, so that every thread has all its copies in flight at once (element-wise, they cost a
+// whole-image CTA tens of microseconds per block).  The caller commits the group and waits for it before its barrier.
+__device__ void cp16(float* dst, const float* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ void load_pw_async(float* dst, const float* __restrict__ src, int K) {
+    if ((uintptr_t)src & 15) { load_pw(dst, src, K, K, K); return; }
+    const int S = w_stride(K), R4 = K / 4;
+    for (int i = threadIdx.x; i < (K + 2) * R4; i += blockDim.x) {      // rows 0..K-1: W, row K: scale, row K+1: shift
+        const int k = i / R4, c = 4 * (i - k * R4);
+        cp16(dst + (k < K ? k * S : K * S + (k - K) * K) + c, src + k * K + c);
+    }
+}
+__device__ void load_floats_async(float* dst, const float* __restrict__ src, int count) {
+    if ((uintptr_t)src & 15) { load_floats(dst, src, count); return; }
+    for (int i = 4 * threadIdx.x; i < count; i += 4 * blockDim.x) cp16(dst + i, src + i);
+}
+
+// dw3x3 + BN of one pixel, the A-operand value of a pointwise contraction of the whole-image block kernels: tp = the top-left
+// tap, ld = the row stride of the plane, w = the channel's DW3 pack row.  The same operations in the same order as the stencils
+// of blk_kernel (written out there, so that its code stays as measured); tests/test_stage4_gpu.py pins the two bit for bit.
+__device__ __forceinline__ float dw3_bn(const float* tp, int ld, const float* w) {
+    float v = 0.f;
+#pragma unroll
+    for (int dy = 0; dy < 3; ++dy)
+#pragma unroll
+        for (int dx = 0; dx < 3; ++dx) v = fmaf(tp[dy * ld + dx], w[dy * 3 + dx], v);
+    return fmaf(v, w[9], w[10]);
+}
+
 // ---- ShuffleNetV2 blocks ------------------------------------------------------------------------------------------------
 struct BlkArgs {
     Planes in, out;
@@ -239,6 +273,267 @@ blk_kernel(const __grid_constant__ BlkArgs p) {
     }
 }
 
+// ---- stride-2 block on whole images -------------------------------------------------------------------------------------
+// When a CTA's 8 warps cover the output map with one 16-pixel tile each, the block runs per image instead of per band: all
+// five weight packs stay resident across the CTA's images (persistent grid), and T holds kS2Chunk pw1 channels at a time.
+// For each chunk, pw1 runs over the whole input map (no halo recompute), then the chunk's dw3x3/2 feeds the matching k-steps
+// of pw2, accumulated in registers across chunks.  The k-steps run in ascending order and every value is computed as in
+// blk_kernel<K, 2>, so the outputs are bit-identical to the banded kernel.
+constexpr int kS2Chunk = 32;
+
+__host__ constexpr size_t blk_s2_image_smem_bytes(int K, int Ho, int Wi) {
+    return ((size_t)3 * pw_smem_floats(K, K) + 24 * K + (size_t)kS2Chunk * (2 * Ho + 1) * (Wi + 2)) * sizeof(float);
+}
+bool blk_s2_whole_image(int K, int Ho, int Wo, int Wi) {
+    return K == 96 && Ho * Wo <= 16 * kWarps && blk_s2_image_smem_bytes(K, Ho, Wi) <= kSmemCap;
+}
+
+template <int K>
+__global__ void __launch_bounds__(kThreads, 1)
+blk_s2_image_kernel(const __grid_constant__ BlkArgs p) {
+    pdl_trigger();
+    static_assert(K % kS2Chunk == 0, "pw1 channel chunks must tile K");
+    constexpr int KS = K / 8, NT = K / 8, S = w_stride(K), CT = kS2Chunk / 8;
+    extern __shared__ __align__(16) float smem[];
+    float* sW1 = smem;
+    float* sW2 = sW1 + pw_smem_floats(K, K);
+    float* sWp = sW2 + pw_smem_floats(K, K);
+    float* sD = sWp + pw_smem_floats(K, K);               // main branch dw3x3/2: [K][12]
+    float* sDp = sD + 12 * K;                             // projection branch dw3x3/2
+    float* T = sDp + 12 * K;                              // [kS2Chunk][2 Ho + 1][Wi + 2]: T row r is input row r - 1
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const int Wt = p.Wi + 2, plT = (2 * p.Ho + 1) * Wt;
+    const int M1 = p.Hi * p.Wi, M2 = p.Ho * p.Wo;
+    const Planes in = p.in, out = p.out;
+    const unsigned short* tin = p.tin[0];
+
+    // pw1 writes the interior of T only: row 0, rows past the input and the side columns stay zero
+    for (int i = threadIdx.x; i < kS2Chunk * plT; i += kThreads) T[i] = 0.f;
+    load_pw_async(sW1, p.pw1[0], K);
+    load_pw_async(sW2, p.pw2[0], K);
+    load_pw_async(sWp, p.pwp, K);
+    load_floats_async(sD, p.dw[0], 12 * K);
+    load_floats_async(sDp, p.dwp, 12 * K);
+    cp_async_commit();
+    cp_async_wait<0>();
+    pdl_wait();
+    __syncthreads();
+
+    // this warp's output tile
+    const int mo = warp * 16;
+    int base[2], offp[2], oo[2]; bool ok[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int m = mo + g + 8 * h, r = m / p.Wo, c = m - r * p.Wo;
+        ok[h] = m < M2;
+        base[h] = ok[h] ? 2 * r * Wt + 2 * c : 0;
+        offp[h] = ok[h] ? in.org + (2 * r - 1) * in.Ws + 2 * c - 1 : in.org;
+        oo[h] = out.org + r * out.Ws + c;
+    }
+    for (int n = blockIdx.x; n < p.items; n += gridDim.x) {
+        const float* ib = in.base + (long long)n * in.sN;
+        float* ob = out.base + (long long)n * out.sN;
+        float acc[NT][4];
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
+        for (int c0 = 0; c0 < K; c0 += kS2Chunk) {
+            // pw1 + BN + ReLU, output channels [c0, c0 + kS2Chunk), over the whole input map; all A fragments of a tile are
+            // loaded before its MMAs
+            for (int m0 = warp * 16; m0 < M1; m0 += kWarps * 16) {
+                int off[2]; bool okin[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = m0 + g + 8 * h, r = m / p.Wi, c = m - r * p.Wi;
+                    okin[h] = m < M1;
+                    off[h] = in.org + r * in.Ws + c;
+                }
+                float af[KS][4];
+#pragma unroll
+                for (int ks = 0; ks < KS; ++ks) {
+                    const long long k0 = (long long)tin[8 * ks + t] * in.sC, k1 = (long long)tin[8 * ks + t + 4] * in.sC;
+                    af[ks][0] = okin[0] ? ib[k0 + off[0]] : 0.f;
+                    af[ks][1] = okin[1] ? ib[k0 + off[1]] : 0.f;
+                    af[ks][2] = okin[0] ? ib[k1 + off[0]] : 0.f;
+                    af[ks][3] = okin[1] ? ib[k1 + off[1]] : 0.f;
+                }
+                float a1[CT][4];
+                warp_gemm_regs<KS, CT>(a1, sW1 + c0, S, af);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (!okin[h]) continue;
+                    const int m = m0 + g + 8 * h, r = m / p.Wi, c = m - r * p.Wi;
+#pragma unroll
+                    for (int nt = 0; nt < CT; ++nt)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = 8 * nt + 2 * t + e;
+                            T[col * plT + (r + 1) * Wt + c + 1] =
+                                fmaxf(fmaf(a1[nt][2 * h + e], sW1[K * S + c0 + col], sW1[K * S + K + c0 + col]), 0.f);
+                        }
+                }
+            }
+            __syncthreads();
+            // dw3x3/2 + BN of the chunk from T: k-steps [c0 / 8, c0 / 8 + CT) of pw2
+            if (mo < M2)
+                warp_gemm_acc<CT, NT>(acc, sW2 + c0 * S, S, [&](int ks, float (&a)[4]) {
+#pragma unroll
+                    for (int q = 0; q < 2; ++q) {
+                        const int k = 8 * ks + t + 4 * q;
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const float v = dw3_bn(T + k * plT + base[h], Wt, sD + 12 * (c0 + k));
+                            a[2 * q + h] = ok[h] ? v : 0.f;
+                        }
+                    }
+                });
+            __syncthreads();      // the next chunk overwrites T
+        }
+        if (mo >= M2) continue;
+        auto store = [&](const float* sc, const unsigned short* tdst) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (!ok[h]) continue;
+#pragma unroll
+                for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = 8 * nt + 2 * t + e;
+                        ob[(long long)tdst[col] * out.sC + oo[h]] = fmaxf(fmaf(acc[nt][2 * h + e], sc[col], sc[K + col]), 0.f);
+                    }
+            }
+        };
+        // main branch: pw2 + BN + ReLU -> planes K..2K-1 of the block
+        store(sW2 + K * S, p.tmain);
+        // projection branch: dw3x3/2 + BN straight from the input planes -> pw + BN + ReLU -> planes 0..K-1
+        warp_gemm<KS, NT>(acc, sWp, S, [&](int ks, float (&a)[4]) {
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+                const int k = 8 * ks + t + 4 * q;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const float v = dw3_bn(ib + (long long)tin[k] * in.sC + offp[h], in.Ws, sDp + 12 * k);
+                    a[2 * q + h] = ok[h] ? v : 0.f;
+                }
+            }
+        });
+        store(sWp + K * S, p.tout[0]);
+    }
+}
+
+// ---- stride-1 chains on whole images, one CTA per SM ----------------------------------------------------------------------
+// A chain whose whole image fits in one SM's shared memory but not in kChainBudget (K = 96: stage4.1-3 at 352x352, 151 KB) runs
+// a persistent grid of one CTA per SM.  The CTA takes all its images through block j before block j+1, so each block's weights
+// are loaded once per CTA, and the loads overlap the compute: block j+1's pw1 matrix is copied into sW1 while block j runs its
+// last pw2, its pw2 matrix and dw pack into sW2 / sD while block j+1 runs its first pw1.  T keeps its zero frame for the whole
+// launch, so pw1 runs over the H x W pixels of the image only, not over the two halo rows outside it.  Every value is computed
+// as in blk_kernel<K, 1>, so the outputs are bit-identical to running the blocks one launch each.
+template <int K>
+__global__ void __launch_bounds__(kThreads, 1)
+blk_chain_kernel(const __grid_constant__ BlkArgs p) {
+    pdl_trigger();
+    constexpr int KS = K / 8, NT = K / 8, S = w_stride(K);
+    extern __shared__ __align__(16) float smem[];
+    float* sW1 = smem;
+    float* sW2 = sW1 + pw_smem_floats(K, K);
+    float* sD = sW2 + pw_smem_floats(K, K);
+    float* T = sD + 12 * K;                               // [K][H + 2][W + 2]: T row r is image row r - 1
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const int Wt = p.Wi + 2, plT = (p.Hi + 2) * Wt, M = p.Hi * p.Wi;
+    const Planes P = p.in;
+
+    for (int i = threadIdx.x; i < K * plT; i += kThreads) T[i] = 0.f;
+    load_pw_async(sW1, p.pw1[0], K);
+    cp_async_commit();
+    load_pw_async(sW2, p.pw2[0], K);
+    load_floats_async(sD, p.dw[0], 12 * K);
+    cp_async_commit();
+    pdl_wait();
+    const int last = blockIdx.x + (p.items - 1 - blockIdx.x) / gridDim.x * gridDim.x;      // this CTA's last image
+    for (int j = 0; j < p.nblk; ++j) {
+        const unsigned short* tin = p.tin[j];
+        const unsigned short* tout = p.tout[j];
+        for (int n = blockIdx.x; n < p.items; n += gridDim.x) {
+            float* ib = P.base + (long long)n * P.sN;
+            cp_async_wait<1>();       // sW1 of block j; its sW2 / sD may still be in flight
+            __syncthreads();
+            // pw1 + BN + ReLU over the image's pixels
+            for (int m0 = warp * 16; m0 < M; m0 += kWarps * 16) {
+                int off[2]; bool ok[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = m0 + g + 8 * h, r = m / p.Wi, c = m - r * p.Wi;
+                    ok[h] = m < M;
+                    off[h] = P.org + r * P.Ws + c;
+                }
+                float acc[NT][4];
+                warp_gemm<KS, NT>(acc, sW1, S, [&](int ks, float (&a)[4]) {
+                    const long long c0 = (long long)tin[8 * ks + t] * P.sC, c1 = (long long)tin[8 * ks + t + 4] * P.sC;
+                    a[0] = ok[0] ? ib[c0 + off[0]] : 0.f;
+                    a[1] = ok[1] ? ib[c0 + off[1]] : 0.f;
+                    a[2] = ok[0] ? ib[c1 + off[0]] : 0.f;
+                    a[3] = ok[1] ? ib[c1 + off[1]] : 0.f;
+                });
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (!ok[h]) continue;
+                    const int m = m0 + g + 8 * h, r = m / p.Wi, c = m - r * p.Wi;
+#pragma unroll
+                    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = 8 * nt + 2 * t + e;
+                            T[col * plT + (r + 1) * Wt + c + 1] = fmaxf(fmaf(acc[nt][2 * h + e], sW1[K * S + col], sW1[K * S + K + col]), 0.f);
+                        }
+                }
+            }
+            cp_async_wait<0>();       // sW2 / sD of block j
+            __syncthreads();
+            if (n == last && j + 1 < p.nblk) { load_pw_async(sW1, p.pw1[j + 1], K); cp_async_commit(); }
+            // dw3x3 + BN from T as the A operand -> pw2 + BN + ReLU -> the block's output planes
+            for (int m0 = warp * 16; m0 < M; m0 += kWarps * 16) {
+                int base[2]; bool ok[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = m0 + g + 8 * h, r = m / p.Wi, c = m - r * p.Wi;
+                    ok[h] = m < M;
+                    base[h] = ok[h] ? r * Wt + c : 0;
+                }
+                float acc[NT][4];
+                warp_gemm<KS, NT>(acc, sW2, S, [&](int ks, float (&a)[4]) {
+#pragma unroll
+                    for (int q = 0; q < 2; ++q) {
+                        const int k = 8 * ks + t + 4 * q;
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const float v = dw3_bn(T + k * plT + base[h], Wt, sD + 12 * k);
+                            a[2 * q + h] = ok[h] ? v : 0.f;
+                        }
+                    }
+                });
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (!ok[h]) continue;
+                    const int m = m0 + g + 8 * h, r = m / p.Wi, c = m - r * p.Wi;
+                    const int o = P.org + r * P.Ws + c;
+#pragma unroll
+                    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = 8 * nt + 2 * t + e;
+                            ib[(long long)tout[col] * P.sC + o] = fmaxf(fmaf(acc[nt][2 * h + e], sW2[K * S + col], sW2[K * S + K + col]), 0.f);
+                        }
+                }
+            }
+            __syncthreads();          // T, sW2 / sD and this block's output planes are consumed next
+            if (n == last && j + 1 < p.nblk) {
+                load_pw_async(sW2, p.pw2[j + 1], K);
+                load_floats_async(sD, p.dw[j + 1], 12 * K);
+                cp_async_commit();
+            }
+        }
+    }
+}
+
 int persistent_grid(long long items, int per_sm) {
     const long long cap = (long long)per_sm * sm_count();
     return (int)(items < cap ? items : cap);
@@ -281,6 +576,18 @@ int run_blk(BlkArgs& a, int N, cudaStream_t s) {
 template <int K>
 int dispatch_blk(int stride, BlkArgs& a, int N, cudaStream_t s) {
     return stride == 1 ? run_blk<K, 1>(a, N, s) : run_blk<K, 2>(a, N, s);
+}
+
+// whole-image kernels: one CTA per SM, a persistent grid over the N images
+template <class Kern>
+int run_whole_image(Kern kern, size_t bytes, BlkArgs& a, int N, cudaStream_t s) {
+    a.R = a.Ho; a.bands = 1; a.items = N;
+    if (int rc = smem_attr(kern, bytes)) return rc;
+    int per_sm = 0;
+    YFV2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, bytes));
+    YFV2_CUDA(launch_k(kern, persistent_grid(N, per_sm > 0 ? per_sm : 1), kThreads, bytes, s, pdl_take(), a));
+    YFV2_LAUNCH_CHECK();
+    return YFV2_OK;
 }
 
 // ---- FPN reducers -------------------------------------------------------------------------------------------------------
@@ -518,7 +825,12 @@ int run_pw_test(const float* x, const float* w, float* out, int N, int P, cudaSt
 
 }  // namespace
 
-bool blk_s1_chainable(int K, int H, int W) { return blk_smem_bytes(K, 1, H, W) <= kChainBudget; }
+// A chain needs a whole image per CTA: within kChainBudget (two CTAs per SM) blk_kernel runs it; K = 96 chains up to one SM's
+// shared memory run on blk_chain_kernel (stage4.1-3 at 352x352, where three launches of 2-row bands recompute most of pw1 as halo).
+bool blk_s1_chainable(int K, int H, int W) {
+    const size_t bytes = blk_smem_bytes(K, 1, H, W);
+    return bytes <= kChainBudget || (K == 96 && bytes <= kSmemCap);
+}
 
 int blk_launch_s1(int K, const Planes& P, int nblk, const ChanTab* tin, const ChanTab* tout, const float* const* w1,
                   const float* const* wdw, const float* const* w2, int N, cudaStream_t s) {
@@ -535,6 +847,8 @@ int blk_launch_s1(int K, const Planes& P, int nblk, const ChanTab* tin, const Ch
         a.pw1[j] = w1[j]; a.dw[j] = wdw[j]; a.pw2[j] = w2[j];
         for (int i = 0; i < K; ++i) { a.tin[j][i] = tin[j].c[i]; a.tout[j][i] = tout[j].c[i]; }
     }
+    const size_t bytes = blk_smem_bytes(K, 1, P.H, P.W);
+    if (nblk > 1 && bytes > kChainBudget) return run_whole_image(blk_chain_kernel<96>, bytes, a, N, s);   // K = 96 (chainable)
     switch (K) {
     case 24: return dispatch_blk<24>(1, a, N, s);
     case 48: return dispatch_blk<48>(1, a, N, s);
@@ -550,9 +864,11 @@ int blk_launch_s2(int K, const Planes& in, const Planes& out, const ChanTab& tin
     a.in = in; a.out = out;
     a.Hi = in.H; a.Wi = in.W; a.Ho = out.H; a.Wo = out.W;
     a.nblk = 1;
-    a.R = blk_rows(K, 2, out.H, in.W, N);
     a.pw1[0] = w1; a.dw[0] = wdwm; a.pw2[0] = w2; a.dwp = wdwp; a.pwp = wp;
     for (int i = 0; i < K; ++i) { a.tin[0][i] = tin.c[i]; a.tout[0][i] = tout.c[i]; a.tmain[i] = tout.c[K + i]; }
+    if (blk_s2_whole_image(K, out.H, out.W, in.W))      // K = 96
+        return run_whole_image(blk_s2_image_kernel<96>, blk_s2_image_smem_bytes(K, out.H, in.W), a, N, s);
+    a.R = blk_rows(K, 2, out.H, in.W, N);
     switch (K) {
     case 24: return dispatch_blk<24>(2, a, N, s);
     case 48: return dispatch_blk<48>(2, a, N, s);

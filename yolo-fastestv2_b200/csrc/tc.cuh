@@ -64,14 +64,14 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// acc[nt] = A(16 x 8 KS) * W(8 KS x 8 NT) for the calling warp's 16-row tile.
+// acc[nt] += A(16 x 8 KS) * W(8 KS x 8 NT) for the calling warp's 16-row tile.
 // load_a(ks, a) fills this lane's A fragment of k-step ks: a[0] = (row g, k 8ks+t), a[1] = (g+8, 8ks+t), a[2] = (g, 8ks+t+4),
 // a[3] = (g+8, 8ks+t+4).  Result: acc[nt][0..1] = (row g, columns 8nt+2t, 8nt+2t+1), acc[nt][2..3] = the same for row g+8.
+// A contraction split into calls over consecutive k ranges (sW advanced by 8 KS rows each time) issues, per accumulator, the
+// MMAs of one call over the whole range in the same order, so its result is bit-identical.
 template <int KS, int NT, class LoadA>
-__device__ __forceinline__ void warp_gemm(float (&acc)[NT][4], const float* __restrict__ sW, int S, LoadA&& load_a) {
+__device__ __forceinline__ void warp_gemm_acc(float (&acc)[NT][4], const float* __restrict__ sW, int S, LoadA&& load_a) {
     const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-#pragma unroll
-    for (int nt = 0; nt < NT; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
 #pragma unroll 2
     for (int ks = 0; ks < KS; ++ks) {
         float a[4];
@@ -91,6 +91,14 @@ __device__ __forceinline__ void warp_gemm(float (&acc)[NT][4], const float* __re
             mma_tf32(acc[nt], ah, bh0, bh1);
         }
     }
+}
+
+// acc[nt] = A * W: warp_gemm_acc from zero
+template <int KS, int NT, class LoadA>
+__device__ __forceinline__ void warp_gemm(float (&acc)[NT][4], const float* __restrict__ sW, int S, LoadA&& load_a) {
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
+    warp_gemm_acc<KS, NT>(acc, sW, S, load_a);
 }
 
 // The same contraction with the KS A fragments already in registers (a[ks] as load_a would fill it), so that one A operand can
