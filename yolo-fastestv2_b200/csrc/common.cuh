@@ -99,6 +99,11 @@ __device__ __forceinline__ void cp_async4(float* smem_dst, const float* gsrc) {
     const unsigned s = (unsigned)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(s), "l"(gsrc) : "memory");
 }
+// 16 bytes (both addresses 16-byte aligned), bypassing L1; src_bytes == 0 reads nothing and zero-fills the 16 bytes
+__device__ __forceinline__ void cp_async16_zfill(void* smem_dst, const void* gsrc, uint32_t src_bytes) {
+    const unsigned s = (unsigned)__cvta_generic_to_shared(smem_dst);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gsrc), "r"(src_bytes) : "memory");
+}
 __device__ __forceinline__ void cp_async_wait_all() {
     asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;\n" ::: "memory");
 }

@@ -12,9 +12,11 @@
 // LDS.128, i.e. 2592 FFMA against ~190 shared-memory instructions (93 % FFMA in the main loop).
 //
 // A work item is (image, band of TRo pooled rows, tile of TWo <= 44 pooled columns):
-//   0. the input patch arrives by one TMA bulk copy per (channel, row) [uint8: uchar4 converting loads; an input whose base
-//      is not 16-byte (fp32) / 4-byte (uint8) aligned: scalar loads], prefetched while the
-//      previous item pools;
+//   0. fp32: the input patch arrives by one TMA bulk copy per (channel, row), issued after the previous item's conv, while it
+//      pools.  uint8: the raw bytes of the next item arrive by 16-byte cp.async (zero-filled outside the image) in the half of
+//      Hs that is free during the conv, issued before the conv; after it they are converted into Xin through a 256-entry
+//      table of v / 255.0f (one correctly rounded division per byte value, so no per-pixel division).  A base that is not
+//      16-byte aligned (or, for uint8, W not a multiple of 16): scalar loads after the conv;
 //   1. conv + BN (scale folded into the weights, shift = accumulator init) for the CR = 2 TRo + 1 conv rows the pool
 //      windows touch; positions outside the conv output become -inf (PyTorch pads max_pool2d with -inf);
 //   2. horizontal 3-max in registers (the one column a thread lacks comes from its right neighbour through shared
@@ -37,8 +39,11 @@ struct StemFArgs {
     const float* wpack;     // [27][24] | scale[24] | shift[24]
     int N, H, W;
     int TRo, TWo, tilesX, tilesY, S;
-    int vec;                // input base 16-byte (fp32) / 4-byte (uint8) aligned: bulk copies / uchar4 loads
+    int vec;                // fp32: base 16-byte aligned -> bulk copies; uint8: base and W multiples of 16 -> cp.async
 };
+
+// bytes per staged uint8 row: the Wst = 4 TWo + 12 columns from ic0, plus up to 12 before them from ic0 & ~15, rounded to 16
+__host__ __device__ __forceinline__ int stem_byte_row(int TWo) { return (4 * TWo + 24 + 15) & ~15; }
 
 __device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
@@ -53,14 +58,21 @@ stem_kernel(const __grid_constant__ StemFArgs p) {
     const int CR = 2 * TRo + 1, IR = 4 * TRo + 3, Wst = 4 * TWo + 12;     // staged column 0 <-> input column 4*ox0 - 4
     const int HSW = 2 * S;
     float* sW = smem;                                  // folded weights + shift
-    float* Xin = sW + kStemW;                          // [3][IR][Wst]
+    float* lut = sW + kStemW;                          // [256] byte v -> v / 255.0f
+    float* Xin = lut + 256;                            // [3][IR][Wst]
     float* Hs = Xin + 3 * IR * Wst;                    // [24][CR][HSW] horizontal maxima; its head doubles as
     float* E = Hs;                                     // [24][CR][S]   first conv column of every strip
+    // [3][IR][Wb] raw uint8 patch of the next item, in the half of Hs that is free from B0 until B2 (E is the other half)
+    const int Wb = stem_byte_row(TWo);
+    uint8_t* Xb = reinterpret_cast<uint8_t*>(Hs + 24 * CR * S);
     const int tid = threadIdx.x;
     {   // BN scale folded into the weights (one rounding per weight), shift kept as the accumulator's start value
         const float* scale = p.wpack + 27 * 24;
         for (int i = tid; i < 27 * 24; i += ST_THREADS) sW[i] = __fmul_rn(__ldg(p.wpack + i), __ldg(scale + (i % 24)));
         if (tid < 24) sW[27 * 24 + tid] = __ldg(scale + 24 + tid);
+        // the `/255.0` of utils/utils.py:368 as a table: the same correctly rounded quotient without a division per pixel
+        if (U8)
+            for (int v = tid; v < 256; v += ST_THREADS) lut[v] = __fdiv_rn((float)v, 255.0f);
     }
     if (tid == 0) { mbar_init(&xbar, 1); fence_mbar_init(); }
     __syncthreads();
@@ -82,7 +94,7 @@ stem_kernel(const __grid_constant__ StemFArgs p) {
                 float v = 0.f;
                 if (iy >= 0 && iy < H && ix >= 0 && ix < W) {
                     const size_t idx = (((size_t)n * 3 + c) * H + iy) * W + ix;
-                    v = U8 ? __fdiv_rn((float)__ldg(reinterpret_cast<const uint8_t*>(p.x) + idx), 255.0f) : __ldg(reinterpret_cast<const float*>(p.x) + idx);
+                    v = U8 ? lut[__ldg(reinterpret_cast<const uint8_t*>(p.x) + idx)] : __ldg(reinterpret_cast<const float*>(p.x) + idx);
                 }
                 Xin[i] = v;
             }
@@ -103,25 +115,44 @@ stem_kernel(const __grid_constant__ StemFArgs p) {
                 }
             }
         } else {
-            const int q4 = Wst / 4;
-            for (int i = tid; i < 3 * IR * q4; i += ST_THREADS) {
-                const int cr = i / q4, j4 = i - cr * q4;
+            // raw bytes -> Xb rows of Wb bytes that start at input column ic0 & ~15, 16 per cp.async: every copy in flight at
+            // once.  The base and W are multiples of 16, so a chunk lies wholly inside or wholly outside the image; outside
+            // ones are zero-filled (byte 0 converts to 0.f)
+            const uint8_t* x8 = reinterpret_cast<const uint8_t*>(p.x);
+            const int a0 = ic0 & ~15, q16 = Wb / 16;
+            for (int i = tid; i < 3 * IR * q16; i += ST_THREADS) {
+                const int cr = i / q16, j = i - cr * q16;
                 const int c = cr / IR, r = cr - c * IR;
-                const int iy = iy0 + r, ix = ic0 + 4 * j4;
-                float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (iy >= 0 && iy < H && ix >= 0 && ix < W) {
-                    const uchar4 u = __ldg(reinterpret_cast<const uchar4*>(reinterpret_cast<const uint8_t*>(p.x) + (((size_t)n * 3 + c) * H + iy) * W + ix));
-                    v = make_float4(__fdiv_rn((float)u.x, 255.0f), __fdiv_rn((float)u.y, 255.0f), __fdiv_rn((float)u.z, 255.0f), __fdiv_rn((float)u.w, 255.0f));
-                }
-                *reinterpret_cast<float4*>(Xin + cr * Wst + 4 * j4) = v;
+                const int iy = iy0 + r, ix = a0 + 16 * j;
+                const bool in = iy >= 0 && iy < H && ix >= 0 && ix < W;
+                cp_async16_zfill(Xb + 16 * i, in ? x8 + (((size_t)n * 3 + c) * H + iy) * W + ix : x8, in ? 16u : 0u);
             }
         }
     };
+    // uint8 with aligned base: Xb (complete, after a barrier) -> Xin, 4 pixels per step
+    auto convert = [&](int item) {
+        const int tx = item % p.tilesX;
+        const int off = (4 * (tx * TWo) - 4) & 15;           // ic0 - (ic0 & ~15)
+        const int q4 = Wst / 4;
+        for (int i = tid; i < 3 * IR * q4; i += ST_THREADS) {
+            const int cr = i / q4, j4 = i - cr * q4;
+            const uint32_t b = *reinterpret_cast<const uint32_t*>(Xb + cr * Wb + off + 4 * j4);
+            *reinterpret_cast<float4*>(Xin + 4 * i) = make_float4(lut[b & 255u], lut[(b >> 8) & 255u], lut[(b >> 16) & 255u], lut[b >> 24]);
+        }
+    };
+    const bool async_u8 = U8 && p.vec;
 
     const int r = tid / S, s = tid - r * S;                  // conv row of the band / strip of 4 conv columns
     const int p_oyl = tid / TWo, p_pc = tid - p_oyl * TWo;   // pooled pixel this thread writes in step 3
     uint32_t xpar = 0;
-    if (blockIdx.x < items) stage(blockIdx.x);
+    if (blockIdx.x < items) {
+        stage(blockIdx.x);
+        if (async_u8) {
+            cp_async_wait_all();
+            __syncthreads();
+            convert(blockIdx.x);
+        }
+    }
     for (int item = blockIdx.x; item < items; item += gridDim.x) {
         const int n = item / (p.tilesX * p.tilesY);
         const int rem = item - n * (p.tilesX * p.tilesY);
@@ -130,7 +161,9 @@ stem_kernel(const __grid_constant__ StemFArgs p) {
         const int rows = min(TRo, HO - oy0), cols = min(TWo, WO - ox0);
         const bool active = r < 2 * rows + 1;
         if (!U8 && p.vec) { mbar_wait(&xbar, xpar); xpar ^= 1u; }
-        __syncthreads();                                      // B0: edge zero-fill / uint8 stores visible; Hs free again
+        __syncthreads();                                      // B0: edge zero-fill / converted uint8 visible; Hs free again
+        const bool more = item + gridDim.x < items;
+        if (async_u8 && more) stage(item + gridDim.x);        // the next item's bytes arrive while this one convolves
 
         // ---- 1. conv: acc[j][ch], j = position 4s+j of conv row r (tile-local) ----------------------------------------
         float h0[24], h1[24];
@@ -197,8 +230,11 @@ stem_kernel(const __grid_constant__ StemFArgs p) {
                 h1[ch] = fmaxf(acc[2][ch], acc[3][ch]);
             }
         }
-        __syncthreads();                                      // B1: every read of Xin is done, E is visible
-        if (item + gridDim.x < items) {
+        if (async_u8 && more) cp_async_wait_all();          // this thread's bytes of the next item have landed
+        __syncthreads();                                      // B1: every read of Xin is done, E and Xb are visible
+        if (async_u8 && more) {
+            convert(item + gridDim.x);
+        } else if (more) {
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of Xin before the async-proxy refill
             stage(item + gridDim.x);                          // overlaps the pooling below
         }
@@ -231,14 +267,17 @@ stem_kernel(const __grid_constant__ StemFArgs p) {
 
 __host__ size_t stem_smem_bytes(int TRo, int TWo, int S) {
     const int CR = 2 * TRo + 1, IR = 4 * TRo + 3, Wst = 4 * TWo + 12;
-    return (size_t)(kStemW + 3 * IR * Wst + 24 * CR * 2 * S + 4) * sizeof(float);
+    return (size_t)(kStemW + 256 + 3 * IR * Wst + 24 * CR * 2 * S + 4) * sizeof(float);
+}
+// the uint8 patch fits the half of Hs that E leaves free
+__host__ bool stem_bytes_fit(int TRo, int TWo, int S) {
+    return 3 * (4 * TRo + 3) * stem_byte_row(TWo) <= 24 * (2 * TRo + 1) * S * (int)sizeof(float);
 }
 }  // namespace
 
 int launch_stem(const StemArgs& a, cudaStream_t s) {
     if (a.H % 4 || a.W % 4 || a.H < 4 || a.W < 4) { set_error("stem: input %dx%d must be a multiple of 4", a.H, a.W); return YFV2_EINVAL; }
     StemFArgs k{a.x, a.out, a.wpack, a.N, a.H, a.W, 0, 0, 0, 0, 0, 0};
-    k.vec = ((uintptr_t)a.x & (a.is_u8 ? 3 : 15)) == 0;
     const int HO = a.H / 4, WO = a.W / 4;
     // tiles of at most 44 pooled columns, as equal as possible; S strips of 4 conv columns cover the 2 TWo + 1 conv columns
     k.tilesX = (WO + 43) / 44;
@@ -251,6 +290,8 @@ int launch_stem(const StemArgs& a, cudaStream_t s) {
     if (k.TRo < 1) k.TRo = 1;
     const size_t bytes = stem_smem_bytes(k.TRo, k.TWo, k.S);
     if ((2 * k.TRo + 1) * k.S > ST_THREADS || k.TRo * k.TWo > ST_THREADS || bytes > kSmemCap - 1024) { set_error("stem: unsupported geometry %dx%d", a.H, a.W); return YFV2_EUNSUPPORTED; }
+    // asynchronous staging needs 16-byte aligned rows (uint8: and room for the bytes); other inputs take the scalar loads
+    k.vec = ((uintptr_t)a.x & 15) == 0 && (!a.is_u8 || (a.W % 16 == 0 && stem_bytes_fit(k.TRo, k.TWo, k.S)));
     k.tilesY = (HO + k.TRo - 1) / k.TRo;
     const int items = a.N * k.tilesX * k.tilesY;
     const int grid = items < 2 * sm_count() ? items : 2 * sm_count();
