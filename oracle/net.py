@@ -57,12 +57,18 @@ def shuffle_block(sd, x, prefix, stride, training=False, update_running=False):
     return torch.cat((proj, m), 1)
 
 
-def backbone(sd, x, training=False, update_running=False, taps=None):
-    """ShuffleNetV2.forward (shufflenetv2.py:102-109) -> (C2, C3)."""
+def stem(sd, x, training=False, update_running=False):
+    """first_conv + maxpool (shufflenetv2.py:74-80,103-104)."""
     p = "backbone."
     x = F.conv2d(x, sd[p + "first_conv.0.weight"], None, 2, 1)
     x = F.relu(_bn(sd, x, p + "first_conv.1", training, update_running))
-    x = F.max_pool2d(x, 3, 2, 1)
+    return F.max_pool2d(x, 3, 2, 1)
+
+
+def backbone(sd, x, training=False, update_running=False, taps=None):
+    """ShuffleNetV2.forward (shufflenetv2.py:102-109) -> (C2, C3)."""
+    p = "backbone."
+    x = stem(sd, x, training, update_running)
     if taps is not None:
         taps["stem"] = x
     outs = []
@@ -76,25 +82,40 @@ def backbone(sd, x, training=False, update_running=False, taps=None):
     return outs[1], outs[2]
 
 
+def dwconv_half(sd, x, prefix, half, training=False, update_running=False):
+    """One half of DWConvblock.forward (fpn.py:12-29): dw5x5+BN+ReLU, pw+BN; half 0 is block.0-4, half 1 block.5-9."""
+    bn = lambda t, i: _bn(sd, t, prefix + "block.%d" % (i + 5 * half), training, update_running)
+    x = F.relu(bn(_dw(sd, x, prefix + "block.%d" % (5 * half), 1, 2), 1))
+    return bn(_pw(sd, x, prefix + "block.%d" % (3 + 5 * half)), 4)
+
+
 def dwconv_block(sd, x, prefix, training=False, update_running=False):
     """DWConvblock.forward (fpn.py:12-29): dw5x5+BN+ReLU, pw+BN, dw5x5+BN+ReLU, pw+BN."""
-    bn = lambda t, n: _bn(sd, t, prefix + "block." + n, training, update_running)
-    x = F.relu(bn(_dw(sd, x, prefix + "block.0", 1, 2), "1"))
-    x = bn(_pw(sd, x, prefix + "block.3"), "4")
-    x = F.relu(bn(_dw(sd, x, prefix + "block.5", 1, 2), "6"))
-    x = bn(_pw(sd, x, prefix + "block.8"), "9")
-    return x
+    x = dwconv_half(sd, x, prefix, 0, training, update_running)
+    return dwconv_half(sd, x, prefix, 1, training, update_running)
+
+
+def reduce_s3(sd, C3, training=False, update_running=False):
+    """S3 = conv1x1_3(C3) + BN + ReLU (fpn.py:51-52)."""
+    p = "fpn.conv1x1_3."
+    return F.relu(_bn(sd, _pw(sd, C3, p + "0"), p + "1", training, update_running))
+
+
+def reduce_s2(sd, C2, C3, training=False, update_running=False):
+    """S2 = conv1x1_2(cat(nearest-up2(C3), C2)) + BN + ReLU (fpn.py:57-59)."""
+    p = "fpn.conv1x1_2."
+    P2 = torch.cat((F.interpolate(C3, scale_factor=2), C2), 1)
+    return F.relu(_bn(sd, _pw(sd, P2, p + "0"), p + "1", training, update_running))
 
 
 def fpn(sd, C2, C3, training=False, update_running=False, taps=None):
     """LightFPN.forward (fpn.py:51-64).  Module execution order matters in train mode only
     through running-stat updates, which are per-layer, so order is free here."""
     p = "fpn."
-    S3 = F.relu(_bn(sd, _pw(sd, C3, p + "conv1x1_3.0"), p + "conv1x1_3.1", training, update_running))
+    S3 = reduce_s3(sd, C3, training, update_running)
     cls_3 = dwconv_block(sd, S3, p + "cls_head_3.", training, update_running)
     reg_3 = dwconv_block(sd, S3, p + "reg_head_3.", training, update_running)
-    P2 = torch.cat((F.interpolate(C3, scale_factor=2), C2), 1)      # nearest, fpn.py:57-58
-    S2 = F.relu(_bn(sd, _pw(sd, P2, p + "conv1x1_2.0"), p + "conv1x1_2.1", training, update_running))
+    S2 = reduce_s2(sd, C2, C3, training, update_running)
     cls_2 = dwconv_block(sd, S2, p + "cls_head_2.", training, update_running)
     reg_2 = dwconv_block(sd, S2, p + "reg_head_2.", training, update_running)
     if taps is not None:
@@ -110,12 +131,14 @@ def forward(sd, x, training=False, update_running=False, taps=None):
     if taps is not None:
         taps["C2"], taps["C3"] = C2, C3
     cls_2, reg_2, cls_3, reg_3 = fpn(sd, C2, C3, training, update_running, taps)
-    out = []
-    for cls_f, reg_f in ((cls_2, reg_2), (cls_3, reg_3)):
-        out.append(_pw(sd, reg_f, "output_reg_layers"))
-        out.append(_pw(sd, cls_f, "output_obj_layers"))      # obj aliases the cls branch, fpn.py:54,61
-        out.append(_pw(sd, cls_f, "output_cls_layers"))
-    return tuple(out)
+    return output_layers(sd, cls_2, reg_2) + output_layers(sd, cls_3, reg_3)
+
+
+def output_layers(sd, cls_f, reg_f):
+    """(reg, obj, cls) logits of one level (detector.py:17-19,28-31)."""
+    return (_pw(sd, reg_f, "output_reg_layers"),
+            _pw(sd, cls_f, "output_obj_layers"),      # obj aliases the cls branch, fpn.py:54,61
+            _pw(sd, cls_f, "output_cls_layers"))
 
 
 def forward_export(sd, x):
