@@ -273,6 +273,178 @@ blk_kernel(const __grid_constant__ BlkArgs p) {
     }
 }
 
+// ---- stride-2 block: a band walked in steps of rows ------------------------------------------------------------------------
+// The K = 24 / 48 stride-2 blocks (stage2.0, stage3.0) keep the bands of blk_rows and one CTA per band, but the CTA walks its
+// band G output rows at a time instead of running pw1 over the whole band first:
+//   * All five weight packs are loaded at once by 16-byte cp.async, with the band's first input rows, and stay resident: the
+//     projection branch does not take over the main branch's buffers.
+//   * Input rows are staged whole (frame columns included) by 16-byte cp.async into a ring X of 4G + 1 rows per channel; the
+//     copies of step s + 1 are issued before step s computes.  pw1 and the projection branch's dw3x3/2 both read X, not the
+//     global planes.
+//   * T holds the 2G + 1 pw1 rows of a step; its bottom row is carried into the next step as that step's top row.
+//   * The pw2 and projection tiles of a step run in one phase over all warps.
+// As in blk_kernel, the band's first step computes the pw1 row above the band, and outside the map the T row is zero.  Every
+// value is computed with the same operations in the same order as blk_kernel<K, 2> (an mma.sync output row depends only on its
+// own A row), so the outputs are bit-identical to it.
+//
+// The kernel keeps the name blk_kernel<K, 2> (in namespace walk) and the grid of one CTA per band: profiler traces and launch
+// models that know the banded kernel describe it unchanged.
+namespace walk {
+constexpr int G = 1;              // output rows per step
+
+__host__ __device__ constexpr int ring_rows(int G) { return 4 * G + 1; }
+// channel stride of X (n floats, n % 4 == 0): the four t lanes of an A-fragment read fall on distinct banks
+__host__ __device__ constexpr int ring_stride(int n) { return n % 32 == 8 || n % 32 == 24 ? n : ring_stride(n + 4); }
+__host__ constexpr size_t smem_bytes(int K, int Wi, int Ws) {
+    return ((size_t)3 * pw_smem_floats(K, K) + 24 * K + (size_t)K * ring_stride(ring_rows(G) * Ws) + (size_t)K * (2 * G + 1) * (Wi + 2))
+           * sizeof(float);
+}
+
+// dw3x3 + BN with the three rows of the stencil at p + row[0..2]: the operations of blk_kernel's stencils, in their order
+__device__ __forceinline__ float dw3_bn_rows(const float* p, const int (&row)[3], const float* w) {
+    float v = 0.f;
+#pragma unroll
+    for (int dy = 0; dy < 3; ++dy)
+#pragma unroll
+        for (int dx = 0; dx < 3; ++dx) v = fmaf(p[row[dy] + dx], w[dy * 3 + dx], v);
+    return fmaf(v, w[9], w[10]);
+}
+
+template <int K, int STRIDE>
+__global__ void __launch_bounds__(kThreads, 2)
+blk_kernel(const __grid_constant__ BlkArgs p) {
+    static_assert(STRIDE == 2, "the band walk runs stride-2 blocks");
+    pdl_trigger();
+    constexpr int KS = K / 8, NT = K / 8, S = w_stride(K), RX = ring_rows(G), RT = 2 * G + 1;
+    extern __shared__ __align__(16) float smem[];
+    float* sW1 = smem;
+    float* sW2 = sW1 + pw_smem_floats(K, K);
+    float* sWp = sW2 + pw_smem_floats(K, K);
+    float* sD = sWp + pw_smem_floats(K, K);               // main branch dw3x3/2: [K][12]
+    float* sDp = sD + 12 * K;                             // projection branch dw3x3/2
+    const Planes in = p.in, out = p.out;
+    const int Ws = in.Ws, CS = ring_stride(RX * Ws);
+    float* X = sDp + 12 * K;                              // [K][CS]: input row iy (-1 .. Hi, frame included) at X row (iy + 1) % RX
+    const int Wt = p.Wi + 2, plT = RT * Wt;
+    float* T = X + K * CS;                                // [K][RT][Wt]: pw1 row of input row iy at T row (iy + 1) % RT
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const unsigned short* tin = p.tin[0];
+
+    for (int i = threadIdx.x; i < K * RT; i += kThreads) { T[i * Wt] = 0.f; T[i * Wt + Wt - 1] = 0.f; }
+    load_pw_async(sW1, p.pw1[0], K);
+    load_pw_async(sW2, p.pw2[0], K);
+    load_pw_async(sWp, p.pwp, K);
+    load_floats_async(sD, p.dw[0], 12 * K);
+    load_floats_async(sDp, p.dwp, 12 * K);
+    cp_async_commit();
+    pdl_wait();
+
+    // input rows [iy0, iy0 + cnt) of image n -> X (plane row iy starts at (iy + 1) Ws: the frame is one pixel wide)
+    const int C4 = Ws / 4;
+    auto stage_rows = [&](int n, int iy0, int cnt) {
+        const float* ib = in.base + (long long)n * in.sN + (long long)(iy0 + 1) * Ws;
+        for (int i = threadIdx.x; i < K * cnt * C4; i += kThreads) {
+            const int kr = i / C4, c = 4 * (i - kr * C4), k = kr / cnt, r = kr - k * cnt;
+            cp16(X + k * CS + (iy0 + 1 + r) % RX * Ws + c, ib + (long long)tin[k] * in.sC + r * Ws + c);
+        }
+        cp_async_commit();
+    };
+
+    {
+        // this CTA's band: output rows [ys, ye) of image n
+        const int n = blockIdx.x / p.bands, ys = (blockIdx.x - n * p.bands) * p.R, ye = min(p.Ho, ys + p.R);
+        float* ob = out.base + (long long)n * out.sN;
+        stage_rows(n, 2 * ys - 1, 2 * min(G, ye - ys) + 1);
+        for (int y = ys; y < ye; y += G) {
+            const int rows = min(G, ye - y);
+            cp_async_wait<0>();
+            __syncthreads();      // this step's input rows have landed; the previous step is done with X and T
+            if (y + G < ye) stage_rows(n, 2 * (y + G), 2 * min(G, ye - y - G));
+            // pw1 + BN + ReLU -> T over the step's new input rows (the top halo row too in the band's first step); rows outside
+            // the map are the depthwise zero padding
+            const int r0 = y == ys ? 2 * y - 1 : 2 * y, M1 = (2 * y + 2 * rows - r0) * p.Wi;
+            for (int m0 = warp * 16; m0 < M1; m0 += kWarps * 16) {
+                int xo[2], to[2]; bool ok[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = m0 + g + 8 * h, r = m / p.Wi, c = m - r * p.Wi, iy = r0 + r;
+                    ok[h] = m < M1 && iy >= 0 && iy < p.Hi;
+                    xo[h] = (iy + 1) % RX * Ws + c + 1;
+                    to[h] = (iy + 1) % RT * Wt + c + 1;
+                }
+                float acc[NT][4];
+                warp_gemm<KS, NT>(acc, sW1, S, [&](int ks, float (&a)[4]) {
+                    const float* x0 = X + (8 * ks + t) * CS;
+                    const float* x1 = x0 + 4 * CS;
+                    a[0] = ok[0] ? x0[xo[0]] : 0.f;
+                    a[1] = ok[1] ? x0[xo[1]] : 0.f;
+                    a[2] = ok[0] ? x1[xo[0]] : 0.f;
+                    a[3] = ok[1] ? x1[xo[1]] : 0.f;
+                });
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (m0 + g + 8 * h >= M1) continue;
+#pragma unroll
+                    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = 8 * nt + 2 * t + e;
+                            const float v = fmaxf(fmaf(acc[nt][2 * h + e], sW1[K * S + col], sW1[K * S + K + col]), 0.f);
+                            T[col * plT + to[h]] = ok[h] ? v : 0.f;
+                        }
+                }
+            }
+            __syncthreads();
+            // even tiles: dw3x3/2 + BN from T -> pw2 + BN + ReLU -> planes K..2K-1 of the block;
+            // odd tiles: dw3x3/2 + BN from X -> pw + BN + ReLU -> planes 0..K-1
+            const int M2 = rows * p.Wo, tiles = (M2 + 15) / 16;
+            for (int tile = warp; tile < 2 * tiles; tile += kWarps) {
+                const bool proj = tile & 1;
+                const int m0 = (tile >> 1) * 16;
+                int row[2][3], oo[2]; bool ok[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = m0 + g + 8 * h, r = m / p.Wo, c = m - r * p.Wo, iy = 2 * (y + r) - 1;
+                    ok[h] = m < M2;
+#pragma unroll
+                    for (int dy = 0; dy < 3; ++dy)
+                        row[h][dy] = ok[h] ? (proj ? (iy + 1 + dy) % RX * Ws : (iy + 1 + dy) % RT * Wt) + 2 * c : 0;
+                    oo[h] = out.org + (y + r) * out.Ws + c;
+                }
+                const float* src = proj ? X : T;
+                const int ld = proj ? CS : plT;
+                const float* sw = proj ? sWp : sW2;
+                const float* sd = proj ? sDp : sD;
+                float acc[NT][4];
+                warp_gemm<KS, NT>(acc, sw, S, [&](int ks, float (&a)[4]) {
+#pragma unroll
+                    for (int q = 0; q < 2; ++q) {
+                        const int k = 8 * ks + t + 4 * q;
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const float v = dw3_bn_rows(src + k * ld, row[h], sd + 12 * k);
+                            a[2 * q + h] = ok[h] ? v : 0.f;
+                        }
+                    }
+                });
+                const unsigned short* tdst = proj ? p.tout[0] : p.tmain;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (!ok[h]) continue;
+#pragma unroll
+                    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = 8 * nt + 2 * t + e;
+                            ob[(long long)tdst[col] * out.sC + oo[h]] = fmaxf(fmaf(acc[nt][2 * h + e], sw[K * S + col], sw[K * S + K + col]), 0.f);
+                        }
+                }
+            }
+        }
+    }
+}
+}  // namespace walk
+
 // ---- stride-2 block on whole images -------------------------------------------------------------------------------------
 // When a CTA's 8 warps cover the output map with one 16-pixel tile each, the block runs per image instead of per band: all
 // five weight packs stay resident across the CTA's images (persistent grid), and T holds kS2Chunk pw1 channels at a time.
@@ -562,13 +734,33 @@ int run_blk(BlkArgs& a, int N, cudaStream_t s) {
     if (int rc = smem_attr(blk_kernel<K, STRIDE>, bytes)) return rc;
     int grid = a.items;
     // A stride-1 block keeps its weights resident in a persistent grid (K=96 at 352x352: 182 -> 120 us on an H100).  The
-    // stride-2 blocks were measured slower that way (stage4.0 610 -> 760 us, stage2.0 463 -> 488 us) and take one CTA per item.
+    // stride-2 blocks were measured slower that way (stage4.0 610 -> 760 us, stage2.0 463 -> 488 us) and take one CTA per item;
+    // K = 24 and 48 run on walk::blk_kernel wherever it fits.
     if (STRIDE == 1 && a.nblk == 1) {
         int per_sm = 0;
         YFV2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, blk_kernel<K, STRIDE>, kThreads, bytes));
         grid = persistent_grid(a.items, per_sm > 0 ? per_sm : 1);
     }
     YFV2_CUDA(launch_k(blk_kernel<K, STRIDE>, grid, kThreads, bytes, s, pdl_take(), a));
+    YFV2_LAUNCH_CHECK();
+    return YFV2_OK;
+}
+
+// The band walk stages whole plane rows by 16-byte copies from planes with a one-pixel frame; the plan's pool planes are such
+// planes, 16-byte aligned.  Wider maps, whose ring and T rows do not fit next to the weights, keep blk_kernel<K, 2>.
+bool blk_s2_walk_fits(int K, const Planes& in) {
+    return (K == 24 || K == 48) && in.pad == 1 && ((uintptr_t)in.base & 15) == 0 && in.Ws % 4 == 0 && in.sC % 4 == 0 &&
+           in.sN % 4 == 0 && walk::smem_bytes(K, in.W, in.Ws) <= kSmemCap;
+}
+
+template <int K>
+int run_blk_walk(BlkArgs& a, int N, cudaStream_t s) {
+    a.bands = (a.Ho + a.R - 1) / a.R;
+    a.items = N * a.bands;
+    auto kern = walk::blk_kernel<K, 2>;
+    const size_t bytes = walk::smem_bytes(K, a.Wi, a.in.Ws);
+    if (int rc = smem_attr(kern, bytes)) return rc;
+    YFV2_CUDA(launch_k(kern, a.items, kThreads, bytes, s, pdl_take(), a));         // one CTA per band
     YFV2_LAUNCH_CHECK();
     return YFV2_OK;
 }
@@ -869,6 +1061,7 @@ int blk_launch_s2(int K, const Planes& in, const Planes& out, const ChanTab& tin
     if (blk_s2_whole_image(K, out.H, out.W, in.W))      // K = 96
         return run_whole_image(blk_s2_image_kernel<96>, blk_s2_image_smem_bytes(K, out.H, in.W), a, N, s);
     a.R = blk_rows(K, 2, out.H, in.W, N);
+    if (blk_s2_walk_fits(K, in)) return K == 24 ? run_blk_walk<24>(a, N, s) : run_blk_walk<48>(a, N, s);
     switch (K) {
     case 24: return dispatch_blk<24>(2, a, N, s);
     case 48: return dispatch_blk<48>(2, a, N, s);
