@@ -278,6 +278,12 @@ YFV2_API int yfv2_forward_range(yfv2_plan* plan, const void* x, int is_u8, const
 YFV2_API int yfv2_debug_gather(const yfv2_plan* plan, const void* workspace, int which, float* out, int* dims4,
                                void* stream);
 
+/* ---- test hook: how a head launch of a forward on `workspace` reads its 5x5 depthwise taps ------------------------------
+ * which: 0 heads2.a, 1 heads2.b, 2 heads3.a, 3 heads3.b.  Returns 1 when the launch stages the input windows in shared memory,
+ * 0 when it reads the planes, < 0 on a bad argument (workspace NULL included: the choice depends on the plane addresses).
+ * Host only: workspace is not dereferenced. */
+YFV2_API int yfv2_debug_heads_staged(const yfv2_plan* plan, const void* workspace, int which);
+
 /* ---- test hook: one pointwise contraction on the tensor-core engine (3xTF32), out[n][p] = sum_k w[n][k]*x[k][p] ----
  * x: [K][P], w: [N][K], out: [N][P], pack_ws: unused (kept for ABI stability), may be NULL. */
 YFV2_API int yfv2_debug_pw_tc(const float* x, const float* w, float* out, float* pack_ws, int K, int N, int P,

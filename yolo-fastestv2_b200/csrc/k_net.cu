@@ -851,14 +851,42 @@ struct HeadArgs {
     float* dst[2][2];              // half 1: branch 0 -> obj rows [0, A), cls rows [A, A + C); branch 1 -> reg rows [0, 4A)
     int split[2], rowsA[2], rowsB[2];
     int N, H, W, chunks;
+    int CS;                        // staged path: channel stride of a window slot (floats); 0: the stencils read the planes
 };
 
 constexpr int kHeadTile = 96;      // output columns of one contraction of the second head half (12 n-tiles of 8)
+constexpr int kHeadSlots = 3;      // window slots of 8 channels (one k-step) in flight
+constexpr size_t kHeadBudget = 113 * 1024;     // two CTAs per SM (the cls and reg CTA of one blockIdx.x)
+
+// The staged path copies, per (item, k-step), the input rows [y0 - 2, y1 + 2] of the item's pixel rows [y0, y1] for 8 channels:
+// at most win rows of Ws floats per channel.  A run of 16 kWarps consecutive pixels spans at most this many map rows.
+__host__ __device__ constexpr int head_win_rows(int H, int W) {
+    return ((W - 1 + 16 * kWarps - 1) / W + 1 < H ? (W - 1 + 16 * kWarps - 1) / W + 1 : H) + 4;
+}
+__host__ constexpr size_t head_weight_bytes(int NP) { return ((size_t)pw_smem_floats(72, NP) + 72 * 28) * sizeof(float); }
 
 // half 0: dw5x5 + BN + ReLU -> pw + BN -> flat planes.  half 1: dw5x5 + BN + ReLU -> folded matrix + bias -> head tensors.
 // HALF 2 (head2_kernel) is half 1 for A + C > 96: the cls branch contracts the same A fragments, kept in registers, against two
 // 96-column tiles of a [192][72] folded matrix; the reg branch (4A <= 32 columns) keeps one tile.  It contracts 48 columns at a
 // time, so that the A fragments (36 registers) and one pass of accumulators (24) leave room for two CTAs per SM.
+//
+// The dw5x5 taps come from a window staged in shared memory where it fits (p.CS > 0, heads_launch): per k-step, the item's rows
+// with their 2-row halo for the k-step's 8 channels, whole framed rows by 16-byte cp.async into a ring of kHeadSlots slots.  The
+// copies of k-step j + 2 of the CTA's sequence (which runs on into its next item) are issued after the barrier of k-step j, when
+// every warp is done with the slot they overwrite; so every warp takes part in every k-step, pixels or not.  A slot keeps the
+// plane's row stride, and its channel stride is 8 or 24 modulo 32 words: the 4 t x 8 g lanes of a tap read hit 32 banks when the
+// fragment row's 8 pixels lie in one map row.  Where they straddle two map rows the offsets of the g lanes jump by Ws - W + 1
+// and t lanes can share a bank (1.25 wavefronts per tap read on average at 22x22, 1.56 at 11x11, 1.0 at 40x40).
+// Elsewhere the taps are read from the planes.  Both compute every value with the same operations in the same order.
+__device__ __forceinline__ float dw5_bn_relu(const float* tp, int ld, const float* w) {
+    float v = 0.f;
+#pragma unroll
+    for (int dy = 0; dy < 5; ++dy)
+#pragma unroll
+        for (int dx = 0; dx < 5; ++dx) v = fmaf(tp[dy * ld + dx], w[dy * 5 + dx], v);
+    return fmaxf(fmaf(v, w[25], w[26]), 0.f);
+}
+
 template <int HALF>
 __device__ __forceinline__ void head_body(const HeadArgs& p) {
     pdl_trigger();
@@ -867,6 +895,7 @@ __device__ __forceinline__ void head_body(const HeadArgs& p) {
     extern __shared__ __align__(16) float smem[];
     float* sW = smem;
     float* sD = sW + pw_smem_floats(72, NP);      // [72][28]: w[25] | scale | shift | 0
+    float* X = sD + 72 * 28;                      // staged path: [kHeadSlots][8][CS]
     const int br = blockIdx.y;
     const int tiles = HALF == 2 && br == 0 ? 2 : 1;
     if (HALF == 0) {
@@ -882,22 +911,61 @@ __device__ __forceinline__ void head_body(const HeadArgs& p) {
     }
     load_floats(sD, p.dw[br], 72 * 28);
     pdl_wait();
-    __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    const int HW = p.H * p.W;
-    const Planes in = p.in[br];
-    for (int item = blockIdx.x; item < p.N * p.chunks; item += gridDim.x) {
-        const int n = item / p.chunks, m0 = (item - n * p.chunks) * 16 * kWarps + 16 * warp;
-        if (m0 >= HW) continue;
-        int off[2]; bool ok[2];
+    const int HW = p.H * p.W, items = p.N * p.chunks, CS = p.CS;
+    const Planes& in = p.in[br];
+    // first pixel row of an item's chunk, and the floats per channel of its window
+    auto chunk_rows = [&](int chunk, int& y0, int& len) {
+        const int m = chunk * 16 * kWarps;
+        y0 = m / p.W;
+        len = ((min(HW, m + 16 * kWarps) - 1) / p.W - y0 + 5) * in.Ws;
+    };
+    // k-step j of this CTA's sequence (k-step j % 9 of its item j / 9) -> slot j % kHeadSlots; warp c copies channel c
+    auto stage = [&](int j) {
+        const int item = blockIdx.x + j / 9 * gridDim.x;
+        if (item < items) {
+            const int n = item / p.chunks;
+            int y0, len;
+            chunk_rows(item - n * p.chunks, y0, len);
+            const float* src = in.base + (long long)n * in.sN + (long long)(8 * (j % 9) + warp) * in.sC + (long long)y0 * in.Ws;
+            float* dst = X + (j % kHeadSlots * 8 + warp) * CS;
+            for (int o = 4 * lane; o < len; o += 128) cp16(dst + o, src + o);
+        }
+        cp_async_commit();
+    };
+    if (CS) {
+        for (int j = 0; j < kHeadSlots - 1; ++j) stage(j);
+    }
+    __syncthreads();
+    for (int item = blockIdx.x, j0 = 0; item < items; item += gridDim.x, j0 += 9) {
+        const int n = item / p.chunks, chunk = item - n * p.chunks, m0 = chunk * 16 * kWarps + 16 * warp;
+        if (!CS && m0 >= HW) continue;
+        int y0, len;
+        chunk_rows(chunk, y0, len);
+        int off[2]; bool ok[2];           // top-left tap in the window (staged) or in the plane
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int m = m0 + g + 8 * h, y = m / p.W, x = m - y * p.W;
             ok[h] = m < HW;
-            off[h] = ok[h] ? in.org + (y - 2) * in.Ws + x - 2 : in.org;
+            off[h] = CS ? (ok[h] ? (y - y0) * in.Ws + x : 0) : ok[h] ? in.org + (y - 2) * in.Ws + x - 2 : in.org;
         }
+        auto load_staged = [&](int ks, float (&a)[4]) {
+            cp_async_wait<kHeadSlots - 2>();
+            __syncthreads();          // k-step j0 + ks has landed; every warp is done with the slot k-step j0 + ks + 2 fills
+            stage(j0 + ks + kHeadSlots - 1);
+            const float* slot = X + (j0 + ks) % kHeadSlots * 8 * CS;
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+                const float* w = sD + 28 * (8 * ks + t + 4 * q);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const float v = dw5_bn_relu(slot + (t + 4 * q) * CS + off[h], in.Ws, w);
+                    a[2 * q + h] = ok[h] ? v : 0.f;
+                }
+            }
+        };
         const float* ib = in.base + (long long)n * in.sN;
-        auto load_a = [&](int ks, float (&a)[4]) {
+        auto load_planes = [&](int ks, float (&a)[4]) {
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
                 const int k = 8 * ks + t + 4 * q;
@@ -905,13 +973,8 @@ __device__ __forceinline__ void head_body(const HeadArgs& p) {
                 const float* pk = ib + (long long)k * in.sC;
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
-                    const float* tp = pk + off[h];
-                    float v = 0.f;
-#pragma unroll
-                    for (int dy = 0; dy < 5; ++dy)
-#pragma unroll
-                        for (int dx = 0; dx < 5; ++dx) v = fmaf(tp[dy * in.Ws + dx], w[dy * 5 + dx], v);
-                    a[2 * q + h] = ok[h] ? fmaxf(fmaf(v, w[25], w[26]), 0.f) : 0.f;
+                    const float v = dw5_bn_relu(pk + off[h], in.Ws, w);
+                    a[2 * q + h] = ok[h] ? v : 0.f;
                 }
             }
         };
@@ -940,30 +1003,36 @@ __device__ __forceinline__ void head_body(const HeadArgs& p) {
                     }
             }
         };
-        if constexpr (HALF < 2) {
-            float acc[NT][4];
-            warp_gemm<9, NT>(acc, sW, S, load_a);
-            store(acc, 0);
-        } else {
-            // The dw5x5 stencil (1800 FMAs per pixel) is computed once; each 96-column tile costs 324 MMAs per warp on it.
-            float af[9][4];
-#pragma unroll
-            for (int ks = 0; ks < 9; ++ks) load_a(ks, af[ks]);
-#pragma unroll 1
-            for (int c0 = 0; c0 < kHeadTile * tiles; c0 += 8 * NT) {
+        // one contraction per path, so that each keeps only its own operands in registers
+        auto contract = [&](auto&& load_a) {
+            if constexpr (HALF < 2) {
                 float acc[NT][4];
-                warp_gemm_regs<9, NT>(acc, sW + c0, S, af);
-                store(acc, c0);
+                warp_gemm<9, NT>(acc, sW, S, load_a);
+                store(acc, 0);
+            } else {
+                // The dw5x5 stencil (1800 FMAs per pixel) is computed once; each 96-column tile costs 324 MMAs per warp on it.
+                float af[9][4];
+#pragma unroll
+                for (int ks = 0; ks < 9; ++ks) load_a(ks, af[ks]);
+#pragma unroll 1
+                for (int c0 = 0; c0 < kHeadTile * tiles; c0 += 8 * NT) {
+                    float acc[NT][4];
+                    warp_gemm_regs<9, NT>(acc, sW + c0, S, af);
+                    store(acc, c0);
+                }
             }
-        }
+        };
+        if (CS) contract(load_staged);
+        else contract(load_planes);
     }
 }
 
+// Two CTAs per SM: 128 registers (half 1: 8 bytes of spill).  Left unbounded, ptxas gives the staged-window build 142 and 146.
 template <int HALF>
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kThreads, 2)
 head_kernel(const __grid_constant__ HeadArgs p) { head_body<HALF>(p); }
 
-// Two CTAs per SM, as half 1 gets on its own: 128 registers with 180 bytes of spill.  Left unbounded, ptxas gives it 144 registers
+// Two CTAs per SM: 128 registers with 16 bytes of spill.  Left unbounded (before the staged window), ptxas gave it 144 registers
 // and one CTA per SM, which measured slower on an H100 (150 classes, batch 256 @352x352: heads2.b 430 us against 363-379 us).
 __global__ void __launch_bounds__(kThreads, 2)
 head2_kernel(const __grid_constant__ HeadArgs p) { head_body<2>(p); }
@@ -1090,9 +1159,30 @@ int fpn_launch(int which, const Planes& c3, const ChanTab& t3, const Planes& c2,
     return which == 1 ? run(fpn_kernel<192>, 192) : run(fpn_kernel<288>, 288);
 }
 
+// weight columns of the kernel that runs head half `half`: 72 (head_kernel<0>), 96 (head_kernel<1>), 192 (head2_kernel); 0: none
+int head_columns(int half, int A, int C) {
+    if (half == 0) return 72;
+    if (A + C <= kHeadTile) return kHeadTile;
+    if (A + C <= 2 * kHeadTile && 4 * A <= kHeadTile) return 2 * kHeadTile;
+    return 0;
+}
+
+// The channel stride of a window slot where the staged window fits, else 0 (the stencils read the planes).  It fits when the planes
+// of both branches allow 16-byte copies of whole rows and kHeadSlots slots fit next to the weights within kHeadBudget.  Tall maps
+// of one or two columns (a chunk spans up to 16 kWarps rows) and very wide maps (one slot of 6 rows exceeds the budget) do not.
+int heads_window_stride(int half, const Planes& sIn, const Planes& tcls, const Planes& treg, int A, int C) {
+    const int np = head_columns(half, A, C);
+    const Planes* in[2] = {half ? &tcls : &sIn, half ? &treg : &sIn};
+    for (const Planes* q : in)
+        if (q->pad != 2 || ((uintptr_t)q->base & 15) || q->Ws % 4 || q->sC % 4 || q->sN % 4 || q->Ws != in[0]->Ws) return 0;
+    const int cs = walk::ring_stride(head_win_rows(in[0]->H, in[0]->W) * in[0]->Ws);
+    return np && head_weight_bytes(np) + (size_t)kHeadSlots * 8 * cs * sizeof(float) <= kHeadBudget ? cs : 0;
+}
+
 int heads_launch(int half, const Planes& sIn, const Planes& tcls, const Planes& treg, const float* const wdw[2], const float* const wpw[2],
                  float* reg, float* obj, float* cls, int A, int C, int N, cudaStream_t s) {
     HeadArgs a{};
+    a.CS = heads_window_stride(half, sIn, tcls, treg, A, C);
     for (int b = 0; b < 2; ++b) { a.dw[b] = wdw[b]; a.pw[b] = wpw[b]; }
     a.out[0] = tcls; a.out[1] = treg;
     if (half == 0) { a.in[0] = sIn; a.in[1] = sIn; }
@@ -1102,7 +1192,7 @@ int heads_launch(int half, const Planes& sIn, const Planes& tcls, const Planes& 
     a.N = N; a.H = sIn.H; a.W = sIn.W;
     a.chunks = (sIn.H * sIn.W + 16 * kWarps - 1) / (16 * kWarps);
     auto run = [&](auto kern, int np) -> int {
-        const size_t bytes = ((size_t)pw_smem_floats(72, np) + 72 * 28) * sizeof(float);
+        const size_t bytes = head_weight_bytes(np) + (size_t)kHeadSlots * 8 * a.CS * sizeof(float);
         if (int rc = smem_attr(kern, bytes)) return rc;
         cudaLaunchConfig_t cfg{};
         cfg.gridDim = dim3((unsigned)persistent_grid((long long)N * a.chunks, 1), 2);
@@ -1115,13 +1205,15 @@ int heads_launch(int half, const Planes& sIn, const Planes& tcls, const Planes& 
         YFV2_LAUNCH_CHECK();
         return YFV2_OK;
     };
-    if (half == 0) return run(head_kernel<0>, 72);
-    if (A + C <= kHeadTile) return run(head_kernel<1>, kHeadTile);
-    if (A + C <= 2 * kHeadTile && 4 * A <= kHeadTile) return run(head2_kernel, 2 * kHeadTile);
+    switch (head_columns(half, A, C)) {
+    case 72: return run(head_kernel<0>, 72);
+    case kHeadTile: return run(head_kernel<1>, kHeadTile);
+    case 2 * kHeadTile: return run(head2_kernel, 2 * kHeadTile);
+    }
     set_error("heads: anchors+classes = %d exceeds two %d-column output tiles", A + C, kHeadTile);
     return YFV2_EUNSUPPORTED;
 }
-static_assert((pw_smem_floats(72, 2 * kHeadTile) + 72 * 28) * sizeof(float) <= kSmemCap, "two head tiles must fit in shared memory");
+static_assert(head_weight_bytes(2 * kHeadTile) <= kSmemCap, "two head tiles must fit in shared memory");
 
 }  // namespace yfv2
 

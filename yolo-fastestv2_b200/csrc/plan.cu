@@ -472,6 +472,7 @@ int fpn_launch(int which, const Planes& c3, const ChanTab& t3, const Planes& c2,
                int N, cudaStream_t s);
 int heads_launch(int half, const Planes& sIn, const Planes& tcls, const Planes& treg, const float* const wdw[2], const float* const wpw[2],
                  float* reg, float* obj, float* cls, int A, int C, int N, cudaStream_t s);
+int heads_window_stride(int half, const Planes& sIn, const Planes& tcls, const Planes& treg, int A, int C);
 }
 
 namespace {
@@ -632,4 +633,15 @@ extern "C" int yfv2_debug_gather(const yfv2_plan* p, const void* workspace, int 
     gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(P, tab, Cn, out, total);
     YFV2_LAUNCH_CHECK();
     return YFV2_OK;
+}
+
+// ---- debug: does head launch `which` (heads2.a, heads2.b, heads3.a, heads3.b) stage its input windows? --------------------
+extern "C" int yfv2_debug_heads_staged(const yfv2_plan* p, const void* workspace, int which) {
+    if (!p || !workspace || which < 0 || which > 3) { set_error("debug_heads_staged: bad argument"); return YFV2_EINVAL; }
+    float* ws = (float*)workspace;
+    const int lv = which / 2, half = which % 2;
+    const Planes sIn = flat_planes(p, ws, lv ? p->off_s3 : p->off_s2, 2 + lv);
+    const Planes t_cls = flat_planes(p, ws, p->off_t[2 * lv], 2 + lv);
+    const Planes t_reg = flat_planes(p, ws, p->off_t[2 * lv + 1], 2 + lv);
+    return heads_window_stride(half, sIn, t_cls, t_reg, p->A, p->C) > 0 ? 1 : 0;
 }
