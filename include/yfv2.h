@@ -186,6 +186,45 @@ typedef struct yfv2_yuv420_frame {
 } yfv2_yuv420_frame;
 YFV2_API int yfv2_resize_yuv420_u8(const yfv2_yuv420_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
 
+/* ---- RGB, BGRA / RGBA, grey and planar RGB frames -> network input: cv2.cvtColor(COLOR_*2BGR) + cv2.resize INTER_LINEAR -------
+ * One descriptor for every 8-bit layout that is a channel move away from packed BGR: channel k of pixel (r, c) is the byte at
+ * ch_k + r*pitch + c*step, with ch_k = b, g, r.  Every such move commutes with the resize, so the result is the bytes of
+ * cv2.resize(cv2.cvtColor(frame, code), (W, H), INTER_LINEAR) for the code named below, with d the address of pixel (0,0):
+ *   BGR  (cv2.imread, no conversion)       b, g, r = d, d+1, d+2;  step 3      (yfv2_resize_bgr_u8 is 2.5 % faster for it)
+ *   RGB  (PIL, most PyTorch data code)     b, g, r = d+2, d+1, d;  step 3      COLOR_RGB2BGR
+ *   BGRA / BGRx (GStreamer, capture APIs)  b, g, r = d, d+1, d+2;  step 4      COLOR_BGRA2BGR (alpha ignored, as cv2 ignores it)
+ *   RGBA / RGBx                            b, g, r = d+2, d+1, d;  step 4      COLOR_RGBA2BGR
+ *   grey (IR / mono cameras)               b, g, r = d, d, d;      step 1      COLOR_GRAY2BGR
+ *   planar CHW RGB (GPU JPEG decoders)     b, g, r = d+2s, d+s, d; step 1      transpose + COLOR_RGB2BGR (s: the channel stride)
+ * frames: N HOST descriptors of frames in device memory; one batch may mix sizes, pitches and layouts.  Needs b, g, r non-null,
+ * w, h > 0, step >= 1, pitch >= step*w and step*w < 2^31.  dst, H, W: as yfv2_resize_bgr_u8.  Descriptors are checked before
+ * anything is launched. */
+typedef struct yfv2_strided_frame {
+    const uint8_t* b;      /* device pointer to the B byte of pixel (0,0) */
+    const uint8_t* g;      /* ... the G byte */
+    const uint8_t* r;      /* ... the R byte */
+    long long pitch;       /* bytes from one row to the next, for all three channels */
+    int step;              /* bytes from one pixel to the next along a row */
+    int w, h;              /* size in pixels */
+} yfv2_strided_frame;
+YFV2_API int yfv2_resize_strided_u8(const yfv2_strided_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
+
+/* ---- packed YUV 4:2:2 frames -> network input: cv2.cvtColor(COLOR_YUV2BGR_YUYV / _UYVY / _YVYU) + cv2.resize INTER_LINEAR ---
+ * What USB (V4L2 YUYV) webcams and HDMI / SDI capture cards (UYVY) deliver.  Two pixels share one 4-byte macropixel: the luma of
+ * pixel (r, c) is at y + r*pitch + 2c, and the U and V of the pair (r, 2j), (r, 2j + 1) at u + r*pitch + 4j and v + r*pitch + 4j:
+ *   YUYV (YUY2): y = d, u = d+1, v = d+3;   UYVY: u = d, y = d+1, v = d+2;   YVYU: y = d, v = d+1, u = d+3.
+ * Each pixel is converted with the BT.601 limited-range fixed point of yfv2_resize_yuv420_u8 (chroma not interpolated), which is
+ * what cv2.cvtColor does for these codes.  Needs y, u, v non-null, w even and > 0 (cv2 asserts an even width), h > 0 (odd allowed),
+ * pitch >= 2*w.  frames, dst, H, W: as yfv2_resize_strided_u8. */
+typedef struct yfv2_yuv422_frame {
+    const uint8_t* y;      /* device pointer to the luma of pixel (0,0) */
+    const uint8_t* u;      /* device pointer to the U of pixels (0,0), (0,1) */
+    const uint8_t* v;      /* device pointer to the V of pixels (0,0), (0,1) */
+    long long pitch;       /* bytes from one row to the next */
+    int w, h;              /* size in pixels, w even */
+} yfv2_yuv422_frame;
+YFV2_API int yfv2_resize_yuv422_u8(const yfv2_yuv422_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
+
 /* ---- whole inference step with HOST buffers (the evaluation() inner loop, utils/utils.py:367-383) ----
  * x_host: pinned uint8 [N,3,H,W]; out_host: pinned [N,max_det,6]; counts_host: pinned [N].
  * Copies in, runs forward_u8 + decode_nms, copies out, all on `stream`; returns without synchronising. */

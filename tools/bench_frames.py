@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Raw-frame inference: device resize (yfv2_resize_bgr_u8) + forward + fused decode/NMS from 1920x1080 BGR frames resident in HBM.
 
-  python tools/bench_frames.py [--steps K --warmup W --batch 256 --frame 1920x1080 --runs 2 --layout bgr|nv12|i420]
+  python tools/bench_frames.py [--steps K --warmup W --batch 256 --frame 1920x1080 --runs 2 --layout bgr|nv12|i420|rgb|...]
 
 Same network, weights (Detector default init under seed 1), target size and NMS thresholds as bench.py.  Two frame batches
 (2 x 1.6 GB at batch 256) are alternated so that no step reads its frames from the 50 MB L2.  Prints one JSON line with, per run:
@@ -14,10 +14,12 @@ columns of each output pixel) plus the planar output written.  `h2d_ms_per_batch
 batch: frames that start on the host are bound by that copy (about 6.2 MB per frame), not by the kernel.
 
 --layout nv12 | i420 feeds the steps YUV 4:2:0 frames of the same size (cv2's single [h*3/2, w] buffer) through
-yfv2_resize_yuv420_u8 instead.  Each run then also times the BGR resize of the same frame size (bgr_resize_us), alternated launch
-by launch with the YUV resize, each after an L2 flush; the touched bytes count the sectors of the luma and chroma rows the YUV
-resize reads; `h2d_ms_per_batch` is the pinned copy of a YUV batch (1.5 bytes per pixel) next to `h2d_bgr_ms_per_batch`; and the
-parity check runs tests/yuv_oracle.py on frames 0 and N-1."""
+yfv2_resize_yuv420_u8 instead; --layout rgb | bgra | rgba | gray | rgb_chw feeds contiguous frames of that layout through
+yfv2_resize_strided_u8, and --layout yuyv | uyvy | yvyu packed 4:2:2 frames through yfv2_resize_yuv422_u8.  Each run then also
+times the BGR resize of the same frame size (bgr_resize_us), alternated launch by launch with the layout's resize, each after an
+L2 flush; the touched bytes count the sectors of the rows (and planes) the layout's resize reads; `h2d_ms_per_batch` is the pinned
+copy of a batch in that layout next to `h2d_bgr_ms_per_batch`; and the parity check runs tests/layout_oracle.py on frames 0 and
+N-1."""
 import argparse
 import ctypes
 import json
@@ -64,6 +66,53 @@ def touched_bytes_yuv420(h, w, H, W, layout):
     return 32 * len(np.unique(np.concatenate(addr) // 32)) + 3 * H * W
 
 
+def touched_bytes_layout(h, w, H, W, layout):
+    """The same count for one contiguous frame of a strided or packed 4:2:2 layout: the sectors of the bytes the kernel reads for
+    the two rows and two columns of each output pixel (three channel bytes; for 4:2:2 the luma and the macropixel's U and V),
+    plus the bytes it writes."""
+    from oracle import resize as ore
+    import layout_oracle as lo
+    sx, _, _ = ore.coeffs(w, W, True)
+    sy, _, _ = ore.coeffs(h, H, False)
+    cols = np.unique(np.concatenate([sx, np.minimum(sx + 1, w - 1)]))[None, :]
+    rows = np.unique(np.clip(np.concatenate([sy, sy + 1]), 0, h - 1))[:, None]
+    if layout == "rgb_chw":
+        addr = [p * h * w + rows * w + cols for p in range(3)]
+    elif layout in lo.MACROPIXEL:
+        oy, ou, _, ov = lo.MACROPIXEL[layout]
+        addr = [rows * 2 * w + 2 * cols + oy, rows * 2 * w + 4 * (cols >> 1) + ou, rows * 2 * w + 4 * (cols >> 1) + ov]
+    else:
+        step = {"rgb": 3, "bgra": 4, "rgba": 4, "gray": 1}[layout]
+        addr = [rows * step * w + step * cols + o for o in ((0,) if layout == "gray" else (0, 1, 2))]
+    return 32 * len(np.unique(np.concatenate([a.reshape(-1) for a in addr]) // 32)) + 3 * H * W
+
+
+def layout_descs(fb, layout):
+    """Descriptors of a [N, ...] batch of contiguous frames of a strided or packed 4:2:2 layout, and the entry that takes them."""
+    import yfv2_engine as eng
+    N = fb.shape[0]
+    if layout in eng.YUV422_LAYOUTS:
+        d = (eng.Yuv422Frame * N)()
+        oy, ou, ov = eng._YUV422_OFFSETS[layout]
+        for i in range(N):
+            p = fb[i].data_ptr()
+            d[i].y, d[i].u, d[i].v, d[i].pitch, d[i].h, d[i].w = p + oy, p + ou, p + ov, fb[i].stride(0), fb.shape[1], fb.shape[2]
+        return d, eng.lib().yfv2_resize_yuv422_u8
+    d = (eng.StridedFrame * N)()
+    for i in range(N):
+        p = fb[i].data_ptr()
+        if layout == "rgb_chw":
+            s = fb[i].stride(0)
+            d[i].b, d[i].g, d[i].r, d[i].pitch, d[i].step = p + 2 * s, p + s, p, fb[i].stride(1), 1
+            d[i].h, d[i].w = fb.shape[2], fb.shape[3]
+        else:
+            ob, og, or_ = eng._BGR_OFFSETS[layout]
+            step = 1 if layout == "gray" else fb.shape[3]
+            d[i].b, d[i].g, d[i].r, d[i].pitch, d[i].step = p + ob, p + og, p + or_, fb[i].stride(0), step
+            d[i].h, d[i].w = fb.shape[1], fb.shape[2]
+    return d, eng.lib().yfv2_resize_strided_u8
+
+
 def yuv420_descs(fb, layout):
     """Descriptors of a [N, h*3/2, w] batch of single-buffer NV12 or I420 frames."""
     import yfv2_engine as eng
@@ -97,7 +146,8 @@ def main():
     ap.add_argument("--batch", type=int, default=256)
     ap.add_argument("--frame", default="1920x1080", help="source frame WxH")
     ap.add_argument("--runs", type=int, default=2, help="measurement runs, alternated within one process")
-    ap.add_argument("--layout", default="bgr", choices=("bgr", "nv12", "i420"), help="source frame format")
+    ap.add_argument("--layout", default="bgr", choices=("bgr", "nv12", "i420", "rgb", "bgra", "rgba", "gray", "rgb_chw", "yuyv",
+                                                        "uyvy", "yvyu"), help="source frame format")
     args = ap.parse_args()
     import yfv2  # noqa: F401
     import yfv2_engine as eng
@@ -123,11 +173,19 @@ def main():
         for i in range(N):
             d[i].data, d[i].w, d[i].h, d[i].pitch = fb[i].data_ptr(), fw, fh, fb[i].stride(0)
         descs.append(d)
-    yuv = args.layout != "bgr"
-    if yuv:
-        import yuv_oracle as yo
-        yframes = [torch.randint(0, 256, (N, fh * 3 // 2, fw), generator=g, dtype=torch.uint8, device=dev) for _ in range(2)]
-        ydescs = [yuv420_descs(fb, args.layout) for fb in yframes]
+    other = args.layout != "bgr"
+    yuv420 = args.layout in ("nv12", "i420")
+    if other:
+        import layout_cases as lc
+        import layout_oracle as lo
+        shape = (fh * 3 // 2, fw) if yuv420 else lc.frame_shape(args.layout, fh, fw)
+        yframes = [torch.randint(0, 256, (N,) + shape, generator=g, dtype=torch.uint8, device=dev) for _ in range(2)]
+        if yuv420:
+            ydescs = [yuv420_descs(fb, args.layout) for fb in yframes]
+            yentry = L.yfv2_resize_yuv420_u8
+        else:
+            ydescs = [layout_descs(fb, args.layout)[0] for fb in yframes]
+            yentry = layout_descs(yframes[0][:1], args.layout)[1]
     x = torch.empty((N, 3, S, S), dtype=torch.uint8, device=dev)
     plan = model._plan_for(x)
     preds = plan.alloc_preds()
@@ -141,12 +199,12 @@ def main():
         if rc:
             raise RuntimeError(L.yfv2_last_error())
 
-    def resize_yuv():
-        rc = L.yfv2_resize_yuv420_u8(ydescs[it[0] % 2], N, S, S, ctypes.c_void_p(x.data_ptr()), sp)
+    def resize_other():
+        rc = yentry(ydescs[it[0] % 2], N, S, S, ctypes.c_void_p(x.data_ptr()), sp)
         if rc:
             raise RuntimeError(L.yfv2_last_error())
 
-    resize = resize_yuv if yuv else resize_bgr
+    resize = resize_other if other else resize_bgr
 
     def detect():
         plan.forward(x, preds)
@@ -165,17 +223,18 @@ def main():
         step()
     torch.cuda.synchronize(dev)
     # parity of the timed path's resize: first and last frame of the batch the last warm-up step resized, against the oracle
-    last = (yframes if yuv else frames)[(it[0] - 1) % 2]
+    last = (yframes if other else frames)[(it[0] - 1) % 2]
     for i in (0, N - 1):
         src = last[i].cpu().numpy()
-        want = yo.resize_frame_planar(src, args.layout, S, S) if yuv else ore.resize_bgr_planar(src, S, S)
+        want = lo.resize_planar(src, args.layout, S, S) if other else ore.resize_bgr_planar(src, S, S)
         if not np.array_equal(x[i].cpu().numpy(), want):
             raise AssertionError("bench_frames parity: resized frame %d differs from the oracle" % i)
 
     flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)     # 256 MB > L2
     per_frame = touched_bytes(fh, fw, S, S, frames[0][0].stride(0))
-    if yuv:
-        per_frame_bgr, per_frame = per_frame, touched_bytes_yuv420(fh, fw, S, S, args.layout)
+    if other:
+        per_frame_bgr, per_frame = per_frame, (touched_bytes_yuv420(fh, fw, S, S, args.layout) if yuv420 else
+                                               touched_bytes_layout(fh, fw, S, S, args.layout))
     peak, peak_src = bench.measured_peak()
     sampler = bench.ClockSampler(0)
     sampler.start()
@@ -188,7 +247,7 @@ def main():
             flush.zero_()
             it[0] += 1
             tot += events_ms(resize, 1, stream)
-            if yuv:                      # the BGR resize of the same frame size, alternated launch by launch
+            if other:                      # the BGR resize of the same frame size, alternated launch by launch
                 flush.zero_()
                 tot_bgr += events_ms(resize_bgr, 1, stream)
         us = 1e3 * tot / reps
@@ -197,7 +256,7 @@ def main():
                      "images_per_s": round(N * args.steps / (ms_step * 1e-3), 1), "resize_us": round(us, 2),
                      "resize_share_of_step": round(us * 1e-3 / (ms_step / args.steps), 4),
                      "resize_GBps": round(gbs, 1), "resize_frac": round(gbs / peak, 4)})
-        if yuv:
+        if other:
             us_bgr = 1e3 * tot_bgr / reps
             runs[-1].update({"bgr_resize_us": round(us_bgr, 2),
                              "bgr_resize_GBps": round(N * per_frame_bgr / (us_bgr * 1e-6) / 1e9, 1)})
@@ -206,9 +265,9 @@ def main():
 
     host = torch.empty((N, fh, fw, 3), dtype=torch.uint8, pin_memory=True)
     h2d = [events_ms(lambda: frames[0].copy_(host, non_blocking=True), 1, stream) for _ in range(3)]
-    if yuv:
+    if other:
         del host
-        yhost = torch.empty((N, fh * 3 // 2, fw), dtype=torch.uint8, pin_memory=True)
+        yhost = torch.empty((N,) + shape, dtype=torch.uint8, pin_memory=True)
         h2d_bgr, h2d = h2d, [events_ms(lambda: yframes[0].copy_(yhost, non_blocking=True), 1, stream) for _ in range(3)]
     power = None
     try:
@@ -228,14 +287,15 @@ def main():
                         % (N, N * fh * fw * 3 / 1e6),
             "parity": "resized frames 0 and %d equal the oracle (oracle/resize.py) byte for byte" % (N - 1),
             "kept_boxes_per_step": int(counts.sum().item())}
-    if yuv:
+    if other:
         line["metric"] = "images/sec %dx%d %s frames -> resize + fwd + decode + NMS at %dx%d" % (fw, fh, args.layout.upper(), S, S)
-        line.update({"layout": args.layout, "frame_bytes": fh * fw * 3 // 2, "bgr_frame_bytes": fh * fw * 3,
+        frame_bytes = int(np.prod(shape))
+        line.update({"layout": args.layout, "frame_bytes": frame_bytes, "bgr_frame_bytes": fh * fw * 3,
                      "bgr_resize_touched_bytes_per_frame": per_frame_bgr, "h2d_bgr_ms_per_batch": round(min(h2d_bgr), 3),
                      "timing": line["timing"] + "; bgr_resize_us: the BGR resize of the same frame size, alternated with it",
                      "h2d_note": "one pinned host->device copy of %d %s frames (%.1f MB); h2d_bgr_ms_per_batch: the same frames as BGR "
-                                 "(%.1f MB)" % (N, args.layout.upper(), N * fh * fw * 1.5 / 1e6, N * fh * fw * 3 / 1e6),
-                     "parity": "resized frames 0 and %d equal the oracle (tests/yuv_oracle.py) byte for byte" % (N - 1)})
+                                 "(%.1f MB)" % (N, args.layout.upper(), N * frame_bytes / 1e6, N * fh * fw * 3 / 1e6),
+                     "parity": "resized frames 0 and %d equal the oracle (tests/layout_oracle.py) byte for byte" % (N - 1)})
     print(json.dumps(line), flush=True)
 
 

@@ -1,10 +1,14 @@
 // Raw-frame resize: cv2.resize(img, (W, H), interpolation=cv2.INTER_LINEAR) (the host step of test.py:35 and
 // utils/datasets.py:107), written straight into the [N,3,H,W] planar uint8 batch yfv2_forward_u8 consumes (test.py:36-37:
-// res_img.transpose(2, 0, 1)).  Two sources share one kernel body, a template over the source-pixel fetch:
-//   packed HWC BGR frames (yfv2_resize_bgr_u8), and
-//   YUV 4:2:0 frames (yfv2_resize_yuv420_u8: NV12 / NV21 / I420 / YV12), each source pixel converted to BGR exactly as
-//   cv2.cvtColor(COLOR_YUV2BGR_*) does (OpenCV's ITUR_BT_601 fixed point, limited range, chroma not interpolated):
-//     uu = U[r>>1][c>>1] - 128, vv = V[r>>1][c>>1] - 128, y = max(0, Y[r][c] - 16) * 1220542 + (1 << 19)
+// res_img.transpose(2, 0, 1)).  Four sources share one kernel body, a template over the source-pixel fetch:
+//   packed HWC BGR frames (yfv2_resize_bgr_u8);
+//   strided frames (yfv2_resize_strided_u8): channel k of pixel (r, c) at ch_k + r * pitch + c * step, which states packed
+//   RGB / BGRA / RGBA, grey and planar RGB alike (each a channel move away from BGR, and channel moves commute with the resize);
+//   YUV 4:2:0 frames (yfv2_resize_yuv420_u8: NV12 / NV21 / I420 / YV12) and packed YUV 4:2:2 frames (yfv2_resize_yuv422_u8:
+//   YUYV / UYVY / YVYU), each source pixel converted to BGR exactly as cv2.cvtColor(COLOR_YUV2BGR_*) does (OpenCV's ITUR_BT_601
+//   fixed point, limited range, chroma not interpolated; (U, V) is the sample of the pixel's 2x2 block for 4:2:0, of its
+//   two-pixel macropixel for 4:2:2):
+//     uu = U - 128, vv = V - 128, y = max(0, Y[r][c] - 16) * 1220542 + (1 << 19)
 //     B = sat_u8((y + 2116026 uu) >> 20), G = sat_u8((y - 852492 vv - 409993 uu) >> 20), R = sat_u8((y + 1673527 vv) >> 20).
 // The resize is bit-identical to OpenCV's x86 8-bit path, all integer after the coefficients:
 //   coefficients per axis: f = fl32((d + 0.5) * (n / m) - 0.5) (product and difference rounded in double), s = floor(f),
@@ -12,10 +16,12 @@
 //     along y the weights keep the unclamped fraction and the two rows are clamped.
 //   horizontal: S = src[sx] * a0 + src[min(sx + 1, w - 1)] * a1 (int32, per channel)
 //   vertical:   out = sat_u8((((S0 >> 4) * b0 >> 16) + ((S1 >> 4) * b1 >> 16) + 2) >> 2)
-// oracle/resize.py restates the resize in numpy, tests/yuv_oracle.py the colour conversion.  One thread per output pixel (all
-// three channels); a warp covers 32 consecutive x of one row, so each plane store of a warp is one contiguous 32-byte run.  The
-// coefficients are recomputed per thread (four double operations): cheaper than a table round trip, and the call needs no
-// workspace.
+// oracle/resize.py restates the resize in numpy, tests/yuv_oracle.py the colour conversion and tests/layout_oracle.py the channel
+// moves.  One thread per output pixel (all three channels); a warp covers 32 consecutive x of one row, so each plane store of a
+// warp is one contiguous 32-byte run.  The coefficients are recomputed per thread (four double operations): cheaper than a table
+// round trip, and the call needs no workspace.
+#include <climits>
+
 #include "common.cuh"
 
 namespace yfv2 {
@@ -24,10 +30,12 @@ namespace {
 constexpr int kResizeBx = 64, kResizeBy = 4;
 constexpr int kResizeMaxSide = 32768;
 
-// Packed HWC BGR: pixel (r, c) is the three bytes at data + r * pitch + 3c.
+// Packed HWC BGR: pixel (r, c) is the three bytes at data + r * pitch + 3c.  StridedSource states this layout too, but is 2.5 %
+// slower on it (DESIGN.md §7), so BGR keeps its own fetch.
 struct BgrSource {
     using Desc = yfv2_frame;
     static constexpr int kChunk = 128;   // frames per launch: their 24-byte descriptors travel as kernel parameters (3 KB)
+    static constexpr int kMinBlocks = 0;
     const uint8_t* row;
     __device__ __forceinline__ BgrSource(const yfv2_frame& f, int r) : row(f.data + (long long)r * f.pitch) {}
     // B, G, R of pixels (r, c0) and (r, c1)
@@ -40,9 +48,32 @@ struct BgrSource {
     }
 };
 
+// Strided: channel k of pixel (r, c) at ch_k + r * pitch + c * step (B, G, R).  Packed BGR / RGB / BGRA / RGBA, grey and planar
+// RGB differ only in the descriptor's values, so nothing here branches on the layout.
+struct StridedSource {
+    using Desc = yfv2_strided_frame;
+    static constexpr int kChunk = 80;    // 48-byte descriptors: 3.75 KB of kernel parameters, under the 4 KB launch limit
+    static constexpr int kMinBlocks = 8;
+    const uint8_t* ch[3];
+    int step;
+    __device__ __forceinline__ StridedSource(const yfv2_strided_frame& f, int r) : step(f.step) {
+        const long long off = (long long)r * f.pitch;
+        ch[0] = f.b + off; ch[1] = f.g + off; ch[2] = f.r + off;
+    }
+    // B, G, R of pixels (r, c0) and (r, c1)
+    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
+        const int k0 = c0 * step, k1 = c1 * step;     // step * w < 2^31, checked on the host
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            p0[c] = __ldg(ch[c] + k0);
+            p1[c] = __ldg(ch[c] + k1);
+        }
+    }
+};
+
 __device__ __forceinline__ int sat_u8(int v) { return min(max(v, 0), 255); }
 
-// cv2.cvtColor's YUV 4:2:0 -> BGR of one pixel (OpenCV ITUR_BT_601: 20-bit fixed point, limited range)
+// cv2.cvtColor's YUV -> BGR of one pixel, 4:2:0 and 4:2:2 alike (OpenCV ITUR_BT_601: 20-bit fixed point, limited range)
 __device__ __forceinline__ void yuv_to_bgr(int y, int uu, int vv, int (&bgr)[3]) {
     const int yy = max(0, y - 16) * 1220542 + (1 << 19);
     bgr[0] = sat_u8((yy + 2116026 * uu) >> 20);
@@ -55,6 +86,7 @@ __device__ __forceinline__ void yuv_to_bgr(int y, int uu, int vv, int (&bgr)[3])
 struct Yuv420Source {
     using Desc = yfv2_yuv420_frame;
     static constexpr int kChunk = 64;    // 56-byte descriptors: 3.5 KB of kernel parameters, under the 4 KB launch limit
+    static constexpr int kMinBlocks = 0;
     const uint8_t* luma;
     const uint8_t* u;
     const uint8_t* v;
@@ -69,6 +101,29 @@ struct Yuv420Source {
         if (k1 != k0) { u1 = __ldg(u + k1) - 128; v1 = __ldg(v + k1) - 128; }   // c0, c1 in different chroma columns
         yuv_to_bgr(__ldg(luma + c0), u0, v0, p0);
         yuv_to_bgr(__ldg(luma + c1), u1, v1, p1);
+    }
+};
+
+// Packed YUV 4:2:2: luma of (r, c) at y + r * pitch + 2c; U and V of the macropixel (r, 2j), (r, 2j + 1) at u / v + r * pitch + 4j.
+// YUYV, UYVY and YVYU differ only in the three pointers.
+struct Yuv422Source {
+    using Desc = yfv2_yuv422_frame;
+    static constexpr int kChunk = 96;    // 40-byte descriptors: 3.75 KB of kernel parameters
+    static constexpr int kMinBlocks = 8;
+    const uint8_t* luma;
+    const uint8_t* u;
+    const uint8_t* v;
+    __device__ __forceinline__ Yuv422Source(const yfv2_yuv422_frame& f, int r) {
+        const long long off = (long long)r * f.pitch;
+        luma = f.y + off; u = f.u + off; v = f.v + off;
+    }
+    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
+        const int k0 = (c0 >> 1) * 4, k1 = (c1 >> 1) * 4;
+        const int u0 = __ldg(u + k0) - 128, v0 = __ldg(v + k0) - 128;
+        int u1 = u0, v1 = v0;
+        if (k1 != k0) { u1 = __ldg(u + k1) - 128; v1 = __ldg(v + k1) - 128; }   // c0, c1 in different macropixels
+        yuv_to_bgr(__ldg(luma + 2 * c0), u0, v0, p0);
+        yuv_to_bgr(__ldg(luma + 2 * c1), u1, v1, p1);
     }
 };
 
@@ -90,8 +145,10 @@ __device__ __forceinline__ float src_coord(int d, int n, int m, int& s) {
 __device__ __forceinline__ int weight0(float f) { return __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f)); }
 __device__ __forceinline__ int weight1(float f) { return __float2int_rn(__fmul_rn(f, 2048.f)); }
 
+// Src::kMinBlocks 8 holds a fetch to 32 registers (the strided fetch's three row pointers take 34 unbounded), so an SM keeps its
+// full 2048 threads in flight: the kernel waits on DRAM, not on issue.  BGR and 4:2:0 use 32 registers unbounded (0: no bound).
 template <class Src>
-__global__ void __launch_bounds__(kResizeBx * kResizeBy)
+__global__ void __launch_bounds__(kResizeBx * kResizeBy, Src::kMinBlocks)
 resize_kernel(const __grid_constant__ ResizeChunk<Src> a) {
     const int x = blockIdx.x * kResizeBx + threadIdx.x;
     const int y = blockIdx.y * kResizeBy + threadIdx.y;
@@ -143,16 +200,22 @@ int launch_resize(const typename Src::Desc* frames, int N, int H, int W, uint8_t
     return YFV2_OK;
 }
 
+// The checks every entry makes on its call before it looks at the frames.
+bool bad_call(const char* fn, const void* frames, int N, int H, int W, const uint8_t* dst) {
+    if (!frames || !dst || N <= 0) { set_error("%s: null frames / dst or N <= 0", fn); return true; }
+    if (H <= 0 || W <= 0 || H > kResizeMaxSide || W > kResizeMaxSide) {
+        set_error("%s: target %dx%d outside 1..%d", fn, W, H, kResizeMaxSide);
+        return true;
+    }
+    return false;
+}
+
 }  // namespace
 }  // namespace yfv2
 
 extern "C" int yfv2_resize_bgr_u8(const yfv2_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
     using namespace yfv2;
-    if (!frames || !dst || N <= 0) { set_error("resize_bgr_u8: null frames / dst or N <= 0"); return YFV2_EINVAL; }
-    if (H <= 0 || W <= 0 || H > kResizeMaxSide || W > kResizeMaxSide) {
-        set_error("resize_bgr_u8: target %dx%d outside 1..%d", W, H, kResizeMaxSide);
-        return YFV2_EINVAL;
-    }
+    if (bad_call("resize_bgr_u8", frames, N, H, W, dst)) return YFV2_EINVAL;
     for (int n = 0; n < N; ++n) {
         const yfv2_frame& f = frames[n];
         if (!f.data || f.w <= 0 || f.h <= 0 || f.pitch < 3LL * f.w) {
@@ -166,11 +229,7 @@ extern "C" int yfv2_resize_bgr_u8(const yfv2_frame* frames, int N, int H, int W,
 
 extern "C" int yfv2_resize_yuv420_u8(const yfv2_yuv420_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
     using namespace yfv2;
-    if (!frames || !dst || N <= 0) { set_error("resize_yuv420_u8: null frames / dst or N <= 0"); return YFV2_EINVAL; }
-    if (H <= 0 || W <= 0 || H > kResizeMaxSide || W > kResizeMaxSide) {
-        set_error("resize_yuv420_u8: target %dx%d outside 1..%d", W, H, kResizeMaxSide);
-        return YFV2_EINVAL;
-    }
+    if (bad_call("resize_yuv420_u8", frames, N, H, W, dst)) return YFV2_EINVAL;
     for (int n = 0; n < N; ++n) {
         const yfv2_yuv420_frame& f = frames[n];
         const char* why = nullptr;
@@ -186,4 +245,42 @@ extern "C" int yfv2_resize_yuv420_u8(const yfv2_yuv420_frame* frames, int N, int
         }
     }
     return launch_resize<Yuv420Source>(frames, N, H, W, dst, stream);
+}
+
+extern "C" int yfv2_resize_strided_u8(const yfv2_strided_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
+    using namespace yfv2;
+    if (bad_call("resize_strided_u8", frames, N, H, W, dst)) return YFV2_EINVAL;
+    for (int n = 0; n < N; ++n) {
+        const yfv2_strided_frame& f = frames[n];
+        const char* why = nullptr;
+        if (!f.b || !f.g || !f.r) why = "null channel pointer";
+        else if (f.w <= 0 || f.h <= 0) why = "w and h must be > 0";
+        else if (f.step < 1) why = "step must be >= 1";
+        else if ((long long)f.step * f.w > INT_MAX) why = "step * w must be < 2^31";
+        else if (f.pitch < (long long)f.step * f.w) why = "pitch < step * w";
+        if (why) {
+            set_error("resize_strided_u8: frame %d: %s (b %p, g %p, r %p, %dx%d, pitch %lld, step %d)", n, why, (const void*)f.b,
+                      (const void*)f.g, (const void*)f.r, f.w, f.h, f.pitch, f.step);
+            return YFV2_EINVAL;
+        }
+    }
+    return launch_resize<StridedSource>(frames, N, H, W, dst, stream);
+}
+
+extern "C" int yfv2_resize_yuv422_u8(const yfv2_yuv422_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
+    using namespace yfv2;
+    if (bad_call("resize_yuv422_u8", frames, N, H, W, dst)) return YFV2_EINVAL;
+    for (int n = 0; n < N; ++n) {
+        const yfv2_yuv422_frame& f = frames[n];
+        const char* why = nullptr;
+        if (!f.y || !f.u || !f.v) why = "null plane pointer";
+        else if (f.w <= 0 || f.h <= 0 || (f.w & 1)) why = "w must be even and > 0, h > 0";
+        else if (f.pitch < 2LL * f.w) why = "pitch < 2 * w";
+        if (why) {
+            set_error("resize_yuv422_u8: frame %d: %s (y %p, u %p, v %p, %dx%d, pitch %lld)", n, why, (const void*)f.y,
+                      (const void*)f.u, (const void*)f.v, f.w, f.h, f.pitch);
+            return YFV2_EINVAL;
+        }
+    }
+    return launch_resize<Yuv422Source>(frames, N, H, W, dst, stream);
 }

@@ -34,6 +34,18 @@ class Yuv420Frame(ctypes.Structure):
                 ("uv_pitch", ctypes.c_longlong), ("uv_step", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int)]
 
 
+class StridedFrame(ctypes.Structure):
+    """yfv2_strided_frame: channel k of pixel (r, c) at ch_k + r*pitch + c*step (RGB, BGRA / RGBA, grey, planar RGB)."""
+    _fields_ = [("b", ctypes.c_void_p), ("g", ctypes.c_void_p), ("r", ctypes.c_void_p), ("pitch", ctypes.c_longlong),
+                ("step", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int)]
+
+
+class Yuv422Frame(ctypes.Structure):
+    """yfv2_yuv422_frame: one packed YUV 4:2:2 source frame (YUYV / UYVY / YVYU) in device memory."""
+    _fields_ = [("y", ctypes.c_void_p), ("u", ctypes.c_void_p), ("v", ctypes.c_void_p), ("pitch", ctypes.c_longlong),
+                ("w", ctypes.c_int), ("h", ctypes.c_int)]
+
+
 # name -> (restype, argtypes); must list every prototype of include/yfv2.h (tests check this)
 PROTOTYPES = {
     "yfv2_abi_version": (ctypes.c_int, []),
@@ -68,6 +80,10 @@ PROTOTYPES = {
     "yfv2_resize_bgr_u8": (ctypes.c_int, [ctypes.POINTER(Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                           ctypes.c_void_p]),
     "yfv2_resize_yuv420_u8": (ctypes.c_int, [ctypes.POINTER(Yuv420Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                             ctypes.c_void_p]),
+    "yfv2_resize_strided_u8": (ctypes.c_int, [ctypes.POINTER(StridedFrame), ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                              ctypes.c_void_p, ctypes.c_void_p]),
+    "yfv2_resize_yuv422_u8": (ctypes.c_int, [ctypes.POINTER(Yuv422Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                              ctypes.c_void_p]),
     "yfv2_detect_u8_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                            ctypes.POINTER(ctypes.c_double), ctypes.c_float, ctypes.c_double, ctypes.c_int,
@@ -599,6 +615,156 @@ def resize_yuv420(frames, W, H, layout, device=None, out=None):
         d.y, d.y_pitch, d.h, d.w = y.data_ptr(), y.stride(0), y.shape[0], y.shape[1]
     with torch.cuda.device(device):
         _check(lib().yfv2_resize_yuv420_u8(descs, N, H, W, ctypes.c_void_p(out.data_ptr()), _stream(device)), "resize_yuv420_u8")
+    return out
+
+
+# Layouts yfv2_resize_strided_u8 takes: the byte offsets of B, G, R within a pixel of each packed one, and the number of bytes
+# per pixel of each packed one.  "rgb_chw" ([3, h, w], R plane first) is built from its channel stride instead.
+STRIDED_LAYOUTS = ("rgb", "bgra", "rgba", "gray", "rgb_chw")
+_BGR_OFFSETS = {"rgb": (2, 1, 0), "bgra": (0, 1, 2), "rgba": (2, 1, 0), "gray": (0, 0, 0)}
+# packed YUV 4:2:2 (yfv2_resize_yuv422_u8): the byte offsets of the first Y, of U and of V within a 4-byte macropixel
+YUV422_LAYOUTS = ("yuyv", "uyvy", "yvyu")
+_YUV422_OFFSETS = {"yuyv": (0, 1, 3), "uyvy": (1, 0, 2), "yvyu": (0, 3, 1)}
+_CHANNELS = {"rgb": 3, "bgra": 4, "rgba": 4, "yuyv": 2, "uyvy": 2, "yvyu": 2}
+LAYOUTS = ("bgr",) + YUV420_LAYOUTS + STRIDED_LAYOUTS + YUV422_LAYOUTS
+# the entry point (descriptor kind) of each layout
+_KIND = dict([("bgr", "bgr")] + [(k, "yuv420") for k in YUV420_LAYOUTS] + [(k, "strided") for k in STRIDED_LAYOUTS]
+             + [(k, "yuv422") for k in YUV422_LAYOUTS])
+
+
+def frame_size(frame, layout):
+    """(h, w) in pixels of a frame in the given layout, as resize_frames takes it."""
+    if layout in YUV420_LAYOUTS:
+        if isinstance(frame, (tuple, list)):
+            return tuple(frame[0].shape[:2])
+        return frame.shape[0] // 3 * 2, frame.shape[1]
+    return tuple(frame.shape[1:3]) if layout == "rgb_chw" else tuple(frame.shape[:2])
+
+
+def _layout_frame(f, layout, i):
+    """Frame i of a strided or 4:2:2 layout as a uint8 tensor of the layout's shape, checked, not copied."""
+    shape = ("[3, h, w]" if layout == "rgb_chw" else "[h, w]" if layout == "gray" else "[h, w, %d]" % _CHANNELS[layout])
+    if not isinstance(f, torch.Tensor):
+        import numpy as np
+        f = np.asarray(f)
+        if f.dtype != np.uint8:
+            raise Yfv2Error("resize_frames: frame %d (%s) must be uint8 %s, got %s %s" % (i, layout, shape, f.dtype, f.shape))
+        f = torch.from_numpy(f if min(f.strides, default=0) >= 0 else np.ascontiguousarray(f))
+    ok = f.dtype == torch.uint8 and f.dim() == (2 if layout == "gray" else 3) and f.numel() > 0
+    if ok and layout == "rgb_chw":
+        ok = f.shape[0] == 3
+    elif ok and layout != "gray":
+        ok = f.shape[2] == _CHANNELS[layout]
+    if not ok:
+        raise Yfv2Error("resize_frames: frame %d (%s) must be uint8 %s with h, w > 0, got %s %s"
+                        % (i, layout, shape, f.dtype, tuple(f.shape)))
+    if layout in YUV422_LAYOUTS and f.shape[1] % 2:
+        raise Yfv2Error("resize_frames: frame %d (%s): 4:2:2 needs an even width (two pixels per macropixel), got w = %d"
+                        % (i, layout, f.shape[1]))
+    return f
+
+
+def _check_frame(f, layout, i):
+    """Checks frame i against its layout without launching anything; returns what the layout's resize takes."""
+    kind = _KIND[layout]
+    if kind == "bgr":
+        if isinstance(f, torch.Tensor):
+            ok = f.dtype == torch.uint8
+        else:
+            import numpy as np
+            f = np.asarray(f)
+            ok = f.dtype == np.uint8
+        if not ok or f.ndim != 3 or f.shape[2] != 3:
+            raise Yfv2Error("resize_frames: frame %d (bgr) must be uint8 [h, w, 3], got %s %s" % (i, f.dtype, tuple(f.shape)))
+        return f
+    if kind == "yuv420":
+        _yuv420_planes(f, layout, i)
+        return f
+    return _layout_frame(f, layout, i)
+
+
+def _resize_layout_run(frames, layouts, W, H, device, out):
+    """One yfv2_resize_strided_u8 or yfv2_resize_yuv422_u8 call for checked frames of one descriptor kind."""
+    N = len(frames)
+    strided = _KIND[layouts[0]] == "strided"
+    descs = ((StridedFrame if strided else Yuv422Frame) * N)()
+    keep = []          # device copies stay referenced until the launch is queued: a freed block could take the next frame's copy
+    for d, f, lay in zip(descs, frames, layouts):
+        f = f.to(device)
+        if lay == "rgb_chw":                                 # any channel and row stride, unit column stride
+            if f.stride(2) != 1 or f.stride(1) < f.shape[2]:
+                f = f.contiguous()
+            p, s = f.data_ptr(), f.stride(0)
+            d.b, d.g, d.r, d.pitch, d.step = p + 2 * s, p + s, p, f.stride(1), 1
+            d.h, d.w = f.shape[1], f.shape[2]
+        else:
+            step = 1 if lay == "gray" else _CHANNELS[lay]
+            if f.stride(1) != step or (lay != "gray" and f.stride(2) != 1) or f.stride(0) < step * f.shape[1]:
+                f = f.contiguous()
+            p = f.data_ptr()
+            if strided:
+                ob, og, or_ = _BGR_OFFSETS[lay]
+                d.b, d.g, d.r, d.step = p + ob, p + og, p + or_, step
+            else:
+                oy, ou, ov = _YUV422_OFFSETS[lay]
+                d.y, d.u, d.v = p + oy, p + ou, p + ov
+            d.pitch, d.h, d.w = f.stride(0), f.shape[0], f.shape[1]
+        keep.append(f)
+    fn, what = ((lib().yfv2_resize_strided_u8, "resize_strided_u8") if strided else
+                (lib().yfv2_resize_yuv422_u8, "resize_yuv422_u8"))
+    with torch.cuda.device(device):
+        _check(fn(descs, N, H, W, ctypes.c_void_p(out.data_ptr()), _stream(device)), what)
+
+
+def resize_frames(frames, W, H, layout, device=None, out=None):
+    """cv2.resize(cv2.cvtColor(frame, code), (W, H), interpolation=cv2.INTER_LINEAR) of every frame, transposed to the
+    [N, 3, H, W] uint8 batch the network takes, bit for bit, for every frame layout the library reads.  layout: one name, or a
+    list with one name per frame (one batch may mix layouts and sizes):
+      "bgr"                             [h, w, 3], no conversion (as resize_bgr)
+      "nv12" | "nv21" | "i420" | "yv12" cv2's [h*3/2, w] buffer or its planes, COLOR_YUV2BGR_<LAYOUT> (as resize_yuv420)
+      "rgb"                             [h, w, 3], COLOR_RGB2BGR
+      "bgra" | "rgba"                   [h, w, 4], COLOR_BGRA2BGR / COLOR_RGBA2BGR (alpha ignored)
+      "gray"                            [h, w], COLOR_GRAY2BGR
+      "rgb_chw"                         [3, h, w] planar RGB (torchvision's decode_jpeg): transpose + COLOR_RGB2BGR
+      "yuyv" | "uyvy" | "yvyu"          [h, w, 2] packed 4:2:2 (w even), COLOR_YUV2BGR_<LAYOUT>
+    Frames are numpy arrays or CUDA tensors; CUDA views with larger row strides or crop offsets are read in place (for
+    "rgb_chw" any channel and row stride with unit column stride), host arrays are copied to `device`.  Consecutive frames of
+    one descriptor kind go to one call (yfv2_resize_bgr_u8 / _yuv420_u8 / _strided_u8 / _yuv422_u8), each into its slice of
+    `out`.  Every frame is checked before anything is copied or launched."""
+    frames = list(frames)
+    layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
+    for lay in layouts if layouts else [layout]:
+        if not isinstance(lay, str) or lay not in LAYOUTS:
+            raise Yfv2Error("resize_frames: layout must be one of %s, got %r" % (", ".join(LAYOUTS), lay))
+    if not frames:
+        raise Yfv2Error("resize_frames: no frames")
+    if len(layouts) != len(frames):
+        raise Yfv2Error("resize_frames: %d layouts for %d frames" % (len(layouts), len(frames)))
+    checked = [_check_frame(f, lay, i) for i, (f, lay) in enumerate(zip(frames, layouts))]
+    if device is None:
+        cuda = [t.device for f in checked for t in (f if isinstance(f, (tuple, list)) else (f,))
+                if isinstance(t, torch.Tensor) and t.is_cuda]
+        device = cuda[0] if cuda else torch.device("cuda", torch.cuda.current_device())
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise Yfv2Error("resize_frames: runs on CUDA devices only (no CPU fallback)")
+    N = len(frames)
+    if out is None:
+        out = torch.empty((N, 3, H, W), dtype=torch.uint8, device=device)
+    elif tuple(out.shape) != (N, 3, H, W) or out.dtype != torch.uint8 or not out.is_contiguous() or out.device != device:
+        raise Yfv2Error("resize_frames: out must be a contiguous uint8 tensor of shape %s on %s" % ((N, 3, H, W), device))
+    i = 0
+    while i < N:
+        kind, j = _KIND[layouts[i]], i + 1
+        while j < N and _KIND[layouts[j]] == kind:
+            j += 1
+        if kind == "bgr":
+            resize_bgr(checked[i:j], W, H, device, out[i:j])
+        elif kind == "yuv420":
+            resize_yuv420(checked[i:j], W, H, layouts[i:j], device, out[i:j])
+        else:
+            _resize_layout_run(checked[i:j], layouts[i:j], W, H, device, out[i:j])
+        i = j
     return out
 
 
