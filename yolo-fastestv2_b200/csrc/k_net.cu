@@ -92,6 +92,7 @@ struct BlkArgs {
     unsigned short tin[kMaxChain][96];
     unsigned short tout[kMaxChain][96];        // stride 2: projection branch output (channels 0..K-1 of the block)
     unsigned short tmain[96];                  // stride 2: main branch output (channels K..2K-1)
+    int G;                                     // walk::blk_kernel<K, 1>: output rows per step
 };
 
 __host__ __device__ constexpr int blk_rin(int stride, int R) { return stride * (R - 1) + 3; }
@@ -313,7 +314,7 @@ __device__ __forceinline__ float dw3_bn_rows(const float* p, const int (&row)[3]
 template <int K, int STRIDE>
 __global__ void __launch_bounds__(kThreads, 2)
 blk_kernel(const __grid_constant__ BlkArgs p) {
-    static_assert(STRIDE == 2, "the band walk runs stride-2 blocks");
+    static_assert(STRIDE == 2, "blk_kernel<K, 1> is specialised below");
     pdl_trigger();
     constexpr int KS = K / 8, NT = K / 8, S = w_stride(K), RX = ring_rows(G), RT = 2 * G + 1;
     extern __shared__ __align__(16) float smem[];
@@ -443,6 +444,165 @@ blk_kernel(const __grid_constant__ BlkArgs p) {
         }
     }
 }
+
+// ---- stride-1 block: bands walked in steps of rows by a persistent grid -----------------------------------------------------
+// A single K = 24 / 48 stride-1 block (stage2.1-3, stage3.1-7) keeps the bands of blk_rows and the persistent grid of
+// blk_kernel<K, 1>, and walks each band G output rows at a time (G = BlkArgs::G, chosen by the host from the map width):
+//   * pw1, pw2 and the dw pack are loaded once per CTA by 16-byte cp.async, issued before pdl_wait and resident for the launch.
+//   * Input rows are staged whole (frame columns included) by 16-byte cp.async into a ring X of 2G + 2 rows per channel, in the
+//     order the CTA consumes them (X row j of the CTA's sequence at slot j % (2G + 2)).  The copies of step s + 1 are issued
+//     before step s computes; in an item's last step they are the first rows of the CTA's next item, when both fit in the ring.
+//   * A step runs pw1 + BN + ReLU over its new input rows into a ring T of G + 2 pw1 rows (the band's first step also over the
+//     row above and the row below the step), a barrier, then dw3x3 + BN from T as the A operand of pw2 + BN + ReLU -> planes.
+//   * Pass k of the persistent loop takes item k gridDim + blockIdx.x for even k and k gridDim + gridDim - 1 - blockIdx.x for odd
+//     k, so a CTA that takes a band of an image's tall head in one pass takes a short tail band in the next.
+// Every value is computed with the operations of blk_kernel<K, 1> in their order, so the outputs are bit-identical to it.
+__host__ __device__ constexpr int s1_ring_rows(int G) { return 2 * G + 2; }
+__host__ constexpr size_t s1_smem_bytes(int K, int G, int Wi, int Ws) {
+    return ((size_t)2 * pw_smem_floats(K, K) + 12 * K + (size_t)K * ring_stride(s1_ring_rows(G) * Ws) + (size_t)K * (G + 2) * (Wi + 2))
+           * sizeof(float);
+}
+
+template <int K>
+__device__ __forceinline__ void blk_s1_walk(const BlkArgs& p) {
+    pdl_trigger();
+    constexpr int KS = K / 8, NT = K / 8, S = w_stride(K);
+    extern __shared__ __align__(16) float smem[];
+    float* sW1 = smem;
+    float* sW2 = sW1 + pw_smem_floats(K, K);
+    float* sD = sW2 + pw_smem_floats(K, K);               // [K][12]: w[9] | scale | shift | 0
+    const Planes in = p.in, out = p.out;
+    const int Gs = p.G, RX = s1_ring_rows(Gs), RT = Gs + 2, Ws = in.Ws, CS = ring_stride(RX * Ws);
+    float* X = sD + 12 * K;                               // [K][CS]: X row j of the CTA's sequence at row j % RX
+    const int Wt = p.Wi + 2, plT = RT * Wt;
+    float* T = X + K * CS;                                // [K][RT][Wt]: pw1 row of input row iy at T row (iy + 1) % RT
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const unsigned short* tin = p.tin[0];
+    const unsigned short* tout = p.tout[0];
+
+    for (int i = threadIdx.x; i < K * RT; i += kThreads) { T[i * Wt] = 0.f; T[i * Wt + Wt - 1] = 0.f; }
+    load_pw_async(sW1, p.pw1[0], K);
+    load_pw_async(sW2, p.pw2[0], K);
+    load_floats_async(sD, p.dw[0], 12 * K);
+    cp_async_commit();
+    pdl_wait();
+
+    // input rows [iy0, iy0 + cnt) of image n -> X rows seq0 .. seq0 + cnt - 1 of the sequence; rows outside the map are not
+    // copied (pw1 writes zeros for them).  Plane row iy starts at (iy + 1) Ws: the frame is one pixel wide.
+    const int C4 = Ws / 4;
+    auto stage_rows = [&](int n, int iy0, int cnt, int seq0) {
+        const float* ib = in.base + (long long)n * in.sN + (long long)(iy0 + 1) * Ws;
+        for (int i = threadIdx.x; i < K * cnt * C4; i += kThreads) {
+            const int kr = i / C4, c = 4 * (i - kr * C4), k = kr / cnt, r = kr - k * cnt;
+            if (iy0 + r >= 0 && iy0 + r < p.Hi) cp16(X + k * CS + (seq0 + r) % RX * Ws + c, ib + (long long)tin[k] * in.sC + r * Ws + c);
+        }
+        cp_async_commit();
+    };
+    auto item_of = [&](int pass) { return pass * (int)gridDim.x + (pass & 1 ? gridDim.x - 1 - blockIdx.x : blockIdx.x); };
+    // the first step of band `item` reads its input rows [ys - 1, ys + rows + 1)
+    auto first_rows = [&](int item, int& n, int& ys, int& ye) {
+        n = item / p.bands; ys = (item - n * p.bands) * p.R; ye = min(p.Ho, ys + p.R);
+        return min(Gs, ye - ys) + 2;
+    };
+
+    int sb = 0, na = 0;         // sequence index of the current step's first X row; X rows in flight for the next step (0: none)
+    for (int pass = 0, item = item_of(0); item < p.items; item = item_of(++pass)) {
+        int n, ys, ye;
+        const int a0 = first_rows(item, n, ys, ye);
+        if (na == 0) { na = a0; stage_rows(n, ys - 1, a0, sb); }      // not issued by the previous item's last step
+        float* ob = out.base + (long long)n * out.sN;
+        for (int y = ys; y < ye; y += Gs) {
+            const int rows = min(Gs, ye - y), r0 = y == ys ? y - 1 : y + 1, a = na;    // X rows sb .. sb + a - 1: input rows r0 ..
+            cp_async_wait<0>();
+            __syncthreads();      // this step's input rows have landed; the previous step is done with X and T
+            na = 0;
+            if (y + Gs < ye) {
+                na = min(Gs, ye - y - Gs);
+                stage_rows(n, y + Gs + 1, na, sb + a);
+            } else if (item_of(pass + 1) < p.items) {
+                int n2, ys2, ye2;
+                const int a2 = first_rows(item_of(pass + 1), n2, ys2, ye2);
+                if (a + a2 <= RX) { na = a2; stage_rows(n2, ys2 - 1, a2, sb + a); }
+            }
+            // pw1 + BN + ReLU -> T over the step's input rows; rows outside the map are the depthwise zero padding
+            const int M1 = a * p.Wi;
+            for (int m0 = warp * 16; m0 < M1; m0 += kWarps * 16) {
+                int xo[2], to[2]; bool ok[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = m0 + g + 8 * h, r = m / p.Wi, c = m - r * p.Wi, iy = r0 + r;
+                    ok[h] = m < M1 && iy >= 0 && iy < p.Hi;
+                    xo[h] = (sb + r) % RX * Ws + c + 1;
+                    to[h] = (iy + 1) % RT * Wt + c + 1;
+                }
+                float acc[NT][4];
+                warp_gemm<KS, NT>(acc, sW1, S, [&](int ks, float (&a)[4]) {
+                    const float* x0 = X + (8 * ks + t) * CS;
+                    const float* x1 = x0 + 4 * CS;
+                    a[0] = ok[0] ? x0[xo[0]] : 0.f;
+                    a[1] = ok[1] ? x0[xo[1]] : 0.f;
+                    a[2] = ok[0] ? x1[xo[0]] : 0.f;
+                    a[3] = ok[1] ? x1[xo[1]] : 0.f;
+                });
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (m0 + g + 8 * h >= M1) continue;
+#pragma unroll
+                    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = 8 * nt + 2 * t + e;
+                            const float v = fmaxf(fmaf(acc[nt][2 * h + e], sW1[K * S + col], sW1[K * S + K + col]), 0.f);
+                            T[col * plT + to[h]] = ok[h] ? v : 0.f;
+                        }
+                }
+            }
+            __syncthreads();
+            // dw3x3 + BN from T as the A operand -> pw2 + BN + ReLU -> output planes
+            const int M2 = rows * p.Wo;
+            for (int m0 = warp * 16; m0 < M2; m0 += kWarps * 16) {
+                int row[2][3], oo[2]; bool ok[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = m0 + g + 8 * h, r = m / p.Wo, c = m - r * p.Wo;
+                    ok[h] = m < M2;
+#pragma unroll
+                    for (int dy = 0; dy < 3; ++dy) row[h][dy] = ok[h] ? (y + r + dy) % RT * Wt + c : 0;
+                    oo[h] = out.org + (y + r) * out.Ws + c;
+                }
+                float acc[NT][4];
+                warp_gemm<KS, NT>(acc, sW2, S, [&](int ks, float (&a)[4]) {
+#pragma unroll
+                    for (int q = 0; q < 2; ++q) {
+                        const int k = 8 * ks + t + 4 * q;
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const float v = dw3_bn_rows(T + k * plT, row[h], sD + 12 * k);
+                            a[2 * q + h] = ok[h] ? v : 0.f;
+                        }
+                    }
+                });
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (!ok[h]) continue;
+#pragma unroll
+                    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = 8 * nt + 2 * t + e;
+                            ob[(long long)tout[col] * out.sC + oo[h]] = fmaxf(fmaf(acc[nt][2 * h + e], sW2[K * S + col], sW2[K * S + K + col]), 0.f);
+                        }
+                }
+            }
+            sb += a;
+        }
+    }
+}
+
+template <>
+__global__ void __launch_bounds__(kThreads, 2) blk_kernel<24, 1>(const __grid_constant__ BlkArgs p) { blk_s1_walk<24>(p); }
+template <>
+__global__ void __launch_bounds__(kThreads, 2) blk_kernel<48, 1>(const __grid_constant__ BlkArgs p) { blk_s1_walk<48>(p); }
 }  // namespace walk
 
 // ---- stride-2 block on whole images -------------------------------------------------------------------------------------
@@ -753,14 +913,34 @@ bool blk_s2_walk_fits(int K, const Planes& in) {
            in.sN % 4 == 0 && walk::smem_bytes(K, in.W, in.Ws) <= kSmemCap;
 }
 
-template <int K>
+// The stride-1 walk takes the largest step of at most s1_step_max(K) rows whose rings fit next to the weights within
+// kS1WalkBudget (two CTAs per SM), on the same planes as the stride-2 walk; 0 where no step fits (past 158 columns at K = 24, 62
+// at K = 48) and for K = 96, which keep blk_kernel<K, 1>.  The caps are the fastest steps measured at 352x352 (DESIGN.md §5):
+// 4 rows at K = 24 (44 columns), 3 at K = 48 (22 columns).
+constexpr size_t kS1WalkBudget = 113 * 1024;
+constexpr int s1_step_max(int K) { return K == 24 ? 4 : 3; }
+int blk_s1_walk_step(int K, const Planes& P) {
+    if (!((K == 24 || K == 48) && P.pad == 1 && ((uintptr_t)P.base & 15) == 0 && P.Ws % 4 == 0 && P.sC % 4 == 0 && P.sN % 4 == 0))
+        return 0;
+    for (int G = s1_step_max(K); G >= 1; --G)
+        if (walk::s1_smem_bytes(K, G, P.W, P.Ws) <= kS1WalkBudget) return G;
+    return 0;
+}
+
+template <int K, int STRIDE>
 int run_blk_walk(BlkArgs& a, int N, cudaStream_t s) {
     a.bands = (a.Ho + a.R - 1) / a.R;
     a.items = N * a.bands;
-    auto kern = walk::blk_kernel<K, 2>;
-    const size_t bytes = walk::smem_bytes(K, a.Wi, a.in.Ws);
+    auto kern = walk::blk_kernel<K, STRIDE>;
+    const size_t bytes = STRIDE == 2 ? walk::smem_bytes(K, a.Wi, a.in.Ws) : walk::s1_smem_bytes(K, a.G, a.Wi, a.in.Ws);
     if (int rc = smem_attr(kern, bytes)) return rc;
-    YFV2_CUDA(launch_k(kern, a.items, kThreads, bytes, s, pdl_take(), a));         // one CTA per band
+    int grid = a.items;       // stride 2: one CTA per band; stride 1: the persistent grid of blk_kernel<K, 1>
+    if (STRIDE == 1) {
+        int per_sm = 0;
+        YFV2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, bytes));
+        grid = persistent_grid(a.items, per_sm > 0 ? per_sm : 1);
+    }
+    YFV2_CUDA(launch_k(kern, grid, kThreads, bytes, s, pdl_take(), a));
     YFV2_LAUNCH_CHECK();
     return YFV2_OK;
 }
@@ -1110,6 +1290,7 @@ int blk_launch_s1(int K, const Planes& P, int nblk, const ChanTab* tin, const Ch
     }
     const size_t bytes = blk_smem_bytes(K, 1, P.H, P.W);
     if (nblk > 1 && bytes > kChainBudget) return run_whole_image(blk_chain_kernel<96>, bytes, a, N, s);   // K = 96 (chainable)
+    if (nblk == 1 && (a.G = blk_s1_walk_step(K, P)) > 0) return K == 24 ? run_blk_walk<24, 1>(a, N, s) : run_blk_walk<48, 1>(a, N, s);
     switch (K) {
     case 24: return dispatch_blk<24>(1, a, N, s);
     case 48: return dispatch_blk<48>(1, a, N, s);
@@ -1130,7 +1311,7 @@ int blk_launch_s2(int K, const Planes& in, const Planes& out, const ChanTab& tin
     if (blk_s2_whole_image(K, out.H, out.W, in.W))      // K = 96
         return run_whole_image(blk_s2_image_kernel<96>, blk_s2_image_smem_bytes(K, out.H, in.W), a, N, s);
     a.R = blk_rows(K, 2, out.H, in.W, N);
-    if (blk_s2_walk_fits(K, in)) return K == 24 ? run_blk_walk<24>(a, N, s) : run_blk_walk<48>(a, N, s);
+    if (blk_s2_walk_fits(K, in)) return K == 24 ? run_blk_walk<24, 2>(a, N, s) : run_blk_walk<48, 2>(a, N, s);
     switch (K) {
     case 24: return dispatch_blk<24>(2, a, N, s);
     case 48: return dispatch_blk<48>(2, a, N, s);
