@@ -131,6 +131,35 @@ YFV2_API int yfv2_decode_nms(const float* const preds[6], int N, int H, int W, i
                     const int* class_filter, int n_filter, int max_det, float max_wh,
                     float* out, int* counts, int* kept_idx, void* workspace, void* stream);
 
+/* ---- detections of regions (tiles, zones) of frames -> one list per frame in frame pixels: a cross-region NMS --------------
+ * No reference counterpart: the reference detects on whole images (test.py:34-68).  Region t is a crop (x0, y0, w, h) of frame
+ * `frame`, stretched to the W x H network input; dets [T, max_det_in, 6] / counts [T] are its rows as yfv2_nms / yfv2_decode_nms
+ * write them (x1, y1, x2, y2, conf, cls in network-input pixels; the first min(max(counts[t], 0), max_det_in) rows are read).
+ * regions: T HOST descriptors, the regions of one frame contiguous and frame indices ascending (a frame may have none).
+ * Per frame, bit-exact to tests/region_oracle.py:
+ *   1. mapping: sx = (double)w / W, sy = (double)h / H, x' = x*sx + x0, y' = y*sy + y0, each a rounded fp64 product then a
+ *      rounded fp64 sum (no FMA); conf and cls are copied.  With x0 = y0 = 0 this is the x * (w / W) of test.py:57-68.
+ *   2. order: conf descending, ties by region t, then by row; rows whose conf is NaN are dropped.
+ *   3. greedy: walking that order, row j is kept unless an already kept row i has t(i) != t(j) (rows of one region were already
+ *      separated by its own NMS), the same cls, and overlap(i, j) > thr.
+ *   4. overlap in fp64, no +1: inter = max(0, min(x2) - max(x1)) * max(0, min(y2) - max(y1)), area = (x2 - x1) * (y2 - y1),
+ *      with min(a, b) = a < b ? a : b, max(a, b) = a > b ? a : b and a = the kept row's value; metric 0 (IoU):
+ *      inter / (area_i + area_j - inter), metric 1 (IoS): inter / min(area_i, area_j).  A NaN overlap never suppresses.
+ *   5. at most max_det rows per frame.
+ * out: [F, max_det, 6] float64 in that order (rows past out_counts[f]: zeros); out_counts [F]; kept_src (optional, may be NULL):
+ * [F, max_det] t * max_det_in + row of each kept row (-1 past the count).  Checked before any launch (YFV2_EINVAL, naming the bad
+ * region or argument): non-null pointers, T, F, W, H >= 1, 1 <= max_det_in, max_det <= 4096, metric 0 or 1, thr not NaN,
+ * T * max_det_in < 2^31; per region w, h >= 1, x0, y0 >= 0, frame in [0, F) and not decreasing; per frame its regions x
+ * max_det_in <= YFV2_NMS_MAX_CAND and at most YFV2_MERGE_MAX_REGIONS regions.  No workspace. */
+#define YFV2_MERGE_MAX_REGIONS 1024
+typedef struct yfv2_region {
+    int frame;             /* index of the frame the region belongs to */
+    int x0, y0, w, h;      /* the crop, in pixels of that frame */
+} yfv2_region;
+YFV2_API int yfv2_merge_regions(const float* dets, const int* counts, const yfv2_region* regions, int T, int max_det_in, int F,
+                                int H, int W, double thr, int metric, int max_det, double* out, int* out_counts, int* kept_src,
+                                void* stream);
+
 /* ---- get_batch_statistics (utils/utils.py:184-230): true-positive flags of NMS output rows ----------------
  * dets [N,max_det,6] / counts [N] as yfv2_nms writes them; targets [nt,6] rows (image, class, x1, y1, x2, y2) in
  * pixels (what evaluation() builds at utils/utils.py:372-375), nt <= 8192.  tp [N,max_det] receives 1.0 for a true

@@ -11,9 +11,14 @@
 // in fp32 compared as double against the threshold, stable descending order (ties by original row),
 // and no FMA contraction anywhere in that arithmetic — every step uses the __f*_rn intrinsics.
 #include <float.h>
+#include <limits.h>
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+
+#include <algorithm>
+#include <memory>
+#include <new>
 
 #include "common.cuh"
 
@@ -444,6 +449,21 @@ __device__ void bitonic_sort_desc_reg(unsigned long long* keys) {
 #pragma unroll
     for (int m = 0; m < E; ++m) keys[E * t + m] = v[m];
     __syncthreads();
+}
+
+// Sorts the first `cnt` keys descending: pads them with zeros to n2 = the power of two >= max(cnt, 64) (the buffer must hold n2)
+// and runs the register network for 256..2048 keys, the shared-memory one otherwise.  All threads of the CTA call this.
+// (sort_and_suppress spells the same dispatch out inline: calling this helper there changes its register allocation.)
+__device__ __forceinline__ void sort_keys_desc(unsigned long long* keys, int cnt) {
+    int n2 = 64;
+    while (n2 < cnt) n2 <<= 1;
+    for (int i = cnt + threadIdx.x; i < n2; i += NT) keys[i] = 0ull;
+    __syncthreads();
+    if (n2 == NT) bitonic_sort_desc_reg<1>(keys);
+    else if (n2 == 2 * NT) bitonic_sort_desc_reg<2>(keys);
+    else if (n2 == 4 * NT) bitonic_sort_desc_reg<4>(keys);
+    else if (n2 == 8 * NT) bitonic_sort_desc_reg<8>(keys);
+    else bitonic_sort_desc(keys, n2);
 }
 
 // Sort the pushed candidates and run the blocked greedy suppression.  All threads of the CTA call this.
@@ -991,6 +1011,207 @@ decode_nms_kernel(PostGeom g, NmsParams p) {
     sort_and_suppress<PROF>(s, p, n, tstart);
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Cross-region merge (yfv2_merge_regions): the NMS rows of T region images -> one list per frame in frame pixels.  One CTA per
+// frame.  The region descriptors of a launch's frames travel in the kernel parameters; the rows are read from global memory and
+// mapped to frame pixels on the fly, and only the kept boxes are held in shared memory (fp64).
+constexpr int kMergeFrames = 128;              // frames per launch
+constexpr int kMergeChunk = 64;                // candidates per step of the blocked greedy pass
+
+struct MergeArgs {
+    const float* dets;           // [T, max_det_in, 6]
+    const int* counts;           // [T]
+    double* out;                 // [F, max_det, 6]
+    int* out_counts;             // [F]
+    int* kept_src;               // [F, max_det] or null
+    double thr;
+    int W, H, max_det_in, max_det, metric;
+    int f0;                      // first frame of the launch
+    int t0;                      // global index of the launch's first region
+    int MCp;                     // key buffer: pow2 >= max(64, the largest frame's candidate slots)
+    int KC;                      // kept-box capacity: min(max_det, the largest frame's candidate slots)
+    int rbeg[kMergeFrames + 1];  // regions of frame f0 + i: [rbeg[i], rbeg[i + 1]) of reg[]
+    int4 reg[YFV2_MERGE_MAX_REGIONS];   // x0, y0, w, h
+};
+
+struct MergeSmem {
+    unsigned long long* keys;   // [MCp]  (sortable conf << 32) | ~(t_local * max_det_in + row)
+    double4* kbox;              // [KC]   kept boxes, frame pixels
+    float* kcls;                // [KC]
+    unsigned short* kt;         // [KC]   region of each kept box, relative to the frame's first
+    double4* chbox;             // [64]   the chunk's candidates
+    float* chcls;               // [64]
+    unsigned short* cht;        // [64]
+    unsigned int* cmask;        // [64][2] kill rows inside the chunk
+    unsigned int* misc;         // [0] candidates pushed, [1..2] dead bits of the chunk, [3..4] kept bits of the chunk
+};
+
+__host__ __device__ __forceinline__ unsigned char* merge_layout(MergeSmem& s, unsigned char* base, int MCp, int KC) {
+    s.keys = take<unsigned long long>(base, MCp);
+    s.kbox = take<double4>(base, KC);
+    s.chbox = take<double4>(base, kMergeChunk);
+    s.kcls = take<float>(base, KC);
+    s.chcls = take<float>(base, kMergeChunk);
+    s.cmask = take<unsigned int>(base, 2 * kMergeChunk);
+    s.misc = take<unsigned int>(base, 8);
+    s.kt = take<unsigned short>(base, KC);
+    s.cht = take<unsigned short>(base, kMergeChunk);
+    return base;
+}
+
+inline size_t merge_smem_bytes(int MCp, int KC) {
+    MergeSmem s;
+    return reinterpret_cast<size_t>(merge_layout(s, nullptr, MCp, KC));
+}
+
+// min / max as the contract defines them (region_oracle.py uses the same comparisons, so NaN coordinates agree)
+__device__ __forceinline__ double dmin(double a, double b) { return a < b ? a : b; }
+__device__ __forceinline__ double dmax(double a, double b) { return a > b ? a : b; }
+
+// fp64 overlap of box a (kept, or earlier in the order) and box b, strictly above thr.  metric 0: IoU = inter / (a_a + a_b - inter);
+// 1: IoS = inter / min(a_a, a_b).  No +1 in the widths (torchvision's convention); every operation rounded on its own; a NaN
+// quotient compares false.  Unlike iou_gt (fp32, class offsets) the class test is the caller's.
+__device__ __forceinline__ bool overlap_gt(const double4& a, const double4& b, double thr, int metric) {
+    const double iw = dmax(0.0, __dsub_rn(dmin(a.z, b.z), dmax(a.x, b.x)));
+    const double ih = dmax(0.0, __dsub_rn(dmin(a.w, b.w), dmax(a.y, b.y)));
+    const double inter = __dmul_rn(iw, ih);
+    const double aa = __dmul_rn(__dsub_rn(a.z, a.x), __dsub_rn(a.w, a.y));
+    const double ab = __dmul_rn(__dsub_rn(b.z, b.x), __dsub_rn(b.w, b.y));
+    const double den = metric ? dmin(aa, ab) : __dsub_rn(__dadd_rn(aa, ab), inter);
+    return __ddiv_rn(inter, den) > thr;
+}
+
+__global__ void __launch_bounds__(NT)
+merge_regions_kernel(const __grid_constant__ MergeArgs a) {
+    extern __shared__ __align__(32) unsigned char smraw[];
+    MergeSmem s;
+    merge_layout(s, smraw, a.MCp, a.KC);
+    const int t = threadIdx.x, fl = blockIdx.x, f = a.f0 + fl;
+    const int rb = a.rbeg[fl], nreg = a.rbeg[fl + 1] - rb;
+    const int mdi = a.max_det_in;
+    const long long tg0 = (long long)a.t0 + rb;                  // global index of the frame's first region
+    if (t == 0) s.misc[0] = 0u;
+    __syncthreads();
+    // candidates: rows below each region's count whose conf is not NaN, keyed by (conf, then lower t, then lower row first)
+    const int nslots = nreg * mdi;
+    for (int base = 0; base < nslots; base += NT) {
+        const int slot = base + t;
+        bool want = false;
+        unsigned long long key = 0ull;
+        if (slot < nslots) {
+            const int tl = slot / mdi, row = slot - tl * mdi;
+            const int cnt = min(max(__ldg(a.counts + tg0 + tl), 0), mdi);
+            if (row < cnt) {
+                const float conf = __ldg(a.dets + ((tg0 + tl) * mdi + row) * 6 + 4);
+                if (!isnan(conf)) {
+                    want = true;
+                    // + 0 turns -0 into +0, so that the two zeros tie like any equal confidences
+                    key = ((unsigned long long)f2sortable(__fadd_rn(conf, 0.0f)) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)slot);
+                }
+            }
+        }
+        const unsigned int bal = __ballot_sync(0xffffffffu, want);
+        unsigned int pos = 0;
+        if ((t & 31) == 0 && bal) pos = atomicAdd(&s.misc[0], (unsigned int)__popc(bal));
+        pos = __shfl_sync(0xffffffffu, pos, 0) + __popc(bal & ((1u << (t & 31)) - 1u));
+        if (want) s.keys[pos] = key;
+    }
+    __syncthreads();
+    const int cnt = (int)s.misc[0];
+    sort_keys_desc(s.keys, cnt);
+
+    double* out = a.out + (long long)f * a.max_det * 6;
+    int* ksrc = a.kept_src ? a.kept_src + (long long)f * a.max_det : nullptr;
+    int nk = 0;
+    for (int c0 = 0; c0 < cnt && nk < a.max_det; c0 += kMergeChunk) {
+        const int cn = min(kMergeChunk, cnt - c0);
+        if (t < cn) {                                        // stage the chunk: rows mapped to frame pixels
+            const unsigned int slot = 0xFFFFFFFFu - (unsigned int)(s.keys[c0 + t] & 0xFFFFFFFFull);
+            const int tl = (int)slot / mdi, row = (int)slot - tl * mdi;
+            const float* r = a.dets + ((tg0 + tl) * mdi + row) * 6;
+            const int4 g = a.reg[rb + tl];
+            const double sx = __ddiv_rn((double)g.z, (double)a.W), sy = __ddiv_rn((double)g.w, (double)a.H);
+            const double x0 = (double)g.x, y0 = (double)g.y;
+            s.chbox[t] = make_double4(__dadd_rn(__dmul_rn((double)__ldg(r), sx), x0), __dadd_rn(__dmul_rn((double)__ldg(r + 1), sy), y0),
+                                      __dadd_rn(__dmul_rn((double)__ldg(r + 2), sx), x0), __dadd_rn(__dmul_rn((double)__ldg(r + 3), sy), y0));
+            s.chcls[t] = __ldg(r + 5);
+            s.cht[t] = (unsigned short)tl;
+        }
+        if (t < 2 * kMergeChunk) s.cmask[t] = 0u;
+        if (t == 0) { s.misc[1] = 0u; s.misc[2] = 0u; }
+        __syncthreads();
+        {   // (a) the chunk against every box kept so far, four threads per candidate
+            const int j = t & (kMergeChunk - 1), q = t / kMergeChunk;
+            if (j < cn) {
+                const double4 bj = s.chbox[j];
+                const float cj = s.chcls[j];
+                const unsigned short tj = s.cht[j];
+                bool dead = false;
+                for (int i = q; i < nk && !dead; i += NT / kMergeChunk)
+                    dead = s.kt[i] != tj && s.kcls[i] == cj && overlap_gt(s.kbox[i], bj, a.thr, a.metric);
+                if (dead) atomicOr(&s.misc[1 + (j >> 5)], 1u << (j & 31));
+            }
+        }
+        __syncthreads();
+        unsigned long long alive = ~(((unsigned long long)s.misc[2] << 32) | s.misc[1]);
+        if (cn < 64) alive &= (1ull << cn) - 1ull;
+        {   // (b) pairs inside the chunk among the survivors of (a): candidate i against 16 of the later ones per thread
+            const int i = t >> 2, jq = t & 3;
+            if ((alive >> i) & 1ull) {
+                const double4 bi = s.chbox[i];
+                const float ci = s.chcls[i];
+                const unsigned short ti = s.cht[i];
+                unsigned int bits = 0u;
+                for (int e = 0; e < 16; ++e) {
+                    const int j = jq * 16 + e;
+                    if (j > i && ((alive >> j) & 1ull) && s.cht[j] != ti && s.chcls[j] == ci && overlap_gt(bi, s.chbox[j], a.thr, a.metric))
+                        bits |= 1u << e;
+                }
+                if (bits) atomicOr(&s.cmask[2 * i + (jq >> 1)], bits << ((jq & 1) * 16));
+            }
+        }
+        __syncthreads();
+        if (t < 32) {                                        // (c) greedy resolve, as in sort_and_suppress
+            unsigned int lo = (unsigned int)alive, hi = (unsigned int)(alive >> 32), klo = 0u, khi = 0u;
+            int room = a.max_det - nk;
+            while (lo && room > 0) {
+                const int i = __ffs((int)lo) - 1;
+                klo |= 1u << i;
+                --room;
+                lo &= ~(1u << i) & ~s.cmask[2 * i];
+                hi &= ~s.cmask[2 * i + 1];
+            }
+            while (hi && room > 0) {
+                const int i = __ffs((int)hi) - 1;
+                khi |= 1u << i;
+                --room;
+                hi &= ~(1u << i) & ~s.cmask[2 * (i + 32) + 1];
+            }
+            if (t == 0) { s.misc[3] = klo; s.misc[4] = khi; }
+        }
+        __syncthreads();
+        const unsigned long long kept = ((unsigned long long)s.misc[4] << 32) | (unsigned long long)s.misc[3];
+        if (t < cn && ((kept >> t) & 1ull)) {                // (d) append
+            const int pos = nk + __popcll(kept & ((1ull << t) - 1ull));
+            const double4 b = s.chbox[t];
+            s.kbox[pos] = b;
+            s.kcls[pos] = s.chcls[t];
+            s.kt[pos] = s.cht[t];
+            const unsigned int slot = 0xFFFFFFFFu - (unsigned int)(s.keys[c0 + t] & 0xFFFFFFFFull);
+            double* o = out + pos * 6;
+            o[0] = b.x; o[1] = b.y; o[2] = b.z; o[3] = b.w;
+            o[4] = (double)__ldg(a.dets + (tg0 * mdi + slot) * 6 + 4);     // (the key holds conf + 0)
+            o[5] = (double)s.chcls[t];
+            if (ksrc) ksrc[pos] = (int)(tg0 * mdi + slot);
+        }
+        nk += __popcll(kept);
+        __syncthreads();
+    }
+    if (t == 0) a.out_counts[f] = nk;
+    for (int i = nk * 6 + t; i < a.max_det * 6; i += NT) out[i] = 0.0;
+    if (ksrc) for (int i = nk + t; i < a.max_det; i += NT) ksrc[i] = -1;
+}
+
 long long* g_nms_prof = nullptr;       // yfv2_debug_nms_profile
 
 int fill_geom(PostGeom& g, const float* const preds[6], int N, int H, int W, int A, int C, const double* anchors_host) {
@@ -1133,5 +1354,73 @@ extern "C" int yfv2_decode_nms(const float* const preds[6], int N, int H, int W,
  * int64 on the device, or NULL to switch the instrumented kernel off again.  Process-wide; not for concurrent use. */
 extern "C" int yfv2_debug_nms_profile(long long* dev_buf) {
     g_nms_prof = dev_buf;
+    return YFV2_OK;
+}
+
+extern "C" int yfv2_merge_regions(const float* dets, const int* counts, const yfv2_region* regions, int T, int max_det_in, int F,
+                                  int H, int W, double thr, int metric, int max_det, double* out, int* out_counts, int* kept_src,
+                                  void* stream) {
+    if (!dets || !counts || !regions || !out || !out_counts) { set_error("merge_regions: null dets / counts / regions / out / out_counts"); return YFV2_EINVAL; }
+    if (T < 1 || F < 1 || W < 1 || H < 1) { set_error("merge_regions: need T, F, W, H >= 1 (T=%d F=%d W=%d H=%d)", T, F, W, H); return YFV2_EINVAL; }
+    if (max_det_in < 1 || max_det_in > 4096 || max_det < 1 || max_det > 4096) {
+        set_error("merge_regions: max_det_in=%d and max_det=%d must be in 1..4096", max_det_in, max_det);
+        return YFV2_EINVAL;
+    }
+    if (metric != 0 && metric != 1) { set_error("merge_regions: metric=%d (0: IoU, 1: IoS)", metric); return YFV2_EINVAL; }
+    if (thr != thr) { set_error("merge_regions: thr is NaN"); return YFV2_EINVAL; }
+    if ((long long)T * max_det_in > INT_MAX) { set_error("merge_regions: T * max_det_in = %lld rows exceeds 2^31 - 1", (long long)T * max_det_in); return YFV2_EINVAL; }
+    int run = 0;                                                   // regions of the current frame
+    for (int t = 0; t < T; ++t) {
+        const yfv2_region& r = regions[t];
+        const char* why = nullptr;
+        if (r.w < 1 || r.h < 1) why = "w and h must be >= 1";
+        else if (r.x0 < 0 || r.y0 < 0) why = "x0 and y0 must be >= 0";
+        else if (r.frame < 0 || r.frame >= F) why = "frame outside [0, F)";
+        else if (t && r.frame < regions[t - 1].frame) why = "frame index decreases (regions of a frame must be contiguous, frames ascending)";
+        if (why) {
+            set_error("merge_regions: region %d: %s (frame %d of F=%d, x0 %d, y0 %d, %dx%d)", t, why, r.frame, F, r.x0, r.y0, r.w, r.h);
+            return YFV2_EINVAL;
+        }
+        run = (t && r.frame == regions[t - 1].frame) ? run + 1 : 1;
+        if (run > YFV2_MERGE_MAX_REGIONS || (long long)run * max_det_in > YFV2_NMS_MAX_CAND) {
+            set_error("merge_regions: region %d: frame %d has %d regions x max_det_in %d: more than %d regions or %d candidates", t,
+                      r.frame, run, max_det_in, YFV2_MERGE_MAX_REGIONS, YFV2_NMS_MAX_CAND);
+            return YFV2_EINVAL;
+        }
+    }
+    // launches of whole frames: at most kMergeFrames frames and YFV2_MERGE_MAX_REGIONS regions each
+    std::unique_ptr<MergeArgs> ap(new (std::nothrow) MergeArgs);  // 17 KB of kernel parameters: on the heap, not the stack
+    if (!ap) { set_error("merge_regions: host allocation failed"); return YFV2_ENOMEM; }
+    MergeArgs& a = *ap;
+    a.dets = dets; a.counts = counts; a.out = out; a.out_counts = out_counts; a.kept_src = kept_src;
+    a.thr = thr; a.W = W; a.H = H; a.max_det_in = max_det_in; a.max_det = max_det; a.metric = metric;
+    int t = 0;
+    for (int f0 = 0; f0 < F;) {
+        int nf = 0, nr = 0, most = 0;
+        const int t0 = t;
+        while (f0 + nf < F && nf < kMergeFrames) {
+            int e = t;
+            while (e < T && regions[e].frame == f0 + nf) ++e;
+            if (nr + (e - t) > YFV2_MERGE_MAX_REGIONS) break;
+            a.rbeg[nf] = nr;
+            for (int k = t; k < e; ++k) a.reg[nr + k - t] = make_int4(regions[k].x0, regions[k].y0, regions[k].w, regions[k].h);
+            nr += e - t;
+            most = std::max(most, e - t);
+            t = e;
+            ++nf;
+        }
+        a.rbeg[nf] = nr;
+        a.f0 = f0; a.t0 = t0;
+        const int slots = most * max_det_in;
+        a.MCp = 64;
+        while (a.MCp < slots) a.MCp <<= 1;
+        a.KC = std::max(1, std::min(max_det, slots));
+        const size_t bytes = merge_smem_bytes(a.MCp, a.KC);
+        if (bytes > kSmemCap) { set_error("merge_regions: %zu bytes of shared memory needed", bytes); return YFV2_EUNSUPPORTED; }
+        YFV2_CUDA(cudaFuncSetAttribute(merge_regions_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+        merge_regions_kernel<<<nf, NT, bytes, (cudaStream_t)stream>>>(a);
+        YFV2_LAUNCH_CHECK();
+        f0 += nf;
+    }
     return YFV2_OK;
 }

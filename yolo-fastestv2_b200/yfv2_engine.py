@@ -46,6 +46,11 @@ class Yuv422Frame(ctypes.Structure):
                 ("w", ctypes.c_int), ("h", ctypes.c_int)]
 
 
+class Region(ctypes.Structure):
+    """yfv2_region: a crop (x0, y0, w, h) of frame `frame` whose NMS rows yfv2_merge_regions maps back and merges."""
+    _fields_ = [("frame", ctypes.c_int), ("x0", ctypes.c_int), ("y0", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int)]
+
+
 # name -> (restype, argtypes); must list every prototype of include/yfv2.h (tests check this)
 PROTOTYPES = {
     "yfv2_abi_version": (ctypes.c_int, []),
@@ -74,6 +79,9 @@ PROTOTYPES = {
                                        ctypes.POINTER(ctypes.c_double), ctypes.c_float, ctypes.c_double, ctypes.c_void_p,
                                        ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p,
                                        ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "yfv2_merge_regions": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Region), ctypes.c_int, ctypes.c_int,
+                                          ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_int, ctypes.c_int,
+                                          ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "yfv2_batch_statistics": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                              ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]),
     "yfv2_aug_contrast_brightness": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_longlong, ctypes.c_void_p]),
@@ -439,6 +447,44 @@ def decode_nms(preds, cfg, conf_thres=0.3, iou_thres=0.45, classes=None, max_det
     return out, counts, idx
 
 
+MERGE_METRICS = {"iou": 0, "ios": 1}
+
+
+def merge_regions(dets, counts, regions, F, W, H, thr, metric, max_det):
+    """yfv2_merge_regions: the NMS rows of T region images -> one list per frame in frame pixels (a cross-region NMS, see
+    include/yfv2.h).  dets: CUDA float32 [T, max_det_in, 6] and counts int32 [T], as decode_nms / nms return them for the region
+    images; regions: T tuples (frame, x0, y0, w, h), the regions of one frame contiguous, frames ascending; F frames; W x H the
+    network input the regions were stretched to; metric "iou" | "ios" (or 0 | 1).  Returns CUDA tensors (out float64
+    [F, max_det, 6], counts int32 [F], kept_src int32 [F, max_det]: t * max_det_in + row of each kept row, -1 past the count)."""
+    _require_cuda(dets, "dets")
+    _require_cuda(counts, "counts")
+    if dets.dim() != 3 or dets.shape[2] != 6 or dets.dtype != torch.float32:
+        raise Yfv2Error("merge_regions: dets must be float32 [T, max_det_in, 6], got %s %s" % (dets.dtype, tuple(dets.shape)))
+    T, max_det_in = dets.shape[0], dets.shape[1]
+    if counts.dtype != torch.int32 or tuple(counts.shape) != (T,):
+        raise Yfv2Error("merge_regions: counts must be int32 [%d], got %s %s" % (T, counts.dtype, tuple(counts.shape)))
+    regions = list(regions)
+    if len(regions) != T:
+        raise Yfv2Error("merge_regions: %d regions for %d row blocks" % (len(regions), T))
+    m = MERGE_METRICS.get(metric, metric)
+    if m not in (0, 1):
+        raise Yfv2Error("merge_regions: metric must be 'iou' or 'ios', got %r" % (metric,))
+    dets, counts = dets.contiguous(), counts.contiguous()
+    descs = (Region * max(T, 1))()
+    for d, r in zip(descs, regions):
+        d.frame, d.x0, d.y0, d.w, d.h = (int(v) for v in r)
+    dev = dets.device
+    out = torch.empty((max(F, 0), max_det, 6), dtype=torch.float64, device=dev)
+    out_counts = torch.empty((max(F, 0),), dtype=torch.int32, device=dev)
+    kept = torch.empty((max(F, 0), max_det), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _check(lib().yfv2_merge_regions(ctypes.c_void_p(dets.data_ptr()), ctypes.c_void_p(counts.data_ptr()), descs, T, max_det_in, F,
+                                        H, W, ctypes.c_double(thr), m, max_det, ctypes.c_void_p(out.data_ptr()),
+                                        ctypes.c_void_p(out_counts.data_ptr()), ctypes.c_void_p(kept.data_ptr()), _stream(dev)),
+               "merge_regions")
+    return out, out_counts, kept
+
+
 def batch_statistics(out, counts, targets, iou_threshold):
     """True-positive flags [N,max_det] (float 0/1) of NMS output rows against pixel-xyxy targets [nt,6] (device)."""
     _require_cuda(out, "out")
@@ -766,6 +812,36 @@ def resize_frames(frames, W, H, layout, device=None, out=None):
             _resize_layout_run(checked[i:j], layouts[i:j], W, H, device, out[i:j])
         i = j
     return out
+
+
+def crop_frame(frame, layout, x0, y0, w, h):
+    """The w x h window at (x0, y0) of a frame, in the form resize_frames takes for `layout`, as a view (nothing is copied):
+    resize_frames of the crop gives the bytes of cv2.resize(cv2.cvtColor(frame, COLOR_<LAYOUT>2BGR)[y0:y0+h, x0:x0+w]).  HWC
+    layouts and grey are sliced in place, "rgb_chw" as [3, h, w].  A 4:2:0 frame (a single [h*3/2, w] buffer or its planes)
+    becomes a tuple of cropped planes, (y, uv) for NV12 / NV21 and (y, u, v) for I420 / YV12; x0, y0, w, h must then be even, so
+    that the 2x2 chroma blocks of the crop are those of the frame.  Packed 4:2:2 needs even x0 and w (whole macropixels)."""
+    if layout not in LAYOUTS:
+        raise Yfv2Error("crop_frame: layout must be one of %s, got %r" % (", ".join(LAYOUTS), layout))
+    f = _check_frame(frame, layout, 0)
+    fh, fw = frame_size(f, layout)
+    x0, y0, w, h = int(x0), int(y0), int(w), int(h)
+    if w < 1 or h < 1 or x0 < 0 or y0 < 0 or x0 + w > fw or y0 + h > fh:
+        raise Yfv2Error("crop_frame: window (x0 %d, y0 %d, %dx%d) is not inside the %dx%d frame" % (x0, y0, w, h, fw, fh))
+    if layout in YUV420_LAYOUTS and (x0 | y0 | w | h) & 1:
+        raise Yfv2Error("crop_frame: %s crops need even x0, y0, w and h (2x2 chroma blocks), got (x0 %d, y0 %d, %dx%d)"
+                        % (layout, x0, y0, w, h))
+    if layout in YUV422_LAYOUTS and (x0 | w) & 1:
+        raise Yfv2Error("crop_frame: %s crops need even x0 and w (two pixels per macropixel), got x0 %d, w %d" % (layout, x0, w))
+    if layout in YUV420_LAYOUTS:
+        y, u, v = _yuv420_planes(f, layout, 0)
+        cy = slice(y0 // 2, (y0 + h) // 2)
+        if layout in ("nv12", "nv21"):
+            return y[y0:y0 + h, x0:x0 + w], u[cy, x0:x0 + w]
+        cx = slice(x0 // 2, (x0 + w) // 2)
+        return y[y0:y0 + h, x0:x0 + w], u[cy, cx], v[cy, cx]
+    if layout == "rgb_chw":
+        return f[:, y0:y0 + h, x0:x0 + w]
+    return f[y0:y0 + h, x0:x0 + w]
 
 
 def debug_pw_tc(x, w):
