@@ -346,6 +346,35 @@ YFV2_API int yfv2_forward_range(yfv2_plan* plan, const void* x, int is_u8, const
 YFV2_API int yfv2_debug_gather(const yfv2_plan* plan, const void* workspace, int which, float* out, int* dims4,
                                void* stream);
 
+/* ---- test hooks: the native trainer's program and where it keeps every tensor in the workspace -----------------------
+ * Host only: nothing is launched and no device memory is read.  yfv2_trainer_debug_ops / _tensors write min(cap, count) records
+ * and return the count in *n (cap 0 with a NULL array queries it).  An op reads tensors a (and b), writes tensor y:
+ *   kind: 0 stem (3x3 s2 conv, weight pw), 1 BatchNorm train (+ReLU if relu; gamma pg, beta pb, layer bn; aux: workspace float
+ *         offset of 2C doubles of fp64 sums, then mean[C] at aux + 4C and invstd[C] at aux + 5C), 2 max-pool 3x3 s2 p1 (aux: int32
+ *         argmax per output element), 3 1x1 conv (M outputs, weight pw, bias pbias), 4 depthwise conv (ks, stride, weight pw),
+ *         5 nearest 2x up-sampling, 6 odd channels of a, 7 [even channels of a | b], 8 [a | b] (channel concat).
+ *   Parameter indices are model.parameters() positions, -1 where the op has none; aux is -1 for kinds without private storage.
+ * A tensor's activation and gradient are dense NCHW [N, C, H, W] at workspace float offsets off / goff; ext >= 0 marks head tensor
+ * `ext` (the caller's preds / dpreds, off = goff = -1) and ext = -2 the input image.
+ * layout_host[8] receives, in floats: workspace size, then the offset of the fan-in gradient scratch, the offset and size of the
+ * parameter-gradient scratch (a shared layer's second use), the offset and size of the flat gradient slot, the offset and size of
+ * the per-block weight-gradient partials. */
+typedef struct yfv2_trainer_op {
+    int kind;
+    int a, b, y;                 /* tensor ids (b = -1 for one-input ops) */
+    int pw, pg, pb, pbias, bn;
+    int relu, ks, stride, M;
+    long long aux;
+} yfv2_trainer_op;
+typedef struct yfv2_trainer_tensor {
+    long long off, goff;
+    int C, H, W;
+    int ext;
+} yfv2_trainer_tensor;
+YFV2_API int yfv2_trainer_debug_ops(const yfv2_trainer* t, yfv2_trainer_op* ops_host, int cap, int* n);
+YFV2_API int yfv2_trainer_debug_tensors(const yfv2_trainer* t, yfv2_trainer_tensor* tens_host, int cap, int* n);
+YFV2_API int yfv2_trainer_debug_layout(const yfv2_trainer* t, long long* layout_host);
+
 /* ---- test hook: how a head launch of a forward on `workspace` reads its 5x5 depthwise taps ------------------------------
  * which: 0 heads2.a, 1 heads2.b, 2 heads3.a, 3 heads3.b.  Returns 1 when the launch stages the input windows in shared memory,
  * 0 when it reads the planes, < 0 on a bad argument (workspace NULL included: the choice depends on the plane addresses).

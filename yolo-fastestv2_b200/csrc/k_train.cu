@@ -639,7 +639,8 @@ bn_apply_kernel(const float* __restrict__ x, const float* __restrict__ mean, con
     const float* xp = x + pl * HW;
     float* yp = y + pl * HW;
     const int p0 = blockIdx.y * 1024 + threadIdx.x * 4;
-    auto f = [&](float v) { float r = (v - mu) * is * ga + be; return relu ? fmaxf(r, 0.f) : r; };      // same association as before
+    // ReLU as torch's threshold (r <= 0 ? 0 : r): a NaN passes through, where fmaxf(NaN, 0) would return 0
+    auto f = [&](float v) { float r = (v - mu) * is * ga + be; return relu ? (r <= 0.f ? 0.f : r) : r; };      // same association as before
     if ((HW & 3) == 0 && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0) {
         if (p0 < HW) {
             const float4 v = __ldg(reinterpret_cast<const float4*>(xp + p0));
@@ -651,7 +652,8 @@ bn_apply_kernel(const float* __restrict__ x, const float* __restrict__ mean, con
     }
 }
 
-// sums[c] = (sum dy, sum dy*xhat) with the ReLU mask applied (y > 0); grid (C, slices), whole planes per block
+// sums[c] = (sum dy, sum dy*xhat) with the ReLU mask applied (dy zeroed where y <= 0, as threshold_backward: a NaN y passes dy);
+// grid (C, slices), whole planes per block
 __global__ void __launch_bounds__(256)
 bn_bwd_reduce_kernel(const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ dy, const float* __restrict__ mean,
                      const float* __restrict__ invstd, double* __restrict__ sums, int N, int C, int HW, int relu) {
@@ -662,7 +664,7 @@ bn_bwd_reduce_kernel(const float* __restrict__ x, const float* __restrict__ y, c
         const long long base = ((long long)n * C + c) * HW;
         for (int p = threadIdx.x; p < HW; p += 256) {
             float d = __ldg(dy + base + p);
-            if (relu && !(__ldg(y + base + p) > 0.f)) d = 0.f;
+            if (relu && __ldg(y + base + p) <= 0.f) d = 0.f;
             s1 += d; s2 += (double)d * ((__ldg(x + base + p) - mu) * is);
         }
     }
@@ -693,7 +695,7 @@ bn_bwd_apply_kernel(const float* __restrict__ x, const float* __restrict__ y, co
         const int p = p0 + q;
         if (p < HW) {
             float d = __ldg(dy + base + p);
-            if (relu && !(__ldg(y + base + p) > 0.f)) d = 0.f;
+            if (relu && __ldg(y + base + p) <= 0.f) d = 0.f;
             const float xh = (__ldg(x + base + p) - mu) * is;
             dx[base + p] = ga * is * (d - sd - xh * sdx);
         }
@@ -722,7 +724,8 @@ __global__ void maxpool_fwd_kernel(const float* __restrict__ x, float* __restric
                 const int ix = 2 * ox - 1 + kx;
                 if (ix < 0 || ix >= W) continue;
                 const float v = xp[iy * W + ix];
-                if (v > best || bi < 0) { best = v; bi = iy * W + ix; }      // first maximum, as ATen's max_pool2d
+                // ATen's max_pool2d rule: the first maximum, but a NaN always wins (so the last NaN of the window is kept)
+                if (v > best || isnan(v) || bi < 0) { best = v; bi = iy * W + ix; }
             }
         }
         y[i] = best; idx[i] = bi;
@@ -887,7 +890,9 @@ extern "C" YFV2_API int yfv2_op_stem_wgrad(const float* x, const float* dy, floa
 // scratch: 2*C doubles.  save_mean / save_invstd: [C] each.  running_* may be null (no update).
 extern "C" YFV2_API int yfv2_op_bn_train_fwd(const float* x, const float* gamma, const float* beta, float* running_mean, float* running_var, float* y,
                                              float* save_mean, float* save_invstd, double* scratch, int N, int C, int HW, int relu, void* stream) {
-    ARGCHK(x && gamma && beta && y && save_mean && save_invstd && scratch, "bn_train_fwd: bad arguments");
+    ARGCHK(x && gamma && beta && y && save_mean && save_invstd && scratch && N > 0 && C > 0 && HW > 0, "bn_train_fwd: bad arguments");
+    // F.batch_norm in training mode refuses one value per channel (its variance is undefined)
+    ARGCHK((long long)N * HW > 1, "bn_train_fwd: expected more than 1 value per channel when training");
     cudaStream_t s = (cudaStream_t)stream;
     YFV2_CUDA(cudaMemsetAsync(scratch, 0, (size_t)2 * C * sizeof(double), s));
     const long long per = (long long)N * HW;

@@ -58,7 +58,7 @@ struct yfv2_trainer {
     std::vector<long long> pnumel;
     long long ptotal = 0;
     long long ws_floats = 0;
-    long long gflat_off = 0, scratch_off = 0, pscratch_off = 0, wscratch_off = 0;
+    long long gflat_off = 0, scratch_off = 0, pscratch_off = 0, wscratch_off = 0, pscratch_floats = 0;
     int x_ten = -1;
     int out_ten[6];
     // CUDA-graph replay of the two static programs (~1000 launches per step otherwise: the step is host-bound at 8 GPUs): a
@@ -235,8 +235,11 @@ void build(yfv2_trainer& t) {
     long long biggest = 0, pbig = 0;
     for (const Ten& x_ : t.tens) if (x_.ext == -1) biggest = std::max(biggest, (long long)t.N * x_.C * x_.H * x_.W);
     for (long long n : t.pnumel) pbig = std::max(pbig, n);
+    // the second use of a shared output convolution puts its bias gradient right behind the weight's (run_backward)
+    for (int w : {w_reg, w_obj, w_cls}) pbig = std::max(pbig, t.pnumel[w] + t.pnumel[w + 1]);
     t.scratch_off = b.alloc(biggest);
     t.pscratch_off = b.alloc(pbig);
+    t.pscratch_floats = pbig;
     t.gflat_off = b.alloc(t.ptotal);
     t.wscratch_off = b.alloc(kWScratchFloats);
 }
@@ -304,6 +307,10 @@ extern "C" int yfv2_trainer_create(yfv2_trainer** out, int device, int N, int H,
         set_error("trainer_create: bad arguments (N=%d H=%d W=%d A=%d C=%d; H, W multiples of 32)", N, H, W, A, C);
         return YFV2_EINVAL;
     }
+    if ((long long)N * (H / 32) * (W / 32) == 1) {      // every stride-32 BatchNorm would normalise one value (F.batch_norm refuses)
+        set_error("trainer_create: expected more than 1 value per channel when training (N=%d, %dx%d: one value at stride 32)", N, H, W);
+        return YFV2_EINVAL;
+    }
     yfv2_trainer* t = new (std::nothrow) yfv2_trainer();
     if (!t) { set_error("trainer_create: out of host memory"); return YFV2_ENOMEM; }
     t->device = device; t->N = N; t->H = H; t->W = W; t->A = A; t->C = C;
@@ -336,6 +343,37 @@ extern "C" int yfv2_trainer_grad_floats(const yfv2_trainer* t, long long* n) {
 extern "C" int yfv2_trainer_param_offset(const yfv2_trainer* t, int index, long long* offset, long long* numel) {
     if (!t || index < 0 || index >= (int)t->poff.size() || !offset || !numel) { set_error("trainer_param_offset: bad argument"); return YFV2_EINVAL; }
     *offset = t->poff[index]; *numel = t->pnumel[index];
+    return YFV2_OK;
+}
+
+extern "C" int yfv2_trainer_debug_ops(const yfv2_trainer* t, yfv2_trainer_op* ops_host, int cap, int* n) {
+    if (!t || !n || cap < 0 || (cap > 0 && !ops_host)) { set_error("trainer_debug_ops: bad argument"); return YFV2_EINVAL; }
+    *n = (int)t->ops.size();
+    for (int i = 0; i < cap && i < *n; ++i) {
+        const Op& o = t->ops[i];
+        yfv2_trainer_op& d = ops_host[i];
+        d.kind = o.kind; d.a = o.a; d.b = o.b; d.y = o.y;
+        d.pw = o.pw; d.pg = o.pg; d.pb = o.pb; d.pbias = o.pbias; d.bn = o.bn;
+        d.relu = o.relu; d.ks = o.ks; d.stride = o.stride; d.M = o.M;
+        d.aux = o.kind == K_BN || o.kind == K_POOL ? o.aux : -1;
+    }
+    return YFV2_OK;
+}
+extern "C" int yfv2_trainer_debug_tensors(const yfv2_trainer* t, yfv2_trainer_tensor* tens_host, int cap, int* n) {
+    if (!t || !n || cap < 0 || (cap > 0 && !tens_host)) { set_error("trainer_debug_tensors: bad argument"); return YFV2_EINVAL; }
+    *n = (int)t->tens.size();
+    for (int i = 0; i < cap && i < *n; ++i) {
+        const Ten& x = t->tens[i];
+        yfv2_trainer_tensor& d = tens_host[i];
+        d.off = x.off; d.goff = x.goff; d.C = x.C; d.H = x.H; d.W = x.W; d.ext = x.ext;
+    }
+    return YFV2_OK;
+}
+extern "C" int yfv2_trainer_debug_layout(const yfv2_trainer* t, long long* layout_host) {
+    if (!t || !layout_host) { set_error("trainer_debug_layout: bad argument"); return YFV2_EINVAL; }
+    const long long v[8] = {t->ws_floats, t->scratch_off, t->pscratch_off, t->pscratch_floats, t->gflat_off, t->ptotal,
+                            t->wscratch_off, kWScratchFloats};
+    for (int i = 0; i < 8; ++i) layout_host[i] = v[i];
     return YFV2_OK;
 }
 

@@ -125,6 +125,7 @@ class Detector(nn.Module):
             from model import train_ops
             self.invalidate_packed()                      # the BN running statistics are updated through raw pointers
             x = x.float() if x.dtype != torch.float32 else x
+            yfv2_engine.check_bn_batch(x.shape[0], x.shape[2], x.shape[3])
             # default: the native trainer (csrc/trainer.cu), one C-ABI call for the forward and one for the backward;
             # YFV2_TRAIN_PYOPS=1 keeps the op-by-op autograd composition (the path the operator tests pin)
             if os.environ.get("YFV2_TRAIN_PYOPS") or x.shape[2] % 32 or x.shape[3] % 32:

@@ -92,6 +92,8 @@ class BnTrain(torch.autograd.Function):
     def forward(ctx, x, gamma, beta, running_mean, running_var, relu):
         x = _c(x)
         N, C, H, W = x.shape
+        if N * H * W == 1:                                   # F.batch_norm's refusal (the kernel refuses it too)
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s" % (x.shape,))
         y = torch.empty_like(x)
         mean = torch.empty(C, dtype=torch.float32, device=x.device)
         invstd = torch.empty(C, dtype=torch.float32, device=x.device)

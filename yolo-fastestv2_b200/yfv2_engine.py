@@ -46,6 +46,52 @@ class Yuv422Frame(ctypes.Structure):
                 ("w", ctypes.c_int), ("h", ctypes.c_int)]
 
 
+class TrainerOp(ctypes.Structure):
+    """yfv2_trainer_op: one op of the native trainer's program (test hook)."""
+    _fields_ = [(f, ctypes.c_int) for f in ("kind", "a", "b", "y", "pw", "pg", "pb", "pbias", "bn", "relu", "ks", "stride", "M")] + \
+               [("aux", ctypes.c_longlong)]
+
+
+class TrainerTensor(ctypes.Structure):
+    """yfv2_trainer_tensor: where the trainer keeps one tensor and its gradient (test hook)."""
+    _fields_ = [("off", ctypes.c_longlong), ("goff", ctypes.c_longlong), ("C", ctypes.c_int), ("H", ctypes.c_int), ("W", ctypes.c_int),
+                ("ext", ctypes.c_int)]
+
+
+TRAINER_OP_KINDS = ("stem", "bn", "pool", "pw", "dw", "up", "odd", "cate", "cat2")       # yfv2_trainer_op.kind
+TRAINER_LAYOUT = ("ws_floats", "scratch_off", "pscratch_off", "pscratch_floats", "gflat_off", "gflat_floats", "wscratch_off",
+                  "wscratch_floats")                                                     # yfv2_trainer_debug_layout
+
+
+def trainer_program(handle):
+    """(ops, tensors, layout) of a yfv2_trainer handle as lists of dicts / a dict; host only (test hook)."""
+    L, n = lib(), ctypes.c_int()
+    _check(L.yfv2_trainer_debug_ops(handle, None, 0, ctypes.byref(n)), "trainer_debug_ops")
+    ops = (TrainerOp * n.value)()
+    _check(L.yfv2_trainer_debug_ops(handle, ops, n.value, ctypes.byref(n)), "trainer_debug_ops")
+    _check(L.yfv2_trainer_debug_tensors(handle, None, 0, ctypes.byref(n)), "trainer_debug_tensors")
+    tens = (TrainerTensor * n.value)()
+    _check(L.yfv2_trainer_debug_tensors(handle, tens, n.value, ctypes.byref(n)), "trainer_debug_tensors")
+    lay = (ctypes.c_longlong * len(TRAINER_LAYOUT))()
+    _check(L.yfv2_trainer_debug_layout(handle, lay), "trainer_debug_layout")
+    as_dict = lambda s: {f: getattr(s, f) for f, _ in s._fields_}
+    ops = [as_dict(o) for o in ops]
+    for o in ops:
+        o["kind"] = TRAINER_OP_KINDS[o["kind"]]
+    return ops, [as_dict(t) for t in tens], dict(zip(TRAINER_LAYOUT, lay))
+
+
+def check_bn_batch(N, H, W):
+    """F.batch_norm in training mode refuses a layer with one value per channel; the deepest BatchNorm layers of the network run
+    at stride 32 (stem 3x3 s2, max-pool 3x3 s2 p1 and three stride-2 blocks: each (h - 1) // 2 + 1), the first of them on the
+    96 channels of stage4.0's projection branch.  Raised before anything is launched, as the reference raises at that layer."""
+    h, w = H // 2, W // 2
+    for _ in range(4):
+        h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+    if N * h * w == 1:
+        raise ValueError("Expected more than 1 value per channel when training, got input size torch.Size([%d, 96, %d, %d])" % (N, h, w))
+
+
 class Region(ctypes.Structure):
     """yfv2_region: a crop (x0, y0, w, h) of frame `frame` whose NMS rows yfv2_merge_regions maps back and merges."""
     _fields_ = [("frame", ctypes.c_int), ("x0", ctypes.c_int), ("y0", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int)]
@@ -124,6 +170,9 @@ PROTOTYPES = {
     "yfv2_train_forward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, _c_void_pp, _c_void_pp, _c_void_pp, ctypes.c_void_p, ctypes.c_void_p]),
     "yfv2_train_backward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, _c_void_pp, _c_void_pp, _c_void_pp, ctypes.c_void_p, ctypes.c_int,
                                            ctypes.c_void_p, ctypes.c_void_p]),
+    "yfv2_trainer_debug_ops": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
+    "yfv2_trainer_debug_tensors": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
+    "yfv2_trainer_debug_layout": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_longlong)]),
     "yfv2_plan_stage_name": (ctypes.c_char_p, [ctypes.c_void_p, ctypes.c_int]),
     "yfv2_plan_stage_group": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     "yfv2_forward_range": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, _c_void_pp,
@@ -220,6 +269,10 @@ class Trainer:
                 self._h = ctypes.c_void_p()
         except Exception:
             pass
+
+    def program(self):
+        """(ops, tensors, layout) of the trainer's static program (trainer_program; host only)."""
+        return trainer_program(self._h)
 
     def alloc_preds(self):
         out = []
