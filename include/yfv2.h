@@ -176,6 +176,34 @@ YFV2_API int yfv2_batch_statistics(const float* dets, const int* counts, int N, 
 YFV2_API int yfv2_aug_contrast_brightness(const uint8_t* img, uint8_t* out, const float* alpha, const float* beta, int N,
                                           long long bytes_per_image, void* stream);
 
+/* ---- img_aug with random_resize and augment_hsv (utils/datasets.py:63-68 with :66-67 enabled) on the device -------------
+ * One pass over img [N,3,H,W] (planar B, G, R uint8, the training batch) into out, per image in img_aug's order:
+ *   YFV2_AUG_CONTRAST  contrast_and_brightness (:10-16), the arithmetic of yfv2_aug_contrast_brightness, on every source byte;
+ *   YFV2_AUG_RESIZE    random_resize (:54-61): cv2.resize(cv2.resize(img, (rw, rh)), (W, H)), both INTER_LINEAR with the
+ *                      arithmetic of yfv2_resize_bgr_u8; the rw x rh image is recomputed where read, never stored;
+ *   YFV2_AUG_HSV       augment_hsv (:39-51): cv2.cvtColor(COLOR_BGR2HSV), the image's three LUTs on H, S, V,
+ *                      cv2.cvtColor(COLOR_HSV2BGR), both conversions bit-identical to OpenCV 4.13's 8-bit paths (x86,
+ *                      with the HSV2BGR rounding of the last W mod 32 pixels of a row, see yfv2_debug_hsv2bgr).
+ * params: HOST array [N]; alpha / beta are read with YFV2_AUG_CONTRAST, rw / rh (1 <= rw <= W, 1 <= rh <= H; the reference
+ * draws int(W * uniform(0.8, 1)), then int(H * uniform(0.8, 1))) with YFV2_AUG_RESIZE.  luts: device [N][3][256] uint8 (hue,
+ * saturation, value LUTs as datasets.py:44-47 build them from the image's gains), required with YFV2_AUG_HSV, else ignored.
+ * In place (img == out) is allowed without YFV2_AUG_RESIZE; any other overlap is refused.  H, W <= 32768.  Every argument is
+ * checked before anything is launched (YFV2_EINVAL). */
+#define YFV2_AUG_CONTRAST 1
+#define YFV2_AUG_RESIZE   2
+#define YFV2_AUG_HSV      4
+typedef struct yfv2_aug_params {
+    float alpha, beta;     /* contrast_and_brightness */
+    int rw, rh;            /* random_resize's intermediate size */
+} yfv2_aug_params;
+YFV2_API int yfv2_aug_batch(const uint8_t* img, uint8_t* out, int N, int H, int W, const yfv2_aug_params* params,
+                            const uint8_t* luts, int flags, void* stream);
+/* Test hooks: n packed 3-byte pixels through the device's cv2.cvtColor COLOR_BGR2HSV / COLOR_HSV2BGR (any input bytes).  cv2's
+ * 8-bit HSV2BGR rounds the last (row_w mod 32) pixels of each row differently from the others (OpenCV 4.13 x86: vector code
+ * truncates, the scalar tail rounds), so the pixels are taken as rows of row_w. */
+YFV2_API int yfv2_debug_bgr2hsv(const uint8_t* in, uint8_t* out, long long n, void* stream);
+YFV2_API int yfv2_debug_hsv2bgr(const uint8_t* in, uint8_t* out, long long n, int row_w, void* stream);
+
 /* ---- raw frames -> network input: cv2.resize(img, (W, H), interpolation=cv2.INTER_LINEAR) on the device ----------------
  * The resize the reference runs on the host before every forward (test.py:35; utils/datasets.py:107 for training and
  * validation), fused with the HWC -> CHW transpose of test.py:36-37.  frames: N HOST descriptors of packed HWC BGR uint8 frames

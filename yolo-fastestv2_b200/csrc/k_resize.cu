@@ -20,9 +20,11 @@
 // moves.  One thread per output pixel (all three channels); a warp covers 32 consecutive x of one row, so each plane store of a
 // warp is one contiguous 32-byte run.  The coefficients are recomputed per thread (four double operations): cheaper than a table
 // round trip, and the call needs no workspace.
+// aug_resize_kernel (yfv2_aug_batch, k_aug.cu) runs random_resize as the second resize over a fetch that computes the pixels of
+// the first from the planar source where they are read (DESIGN.md §9).
 #include <climits>
 
-#include "common.cuh"
+#include "aug.cuh"
 
 namespace yfv2 {
 namespace {
@@ -183,6 +185,34 @@ resize_kernel(const __grid_constant__ ResizeChunk<Src> a) {
     }
 }
 
+// Output pixel (x, y) of the resize of fr (w x h source pixels) to W x H: B, G, R in v.  resize_kernel's arithmetic, for the
+// augmentation's nested resize (resize_kernel keeps its own copy of these lines so that its code stays as it was).
+template <class Src>
+__device__ __forceinline__ void resize_pixel(const typename Src::Desc& fr, int w, int h, int x, int y, int W, int H, int (&v)[3]) {
+    int sx;
+    float fx = src_coord(x, w, W, sx);
+    if (sx < 0) { fx = 0.f; sx = 0; }
+    if (sx >= w - 1) { fx = 0.f; sx = w - 1; }
+    const int a0 = weight0(fx), a1 = weight1(fx);
+    const int x1 = min(sx + 1, w - 1);
+
+    int sy;
+    const float fy = src_coord(y, h, H, sy);
+    const int b0 = weight0(fy), b1 = weight1(fy);
+    const int r0 = min(max(sy, 0), h - 1), r1 = min(max(sy + 1, 0), h - 1);
+
+    const Src row0(fr, r0), row1(fr, r1);
+    int p00[3], p01[3], p10[3], p11[3];          // [row][column] source pixels, B G R
+    row0.fetch(sx, x1, p00, p01);
+    row1.fetch(sx, x1, p10, p11);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const int S0 = p00[c] * a0 + p01[c] * a1;
+        const int S1 = p10[c] * a0 + p11[c] * a1;
+        v[c] = sat_u8(((((S0 >> 4) * b0) >> 16) + (((S1 >> 4) * b1) >> 16) + 2) >> 2);
+    }
+}
+
 // Launches the checked descriptors Src::kChunk frames at a time.
 template <class Src>
 int launch_resize(const typename Src::Desc* frames, int N, int H, int W, uint8_t* dst, void* stream) {
@@ -198,6 +228,66 @@ int launch_resize(const typename Src::Desc* frames, int N, int H, int W, uint8_t
         YFV2_LAUNCH_CHECK();
     }
     return YFV2_OK;
+}
+
+// Image n of an augmentation chunk: its planar [3][H][W] source bytes and parameters
+struct AugFrame {
+    const uint8_t* img;
+    int W, H;
+    yfv2_aug_params p;
+};
+
+// Source pixels of the augmentation, through contrast_and_brightness (alpha 1, beta 0 leave them unchanged)
+struct PlanarSource {
+    using Desc = AugFrame;
+    const uint8_t* row;
+    size_t plane;
+    float alpha, beta;
+    __device__ __forceinline__ PlanarSource(const AugFrame& f, int r)
+        : row(f.img + (size_t)r * f.W), plane((size_t)f.H * f.W), alpha(f.p.alpha), beta(f.p.beta) {}
+    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            p0[c] = (int)aug_byte(__ldg(row + c * plane + c0), alpha, beta);
+            p1[c] = (int)aug_byte(__ldg(row + c * plane + c1), alpha, beta);
+        }
+    }
+};
+
+// Pixels of random_resize's rw x rh intermediate cv2.resize(img, (rw, rh)), each computed from the source where it is read,
+// so the intermediate image is never stored
+struct NestedSource {
+    using Desc = AugFrame;
+    const AugFrame& f;
+    int r;
+    __device__ __forceinline__ NestedSource(const AugFrame& f_, int r_) : f(f_), r(r_) {}
+    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
+        resize_pixel<PlanarSource>(f, f.W, f.H, c0, r, f.p.rw, f.p.rh, p0);
+        resize_pixel<PlanarSource>(f, f.W, f.H, c1, r, f.p.rw, f.p.rh, p1);
+    }
+};
+
+// yfv2_aug_batch with the resize: one thread per output pixel of image blockIdx.z, the second resize over NestedSource, then
+// augment_hsv on the pixel when the chunk has LUTs
+__global__ void __launch_bounds__(kResizeBx * kResizeBy)
+aug_resize_kernel(const __grid_constant__ AugChunk a) {
+    __shared__ HsvSmem t;
+    const bool hsv = a.luts != nullptr;
+    if (hsv) {
+        stage_hsv(t, a.luts + (size_t)blockIdx.z * 768);
+        __syncthreads();
+    }
+    const int x = blockIdx.x * kResizeBx + threadIdx.x;
+    const int y = blockIdx.y * kResizeBy + threadIdx.y;
+    if (x >= a.W || y >= a.H) return;
+    const size_t plane = (size_t)a.H * a.W;
+    const AugFrame f{a.img + (size_t)blockIdx.z * 3 * plane, a.W, a.H, a.im[blockIdx.z]};
+    int v[3];
+    resize_pixel<NestedSource>(f, f.p.rw, f.p.rh, x, y, a.W, a.H, v);
+    if (hsv) hsv_lut_pixel(v[0], v[1], v[2], x, a.W, t);
+    uint8_t* out = a.out + (size_t)blockIdx.z * 3 * plane + (size_t)y * a.W + x;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out[c * plane] = (uint8_t)v[c];
 }
 
 // The checks every entry makes on its call before it looks at the frames.
@@ -284,3 +374,14 @@ extern "C" int yfv2_resize_yuv422_u8(const yfv2_yuv422_frame* frames, int N, int
     }
     return launch_resize<Yuv422Source>(frames, N, H, W, dst, stream);
 }
+
+namespace yfv2 {
+
+int launch_aug_resize(const AugChunk& a, int cnt, cudaStream_t stream) {
+    const dim3 grid((unsigned)((a.W + kResizeBx - 1) / kResizeBx), (unsigned)((a.H + kResizeBy - 1) / kResizeBy), (unsigned)cnt);
+    aug_resize_kernel<<<grid, dim3(kResizeBx, kResizeBy), 0, stream>>>(a);
+    YFV2_LAUNCH_CHECK();
+    return YFV2_OK;
+}
+
+}  // namespace yfv2

@@ -72,7 +72,11 @@ def main(argv=None):
     ap.add_argument("--save-dir", type=str, default="weights")
     ap.add_argument("--device-aug", action="store_true", help="run contrast_and_brightness (utils/datasets.py:10-16) on the uint8 batch "
                                                               "on the GPU (csrc/k_aug.cu) instead of per image in the data-loader workers")
+    ap.add_argument("--device-aug-resize", action="store_true", help="with --device-aug: add random_resize (utils/datasets.py:54-61)")
+    ap.add_argument("--device-aug-hsv", action="store_true", help="with --device-aug: add augment_hsv (utils/datasets.py:39-51)")
     opt = ap.parse_args(argv)
+    if (opt.device_aug_resize or opt.device_aug_hsv) and not opt.device_aug:
+        ap.error("--device-aug-resize and --device-aug-hsv need --device-aug")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -135,7 +139,8 @@ def main(argv=None):
             imgs = imgs.to(device, non_blocking=True)
             if opt.device_aug and imgs.dtype == torch.uint8:
                 import utils.device_aug
-                imgs = utils.device_aug.img_aug_batch(imgs, out=imgs)                 # datasets.py:63-68 on the device, in place
+                imgs = utils.device_aug.img_aug_batch(imgs, out=imgs, random_resize=opt.device_aug_resize,   # datasets.py:63-68
+                                                      augment_hsv=opt.device_aug_hsv)                  # on the device, in place
             imgs = imgs.float() / 255.0                                           # train.py:101
             targets = targets.to(device, non_blocking=True)
             preds = net(imgs)

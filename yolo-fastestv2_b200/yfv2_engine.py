@@ -97,6 +97,14 @@ class Region(ctypes.Structure):
     _fields_ = [("frame", ctypes.c_int), ("x0", ctypes.c_int), ("y0", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int)]
 
 
+class AugParams(ctypes.Structure):
+    """yfv2_aug_params: one image's contrast (alpha, beta) and random_resize size (rw, rh)."""
+    _fields_ = [("alpha", ctypes.c_float), ("beta", ctypes.c_float), ("rw", ctypes.c_int), ("rh", ctypes.c_int)]
+
+
+AUG_CONTRAST, AUG_RESIZE, AUG_HSV = 1, 2, 4          # yfv2_aug_batch flags (include/yfv2.h)
+
+
 # name -> (restype, argtypes); must list every prototype of include/yfv2.h (tests check this)
 PROTOTYPES = {
     "yfv2_abi_version": (ctypes.c_int, []),
@@ -131,6 +139,10 @@ PROTOTYPES = {
     "yfv2_batch_statistics": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                              ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]),
     "yfv2_aug_contrast_brightness": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_longlong, ctypes.c_void_p]),
+    "yfv2_aug_batch": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                      ctypes.POINTER(AugParams), ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]),
+    "yfv2_debug_bgr2hsv": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_void_p]),
+    "yfv2_debug_hsv2bgr": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_int, ctypes.c_void_p]),
     "yfv2_resize_bgr_u8": (ctypes.c_int, [ctypes.POINTER(Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                           ctypes.c_void_p]),
     "yfv2_resize_yuv420_u8": (ctypes.c_int, [ctypes.POINTER(Yuv420Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
@@ -571,6 +583,82 @@ def contrast_and_brightness(imgs, alpha, beta, out=None):
                                                   ctypes.c_void_p(alpha.data_ptr()), ctypes.c_void_p(beta.data_ptr()), N,
                                                   imgs.numel() // N, _stream(imgs.device)), "aug_contrast_brightness")
     return out
+
+
+def hsv_luts(r):
+    """augment_hsv's LUTs (utils/datasets.py:44-47) for gains r [N, 3] (hue, saturation, value): uint8 [N, 3, 256], built with
+    the reference's arithmetic (int16 x times the float64 gain, floor-mod 180 / clip to 0..255, truncation to uint8)."""
+    import numpy as np
+    r = np.asarray(r, dtype=np.float64).reshape(-1, 3)
+    x = np.arange(0, 256, dtype=np.int16)
+    out = np.empty((r.shape[0], 3, 256), np.uint8)
+    for n, g in enumerate(r):
+        out[n, 0] = ((x * g[0]) % 180).astype(np.uint8)
+        out[n, 1] = np.clip(x * g[1], 0, 255).astype(np.uint8)
+        out[n, 2] = np.clip(x * g[2], 0, 255).astype(np.uint8)
+    return out
+
+
+def augment_batch(imgs, alpha=None, beta=None, rw=None, rh=None, luts=None, out=None):
+    """img_aug (utils/datasets.py:63-68) with random_resize and augment_hsv enabled, on a CUDA uint8 [N, 3, H, W] batch, in the
+    reference's order: contrast_and_brightness (alpha, beta: [N]), then random_resize (rw, rh: [N] intermediate sizes), then
+    augment_hsv (luts: uint8 [N, 3, 256], see hsv_luts).  A step whose arguments are None is skipped.  Returns a new tensor (or
+    writes `out`; `out` may be `imgs` when there is no resize)."""
+    _require_cuda(imgs, "imgs")
+    if imgs.dtype != torch.uint8 or imgs.dim() != 4 or imgs.shape[1] != 3:
+        raise TypeError("augment_batch expects uint8 [N, 3, H, W] images")
+    imgs = imgs.contiguous()
+    N, _, H, W = imgs.shape
+    flags = 0
+    params = (AugParams * N)()
+    if alpha is not None:
+        flags |= AUG_CONTRAST
+        a = [float(v) for v in alpha]
+        b = [float(v) for v in beta]
+        if len(a) != N or len(b) != N:
+            raise ValueError("one (alpha, beta) pair per image")
+        for i in range(N):
+            params[i].alpha, params[i].beta = a[i], b[i]
+    if rw is not None:
+        flags |= AUG_RESIZE
+        w, h = [int(v) for v in rw], [int(v) for v in rh]
+        if len(w) != N or len(h) != N:
+            raise ValueError("one (rw, rh) pair per image")
+        for i in range(N):
+            params[i].rw, params[i].rh = w[i], h[i]
+    lut_dev = None
+    if luts is not None:
+        flags |= AUG_HSV
+        lut_dev = torch.as_tensor(luts, dtype=torch.uint8).to(imgs.device).contiguous()
+        if tuple(lut_dev.shape) != (N, 3, 256):
+            raise ValueError("luts must be [N, 3, 256]")
+    if out is None:
+        out = torch.empty_like(imgs)
+    with torch.cuda.device(imgs.device):
+        _check(lib().yfv2_aug_batch(ctypes.c_void_p(imgs.data_ptr()), ctypes.c_void_p(out.data_ptr()), N, H, W, params,
+                                    ctypes.c_void_p(lut_dev.data_ptr()) if lut_dev is not None else None, flags,
+                                    _stream(imgs.device)), "aug_batch")
+    return out
+
+
+def _hsv_debug(fn, what, pixels, *row_w):
+    """Test hook: uint8 [..., 3] CUDA pixels through the device's cv2.cvtColor conversion."""
+    _require_cuda(pixels, "pixels")
+    pixels = pixels.contiguous()
+    out = torch.empty_like(pixels)
+    with torch.cuda.device(pixels.device):
+        _check(fn(ctypes.c_void_p(pixels.data_ptr()), ctypes.c_void_p(out.data_ptr()), pixels.numel() // 3, *row_w,
+                  _stream(pixels.device)), what)
+    return out
+
+
+def debug_bgr2hsv(pixels):
+    return _hsv_debug(lib().yfv2_debug_bgr2hsv, "debug_bgr2hsv", pixels)
+
+
+def debug_hsv2bgr(pixels):
+    """pixels [h, w, 3]: cv2.cvtColor(pixels, COLOR_HSV2BGR), which rounds the tail of each w-pixel row its own way."""
+    return _hsv_debug(lib().yfv2_debug_hsv2bgr, "debug_hsv2bgr", pixels, pixels.shape[-2] if pixels.dim() >= 2 else 1)
 
 
 def _frame_on_device(f, device):
