@@ -198,6 +198,28 @@ typedef struct yfv2_aug_params {
 } yfv2_aug_params;
 YFV2_API int yfv2_aug_batch(const uint8_t* img, uint8_t* out, int N, int H, int W, const yfv2_aug_params* params,
                             const uint8_t* luts, int flags, void* stream);
+/* ---- img_aug with every line enabled: yfv2_aug_batch plus motion_blur (utils/datasets.py:18-37, img_aug's second step) ----
+ * Takes yfv2_aug_batch's arguments and flags, plus YFV2_AUG_BLUR, and runs contrast -> motion_blur -> random_resize ->
+ * augment_hsv per image.  blur: HOST array [N], one descriptor per image: ksize 0 is an image that drew no blur (the reference's
+ * randint(1, 2) == 2); ksize 2 or 3 is the drawn degree, with taps[0 .. ksize^2 - 1] the fp32 kernel in row-major order as
+ * cv2.filter2D receives it (cv2.warpAffine of diag(ones(degree)) by getRotationMatrix2D((degree/2, degree/2), angle, 1), over
+ * degree, rounded to fp32; yfv2_engine.motion_blur_taps computes it).  A blurred image is
+ *   cv2.filter2D(img, -1, taps): anchor (ksize/2, ksize/2), BORDER_REFLECT_101 per channel, per byte the fp32 fused multiply-add
+ *     chain over the nonzero taps in row-major order from 0, rounded half to even and saturated;
+ *   cv2.normalize(., 0, 255, NORM_MINMAX): min and max over all three channels, scale = 255 * (1 / (max - min)) (0 when the
+ *     image is constant), shift = -min * scale in fp64, byte = rint(fmaf(x, (float)scale, (float)shift)) saturated.
+ * workspace: device, at least yfv2_aug_blur_workspace_bytes(N, H, W) bytes, overlapping neither img nor out; required with
+ * YFV2_AUG_BLUR (it holds each blurred image between the two passes), else ignored, as is blur.  Without YFV2_AUG_BLUR the
+ * call is yfv2_aug_batch.  Every argument, ksize and tap is checked before anything is launched (YFV2_EINVAL). */
+#define YFV2_AUG_BLUR     8
+typedef struct yfv2_aug_blur {
+    int ksize;             /* 0 (no blur), 2 or 3 */
+    float taps[9];         /* [ksize][ksize] row-major */
+} yfv2_aug_blur;
+YFV2_API int yfv2_aug_blur_workspace_bytes(int N, int H, int W, size_t* bytes);
+YFV2_API int yfv2_aug_batch_blur(const uint8_t* img, uint8_t* out, int N, int H, int W, const yfv2_aug_params* params,
+                                 const uint8_t* luts, const yfv2_aug_blur* blur, int flags, void* workspace,
+                                 size_t workspace_bytes, void* stream);
 /* Test hooks: n packed 3-byte pixels through the device's cv2.cvtColor COLOR_BGR2HSV / COLOR_HSV2BGR (any input bytes).  cv2's
  * 8-bit HSV2BGR rounds the last (row_w mod 32) pixels of each row differently from the others (OpenCV 4.13 x86: vector code
  * truncates, the scalar tail rounds), so the pixels are taken as rows of row_w. */

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Training-batch augmentation on the device: img_aug (utils/datasets.py:63-68) with random_resize and augment_hsv enabled.
+"""Training-batch augmentation on the device: img_aug (utils/datasets.py:63-68) with motion_blur, random_resize and augment_hsv
+enabled.
 
   python tools/bench_aug.py [--batch 256 --size 352 --iters 50 --host-images 16]
 
@@ -7,9 +8,12 @@ Times, on a uint8 [batch, 3, size, size] batch resident in HBM, each launch afte
 around the launch alone:
   contrast_us           yfv2_aug_contrast_brightness (the existing kernel, out of place);
   hsv_us / resize_us / all_us   yfv2_aug_batch with contrast + augment_hsv, contrast + random_resize, and all three;
+  blur_us / blur_all_us  yfv2_aug_batch_blur with motion_blur alone and with all four steps, every image blurred (half of them
+                         degree 2, half 3; the reference blurs half of its images, see datasets.py:19);
   *_GBps                 the batch read once plus the batch written once, over the time (the elementwise modes' minimum traffic;
                          the resize modes read about (rw*rh)/(W*H) of each source image more than once, which this does not count).
-host_*_us: the reference's own contrast_and_brightness, random_resize and augment_hsv per image on one core
+host_*_us: the reference's own contrast_and_brightness, motion_blur (blurred images only), random_resize and augment_hsv per
+image on one core
 (cv2.setNumThreads(1)), when the reference checkout is on PYTHONPATH; otherwise they are reported as not measured.
 Prints one JSON line with the GPU name and power limit."""
 import argparse
@@ -66,7 +70,17 @@ def host_times(n_img, size):
     rs = np.random.RandomState(0)
     imgs = [rs.randint(0, 256, (size, size, 3)).astype(np.uint8) for _ in range(n_img)]
     out = {}
-    for name, fn in (("contrast", ds.contrast_and_brightness), ("random_resize", ds.random_resize), ("augment_hsv", ds.augment_hsv)):
+    import random
+
+    def blurred(img):                                                # motion_blur with its randint(1, 2) forced to 1
+        real = random.randint
+        random.randint = lambda lo, hi: 1 if (lo, hi) == (1, 2) else real(lo, hi)
+        try:
+            return ds.motion_blur(img)
+        finally:
+            random.randint = real
+    for name, fn in (("contrast", ds.contrast_and_brightness), ("motion_blur", blurred), ("random_resize", ds.random_resize),
+                     ("augment_hsv", ds.augment_hsv)):
         fn(imgs[0])
         t0 = time.perf_counter()
         for im in imgs:
@@ -97,10 +111,22 @@ def main():
     at, bt = torch.tensor(a, dtype=torch.float32, device="cuda"), torch.tensor(b, dtype=torch.float32, device="cuda")
     lut_t = torch.from_numpy(luts).cuda()
     params = (eng.AugParams * N)(*[eng.AugParams(float(a[i]), float(b[i]), int(rw[i]), int(rh[i])) for i in range(N)])
+    blur = [(2 + i % 2, float(rs.uniform(-360, 360))) for i in range(N)]
+    desc = (eng.AugBlur * N)()
+    for i, (d, ang) in enumerate(blur):
+        desc[i].ksize = d
+        for j, v in enumerate(eng.motion_blur_taps(d, ang).ravel()):
+            desc[i].taps[j] = float(v)
+    nb = ctypes.c_size_t()
+    eng._check(eng.lib().yfv2_aug_blur_workspace_bytes(N, S, S, ctypes.byref(nb)), "aug_blur_workspace_bytes")
+    ws = torch.empty(nb.value, dtype=torch.uint8, device="cuda")
     L, stream = eng.lib(), eng._stream(x.device)
 
     def launch(flags):                                               # arguments built once: the events time the launch alone
         p = lambda t: ctypes.c_void_p(t.data_ptr())                  # noqa: E731
+        if flags & eng.AUG_BLUR:
+            return lambda: eng._check(L.yfv2_aug_batch_blur(p(x), p(out), N, S, S, params, p(lut_t), desc, flags, p(ws), nb.value,
+                                                            stream), "aug_batch_blur")
         return lambda: eng._check(L.yfv2_aug_batch(p(x), p(out), N, S, S, params, p(lut_t), flags, stream), "aug_batch")
 
     modes = {
@@ -110,8 +136,12 @@ def main():
         "hsv": launch(eng.AUG_CONTRAST | eng.AUG_HSV),
         "resize": launch(eng.AUG_CONTRAST | eng.AUG_RESIZE),
         "all": launch(eng.AUG_CONTRAST | eng.AUG_RESIZE | eng.AUG_HSV),
+        "blur": launch(eng.AUG_BLUR),
+        "blur_all": launch(eng.AUG_CONTRAST | eng.AUG_RESIZE | eng.AUG_HSV | eng.AUG_BLUR),
     }
     assert torch.equal(eng.augment_batch(x, a, b, rw, rh, luts), (modes["all"](), out)[1])      # the timed call is the API's
+    assert torch.equal(eng.augment_batch(x, blur=blur), (modes["blur"](), out)[1])
+    assert torch.equal(eng.augment_batch(x, a, b, rw, rh, luts, blur=blur), (modes["blur_all"](), out)[1])
     res = {"gpu": gpu_info(), "batch": N, "size": S, "iters": args.iters}
     moved = 2 * x.numel()
     for name, fn in modes.items():

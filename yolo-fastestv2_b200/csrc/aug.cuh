@@ -95,7 +95,50 @@ struct AugChunk {
     int H, W;
 };
 
-// k_resize.cu: contrast -> random_resize -> (augment_hsv) on the chunk's cnt images; img and out do not overlap
-int launch_aug_resize(const AugChunk& a, int cnt, cudaStream_t stream);
+// A chunk with motion_blur: image n of the chunk with bit n of `blurred` set was filtered by the first pass into
+// ws + n * 3 * H * W, whose byte minimum and maximum are mm[2 n + 1] = 255 - min and mm[2 n] = max; the second pass reads it
+// there through cv2.normalize's byte map instead of reading img through contrast.  The other images take the AugChunk path.
+struct AugBlurChunk : AugChunk {
+    const uint8_t* ws;     // image 0 of the chunk
+    const unsigned* mm;    // image 0 of the chunk
+    unsigned blurred[kAugChunk / 32];
+};
+
+// augment_hsv's state plus the image's 256-byte map from source byte to the byte the later steps see: contrast for an image
+// without blur, normalize for a blurred one (both are functions of the byte alone)
+struct BlurSmem : HsvSmem {
+    uint8_t map[256];
+};
+
+template <class Chunk> struct AugTraits {
+    static constexpr bool kBlur = false;
+    using Smem = HsvSmem;
+};
+template <> struct AugTraits<AugBlurChunk> {
+    static constexpr bool kBlur = true;
+    using Smem = BlurSmem;
+};
+
+// cv2.normalize(NORM_MINMAX, 0..255) of byte x in an image whose bytes span smin..smax
+__device__ __forceinline__ unsigned normalize_byte(unsigned x, unsigned smin, unsigned smax) {
+    const double d = (double)smax - (double)smin;
+    const double scale = d > 2.220446049250313e-16 ? 255.0 * (1.0 / d) : 0.0;
+    const double shift = 0.0 - (double)smin * scale;
+    const float y = __fmaf_rn((float)x, (float)scale, (float)shift);
+    return (unsigned)fminf(fmaxf(rintf(y), 0.f), 255.f);
+}
+
+// Fills t.map for image n of the chunk (256 threads or more; the caller synchronises) and returns where its bytes are read
+__device__ __forceinline__ const uint8_t* stage_map(BlurSmem& t, const AugBlurChunk& a, int n, size_t image_bytes) {
+    const int i = threadIdx.x + threadIdx.y * blockDim.x;
+    const bool bl = (a.blurred[n >> 5] >> (n & 31)) & 1u;
+    if (i < 256) t.map[i] = (uint8_t)(bl ? normalize_byte(i, 255u - a.mm[2 * n + 1], a.mm[2 * n]) : aug_byte(i, a.im[n].alpha, a.im[n].beta));
+    return (bl ? a.ws : a.img) + (size_t)n * image_bytes;
+}
+
+// k_resize.cu: contrast -> random_resize -> (augment_hsv) on the chunk's cnt images; img and out do not overlap.  With an
+// AugBlurChunk the blurred images are read from the workspace through their normalize map.
+template <class Chunk>
+int launch_aug_resize(const Chunk& a, int cnt, cudaStream_t stream);
 
 }  // namespace yfv2

@@ -6,6 +6,10 @@
 //
 // yfv2_aug_batch adds random_resize and augment_hsv (:54-61, :39-51) in img_aug's order; without the resize this file's
 // aug_pixel_kernel runs it elementwise, with it k_resize.cu's aug_resize_kernel (aug.cuh holds the shared pixel arithmetic).
+// yfv2_aug_batch_blur adds motion_blur (:18-37) between contrast and the resize: blur_kernel filters each blurred image into the
+// workspace and reduces its byte range, then the same two kernels read it there through cv2.normalize's byte map.
+#include <cmath>
+
 #include "aug.cuh"
 
 namespace yfv2 {
@@ -39,10 +43,16 @@ contrast_brightness_kernel(const uint8_t* __restrict__ img, uint8_t* __restrict_
     }
 }
 
-// contrast, then augment_hsv when hsv is set, on the B, G, R of plane pixel e (row width W)
-__device__ __forceinline__ void aug_pixel(unsigned& b, unsigned& g, unsigned& r, float al, float be, bool hsv, int e, int W,
-                                          const HsvSmem& t) {
-    b = aug_byte(b, al, be); g = aug_byte(g, al, be); r = aug_byte(r, al, be);
+// contrast (with kMap: the image's byte map instead), then augment_hsv when hsv is set, on the B, G, R of plane pixel e (row
+// width W)
+template <bool kMap>
+__device__ __forceinline__ void aug_pixel(unsigned& b, unsigned& g, unsigned& r, float al, float be, const uint8_t* map, bool hsv,
+                                          int e, int W, const HsvSmem& t) {
+    if (kMap) {
+        b = map[b]; g = map[g]; r = map[r];
+    } else {
+        b = aug_byte(b, al, be); g = aug_byte(g, al, be); r = aug_byte(r, al, be);
+    }
     if (hsv) {
         int ib = (int)b, ig = (int)g, ir = (int)r;
         hsv_lut_pixel(ib, ig, ir, (W & 31) ? e % W : 0, W, t);          // only rows with a tail need the column
@@ -52,10 +62,12 @@ __device__ __forceinline__ void aug_pixel(unsigned& b, unsigned& g, unsigned& r,
 
 // yfv2_aug_batch without the resize: image blockIdx.y of the chunk, elementwise over its plane-sized B, G and R planes; 16
 // pixels per thread and trip (one uint4 per plane) when vec_ok.  Each pixel is read before it is written by the same thread,
-// so img == out is allowed.
+// so img == out is allowed.  With an AugBlurChunk a blurred image is read from the workspace through its normalize map.
+template <class Chunk>
 __global__ void __launch_bounds__(256)
-aug_pixel_kernel(const __grid_constant__ AugChunk a, long long plane, int vec_ok) {
-    __shared__ HsvSmem t;
+aug_pixel_kernel(const __grid_constant__ Chunk a, long long plane, int vec_ok) {
+    constexpr bool kBlur = AugTraits<Chunk>::kBlur;
+    __shared__ typename AugTraits<Chunk>::Smem t;
     const int n = blockIdx.y;
     const bool hsv = a.luts != nullptr;
     if (hsv) {
@@ -64,6 +76,12 @@ aug_pixel_kernel(const __grid_constant__ AugChunk a, long long plane, int vec_ok
     }
     const float al = a.im[n].alpha, be = a.im[n].beta;
     const uint8_t* src = a.img + (size_t)n * 3 * plane;
+    const uint8_t* map = nullptr;
+    if constexpr (kBlur) {
+        src = stage_map(t, a, n, 3 * plane);
+        map = t.map;
+        __syncthreads();
+    }
     uint8_t* dst = a.out + (size_t)n * 3 * plane;
     const long long stride = (long long)gridDim.x * blockDim.x;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -80,7 +98,7 @@ aug_pixel_kernel(const __grid_constant__ AugChunk a, long long plane, int vec_ok
             for (int k = 0; k < 16; ++k) {
                 const int w = k >> 2, sh = 8 * (k & 3);
                 unsigned b = (wb[w] >> sh) & 0xffu, g = (wg[w] >> sh) & 0xffu, r = (wr[w] >> sh) & 0xffu;
-                aug_pixel(b, g, r, al, be, hsv, (int)(v * 16 + k), a.W, t);
+                aug_pixel<kBlur>(b, g, r, al, be, map, hsv, (int)(v * 16 + k), a.W, t);
                 ob[w] |= b << sh; og[w] |= g << sh; orr[w] |= r << sh;
             }
             reinterpret_cast<uint4*>(dst)[v] = make_uint4(ob[0], ob[1], ob[2], ob[3]);
@@ -91,8 +109,86 @@ aug_pixel_kernel(const __grid_constant__ AugChunk a, long long plane, int vec_ok
     }
     for (long long e = e0 + i; e < plane; e += stride) {
         unsigned b = src[e], g = src[plane + e], r = src[2 * plane + e];
-        aug_pixel(b, g, r, al, be, hsv, (int)e, a.W, t);
+        aug_pixel<kBlur>(b, g, r, al, be, map, hsv, (int)e, a.W, t);
         dst[e] = (uint8_t)b; dst[plane + e] = (uint8_t)g; dst[2 * plane + e] = (uint8_t)r;
+    }
+}
+
+// ---- motion_blur's first pass: contrast -> cv2.filter2D into the workspace, and the image's byte minimum and maximum ----------
+// One CTA of 32 x 8 threads per 32 x 32 output tile of one blurred image (blockIdx.z).  The tile and a one-pixel
+// BORDER_REFLECT_101 halo, through contrast, are staged as fp32 in shared memory; each thread runs the fused chain over the
+// taps for 4 rows x 3 channels.  A 2 x 2 kernel (anchor (1, 1): offsets -1..0) travels in the upper left of a 3 x 3 over
+// offsets -1..1 with zeros elsewhere: an fma with a zero tap adds +0 to a sum that is >= 0, so the chain is unchanged.
+constexpr int kBlurMax = 64;                        // blurred images per launch (their taps travel as kernel parameters)
+constexpr int kBlurTx = 32, kBlurTy = 8, kBlurRows = 4;
+struct BlurImage {
+    int n;                                          // image index in the batch
+    float alpha, beta;                              // contrast (1, 0 when off)
+    float taps[9];                                  // 3 x 3 row-major over offsets -1..1
+};
+struct BlurPass {
+    BlurImage im[kBlurMax];
+    const uint8_t* img;                             // image 0 of the batch
+    uint8_t* ws;                                    // image 0 of the batch; mm = the min / max slots, 2 per image
+    unsigned* mm;
+    int H, W;
+};
+
+// BORDER_REFLECT_101 of index i in -1..n (cv2 maps every index of a 1-long axis to 0)
+__device__ __forceinline__ int reflect101(int i, int n) {
+    if (n == 1) return 0;
+    i = i < 0 ? -i : i;
+    return i >= n ? 2 * n - 2 - i : i;
+}
+
+__global__ void __launch_bounds__(kBlurTx * kBlurTy)
+blur_kernel(const __grid_constant__ BlurPass p) {
+    constexpr int TW = kBlurTx + 2, TH = kBlurTy * kBlurRows + 2, NT = kBlurTx * kBlurTy;
+    __shared__ float s[3][TH][TW];
+    __shared__ unsigned red[2][NT / 32];
+    const BlurImage& im = p.im[blockIdx.z];
+    const int H = p.H, W = p.W, tid = threadIdx.y * kBlurTx + threadIdx.x;
+    const size_t plane = (size_t)H * W;
+    const uint8_t* src = p.img + (size_t)im.n * 3 * plane;
+    const int x0 = blockIdx.x * kBlurTx, y0 = blockIdx.y * (kBlurTy * kBlurRows);
+    for (int i = tid; i < 3 * TH * TW; i += NT) {
+        const int c = i / (TH * TW), r = (i / TW) % TH, q = i % TW;
+        const int y = reflect101(min(y0 + r - 1, H), H), x = reflect101(min(x0 + q - 1, W), W);   // beyond W or H: never used
+        s[c][r][q] = (float)aug_byte(__ldg(src + c * plane + (size_t)y * W + x), im.alpha, im.beta);
+    }
+    float k[9];
+#pragma unroll
+    for (int j = 0; j < 9; ++j) k[j] = im.taps[j];
+    __syncthreads();
+    unsigned lo = 255u, hi = 0u;
+    uint8_t* dst = p.ws + (size_t)im.n * 3 * plane;
+    const int x = x0 + threadIdx.x;
+#pragma unroll
+    for (int rr = 0; rr < kBlurRows; ++rr) {
+        const int ty = threadIdx.y + rr * kBlurTy, y = y0 + ty;
+        if (x < W && y < H) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                float acc = 0.f;
+#pragma unroll
+                for (int i = 0; i < 3; ++i)
+#pragma unroll
+                    for (int j = 0; j < 3; ++j) acc = __fmaf_rn(s[c][ty + i][threadIdx.x + j], k[3 * i + j], acc);
+                const unsigned v = (unsigned)fminf(fmaxf(rintf(acc), 0.f), 255.f);
+                dst[c * plane + (size_t)y * W + x] = (uint8_t)v;
+                lo = min(lo, v);
+                hi = max(hi, v);
+            }
+        }
+    }
+    lo = __reduce_min_sync(0xffffffffu, lo);
+    hi = __reduce_max_sync(0xffffffffu, hi);
+    if ((tid & 31) == 0) { red[0][tid >> 5] = lo; red[1][tid >> 5] = hi; }
+    __syncthreads();
+    if (tid == 0) {
+        for (int w = 1; w < NT / 32; ++w) { lo = min(lo, red[0][w]); hi = max(hi, red[1][w]); }
+        atomicMax(p.mm + 2 * im.n, hi);
+        atomicMax(p.mm + 2 * im.n + 1, 255u - lo);
     }
 }
 
@@ -125,6 +221,129 @@ int debug_hsv(const uint8_t* in, uint8_t* out, long long n, int row_w, int to_hs
 
 constexpr int kAugMaxSide = 32768;
 
+// The blur workspace: [N][3][H][W] filtered bytes, then (256-byte aligned) the [N][2] min / max slots
+size_t blur_ws_mm_offset(int N, int H, int W) { return ((size_t)N * 3 * H * W + 255) & ~(size_t)255; }
+size_t blur_ws_bytes(int N, int H, int W) { return blur_ws_mm_offset(N, H, W) + (size_t)N * 2 * sizeof(unsigned); }
+
+bool overlaps(uintptr_t a, size_t na, uintptr_t b, size_t nb) { return a < b + nb && b < a + na; }
+
+// yfv2_aug_batch (allowed = YFV2_AUG_ALL, blur null) and yfv2_aug_batch_blur: every check, then the launches
+int aug_batch(const char* fn, int allowed, const uint8_t* img, uint8_t* out, int N, int H, int W, const yfv2_aug_params* params,
+              const uint8_t* luts, const yfv2_aug_blur* blur, int flags, uint8_t* ws, size_t ws_bytes, void* stream) {
+    if (!img || !out || !params || N <= 0) { set_error("%s: null img / out / params or N <= 0", fn); return YFV2_EINVAL; }
+    if (H <= 0 || W <= 0 || H > kAugMaxSide || W > kAugMaxSide) {
+        set_error("%s: image %dx%d outside 1..%d", fn, W, H, kAugMaxSide);
+        return YFV2_EINVAL;
+    }
+    if (flags & ~allowed) { set_error("%s: unknown flags 0x%x", fn, flags & ~allowed); return YFV2_EINVAL; }
+    const bool resize = flags & YFV2_AUG_RESIZE, hsv = flags & YFV2_AUG_HSV, contrast = flags & YFV2_AUG_CONTRAST;
+    const bool blurring = flags & YFV2_AUG_BLUR;
+    if (hsv && !luts) { set_error("%s: YFV2_AUG_HSV needs luts", fn); return YFV2_EINVAL; }
+    const size_t plane = (size_t)H * W, bytes = (size_t)N * 3 * plane;
+    int nblur = 0;
+    if (blurring) {
+        if (!blur) { set_error("%s: YFV2_AUG_BLUR needs blur descriptors", fn); return YFV2_EINVAL; }
+        if (!ws || ws_bytes < blur_ws_bytes(N, H, W)) {
+            set_error("%s: YFV2_AUG_BLUR needs a workspace of %zu bytes (got %zu%s)", fn, blur_ws_bytes(N, H, W), ws_bytes,
+                      ws ? "" : ", null");
+            return YFV2_EINVAL;
+        }
+        for (int n = 0; n < N; ++n) {
+            const int k = blur[n].ksize;
+            if (k != 0 && k != 2 && k != 3) { set_error("%s: image %d: blur ksize %d not 0, 2 or 3", fn, n, k); return YFV2_EINVAL; }
+            for (int j = 0; j < k * k; ++j) {
+                if (!std::isfinite(blur[n].taps[j])) { set_error("%s: image %d: blur tap %d is not finite", fn, n, j); return YFV2_EINVAL; }
+            }
+            nblur += k != 0;
+        }
+    }
+    const uintptr_t pi = reinterpret_cast<uintptr_t>(img), po = reinterpret_cast<uintptr_t>(out);
+    if (pi < po + bytes && po < pi + bytes && (resize || pi != po)) {
+        set_error("%s: img and out overlap (%s)", fn, resize ? "YFV2_AUG_RESIZE reads neighbours: use another buffer"
+                                                            : "only img == out is allowed");
+        return YFV2_EINVAL;
+    }
+    const uintptr_t pw = reinterpret_cast<uintptr_t>(ws);
+    if (blurring && (overlaps(pw, ws_bytes, pi, bytes) || overlaps(pw, ws_bytes, po, bytes))) {
+        set_error("%s: the workspace overlaps img or out", fn);
+        return YFV2_EINVAL;
+    }
+    if (resize) {
+        for (int n = 0; n < N; ++n) {
+            if (params[n].rw < 1 || params[n].rw > W || params[n].rh < 1 || params[n].rh > H) {
+                set_error("%s: image %d: random_resize size %dx%d outside 1..%d x 1..%d", fn, n, params[n].rw, params[n].rh, W, H);
+                return YFV2_EINVAL;
+            }
+        }
+    }
+    unsigned* mm = nblur ? reinterpret_cast<unsigned*>(ws + blur_ws_mm_offset(N, H, W)) : nullptr;
+    if (nblur) {                                     // first pass: every blurred image into the workspace
+        YFV2_CUDA(cudaMemsetAsync(mm, 0, (size_t)N * 2 * sizeof(unsigned), (cudaStream_t)stream));
+        BlurPass bp{};
+        bp.img = img; bp.ws = ws; bp.mm = mm; bp.H = H; bp.W = W;
+        const dim3 block(kBlurTx, kBlurTy);
+        int cnt = 0;
+        for (int n = 0; n < N; ++n) {
+            const int k = blur[n].ksize;
+            if (k) {
+                BlurImage& b = bp.im[cnt++];
+                b.n = n;
+                b.alpha = contrast ? params[n].alpha : 1.f;
+                b.beta = contrast ? params[n].beta : 0.f;
+                for (int j = 0; j < 9; ++j) b.taps[j] = 0.f;
+                for (int i = 0; i < k; ++i)
+                    for (int j = 0; j < k; ++j) b.taps[3 * i + j] = blur[n].taps[k * i + j];
+            }
+            if (cnt == kBlurMax || (cnt && n == N - 1)) {
+                const dim3 grid((unsigned)((W + kBlurTx - 1) / kBlurTx), (unsigned)((H + kBlurTy * kBlurRows - 1) / (kBlurTy * kBlurRows)),
+                                (unsigned)cnt);
+                blur_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(bp);
+                YFV2_LAUNCH_CHECK();
+                cnt = 0;
+            }
+        }
+    }
+    const int vec_ok = pi % 16 == 0 && po % 16 == 0 && plane % 16 == 0;
+    long long blocks = ((long long)(plane / 16) + 255) / 256;
+    if (blocks < 1) blocks = 1;
+    if (blocks > 4 * sm_count()) blocks = 4 * sm_count();
+    for (int n0 = 0; n0 < N; n0 += kAugChunk) {
+        const int cnt = N - n0 < kAugChunk ? N - n0 : kAugChunk;
+        AugBlurChunk a{};
+        for (int i = 0; i < cnt; ++i) {
+            a.im[i] = params[n0 + i];
+            if (!contrast) { a.im[i].alpha = 1.f; a.im[i].beta = 0.f; }
+            if (nblur && blur[n0 + i].ksize) a.blurred[i >> 5] |= 1u << (i & 31);
+        }
+        a.img = img + (size_t)n0 * 3 * plane;
+        a.out = out + (size_t)n0 * 3 * plane;
+        a.luts = hsv ? luts + (size_t)n0 * 768 : nullptr;
+        a.H = H; a.W = W;
+        bool any = false;
+        for (unsigned m : a.blurred) any |= m != 0;
+        if (any) {                                   // second pass with the workspace: only chunks with a blurred image
+            a.ws = ws + (size_t)n0 * 3 * plane;
+            a.mm = mm + 2 * n0;
+            if (resize) {
+                const int rc = launch_aug_resize(a, cnt, (cudaStream_t)stream);
+                if (rc != YFV2_OK) return rc;
+            } else {
+                aug_pixel_kernel<AugBlurChunk><<<dim3((unsigned)blocks, (unsigned)cnt), 256, 0, (cudaStream_t)stream>>>(
+                    a, (long long)plane, vec_ok && pw % 16 == 0);
+                YFV2_LAUNCH_CHECK();
+            }
+        } else if (resize) {
+            const int rc = launch_aug_resize(static_cast<const AugChunk&>(a), cnt, (cudaStream_t)stream);
+            if (rc != YFV2_OK) return rc;
+        } else {
+            aug_pixel_kernel<AugChunk><<<dim3((unsigned)blocks, (unsigned)cnt), 256, 0, (cudaStream_t)stream>>>(
+                static_cast<const AugChunk&>(a), (long long)plane, vec_ok);
+            YFV2_LAUNCH_CHECK();
+        }
+    }
+    return YFV2_OK;
+}
+
 }  // namespace
 }  // namespace yfv2
 
@@ -143,54 +362,24 @@ extern "C" int yfv2_aug_contrast_brightness(const uint8_t* img, uint8_t* out, co
 
 extern "C" int yfv2_aug_batch(const uint8_t* img, uint8_t* out, int N, int H, int W, const yfv2_aug_params* params,
                               const uint8_t* luts, int flags, void* stream) {
+    return yfv2::aug_batch("aug_batch", YFV2_AUG_ALL, img, out, N, H, W, params, luts, nullptr, flags, nullptr, 0, stream);
+}
+
+extern "C" int yfv2_aug_blur_workspace_bytes(int N, int H, int W, size_t* bytes) {
     using namespace yfv2;
-    if (!img || !out || !params || N <= 0) { set_error("aug_batch: null img / out / params or N <= 0"); return YFV2_EINVAL; }
-    if (H <= 0 || W <= 0 || H > kAugMaxSide || W > kAugMaxSide) {
-        set_error("aug_batch: image %dx%d outside 1..%d", W, H, kAugMaxSide);
+    if (!bytes || N <= 0 || H <= 0 || W <= 0 || H > kAugMaxSide || W > kAugMaxSide) {
+        set_error("aug_blur_workspace_bytes: null bytes, N <= 0 or image %dx%d outside 1..%d", W, H, kAugMaxSide);
         return YFV2_EINVAL;
     }
-    if (flags & ~YFV2_AUG_ALL) { set_error("aug_batch: unknown flags 0x%x", flags & ~YFV2_AUG_ALL); return YFV2_EINVAL; }
-    const bool resize = flags & YFV2_AUG_RESIZE, hsv = flags & YFV2_AUG_HSV, contrast = flags & YFV2_AUG_CONTRAST;
-    if (hsv && !luts) { set_error("aug_batch: YFV2_AUG_HSV needs luts"); return YFV2_EINVAL; }
-    const size_t plane = (size_t)H * W, bytes = (size_t)N * 3 * plane;
-    const uintptr_t pi = reinterpret_cast<uintptr_t>(img), po = reinterpret_cast<uintptr_t>(out);
-    if (pi < po + bytes && po < pi + bytes && (resize || pi != po)) {
-        set_error("aug_batch: img and out overlap (%s)", resize ? "YFV2_AUG_RESIZE reads neighbours: use another buffer"
-                                                               : "only img == out is allowed");
-        return YFV2_EINVAL;
-    }
-    if (resize) {
-        for (int n = 0; n < N; ++n) {
-            if (params[n].rw < 1 || params[n].rw > W || params[n].rh < 1 || params[n].rh > H) {
-                set_error("aug_batch: image %d: random_resize size %dx%d outside 1..%d x 1..%d", n, params[n].rw, params[n].rh, W, H);
-                return YFV2_EINVAL;
-            }
-        }
-    }
-    const int vec_ok = pi % 16 == 0 && po % 16 == 0 && plane % 16 == 0;
-    long long blocks = ((long long)(plane / 16) + 255) / 256;
-    if (blocks < 1) blocks = 1;
-    if (blocks > 4 * sm_count()) blocks = 4 * sm_count();
-    for (int n0 = 0; n0 < N; n0 += kAugChunk) {
-        const int cnt = N - n0 < kAugChunk ? N - n0 : kAugChunk;
-        AugChunk a{};
-        for (int i = 0; i < cnt; ++i) {
-            a.im[i] = params[n0 + i];
-            if (!contrast) { a.im[i].alpha = 1.f; a.im[i].beta = 0.f; }
-        }
-        a.img = img + (size_t)n0 * 3 * plane;
-        a.out = out + (size_t)n0 * 3 * plane;
-        a.luts = hsv ? luts + (size_t)n0 * 768 : nullptr;
-        a.H = H; a.W = W;
-        if (resize) {
-            const int rc = launch_aug_resize(a, cnt, (cudaStream_t)stream);
-            if (rc != YFV2_OK) return rc;
-        } else {
-            aug_pixel_kernel<<<dim3((unsigned)blocks, (unsigned)cnt), 256, 0, (cudaStream_t)stream>>>(a, (long long)plane, vec_ok);
-            YFV2_LAUNCH_CHECK();
-        }
-    }
+    *bytes = blur_ws_bytes(N, H, W);
     return YFV2_OK;
+}
+
+extern "C" int yfv2_aug_batch_blur(const uint8_t* img, uint8_t* out, int N, int H, int W, const yfv2_aug_params* params,
+                                   const uint8_t* luts, const yfv2_aug_blur* blur, int flags, void* workspace,
+                                   size_t workspace_bytes, void* stream) {
+    return yfv2::aug_batch("aug_batch_blur", YFV2_AUG_ALL | YFV2_AUG_BLUR, img, out, N, H, W, params, luts, blur, flags,
+                           static_cast<uint8_t*>(workspace), workspace_bytes, stream);
 }
 
 extern "C" int yfv2_debug_bgr2hsv(const uint8_t* in, uint8_t* out, long long n, void* stream) {

@@ -254,36 +254,69 @@ struct PlanarSource {
     }
 };
 
+// motion_blur's output in the workspace, read through the image's normalize map (staged in shared memory)
+struct MapFrame : AugFrame {
+    const uint8_t* map;
+};
+struct MappedSource {
+    using Desc = MapFrame;
+    const uint8_t* row;
+    size_t plane;
+    const uint8_t* map;
+    __device__ __forceinline__ MappedSource(const MapFrame& f, int r)
+        : row(f.img + (size_t)r * f.W), plane((size_t)f.H * f.W), map(f.map) {}
+    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            p0[c] = map[__ldg(row + c * plane + c0)];
+            p1[c] = map[__ldg(row + c * plane + c1)];
+        }
+    }
+};
+
 // Pixels of random_resize's rw x rh intermediate cv2.resize(img, (rw, rh)), each computed from the source where it is read,
 // so the intermediate image is never stored
+template <class Inner>
 struct NestedSource {
-    using Desc = AugFrame;
-    const AugFrame& f;
+    using Desc = typename Inner::Desc;
+    const Desc& f;
     int r;
-    __device__ __forceinline__ NestedSource(const AugFrame& f_, int r_) : f(f_), r(r_) {}
+    __device__ __forceinline__ NestedSource(const Desc& f_, int r_) : f(f_), r(r_) {}
     __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
-        resize_pixel<PlanarSource>(f, f.W, f.H, c0, r, f.p.rw, f.p.rh, p0);
-        resize_pixel<PlanarSource>(f, f.W, f.H, c1, r, f.p.rw, f.p.rh, p1);
+        resize_pixel<Inner>(f, f.W, f.H, c0, r, f.p.rw, f.p.rh, p0);
+        resize_pixel<Inner>(f, f.W, f.H, c1, r, f.p.rw, f.p.rh, p1);
     }
 };
 
 // yfv2_aug_batch with the resize: one thread per output pixel of image blockIdx.z, the second resize over NestedSource, then
-// augment_hsv on the pixel when the chunk has LUTs
+// augment_hsv on the pixel when the chunk has LUTs.  With an AugBlurChunk the source bytes go through the image's byte map
+// (MappedSource), read from the workspace for a blurred image.
+template <class Chunk>
 __global__ void __launch_bounds__(kResizeBx * kResizeBy)
-aug_resize_kernel(const __grid_constant__ AugChunk a) {
-    __shared__ HsvSmem t;
+aug_resize_kernel(const __grid_constant__ Chunk a) {
+    __shared__ typename AugTraits<Chunk>::Smem t;
     const bool hsv = a.luts != nullptr;
     if (hsv) {
         stage_hsv(t, a.luts + (size_t)blockIdx.z * 768);
+        __syncthreads();
+    }
+    const uint8_t* img = nullptr;                      // with an AugBlurChunk: where the image's bytes are read
+    if constexpr (AugTraits<Chunk>::kBlur) {
+        img = stage_map(t, a, blockIdx.z, 3 * (size_t)a.H * a.W);
         __syncthreads();
     }
     const int x = blockIdx.x * kResizeBx + threadIdx.x;
     const int y = blockIdx.y * kResizeBy + threadIdx.y;
     if (x >= a.W || y >= a.H) return;
     const size_t plane = (size_t)a.H * a.W;
-    const AugFrame f{a.img + (size_t)blockIdx.z * 3 * plane, a.W, a.H, a.im[blockIdx.z]};
     int v[3];
-    resize_pixel<NestedSource>(f, f.p.rw, f.p.rh, x, y, a.W, a.H, v);
+    if constexpr (AugTraits<Chunk>::kBlur) {
+        const MapFrame f{{img, a.W, a.H, a.im[blockIdx.z]}, t.map};
+        resize_pixel<NestedSource<MappedSource>>(f, f.p.rw, f.p.rh, x, y, a.W, a.H, v);
+    } else {
+        const AugFrame f{a.img + (size_t)blockIdx.z * 3 * plane, a.W, a.H, a.im[blockIdx.z]};
+        resize_pixel<NestedSource<PlanarSource>>(f, f.p.rw, f.p.rh, x, y, a.W, a.H, v);
+    }
     if (hsv) hsv_lut_pixel(v[0], v[1], v[2], x, a.W, t);
     uint8_t* out = a.out + (size_t)blockIdx.z * 3 * plane + (size_t)y * a.W + x;
 #pragma unroll
@@ -377,11 +410,14 @@ extern "C" int yfv2_resize_yuv422_u8(const yfv2_yuv422_frame* frames, int N, int
 
 namespace yfv2 {
 
-int launch_aug_resize(const AugChunk& a, int cnt, cudaStream_t stream) {
+template <class Chunk>
+int launch_aug_resize(const Chunk& a, int cnt, cudaStream_t stream) {
     const dim3 grid((unsigned)((a.W + kResizeBx - 1) / kResizeBx), (unsigned)((a.H + kResizeBy - 1) / kResizeBy), (unsigned)cnt);
-    aug_resize_kernel<<<grid, dim3(kResizeBx, kResizeBy), 0, stream>>>(a);
+    aug_resize_kernel<Chunk><<<grid, dim3(kResizeBx, kResizeBy), 0, stream>>>(a);
     YFV2_LAUNCH_CHECK();
     return YFV2_OK;
 }
+template int launch_aug_resize<AugChunk>(const AugChunk&, int, cudaStream_t);
+template int launch_aug_resize<AugBlurChunk>(const AugBlurChunk&, int, cudaStream_t);
 
 }  // namespace yfv2

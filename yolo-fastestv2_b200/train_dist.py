@@ -74,9 +74,10 @@ def main(argv=None):
                                                               "on the GPU (csrc/k_aug.cu) instead of per image in the data-loader workers")
     ap.add_argument("--device-aug-resize", action="store_true", help="with --device-aug: add random_resize (utils/datasets.py:54-61)")
     ap.add_argument("--device-aug-hsv", action="store_true", help="with --device-aug: add augment_hsv (utils/datasets.py:39-51)")
+    ap.add_argument("--device-aug-blur", action="store_true", help="with --device-aug: add motion_blur (utils/datasets.py:18-37)")
     opt = ap.parse_args(argv)
-    if (opt.device_aug_resize or opt.device_aug_hsv) and not opt.device_aug:
-        ap.error("--device-aug-resize and --device-aug-hsv need --device-aug")
+    if (opt.device_aug_resize or opt.device_aug_hsv or opt.device_aug_blur) and not opt.device_aug:
+        ap.error("--device-aug-resize, --device-aug-hsv and --device-aug-blur need --device-aug")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -140,7 +141,8 @@ def main(argv=None):
             if opt.device_aug and imgs.dtype == torch.uint8:
                 import utils.device_aug
                 imgs = utils.device_aug.img_aug_batch(imgs, out=imgs, random_resize=opt.device_aug_resize,   # datasets.py:63-68
-                                                      augment_hsv=opt.device_aug_hsv)                  # on the device, in place
+                                                      augment_hsv=opt.device_aug_hsv,                  # on the device, in place
+                                                      motion_blur=opt.device_aug_blur)
             imgs = imgs.float() / 255.0                                           # train.py:101
             targets = targets.to(device, non_blocking=True)
             preds = net(imgs)

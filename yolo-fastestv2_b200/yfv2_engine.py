@@ -103,6 +103,12 @@ class AugParams(ctypes.Structure):
 
 
 AUG_CONTRAST, AUG_RESIZE, AUG_HSV = 1, 2, 4          # yfv2_aug_batch flags (include/yfv2.h)
+AUG_BLUR = 8                                         # yfv2_aug_batch_blur adds motion_blur
+
+
+class AugBlur(ctypes.Structure):
+    """yfv2_aug_blur: one image's motion_blur kernel (ksize 0: the image drew no blur)."""
+    _fields_ = [("ksize", ctypes.c_int), ("taps", ctypes.c_float * 9)]
 
 
 # name -> (restype, argtypes); must list every prototype of include/yfv2.h (tests check this)
@@ -141,6 +147,10 @@ PROTOTYPES = {
     "yfv2_aug_contrast_brightness": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_longlong, ctypes.c_void_p]),
     "yfv2_aug_batch": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                       ctypes.POINTER(AugParams), ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]),
+    "yfv2_aug_blur_workspace_bytes": (ctypes.c_int, [ctypes.c_int] * 3 + [ctypes.POINTER(ctypes.c_size_t)]),
+    "yfv2_aug_batch_blur": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                           ctypes.POINTER(AugParams), ctypes.c_void_p, ctypes.POINTER(AugBlur), ctypes.c_int,
+                                           ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
     "yfv2_debug_bgr2hsv": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_void_p]),
     "yfv2_debug_hsv2bgr": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_int, ctypes.c_void_p]),
     "yfv2_resize_bgr_u8": (ctypes.c_int, [ctypes.POINTER(Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
@@ -599,11 +609,45 @@ def hsv_luts(r):
     return out
 
 
-def augment_batch(imgs, alpha=None, beta=None, rw=None, rh=None, luts=None, out=None):
-    """img_aug (utils/datasets.py:63-68) with random_resize and augment_hsv enabled, on a CUDA uint8 [N, 3, H, W] batch, in the
-    reference's order: contrast_and_brightness (alpha, beta: [N]), then random_resize (rw, rh: [N] intermediate sizes), then
-    augment_hsv (luts: uint8 [N, 3, 256], see hsv_luts).  A step whose arguments are None is skipped.  Returns a new tensor (or
-    writes `out`; `out` may be `imgs` when there is no resize)."""
+def motion_blur_taps(degree, angle):
+    """motion_blur's kernel (utils/datasets.py:25-29) as filter2D applies it: fp32 [degree, degree], degree 2 or 3.
+
+    cv2.warpAffine(np.diag(np.ones(degree)), cv2.getRotationMatrix2D((degree/2, degree/2), angle, 1), (degree, degree)) / degree
+    restated without cv2: the rotation with libm cos / sin in fp64, inverted as warpAffine inverts it, each destination pixel's
+    source position in warpAffine's fixed point (cvRound of the 1024-scaled terms, + 16, >> 5: 1/32-pixel steps), fp32 bilinear
+    weights, pixels outside the 0/1 diagonal image read as 0, the fp64 weighted sum; then / degree in fp64 and rounded to fp32."""
+    import math
+    import numpy as np
+    if degree not in (2, 3):
+        raise ValueError("motion_blur degree must be 2 or 3")
+    f32 = np.float32
+    c = degree / 2
+    a = angle * (3.1415926535897932384626433832795 / 180)
+    al, be = math.cos(a), math.sin(a)
+    m = [al, be, (1 - al) * c - be * c, -be, al, be * c + (1 - al) * c]          # getRotationMatrix2D
+    d = m[0] * m[4] - m[1] * m[3]
+    d = 1.0 / d if d != 0 else 0.0
+    i00, i01, i10, i11 = m[4] * d, -m[1] * d, -m[3] * d, m[0] * d                # the inverse warpAffine maps with
+    i02, i12 = -i00 * m[2] - i01 * m[5], -i10 * m[2] - i11 * m[5]
+    k = np.zeros((degree, degree))
+    for y in range(degree):
+        x0, y0 = round((i01 * y + i02) * 1024) + 16, round((i11 * y + i12) * 1024) + 16    # round(): half to even, as cvRound
+        for x in range(degree):
+            X, Y = (x0 + round(i00 * x * 1024)) >> 5, (y0 + round(i10 * x * 1024)) >> 5
+            sx, sy, vx, vy = X >> 5, Y >> 5, f32((X & 31) / 32), f32((Y & 31) / 32)
+            w = ((f32(1) - vy) * (f32(1) - vx), (f32(1) - vy) * vx, vy * (f32(1) - vx), vy * vx)
+            s = 0.0
+            for (r, q), wk in zip(((sy, sx), (sy, sx + 1), (sy + 1, sx), (sy + 1, sx + 1)), w):
+                s = s + (1.0 if r == q and 0 <= r < degree else 0.0) * float(wk)
+            k[y, x] = s
+    return (k / degree).astype(f32)
+
+
+def augment_batch(imgs, alpha=None, beta=None, rw=None, rh=None, luts=None, out=None, blur=None):
+    """img_aug (utils/datasets.py:63-68) on a CUDA uint8 [N, 3, H, W] batch, in the reference's order: contrast_and_brightness
+    (alpha, beta: [N]), then motion_blur (blur: [N] of None for an image that drew no blur, or its (degree, angle)), then
+    random_resize (rw, rh: [N] intermediate sizes), then augment_hsv (luts: uint8 [N, 3, 256], see hsv_luts).  A step whose
+    arguments are None is skipped.  Returns a new tensor (or writes `out`; `out` may be `imgs` when there is no resize)."""
     _require_cuda(imgs, "imgs")
     if imgs.dtype != torch.uint8 or imgs.dim() != 4 or imgs.shape[1] != 3:
         raise TypeError("augment_batch expects uint8 [N, 3, H, W] images")
@@ -634,10 +678,25 @@ def augment_batch(imgs, alpha=None, beta=None, rw=None, rh=None, luts=None, out=
             raise ValueError("luts must be [N, 3, 256]")
     if out is None:
         out = torch.empty_like(imgs)
+    p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None             # noqa: E731
     with torch.cuda.device(imgs.device):
-        _check(lib().yfv2_aug_batch(ctypes.c_void_p(imgs.data_ptr()), ctypes.c_void_p(out.data_ptr()), N, H, W, params,
-                                    ctypes.c_void_p(lut_dev.data_ptr()) if lut_dev is not None else None, flags,
-                                    _stream(imgs.device)), "aug_batch")
+        if blur is None:
+            _check(lib().yfv2_aug_batch(p(imgs), p(out), N, H, W, params, p(lut_dev), flags, _stream(imgs.device)), "aug_batch")
+            return out
+        if len(blur) != N:
+            raise ValueError("one blur entry (None or (degree, angle)) per image")
+        desc = (AugBlur * N)()
+        for i, d in enumerate(blur):
+            if d is not None:
+                k = motion_blur_taps(int(d[0]), float(d[1]))
+                desc[i].ksize = k.shape[0]
+                for j, v in enumerate(k.ravel()):
+                    desc[i].taps[j] = float(v)
+        nb = ctypes.c_size_t()
+        _check(lib().yfv2_aug_blur_workspace_bytes(N, H, W, ctypes.byref(nb)), "aug_blur_workspace_bytes")
+        ws = torch.empty(nb.value, dtype=torch.uint8, device=imgs.device)
+        _check(lib().yfv2_aug_batch_blur(p(imgs), p(out), N, H, W, params, p(lut_dev), desc, flags | AUG_BLUR, p(ws), nb.value,
+                                         _stream(imgs.device)), "aug_batch_blur")
     return out
 
 
