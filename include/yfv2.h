@@ -425,11 +425,28 @@ YFV2_API int yfv2_trainer_debug_ops(const yfv2_trainer* t, yfv2_trainer_op* ops_
 YFV2_API int yfv2_trainer_debug_tensors(const yfv2_trainer* t, yfv2_trainer_tensor* tens_host, int cap, int* n);
 YFV2_API int yfv2_trainer_debug_layout(const yfv2_trainer* t, long long* layout_host);
 
-/* ---- test hook: how a head launch of a forward on `workspace` reads its 5x5 depthwise taps ------------------------------
- * which: 0 heads2.a, 1 heads2.b, 2 heads3.a, 3 heads3.b.  Returns 1 when the launch stages the input windows in shared memory,
- * 0 when it reads the planes, < 0 on a bad argument (workspace NULL included: the choice depends on the plane addresses).
- * Host only: workspace is not dereferenced. */
-YFV2_API int yfv2_debug_heads_staged(const yfv2_plan* plan, const void* workspace, int which);
+/* ---- test hook: the kernel launches of a whole forward, as the forward itself chooses them ----------------------------------
+ * Host only: nothing is launched and workspace is not dereferenced; its address decides the kernels that need 16-byte-aligned
+ * planes (NULL: a 16-byte-aligned workspace).  is_u8: a uint8 input; sms: the GPU's multiprocessors (0: this device's count, 132
+ * without a device).  Writes min(cap, count) records and returns the count in *n (cap 0 with a NULL array queries it); an argument
+ * the forward would refuse is refused here with the same code and message.
+ *   kernel:   the demangled name after yfv2::(anonymous namespace)::, without spaces ("walk::blk_kernel<24,2>", "head2_kernel")
+ *   grid:     fixed grid; persistent: grid[0] is the SM count, and the launch runs min(items, CTAs per SM by occupancy x grid[0])
+ *             CTAs that walk the items
+ *   R, bands: block launches: rows per band, bands per image (items = N x bands); G: the step of walk::blk_kernel<K,1>, 0 elsewhere
+ *   window_stride: heads: channel stride (floats) of a staged 5x5 window slot; 0: the stencils read the planes */
+typedef struct yfv2_launch {
+    char kernel[32];
+    int first, last;             /* fused stages [first, last) (yfv2_plan_stage_name) */
+    long long smem;              /* dynamic shared memory, bytes */
+    int grid[3];
+    int persistent;
+    int items;
+    int R, bands, G;
+    int window_stride;
+} yfv2_launch;
+YFV2_API int yfv2_plan_debug_launches(const yfv2_plan* plan, const void* workspace, int is_u8, int sms, yfv2_launch* out, int cap,
+                                      int* n);
 
 /* ---- test hook: one pointwise contraction on the tensor-core engine (3xTF32), out[n][p] = sum_k w[n][k]*x[k][p] ----
  * x: [K][P], w: [N][K], out: [N][P], pack_ws: unused (kept for ABI stability), may be NULL. */

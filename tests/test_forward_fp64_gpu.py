@@ -1,6 +1,7 @@
 """Every kernel launch of the forward, one at a time, against an fp64 restatement of the same operation (oracle/net.py with
-float64 weights), at band geometries picked with the dispatch model (tests/net_dispatch.py) so that together the cases reach
-every (launch site, variant) cell: one-row, multi-row and partial-last bands, chains, whole-image kernels, both head kernels.
+float64 weights), at band geometries picked from the library's launch records (tests/net_dispatch.py) so that together the cases
+reach every (launch site, variant) cell: one-row, multi-row and partial-last bands on the band walks and on the banded kernels,
+chains, whole-image kernels, both head kernels with and without staged windows.
 
 Each launch is fed the input the GPU actually consumed (the taps gathered right before it runs, sliced on the device to the
 checked images and promoted to float64), so error does not compound across launches and one tight bound holds for all of them.
@@ -43,6 +44,10 @@ CASES = {
     "24x992x320": (24, 992, 320, 3, 80, (0, 23)),      # the same with a partial last band
     "2x96x128c150": (2, 96, 128, 3, 150, None),        # head2_kernel
     "2x128x128a2c20": (2, 128, 128, 2, 20, None),      # other anchor and class counts
+    "1x128x1280": (1, 128, 1280, 3, 80, None),         # past every walk's fit limit: banded K = 24 / 48 kernels, R = 1
+    "24x352x1280": (24, 352, 1280, 3, 80, (0, 23)),    # banded blk_kernel<24, 1> and <48, 1>, R > 1
+    "48x256x1280": (48, 256, 1280, 3, 80, (0, 47)),    # banded blk_kernel<48, 1> with a partial last band
+    "1x960x32c150": (1, 960, 32, 3, 150, None),        # head2_kernel reading the planes (a 2-column map)
 }
 SEED = {name: 1000 + 10 * i for i, name in enumerate(CASES)}
 
@@ -55,7 +60,7 @@ def case_cells(sms):
 
 
 def test_cases_cover_every_reachable_cell():
-    """With 132 SMs (H100 SXM), the cases reach every cell any plan of the dispatch model's search space reaches."""
+    """With 132 SMs (H100 SXM), the cases reach every cell any plan of the search space reaches."""
     assert set(nd.reachable(132)) == nd.ALL_CELLS
     missing = nd.ALL_CELLS - case_cells(132)
     assert not missing, {cl: nd.find_case(cl, 132) for cl in missing}
@@ -102,9 +107,8 @@ def reference(L, sd, ins):
         return [onet.stem(sd, ins[0])]
     if L.blocks:
         y = ins[0]
-        for b in L.blocks:
-            bname, _, stride, _ = nd.BLOCKS[b]
-            y = onet.shuffle_block(sd, y, "backbone.%s." % bname, stride)
+        for bname in L.names:
+            y = onet.shuffle_block(sd, y, "backbone.%s." % bname, nd.block_stride(bname))
         return [y]
     if name == "fpn.S3":
         return [onet.reduce_s3(sd, ins[0])]
@@ -141,9 +145,10 @@ def test_every_launch_against_fp64(name):
     preds = m(x)
     full = [p[idx].double().cpu() for p in preds]
     plan = next(iter(m._plans.values()))
-    model = nd.launches(n, h, w, a, c, sm_count())
-    assert plan.stage_names == nd.STAGE_NAMES and plan.stage_groups == nd.stage_groups(h, w)
-    assert plan.forward_launches == len(model)
+    model = nd.plan_launches(plan)
+    groups = plan.stage_groups
+    assert plan.stage_names == nd.STAGE_NAMES and plan.forward_launches == len(model)
+    assert [(L.first, L.last) for L in model] == [(g, g + groups.count(g)) for g in sorted(set(groups))]
     x64 = x[idx].double().cpu()
     rows = []
     for L in model:
@@ -161,7 +166,7 @@ def test_every_launch_against_fp64(name):
     # the stem again, on uint8 pixels: the reference divides by 255 in fp64
     xu8 = (x * 255).to(torch.uint8)
     plan.forward_range(xu8, preds, 0, 1)
-    L = nd.launches(n, h, w, a, c, sm_count(), u8=True)[0]
+    L = nd.plan_launches(plan, u8=True)[0]
     rows.append((L, nerr(gather(plan, 0, idx), onet.stem(sd64, xu8[idx].double().cpu() / 255))))
     with torch.no_grad():
         ref = onet.forward(sd64, x64)
@@ -177,7 +182,8 @@ def test_every_launch_against_fp64(name):
     assert e2e <= E2E_BOUND, e2e
 
 
-KERNEL_RE = re.compile(r"\b(stem_kernel|blk_kernel|blk_s2_image_kernel|blk_chain_kernel|fpn_kernel|head_kernel|head2_kernel)(<[^>]*>)?")
+KERNEL_RE = re.compile(r"\b(stem_kernel|(?:walk::)?blk_kernel|blk_s2_image_kernel|blk_chain_kernel|fpn_kernel|head_kernel|head2_kernel)"
+                       r"(<[^>]*>)?")
 # The activity tracer keeps only device records whose timestamps, converted to the host clock, fall inside the session's
 # window; a forward of microsecond kernels recorded right at a window edge can lose records to that conversion.  The recorded
 # forward therefore sits in the middle of its session, with this much idle host time on either side.
@@ -222,14 +228,14 @@ def traced_launches(fn, path):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(CASES))
 def test_launches_match_the_dispatch_model(name, tmp_path, tracer_ready):
-    """Kernel names and, where the host code fixes them, grids of one forward, from a CUDA activity trace."""
+    """Kernel names and, where the launch records fix them, grids of one forward, from a CUDA activity trace."""
     m, _, x, _ = setup(name)
     n, h, w, a, c, _ = CASES[name]
     preds = m(x)
     plan = next(iter(m._plans.values()))
     got = traced_launches(lambda: plan.forward(x, preds), tmp_path / "forward.json")
     sms = sm_count()
-    model = nd.launches(n, h, w, a, c, sms)
+    model = nd.plan_launches(plan)
     table = "\n".join("  corr %d ts %.1f %s grid %s" % (corr, ts, k, grid) for k, grid, corr, ts in got)
     assert [k for k, _, _, _ in got] == [L.kernel for L in model], "model %s, trace:\n%s" % ([L.kernel for L in model], table)
     for L, (_, grid, _, _) in zip(model, got):

@@ -36,18 +36,16 @@ def test_matches_the_global_load_heads(golden_dir, n, h, w, a, c, images):
 
 
 def staged(n, h, w, a, c):
-    """yfv2_debug_heads_staged of heads2.a, heads2.b, heads3.a, heads3.b for the plan and workspace a forward of (n, h, w, a, c)
-    runs on."""
-    import yfv2_engine
+    """1 where heads2.a, heads2.b, heads3.a, heads3.b stage their input windows (a record with a window stride), 0 where they read
+    the planes, for the plan and workspace a forward of (n, h, w, a, c) runs on."""
     m = MK.make_model(synth.make_state_dict(5, classes=c, anchor_num=a), a, c)
     m(synth.make_images(6, n, h, w).cuda())
     plan = next(iter(m._plans.values()))
-    ws = ctypes.c_void_p(plan.workspace.data_ptr())
-    return [yfv2_engine.lib().yfv2_debug_heads_staged(plan._h, ws, i) for i in range(4)]
+    return [int(r["window_stride"] > 0) for r in plan.launches() if r["kernel"].startswith("head")]
 
 
 @pytest.mark.gpu
-def test_staged_path_on_both_sides_of_the_fit_rule():
+def test_window_stride_on_both_sides_of_the_fit_rule():
     """The window (11 rows x 28 floats at 22x22, three 8-channel slots) fits next to the weights of all three kernels with two CTAs
     per SM at 352^2, 640^2 and 150 classes; at 32x2560 the 2x160 map's slot of 6 rows x 164 floats does not, while its 1x80 map
     does; at 4096x32 the 128x1 map's chunks span 128 rows and do not fit either."""
@@ -57,7 +55,7 @@ def test_staged_path_on_both_sides_of_the_fit_rule():
     assert staged(1, 32, 2560, 3, 80) == [0, 0, 1, 1]
     assert staged(1, 4096, 32, 3, 80) == [1, 1, 0, 0]
     import yfv2_engine
-    assert yfv2_engine.lib().yfv2_debug_heads_staged(None, None, 0) < 0
+    assert yfv2_engine.lib().yfv2_plan_debug_launches(None, None, 0, 0, None, 0, ctypes.byref(ctypes.c_int())) < 0
 
 
 @pytest.mark.gpu

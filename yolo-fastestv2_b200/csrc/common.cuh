@@ -125,19 +125,59 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
 bool pdl_take();                 // true if the next launch may overlap its predecessor; arms the flag
 void pdl_reset();                // next launch is a plain one
 bool pdl_allowed();              // PDL enabled for the current API call
-template <class Arg, class Kern>
-cudaError_t launch_k(Kern kern, int grid, int block, size_t smem, cudaStream_t s, bool pdl, const Arg& arg) {
+// kern: a __global__ function taking one argument struct, arg: that struct
+inline cudaError_t launch_k(const void* kern, dim3 grid, int block, size_t smem, cudaStream_t s, bool pdl, const void* arg) {
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    cfg.gridDim = grid; cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = smem; cfg.stream = s;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kern, arg);
+    void* args[1] = {const_cast<void*>(arg)};
+    return cudaLaunchKernelExC(&cfg, kern, args);
 }
 
-// ---- kernel launchers (defined in the k_*.cu files) ---------------------------------------------------
+// ---- the forward's launches: described on the host (plan.cu plan_launches), then launched --------------------
+// Every kernel a forward can launch.  kernel_ref() maps an id to the __global__ function and its name, both from one
+// YFV2_KERNEL_REF expression: the name is the demangled symbol after yfv2::(anonymous namespace)::, without spaces.
+enum class KernelId {
+    stem_f32, stem_u8, chain96, s2_image96, fpn192, fpn288, head0, head1, head2,
+    blk24_s1, blk24_s2, blk48_s1, blk48_s2, blk96_s1, blk96_s2,     // blk_kernel<K, STRIDE>
+    walk24_s1, walk48_s1, walk24_s2, walk48_s2,                     // walk::blk_kernel<K, STRIDE>
+};
+struct KernelRef { const void* fn; const char* name; };
+#define YFV2_KERNEL_REF(...) yfv2::KernelRef{reinterpret_cast<const void*>(&__VA_ARGS__), #__VA_ARGS__}
+KernelRef kernel_ref(KernelId k);           // k_net.cu
+KernelRef stem_kernel_ref(bool u8);         // k_stem.cu
+
+constexpr int kThreads = 256;               // threads per CTA of every forward kernel
+
+// One kernel launch of a forward: what it runs over which fused stages, with which grid and shared memory.
+struct Launch {
+    KernelId kernel;
+    int first, last;            // fused stages [first, last) of the plan
+    size_t smem;                // dynamic shared memory, bytes
+    dim3 grid;                  // fixed grid; persistent: grid.x is the SM count, and the launch takes
+    bool persistent;            //   min(items, CTAs per SM by occupancy x grid.x) CTAs that walk the items
+    int items;                  // work items the grid walks
+    int R, bands, G;            // block launches: rows per band, bands per image, walk step (walk::blk_kernel<K, 1>)
+    int CS;                     // heads: channel stride of a staged window slot (floats); 0: the stencils read the planes
+    struct { int TRo, TWo, S, tilesX, tilesY; bool vec; } stem;    // stem tiling; vec: staged asynchronously if x is aligned
+};
+
+// Records of single launches (k_net.cu, k_stem.cu); an argument error is set_error + its code
+int describe_stem(int N, int H, int W, int is_u8, int sms, Launch& L);
+int describe_blk_s1(int K, const Planes& P, int nblk, int N, int sms, Launch& L);
+int describe_blk_s2(int K, const Planes& in, const Planes& out, int N, int sms, Launch& L);
+int describe_fpn(int which, int H, int W, int N, int sms, Launch& L);
+int describe_heads(int half, const Planes& sIn, const Planes& tcls, const Planes& treg, int A, int C, int N, int sms, Launch& L);
+
+// The one launch path: shared-memory attribute, the occupancy-sized grid of a persistent launch, the launch, its check
+int launch(const Launch& L, const void* args, cudaStream_t s);
+
+// Argument structs of the launches, filled from the record (k_net.cu, k_stem.cu)
 struct StemArgs {
+    const Launch& launch;    // describe_stem's record
     const void* x;       // [N,3,H,W] fp32 or uint8
     int is_u8;
     int N, H, W;         // input dims
@@ -145,6 +185,14 @@ struct StemArgs {
     const float* wpack;  // STEM layout
 };
 int launch_stem(const StemArgs& a, cudaStream_t s);
+int blk_launch_s1(const Launch& L, int K, const Planes& P, const ChanTab* tin, const ChanTab* tout, const float* const* w1,
+                  const float* const* wdw, const float* const* w2, cudaStream_t s);
+int blk_launch_s2(const Launch& L, int K, const Planes& in, const Planes& out, const ChanTab& tin, const ChanTab& tout, const float* wdwp,
+                  const float* wp, const float* w1, const float* wdwm, const float* w2, cudaStream_t s);
+int fpn_launch(const Launch& L, const Planes& c3, const ChanTab& t3, const Planes& c2, const ChanTab& t2, const Planes& out,
+               const float* pw, int N, cudaStream_t s);
+int heads_launch(const Launch& L, int half, const Planes& sIn, const Planes& tcls, const Planes& treg, const float* const wdw[2],
+                 const float* const wpw[2], float* reg, float* obj, float* cls, int A, int C, int N, cudaStream_t s);
 
 // conv1x1 backward with an optional scratch for per-block partial weight gradients (k_train.cu; the C-ABI operator passes none)
 int conv1x1_bwd_impl(const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias, int N, int K, int M, int HW,

@@ -21,8 +21,7 @@ namespace yfv2 {
 namespace {
 using namespace tc;
 
-constexpr int kThreads = 256;                 // 8 warps, one 16-pixel row tile each at a time
-constexpr int kWarps = kThreads / 32;
+constexpr int kWarps = kThreads / 32;         // 8 warps, one 16-pixel row tile each at a time
 constexpr int kMaxChain = 7;
 constexpr size_t kChainBudget = 110 * 1024;   // whole-image bands below this keep two CTAs per SM
 constexpr size_t kBandBudget = 110 * 1024;
@@ -288,8 +287,7 @@ blk_kernel(const __grid_constant__ BlkArgs p) {
 // value is computed with the same operations in the same order as blk_kernel<K, 2> (an mma.sync output row depends only on its
 // own A row), so the outputs are bit-identical to it.
 //
-// The kernel keeps the name blk_kernel<K, 2> (in namespace walk) and the grid of one CTA per band: profiler traces and launch
-// models that know the banded kernel describe it unchanged.
+// The kernel keeps the grid of one CTA per band; profiler traces and the launch records name it walk::blk_kernel<K, 2>.
 namespace walk {
 constexpr int G = 1;              // output rows per step
 
@@ -866,44 +864,12 @@ blk_chain_kernel(const __grid_constant__ BlkArgs p) {
     }
 }
 
-int persistent_grid(long long items, int per_sm) {
-    const long long cap = (long long)per_sm * sm_count();
-    return (int)(items < cap ? items : cap);
-}
-
-template <class Kern>
-int smem_attr(Kern kern, size_t bytes) {
-    YFV2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    return YFV2_OK;
-}
-
 // rows per band: the largest band within the budget, shrunk while the grid would leave SMs idle
-int blk_rows(int K, int stride, int Ho, int Wi, int N) {
+int blk_rows(int K, int stride, int Ho, int Wi, int N, int sms) {
     int R = Ho;
     while (R > 1 && blk_smem_bytes(K, stride, R, Wi) > kBandBudget) --R;
-    while (R > 1 && (size_t)N * ((Ho + R - 1) / R) < (size_t)2 * sm_count()) R = (R + 1) / 2;
+    while (R > 1 && (size_t)N * ((Ho + R - 1) / R) < (size_t)2 * sms) R = (R + 1) / 2;
     return R;
-}
-
-template <int K, int STRIDE>
-int run_blk(BlkArgs& a, int N, cudaStream_t s) {
-    a.bands = (a.Ho + a.R - 1) / a.R;
-    a.items = N * a.bands;
-    const size_t bytes = blk_smem_bytes(K, STRIDE, a.R, a.Wi);
-    if (bytes > kSmemCap) { set_error("block: a %d-row band of %d columns does not fit in shared memory", a.R, a.Wi); return YFV2_EUNSUPPORTED; }
-    if (int rc = smem_attr(blk_kernel<K, STRIDE>, bytes)) return rc;
-    int grid = a.items;
-    // A stride-1 block keeps its weights resident in a persistent grid (K=96 at 352x352: 182 -> 120 us on an H100).  The
-    // stride-2 blocks were measured slower that way (stage4.0 610 -> 760 us, stage2.0 463 -> 488 us) and take one CTA per item;
-    // K = 24 and 48 run on walk::blk_kernel wherever it fits.
-    if (STRIDE == 1 && a.nblk == 1) {
-        int per_sm = 0;
-        YFV2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, blk_kernel<K, STRIDE>, kThreads, bytes));
-        grid = persistent_grid(a.items, per_sm > 0 ? per_sm : 1);
-    }
-    YFV2_CUDA(launch_k(blk_kernel<K, STRIDE>, grid, kThreads, bytes, s, pdl_take(), a));
-    YFV2_LAUNCH_CHECK();
-    return YFV2_OK;
 }
 
 // The band walk stages whole plane rows by 16-byte copies from planes with a one-pixel frame; the plan's pool planes are such
@@ -927,40 +893,22 @@ int blk_s1_walk_step(int K, const Planes& P) {
     return 0;
 }
 
-template <int K, int STRIDE>
-int run_blk_walk(BlkArgs& a, int N, cudaStream_t s) {
-    a.bands = (a.Ho + a.R - 1) / a.R;
-    a.items = N * a.bands;
-    auto kern = walk::blk_kernel<K, STRIDE>;
-    const size_t bytes = STRIDE == 2 ? walk::smem_bytes(K, a.Wi, a.in.Ws) : walk::s1_smem_bytes(K, a.G, a.Wi, a.in.Ws);
-    if (int rc = smem_attr(kern, bytes)) return rc;
-    int grid = a.items;       // stride 2: one CTA per band; stride 1: the persistent grid of blk_kernel<K, 1>
-    if (STRIDE == 1) {
-        int per_sm = 0;
-        YFV2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, bytes));
-        grid = persistent_grid(a.items, per_sm > 0 ? per_sm : 1);
-    }
-    YFV2_CUDA(launch_k(kern, grid, kThreads, bytes, s, pdl_take(), a));
-    YFV2_LAUNCH_CHECK();
-    return YFV2_OK;
+// R rows per band of Ho output rows, N images
+void set_bands(Launch& L, int R, int Ho, int N) {
+    L.R = R;
+    L.bands = (Ho + R - 1) / R;
+    L.items = N * L.bands;
 }
-
-template <int K>
-int dispatch_blk(int stride, BlkArgs& a, int N, cudaStream_t s) {
-    return stride == 1 ? run_blk<K, 1>(a, N, s) : run_blk<K, 2>(a, N, s);
+// a grid of CTAs on each of sms SMs (as many as occupancy allows), at most one per item
+void set_persistent(Launch& L, int sms) {
+    L.persistent = true;
+    L.grid = dim3((unsigned)sms);
 }
-
-// whole-image kernels: one CTA per SM, a persistent grid over the N images
-template <class Kern>
-int run_whole_image(Kern kern, size_t bytes, BlkArgs& a, int N, cudaStream_t s) {
-    a.R = a.Ho; a.bands = 1; a.items = N;
-    if (int rc = smem_attr(kern, bytes)) return rc;
-    int per_sm = 0;
-    YFV2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, bytes));
-    YFV2_CUDA(launch_k(kern, persistent_grid(N, per_sm > 0 ? per_sm : 1), kThreads, bytes, s, pdl_take(), a));
-    YFV2_LAUNCH_CHECK();
-    return YFV2_OK;
-}
+// blk_kernel<K, STRIDE> and walk::blk_kernel<K, STRIDE> (K = 24 / 48 only) by [STRIDE - 1][K = 24, 48, 96]
+constexpr KernelId kBlkKernel[2][3] = {{KernelId::blk24_s1, KernelId::blk48_s1, KernelId::blk96_s1},
+                                       {KernelId::blk24_s2, KernelId::blk48_s2, KernelId::blk96_s2}};
+constexpr KernelId kWalkKernel[2][2] = {{KernelId::walk24_s1, KernelId::walk48_s1}, {KernelId::walk24_s2, KernelId::walk48_s2}};
+int width_index(int K) { return K == 24 ? 0 : K == 48 ? 1 : 2; }
 
 // ---- FPN reducers -------------------------------------------------------------------------------------------------------
 struct FpnArgs {
@@ -1050,7 +998,7 @@ __host__ constexpr size_t head_weight_bytes(int NP) { return ((size_t)pw_smem_fl
 // 96-column tiles of a [192][72] folded matrix; the reg branch (4A <= 32 columns) keeps one tile.  It contracts 48 columns at a
 // time, so that the A fragments (36 registers) and one pass of accumulators (24) leave room for two CTAs per SM.
 //
-// The dw5x5 taps come from a window staged in shared memory where it fits (p.CS > 0, heads_launch): per k-step, the item's rows
+// The dw5x5 taps come from a window staged in shared memory where it fits (p.CS > 0, describe_heads): per k-step, the item's rows
 // with their 2-row halo for the k-step's 8 channels, whole framed rows by 16-byte cp.async into a ring of kHeadSlots slots.  The
 // copies of k-step j + 2 of the CTA's sequence (which runs on into its next item) are issued after the barrier of k-step j, when
 // every warp is done with the slot they overwrite; so every warp takes part in every k-step, pixels or not.  A slot keeps the
@@ -1258,7 +1206,7 @@ pw_test_kernel(const float* __restrict__ x, const float* __restrict__ w, float* 
 template <int K, int NP>
 int run_pw_test(const float* x, const float* w, float* out, int N, int P, cudaStream_t s) {
     const size_t bytes = (size_t)K * w_stride(NP) * sizeof(float);
-    if (int rc = smem_attr(pw_test_kernel<K, NP>, bytes)) return rc;
+    YFV2_CUDA(cudaFuncSetAttribute(pw_test_kernel<K, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     pw_test_kernel<K, NP><<<(P + 16 * kWarps - 1) / (16 * kWarps), kThreads, bytes, s>>>(x, w, out, N, P);
     YFV2_LAUNCH_CHECK();
     return YFV2_OK;
@@ -1273,73 +1221,148 @@ bool blk_s1_chainable(int K, int H, int W) {
     return bytes <= kChainBudget || (K == 96 && bytes <= kSmemCap);
 }
 
-int blk_launch_s1(int K, const Planes& P, int nblk, const ChanTab* tin, const ChanTab* tout, const float* const* w1,
-                  const float* const* wdw, const float* const* w2, int N, cudaStream_t s) {
+// The first reference to a kernel from host code orders the kernels in the cubin: the cases keep the order of the launchers they
+// replaced, so the SASS dump of the library compares byte for byte across such host-only changes.
+KernelRef kernel_ref(KernelId k) {
+    switch (k) {
+    case KernelId::stem_f32: return stem_kernel_ref(false);
+    case KernelId::stem_u8: return stem_kernel_ref(true);
+    case KernelId::chain96: return YFV2_KERNEL_REF(blk_chain_kernel<96>);
+    case KernelId::s2_image96: return YFV2_KERNEL_REF(blk_s2_image_kernel<96>);
+    case KernelId::fpn192: return YFV2_KERNEL_REF(fpn_kernel<192>);
+    case KernelId::fpn288: return YFV2_KERNEL_REF(fpn_kernel<288>);
+    case KernelId::head0: return YFV2_KERNEL_REF(head_kernel<0>);
+    case KernelId::head1: return YFV2_KERNEL_REF(head_kernel<1>);
+    case KernelId::head2: return YFV2_KERNEL_REF(head2_kernel);
+    case KernelId::blk24_s1: return YFV2_KERNEL_REF(blk_kernel<24,1>);
+    case KernelId::blk24_s2: return YFV2_KERNEL_REF(blk_kernel<24,2>);
+    case KernelId::blk48_s1: return YFV2_KERNEL_REF(blk_kernel<48,1>);
+    case KernelId::blk48_s2: return YFV2_KERNEL_REF(blk_kernel<48,2>);
+    case KernelId::blk96_s1: return YFV2_KERNEL_REF(blk_kernel<96,1>);
+    case KernelId::blk96_s2: return YFV2_KERNEL_REF(blk_kernel<96,2>);
+    case KernelId::walk24_s1: return YFV2_KERNEL_REF(walk::blk_kernel<24,1>);
+    case KernelId::walk48_s1: return YFV2_KERNEL_REF(walk::blk_kernel<48,1>);
+    case KernelId::walk24_s2: return YFV2_KERNEL_REF(walk::blk_kernel<24,2>);
+    case KernelId::walk48_s2: return YFV2_KERNEL_REF(walk::blk_kernel<48,2>);
+    }
+    return KernelRef{nullptr, "?"};
+}
+
+int launch(const Launch& L, const void* args, cudaStream_t s) {
+    const KernelRef k = kernel_ref(L.kernel);
+    YFV2_CUDA(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
+    dim3 grid = L.grid;
+    if (L.persistent) {
+        int per_sm = 0;
+        YFV2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.fn, kThreads, L.smem));
+        const long long cap = (long long)(per_sm > 0 ? per_sm : 1) * L.grid.x;
+        grid.x = (unsigned)(L.items < cap ? L.items : cap);
+    }
+    YFV2_CUDA(launch_k(k.fn, grid, kThreads, L.smem, s, pdl_take(), args));
+    YFV2_LAUNCH_CHECK();
+    return YFV2_OK;
+}
+
+// A stride-1 block keeps its weights resident in a persistent grid (K=96 at 352x352: 182 -> 120 us on an H100); K = 24 and 48 run
+// on walk::blk_kernel wherever it fits.  A chain owns whole images: on blk_kernel one CTA per image, past kChainBudget (K = 96,
+// chainable) on blk_chain_kernel, one CTA per SM.
+int describe_blk_s1(int K, const Planes& P, int nblk, int N, int sms, Launch& L) {
     if (nblk < 1 || nblk > kMaxChain || (nblk > 1 && !blk_s1_chainable(K, P.H, P.W))) {
         set_error("block: a chain of %d stride-1 blocks needs a whole %dx%d image per CTA", nblk, P.H, P.W);
         return YFV2_EINVAL;
     }
+    if (K != 24 && K != 48 && K != 96) { set_error("block: unsupported width %d", K); return YFV2_EUNSUPPORTED; }
+    if (nblk > 1) {
+        set_bands(L, P.H, P.H, N);
+        L.smem = blk_smem_bytes(K, 1, P.H, P.W);
+        if (L.smem > kChainBudget) { L.kernel = KernelId::chain96; set_persistent(L, sms); }
+        else { L.kernel = kBlkKernel[0][width_index(K)]; L.grid = dim3((unsigned)L.items); }
+        return YFV2_OK;
+    }
+    set_bands(L, blk_rows(K, 1, P.H, P.W, N, sms), P.H, N);
+    set_persistent(L, sms);
+    if ((L.G = blk_s1_walk_step(K, P)) > 0) {
+        L.kernel = kWalkKernel[0][width_index(K)];
+        L.smem = walk::s1_smem_bytes(K, L.G, P.W, P.Ws);
+        return YFV2_OK;
+    }
+    L.kernel = kBlkKernel[0][width_index(K)];
+    L.smem = blk_smem_bytes(K, 1, L.R, P.W);
+    if (L.smem > kSmemCap) { set_error("block: a %d-row band of %d columns does not fit in shared memory", L.R, P.W); return YFV2_EUNSUPPORTED; }
+    return YFV2_OK;
+}
+
+// The stride-2 blocks were measured slower in a persistent grid (stage4.0 610 -> 760 us, stage2.0 463 -> 488 us) and take one CTA
+// per band; K = 24 and 48 run on walk::blk_kernel wherever it fits.  Small stage4.0 maps run on whole images, one CTA per SM.
+int describe_blk_s2(int K, const Planes& in, const Planes& out, int N, int sms, Launch& L) {
+    if (K != 24 && K != 48 && K != 96) { set_error("block: unsupported width %d", K); return YFV2_EUNSUPPORTED; }
+    if (blk_s2_whole_image(K, out.H, out.W, in.W)) {      // K = 96
+        L.kernel = KernelId::s2_image96;
+        L.smem = blk_s2_image_smem_bytes(K, out.H, in.W);
+        set_bands(L, out.H, out.H, N);
+        set_persistent(L, sms);
+        return YFV2_OK;
+    }
+    set_bands(L, blk_rows(K, 2, out.H, in.W, N, sms), out.H, N);
+    L.grid = dim3((unsigned)L.items);
+    if (blk_s2_walk_fits(K, in)) {
+        L.kernel = kWalkKernel[1][width_index(K)];
+        L.smem = walk::smem_bytes(K, in.W, in.Ws);
+        return YFV2_OK;
+    }
+    L.kernel = kBlkKernel[1][width_index(K)];
+    L.smem = blk_smem_bytes(K, 2, L.R, in.W);
+    if (L.smem > kSmemCap) { set_error("block: a %d-row band of %d columns does not fit in shared memory", L.R, in.W); return YFV2_EUNSUPPORTED; }
+    return YFV2_OK;
+}
+
+int blk_launch_s1(const Launch& L, int K, const Planes& P, const ChanTab* tin, const ChanTab* tout, const float* const* w1,
+                  const float* const* wdw, const float* const* w2, cudaStream_t s) {
     BlkArgs a{};
     a.in = P; a.out = P;
     a.Hi = a.Ho = P.H; a.Wi = a.Wo = P.W;
-    a.nblk = nblk;
-    a.R = nblk > 1 ? P.H : blk_rows(K, 1, P.H, P.W, N);
-    for (int j = 0; j < nblk; ++j) {
+    a.nblk = L.last - L.first;
+    a.R = L.R; a.bands = L.bands; a.items = L.items; a.G = L.G;
+    for (int j = 0; j < a.nblk; ++j) {
         a.pw1[j] = w1[j]; a.dw[j] = wdw[j]; a.pw2[j] = w2[j];
         for (int i = 0; i < K; ++i) { a.tin[j][i] = tin[j].c[i]; a.tout[j][i] = tout[j].c[i]; }
     }
-    const size_t bytes = blk_smem_bytes(K, 1, P.H, P.W);
-    if (nblk > 1 && bytes > kChainBudget) return run_whole_image(blk_chain_kernel<96>, bytes, a, N, s);   // K = 96 (chainable)
-    if (nblk == 1 && (a.G = blk_s1_walk_step(K, P)) > 0) return K == 24 ? run_blk_walk<24, 1>(a, N, s) : run_blk_walk<48, 1>(a, N, s);
-    switch (K) {
-    case 24: return dispatch_blk<24>(1, a, N, s);
-    case 48: return dispatch_blk<48>(1, a, N, s);
-    case 96: return dispatch_blk<96>(1, a, N, s);
-    }
-    set_error("block: unsupported width %d", K);
-    return YFV2_EUNSUPPORTED;
+    return launch(L, &a, s);
 }
 
-int blk_launch_s2(int K, const Planes& in, const Planes& out, const ChanTab& tin, const ChanTab& tout, const float* wdwp, const float* wp,
-                  const float* w1, const float* wdwm, const float* w2, int N, cudaStream_t s) {
+int blk_launch_s2(const Launch& L, int K, const Planes& in, const Planes& out, const ChanTab& tin, const ChanTab& tout,
+                  const float* wdwp, const float* wp, const float* w1, const float* wdwm, const float* w2, cudaStream_t s) {
     BlkArgs a{};
     a.in = in; a.out = out;
     a.Hi = in.H; a.Wi = in.W; a.Ho = out.H; a.Wo = out.W;
     a.nblk = 1;
+    a.R = L.R; a.bands = L.bands; a.items = L.items;
     a.pw1[0] = w1; a.dw[0] = wdwm; a.pw2[0] = w2; a.dwp = wdwp; a.pwp = wp;
     for (int i = 0; i < K; ++i) { a.tin[0][i] = tin.c[i]; a.tout[0][i] = tout.c[i]; a.tmain[i] = tout.c[K + i]; }
-    if (blk_s2_whole_image(K, out.H, out.W, in.W))      // K = 96
-        return run_whole_image(blk_s2_image_kernel<96>, blk_s2_image_smem_bytes(K, out.H, in.W), a, N, s);
-    a.R = blk_rows(K, 2, out.H, in.W, N);
-    if (blk_s2_walk_fits(K, in)) return K == 24 ? run_blk_walk<24, 2>(a, N, s) : run_blk_walk<48, 2>(a, N, s);
-    switch (K) {
-    case 24: return dispatch_blk<24>(2, a, N, s);
-    case 48: return dispatch_blk<48>(2, a, N, s);
-    case 96: return dispatch_blk<96>(2, a, N, s);
-    }
-    set_error("block: unsupported width %d", K);
-    return YFV2_EUNSUPPORTED;
+    return launch(L, &a, s);
 }
 
-// which = 1: S3 from C3; which = 2: S2 from cat(up2(C3), C2)
-int fpn_launch(int which, const Planes& c3, const ChanTab& t3, const Planes& c2, const ChanTab& t2, const Planes& out, const float* pw,
-               int N, cudaStream_t s) {
+// which = 1: S3 from C3; which = 2: S2 from cat(up2(C3), C2); an H x W output map, chunks of 16 kWarps pixels per image
+int describe_fpn(int which, int H, int W, int N, int sms, Launch& L) {
+    L.kernel = which == 1 ? KernelId::fpn192 : KernelId::fpn288;
+    L.smem = (size_t)pw_smem_floats(which == 1 ? 192 : 288, 72) * sizeof(float);
+    L.items = N * ((H * W + 16 * kWarps - 1) / (16 * kWarps));
+    L.grid = dim3((unsigned)(L.items < 2 * sms ? L.items : 2 * sms));
+    return YFV2_OK;
+}
+
+int fpn_launch(const Launch& L, const Planes& c3, const ChanTab& t3, const Planes& c2, const ChanTab& t2, const Planes& out,
+               const float* pw, int N, cudaStream_t s) {
     FpnArgs a{};
     a.c3 = c3; a.c2 = c2; a.out = out; a.pw = pw;
     for (int i = 0; i < 192; ++i) a.t3[i] = t3.c[i];
     for (int i = 0; i < 96; ++i) a.t2[i] = t2.c[i];
     a.N = N; a.H = out.H; a.W = out.W;
-    a.chunks = (out.H * out.W + 16 * kWarps - 1) / (16 * kWarps);
-    auto run = [&](auto kern, int kin) -> int {
-        const size_t bytes = (size_t)pw_smem_floats(kin, 72) * sizeof(float);
-        if (int rc = smem_attr(kern, bytes)) return rc;
-        YFV2_CUDA(launch_k(kern, persistent_grid((long long)N * a.chunks, 2), kThreads, bytes, s, pdl_take(), a));
-        YFV2_LAUNCH_CHECK();
-        return YFV2_OK;
-    };
-    return which == 1 ? run(fpn_kernel<192>, 192) : run(fpn_kernel<288>, 288);
+    a.chunks = L.items / N;
+    return launch(L, &a, s);
 }
 
+namespace {
 // weight columns of the kernel that runs head half `half`: 72 (head_kernel<0>), 96 (head_kernel<1>), 192 (head2_kernel); 0: none
 int head_columns(int half, int A, int C) {
     if (half == 0) return 72;
@@ -1349,21 +1372,34 @@ int head_columns(int half, int A, int C) {
 }
 
 // The channel stride of a window slot where the staged window fits, else 0 (the stencils read the planes).  It fits when the planes
-// of both branches allow 16-byte copies of whole rows and kHeadSlots slots fit next to the weights within kHeadBudget.  Tall maps
-// of one or two columns (a chunk spans up to 16 kWarps rows) and very wide maps (one slot of 6 rows exceeds the budget) do not.
-int heads_window_stride(int half, const Planes& sIn, const Planes& tcls, const Planes& treg, int A, int C) {
-    const int np = head_columns(half, A, C);
+// of both branches allow 16-byte copies of whole rows and kHeadSlots slots fit next to the np weight columns within kHeadBudget.
+// Tall maps of one or two columns (a chunk spans up to 16 kWarps rows) and very wide maps (one slot of 6 rows exceeds the budget)
+// do not.
+int heads_window_stride(int half, int np, const Planes& sIn, const Planes& tcls, const Planes& treg) {
     const Planes* in[2] = {half ? &tcls : &sIn, half ? &treg : &sIn};
     for (const Planes* q : in)
         if (q->pad != 2 || ((uintptr_t)q->base & 15) || q->Ws % 4 || q->sC % 4 || q->sN % 4 || q->Ws != in[0]->Ws) return 0;
     const int cs = walk::ring_stride(head_win_rows(in[0]->H, in[0]->W) * in[0]->Ws);
-    return np && head_weight_bytes(np) + (size_t)kHeadSlots * 8 * cs * sizeof(float) <= kHeadBudget ? cs : 0;
+    return head_weight_bytes(np) + (size_t)kHeadSlots * 8 * cs * sizeof(float) <= kHeadBudget ? cs : 0;
+}
+}  // namespace
+
+// One CTA per SM and branch (grid.y: cls, reg), each walking (image, chunk of 16 kWarps pixels) items
+int describe_heads(int half, const Planes& sIn, const Planes& tcls, const Planes& treg, int A, int C, int N, int sms, Launch& L) {
+    const int np = head_columns(half, A, C);
+    if (!np) { set_error("heads: anchors+classes = %d exceeds two %d-column output tiles", A + C, kHeadTile); return YFV2_EUNSUPPORTED; }
+    L.kernel = np == 72 ? KernelId::head0 : np == kHeadTile ? KernelId::head1 : KernelId::head2;
+    L.CS = heads_window_stride(half, np, sIn, tcls, treg);
+    L.smem = head_weight_bytes(np) + (size_t)kHeadSlots * 8 * L.CS * sizeof(float);
+    L.items = N * ((sIn.H * sIn.W + 16 * kWarps - 1) / (16 * kWarps));
+    L.grid = dim3((unsigned)(L.items < sms ? L.items : sms), 2);
+    return YFV2_OK;
 }
 
-int heads_launch(int half, const Planes& sIn, const Planes& tcls, const Planes& treg, const float* const wdw[2], const float* const wpw[2],
-                 float* reg, float* obj, float* cls, int A, int C, int N, cudaStream_t s) {
+int heads_launch(const Launch& L, int half, const Planes& sIn, const Planes& tcls, const Planes& treg, const float* const wdw[2],
+                 const float* const wpw[2], float* reg, float* obj, float* cls, int A, int C, int N, cudaStream_t s) {
     HeadArgs a{};
-    a.CS = heads_window_stride(half, sIn, tcls, treg, A, C);
+    a.CS = L.CS;
     for (int b = 0; b < 2; ++b) { a.dw[b] = wdw[b]; a.pw[b] = wpw[b]; }
     a.out[0] = tcls; a.out[1] = treg;
     if (half == 0) { a.in[0] = sIn; a.in[1] = sIn; }
@@ -1371,28 +1407,8 @@ int heads_launch(int half, const Planes& sIn, const Planes& tcls, const Planes& 
     a.dst[0][0] = obj; a.dst[0][1] = cls; a.split[0] = A; a.rowsA[0] = A; a.rowsB[0] = C;
     a.dst[1][0] = reg; a.dst[1][1] = reg; a.split[1] = 4 * A; a.rowsA[1] = 4 * A; a.rowsB[1] = 0;
     a.N = N; a.H = sIn.H; a.W = sIn.W;
-    a.chunks = (sIn.H * sIn.W + 16 * kWarps - 1) / (16 * kWarps);
-    auto run = [&](auto kern, int np) -> int {
-        const size_t bytes = head_weight_bytes(np) + (size_t)kHeadSlots * 8 * a.CS * sizeof(float);
-        if (int rc = smem_attr(kern, bytes)) return rc;
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3((unsigned)persistent_grid((long long)N * a.chunks, 1), 2);
-        cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = bytes; cfg.stream = s;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = at; cfg.numAttrs = pdl_take() ? 1 : 0;
-        YFV2_CUDA(cudaLaunchKernelEx(&cfg, kern, a));
-        YFV2_LAUNCH_CHECK();
-        return YFV2_OK;
-    };
-    switch (head_columns(half, A, C)) {
-    case 72: return run(head_kernel<0>, 72);
-    case kHeadTile: return run(head_kernel<1>, kHeadTile);
-    case 2 * kHeadTile: return run(head2_kernel, 2 * kHeadTile);
-    }
-    set_error("heads: anchors+classes = %d exceeds two %d-column output tiles", A + C, kHeadTile);
-    return YFV2_EUNSUPPORTED;
+    a.chunks = L.items / N;
+    return launch(L, &a, s);
 }
 static_assert(head_weight_bytes(2 * kHeadTile) <= kSmemCap, "two head tiles must fit in shared memory");
 

@@ -276,9 +276,19 @@ __host__ bool stem_bytes_fit(int TRo, int TWo, int S) {
 }  // namespace
 
 int launch_stem(const StemArgs& a, cudaStream_t s) {
-    if (a.H % 4 || a.W % 4 || a.H < 4 || a.W < 4) { set_error("stem: input %dx%d must be a multiple of 4", a.H, a.W); return YFV2_EINVAL; }
-    StemFArgs k{a.x, a.out, a.wpack, a.N, a.H, a.W, 0, 0, 0, 0, 0, 0};
-    const int HO = a.H / 4, WO = a.W / 4;
+    const auto& t = a.launch.stem;
+    const StemFArgs k{a.x, a.out, a.wpack, a.N, a.H, a.W, t.TRo, t.TWo, t.tilesX, t.tilesY, t.S, ((uintptr_t)a.x & 15) == 0 && t.vec};
+    return launch(a.launch, &k, s);
+}
+
+static_assert(ST_THREADS == kThreads, "launch() runs every forward kernel with kThreads threads");
+
+KernelRef stem_kernel_ref(bool u8) { return u8 ? YFV2_KERNEL_REF(stem_kernel<true>) : YFV2_KERNEL_REF(stem_kernel<false>); }
+
+int describe_stem(int N, int H, int W, int is_u8, int sms, Launch& L) {
+    if (H % 4 || W % 4 || H < 4 || W < 4) { set_error("stem: input %dx%d must be a multiple of 4", H, W); return YFV2_EINVAL; }
+    auto& k = L.stem;
+    const int HO = H / 4, WO = W / 4;
     // tiles of at most 44 pooled columns, as equal as possible; S strips of 4 conv columns cover the 2 TWo + 1 conv columns
     k.tilesX = (WO + 43) / 44;
     k.TWo = (WO + k.tilesX - 1) / k.tilesX;
@@ -289,20 +299,14 @@ int launch_stem(const StemArgs& a, cudaStream_t s) {
     while (k.TRo > 1 && stem_smem_bytes(k.TRo, k.TWo, k.S) > 112 * 1024) --k.TRo;
     if (k.TRo < 1) k.TRo = 1;
     const size_t bytes = stem_smem_bytes(k.TRo, k.TWo, k.S);
-    if ((2 * k.TRo + 1) * k.S > ST_THREADS || k.TRo * k.TWo > ST_THREADS || bytes > kSmemCap - 1024) { set_error("stem: unsupported geometry %dx%d", a.H, a.W); return YFV2_EUNSUPPORTED; }
+    if ((2 * k.TRo + 1) * k.S > ST_THREADS || k.TRo * k.TWo > ST_THREADS || bytes > kSmemCap - 1024) { set_error("stem: unsupported geometry %dx%d", H, W); return YFV2_EUNSUPPORTED; }
     // asynchronous staging needs 16-byte aligned rows (uint8: and room for the bytes); other inputs take the scalar loads
-    k.vec = ((uintptr_t)a.x & 15) == 0 && (!a.is_u8 || (a.W % 16 == 0 && stem_bytes_fit(k.TRo, k.TWo, k.S)));
+    k.vec = !is_u8 || (W % 16 == 0 && stem_bytes_fit(k.TRo, k.TWo, k.S));
     k.tilesY = (HO + k.TRo - 1) / k.TRo;
-    const int items = a.N * k.tilesX * k.tilesY;
-    const int grid = items < 2 * sm_count() ? items : 2 * sm_count();
-    if (a.is_u8) {
-        YFV2_CUDA(cudaFuncSetAttribute(stem_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-        YFV2_CUDA(launch_k(stem_kernel<true>, grid, ST_THREADS, bytes, s, pdl_take(), k));
-    } else {
-        YFV2_CUDA(cudaFuncSetAttribute(stem_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-        YFV2_CUDA(launch_k(stem_kernel<false>, grid, ST_THREADS, bytes, s, pdl_take(), k));
-    }
-    YFV2_LAUNCH_CHECK();
+    L.kernel = is_u8 ? KernelId::stem_u8 : KernelId::stem_f32;
+    L.smem = bytes;
+    L.items = N * k.tilesX * k.tilesY;
+    L.grid = dim3((unsigned)(L.items < 2 * sms ? L.items : 2 * sms));
     return YFV2_OK;
 }
 

@@ -18,6 +18,9 @@ namespace yfv2 {
 
 bool blk_s1_chainable(int K, int H, int W);      // k_net.cu
 
+enum class StageKind { stem, block_s1, block_s2, fpn, heads };
+constexpr int kMaxStages = 64;
+
 static thread_local char g_err[512] = "";
 
 void set_error(const char* fmt, ...) {
@@ -173,7 +176,8 @@ struct yfv2_plan {
     size_t pk_foldw[4];                // heads' second pointwise + BN + output conv folded into one matrix [NPt][72] | bias[NPt]
     int fold_rows[4];                  // NPt: 96 or 192 output columns (one or two tiles of the head kernel)
     int n_stages;
-    struct Stage { int kind, a, b; char name[24]; int group; } stages[64];   // group: first stage of the launch this stage shares
+    // group: the first stage of the launch this stage shares
+    struct Stage { StageKind kind; int a, b; char name[24]; int group; } stages[kMaxStages];
 };
 
 namespace {
@@ -296,25 +300,28 @@ extern "C" int yfv2_plan_create(yfv2_plan** out, int device, int N, int H, int W
     }
     p->pk_floats = pk;
 
-    auto add = [&](int kind, int a, int b, const char* fmt, int x, int y) {
+    auto add = [&](StageKind kind, int a, int b, const char* fmt, int x, int y) {
         yfv2_plan::Stage& st = p->stages[p->n_stages++];
         st.kind = kind; st.a = a; st.b = b;
         snprintf(st.name, sizeof(st.name), fmt, x, y);
     };
-    add(0, 0, 0, "stem", 0, 0);
+    add(StageKind::stem, 0, 0, "stem", 0, 0);
     for (int b = 0, st = 0, rep = 0; b < kNumBlocks; ++b) {
-        add(p->blk_stride[b] == 2 ? 11 : 10, b, 0, "stage%d.%d", st + 2, rep);
+        add(p->blk_stride[b] == 2 ? StageKind::block_s2 : StageKind::block_s1, b, 0, "stage%d.%d", st + 2, rep);
         if (++rep == kStageRepeats[st]) { rep = 0; ++st; }
     }
-    add(14, 1, 0, "fpn.S3", 0, 0); add(14, 2, 0, "fpn.S2", 0, 0);
-    for (int lv = 0; lv < 2; ++lv) { add(15, lv, 0, "heads%d.a", lv + 2, 0); add(15, lv, 1, "heads%d.b", lv + 2, 0); }
+    add(StageKind::fpn, 1, 0, "fpn.S3", 0, 0); add(StageKind::fpn, 2, 0, "fpn.S2", 0, 0);
+    for (int lv = 0; lv < 2; ++lv) {
+        add(StageKind::heads, lv, 0, "heads%d.a", lv + 2, 0);
+        add(StageKind::heads, lv, 1, "heads%d.b", lv + 2, 0);
+    }
     // launch groups: consecutive stride-1 blocks of a stage run as one chained launch when an image fits (k_net.cu)
     p->launches = 0;
     for (int i = 0; i < p->n_stages; ++i) {
         yfv2_plan::Stage& st = p->stages[i];
         st.group = i;
-        if (i > 0 && st.kind == 10 && p->stages[i - 1].kind == 10 && p->blk_K[st.a] == p->blk_K[p->stages[i - 1].a] &&
-            i - p->stages[i - 1].group < 7 && blk_s1_chainable(p->blk_K[st.a], p->h[p->blk_res[st.a]], p->w[p->blk_res[st.a]]))
+        if (i > 0 && st.kind == StageKind::block_s1 && p->stages[i - 1].kind == StageKind::block_s1 &&
+            p->blk_K[st.a] == p->blk_K[p->stages[i - 1].a] && i - p->stages[i - 1].group < 7 && blk_s1_chainable(p->blk_K[st.a], p->h[p->blk_res[st.a]], p->w[p->blk_res[st.a]]))
             st.group = p->stages[i - 1].group;
         if (st.group == i) ++p->launches;
     }
@@ -462,21 +469,51 @@ extern "C" int yfv2_pack_weights(yfv2_plan* p, const float* const* params, const
     return YFV2_OK;
 }
 
-namespace yfv2 {
-// k_net.cu
-int blk_launch_s1(int K, const Planes& P, int nblk, const ChanTab* tin, const ChanTab* tout, const float* const* w1,
-                  const float* const* wdw, const float* const* w2, int N, cudaStream_t s);
-int blk_launch_s2(int K, const Planes& in, const Planes& out, const ChanTab& tin, const ChanTab& tout, const float* wdwp, const float* wp,
-                  const float* w1, const float* wdwm, const float* w2, int N, cudaStream_t s);
-int fpn_launch(int which, const Planes& c3, const ChanTab& t3, const Planes& c2, const ChanTab& t2, const Planes& out, const float* pw,
-               int N, cudaStream_t s);
-int heads_launch(int half, const Planes& sIn, const Planes& tcls, const Planes& treg, const float* const wdw[2], const float* const wpw[2],
-                 float* reg, float* obj, float* cls, int A, int C, int N, cudaStream_t s);
-int heads_window_stride(int half, const Planes& sIn, const Planes& tcls, const Planes& treg, int A, int C);
+namespace {
+// the input of head level lv (S2 or S3) and its mid-head scratch of the cls and reg branches
+void head_planes(const yfv2_plan* p, float* ws, int lv, Planes& sIn, Planes& t_cls, Planes& t_reg) {
+    sIn = flat_planes(p, ws, lv ? p->off_s3 : p->off_s2, 2 + lv);
+    t_cls = flat_planes(p, ws, p->off_t[2 * lv], 2 + lv);
+    t_reg = flat_planes(p, ws, p->off_t[2 * lv + 1], 2 + lv);
 }
 
-namespace {
-// Runs fused stages [first, last) of the forward; each stage is exactly one kernel launch.
+// The launches of fused stages [first, last) of a forward on workspace ws over sms SMs, in order: each stage is one launch, except
+// that consecutive stride-1 blocks of one launch group inside the range run as one chained launch.  ws decides the kernels that
+// need 16-byte-aligned planes (the band walks, the heads' staged windows); it is not dereferenced.  Host only.
+int plan_launches(const yfv2_plan* p, float* ws, int is_u8, int sms, int first, int last, Launch* out, int* n) {
+    *n = 0;
+    for (int si = first; si < last; ++si) {
+        const yfv2_plan::Stage& st = p->stages[si];
+        Launch& L = out[(*n)++] = Launch{};
+        L.first = si;
+        const int b = st.a;
+        switch (st.kind) {
+        case StageKind::stem: TRY(describe_stem(p->N, p->H, p->W, is_u8, sms, L)); break;
+        case StageKind::block_s1: {
+            int nb = 1;
+            while (si + nb < last && p->stages[si + nb].group == st.group) ++nb;
+            TRY(describe_blk_s1(p->blk_K[b], pool_planes(p, ws, p->blk_res[b]), nb, p->N, sms, L));
+            si += nb - 1;
+        } break;
+        case StageKind::block_s2:
+            TRY(describe_blk_s2(p->blk_K[b], pool_planes(p, ws, p->blk_res[b] - 1), pool_planes(p, ws, p->blk_res[b]), p->N, sms, L));
+            break;
+        case StageKind::fpn: {
+            const int r = st.a == 1 ? 3 : 2;
+            TRY(describe_fpn(st.a, p->h[r], p->w[r], p->N, sms, L));
+        } break;
+        case StageKind::heads: {
+            Planes sIn, t_cls, t_reg;
+            head_planes(p, ws, st.a, sIn, t_cls, t_reg);
+            TRY(describe_heads(st.b, sIn, t_cls, t_reg, p->A, p->C, p->N, sms, L));
+        } break;
+        }
+        L.last = si + 1;
+    }
+    return YFV2_OK;
+}
+
+// Runs fused stages [first, last) of the forward: the launches plan_launches describes, each with its arguments.
 int forward_impl(yfv2_plan* p, const void* x, int is_u8, const void* packed, float* const preds[6], void* workspace,
                  int first, int last, cudaStream_t s) {
     if (!p || !x || !packed || !preds || !workspace) { set_error("forward: null argument"); return YFV2_EINVAL; }
@@ -485,64 +522,59 @@ int forward_impl(yfv2_plan* p, const void* x, int is_u8, const void* packed, flo
     if (first < 0 || last > p->n_stages || first > last) { set_error("forward: bad stage range [%d,%d)", first, last); return YFV2_EINVAL; }
     float* ws = (float*)workspace;
     const float* pk = (const float*)packed;
+    Launch launches[kMaxStages];
+    int n = 0;
+    TRY(plan_launches(p, ws, is_u8, sm_count(), first, last, launches, &n));
     pdl_reset();                                            // the first kernel of this call is serialized normally
     if (p->ws_zeroed != workspace) {
         // the zero frames around every plane are never written afterwards (kernels store interior pixels only)
         YFV2_CUDA(cudaMemsetAsync(workspace, 0, p->ws_floats * sizeof(float), s));
         p->ws_zeroed = workspace;
     }
-    struct { Planes c3, c2, s3, s2; ChanTab t3, t2; } f;
-    f.c3 = pool_planes(p, ws, 3); f.t3 = p->c3;
-    f.c2 = pool_planes(p, ws, 2); f.t2 = p->c2;
-    f.s3 = flat_planes(p, ws, p->off_s3, 3);
-    f.s2 = flat_planes(p, ws, p->off_s2, 2);
-    for (int si = first; si < last; ++si) {
-        const yfv2_plan::Stage& st = p->stages[si];
+    for (int i = 0; i < n; ++i) {
+        const Launch& L = launches[i];
+        const yfv2_plan::Stage& st = p->stages[L.first];
         const int b = st.a;
         switch (st.kind) {
-        case 0: {
-            StemArgs a{x, is_u8, p->N, p->H, p->W, pool_planes(p, ws, 0), pk + p->pk_stem};
+        case StageKind::stem: {
+            StemArgs a{L, x, is_u8, p->N, p->H, p->W, pool_planes(p, ws, 0), pk + p->pk_stem};
             TRY(launch_stem(a, s));
         } break;
-        case 15: {
+        case StageKind::heads: {
             const int lv = st.a, half = st.b;
-            const Planes sIn = lv ? f.s3 : f.s2;
-            const Planes t_cls = flat_planes(p, ws, p->off_t[2 * lv], 2 + lv);
-            const Planes t_reg = flat_planes(p, ws, p->off_t[2 * lv + 1], 2 + lv);
+            Planes sIn, t_cls, t_reg;
+            head_planes(p, ws, lv, sIn, t_cls, t_reg);
             const float* w_cls = pk + p->pk_head[2 * lv];
             const float* w_reg = pk + p->pk_head[2 * lv + 1];
             // each half of a head pack is DW5 | PW
             const size_t dwn = dw5_pack_floats(kFpnDepth), half_off = (size_t)half * (dwn + pw_pack_floats(kFpnDepth, kFpnDepth));
             const float* wdw[2] = {w_cls + half_off, w_reg + half_off};
             const float* wpw[2] = {half ? pk + p->pk_foldw[2 * lv] : w_cls + dwn, half ? pk + p->pk_foldw[2 * lv + 1] : w_reg + dwn};
-            TRY(heads_launch(half, sIn, t_cls, t_reg, wdw, wpw, preds[3 * lv], preds[3 * lv + 1], preds[3 * lv + 2], p->A, p->C, p->N, s));
+            TRY(heads_launch(L, half, sIn, t_cls, t_reg, wdw, wpw, preds[3 * lv], preds[3 * lv + 1], preds[3 * lv + 2], p->A, p->C,
+                             p->N, s));
         } break;
-        case 10: {   // fused stride-1 blocks; consecutive blocks of a stage inside [first, last) share one launch when
-                     // an image fits in one CTA's shared memory (k_net.cu)
+        case StageKind::block_s1: {   // fused stride-1 blocks [L.first, L.last)
             const int K = p->blk_K[b];
-            int nb = 1;
-            while (si + nb < last && p->stages[si + nb].group == st.group) ++nb;
             const float *w1[7], *w2[7], *wd[7];
-            for (int j = 0; j < nb; ++j) {
+            for (int j = 0; j < L.last - L.first; ++j) {
                 const float* d = pk + p->pk_block[b + j];
                 const int pwn = pw_pack_floats(K, K);
                 w1[j] = d; wd[j] = d + pwn; w2[j] = d + pwn + dw3_pack_floats(K);
             }
-            TRY(blk_launch_s1(K, pool_planes(p, ws, p->blk_res[b]), nb, &p->tin[b], &p->tout[b], w1, wd, w2, p->N, s));
-            si += nb - 1;
+            TRY(blk_launch_s1(L, K, pool_planes(p, ws, p->blk_res[b]), &p->tin[b], &p->tout[b], w1, wd, w2, s));
         } break;
-        case 11: {   // fused stride-2 block; pack order DWp | PWp | PW1 | DW | PW2
+        case StageKind::block_s2: {   // fused stride-2 block; pack order DWp | PWp | PW1 | DW | PW2
             const int K = p->blk_K[b];
             const float* d = pk + p->pk_block[b];
             const int dwn = dw3_pack_floats(K), pwn = pw_pack_floats(K, K);
-            TRY(blk_launch_s2(K, pool_planes(p, ws, p->blk_res[b] - 1), pool_planes(p, ws, p->blk_res[b]), p->tin[b], p->tout[b],
-                              d, d + dwn, d + dwn + pwn, d + dwn + 2 * pwn, d + 2 * dwn + 2 * pwn, p->N, s));
+            TRY(blk_launch_s2(L, K, pool_planes(p, ws, p->blk_res[b] - 1), pool_planes(p, ws, p->blk_res[b]), p->tin[b], p->tout[b],
+                              d, d + dwn, d + dwn + pwn, d + dwn + 2 * pwn, d + 2 * dwn + 2 * pwn, s));
         } break;
-        case 14: {   // FPN reducers
-            if (st.a == 1) { TRY(fpn_launch(1, f.c3, f.t3, f.c2, f.t2, f.s3, pk + p->pk_fpn3, p->N, s)); }
-            else { TRY(fpn_launch(2, f.c3, f.t3, f.c2, f.t2, f.s2, pk + p->pk_fpn2, p->N, s)); }
+        case StageKind::fpn: {        // FPN reducers: S3 from C3, S2 from cat(up2(C3), C2)
+            const Planes c3 = pool_planes(p, ws, 3), c2 = pool_planes(p, ws, 2);
+            const Planes out = st.a == 1 ? flat_planes(p, ws, p->off_s3, 3) : flat_planes(p, ws, p->off_s2, 2);
+            TRY(fpn_launch(L, c3, p->c3, c2, p->c2, out, pk + (st.a == 1 ? p->pk_fpn3 : p->pk_fpn2), p->N, s));
         } break;
-        default: set_error("forward: unknown stage kind %d", st.kind); return YFV2_EINVAL;
         }
     }
     return YFV2_OK;
@@ -635,13 +667,23 @@ extern "C" int yfv2_debug_gather(const yfv2_plan* p, const void* workspace, int 
     return YFV2_OK;
 }
 
-// ---- debug: does head launch `which` (heads2.a, heads2.b, heads3.a, heads3.b) stage its input windows? --------------------
-extern "C" int yfv2_debug_heads_staged(const yfv2_plan* p, const void* workspace, int which) {
-    if (!p || !workspace || which < 0 || which > 3) { set_error("debug_heads_staged: bad argument"); return YFV2_EINVAL; }
-    float* ws = (float*)workspace;
-    const int lv = which / 2, half = which % 2;
-    const Planes sIn = flat_planes(p, ws, lv ? p->off_s3 : p->off_s2, 2 + lv);
-    const Planes t_cls = flat_planes(p, ws, p->off_t[2 * lv], 2 + lv);
-    const Planes t_reg = flat_planes(p, ws, p->off_t[2 * lv + 1], 2 + lv);
-    return heads_window_stride(half, sIn, t_cls, t_reg, p->A, p->C) > 0 ? 1 : 0;
+// ---- test hook: the launch records of a whole forward ---------------------------------------------------------------------
+extern "C" int yfv2_plan_debug_launches(const yfv2_plan* p, const void* workspace, int is_u8, int sms, yfv2_launch* out, int cap,
+                                        int* n) {
+    if (!p || !n || sms < 0 || cap < 0 || (cap > 0 && !out)) { set_error("plan_debug_launches: bad argument"); return YFV2_EINVAL; }
+    // NULL: any 16-byte-aligned workspace (its address is only tested for alignment)
+    float* ws = workspace ? (float*)workspace : reinterpret_cast<float*>((uintptr_t)256);
+    Launch launches[kMaxStages];
+    TRY(plan_launches(p, ws, is_u8, sms ? sms : sm_count(), 0, p->n_stages, launches, n));
+    for (int i = 0; i < cap && i < *n; ++i) {
+        const Launch& L = launches[i];
+        yfv2_launch& d = out[i];
+        snprintf(d.kernel, sizeof(d.kernel), "%s", kernel_ref(L.kernel).name);
+        d.first = L.first; d.last = L.last;
+        d.smem = (long long)L.smem;
+        d.grid[0] = (int)L.grid.x; d.grid[1] = (int)L.grid.y; d.grid[2] = (int)L.grid.z;
+        d.persistent = L.persistent; d.items = L.items;
+        d.R = L.R; d.bands = L.bands; d.G = L.G; d.window_stride = L.CS;
+    }
+    return YFV2_OK;
 }

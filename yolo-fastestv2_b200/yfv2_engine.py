@@ -81,6 +81,28 @@ def trainer_program(handle):
     return ops, [as_dict(t) for t in tens], dict(zip(TRAINER_LAYOUT, lay))
 
 
+class LaunchRecord(ctypes.Structure):
+    """yfv2_launch: one kernel launch of a forward, as the forward chooses it (test hook)."""
+    _fields_ = [("kernel", ctypes.c_char * 32), ("first", ctypes.c_int), ("last", ctypes.c_int), ("smem", ctypes.c_longlong),
+                ("grid", ctypes.c_int * 3)] + [(f, ctypes.c_int) for f in ("persistent", "items", "R", "bands", "G", "window_stride")]
+
+
+def plan_launches(handle, workspace=None, is_u8=False, sms=0):
+    """The kernel launches of a whole forward of a yfv2_plan handle, in order, as dicts (yfv2_plan_debug_launches; host only).
+    workspace None: a 16-byte-aligned workspace; sms 0: this device's SM count."""
+    L, n = lib(), ctypes.c_int()
+    ws = ctypes.c_void_p(workspace)
+    _check(L.yfv2_plan_debug_launches(handle, ws, int(is_u8), sms, None, 0, ctypes.byref(n)), "plan_debug_launches")
+    recs = (LaunchRecord * n.value)()
+    _check(L.yfv2_plan_debug_launches(handle, ws, int(is_u8), sms, recs, n.value, ctypes.byref(n)), "plan_debug_launches")
+    out = []
+    for r in recs:
+        d = {f: getattr(r, f) for f, _ in r._fields_}
+        d["kernel"], d["grid"], d["persistent"] = r.kernel.decode(), tuple(r.grid), bool(r.persistent)
+        out.append(d)
+    return out
+
+
 def check_bn_batch(N, H, W):
     """F.batch_norm in training mode refuses a layer with one value per channel; the deepest BatchNorm layers of the network run
     at stride 32 (stem 3x3 s2, max-pool 3x3 s2 p1 and three stride-2 blocks: each (h - 1) // 2 + 1), the first of them on the
@@ -204,7 +226,8 @@ PROTOTYPES = {
     "yfv2_debug_gather": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
                                          ctypes.POINTER(ctypes.c_int), ctypes.c_void_p]),
     "yfv2_debug_nms_profile": (ctypes.c_int, [ctypes.c_void_p]),
-    "yfv2_debug_heads_staged": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]),
+    "yfv2_plan_debug_launches": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                                ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
     "yfv2_ncnn_post": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                       ctypes.POINTER(ctypes.c_float), ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                       ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
@@ -433,6 +456,10 @@ class Plan:
                                             ctypes.c_void_p(self.packed.data_ptr()), _ptr_array(preds),
                                             ctypes.c_void_p(self.workspace.data_ptr()), first, last, _stream(self.device)),
                    "forward_range")
+
+    def launches(self, is_u8=False, sms=0):
+        """The kernel launches of a forward on this plan's workspace (plan_launches; host only)."""
+        return plan_launches(self._h, self.workspace.data_ptr(), is_u8, sms)
 
     def debug_gather(self, which):
         """Dense NCHW copy of an intermediate tensor of the last forward (test hook, see yfv2.h)."""
