@@ -304,6 +304,48 @@ typedef struct yfv2_yuv422_frame {
 } yfv2_yuv422_frame;
 YFV2_API int yfv2_resize_yuv422_u8(const yfv2_yuv422_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
 
+/* ---- JPEG files -> packed HWC BGR frames: cv2.imread(path) (test.py:34; utils/datasets.py:106) on the device -----------------
+ * The bytes OpenCV 4.13 (libjpeg-turbo 3.1) returns for IMREAD_COLOR: ISLOW IDCT, fancy upsampling, jdcolor's YCbCr -> BGR, grey
+ * replicated to B = G = R, and the EXIF orientation applied.  Supported: baseline sequential Huffman-coded DCT (SOF0, SOF1) with
+ * 8-bit samples, 1 or 3 components, luma sampling 1x1, 2x1, 2x2, 1x2 or 4x1 with 1x1 chroma, restart intervals, one scan.  Anything
+ * else (progressive, arithmetic, lossless, hierarchical, 12/16-bit, 2 or 4 components, Adobe RGB, several scans, other sampling,
+ * not a JPEG) is refused per file by the parse, with a reason.
+ *
+ * yfv2_jpeg_parse (host only, no device needed): the N files lie in one host buffer, file i at files_host[offsets_host[i] ..
+ * offsets_host[i+1]).  Fills info_host[N] (status 0 or a YFV2_E* code with its reason; size after orientation; frame_offset) and
+ * the sizes the decode needs: meta_bytes (the blob), workspace_bytes, frames_bytes (the arena; frame i is [h][w][3] BGR at
+ * frame_offset, rows 3*w apart, usable as a yfv2_frame as it is).  With meta_host NULL only the sizes are computed; otherwise the
+ * blob (decode tables, geometry and the byte range of every entropy-coded segment) is written into meta_host[meta_cap].  Returns
+ * the first refused file's code (yfv2_last_error names it), YFV2_ENOMEM when meta_cap is too small.
+ *
+ * yfv2_jpeg_decode: files (device) is a copy of the same buffer, files_bytes long; meta_dev a device copy of the blob, meta_host the
+ * blob itself (checked, with the buffer sizes, before anything is launched).  Writes every frame into `frames` and a per-image flag
+ * word into errors[N] (device int32; 1: a segment ran out of data, 2: an invalid Huffman code; the image is then decoded as libjpeg
+ * would continue, zero bits past the end).  phases: YFV2_JPEG_ALL, or the subset of the three launches to run in this call (entropy
+ * decode into the workspace, IDCT into planes in the workspace, upsample + colour into frames), for timing them separately.
+ * Nothing is allocated and nothing synchronises. */
+#define YFV2_JPEG_ENTROPY 1
+#define YFV2_JPEG_IDCT    2
+#define YFV2_JPEG_COLOR   4
+#define YFV2_JPEG_ALL     7
+typedef struct yfv2_jpeg_info {
+    int status;            /* 0, or why the file is refused: YFV2_EUNSUPPORTED (out of scope) or YFV2_EINVAL (malformed) */
+    int w, h;              /* the decoded frame's size, EXIF orientation applied */
+    int components;        /* 1 (grey) or 3 (YCbCr) */
+    int h_samp, v_samp;    /* luma sampling factors (1, 1 for grey) */
+    int orientation;       /* EXIF orientation 1..8 (1 without EXIF) */
+    int restart_interval;  /* MCUs per restart interval, 0: none */
+    int segments;          /* entropy-coded segments, each decoded by one thread */
+    int reserved;
+    long long frame_offset;/* byte offset of the frame in the arena */
+    char reason[96];       /* status != 0: what is refused */
+} yfv2_jpeg_info;
+YFV2_API int yfv2_jpeg_parse(const uint8_t* files_host, const long long* offsets_host, int N, yfv2_jpeg_info* info_host,
+                             void* meta_host, size_t meta_cap, size_t* meta_bytes, size_t* workspace_bytes, size_t* frames_bytes);
+YFV2_API int yfv2_jpeg_decode(const void* meta_host, const void* meta_dev, size_t meta_bytes, const uint8_t* files, size_t files_bytes,
+                              uint8_t* frames, size_t frames_bytes, int* errors, void* workspace, size_t workspace_bytes, int phases,
+                              void* stream);
+
 /* ---- whole inference step with HOST buffers (the evaluation() inner loop, utils/utils.py:367-383) ----
  * x_host: pinned uint8 [N,3,H,W]; out_host: pinned [N,max_det,6]; counts_host: pinned [N].
  * Copies in, runs forward_u8 + decode_nms, copies out, all on `stream`; returns without synchronising. */

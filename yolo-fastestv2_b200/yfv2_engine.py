@@ -133,6 +133,16 @@ class AugBlur(ctypes.Structure):
     _fields_ = [("ksize", ctypes.c_int), ("taps", ctypes.c_float * 9)]
 
 
+class JpegInfo(ctypes.Structure):
+    """yfv2_jpeg_info: what yfv2_jpeg_parse found in one file."""
+    _fields_ = [("status", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int), ("components", ctypes.c_int),
+                ("h_samp", ctypes.c_int), ("v_samp", ctypes.c_int), ("orientation", ctypes.c_int), ("restart_interval", ctypes.c_int),
+                ("segments", ctypes.c_int), ("reserved", ctypes.c_int), ("frame_offset", ctypes.c_longlong), ("reason", ctypes.c_char * 96)]
+
+
+JPEG_ENTROPY, JPEG_IDCT, JPEG_COLOR, JPEG_ALL = 1, 2, 4, 7     # yfv2_jpeg_decode phases
+
+
 # name -> (restype, argtypes); must list every prototype of include/yfv2.h (tests check this)
 PROTOTYPES = {
     "yfv2_abi_version": (ctypes.c_int, []),
@@ -228,6 +238,10 @@ PROTOTYPES = {
     "yfv2_debug_nms_profile": (ctypes.c_int, [ctypes.c_void_p]),
     "yfv2_plan_debug_launches": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                 ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
+    "yfv2_jpeg_parse": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
+                                       ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t)]),
+    "yfv2_jpeg_decode": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p,
+                                        ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p]),
     "yfv2_ncnn_post": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                       ctypes.POINTER(ctypes.c_float), ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                       ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
@@ -786,6 +800,111 @@ def resize_bgr(frames, W, H, device=None, out=None):
     with torch.cuda.device(device):
         _check(lib().yfv2_resize_bgr_u8(descs, N, H, W, ctypes.c_void_p(out.data_ptr()), _stream(device)), "resize_bgr_u8")
     return out
+
+
+def _jpeg_name(names, i):
+    return str(names[i]) if names is not None else "file %d" % i
+
+
+def _jpeg_pack(files, pin):
+    """The files in one host uint8 tensor (pinned for an asynchronous copy when pin) and the int64 offsets of each (N + 1)."""
+    import numpy as np
+    arrs = []
+    for i, f in enumerate(files):
+        if isinstance(f, (bytes, bytearray, memoryview)):
+            arrs.append(np.frombuffer(f, np.uint8))
+        elif isinstance(f, np.ndarray) and f.dtype == np.uint8:
+            arrs.append(np.ascontiguousarray(f).reshape(-1))
+        else:
+            raise Yfv2Error("decode_jpeg: file %d must be bytes or a uint8 numpy buffer, got %s" % (i, type(f).__name__))
+    offsets = np.zeros(len(arrs) + 1, np.int64)
+    offsets[1:] = np.cumsum([a.size for a in arrs])
+    host = torch.empty(max(int(offsets[-1]), 1), dtype=torch.uint8, pin_memory=pin)
+    hv = host.numpy()
+    for a, o in zip(arrs, offsets):
+        hv[o:o + a.size] = a
+    return host, offsets
+
+
+def parse_jpeg(files, names=None, blob=False, pin=False):
+    """yfv2_jpeg_parse of files (bytes or uint8 numpy buffers), on the host only: (infos, blob, (workspace_bytes, frames_bytes),
+    host buffer, offsets).  infos: one dict per file (status, w, h, components, h_samp, v_samp, orientation, restart_interval,
+    segments, frame_offset, reason).  Raises Yfv2Error naming every refused file and its reason; blob (a host uint8 tensor, pinned
+    when pin) is None unless asked for."""
+    files = list(files)
+    if not files:
+        raise Yfv2Error("decode_jpeg: no files")
+    host, offsets = _jpeg_pack(files, pin)
+    N = len(files)
+    infos = (JpegInfo * N)()
+    meta, ws, fr = ctypes.c_size_t(), ctypes.c_size_t(), ctypes.c_size_t()
+    L = lib()
+    off = ctypes.c_void_p(offsets.ctypes.data)
+    rc = L.yfv2_jpeg_parse(ctypes.c_void_p(host.data_ptr()), off, N, infos, None, 0, ctypes.byref(meta), ctypes.byref(ws), ctypes.byref(fr))
+    if rc != 0:
+        bad = ["%s: %s" % (_jpeg_name(names, i), infos[i].reason.decode("utf-8", "replace")) for i in range(N) if infos[i].status]
+        if not bad:
+            _check(rc, "jpeg_parse")
+        raise Yfv2Error("decode_jpeg: %d of %d files refused: %s" % (len(bad), N, "; ".join(bad)))
+    out = None
+    if blob:
+        out = torch.empty(meta.value, dtype=torch.uint8, pin_memory=pin)
+        _check(L.yfv2_jpeg_parse(ctypes.c_void_p(host.data_ptr()), off, N, infos, ctypes.c_void_p(out.data_ptr()), out.numel(),
+                                 ctypes.byref(meta), ctypes.byref(ws), ctypes.byref(fr)), "jpeg_parse")
+    keys = [k for k, _ in JpegInfo._fields_ if k != "reserved"]
+    dicts = [{k: (getattr(i, k).decode() if k == "reason" else getattr(i, k)) for k in keys} for i in infos]
+    return dicts, out, (ws.value, fr.value), host, offsets
+
+
+class JpegBatch:
+    """Files parsed on the host and copied to `device` once (one H2D copy of the packed files, one of the blob), with the workspace,
+    the frame arena and the error flags allocated: decode() launches the three phases (or a subset) on the current stream without
+    synchronising, check() waits for the flags and raises on any, frames() are [h, w, 3] uint8 views into the arena."""
+
+    def __init__(self, files, device=None, names=None):
+        device = torch.device(device if device is not None else torch.device("cuda", torch.cuda.current_device()))
+        if device.type != "cuda":
+            raise Yfv2Error("decode_jpeg: runs on CUDA devices only (no CPU fallback)")
+        self.device, self.names = device, names
+        self.infos, self.blob, (ws_b, fr_b), host, offsets = parse_jpeg(files, names, blob=True, pin=True)
+        self.files_bytes = int(offsets[-1])
+        with torch.cuda.device(device):
+            self.files = host.to(device, non_blocking=True)
+            self.meta = self.blob.to(device, non_blocking=True)
+            self.workspace = torch.empty(max(ws_b, 1), dtype=torch.uint8, device=device)
+            self.arena = torch.empty(max(fr_b, 1), dtype=torch.uint8, device=device)
+            self.errors = torch.zeros(len(self.infos), dtype=torch.int32, device=device)
+        self._host = host                                # the pinned source of the asynchronous copy
+        self._sizes = (ws_b, fr_b)
+
+    def decode(self, phases=JPEG_ALL):
+        p = lambda t: ctypes.c_void_p(t.data_ptr())     # noqa: E731
+        with torch.cuda.device(self.device):
+            _check(lib().yfv2_jpeg_decode(p(self.blob), p(self.meta), self.blob.numel(), p(self.files), self.files_bytes, p(self.arena),
+                                          self._sizes[1], p(self.errors), p(self.workspace), self._sizes[0], phases,
+                                          _stream(self.device)), "jpeg_decode")
+
+    def check(self):
+        errs = self.errors.cpu().tolist()
+        bad = [(i, e) for i, e in enumerate(errs) if e]
+        if bad:
+            what = {1: "entropy-coded data ran out (truncated or corrupt)", 2: "invalid Huffman code", 3: "truncated, invalid Huffman code"}
+            raise Yfv2Error("decode_jpeg: %d of %d files failed to decode: %s" % (
+                len(bad), len(errs), "; ".join("%s: %s" % (_jpeg_name(self.names, i), what.get(e, "error %d" % e)) for i, e in bad)))
+
+    def frames(self):
+        return [self.arena[i["frame_offset"]:i["frame_offset"] + 3 * i["w"] * i["h"]].view(i["h"], i["w"], 3) for i in self.infos]
+
+
+def decode_jpeg(files, device=None, names=None):
+    """cv2.imread of JPEG files on the device: files are bytes or uint8 numpy buffers (a file's contents); returns one CUDA uint8
+    [h, w, 3] BGR tensor per file, views into one arena, bit-identical to cv2.imdecode(buf, IMREAD_COLOR) / cv2.imread (EXIF
+    orientation applied).  A file outside the supported subset (include/yfv2.h) raises Yfv2Error before anything is launched,
+    naming it (names[i] when given) and why; so does a file whose entropy-coded data is cut short or corrupt, after the decode."""
+    b = JpegBatch(files, device, names)
+    b.decode()
+    b.check()
+    return b.frames()
 
 
 YUV420_LAYOUTS = ("nv12", "nv21", "i420", "yv12")
