@@ -320,9 +320,11 @@ YFV2_API int yfv2_resize_yuv422_u8(const yfv2_yuv422_frame* frames, int N, int H
  *
  * yfv2_jpeg_decode: files (device) is a copy of the same buffer, files_bytes long; meta_dev a device copy of the blob, meta_host the
  * blob itself (checked, with the buffer sizes, before anything is launched).  Writes every frame into `frames` and a per-image flag
- * word into errors[N] (device int32; 1: a segment ran out of data, 2: an invalid Huffman code; the image is then decoded as libjpeg
- * would continue, zero bits past the end).  phases: YFV2_JPEG_ALL, or the subset of the three launches to run in this call (entropy
- * decode into the workspace, IDCT into planes in the workspace, upsample + colour into frames), for timing them separately.
+ * word into errors[N] (device int32; 1: a segment ran out of data or the file ends inside the scan, 2: an invalid Huffman code,
+ * 4: RSTn markers out of sequence; the frame is still written, from zero bits past a segment's end, but is not promised to equal
+ * cv2's: a frame with no flag set is cv2's byte for byte).  phases: YFV2_JPEG_ALL, or the subset of the three launches to run in
+ * this call (entropy decode into the workspace, IDCT into planes in the workspace, upsample + colour into frames), for timing them
+ * separately.
  * Nothing is allocated and nothing synchronises. */
 #define YFV2_JPEG_ENTROPY 1
 #define YFV2_JPEG_IDCT    2

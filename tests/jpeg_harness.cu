@@ -1,13 +1,17 @@
-// CPU build of the JPEG decode (tests/test_jpeg_cpu.py compiles it with nvcc): yfv2_jpeg_parse from libyfv2.so, then the three
-// phases through the same jpeg.cuh functions the device kernels call, one file at a time.
+// CPU build of the JPEG decode (tests/test_jpeg_cpu.py compiles it with nvcc): yfv2_jpeg_parse, then the three phases through the
+// same jpeg.cuh functions the device kernels call, one file at a time.
 //   jpeg_harness IN OUT [IN OUT ...]  -> one line per file: "<parse status> <w> <h> <error flags>"; OUT receives the BGR bytes.
-// Each file is read into a buffer of exactly its size, so an address-sanitised build sees any read past its end.
+// Each file is read into a buffer of exactly its size, and the parser (k_jpeg.cu) is compiled into this program rather than taken
+// from libyfv2.so, so an address-sanitised build sees any read past a file's end, by the parse or by the decode.
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
 
-#include "../include/yfv2.h"
-#include "../yolo-fastestv2_b200/csrc/jpeg.cuh"
+#include "../yolo-fastestv2_b200/csrc/k_jpeg.cu"
+
+namespace yfv2 {
+void set_error(const char*, ...) {}   // the library keeps the message for yfv2_last_error; the harness prints info.reason
+}  // namespace yfv2
 
 using namespace yfv2::jpeg;
 

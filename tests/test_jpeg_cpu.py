@@ -84,17 +84,15 @@ def test_parse_and_decode_refuse_bad_arguments(golden):
 
 @pytest.fixture(scope="module")
 def harness(tmp_path_factory):
-    """tests/jpeg_harness.cu built for the host against libyfv2.so (address-sanitised where the toolchain supports it)."""
-    import yfv2_engine
-    lib = yfv2_engine.lib()._name
+    """tests/jpeg_harness.cu built for the host with the parser compiled in (address-sanitised where the toolchain supports it;
+    otherwise a plain build, which still compares bytes but no longer sees reads past a file's end)."""
     if not os.path.exists(NVCC) and shutil.which("nvcc") is None:
         pytest.skip("no nvcc")
     nvcc = NVCC if os.path.exists(NVCC) else shutil.which("nvcc")
     d = tmp_path_factory.mktemp("jpeg_harness")
     exe = str(d / "harness")
-    libdir = os.path.dirname(lib)
-    base = [nvcc, "-std=c++17", "-O1", "-Wno-deprecated-gpu-targets", os.path.join(ROOT, "tests", "jpeg_harness.cu"), "-o", exe,
-            "-L", libdir, "-lyfv2", "-Xlinker", "-rpath=" + libdir]
+    base = [nvcc, "-std=c++17", "-O1", "-Wno-deprecated-gpu-targets", "-gencode", "arch=compute_90a,code=sm_90a",
+            os.path.join(ROOT, "tests", "jpeg_harness.cu"), "-o", exe]
     r = subprocess.run(base[:4] + ["-Xcompiler", "-fsanitize=address", "-Xlinker", "-lasan"] + base[4:], capture_output=True, text=True)
     if r.returncode != 0:
         subprocess.run(base, check=True, capture_output=True)

@@ -1,7 +1,7 @@
 // Baseline JPEG decode: the decode tables the host parser (k_jpeg.cu) packs into the metadata blob, and the per-segment, per-block
 // and per-pixel functions of the three device phases.  Everything below is __host__ __device__, so tests/jpeg_harness.cu runs the
 // same functions on the CPU.  The arithmetic is libjpeg-turbo's (what cv2.imread decodes with): jdhuff's bit reader and Huffman
-// decode, jidctint's jpeg_idct_islow with its range-limit table, jdsample's fancy upsampling and jdcolor's YCbCr -> RGB tables.
+// decode, jpeg_idct_islow as its x86 SIMD code computes it, jdsample's fancy upsampling and jdcolor's YCbCr -> RGB tables.
 #pragma once
 #include <stdint.h>
 
@@ -17,8 +17,9 @@ namespace jpeg {
 constexpr uint32_t kMagic = 0x3147504a;   // "JPG1": a blob yfv2_jpeg_parse wrote
 constexpr int kMaxSide = 32768;           // the resize's limit
 constexpr int kFastBits = 9;              // first-level Huffman lookup
-constexpr int kErrShort = 1;              // an entropy-coded segment ran out of data (zero bits were decoded)
+constexpr int kErrShort = 1;              // a segment ran out of data (zero bits were decoded), or the file ends inside the scan
 constexpr int kErrCode = 2;               // a bit pattern that is no Huffman code of its table
+constexpr int kErrRestart = 4;            // RSTn markers out of sequence: libjpeg resyncs and its intervals get other data
 
 struct alignas(16) Huff {           // 16-byte aligned: the entropy kernel copies tables with 16-byte accesses
     uint16_t fast[1 << kFastBits];   // (length << 8) | symbol of the code the next kFastBits bits start with; 0: a longer code
@@ -55,7 +56,8 @@ struct Image {
 };
 
 struct Seg {
-    int img, mcu0, nmcu, pad_;
+    int img, mcu0, nmcu;
+    int err;                // kErr* flags the parse found: kErrShort when the file ends inside the scan, kErrRestart
     long long begin, end;   // bytes of the file arena, RSTn / end-of-scan markers excluded
 };
 
@@ -167,7 +169,7 @@ JPEG_HD void decode_block(Bits& b, const Huff& dc, const Huff& ac, int& pred, in
 JPEG_HD int decode_segment(const Image& im, const Seg& s, const uint8_t* files, uint8_t* ws, const Huff* dc, const Huff* ac) {
     Bits b{files + s.begin, files + s.end, 0, 0, 0};
     int pred[3] = {0, 0, 0};
-    int err = 0;
+    int err = s.err;
     for (int m = s.mcu0; m < s.mcu0 + s.nmcu; ++m) {
         const int mx = m % im.mcux, my = m / im.mcux;
         for (int c = 0; c < im.ncomp; ++c) {
@@ -185,72 +187,59 @@ JPEG_HD int decode_segment(const Image& im, const Seg& s, const uint8_t* files, 
 }
 
 // ---- dequantise + IDCT --------------------------------------------------------------------------------------------------------
-// jidctint.c's post-IDCT range limit: the index is masked with 1023, so values far outside 0..255 wrap instead of clamping
-JPEG_HD int idct_range_limit(long long x) {
-    const int t = (int)(x & 1023);
-    return t < 128 ? t + 128 : t < 512 ? 255 : t < 896 ? 0 : t - 896;
+// jpeg_idct_islow (CONST_BITS 13, PASS1_BITS 2) as libjpeg-turbo's x86 SIMD code computes it (jsimd_idct_islow, jidctint-sse2.asm
+// and jidctint-avx2.asm), which is what cv2.imread runs on x86-64.  It equals jidctint.c while every value fits in int16, which
+// encoder output always does.  Corrupt or hand-made coefficients do not, and then the SIMD arithmetic decides the pixels:
+//  - dequantisation keeps the low 16 bits of coef * q (pmullw);
+//  - in0 + in4, in0 - in4, in7 + in3 and in5 + in1 are 16-bit sums that wrap (paddw / psubw);
+//  - the products and their sums are 32-bit and wrap (pmaddwd / paddd), so they are computed here in uint32_t;
+//  - each pass's descaled outputs saturate to int16 (packssdw); pass 2's then saturate to -128..127 (packsswb) before + 128,
+//    which clamps where jidctint.c's range-limit table (indexed & 1023) would wrap;
+//  - when rows 1-7 of the block's coefficients are all zero, pass 1 writes the dequantised row 0 shifted left by 2 in 16 bits
+//    (psllw), which wraps where the full pass would saturate.
+JPEG_HD int wrap16(uint32_t x) { return (int16_t)(uint16_t)x; }
+JPEG_HD int clampi(int x, int lo, int hi) { return x < lo ? lo : x > hi ? hi : x; }
+
+// One 1-D transform of 8 int16 inputs in[0], in[st], ..., in[7 * st]; out[k] = the descaled output k (>> S) in 32 bits
+template <int S>
+JPEG_HD void islow_1d(const int* in, int st, int* out) {
+    using u = uint32_t;
+    constexpr int F0298 = 2446, F0390 = 3196, F0541 = 4433, F0765 = 6270, F0899 = 7373, F1175 = 9633, F1501 = 12299,
+                  F1847 = 15137, F1961 = 16069, F2053 = 16819, F2562 = 20995, F3072 = 25172;
+    const u i0 = (u)in[0], i1 = (u)in[st], i2 = (u)in[2 * st], i3 = (u)in[3 * st], i4 = (u)in[4 * st], i5 = (u)in[5 * st],
+            i6 = (u)in[6 * st], i7 = (u)in[7 * st];
+    const u tmp3 = i2 * (u)(F0541 + F0765) + i6 * (u)F0541, tmp2 = i2 * (u)F0541 + i6 * (u)(F0541 - F1847);
+    const u tmp0 = (u)wrap16(i0 + i4) << 13, tmp1 = (u)wrap16(i0 - i4) << 13;
+    const u t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
+    const u z3 = (u)wrap16(i7 + i3), z4 = (u)wrap16(i5 + i1);
+    const u za = z3 * (u)(F1175 - F1961) + z4 * (u)F1175, zb = z3 * (u)F1175 + z4 * (u)(F1175 - F0390);
+    const u o0 = i7 * (u)(F0298 - F0899) + i1 * (u)-F0899 + za, o3 = i7 * (u)-F0899 + i1 * (u)(F1501 - F0899) + zb;
+    const u o1 = i5 * (u)(F2053 - F2562) + i3 * (u)-F2562 + zb, o2 = i5 * (u)-F2562 + i3 * (u)(F3072 - F2562) + za;
+    constexpr u R = 1u << (S - 1);
+    out[0] = (int)(t10 + o3 + R) >> S; out[7] = (int)(t10 - o3 + R) >> S;
+    out[1] = (int)(t11 + o2 + R) >> S; out[6] = (int)(t11 - o2 + R) >> S;
+    out[2] = (int)(t12 + o1 + R) >> S; out[5] = (int)(t12 - o1 + R) >> S;
+    out[3] = (int)(t13 + o0 + R) >> S; out[4] = (int)(t13 - o0 + R) >> S;
 }
 
-// jpeg_idct_islow (CONST_BITS 13, PASS1_BITS 2) in 64-bit arithmetic like its JLONG.  The zero-AC shortcuts of both passes give
-// the same values as the full computation, so they are not restated.
 JPEG_HD void idct_islow(const int16_t* coef, const uint16_t* q, uint8_t* out, int pitch) {
-    constexpr int CB = 13, P1 = 2;
-    constexpr long long F0298 = 2446, F0390 = 3196, F0541 = 4433, F0765 = 6270, F0899 = 7373, F1175 = 9633, F1501 = 12299,
-                        F1847 = 15137, F1961 = 16069, F2053 = 16819, F2562 = 20995, F3072 = 25172;
-    int ws[64];
+    int in[64], ws[64], o[8];
+    bool ac = false;                                       // any coefficient in rows 1-7 (the SIMD's zero-column test)
+    for (int k = 0; k < 64; ++k) {
+        in[k] = wrap16((uint32_t)(coef[k] * (int)q[k]));
+        ac = ac || (k >= 8 && coef[k] != 0);
+    }
     for (int c = 0; c < 8; ++c) {
-        long long in[8];
-        for (int r = 0; r < 8; ++r) in[r] = (long long)(coef[r * 8 + c] * (int)q[r * 8 + c]);
-        long long z2 = in[2], z3 = in[6];
-        long long z1 = (z2 + z3) * F0541;
-        long long tmp2 = z1 + z3 * -F1847, tmp3 = z1 + z2 * F0765;
-        long long tmp0 = (in[0] + in[4]) * (1LL << CB), tmp1 = (in[0] - in[4]) * (1LL << CB);
-        const long long tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
-        tmp0 = in[7]; tmp1 = in[5]; tmp2 = in[3]; tmp3 = in[1];
-        z1 = tmp0 + tmp3; z2 = tmp1 + tmp2; z3 = tmp0 + tmp2;
-        long long z4 = tmp1 + tmp3;
-        const long long z5 = (z3 + z4) * F1175;
-        tmp0 *= F0298; tmp1 *= F2053; tmp2 *= F3072; tmp3 *= F1501;
-        z1 *= -F0899; z2 *= -F2562; z3 *= -F1961; z4 *= -F0390;
-        z3 += z5; z4 += z5;
-        tmp0 += z1 + z3; tmp1 += z2 + z4; tmp2 += z2 + z3; tmp3 += z1 + z4;
-        constexpr int S = CB - P1;
-        constexpr long long R = 1LL << (S - 1);
-        ws[0 * 8 + c] = (int)((tmp10 + tmp3 + R) >> S);
-        ws[7 * 8 + c] = (int)((tmp10 - tmp3 + R) >> S);
-        ws[1 * 8 + c] = (int)((tmp11 + tmp2 + R) >> S);
-        ws[6 * 8 + c] = (int)((tmp11 - tmp2 + R) >> S);
-        ws[2 * 8 + c] = (int)((tmp12 + tmp1 + R) >> S);
-        ws[5 * 8 + c] = (int)((tmp12 - tmp1 + R) >> S);
-        ws[3 * 8 + c] = (int)((tmp13 + tmp0 + R) >> S);
-        ws[4 * 8 + c] = (int)((tmp13 - tmp0 + R) >> S);
+        if (!ac) {
+            for (int r = 0; r < 8; ++r) ws[r * 8 + c] = wrap16((uint32_t)in[c] << 2);
+            continue;
+        }
+        islow_1d<11>(in + c, 8, o);
+        for (int r = 0; r < 8; ++r) ws[r * 8 + c] = clampi(o[r], -32768, 32767);
     }
     for (int r = 0; r < 8; ++r) {
-        const int* w = ws + r * 8;
-        long long z2 = w[2], z3 = w[6];
-        long long z1 = (z2 + z3) * F0541;
-        long long tmp2 = z1 + z3 * -F1847, tmp3 = z1 + z2 * F0765;
-        long long tmp0 = ((long long)w[0] + w[4]) * (1LL << CB), tmp1 = ((long long)w[0] - w[4]) * (1LL << CB);
-        const long long tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
-        tmp0 = w[7]; tmp1 = w[5]; tmp2 = w[3]; tmp3 = w[1];
-        z1 = tmp0 + tmp3; z2 = tmp1 + tmp2; z3 = tmp0 + tmp2;
-        long long z4 = tmp1 + tmp3;
-        const long long z5 = (z3 + z4) * F1175;
-        tmp0 *= F0298; tmp1 *= F2053; tmp2 *= F3072; tmp3 *= F1501;
-        z1 *= -F0899; z2 *= -F2562; z3 *= -F1961; z4 *= -F0390;
-        z3 += z5; z4 += z5;
-        tmp0 += z1 + z3; tmp1 += z2 + z4; tmp2 += z2 + z3; tmp3 += z1 + z4;
-        constexpr int S = CB + P1 + 3;
-        constexpr long long R = 1LL << (S - 1);
-        uint8_t* o = out + (long long)r * pitch;
-        o[0] = (uint8_t)idct_range_limit((tmp10 + tmp3 + R) >> S);
-        o[7] = (uint8_t)idct_range_limit((tmp10 - tmp3 + R) >> S);
-        o[1] = (uint8_t)idct_range_limit((tmp11 + tmp2 + R) >> S);
-        o[6] = (uint8_t)idct_range_limit((tmp11 - tmp2 + R) >> S);
-        o[2] = (uint8_t)idct_range_limit((tmp12 + tmp1 + R) >> S);
-        o[5] = (uint8_t)idct_range_limit((tmp12 - tmp1 + R) >> S);
-        o[3] = (uint8_t)idct_range_limit((tmp13 + tmp0 + R) >> S);
-        o[4] = (uint8_t)idct_range_limit((tmp13 - tmp0 + R) >> S);
+        islow_1d<18>(ws + r * 8, 1, o);
+        for (int c = 0; c < 8; ++c) out[(long long)r * pitch + c] = (uint8_t)(clampi(o[c], -128, 127) + 128);
     }
 }
 

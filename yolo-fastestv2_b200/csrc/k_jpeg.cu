@@ -102,7 +102,7 @@ void build_huff(const RawHuff& raw, bool dc, Huff& t) {
 
 // EXIF orientation (tag 0x0112 of IFD0) from an APP1 payload starting "Exif\0\0"; 1 when absent or out of range
 int exif_orientation(const uint8_t* p, int n) {
-    if (n < 14 || memcmp(p, "Exif\0\0", 6) != 0) return 0;
+    if (n < 14 || memcmp(p, "Exif\0\0", 6) != 0) return 1;
     const uint8_t* t = p + 6;
     const int tn = n - 6;
     bool le;
@@ -120,10 +120,9 @@ int exif_orientation(const uint8_t* p, int n) {
     const int cnt = u16((int)ifd);
     for (int i = 0; i < cnt; ++i) {
         const long long e = (long long)ifd + 2 + 12LL * i;
-        if (e + 12 > tn) break;
+        if (e + 10 > tn) break;   // OpenCV reads an entry whose last 2 bytes (past the 16-bit value) are cut off
         if (u16((int)e) == 0x0112) {
-            const int type = u16((int)e + 2);
-            const int v = type == 3 ? u16((int)e + 8) : type == 4 ? (int)u32((int)e + 8) : 0;
+            const int v = u16((int)e + 8);   // OpenCV's ExifReader: a 16-bit word at the value offset, whatever the type and count
             return v >= 1 && v <= 8 ? v : 1;
         }
     }
@@ -147,13 +146,16 @@ const char* sof_name(int m) {
     }
 }
 
-// Offset just past the entropy-coded data starting at `pos`; appends one [begin, end) range per RSTn-delimited piece
-size_t scan_entropy(const uint8_t* f, size_t size, size_t pos, long long file_off, std::vector<std::pair<long long, long long>>& r) {
+// Offset just past the entropy-coded data starting at `pos`; appends one [begin, end) range per RSTn-delimited piece, and to
+// `ends` the marker byte after it (-1: the file ends first)
+size_t scan_entropy(const uint8_t* f, size_t size, size_t pos, long long file_off, std::vector<std::pair<long long, long long>>& r,
+                    std::vector<int>& ends) {
     size_t begin = pos, i = pos;
     while (true) {
         const void* q = i < size ? memchr(f + i, 0xFF, size - i) : nullptr;
         if (!q) {                                            // no end-of-scan marker: a truncated file, the last piece ends there
             r.emplace_back(file_off + (long long)begin, file_off + (long long)size);
+            ends.push_back(-1);
             return size;
         }
         i = (const uint8_t*)q - f;
@@ -161,10 +163,12 @@ size_t scan_entropy(const uint8_t* f, size_t size, size_t pos, long long file_of
         while (j < size && f[j] == 0xFF) ++j;
         if (j >= size) {
             r.emplace_back(file_off + (long long)begin, file_off + (long long)i);
+            ends.push_back(-1);
             return size;
         }
         if (f[j] == 0x00) { i = j + 1; continue; }
         r.emplace_back(file_off + (long long)begin, file_off + (long long)i);
+        ends.push_back(f[j]);
         if (f[j] >= 0xD0 && f[j] <= 0xD7) { begin = i = j + 1; continue; }
         return i;                                            // the marker that ends the scan
     }
@@ -279,7 +283,7 @@ void parse_file(const uint8_t* f, size_t size, long long file_off, Parsed& P) {
             if (n < 2) refuse(YFV2_EINVAL, "bad DRI segment");
             P.restart = be16(s);
         } else if (m == 0xE0) {
-            if (n >= 5 && memcmp(s, "JFIF\0", 5) == 0) jfif = true;
+            if (n >= 14 && memcmp(s, "JFIF\0", 5) == 0) jfif = true;   // jdmarker's examine_app0 ignores a shorter one
         } else if (m == 0xE1) {
             if (!exif_seen && n >= 6 && memcmp(s, "Exif\0\0", 6) == 0) {
                 exif_seen = true;
@@ -315,15 +319,28 @@ void parse_file(const uint8_t* f, size_t size, long long file_off, Parsed& P) {
             const int mcux = (P.w + 8 * hmax - 1) / (8 * hmax), mcuy = (P.h + 8 * vmax - 1) / (8 * vmax);
             const long long mcus = (long long)mcux * mcuy;
             std::vector<std::pair<long long, long long>> ranges;
-            pos = scan_entropy(f, size, pos, file_off, ranges);
+            std::vector<int> ends;
+            pos = scan_entropy(f, size, pos, file_off, ranges, ends);
             const long long nseg = P.restart ? (mcus + P.restart - 1) / P.restart : 1;
             P.segs.clear();
             for (long long k = 0; k < nseg; ++k) {
                 Seg g{};
                 g.mcu0 = (int)(k * (P.restart ? P.restart : mcus));
                 g.nmcu = (int)(P.restart ? (mcus - g.mcu0 < P.restart ? mcus - g.mcu0 : P.restart) : mcus);
-                if (k < (long long)ranges.size()) { g.begin = ranges[k].first; g.end = ranges[k].second; }
-                else { g.begin = g.end = ranges.back().second; }   // a missing interval decodes from no data (flagged)
+                if (k < (long long)ranges.size()) {
+                    g.begin = ranges[k].first;
+                    g.end = ranges[k].second;
+                    // cv2.imdecode returns no image when the file ends inside the scan
+                    if (ends[k] < 0) g.err |= kErrShort;
+                    // The interval ends at RST(k mod 8).  libjpeg's jpeg_resync_to_restart takes a marker 1 or 2 numbers ahead
+                    // as a missing one (this interval decodes from no data) and 1 or 2 behind as a stale one (the data after it
+                    // is skipped): its intervals then hold other data than these segments.  A marker 3 to 5 away it takes as the
+                    // expected one, as the segments here do.
+                    const int d = (ends[k] - 0xD0 - (int)k) & 7;
+                    if (k + 1 < nseg && ends[k] >= 0xD0 && ends[k] <= 0xD7 && (d == 1 || d == 2 || d == 6 || d == 7)) g.err |= kErrRestart;
+                } else {
+                    g.begin = g.end = ranges.back().second;      // a missing interval decodes from no data (flagged)
+                }
                 P.segs.push_back(g);
             }
             {

@@ -888,9 +888,10 @@ class JpegBatch:
         errs = self.errors.cpu().tolist()
         bad = [(i, e) for i, e in enumerate(errs) if e]
         if bad:
-            what = {1: "entropy-coded data ran out (truncated or corrupt)", 2: "invalid Huffman code", 3: "truncated, invalid Huffman code"}
+            what = ("entropy-coded data ran out (truncated or corrupt)", "invalid Huffman code", "restart markers out of sequence")
+            why = lambda e: ", ".join(w for b, w in enumerate(what) if e >> b & 1) or "error %d" % e  # noqa: E731
             raise Yfv2Error("decode_jpeg: %d of %d files failed to decode: %s" % (
-                len(bad), len(errs), "; ".join("%s: %s" % (_jpeg_name(self.names, i), what.get(e, "error %d" % e)) for i, e in bad)))
+                len(bad), len(errs), "; ".join("%s: %s" % (_jpeg_name(self.names, i), why(e)) for i, e in bad)))
 
     def frames(self):
         return [self.arena[i["frame_offset"]:i["frame_offset"] + 3 * i["w"] * i["h"]].view(i["h"], i["w"], 3) for i in self.infos]
