@@ -307,43 +307,57 @@ YFV2_API int yfv2_resize_yuv422_u8(const yfv2_yuv422_frame* frames, int N, int H
 /* ---- JPEG files -> packed HWC BGR frames: cv2.imread(path) (test.py:34; utils/datasets.py:106) on the device -----------------
  * The bytes OpenCV 4.13 (libjpeg-turbo 3.1) returns for IMREAD_COLOR: ISLOW IDCT, fancy upsampling, jdcolor's YCbCr -> BGR, grey
  * replicated to B = G = R, and the EXIF orientation applied.  Supported: baseline sequential Huffman-coded DCT (SOF0, SOF1) with
- * 8-bit samples, 1 or 3 components, luma sampling 1x1, 2x1, 2x2, 1x2 or 4x1 with 1x1 chroma, restart intervals, one scan.  Anything
- * else (progressive, arithmetic, lossless, hierarchical, 12/16-bit, 2 or 4 components, Adobe RGB, several scans, other sampling,
- * not a JPEG) is refused per file by the parse, with a reason.
+ * 8-bit samples, 1 or 3 components, luma sampling 1x1, 2x1, 2x2, 1x2 or 4x1 with 1x1 chroma, restart intervals, one scan; with
+ * flags YFV2_JPEG_PROGRESSIVE also progressive Huffman-coded DCT (SOF2) within the same limits, up to 128 scans, tables and restart
+ * intervals redefined between scans.  Anything else (progressive without the flag, arithmetic, lossless, hierarchical, 12/16-bit,
+ * 2 or 4 components, Adobe RGB, several scans of a baseline file, other sampling, not a JPEG) is refused per file by the parse,
+ * with a reason.  A progressive file is also refused, its reason naming the scan, component or coefficient, when a scan breaks
+ * libjpeg's progression rules (YFV2_EINVAL: a DC scan with Se != 0; an AC scan with Ss > Se, Se > 63 or several components; Ah != 0
+ * with Al != Ah - 1; Al > 13: cv2 returns no image), when it goes against what earlier scans sent (YFV2_EUNSUPPORTED: AC before
+ * the component's DC, or Ah other than the bits already known), when a coefficient is never sent or not refined to its last bit
+ * (YFV2_EUNSUPPORTED: libjpeg smooths such blocks), when a scan lists its components out of frame order (YFV2_EUNSUPPORTED:
+ * libjpeg decodes it, this decoder does not), or when it has more than 128 scans.  A progressive file that ends before its
+ * EOI is accepted and flagged 1: cv2.imdecode returns no image for it.
  *
- * yfv2_jpeg_parse (host only, no device needed): the N files lie in one host buffer, file i at files_host[offsets_host[i] ..
+ * yfv2_jpeg_parse_ex (host only, no device needed): the N files lie in one host buffer, file i at files_host[offsets_host[i] ..
  * offsets_host[i+1]).  Fills info_host[N] (status 0 or a YFV2_E* code with its reason; size after orientation; frame_offset) and
  * the sizes the decode needs: meta_bytes (the blob), workspace_bytes, frames_bytes (the arena; frame i is [h][w][3] BGR at
  * frame_offset, rows 3*w apart, usable as a yfv2_frame as it is).  With meta_host NULL only the sizes are computed; otherwise the
  * blob (decode tables, geometry and the byte range of every entropy-coded segment) is written into meta_host[meta_cap].  Returns
- * the first refused file's code (yfv2_last_error names it), YFV2_ENOMEM when meta_cap is too small.
+ * the first refused file's code (yfv2_last_error names it), YFV2_ENOMEM when meta_cap is too small, YFV2_EINVAL for flag bits other
+ * than YFV2_JPEG_PROGRESSIVE.  yfv2_jpeg_parse is yfv2_jpeg_parse_ex with flags 0.
  *
  * yfv2_jpeg_decode: files (device) is a copy of the same buffer, files_bytes long; meta_dev a device copy of the blob, meta_host the
  * blob itself (checked, with the buffer sizes, before anything is launched).  Writes every frame into `frames` and a per-image flag
- * word into errors[N] (device int32; 1: a segment ran out of data or the file ends inside the scan, 2: an invalid Huffman code,
+ * word into errors[N] (device int32; 1: a segment ran out of data, the file ends inside the scan or a progressive file before its
+ * EOI, 2: an invalid Huffman code or a progressive scan's run past its band,
  * 4: RSTn markers out of sequence; the frame is still written, from zero bits past a segment's end, but is not promised to equal
  * cv2's: a frame with no flag set is cv2's byte for byte).  phases: YFV2_JPEG_ALL, or the subset of the three launches to run in
  * this call (entropy decode into the workspace, IDCT into planes in the workspace, upsample + colour into frames), for timing them
- * separately.
+ * separately.  YFV2_JPEG_ENTROPY includes the progressive images' scans: their coefficients are zeroed, then one launch per level of
+ * scans that depend on each other.
  * Nothing is allocated and nothing synchronises. */
 #define YFV2_JPEG_ENTROPY 1
 #define YFV2_JPEG_IDCT    2
 #define YFV2_JPEG_COLOR   4
 #define YFV2_JPEG_ALL     7
+#define YFV2_JPEG_PROGRESSIVE 1   /* yfv2_jpeg_parse_ex flags: accept progressive files */
 typedef struct yfv2_jpeg_info {
     int status;            /* 0, or why the file is refused: YFV2_EUNSUPPORTED (out of scope) or YFV2_EINVAL (malformed) */
     int w, h;              /* the decoded frame's size, EXIF orientation applied */
     int components;        /* 1 (grey) or 3 (YCbCr) */
     int h_samp, v_samp;    /* luma sampling factors (1, 1 for grey) */
     int orientation;       /* EXIF orientation 1..8 (1 without EXIF) */
-    int restart_interval;  /* MCUs per restart interval, 0: none */
-    int segments;          /* entropy-coded segments, each decoded by one thread */
-    int reserved;
+    int restart_interval;  /* MCUs per restart interval (of the first scan), 0: none */
+    int segments;          /* entropy-coded segments of all scans, each decoded by one thread */
+    int scans;             /* 1, or a progressive file's scans */
     long long frame_offset;/* byte offset of the frame in the arena */
     char reason[96];       /* status != 0: what is refused */
 } yfv2_jpeg_info;
 YFV2_API int yfv2_jpeg_parse(const uint8_t* files_host, const long long* offsets_host, int N, yfv2_jpeg_info* info_host,
                              void* meta_host, size_t meta_cap, size_t* meta_bytes, size_t* workspace_bytes, size_t* frames_bytes);
+YFV2_API int yfv2_jpeg_parse_ex(const uint8_t* files_host, const long long* offsets_host, int N, int flags, yfv2_jpeg_info* info_host,
+                                void* meta_host, size_t meta_cap, size_t* meta_bytes, size_t* workspace_bytes, size_t* frames_bytes);
 YFV2_API int yfv2_jpeg_decode(const void* meta_host, const void* meta_dev, size_t meta_bytes, const uint8_t* files, size_t files_bytes,
                               uint8_t* frames, size_t frames_bytes, int* errors, void* workspace, size_t workspace_bytes, int phases,
                               void* stream);

@@ -2,7 +2,12 @@
 """JPEG decode on the device (yfv2_engine.decode_jpeg) at batch: 256 and 1024 files of the reference's two photos (500x334 and
 500x375, 4:2:0, no restart markers) repeated, and of the 1920x1080 4:2:0 fixture (tests/golden/jpeg_cases.npz).
 
-  python tools/bench_jpeg.py [--batches 256,1024 --reps 5]
+  python tools/bench_jpeg.py [--batches 256,1024 --reps 5] [--progressive]
+
+--progressive runs the same rows on progressive files (decode_jpeg(progressive=True)): the two photos re-coded losslessly as
+progressive files with cv2's script (tests/golden/jpeg_progressive.npz, tx_cv2_*: the same coefficients as the baseline rows'
+photos) and the progressive 1080p fixture, and adds entropy_level_ms (the entropy phase's kernels per level, from
+torch.profiler) and blob_bytes_per_file.
 
 Prints one JSON line per (files, batch) with:
   parse_ms        yfv2_jpeg_parse of the batch on the host (one core; both calls: sizes, then the blob), median;
@@ -61,14 +66,39 @@ def event_ms(fn, reps):
     return float(np.median(ts))
 
 
+def level_ms(fn, reps):
+    """Median device time of each prog_entropy_kernel launch of fn (one per level, in launch order), from torch.profiler"""
+    from torch.profiler import ProfilerActivity, profile
+    fn()
+    torch.cuda.synchronize()
+    runs = []
+    for _ in range(reps):
+        with profile(activities=[ProfilerActivity.CUDA]) as p:
+            fn()
+            torch.cuda.synchronize()
+        ev = sorted((e for e in p.events() if "prog_entropy_kernel" in e.name and e.device_type.name == "CUDA"),
+                    key=lambda e: e.time_range.start)
+        runs.append([e.time_range.elapsed_us() / 1e3 for e in ev])
+    n = max(len(r) for r in runs)                            # the profiler can drop an event of a rep: medians of complete reps
+    full = [r for r in runs if len(r) == n]
+    return [float(np.median([r[k] for r in full])) for k in range(n)]
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batches", default="256,1024")
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--progressive", action="store_true")
     args = ap.parse_args()
     gdir = os.path.join(ROOT, "tests", "golden")
-    photos = [np.fromfile(os.path.join(gdir, s + ".jpg"), np.uint8) for s in ("000139", "000004")]
-    fullhd = [np.load(os.path.join(gdir, "jpeg_cases.npz"))["jpg_fullhd_420"]]
+    prog = args.progressive
+    if prog:
+        pg = np.load(os.path.join(gdir, "jpeg_progressive.npz"))
+        photos = [pg["jpg_tx_cv2_" + s] for s in ("000139", "000004")]
+        fullhd = [pg["jpg_cv2_fullhd_420"]]
+    else:
+        photos = [np.fromfile(os.path.join(gdir, s + ".jpg"), np.uint8) for s in ("000139", "000004")]
+        fullhd = [np.load(os.path.join(gdir, "jpeg_cases.npz"))["jpg_fullhd_420"]]
     try:
         import torchvision.io as tvio
     except Exception:                                      # noqa: BLE001  (nvJPEG is optional context)
@@ -78,16 +108,22 @@ def main():
     for label, src in (("photos", photos), ("fullhd", fullhd)):
         for bi, n in enumerate(int(b) for b in args.batches.split(",")):
             files = [src[i % len(src)] for i in range(n)]
-            eng.decode_jpeg(files[:8], "cuda")                             # warm-up: module load
-            res = {"files": label, "batch": n, "bytes_per_file": int(np.mean([f.size for f in files])), "gpu": card}
-            res["parse_ms"] = host_ms(lambda: eng.parse_jpeg(files, blob=True), args.reps)
-            res["decode_ms"] = host_ms(lambda: eng.decode_jpeg(files, "cuda"), args.reps)
-            b = eng.JpegBatch(files, "cuda")
+            kw = {"progressive": True} if prog else {}
+            eng.decode_jpeg(files[:8], "cuda", **kw)                        # warm-up: module load
+            res = {"files": label + ("_progressive" if prog else ""), "batch": n, "bytes_per_file": int(np.mean([f.size for f in files])),
+                   "gpu": card}
+            res["parse_ms"] = host_ms(lambda: eng.parse_jpeg(files, blob=True, **kw), args.reps)
+            res["decode_ms"] = host_ms(lambda: eng.decode_jpeg(files, "cuda", **kw), args.reps)
+            b = eng.JpegBatch(files, "cuda", **kw)
             b.decode()
             b.check()
             for ph, key in ((eng.JPEG_ENTROPY, "entropy_ms"), (eng.JPEG_IDCT, "idct_ms"), (eng.JPEG_COLOR, "color_ms")):
                 res[key] = event_ms(lambda: b.decode(ph), args.reps)
             res["segments"] = sum(i["segments"] for i in b.infos)
+            if prog:
+                res["scans"] = sum(i["scans"] for i in b.infos)
+                res["blob_bytes_per_file"] = b.blob.numel() // n
+                res["entropy_level_ms"] = level_ms(lambda: b.decode(eng.JPEG_ENTROPY), args.reps)
             del b
             res["img_per_s"] = n / res["decode_ms"] * 1e3
             if label == "photos" and bi == 0:
@@ -101,8 +137,8 @@ def main():
                 torch.manual_seed(1)
                 m = det.Detector(80, 3, True).cuda().eval()
                 cfg = synth.coco_cfg()
-                uf.detect_files(m, paths[:8], cfg)
-                res["detect_ms"] = host_ms(lambda: uf.detect_files(m, paths, cfg, 0.3, 0.4), args.reps)
+                uf.detect_files(m, paths[:8], cfg, **kw)
+                res["detect_ms"] = host_ms(lambda: uf.detect_files(m, paths, cfg, 0.3, 0.4, **kw), args.reps)
             if tvio is not None:
                 ts = [torch.from_numpy(f) for f in files]
                 tvio.decode_jpeg(ts[:8], device="cuda")

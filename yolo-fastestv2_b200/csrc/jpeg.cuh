@@ -61,6 +61,27 @@ struct Seg {
     long long begin, end;   // bytes of the file arena, RSTn / end-of-scan markers excluded
 };
 
+// ---- progressive images (yfv2_jpeg_parse_ex with YFV2_JPEG_PROGRESSIVE) ----------------------------------------------------
+// A progressive image's Image record has nseg = 0; its scans, their tables and their segments are in the arrays below.  Each scan
+// has a level: 1 + the highest level of the image's earlier scans whose (component, coefficient) sets it overlaps, so the scans of
+// one level write disjoint coefficients and read only what lower levels wrote.  The decode runs one launch per level.
+constexpr int kMaxScans = 128;            // scans per progressive file (libjpeg's default script, cv2's and Pillow's: 10, 6 for grey)
+
+struct Scan {
+    int ncomp, comp[3];   // the scan's components (indices into Image::comp, frame order); an AC scan has one
+    int ss, se, ah, al;   // spectral selection and successive approximation
+    int tab[3];           // Huff pool index of scan component k's DC table (DC first scans) or tab[0] the AC table; -1: none
+    int upr, units;       // units per row and units: MCUs when interleaved, else the component's ceil(dw / 8) x ceil(dh / 8) blocks
+    int level;
+};
+
+struct PSeg {
+    int img, scan, level;   // image, Scan index, the scan's level
+    int unit0, nunit;       // its MCUs (interleaved) or blocks (one component) in scan order
+    int err;                // kErr* flags the parse found (kErrShort also when the file ends before its EOI)
+    long long begin, end;   // bytes of the file arena, RSTn / end-of-scan markers excluded
+};
+
 struct Header {
     uint32_t magic;
     int n, nseg, max_blocks;     // images, segments, most blocks of one image
@@ -70,6 +91,10 @@ struct Header {
     long long workspace;         // workspace bytes the decode needs
     long long frames;            // arena bytes
     long long files;             // bytes of the file arena the segments point into
+    // progressive images; all zero when the batch has none
+    int nscan, nhuff, npseg, nlevel;                  // scans, pooled Huffman tables, segments, levels
+    long long scan_off, huff_off, pseg_off, lvl_off;  // Scan[nscan], Huff[nhuff], PSeg[npseg] (sorted by level), int[nlevel + 1]
+    long long prog_coef;         // workspace bytes [0, prog_coef) hold the progressive images' coefficients, zeroed before decode
 };
 
 // jpeg_natural_order with libjpeg's 16 extra entries, so a corrupt run past coefficient 63 lands on 63
@@ -185,6 +210,138 @@ JPEG_HD int decode_segment(const Image& im, const Seg& s, const uint8_t* files, 
     if (b.n < b.zeros) err |= kErrShort;   // some of the shifted-in zeros were decoded
     return err;
 }
+
+// ---- progressive entropy decode (libjpeg-turbo's jdphuff.c) -------------------------------------------------------------------
+// Each function decodes one block of one scan into coefficients earlier scans may have set; none zeroes a block (the decode zeroes
+// every progressive image's coefficients once, before its first scan).  A run that carries an AC symbol past the scan's band
+// (never in an encoder's output) writes outside the band, as libjpeg does, and sets kErrCode: scans of one level are decoded in
+// parallel on the premise that their bands are disjoint, so such a frame is not promised to be cv2's.
+JPEG_HD void prog_dc_first(Bits& b, const Huff& t, int al, int& pred, int16_t* blk, int& err) {
+    if (b.n < 32) b.fill();
+    const int s = huff_decode(b, t, err);
+    if (s) pred += receive_extend(b, s);
+    blk[0] = (int16_t)((uint32_t)pred << al);
+}
+
+JPEG_HD void prog_dc_refine(Bits& b, int al, int16_t* blk) {
+    if (b.n < 32) b.fill();
+    if (b.peek(1)) blk[0] = (int16_t)(blk[0] | (1 << al));
+    b.n -= 1;
+}
+
+JPEG_HD void prog_ac_first(Bits& b, const Huff& t, int ss, int se, int al, int& eobrun, int16_t* blk, int& err) {
+    if (eobrun > 0) {
+        --eobrun;
+        return;
+    }
+    for (int k = ss; k <= se; ++k) {
+        if (b.n < 32) b.fill();
+        const int rs = huff_decode(b, t, err);
+        const int r = rs >> 4, s = rs & 15;
+        if (s) {
+            k += r;
+            if (k > se) err |= kErrCode;
+            blk[natural(k)] = (int16_t)((uint32_t)receive_extend(b, s) << al);
+        } else if (r == 15) {
+            k += 15;
+        } else {
+            eobrun = 1 << r;                     // EOBr: this block and 2^r - 1 + r more bits' worth of blocks end here
+            if (r) {
+                eobrun += b.peek(r);
+                b.n -= r;
+            }
+            --eobrun;
+            break;
+        }
+    }
+}
+
+// One correction bit onto a coefficient already nonzero: its magnitude gains 1 << al unless that bit is already set
+JPEG_HD void prog_correct(Bits& b, int16_t& c, int p1) {
+    if (b.n < 32) b.fill();
+    if (b.peek(1) && (c & p1) == 0) c = (int16_t)(c >= 0 ? c + p1 : c - p1);
+    b.n -= 1;
+}
+
+// A symbol's size other than 1 is taken as 1 (libjpeg-turbo warns and goes on), so it is not flagged
+JPEG_HD void prog_ac_refine(Bits& b, const Huff& t, int ss, int se, int al, int& eobrun, int16_t* blk, int& err) {
+    const int p1 = 1 << al;
+    int k = ss;
+    if (eobrun == 0) {
+        for (; k <= se; ++k) {
+            if (b.n < 32) b.fill();
+            const int rs = huff_decode(b, t, err);
+            int r = rs >> 4, s = rs & 15;
+            if (s) {
+                s = b.peek(1) ? p1 : -p1;
+                b.n -= 1;
+            } else if (r != 15) {
+                eobrun = 1 << r;
+                if (r) {
+                    eobrun += b.peek(r);
+                    b.n -= r;
+                }
+                break;
+            }
+            do {                                 // skip r zero-history coefficients, correcting the nonzero ones passed
+                int16_t& c = blk[natural(k)];
+                if (c != 0) prog_correct(b, c, p1);
+                else if (--r < 0) break;
+                ++k;
+            } while (k <= se);
+            if (s) {
+                if (k > se) err |= kErrCode;
+                blk[natural(k)] = (int16_t)s;
+            }
+        }
+    }
+    if (eobrun > 0) {                            // in an EOB run: correction bits for the rest of the band
+        for (; k <= se; ++k) {
+            int16_t& c = blk[natural(k)];
+            if (c != 0) prog_correct(b, c, p1);
+        }
+        --eobrun;
+    }
+}
+
+// Every unit of progressive segment s of scan sc into the workspace's coefficients; tabs[k] is the table of scan component k (DC
+// first scans) or tabs[0] the AC table (the pool's, or a copy).  Restarts reset the DC predictors and the EOB run; returns kErr*.
+JPEG_HD int decode_prog_segment(const Image& im, const Scan& sc, const PSeg& s, const uint8_t* files, uint8_t* ws, const Huff* tabs) {
+    Bits b{files + s.begin, files + s.end, 0, 0, 0};
+    int pred[3] = {0, 0, 0}, eobrun = 0;
+    int err = s.err;
+    for (int u = s.unit0; u < s.unit0 + s.nunit; ++u) {
+        if (sc.ncomp > 1) {                      // interleaved (DC only): MCUs as in a baseline scan
+            const int mx = u % im.mcux, my = u / im.mcux;
+            for (int k = 0; k < sc.ncomp; ++k) {
+                const Comp& cp = im.comp[sc.comp[k]];
+                int16_t* coef = reinterpret_cast<int16_t*>(ws + cp.coef);
+                for (int bv = 0; bv < cp.v; ++bv)
+                    for (int bh = 0; bh < cp.h; ++bh) {
+                        int16_t* blk = coef + ((long long)(my * cp.v + bv) * cp.bw + mx * cp.h + bh) * 64;
+                        if (sc.ah == 0) prog_dc_first(b, tabs[k], sc.al, pred[k], blk, err);
+                        else prog_dc_refine(b, sc.al, blk);
+                    }
+            }
+            continue;
+        }
+        const Comp& cp = im.comp[sc.comp[0]];    // one component: its blocks in raster order, whatever the sampling
+        int16_t* blk = reinterpret_cast<int16_t*>(ws + cp.coef) + ((long long)(u / sc.upr) * cp.bw + u % sc.upr) * 64;
+        if (sc.ss == 0) {
+            if (sc.ah == 0) prog_dc_first(b, tabs[0], sc.al, pred[0], blk, err);
+            else prog_dc_refine(b, sc.al, blk);
+        } else if (sc.ah == 0) {
+            prog_ac_first(b, tabs[0], sc.ss, sc.se, sc.al, eobrun, blk, err);
+        } else {
+            prog_ac_refine(b, tabs[0], sc.ss, sc.se, sc.al, eobrun, blk, err);
+        }
+    }
+    if (b.n < b.zeros) err |= kErrShort;
+    return err;
+}
+
+// Tables of scan sc in use: 0 (DC refinement), ncomp (DC first) or 1 (AC)
+JPEG_HD int prog_ntabs(const Scan& sc) { return sc.ss == 0 ? (sc.ah == 0 ? sc.ncomp : 0) : 1; }
 
 // ---- dequantise + IDCT --------------------------------------------------------------------------------------------------------
 // jpeg_idct_islow (CONST_BITS 13, PASS1_BITS 2) as libjpeg-turbo's x86 SIMD code computes it (jsimd_idct_islow, jidctint-sse2.asm

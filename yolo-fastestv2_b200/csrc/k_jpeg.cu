@@ -6,6 +6,9 @@
 //   1. entropy_kernel: one thread per segment, Huffman decode into int16 coefficient blocks in the workspace;
 //   2. idct_kernel:    one thread per block, jpeg_idct_islow into one uint8 plane per component;
 //   3. color_kernel:   one thread per output pixel, upsampling, YCbCr -> BGR and the EXIF orientation into the frame arena.
+// Progressive files (yfv2_jpeg_parse_ex with YFV2_JPEG_PROGRESSIVE) have no baseline segments: phase 1 zeroes their coefficients
+// and runs prog_entropy_kernel once per level of their scans, one thread per segment of a scan (or of one restart interval).
+#include <algorithm>
 #include <climits>
 #include <cstddef>
 #include <cstdarg>
@@ -36,7 +39,48 @@ struct Parsed {
     int id[3] = {}, hs[3] = {}, vs[3] = {}, tq[3] = {};
     Image* im = nullptr;                 // filled at SOS (tables latched there), when the caller wants the blob
     std::vector<Seg> segs;
+    // a progressive file (SOF2 under YFV2_JPEG_PROGRESSIVE): its scans, their tables (Scan::tab indexes huffs) and segments
+    bool prog = false, eoi = false;
+    int restart0 = 0;                    // the first scan's restart interval
+    std::vector<Scan> scans;
+    std::vector<Huff> huffs;
+    std::vector<PSeg> psegs;             // PSeg::scan indexes scans
 };
+
+// One entropy-coded segment of a scan: units [u0, u0 + nu) of the scan, its bytes and the flags found while cutting it
+struct Piece {
+    int u0, nu, err;
+    long long begin, end;
+};
+
+// The segments of a scan of `units` MCUs (or blocks) with restart interval `restart`, from the RSTn-delimited byte ranges
+// scan_entropy found and the marker after each
+std::vector<Piece> cut_scan(long long units, int restart, const std::vector<std::pair<long long, long long>>& ranges,
+                            const std::vector<int>& ends) {
+    const long long nseg = restart ? (units + restart - 1) / restart : 1;
+    std::vector<Piece> out;
+    for (long long k = 0; k < nseg; ++k) {
+        Piece g{};
+        g.u0 = (int)(k * (restart ? restart : units));
+        g.nu = (int)(restart ? (units - g.u0 < restart ? units - g.u0 : restart) : units);
+        if (k < (long long)ranges.size()) {
+            g.begin = ranges[k].first;
+            g.end = ranges[k].second;
+            // cv2.imdecode returns no image when the file ends inside the scan
+            if (ends[k] < 0) g.err |= kErrShort;
+            // The interval ends at RST(k mod 8).  libjpeg's jpeg_resync_to_restart takes a marker 1 or 2 numbers ahead as a
+            // missing one (this interval decodes from no data) and 1 or 2 behind as a stale one (the data after it is skipped):
+            // its intervals then hold other data than these segments.  A marker 3 to 5 away it takes as the expected one, as the
+            // segments here do.
+            const int d = (ends[k] - 0xD0 - (int)k) & 7;
+            if (k + 1 < nseg && ends[k] >= 0xD0 && ends[k] <= 0xD7 && (d == 1 || d == 2 || d == 6 || d == 7)) g.err |= kErrRestart;
+        } else {
+            g.begin = g.end = ranges.back().second;      // a missing interval decodes from no data (flagged)
+        }
+        out.push_back(g);
+    }
+    return out;
+}
 
 struct Refuse {
     int code;
@@ -174,8 +218,165 @@ size_t scan_entropy(const uint8_t* f, size_t size, size_t pos, long long file_of
     }
 }
 
-// One file: validates it against the supported subset, fills P (and P.im's tables when non-null); throws Refuse
-void parse_file(const uint8_t* f, size_t size, long long file_off, Parsed& P) {
+// The frame's geometry into P.im at its first scan: size, sampling, MCU and block grids (tables and quantisation are latched apart)
+void frame_geometry(const Parsed& P, Image* im) {
+    const bool grey = P.ncomp == 1;
+    const int hmax = grey ? 1 : P.hs[0], vmax = grey ? 1 : P.vs[0];
+    im->w = P.w; im->h = P.h; im->ncomp = P.ncomp; im->hmax = hmax; im->vmax = vmax;
+    im->mcux = (P.w + 8 * hmax - 1) / (8 * hmax);
+    im->mcuy = (P.h + 8 * vmax - 1) / (8 * vmax);
+    im->restart = P.restart; im->orient = P.orient;
+    for (int c = 0; c < P.ncomp; ++c) {
+        Comp& cp = im->comp[c];
+        cp.h = grey ? 1 : P.hs[c];
+        cp.v = grey ? 1 : P.vs[c];
+        cp.bw = im->mcux * cp.h;
+        cp.bh = im->mcuy * cp.v;
+        cp.dw = (int)(((long long)P.w * cp.h + hmax - 1) / hmax);
+        cp.dh = (int)(((long long)P.h * cp.v + vmax - 1) / vmax);
+        cp.pitch = 8 * cp.bw;
+    }
+}
+
+// Refusals of a colour space outside the subset, made at the first scan (where libjpeg settles it)
+void check_colour(const Parsed& P, bool jfif, bool adobe, int adobe_transform) {
+    if (P.ncomp == 3 && !jfif) {
+        if (adobe && adobe_transform == 0) refuse(YFV2_EUNSUPPORTED, "RGB-coded (Adobe APP14 transform 0)");
+        if (!adobe && P.id[0] == 'R' && P.id[1] == 'G' && P.id[2] == 'B') refuse(YFV2_EUNSUPPORTED, "RGB-coded (component ids R, G, B)");
+    }
+}
+
+// Per-file state of a progressive parse: libjpeg's coef_bits (the lowest bit known of each coefficient, -1: none yet) and
+// which components have latched their quantisation table
+struct Progress {
+    int bits[3][64];
+    bool latched[3] = {};
+    Progress() { memset(bits, 0xFF, sizeof bits); }
+};
+
+// One SOS of a progressive file (payload s[n], entropy-coded data from pos): validates the scan the way libjpeg-turbo's
+// start_pass_phuff_decoder and latch_quant_tables do, builds its tables, gives it a level and cuts its segments.  Returns the
+// offset past its entropy-coded data.
+size_t prog_scan(const uint8_t* f, size_t size, size_t pos, long long file_off, const uint8_t* s, int n, Parsed& P, Progress& G,
+                 const RawHuff* hdc, const RawHuff* hac, const uint16_t (*qt)[64], const bool* qdef) {
+    const int si = (int)P.scans.size();
+    if (n < 1 || n < 4 + 2 * s[0]) refuse(YFV2_EINVAL, "short scan header");
+    const int ns = s[0];
+    if (ns < 1 || ns > P.ncomp) refuse(YFV2_EINVAL, "progressive scan %d has %d components", si, ns);
+    if (si == kMaxScans) refuse(YFV2_EUNSUPPORTED, "progressive file with more than %d scans", kMaxScans);
+    Scan sc{};
+    sc.ncomp = ns;
+    sc.ss = s[1 + 2 * ns];
+    sc.se = s[2 + 2 * ns];
+    sc.ah = s[3 + 2 * ns] >> 4;
+    sc.al = s[3 + 2 * ns] & 15;
+    sc.tab[0] = sc.tab[1] = sc.tab[2] = -1;
+    int td[3], ta[3];
+    for (int k = 0; k < ns; ++k) {
+        int c = 0;
+        while (c < P.ncomp && P.id[c] != s[1 + 2 * k]) ++c;
+        if (c == P.ncomp) refuse(YFV2_EINVAL, "progressive scan %d: component id %d is not in the frame", si, s[1 + 2 * k]);
+        if (k && c <= sc.comp[k - 1]) refuse(YFV2_EUNSUPPORTED, "progressive scan %d: components not in frame order", si);
+        sc.comp[k] = c;
+        td[k] = s[2 + 2 * k] >> 4;
+        ta[k] = s[2 + 2 * k] & 15;
+    }
+    // libjpeg's JERR_BAD_PROGRESSION: cv2 returns no image
+    const bool dc = sc.ss == 0;
+    if (dc && sc.se != 0) refuse(YFV2_EINVAL, "bad progressive scan %d: a DC scan with Se = %d", si, sc.se);
+    if (!dc && (sc.ss > sc.se || sc.se > 63)) refuse(YFV2_EINVAL, "bad progressive scan %d: coefficients %d..%d", si, sc.ss, sc.se);
+    if (!dc && ns != 1) refuse(YFV2_EINVAL, "bad progressive scan %d: an AC scan of %d components", si, ns);
+    if (sc.ah != 0 && sc.al != sc.ah - 1) refuse(YFV2_EINVAL, "bad progressive scan %d: Ah %d with Al %d", si, sc.ah, sc.al);
+    if (sc.al > 13) refuse(YFV2_EINVAL, "bad progressive scan %d: Al %d", si, sc.al);
+    // libjpeg's JWRN_BOGUS_PROGRESSION: cv2 decodes what the scans say, and this decoder does not follow it there
+    for (int k = 0; k < ns; ++k) {
+        const int c = sc.comp[k];
+        if (!dc && G.bits[c][0] < 0) refuse(YFV2_EUNSUPPORTED, "bogus progressive scan %d: AC of component %d before its DC", si, c);
+        for (int q = sc.ss; q <= sc.se; ++q) {
+            const int expect = G.bits[c][q] < 0 ? 0 : G.bits[c][q];
+            if (sc.ah != expect)
+                refuse(YFV2_EUNSUPPORTED, "bogus progressive scan %d: component %d coefficient %d has Ah %d, %d expected", si, c, q, sc.ah, expect);
+            G.bits[c][q] = sc.al;
+        }
+    }
+    // Huffman tables latched here; a DC refinement reads raw bits and needs none
+    for (int k = 0; k < prog_ntabs(sc); ++k) {
+        const int t = dc ? td[k] : ta[k];
+        const RawHuff* raw = dc ? hdc : hac;
+        if (t > 3 || !raw[t].defined) refuse(YFV2_EINVAL, "scan uses an undefined Huffman table");
+        sc.tab[k] = (int)P.huffs.size();
+        P.huffs.emplace_back();
+        build_huff(raw[t], dc, P.huffs.back());
+    }
+    // a component's quantisation table is latched at its first scan: a later DQT does not change it
+    for (int k = 0; k < ns; ++k) {
+        const int c = sc.comp[k];
+        if (G.latched[c]) continue;
+        if (!qdef[P.tq[c]]) refuse(YFV2_EINVAL, "component %d uses an undefined quantisation table", c);
+        memcpy(P.im->comp[c].q, qt[P.tq[c]], sizeof P.im->comp[c].q);
+        G.latched[c] = true;
+    }
+    for (const Scan& o : P.scans) {                   // a level above every earlier scan it shares a coefficient with
+        bool overlap = o.ss <= sc.se && sc.ss <= o.se;
+        bool shared = false;
+        for (int a = 0; a < o.ncomp; ++a)
+            for (int b = 0; b < ns; ++b) shared = shared || o.comp[a] == sc.comp[b];
+        if (overlap && shared && o.level + 1 > sc.level) sc.level = o.level + 1;
+    }
+    const Image& im = *P.im;
+    if (ns > 1) {
+        sc.upr = im.mcux;
+        sc.units = im.mcux * im.mcuy;
+    } else {
+        const Comp& cp = im.comp[sc.comp[0]];
+        sc.upr = (cp.dw + 7) / 8;
+        sc.units = sc.upr * ((cp.dh + 7) / 8);
+    }
+    if (si == 0) P.restart0 = P.restart;
+    std::vector<std::pair<long long, long long>> ranges;
+    std::vector<int> ends;
+    pos = scan_entropy(f, size, pos, file_off, ranges, ends);
+    for (const Piece& p : cut_scan(sc.units, P.restart, ranges, ends)) {
+        PSeg g{};
+        g.scan = si;
+        g.level = sc.level;
+        g.unit0 = p.u0;
+        g.nunit = p.nu;
+        g.err = p.err;
+        g.begin = p.begin;
+        g.end = p.end;
+        P.psegs.push_back(g);
+    }
+    P.scans.push_back(sc);
+    return pos;
+}
+
+// The end of a progressive file: without its EOI cv2.imdecode returns no image, so the file is flagged; with it, every coefficient
+// must have been refined to its last bit (libjpeg would smooth the blocks of an incomplete one, which is not reproduced)
+void prog_finish(Parsed& P, const Progress& G) {
+    if (!P.eoi) {
+        P.psegs[0].err |= kErrShort;
+        return;
+    }
+    for (int c = 0; c < P.ncomp; ++c)
+        for (int q = 0; q < 64; ++q) {
+            if (G.bits[c][q] < 0) refuse(YFV2_EUNSUPPORTED, "incomplete progressive file: component %d coefficient %d is never sent", c, q);
+            if (G.bits[c][q] > 0)
+                refuse(YFV2_EUNSUPPORTED, "incomplete progressive refinement: component %d coefficient %d ends at Al %d", c, q, G.bits[c][q]);
+        }
+}
+
+// One file: validates it against the supported subset, fills P (and P.im's tables when non-null); throws Refuse.  flags:
+// YFV2_JPEG_PROGRESSIVE accepts progressive (SOF2) files.
+void parse_markers(const uint8_t* f, size_t size, long long file_off, Parsed& P, int flags, Progress& G);
+
+void parse_file(const uint8_t* f, size_t size, long long file_off, Parsed& P, int flags) {
+    Progress G;
+    parse_markers(f, size, file_off, P, flags, G);
+    if (P.prog) prog_finish(P, G);
+}
+
+void parse_markers(const uint8_t* f, size_t size, long long file_off, Parsed& P, int flags, Progress& G) {
     if (size < 2 || f[0] != 0xFF || f[1] != 0xD8) {
         if (size >= 8 && memcmp(f, "\x89PNG\r\n\x1a\n", 8) == 0) refuse(YFV2_EUNSUPPORTED, "not a JPEG (a PNG file)");
         refuse(YFV2_EUNSUPPORTED, "not a JPEG (no SOI marker)");
@@ -204,6 +405,7 @@ void parse_file(const uint8_t* f, size_t size, long long file_off, Parsed& P) {
         const int m = f[pos++];
         if (m == 0xD9) {
             if (!scanned) refuse(YFV2_EINVAL, "no scan before EOI");
+            P.eoi = true;
             return;
         }
         if (m == 0x01 || (m >= 0xD0 && m <= 0xD7)) continue;   // markers without a length
@@ -219,15 +421,17 @@ void parse_file(const uint8_t* f, size_t size, long long file_off, Parsed& P) {
         const uint8_t* s = f + pos + 2;
         const int n = len - 2;
         pos += len;
-        if (scanned) {
+        if (scanned && !P.prog) {                          // a progressive file's tables and scans go on after its first scan
             if (m == 0xDA) refuse(YFV2_EUNSUPPORTED, "more than one scan");
             continue;
         }
-        if (const char* nm = sof_name(m)) refuse(YFV2_EUNSUPPORTED, "%s", nm);
+        const bool prog_sof = m == 0xC2 && (flags & YFV2_JPEG_PROGRESSIVE);
+        if (const char* nm = sof_name(m); nm && !prog_sof) refuse(YFV2_EUNSUPPORTED, "%s", nm);
         if (m == 0xCC) refuse(YFV2_EUNSUPPORTED, "arithmetic coding (DAC)");
-        if (m == 0xC0 || m == 0xC1) {
+        if (m == 0xC0 || m == 0xC1 || prog_sof) {
             if (sof) refuse(YFV2_EINVAL, "two frame headers");
             sof = true;
+            P.prog = prog_sof;
             if (n < 6) refuse(YFV2_EINVAL, "short frame header");
             if (s[0] != 8) refuse(YFV2_EUNSUPPORTED, "%d-bit samples", s[0]);
             P.h = be16(s + 1);
@@ -296,14 +500,20 @@ void parse_file(const uint8_t* f, size_t size, long long file_off, Parsed& P) {
             }
         } else if (m == 0xDA) {
             if (!sof) refuse(YFV2_EINVAL, "scan before the frame header");
+            if (P.prog) {
+                if (!scanned) {
+                    check_colour(P, jfif, adobe, adobe_transform);
+                    frame_geometry(P, P.im);
+                }
+                scanned = true;
+                pos = prog_scan(f, size, pos, file_off, s, n, P, G, hdc, hac, qt, qdef);
+                continue;
+            }
             if (n < 1) refuse(YFV2_EINVAL, "short scan header");
             const int ns = s[0];
             if (n < 4 + 2 * ns) refuse(YFV2_EINVAL, "short scan header");
             if (ns != P.ncomp) refuse(YFV2_EUNSUPPORTED, "more than one scan (this one has %d of %d components)", ns, P.ncomp);
-            if (P.ncomp == 3 && !jfif) {
-                if (adobe && adobe_transform == 0) refuse(YFV2_EUNSUPPORTED, "RGB-coded (Adobe APP14 transform 0)");
-                if (!adobe && P.id[0] == 'R' && P.id[1] == 'G' && P.id[2] == 'B') refuse(YFV2_EUNSUPPORTED, "RGB-coded (component ids R, G, B)");
-            }
+            check_colour(P, jfif, adobe, adobe_transform);
             int td[3], ta[3];
             for (int k = 0; k < ns; ++k) {
                 if (s[1 + 2 * k] != P.id[k]) refuse(YFV2_EUNSUPPORTED, "scan components not in frame order");
@@ -314,52 +524,25 @@ void parse_file(const uint8_t* f, size_t size, long long file_off, Parsed& P) {
                 if (!qdef[P.tq[k]]) refuse(YFV2_EINVAL, "component %d uses an undefined quantisation table", k);
             }
             scanned = true;
-            const bool grey = P.ncomp == 1;
-            const int hmax = grey ? 1 : P.hs[0], vmax = grey ? 1 : P.vs[0];
-            const int mcux = (P.w + 8 * hmax - 1) / (8 * hmax), mcuy = (P.h + 8 * vmax - 1) / (8 * vmax);
-            const long long mcus = (long long)mcux * mcuy;
+            Image* im = P.im;
+            frame_geometry(P, im);
             std::vector<std::pair<long long, long long>> ranges;
             std::vector<int> ends;
             pos = scan_entropy(f, size, pos, file_off, ranges, ends);
-            const long long nseg = P.restart ? (mcus + P.restart - 1) / P.restart : 1;
             P.segs.clear();
-            for (long long k = 0; k < nseg; ++k) {
+            for (const Piece& p : cut_scan((long long)im->mcux * im->mcuy, P.restart, ranges, ends)) {
                 Seg g{};
-                g.mcu0 = (int)(k * (P.restart ? P.restart : mcus));
-                g.nmcu = (int)(P.restart ? (mcus - g.mcu0 < P.restart ? mcus - g.mcu0 : P.restart) : mcus);
-                if (k < (long long)ranges.size()) {
-                    g.begin = ranges[k].first;
-                    g.end = ranges[k].second;
-                    // cv2.imdecode returns no image when the file ends inside the scan
-                    if (ends[k] < 0) g.err |= kErrShort;
-                    // The interval ends at RST(k mod 8).  libjpeg's jpeg_resync_to_restart takes a marker 1 or 2 numbers ahead
-                    // as a missing one (this interval decodes from no data) and 1 or 2 behind as a stale one (the data after it
-                    // is skipped): its intervals then hold other data than these segments.  A marker 3 to 5 away it takes as the
-                    // expected one, as the segments here do.
-                    const int d = (ends[k] - 0xD0 - (int)k) & 7;
-                    if (k + 1 < nseg && ends[k] >= 0xD0 && ends[k] <= 0xD7 && (d == 1 || d == 2 || d == 6 || d == 7)) g.err |= kErrRestart;
-                } else {
-                    g.begin = g.end = ranges.back().second;      // a missing interval decodes from no data (flagged)
-                }
+                g.mcu0 = p.u0;
+                g.nmcu = p.nu;
+                g.err = p.err;
+                g.begin = p.begin;
+                g.end = p.end;
                 P.segs.push_back(g);
             }
-            {
-                Image* im = P.im;
-                im->w = P.w; im->h = P.h; im->ncomp = P.ncomp; im->hmax = hmax; im->vmax = vmax;
-                im->mcux = mcux; im->mcuy = mcuy; im->restart = P.restart; im->orient = P.orient;
-                for (int c = 0; c < P.ncomp; ++c) {
-                    Comp& cp = im->comp[c];
-                    cp.h = grey ? 1 : P.hs[c];
-                    cp.v = grey ? 1 : P.vs[c];
-                    cp.bw = mcux * cp.h;
-                    cp.bh = mcuy * cp.v;
-                    cp.dw = (int)(((long long)P.w * cp.h + hmax - 1) / hmax);
-                    cp.dh = (int)(((long long)P.h * cp.v + vmax - 1) / vmax);
-                    cp.pitch = 8 * cp.bw;
-                    memcpy(cp.q, qt[P.tq[c]], sizeof cp.q);
-                    build_huff(hdc[td[c]], true, im->dc[c]);
-                    build_huff(hac[ta[c]], false, im->ac[c]);
-                }
+            for (int c = 0; c < P.ncomp; ++c) {
+                memcpy(im->comp[c].q, qt[P.tq[c]], sizeof im->comp[c].q);
+                build_huff(hdc[td[c]], true, im->dc[c]);
+                build_huff(hac[ta[c]], false, im->ac[c]);
             }
         }
     }
@@ -407,14 +590,44 @@ __global__ void __launch_bounds__(kColorThreads) color_kernel(const Header* hd, 
     }
 }
 
+// Progressive segment first + blockIdx.x per CTA, all of one level: the warp copies the scan's tables (up to 3 DC or 1 AC) from
+// the blob's pool into shared memory, then lane 0 decodes onto the coefficients lower levels wrote
+__global__ void __launch_bounds__(kEntropyThreads) prog_entropy_kernel(const Header* hd, const uint8_t* files, uint8_t* ws,
+                                                                       int* errors, int first) {
+    __shared__ Huff tabs[3];
+    const uint8_t* blob = reinterpret_cast<const uint8_t*>(hd);
+    const PSeg& s = reinterpret_cast<const PSeg*>(blob + hd->pseg_off)[first + blockIdx.x];
+    const Scan& sc = reinterpret_cast<const Scan*>(blob + hd->scan_off)[s.scan];
+    const Image& im = reinterpret_cast<const Image*>(blob + hd->img_off)[s.img];
+    const Huff* pool = reinterpret_cast<const Huff*>(blob + hd->huff_off);
+    constexpr int kVec = (int)sizeof(Huff) / 16;
+    const int nt = prog_ntabs(sc);
+    for (int i = threadIdx.x; i < nt * kVec; i += kEntropyThreads)
+        reinterpret_cast<uint4*>(tabs)[i] = reinterpret_cast<const uint4*>(pool + sc.tab[i / kVec])[i % kVec];
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    const int err = decode_prog_segment(im, sc, s, files, ws, tabs);
+    if (err) atomicOr(errors + s.img, err);
+}
+
 // The checks yfv2_jpeg_decode makes on a host blob before anything is launched; returns the reason or nullptr
 const char* bad_blob(const uint8_t* blob, size_t bytes, size_t files_bytes, size_t frames_bytes, size_t workspace_bytes) {
     if (bytes < sizeof(Header)) return "meta_bytes smaller than the blob header";
     const Header& hd = *reinterpret_cast<const Header*>(blob);
     if (hd.magic != kMagic) return "meta_host is not a blob yfv2_jpeg_parse wrote";
-    if ((size_t)hd.bytes != bytes || hd.n < 1 || hd.n > 65535 || hd.nseg < hd.n || hd.img_off != align16(sizeof(Header)) ||
+    if ((size_t)hd.bytes != bytes || hd.n < 1 || hd.n > 65535 || hd.nseg < 0 || hd.img_off != align16(sizeof(Header)) ||
         hd.seg_off != align16(hd.img_off + (long long)hd.n * sizeof(Image)) || hd.seg_off + (long long)hd.nseg * (long long)sizeof(Seg) > hd.bytes)
         return "inconsistent blob header (or meta_bytes is not the blob's size)";
+    if (hd.npseg == 0) {
+        if (hd.nscan || hd.nhuff || hd.nlevel || hd.prog_coef) return "inconsistent blob header (progressive arrays)";
+    } else if (hd.nscan < 1 || hd.nhuff < 0 || hd.npseg < 0 || hd.nlevel < 1 || hd.nlevel > kMaxScans ||
+               hd.scan_off != align16(hd.seg_off + (long long)hd.nseg * sizeof(Seg)) ||
+               hd.huff_off != align16(hd.scan_off + (long long)hd.nscan * sizeof(Scan)) ||
+               hd.pseg_off != align16(hd.huff_off + (long long)hd.nhuff * sizeof(Huff)) ||
+               hd.lvl_off != align16(hd.pseg_off + (long long)hd.npseg * sizeof(PSeg)) ||
+               hd.lvl_off + 4LL * (hd.nlevel + 1) != hd.bytes || hd.prog_coef < 0 || hd.prog_coef > hd.workspace) {
+        return "inconsistent blob header (progressive arrays)";
+    }
     if ((size_t)hd.files > files_bytes) return "files_bytes smaller than the files the blob was parsed from";
     if ((size_t)hd.frames > frames_bytes) return "frames_bytes smaller than the blob's frames";
     if ((size_t)hd.workspace > workspace_bytes) return "workspace_bytes smaller than the blob needs";
@@ -436,18 +649,55 @@ const char* bad_blob(const uint8_t* blob, size_t bytes, size_t files_bytes, size
     for (int k = 0; k < hd.nseg; ++k)
         if (segs[k].img < 0 || segs[k].img >= hd.n || segs[k].begin < 0 || segs[k].begin > segs[k].end || segs[k].end > hd.files)
             return "a segment outside the files";
+    if (hd.npseg == 0) return nullptr;
+    const Scan* scans = reinterpret_cast<const Scan*>(blob + hd.scan_off);
+    const PSeg* ps = reinterpret_cast<const PSeg*>(blob + hd.pseg_off);
+    const int* lvl = reinterpret_cast<const int*>(blob + hd.lvl_off);
+    if (lvl[0] != 0 || lvl[hd.nlevel] != hd.npseg) return "inconsistent level starts";
+    for (int l = 0; l < hd.nlevel; ++l)
+        if (lvl[l + 1] < lvl[l]) return "inconsistent level starts";
+    for (int k = 0; k < hd.nscan; ++k) {
+        const Scan& sc = scans[k];
+        if (sc.ncomp < 1 || sc.ncomp > 3 || sc.ss < 0 || sc.se > 63 || sc.ss > sc.se || (sc.ncomp > 1 && sc.ss != 0) || sc.al < 0 ||
+            sc.al > 13 || sc.upr < 1 || sc.units < 0)
+            return "a bad progressive scan record";
+        for (int t = 0; t < prog_ntabs(sc); ++t)
+            if (sc.tab[t] < 0 || sc.tab[t] >= hd.nhuff) return "a progressive scan's table outside the pool";
+    }
+    for (int k = 0; k < hd.npseg; ++k) {
+        const PSeg& g = ps[k];
+        if (g.img < 0 || g.img >= hd.n || g.scan < 0 || g.scan >= hd.nscan || g.begin < 0 || g.begin > g.end || g.end > hd.files)
+            return "a progressive segment outside the files";
+        if (g.level < 0 || g.level >= hd.nlevel || k < lvl[g.level] || k >= lvl[g.level + 1]) return "a progressive segment off its level";
+        const Image& im = ims[g.img];
+        const Scan& sc = scans[g.scan];
+        if (g.unit0 < 0 || g.nunit < 0 || (long long)g.unit0 + g.nunit > sc.units) return "a progressive segment outside its scan";
+        for (int q = 0; q < sc.ncomp; ++q) {
+            if (sc.comp[q] < 0 || sc.comp[q] >= im.ncomp) return "a progressive scan's component outside its image";
+            const Comp& cp = im.comp[sc.comp[q]];
+            if (cp.coef + (long long)cp.bw * cp.bh * 128 > hd.prog_coef) return "a progressive image's coefficients outside their range";
+            const bool fits = sc.ncomp > 1 ? sc.upr == im.mcux && sc.units <= (long long)im.mcux * im.mcuy &&
+                                                 cp.bw >= (long long)im.mcux * cp.h && cp.bh >= (long long)im.mcuy * cp.v
+                                           : sc.upr <= cp.bw && (sc.units + sc.upr - 1) / sc.upr <= cp.bh;
+            if (!fits) return "a progressive scan outside its component's blocks";
+        }
+    }
     return nullptr;
 }
 
 }  // namespace
 }  // namespace yfv2
 
-extern "C" int yfv2_jpeg_parse(const uint8_t* files_host, const long long* offsets_host, int N, yfv2_jpeg_info* info_host,
-                               void* meta_host, size_t meta_cap, size_t* meta_bytes, size_t* workspace_bytes, size_t* frames_bytes) {
+extern "C" int yfv2_jpeg_parse_ex(const uint8_t* files_host, const long long* offsets_host, int N, int flags, yfv2_jpeg_info* info_host,
+                                  void* meta_host, size_t meta_cap, size_t* meta_bytes, size_t* workspace_bytes, size_t* frames_bytes) {
     using namespace yfv2;
     using namespace yfv2::jpeg;
     if (!files_host || !offsets_host || !info_host || N < 1 || N > 65535) {
         set_error("jpeg_parse: null files_host / offsets_host / info_host, or N = %d outside 1..65535", N);
+        return YFV2_EINVAL;
+    }
+    if (flags & ~YFV2_JPEG_PROGRESSIVE) {
+        set_error("jpeg_parse: flags 0x%x has bits other than YFV2_JPEG_PROGRESSIVE", (unsigned)flags);
         return YFV2_EINVAL;
     }
     for (int i = 0; i < N; ++i)
@@ -458,7 +708,12 @@ extern "C" int yfv2_jpeg_parse(const uint8_t* files_host, const long long* offse
     std::vector<Image> ims(meta_host ? N : 1);          // without meta_host one scratch record: the tables are still checked
     int rc = YFV2_OK, first_bad = -1;
     long long nseg = 0, frames = 0, blocks = 0, max_blocks = 0, max_pixels = 0;
+    long long nscan = 0, nhuff = 0, npseg = 0, prog_blocks = 0;
+    int nlevel = 0;
     std::vector<std::vector<Seg>> segs(N);
+    std::vector<Scan> scans;                            // every progressive image's, in file order (when meta_host)
+    std::vector<Huff> huffs;
+    std::vector<PSeg> psegs;
     for (int i = 0; i < N; ++i) {
         yfv2_jpeg_info& inf = info_host[i];
         memset(&inf, 0, sizeof inf);
@@ -466,7 +721,7 @@ extern "C" int yfv2_jpeg_parse(const uint8_t* files_host, const long long* offse
         P.im = &ims[meta_host ? i : 0];
         memset(P.im, 0, sizeof(Image));
         try {
-            parse_file(files_host + offsets_host[i], (size_t)(offsets_host[i + 1] - offsets_host[i]), offsets_host[i], P);
+            parse_file(files_host + offsets_host[i], (size_t)(offsets_host[i + 1] - offsets_host[i]), offsets_host[i], P, flags);
         } catch (const Refuse& r) {
             inf.status = r.code;
             snprintf(inf.reason, sizeof inf.reason, "%s", r.why);
@@ -480,8 +735,9 @@ extern "C" int yfv2_jpeg_parse(const uint8_t* files_host, const long long* offse
         inf.h_samp = P.ncomp == 1 ? 1 : P.hs[0];
         inf.v_samp = P.ncomp == 1 ? 1 : P.vs[0];
         inf.orientation = P.orient;
-        inf.restart_interval = P.restart;
-        inf.segments = (int)P.segs.size();
+        inf.restart_interval = P.prog ? P.restart0 : P.restart;
+        inf.segments = (int)(P.prog ? P.psegs.size() : P.segs.size());
+        inf.scans = P.prog ? (int)P.scans.size() : 1;
         inf.frame_offset = frames;
         const int hm = inf.h_samp, vm = inf.v_samp;
         const long long mcus = (long long)((P.w + 8 * hm - 1) / (8 * hm)) * ((P.h + 8 * vm - 1) / (8 * vm));
@@ -491,12 +747,33 @@ extern "C" int yfv2_jpeg_parse(const uint8_t* files_host, const long long* offse
             im.ow = inf.w; im.oh = inf.h;
             im.frame = frames;
             im.seg0 = (int)nseg;
-            im.nseg = inf.segments;
+            im.nseg = P.prog ? 0 : inf.segments;
+            im.restart = inf.restart_interval;
             im.blocks = nb;
-            for (Seg& g : P.segs) g.img = i;
-            segs[i] = std::move(P.segs);
+            if (P.prog) {
+                for (Scan& sc : P.scans)
+                    for (int t = 0; t < prog_ntabs(sc); ++t) sc.tab[t] += (int)huffs.size();
+                for (PSeg& g : P.psegs) {
+                    g.img = i;
+                    g.scan += (int)scans.size();
+                }
+                scans.insert(scans.end(), P.scans.begin(), P.scans.end());
+                huffs.insert(huffs.end(), P.huffs.begin(), P.huffs.end());
+                psegs.insert(psegs.end(), P.psegs.begin(), P.psegs.end());
+            } else {
+                for (Seg& g : P.segs) g.img = i;
+                segs[i] = std::move(P.segs);
+            }
         }
-        nseg += inf.segments;
+        if (P.prog) {
+            nscan += (long long)P.scans.size();
+            nhuff += (long long)P.huffs.size();
+            npseg += (long long)P.psegs.size();
+            prog_blocks += nb;
+            for (const Scan& sc : P.scans) nlevel = sc.level + 1 > nlevel ? sc.level + 1 : nlevel;
+        } else {
+            nseg += inf.segments;
+        }
         blocks += nb;
         max_blocks = nb > max_blocks ? nb : max_blocks;
         max_pixels = (long long)P.w * P.h > max_pixels ? (long long)P.w * P.h : max_pixels;
@@ -506,13 +783,22 @@ extern "C" int yfv2_jpeg_parse(const uint8_t* files_host, const long long* offse
         set_error("jpeg_parse: file %d: %s", first_bad, info_host[first_bad].reason);
         return rc;
     }
-    if (nseg > INT_MAX || max_blocks > INT_MAX) {
-        set_error("jpeg_parse: %lld segments / %lld blocks in one image are too many", nseg, max_blocks);
+    if (nseg > INT_MAX || npseg > INT_MAX || nscan > INT_MAX || nhuff > INT_MAX || max_blocks > INT_MAX) {
+        set_error("jpeg_parse: %lld segments / %lld blocks in one image are too many", nseg + npseg, max_blocks);
         return YFV2_EUNSUPPORTED;
     }
+    // Header, Image[N], Seg[nseg]; with progressive images also Scan[nscan], Huff[nhuff], PSeg[npseg] and int[nlevel + 1]
     const long long img_off = align16(sizeof(Header));
     const long long seg_off = align16(img_off + (long long)N * sizeof(Image));
-    const long long bytes = seg_off + nseg * (long long)sizeof(Seg);
+    long long bytes = seg_off + nseg * (long long)sizeof(Seg);
+    long long scan_off = 0, huff_off = 0, pseg_off = 0, lvl_off = 0;
+    if (npseg) {
+        scan_off = align16(bytes);
+        huff_off = align16(scan_off + nscan * (long long)sizeof(Scan));
+        pseg_off = align16(huff_off + nhuff * (long long)sizeof(Huff));
+        lvl_off = align16(pseg_off + npseg * (long long)sizeof(PSeg));
+        bytes = lvl_off + 4LL * (nlevel + 1);
+    }
     const long long ws_bytes = blocks * (128 + 64);
     if (meta_bytes) *meta_bytes = (size_t)bytes;
     if (workspace_bytes) *workspace_bytes = (size_t)ws_bytes;
@@ -536,21 +822,47 @@ extern "C" int yfv2_jpeg_parse(const uint8_t* files_host, const long long* offse
     hd.workspace = ws_bytes;
     hd.frames = frames;
     hd.files = offsets_host[N];
-    long long coef = 0, plane = blocks * 128;                // all coefficient blocks, then all planes
+    // The progressive images' coefficient blocks first (one range the decode zeroes), then the others', then all planes
+    long long coef[2] = {0, prog_blocks * 128}, plane = blocks * 128;
     Seg* sp = reinterpret_cast<Seg*>(blob + seg_off);
+    std::vector<bool> prog(N, false);
+    for (const PSeg& g : psegs) prog[g.img] = true;
     for (int i = 0; i < N; ++i) {
         Image& im = ims[i];
         for (int c = 0; c < im.ncomp; ++c) {
             const long long nb = (long long)im.comp[c].bw * im.comp[c].bh;
-            im.comp[c].coef = coef;
+            im.comp[c].coef = coef[prog[i] ? 0 : 1];
             im.comp[c].plane = plane;
-            coef += nb * 128;
+            coef[prog[i] ? 0 : 1] += nb * 128;
             plane += nb * 64;
         }
         for (const Seg& g : segs[i]) *sp++ = g;
     }
     memcpy(blob + img_off, ims.data(), (size_t)N * sizeof(Image));
+    if (npseg) {
+        hd.nscan = (int)nscan;
+        hd.nhuff = (int)nhuff;
+        hd.npseg = (int)npseg;
+        hd.nlevel = nlevel;
+        hd.scan_off = scan_off;
+        hd.huff_off = huff_off;
+        hd.pseg_off = pseg_off;
+        hd.lvl_off = lvl_off;
+        hd.prog_coef = prog_blocks * 128;
+        std::stable_sort(psegs.begin(), psegs.end(), [](const PSeg& a, const PSeg& b) { return a.level < b.level; });
+        int* lvl = reinterpret_cast<int*>(blob + lvl_off);
+        for (const PSeg& g : psegs) ++lvl[g.level + 1];
+        for (int l = 0; l < nlevel; ++l) lvl[l + 1] += lvl[l];
+        memcpy(blob + scan_off, scans.data(), (size_t)nscan * sizeof(Scan));
+        memcpy(blob + huff_off, huffs.data(), (size_t)nhuff * sizeof(Huff));
+        memcpy(blob + pseg_off, psegs.data(), (size_t)npseg * sizeof(PSeg));
+    }
     return YFV2_OK;
+}
+
+extern "C" int yfv2_jpeg_parse(const uint8_t* files_host, const long long* offsets_host, int N, yfv2_jpeg_info* info_host,
+                               void* meta_host, size_t meta_cap, size_t* meta_bytes, size_t* workspace_bytes, size_t* frames_bytes) {
+    return yfv2_jpeg_parse_ex(files_host, offsets_host, N, 0, info_host, meta_host, meta_cap, meta_bytes, workspace_bytes, frames_bytes);
 }
 
 extern "C" int yfv2_jpeg_decode(const void* meta_host, const void* meta_dev, size_t meta_bytes, const uint8_t* files, size_t files_bytes,
@@ -577,8 +889,19 @@ extern "C" int yfv2_jpeg_decode(const void* meta_host, const void* meta_dev, siz
     uint8_t* ws = static_cast<uint8_t*>(workspace);
     if (phases & YFV2_JPEG_ENTROPY) {
         YFV2_CUDA(cudaMemsetAsync(errors, 0, sizeof(int) * hd.n, s));
-        entropy_kernel<<<hd.nseg, kEntropyThreads, 0, s>>>(dhd, files, ws, errors);
-        YFV2_LAUNCH_CHECK();
+        if (hd.nseg) {
+            entropy_kernel<<<hd.nseg, kEntropyThreads, 0, s>>>(dhd, files, ws, errors);
+            YFV2_LAUNCH_CHECK();
+        }
+        if (hd.npseg) {                                  // progressive images: zeroed once, then one launch per level
+            YFV2_CUDA(cudaMemsetAsync(ws, 0, (size_t)hd.prog_coef, s));
+            const int* lvl = reinterpret_cast<const int*>(blob + hd.lvl_off);
+            for (int l = 0; l < hd.nlevel; ++l) {
+                if (lvl[l + 1] == lvl[l]) continue;
+                prog_entropy_kernel<<<lvl[l + 1] - lvl[l], kEntropyThreads, 0, s>>>(dhd, files, ws, errors, lvl[l]);
+                YFV2_LAUNCH_CHECK();
+            }
+        }
     }
     if (phases & YFV2_JPEG_IDCT) {
         const long long gx = (hd.max_blocks + kIdctThreads - 1) / kIdctThreads;

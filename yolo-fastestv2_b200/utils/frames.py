@@ -57,22 +57,22 @@ def detect_frames(model, frames, cfg, conf_thres=0.3, iou_thres=0.4, layout="bgr
     return [to_source_pixels(r, s, cfg) for r, s in zip(rows, sizes)]
 
 
-def read_images(paths, device=None):
+def read_images(paths, device=None, progressive=False):
     """cv2.imread(path) of each JPEG file, decoded on the device (yfv2_engine.decode_jpeg): a list of CUDA uint8 [h, w, 3] BGR
-    tensors with cv2's bytes, EXIF orientation applied.  Files outside the baseline subset decode_jpeg supports (progressive, PNG,
-    BMP, ...) raise Yfv2Error naming the path; read those with cv2.imread."""
+    tensors with cv2's bytes, EXIF orientation applied.  Files outside the subset decode_jpeg supports (progressive unless
+    progressive=True, PNG, BMP, ...) raise Yfv2Error naming the path; read those with cv2.imread."""
     paths = [str(p) for p in paths]
     files = []
     for p in paths:
         with open(p, "rb") as f:
             files.append(f.read())
-    return yfv2_engine.decode_jpeg(files, device, names=paths)
+    return yfv2_engine.decode_jpeg(files, device, names=paths, progressive=progressive)
 
 
-def detect_files(model, paths, cfg, conf_thres=0.3, iou_thres=0.4):
+def detect_files(model, paths, cfg, conf_thres=0.3, iou_thres=0.4, progressive=False):
     """What test.py:34-68 computes for each image file: read_images, then detect_frames.  A list of float64 CPU [n_i, 6] tensors
-    (x1, y1, x2, y2, conf, cls) in each file's pixels, descending conf."""
-    frames = read_images(paths, next(model.parameters()).device)
+    (x1, y1, x2, y2, conf, cls) in each file's pixels, descending conf.  progressive: read progressive JPEG files too."""
+    frames = read_images(paths, next(model.parameters()).device, progressive)
     return detect_frames(model, frames, cfg, conf_thres, iou_thres)
 
 

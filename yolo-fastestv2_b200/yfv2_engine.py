@@ -137,10 +137,11 @@ class JpegInfo(ctypes.Structure):
     """yfv2_jpeg_info: what yfv2_jpeg_parse found in one file."""
     _fields_ = [("status", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int), ("components", ctypes.c_int),
                 ("h_samp", ctypes.c_int), ("v_samp", ctypes.c_int), ("orientation", ctypes.c_int), ("restart_interval", ctypes.c_int),
-                ("segments", ctypes.c_int), ("reserved", ctypes.c_int), ("frame_offset", ctypes.c_longlong), ("reason", ctypes.c_char * 96)]
+                ("segments", ctypes.c_int), ("scans", ctypes.c_int), ("frame_offset", ctypes.c_longlong), ("reason", ctypes.c_char * 96)]
 
 
 JPEG_ENTROPY, JPEG_IDCT, JPEG_COLOR, JPEG_ALL = 1, 2, 4, 7     # yfv2_jpeg_decode phases
+JPEG_PROGRESSIVE = 1                                          # yfv2_jpeg_parse_ex flags
 
 
 # name -> (restype, argtypes); must list every prototype of include/yfv2.h (tests check this)
@@ -240,6 +241,9 @@ PROTOTYPES = {
                                                 ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
     "yfv2_jpeg_parse": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
                                        ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t)]),
+    "yfv2_jpeg_parse_ex": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                                          ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t),
+                                          ctypes.POINTER(ctypes.c_size_t)]),
     "yfv2_jpeg_decode": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p,
                                         ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p]),
     "yfv2_ncnn_post": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
@@ -826,11 +830,11 @@ def _jpeg_pack(files, pin):
     return host, offsets
 
 
-def parse_jpeg(files, names=None, blob=False, pin=False):
-    """yfv2_jpeg_parse of files (bytes or uint8 numpy buffers), on the host only: (infos, blob, (workspace_bytes, frames_bytes),
+def parse_jpeg(files, names=None, blob=False, pin=False, progressive=False):
+    """yfv2_jpeg_parse_ex of files (bytes or uint8 numpy buffers), on the host only: (infos, blob, (workspace_bytes, frames_bytes),
     host buffer, offsets).  infos: one dict per file (status, w, h, components, h_samp, v_samp, orientation, restart_interval,
-    segments, frame_offset, reason).  Raises Yfv2Error naming every refused file and its reason; blob (a host uint8 tensor, pinned
-    when pin) is None unless asked for."""
+    segments, scans, frame_offset, reason).  Raises Yfv2Error naming every refused file and its reason; blob (a host uint8 tensor,
+    pinned when pin) is None unless asked for.  progressive: accept progressive files too (flags YFV2_JPEG_PROGRESSIVE)."""
     files = list(files)
     if not files:
         raise Yfv2Error("decode_jpeg: no files")
@@ -840,7 +844,9 @@ def parse_jpeg(files, names=None, blob=False, pin=False):
     meta, ws, fr = ctypes.c_size_t(), ctypes.c_size_t(), ctypes.c_size_t()
     L = lib()
     off = ctypes.c_void_p(offsets.ctypes.data)
-    rc = L.yfv2_jpeg_parse(ctypes.c_void_p(host.data_ptr()), off, N, infos, None, 0, ctypes.byref(meta), ctypes.byref(ws), ctypes.byref(fr))
+    flags = JPEG_PROGRESSIVE if progressive else 0
+    rc = L.yfv2_jpeg_parse_ex(ctypes.c_void_p(host.data_ptr()), off, N, flags, infos, None, 0, ctypes.byref(meta), ctypes.byref(ws),
+                              ctypes.byref(fr))
     if rc != 0:
         bad = ["%s: %s" % (_jpeg_name(names, i), infos[i].reason.decode("utf-8", "replace")) for i in range(N) if infos[i].status]
         if not bad:
@@ -849,9 +855,9 @@ def parse_jpeg(files, names=None, blob=False, pin=False):
     out = None
     if blob:
         out = torch.empty(meta.value, dtype=torch.uint8, pin_memory=pin)
-        _check(L.yfv2_jpeg_parse(ctypes.c_void_p(host.data_ptr()), off, N, infos, ctypes.c_void_p(out.data_ptr()), out.numel(),
-                                 ctypes.byref(meta), ctypes.byref(ws), ctypes.byref(fr)), "jpeg_parse")
-    keys = [k for k, _ in JpegInfo._fields_ if k != "reserved"]
+        _check(L.yfv2_jpeg_parse_ex(ctypes.c_void_p(host.data_ptr()), off, N, flags, infos, ctypes.c_void_p(out.data_ptr()),
+                                    out.numel(), ctypes.byref(meta), ctypes.byref(ws), ctypes.byref(fr)), "jpeg_parse")
+    keys = [k for k, _ in JpegInfo._fields_]
     dicts = [{k: (getattr(i, k).decode() if k == "reason" else getattr(i, k)) for k in keys} for i in infos]
     return dicts, out, (ws.value, fr.value), host, offsets
 
@@ -859,14 +865,15 @@ def parse_jpeg(files, names=None, blob=False, pin=False):
 class JpegBatch:
     """Files parsed on the host and copied to `device` once (one H2D copy of the packed files, one of the blob), with the workspace,
     the frame arena and the error flags allocated: decode() launches the three phases (or a subset) on the current stream without
-    synchronising, check() waits for the flags and raises on any, frames() are [h, w, 3] uint8 views into the arena."""
+    synchronising, check() waits for the flags and raises on any, frames() are [h, w, 3] uint8 views into the arena.
+    progressive: accept progressive files too (parse_jpeg)."""
 
-    def __init__(self, files, device=None, names=None):
+    def __init__(self, files, device=None, names=None, progressive=False):
         device = torch.device(device if device is not None else torch.device("cuda", torch.cuda.current_device()))
         if device.type != "cuda":
             raise Yfv2Error("decode_jpeg: runs on CUDA devices only (no CPU fallback)")
         self.device, self.names = device, names
-        self.infos, self.blob, (ws_b, fr_b), host, offsets = parse_jpeg(files, names, blob=True, pin=True)
+        self.infos, self.blob, (ws_b, fr_b), host, offsets = parse_jpeg(files, names, blob=True, pin=True, progressive=progressive)
         self.files_bytes = int(offsets[-1])
         with torch.cuda.device(device):
             self.files = host.to(device, non_blocking=True)
@@ -897,12 +904,14 @@ class JpegBatch:
         return [self.arena[i["frame_offset"]:i["frame_offset"] + 3 * i["w"] * i["h"]].view(i["h"], i["w"], 3) for i in self.infos]
 
 
-def decode_jpeg(files, device=None, names=None):
+def decode_jpeg(files, device=None, names=None, progressive=False):
     """cv2.imread of JPEG files on the device: files are bytes or uint8 numpy buffers (a file's contents); returns one CUDA uint8
     [h, w, 3] BGR tensor per file, views into one arena, bit-identical to cv2.imdecode(buf, IMREAD_COLOR) / cv2.imread (EXIF
     orientation applied).  A file outside the supported subset (include/yfv2.h) raises Yfv2Error before anything is launched,
-    naming it (names[i] when given) and why; so does a file whose entropy-coded data is cut short or corrupt, after the decode."""
-    b = JpegBatch(files, device, names)
+    naming it (names[i] when given) and why; so does a file whose entropy-coded data is cut short or corrupt, after the decode.
+    progressive: decode progressive files too (off, they are refused as outside the subset); a progressive file cut before its
+    end raises as cut short."""
+    b = JpegBatch(files, device, names, progressive)
     b.decode()
     b.check()
     return b.frames()
