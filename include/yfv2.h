@@ -362,6 +362,34 @@ YFV2_API int yfv2_jpeg_decode(const void* meta_host, const void* meta_dev, size_
                               uint8_t* frames, size_t frames_bytes, int* errors, void* workspace, size_t workspace_bytes, int phases,
                               void* stream);
 
+/* ---- anchor k-means (genanchors.py:17-102): R runs of the reference's kmeans over one box set, iteration by iteration ---------
+ * boxes: device [N][2] fp64 (w, h) as genanchors reads them from the label files.  State of run r, all device and caller-owned:
+ * centroids [R][k][2] fp64 (before the first step: the initial picks, boxes[init[r][j]]), assignments [R][N] int32 (before the
+ * first step: all -1), iterations [R] (0), status [R] (YFV2_ANCHOR_ACTIVE), changed [R] (0; every step leaves it 0).
+ * yfv2_anchor_kmeans_step runs one iteration t of every active run, bit-identical to the reference's:
+ *   similarity  IOU's four branches in its order, each a chain of individually rounded fp64 operations (no FMA);
+ *   assignment  the argmin of d = 1 - s (the first minimum, or the first NaN, as np.argmin);
+ *   stop        no assignment changed: YFV2_ANCHOR_CONVERGED, and the centroids are those iteration t used (the reference's
+ *               result after t `iter` lines); t == max_iter: YFV2_ANCHOR_NOT_CONVERGED with the centroids iteration t used;
+ *               a cluster left without members: YFV2_ANCHOR_EMPTY_CLUSTER, with the centroids and assignments of iteration t
+ *               (the reference divides 0 by 0 there and never stops);
+ *   update      otherwise centroid j = (the fp64 sum of its members' w, h, added one after another in increasing box index from
+ *               0.0) / (double)count.
+ * iterations[r] becomes t for the runs it advanced; *active (device int) receives the number of runs still active, the one value
+ * a driver reads back per iteration.  Runs that have stopped are not touched.  Nothing is allocated and nothing synchronises.
+ * yfv2_anchor_avg_iou writes avg_IOU (genanchors.py:34-40) of each run's centroids into avg_iou [R] fp64: per box Python's max
+ * over its k similarities (a first NaN stays, a later one is skipped), summed in box order from 0.0, over N.
+ * Both: N >= 1, 1 <= R <= 65535, k >= 1 and non-null pointers, max_iter >= 1, else YFV2_EINVAL; k > YFV2_ANCHOR_MAX_K:
+ * YFV2_EUNSUPPORTED; checked before anything is launched. */
+#define YFV2_ANCHOR_MAX_K          16   /* two levels x anchor_num <= 8 */
+#define YFV2_ANCHOR_ACTIVE          0
+#define YFV2_ANCHOR_CONVERGED       1
+#define YFV2_ANCHOR_EMPTY_CLUSTER   2
+#define YFV2_ANCHOR_NOT_CONVERGED   3
+YFV2_API int yfv2_anchor_kmeans_step(const double* boxes, int N, int k, int R, int max_iter, double* centroids, int* assignments,
+                                     int* iterations, int* status, int* changed, int* active, void* stream);
+YFV2_API int yfv2_anchor_avg_iou(const double* boxes, int N, int k, int R, const double* centroids, double* avg_iou, void* stream);
+
 /* ---- whole inference step with HOST buffers (the evaluation() inner loop, utils/utils.py:367-383) ----
  * x_host: pinned uint8 [N,3,H,W]; out_host: pinned [N,max_det,6]; counts_host: pinned [N].
  * Copies in, runs forward_u8 + decode_nms, copies out, all on `stream`; returns without synchronising. */

@@ -5,10 +5,12 @@ memory and streams only; every device computation is a kernel inside libyfv2.so.
 There is NO CPU fallback: if the library is missing or the tensors are not on a CUDA device the calls
 raise.
 """
+import collections
 import ctypes
 import os
 import threading
 
+import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -246,6 +248,10 @@ PROTOTYPES = {
                                           ctypes.POINTER(ctypes.c_size_t)]),
     "yfv2_jpeg_decode": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p,
                                         ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p]),
+    "yfv2_anchor_kmeans_step": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int] +
+                                [ctypes.c_void_p] * 7),
+    "yfv2_anchor_avg_iou": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                                           ctypes.c_void_p]),
     "yfv2_ncnn_post": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                       ctypes.POINTER(ctypes.c_float), ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                       ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
@@ -915,6 +921,48 @@ def decode_jpeg(files, device=None, names=None, progressive=False):
     b.decode()
     b.check()
     return b.frames()
+
+
+ANCHOR_ACTIVE, ANCHOR_CONVERGED, ANCHOR_EMPTY_CLUSTER, ANCHOR_NOT_CONVERGED = 0, 1, 2, 3     # yfv2_anchor_kmeans_step status
+KmeansResult = collections.namedtuple("KmeansResult", "centroids iterations status avg_iou assignments")
+
+
+def kmeans_anchors(dims, k, init_idx, max_iter=1000, device=None):
+    """The reference's genanchors kmeans (genanchors.py:67-102) for R runs at once on the device, bit-identical iteration by
+    iteration.  dims: float64 [N, 2] box (w, h); init_idx: [R, k] box indices, run r's initial centroids dims[init_idx[r]].
+    Returns CUDA tensors: centroids float64 [R, k, 2], iterations int32 [R], status int32 [R] (ANCHOR_CONVERGED, or
+    ANCHOR_EMPTY_CLUSTER / ANCHOR_NOT_CONVERGED where the reference would not stop), avg_iou float64 [R] (avg_IOU of the
+    centroids) and assignments int32 [R, N].  A run stopped by an empty cluster or by max_iter returns the centroids and the
+    assignments of its last iteration.  One read-back of the number of active runs per iteration is the only synchronisation."""
+    device = torch.device(device if device is not None else "cuda")
+    X = np.ascontiguousarray(dims, dtype=np.float64)
+    init = np.asarray(init_idx, dtype=np.int64)
+    if X.ndim != 2 or X.shape[1] != 2 or init.ndim != 2 or init.shape[1] != k:
+        raise Yfv2Error("kmeans_anchors: dims must be [N, 2] and init_idx [R, k=%d], got %s and %s" % (k, X.shape, init.shape))
+    N, R = X.shape[0], init.shape[0]
+    if N and init.size and (init.min() < 0 or init.max() >= N):
+        raise Yfv2Error("kmeans_anchors: init_idx holds indices outside [0, %d)" % N)
+    boxes = torch.from_numpy(X).to(device)
+    cent = torch.from_numpy(np.ascontiguousarray(X[init] if N and init.size else np.zeros((R, k, 2)))).to(device)
+    assignments = torch.full((R, N), -1, dtype=torch.int32, device=device)
+    iterations = torch.zeros(R, dtype=torch.int32, device=device)
+    status = torch.zeros(R, dtype=torch.int32, device=device)
+    changed = torch.zeros(R, dtype=torch.int32, device=device)
+    active = torch.zeros(1, dtype=torch.int32, device=device)
+    active_host = torch.zeros(1, dtype=torch.int32).pin_memory()
+    avg = torch.empty(R, dtype=torch.float64, device=device)
+    L, s = lib(), _stream(device)
+    with torch.cuda.device(device):
+        while True:
+            _check(L.yfv2_anchor_kmeans_step(boxes.data_ptr(), N, k, R, max_iter, cent.data_ptr(), assignments.data_ptr(),
+                                             iterations.data_ptr(), status.data_ptr(), changed.data_ptr(), active.data_ptr(), s),
+                   "anchor_kmeans_step")
+            active_host.copy_(active, non_blocking=True)
+            torch.cuda.current_stream(device).synchronize()
+            if active_host.item() == 0:
+                break
+        _check(L.yfv2_anchor_avg_iou(boxes.data_ptr(), N, k, R, cent.data_ptr(), avg.data_ptr(), s), "anchor_avg_iou")
+    return KmeansResult(cent, iterations, status, avg, assignments)
 
 
 YUV420_LAYOUTS = ("nv12", "nv21", "i420", "yv12")
