@@ -361,6 +361,15 @@ YFV2_API int yfv2_jpeg_parse_ex(const uint8_t* files_host, const long long* offs
 YFV2_API int yfv2_jpeg_decode(const void* meta_host, const void* meta_dev, size_t meta_bytes, const uint8_t* files, size_t files_bytes,
                               uint8_t* frames, size_t frames_bytes, int* errors, void* workspace, size_t workspace_bytes, int phases,
                               void* stream);
+/* yfv2_jpeg_decode_resize: JPEG files straight into the network input, cv2.resize(cv2.imread(f), (W, H), INTER_LINEAR) transposed
+ * to CHW (utils/datasets.py:106-110).  The same blob, files and workspace as yfv2_jpeg_decode, checked the same way before anything
+ * is launched, but no frame arena: the entropy and IDCT phases run as in yfv2_jpeg_decode, then one launch upsamples, converts,
+ * orients and resizes every image into dst [N][3][H][W] uint8 (device), 1 <= H, W <= 32768.  Image i is byte for byte
+ * yfv2_jpeg_decode's frame i followed by yfv2_resize_bgr_u8 at (W, H); errors[N] are yfv2_jpeg_decode's flags.  Nothing is
+ * allocated and nothing synchronises. */
+YFV2_API int yfv2_jpeg_decode_resize(const void* meta_host, const void* meta_dev, size_t meta_bytes, const uint8_t* files,
+                                     size_t files_bytes, int H, int W, uint8_t* dst, int* errors, void* workspace,
+                                     size_t workspace_bytes, void* stream);
 
 /* ---- anchor k-means (genanchors.py:17-102): R runs of the reference's kmeans over one box set, iteration by iteration ---------
  * boxes: device [N][2] fp64 (w, h) as genanchors reads them from the label files.  State of run r, all device and caller-owned:

@@ -8,6 +8,9 @@
 //   3. color_kernel:   one thread per output pixel, upsampling, YCbCr -> BGR and the EXIF orientation into the frame arena.
 // Progressive files (yfv2_jpeg_parse_ex with YFV2_JPEG_PROGRESSIVE) have no baseline segments: phase 1 zeroes their coefficients
 // and runs prog_entropy_kernel once per level of their scans, one thread per segment of a scan (or of one restart interval).
+// yfv2_jpeg_decode_resize runs phases 1 and 2 unchanged and replaces phase 3 by decode_resize_kernel: one thread per pixel of the
+// network input, cv2.resize(INTER_LINEAR)'s arithmetic (resize.cuh) over source pixels that bgr_pixel computes from the planes
+// where they are read, so no full-size frame is written.
 #include <algorithm>
 #include <climits>
 #include <cstddef>
@@ -17,6 +20,7 @@
 
 #include "common.cuh"
 #include "jpeg.cuh"
+#include "resize.cuh"
 
 namespace yfv2 {
 namespace {
@@ -26,6 +30,7 @@ using namespace jpeg;
 constexpr int kEntropyThreads = 32;
 constexpr int kIdctThreads = 128;
 constexpr int kColorThreads = 256;
+constexpr int kFusedBx = 64, kFusedBy = 4;   // decode_resize_kernel: resize_kernel's block
 
 // ---- host parser --------------------------------------------------------------------------------------------------------------
 struct RawHuff {
@@ -610,6 +615,48 @@ __global__ void __launch_bounds__(kEntropyThreads) prog_entropy_kernel(const Hea
     if (err) atomicOr(errors + s.img, err);
 }
 
+// The oriented frame of an image as a resize source: pixel (r, c) is computed from the workspace planes by bgr_pixel where the
+// resize reads it (phase 3 without the arena), so the full-size frame is never stored
+struct JpegFrame {
+    const Image* im;
+    const uint8_t* ws;
+};
+struct JpegSource {
+    using Desc = JpegFrame;
+    const Image& im;
+    const uint8_t* ws;
+    int r;
+    __device__ __forceinline__ JpegSource(const JpegFrame& f, int r_) : im(*f.im), ws(f.ws), r(r_) {}
+    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
+        uint8_t b0[3], b1[3];
+        bgr_pixel(im, ws, c0, r, b0);
+        bgr_pixel(im, ws, c1, r, b1);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            p0[c] = b0[c];
+            p1[c] = b1[c];
+        }
+    }
+};
+
+// yfv2_jpeg_decode_resize's phase 3: one thread per output pixel of image blockIdx.z, resize_kernel's geometry (a warp covers 32
+// consecutive x of one row), cv2.resize(INTER_LINEAR) of the oriented frame to W x H into the [n][3][H][W] batch
+__global__ void __launch_bounds__(kFusedBx * kFusedBy) decode_resize_kernel(const Header* hd, const uint8_t* ws, uint8_t* dst, int H,
+                                                                           int W) {
+    const int x = blockIdx.x * kFusedBx + threadIdx.x;
+    const int y = blockIdx.y * kFusedBy + threadIdx.y;
+    if (x >= W || y >= H) return;
+    const uint8_t* blob = reinterpret_cast<const uint8_t*>(hd);
+    const Image& im = reinterpret_cast<const Image*>(blob + hd->img_off)[blockIdx.z];
+    const JpegFrame f{&im, ws};
+    int v[3];
+    resize_pixel<JpegSource>(f, im.ow, im.oh, x, y, W, H, v);
+    const size_t plane = (size_t)H * W;
+    uint8_t* out = dst + (size_t)blockIdx.z * 3 * plane + (size_t)y * W + x;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out[c * plane] = (uint8_t)v[c];
+}
+
 // The checks yfv2_jpeg_decode makes on a host blob before anything is launched; returns the reason or nullptr
 const char* bad_blob(const uint8_t* blob, size_t bytes, size_t files_bytes, size_t frames_bytes, size_t workspace_bytes) {
     if (bytes < sizeof(Header)) return "meta_bytes smaller than the blob header";
@@ -683,6 +730,35 @@ const char* bad_blob(const uint8_t* blob, size_t bytes, size_t files_bytes, size
         }
     }
     return nullptr;
+}
+
+// Phase 1 of yfv2_jpeg_decode and yfv2_jpeg_decode_resize: the flags zeroed, the baseline segments, then the progressive images'
+// coefficients zeroed and one launch per level
+int launch_entropy(const uint8_t* blob, const Header* dhd, const uint8_t* files, uint8_t* ws, int* errors, cudaStream_t s) {
+    const Header& hd = *reinterpret_cast<const Header*>(blob);
+    YFV2_CUDA(cudaMemsetAsync(errors, 0, sizeof(int) * hd.n, s));
+    if (hd.nseg) {
+        entropy_kernel<<<hd.nseg, kEntropyThreads, 0, s>>>(dhd, files, ws, errors);
+        YFV2_LAUNCH_CHECK();
+    }
+    if (hd.npseg) {                                      // progressive images: zeroed once, then one launch per level
+        YFV2_CUDA(cudaMemsetAsync(ws, 0, (size_t)hd.prog_coef, s));
+        const int* lvl = reinterpret_cast<const int*>(blob + hd.lvl_off);
+        for (int l = 0; l < hd.nlevel; ++l) {
+            if (lvl[l + 1] == lvl[l]) continue;
+            prog_entropy_kernel<<<lvl[l + 1] - lvl[l], kEntropyThreads, 0, s>>>(dhd, files, ws, errors, lvl[l]);
+            YFV2_LAUNCH_CHECK();
+        }
+    }
+    return YFV2_OK;
+}
+
+// Phase 2: every image's blocks into its planes
+int launch_idct(const Header& hd, const Header* dhd, uint8_t* ws, cudaStream_t s) {
+    const long long gx = (hd.max_blocks + kIdctThreads - 1) / kIdctThreads;
+    idct_kernel<<<dim3((unsigned)(gx < 4096 ? gx : 4096), (unsigned)hd.n), kIdctThreads, 0, s>>>(dhd, ws);
+    YFV2_LAUNCH_CHECK();
+    return YFV2_OK;
 }
 
 }  // namespace
@@ -887,31 +963,45 @@ extern "C" int yfv2_jpeg_decode(const void* meta_host, const void* meta_dev, siz
     const Header* dhd = static_cast<const Header*>(meta_dev);
     cudaStream_t s = (cudaStream_t)stream;
     uint8_t* ws = static_cast<uint8_t*>(workspace);
-    if (phases & YFV2_JPEG_ENTROPY) {
-        YFV2_CUDA(cudaMemsetAsync(errors, 0, sizeof(int) * hd.n, s));
-        if (hd.nseg) {
-            entropy_kernel<<<hd.nseg, kEntropyThreads, 0, s>>>(dhd, files, ws, errors);
-            YFV2_LAUNCH_CHECK();
-        }
-        if (hd.npseg) {                                  // progressive images: zeroed once, then one launch per level
-            YFV2_CUDA(cudaMemsetAsync(ws, 0, (size_t)hd.prog_coef, s));
-            const int* lvl = reinterpret_cast<const int*>(blob + hd.lvl_off);
-            for (int l = 0; l < hd.nlevel; ++l) {
-                if (lvl[l + 1] == lvl[l]) continue;
-                prog_entropy_kernel<<<lvl[l + 1] - lvl[l], kEntropyThreads, 0, s>>>(dhd, files, ws, errors, lvl[l]);
-                YFV2_LAUNCH_CHECK();
-            }
-        }
-    }
-    if (phases & YFV2_JPEG_IDCT) {
-        const long long gx = (hd.max_blocks + kIdctThreads - 1) / kIdctThreads;
-        idct_kernel<<<dim3((unsigned)(gx < 4096 ? gx : 4096), (unsigned)hd.n), kIdctThreads, 0, s>>>(dhd, ws);
-        YFV2_LAUNCH_CHECK();
-    }
+    if (phases & YFV2_JPEG_ENTROPY)
+        if (const int rc = launch_entropy(blob, dhd, files, ws, errors, s)) return rc;
+    if (phases & YFV2_JPEG_IDCT)
+        if (const int rc = launch_idct(hd, dhd, ws, s)) return rc;
     if (phases & YFV2_JPEG_COLOR) {
         const long long gx = (hd.max_pixels + kColorThreads - 1) / kColorThreads;
         color_kernel<<<dim3((unsigned)(gx < 8192 ? gx : 8192), (unsigned)hd.n), kColorThreads, 0, s>>>(dhd, ws, frames);
         YFV2_LAUNCH_CHECK();
     }
+    return YFV2_OK;
+}
+
+extern "C" int yfv2_jpeg_decode_resize(const void* meta_host, const void* meta_dev, size_t meta_bytes, const uint8_t* files,
+                                       size_t files_bytes, int H, int W, uint8_t* dst, int* errors, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+    using namespace yfv2;
+    using namespace yfv2::jpeg;
+    if (!meta_host || !meta_dev || !files || !dst || !errors || !workspace) {
+        set_error("jpeg_decode_resize: null meta_host / meta_dev / files / dst / errors / workspace");
+        return YFV2_EINVAL;
+    }
+    if (H <= 0 || W <= 0 || H > kMaxSide || W > kMaxSide) {
+        set_error("jpeg_decode_resize: target %dx%d outside 1..%d", W, H, kMaxSide);
+        return YFV2_EINVAL;
+    }
+    const uint8_t* blob = static_cast<const uint8_t*>(meta_host);
+    // no frame arena: the blob's frame offsets are not used, so any arena size passes
+    if (const char* why = bad_blob(blob, meta_bytes, files_bytes, SIZE_MAX, workspace_bytes)) {
+        set_error("jpeg_decode_resize: %s", why);
+        return YFV2_EINVAL;
+    }
+    const Header& hd = *reinterpret_cast<const Header*>(blob);
+    const Header* dhd = static_cast<const Header*>(meta_dev);
+    cudaStream_t s = (cudaStream_t)stream;
+    uint8_t* ws = static_cast<uint8_t*>(workspace);
+    if (const int rc = launch_entropy(blob, dhd, files, ws, errors, s)) return rc;
+    if (const int rc = launch_idct(hd, dhd, ws, s)) return rc;
+    const dim3 grid((unsigned)((W + kFusedBx - 1) / kFusedBx), (unsigned)((H + kFusedBy - 1) / kFusedBy), (unsigned)hd.n);
+    decode_resize_kernel<<<grid, dim3(kFusedBx, kFusedBy), 0, s>>>(dhd, ws, dst, H, W);
+    YFV2_LAUNCH_CHECK();
     return YFV2_OK;
 }

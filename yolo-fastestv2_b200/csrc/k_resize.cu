@@ -22,9 +22,11 @@
 // round trip, and the call needs no workspace.
 // aug_resize_kernel (yfv2_aug_batch, k_aug.cu) runs random_resize as the second resize over a fetch that computes the pixels of
 // the first from the planar source where they are read (DESIGN.md §9).
+// The per-pixel arithmetic is in resize.cuh, shared with the fused JPEG decode + resize (k_jpeg.cu).
 #include <climits>
 
 #include "aug.cuh"
+#include "resize.cuh"
 
 namespace yfv2 {
 namespace {
@@ -72,8 +74,6 @@ struct StridedSource {
         }
     }
 };
-
-__device__ __forceinline__ int sat_u8(int v) { return min(max(v, 0), 255); }
 
 // cv2.cvtColor's YUV -> BGR of one pixel, 4:2:0 and 4:2:2 alike (OpenCV ITUR_BT_601: 20-bit fixed point, limited range)
 __device__ __forceinline__ void yuv_to_bgr(int y, int uu, int vv, int (&bgr)[3]) {
@@ -136,17 +136,6 @@ struct ResizeChunk {
     int H, W;
 };
 
-// fractional source coordinate of target index d: returns the fraction, s = its floor
-__device__ __forceinline__ float src_coord(int d, int n, int m, int& s) {
-    const double scale = (double)n / (double)m;                                          // IEEE division
-    const float f = __double2float_rn(__dadd_rn(__dmul_rn((double)d + 0.5, scale), -0.5));   // no FMA contraction
-    const float fl = floorf(f);
-    s = (int)fl;
-    return __fsub_rn(f, fl);
-}
-__device__ __forceinline__ int weight0(float f) { return __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f)); }
-__device__ __forceinline__ int weight1(float f) { return __float2int_rn(__fmul_rn(f, 2048.f)); }
-
 // Src::kMinBlocks 8 holds a fetch to 32 registers (the strided fetch's three row pointers take 34 unbounded), so an SM keeps its
 // full 2048 threads in flight: the kernel waits on DRAM, not on issue.  BGR and 4:2:0 use 32 registers unbounded (0: no bound).
 template <class Src>
@@ -182,34 +171,6 @@ resize_kernel(const __grid_constant__ ResizeChunk<Src> a) {
         const int S1 = p10[c] * a0 + p11[c] * a1;
         const int v = ((((S0 >> 4) * b0) >> 16) + (((S1 >> 4) * b1) >> 16) + 2) >> 2;
         out[c * plane] = (uint8_t)sat_u8(v);
-    }
-}
-
-// Output pixel (x, y) of the resize of fr (w x h source pixels) to W x H: B, G, R in v.  resize_kernel's arithmetic, for the
-// augmentation's nested resize (resize_kernel keeps its own copy of these lines so that its code stays as it was).
-template <class Src>
-__device__ __forceinline__ void resize_pixel(const typename Src::Desc& fr, int w, int h, int x, int y, int W, int H, int (&v)[3]) {
-    int sx;
-    float fx = src_coord(x, w, W, sx);
-    if (sx < 0) { fx = 0.f; sx = 0; }
-    if (sx >= w - 1) { fx = 0.f; sx = w - 1; }
-    const int a0 = weight0(fx), a1 = weight1(fx);
-    const int x1 = min(sx + 1, w - 1);
-
-    int sy;
-    const float fy = src_coord(y, h, H, sy);
-    const int b0 = weight0(fy), b1 = weight1(fy);
-    const int r0 = min(max(sy, 0), h - 1), r1 = min(max(sy + 1, 0), h - 1);
-
-    const Src row0(fr, r0), row1(fr, r1);
-    int p00[3], p01[3], p10[3], p11[3];          // [row][column] source pixels, B G R
-    row0.fetch(sx, x1, p00, p01);
-    row1.fetch(sx, x1, p10, p11);
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        const int S0 = p00[c] * a0 + p01[c] * a1;
-        const int S1 = p10[c] * a0 + p11[c] * a1;
-        v[c] = sat_u8(((((S0 >> 4) * b0) >> 16) + (((S1 >> 4) * b1) >> 16) + 2) >> 2);
     }
 }
 

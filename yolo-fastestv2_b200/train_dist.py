@@ -15,6 +15,10 @@ What changes is the hot path: model.detector.Detector / utils.loss.compute_loss 
 one flat 243 095-float bucket and every optimizer step issues exactly ONE all-reduce over NCCL (mean over ranks), then the
 reference's SGD.  BatchNorm statistics stay per rank (the reference has no SyncBN).
 
+`--device-decode` (with `--device-aug`) reads the train and validation lists through utils.device_data instead: the loader
+workers read the files and parse the JPEG headers, and each batch is decoded and resized into the network input on the GPU, the
+same bytes as TensorDataset(imgaug=False) (DESIGN.md §13).
+
 `--synthetic N` replaces the dataset by N seeded synthetic images with SURVEY 8(d) config[2] box statistics (no dataset and
 no reference checkout needed: used by the GPU tests and the 8-GPU measurement)."""
 import argparse
@@ -75,7 +79,14 @@ def main(argv=None):
     ap.add_argument("--device-aug-resize", action="store_true", help="with --device-aug: add random_resize (utils/datasets.py:54-61)")
     ap.add_argument("--device-aug-hsv", action="store_true", help="with --device-aug: add augment_hsv (utils/datasets.py:39-51)")
     ap.add_argument("--device-aug-blur", action="store_true", help="with --device-aug: add motion_blur (utils/datasets.py:18-37)")
+    ap.add_argument("--device-decode", action="store_true", help="read the train and validation images with utils.device_data: JPEG "
+                                                                 "decode and resize to the network input on the GPU (needs --device-aug)")
     opt = ap.parse_args(argv)
+    if opt.device_decode and not opt.device_aug:
+        ap.error("--device-decode needs --device-aug: the device loader does not run contrast_and_brightness, which "
+                 "TensorDataset(imgaug=True) applies to training images")
+    if opt.device_decode and opt.synthetic:
+        ap.error("--device-decode reads cfg['train'] and cfg['val']; it does not combine with --synthetic")
     if (opt.device_aug_resize or opt.device_aug_hsv or opt.device_aug_blur) and not opt.device_aug:
         ap.error("--device-aug-resize, --device-aug-hsv and --device-aug-blur need --device-aug")
 
@@ -98,21 +109,31 @@ def main(argv=None):
 
     batch_size = int(cfg["batch_size"] / cfg["subdivisions"])                     # per rank, as train.py:37
     nw = min([os.cpu_count(), batch_size if batch_size > 1 else 0, 8])
-    if opt.synthetic:
-        train_dataset = SyntheticDetection(opt.synthetic, cfg["width"], cfg["height"], cfg["classes"])
-        val_dataset, cf = None, collate_fn
+    if opt.device_decode:                                                         # utils/device_data.py: files decoded on the GPU
+        import utils.device_data
+        train_dataloader = utils.device_data.device_loader(cfg["train"], cfg["width"], cfg["height"], batch_size, device,
+                                                           num_workers=nw, train=True, world=world, rank=rank)
+        sampler = train_dataloader.sampler
+        val_dataloader = None
+        if rank == 0:
+            val_dataloader = utils.device_data.device_loader(cfg["val"], cfg["width"], cfg["height"], batch_size, device,
+                                                             num_workers=nw)
     else:
-        import utils.datasets                                                     # the reference's (not on the hot path)
-        train_dataset = utils.datasets.TensorDataset(cfg["train"], cfg["width"], cfg["height"], imgaug=not opt.device_aug)
-        val_dataset = utils.datasets.TensorDataset(cfg["val"], cfg["width"], cfg["height"], imgaug=False)
-        cf = utils.datasets.collate_fn
-    sampler = DistributedSampler(train_dataset, num_replicas=world, rank=rank, shuffle=True, drop_last=True)
-    train_dataloader = DataLoader(train_dataset, batch_size=batch_size, sampler=sampler, collate_fn=cf, num_workers=nw,
-                                  pin_memory=True, drop_last=True, persistent_workers=nw > 0)
-    val_dataloader = None
-    if val_dataset is not None and rank == 0:
-        val_dataloader = DataLoader(val_dataset, batch_size=batch_size, shuffle=False, collate_fn=cf, num_workers=nw,
-                                    pin_memory=True, drop_last=False, persistent_workers=nw > 0)
+        if opt.synthetic:
+            train_dataset = SyntheticDetection(opt.synthetic, cfg["width"], cfg["height"], cfg["classes"])
+            val_dataset, cf = None, collate_fn
+        else:
+            import utils.datasets                                                     # the reference's (not on the hot path)
+            train_dataset = utils.datasets.TensorDataset(cfg["train"], cfg["width"], cfg["height"], imgaug=not opt.device_aug)
+            val_dataset = utils.datasets.TensorDataset(cfg["val"], cfg["width"], cfg["height"], imgaug=False)
+            cf = utils.datasets.collate_fn
+        sampler = DistributedSampler(train_dataset, num_replicas=world, rank=rank, shuffle=True, drop_last=True)
+        train_dataloader = DataLoader(train_dataset, batch_size=batch_size, sampler=sampler, collate_fn=cf, num_workers=nw,
+                                      pin_memory=True, drop_last=True, persistent_workers=nw > 0)
+        val_dataloader = None
+        if val_dataset is not None and rank == 0:
+            val_dataloader = DataLoader(val_dataset, batch_size=batch_size, shuffle=False, collate_fn=cf, num_workers=nw,
+                                        pin_memory=True, drop_last=False, persistent_workers=nw > 0)
 
     load_param = bool(cfg["pre_weights"]) and os.path.exists(cfg["pre_weights"])
     torch.manual_seed(0)                                                          # identical initial weights on every rank

@@ -71,9 +71,24 @@ def read_images(paths, device=None, progressive=False):
 
 def detect_files(model, paths, cfg, conf_thres=0.3, iou_thres=0.4, progressive=False):
     """What test.py:34-68 computes for each image file: read_images, then detect_frames.  A list of float64 CPU [n_i, 6] tensors
-    (x1, y1, x2, y2, conf, cls) in each file's pixels, descending conf.  progressive: read progressive JPEG files too."""
-    frames = read_images(paths, next(model.parameters()).device, progressive)
-    return detect_frames(model, frames, cfg, conf_thres, iou_thres)
+    (x1, y1, x2, y2, conf, cls) in each file's pixels, descending conf.  progressive: read progressive JPEG files too.  The files
+    are decoded straight into the network input (JpegBatch.decode_resize: the bytes of read_images + resize_bgr, without the
+    full-size frames); they are refused, and raise, as read_images refuses them."""
+    paths = [str(p) for p in paths]
+    files = []
+    for p in paths:
+        with open(p, "rb") as f:
+            files.append(f.read())
+    dev = next(model.parameters()).device
+    W, H = int(cfg["width"]), int(cfg["height"])
+    b = yfv2_engine.JpegBatch(files, dev, names=paths, progressive=progressive)
+    x = torch.empty((len(files), 3, H, W), dtype=torch.uint8, device=dev)
+    b.decode_resize(x, W, H)
+    b.check()
+    with torch.no_grad():
+        preds = model(x)
+    rows = detect(preds, cfg, conf_thres, iou_thres)
+    return [to_source_pixels(r, (i["h"], i["w"]), cfg) for r, i in zip(rows, b.infos)]
 
 
 def _axis_tiles(n, k, overlap, even):

@@ -248,6 +248,9 @@ PROTOTYPES = {
                                           ctypes.POINTER(ctypes.c_size_t)]),
     "yfv2_jpeg_decode": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p,
                                         ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p]),
+    "yfv2_jpeg_decode_resize": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t,
+                                               ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                               ctypes.c_size_t, ctypes.c_void_p]),
     "yfv2_anchor_kmeans_step": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int] +
                                 [ctypes.c_void_p] * 7),
     "yfv2_anchor_avg_iou": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
@@ -836,11 +839,13 @@ def _jpeg_pack(files, pin):
     return host, offsets
 
 
-def parse_jpeg(files, names=None, blob=False, pin=False, progressive=False):
+def parse_jpeg(files, names=None, blob=False, pin=False, progressive=False, strict=True):
     """yfv2_jpeg_parse_ex of files (bytes or uint8 numpy buffers), on the host only: (infos, blob, (workspace_bytes, frames_bytes),
     host buffer, offsets).  infos: one dict per file (status, w, h, components, h_samp, v_samp, orientation, restart_interval,
     segments, scans, frame_offset, reason).  Raises Yfv2Error naming every refused file and its reason; blob (a host uint8 tensor,
-    pinned when pin) is None unless asked for.  progressive: accept progressive files too (flags YFV2_JPEG_PROGRESSIVE)."""
+    pinned when pin) is None unless asked for.  progressive: accept progressive files too (flags YFV2_JPEG_PROGRESSIVE).
+    strict=False: a batch with refused files returns instead of raising, with every file's status and reason in infos, blob None
+    and sizes (0, 0); parse the accepted files again to decode them.  Makes no CUDA call unless pin."""
     files = list(files)
     if not files:
         raise Yfv2Error("decode_jpeg: no files")
@@ -853,61 +858,96 @@ def parse_jpeg(files, names=None, blob=False, pin=False, progressive=False):
     flags = JPEG_PROGRESSIVE if progressive else 0
     rc = L.yfv2_jpeg_parse_ex(ctypes.c_void_p(host.data_ptr()), off, N, flags, infos, None, 0, ctypes.byref(meta), ctypes.byref(ws),
                               ctypes.byref(fr))
+    keys = [k for k, _ in JpegInfo._fields_]
     if rc != 0:
         bad = ["%s: %s" % (_jpeg_name(names, i), infos[i].reason.decode("utf-8", "replace")) for i in range(N) if infos[i].status]
         if not bad:
             _check(rc, "jpeg_parse")
+        if not strict:
+            dicts = [{k: (getattr(i, k).decode("utf-8", "replace") if k == "reason" else getattr(i, k)) for k in keys} for i in infos]
+            return dicts, None, (0, 0), host, offsets
         raise Yfv2Error("decode_jpeg: %d of %d files refused: %s" % (len(bad), N, "; ".join(bad)))
     out = None
     if blob:
         out = torch.empty(meta.value, dtype=torch.uint8, pin_memory=pin)
         _check(L.yfv2_jpeg_parse_ex(ctypes.c_void_p(host.data_ptr()), off, N, flags, infos, ctypes.c_void_p(out.data_ptr()),
                                     out.numel(), ctypes.byref(meta), ctypes.byref(ws), ctypes.byref(fr)), "jpeg_parse")
-    keys = [k for k, _ in JpegInfo._fields_]
     dicts = [{k: (getattr(i, k).decode() if k == "reason" else getattr(i, k)) for k in keys} for i in infos]
     return dicts, out, (ws.value, fr.value), host, offsets
 
 
 class JpegBatch:
-    """Files parsed on the host and copied to `device` once (one H2D copy of the packed files, one of the blob), with the workspace,
-    the frame arena and the error flags allocated: decode() launches the three phases (or a subset) on the current stream without
-    synchronising, check() waits for the flags and raises on any, frames() are [h, w, 3] uint8 views into the arena.
-    progressive: accept progressive files too (parse_jpeg)."""
+    """Files parsed on the host and copied to `device` once (one H2D copy of the packed files, one of the blob), with the workspace
+    and the error flags allocated: decode() launches the three phases (or a subset) on the current stream without synchronising,
+    check() waits for the flags and raises on any, frames() are [h, w, 3] uint8 views into the arena (allocated by the first
+    decode()).  decode_resize(out, W, H) decodes straight into a [N, 3, H, W] network input instead, with no arena.
+    progressive: accept progressive files too (parse_jpeg).  parsed: the result of parse_jpeg(files, blob=True, ...) made
+    elsewhere (another process, say), used instead of parsing `files` (which may then be None)."""
 
-    def __init__(self, files, device=None, names=None, progressive=False):
+    def __init__(self, files, device=None, names=None, progressive=False, parsed=None):
         device = torch.device(device if device is not None else torch.device("cuda", torch.cuda.current_device()))
         if device.type != "cuda":
             raise Yfv2Error("decode_jpeg: runs on CUDA devices only (no CPU fallback)")
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
         self.device, self.names = device, names
-        self.infos, self.blob, (ws_b, fr_b), host, offsets = parse_jpeg(files, names, blob=True, pin=True, progressive=progressive)
+        if parsed is None:
+            parsed = parse_jpeg(files, names, blob=True, pin=True, progressive=progressive)
+        self.infos, self.blob, (ws_b, fr_b), host, offsets = parsed
+        if self.blob is None:
+            raise Yfv2Error("decode_jpeg: the parse result has no blob (parse_jpeg(..., blob=True) of accepted files)")
         self.files_bytes = int(offsets[-1])
         with torch.cuda.device(device):
             self.files = host.to(device, non_blocking=True)
             self.meta = self.blob.to(device, non_blocking=True)
             self.workspace = torch.empty(max(ws_b, 1), dtype=torch.uint8, device=device)
-            self.arena = torch.empty(max(fr_b, 1), dtype=torch.uint8, device=device)
             self.errors = torch.zeros(len(self.infos), dtype=torch.int32, device=device)
+        self.arena = None
         self._host = host                                # the pinned source of the asynchronous copy
         self._sizes = (ws_b, fr_b)
 
     def decode(self, phases=JPEG_ALL):
         p = lambda t: ctypes.c_void_p(t.data_ptr())     # noqa: E731
         with torch.cuda.device(self.device):
+            if self.arena is None:
+                self.arena = torch.empty(max(self._sizes[1], 1), dtype=torch.uint8, device=self.device)
             _check(lib().yfv2_jpeg_decode(p(self.blob), p(self.meta), self.blob.numel(), p(self.files), self.files_bytes, p(self.arena),
                                           self._sizes[1], p(self.errors), p(self.workspace), self._sizes[0], phases,
                                           _stream(self.device)), "jpeg_decode")
 
+    def decode_resize(self, out, W, H):
+        """Every file as cv2.resize(cv2.imread(f), (W, H), INTER_LINEAR) transposed to CHW, into out (a contiguous CUDA uint8
+        [N, 3, H, W] tensor on the batch's device), on the current stream without synchronising; the flags as decode() sets them."""
+        N = len(self.infos)
+        if (not isinstance(out, torch.Tensor) or tuple(out.shape) != (N, 3, H, W) or out.dtype != torch.uint8 or not out.is_contiguous()
+                or out.device != self.device):
+            raise Yfv2Error("decode_resize_jpeg: out must be a contiguous uint8 tensor of shape %s on %s" % ((N, 3, H, W), self.device))
+        p = lambda t: ctypes.c_void_p(t.data_ptr())     # noqa: E731
+        with torch.cuda.device(self.device):
+            _check(lib().yfv2_jpeg_decode_resize(p(self.blob), p(self.meta), self.blob.numel(), p(self.files), self.files_bytes, int(H),
+                                                 int(W), p(out), p(self.errors), p(self.workspace), self._sizes[0],
+                                                 _stream(self.device)), "jpeg_decode_resize")
+        return out
+
+    def flags(self):
+        """The per-file flag words of the last decode (waits for it)."""
+        return self.errors.cpu().tolist()
+
     def check(self):
-        errs = self.errors.cpu().tolist()
+        errs = self.flags()
         bad = [(i, e) for i, e in enumerate(errs) if e]
         if bad:
-            what = ("entropy-coded data ran out (truncated or corrupt)", "invalid Huffman code", "restart markers out of sequence")
-            why = lambda e: ", ".join(w for b, w in enumerate(what) if e >> b & 1) or "error %d" % e  # noqa: E731
             raise Yfv2Error("decode_jpeg: %d of %d files failed to decode: %s" % (
-                len(bad), len(errs), "; ".join("%s: %s" % (_jpeg_name(self.names, i), why(e)) for i, e in bad)))
+                len(bad), len(errs), "; ".join("%s: %s" % (_jpeg_name(self.names, i), jpeg_flag_reason(e)) for i, e in bad)))
 
     def frames(self):
         return [self.arena[i["frame_offset"]:i["frame_offset"] + 3 * i["w"] * i["h"]].view(i["h"], i["w"], 3) for i in self.infos]
+
+
+def jpeg_flag_reason(e):
+    """What a yfv2_jpeg_decode flag word says, in words."""
+    what = ("entropy-coded data ran out (truncated or corrupt)", "invalid Huffman code", "restart markers out of sequence")
+    return ", ".join(w for b, w in enumerate(what) if e >> b & 1) or "error %d" % e
 
 
 def decode_jpeg(files, device=None, names=None, progressive=False):
@@ -921,6 +961,19 @@ def decode_jpeg(files, device=None, names=None, progressive=False):
     b.decode()
     b.check()
     return b.frames()
+
+
+def decode_resize_jpeg(files, W, H, device=None, names=None, progressive=False, out=None):
+    """cv2.resize(cv2.imread(f), (W, H), interpolation=cv2.INTER_LINEAR) of JPEG files, transposed to the [N, 3, H, W] uint8 batch
+    the network takes, in one call (yfv2_jpeg_decode_resize): bit-identical to resize_bgr(decode_jpeg(files), W, H), without the
+    full-size frames.  Refuses and raises as decode_jpeg does; out: a contiguous CUDA uint8 [N, 3, H, W] tensor to write into."""
+    b = JpegBatch(files, device, names, progressive)
+    N = len(b.infos)
+    if out is None:
+        out = torch.empty((N, 3, H, W), dtype=torch.uint8, device=b.device)
+    b.decode_resize(out, W, H)
+    b.check()
+    return out
 
 
 ANCHOR_ACTIVE, ANCHOR_CONVERGED, ANCHOR_EMPTY_CLUSTER, ANCHOR_NOT_CONVERGED = 0, 1, 2, 3     # yfv2_anchor_kmeans_step status
