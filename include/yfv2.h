@@ -429,7 +429,13 @@ YFV2_API int yfv2_loss_read_targets(const void* workspace, int level, int N, int
  *   conv1x1:  y[n][m][p] = sum_k w[m][k] x[n][k][p] (+bias);  bwd outputs are optional (NULL to skip).
  *   dwconv:   depthwise ks x ks (3|5), stride 1|2, pad ks/2.   stem: dense 3x3 s2 p1 with 3 input channels.
  *   bn_train: batch statistics over (N, HW), running-stat update (momentum 0.1, unbiased var), optional fused ReLU;
- *             scratch = 2*C doubles; save_mean / save_invstd feed the backward.
+ *             scratch = 2*C doubles; save_mean / save_invstd feed the backward.  bwd: dgamma / dbeta may be NULL (not written;
+ *             the sums dx needs are still taken), as autograd skips the gradient of a BatchNorm affine with requires_grad=False.
+ *   bn_eval:  a BatchNorm module in .eval() inside a train-mode network (F.batch_norm with training=False, eps 1e-5):
+ *             y = [ReLU]((x - running_mean) * (running_var + eps)^-1/2 * gamma + beta); the running statistics are read, never
+ *             updated.  fwd writes the mean / invstd it used to save_mean / save_invstd.  bwd: dx = g * gamma * invstd,
+ *             dgamma = sum(g * xhat), dbeta = sum(g) (g = dy masked by y > 0 under ReLU; no batch-mean terms, the statistics
+ *             are constants); each of dx, dgamma, dbeta may be NULL, not all three; scratch (2*C doubles) only with dgamma or dbeta.
  *   maxpool:  3x3 s2 p1 with argmax indices;  upsample2: nearest x2. */
 YFV2_API int yfv2_op_conv1x1_fwd(const float* x, const float* w, const float* bias, float* y, int N, int K, int M, int HW, void* stream);
 YFV2_API int yfv2_op_conv1x1_bwd(const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias, int N, int K, int M,
@@ -444,6 +450,11 @@ YFV2_API int yfv2_op_bn_train_fwd(const float* x, const float* gamma, const floa
 YFV2_API int yfv2_op_bn_train_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean,
                                   const float* save_invstd, float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW,
                                   int relu, void* stream);
+YFV2_API int yfv2_op_bn_eval_fwd(const float* x, const float* gamma, const float* beta, const float* running_mean, const float* running_var,
+                                 float* y, float* save_mean, float* save_invstd, int N, int C, int HW, int relu, void* stream);
+YFV2_API int yfv2_op_bn_eval_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean,
+                                 const float* save_invstd, float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW,
+                                 int relu, void* stream);
 YFV2_API int yfv2_op_maxpool_fwd(const float* x, float* y, int* idx, int planes, int H, int W, void* stream);
 YFV2_API int yfv2_op_maxpool_bwd(const float* dy, const int* idx, float* dx, int planes, int H, int W, void* stream);
 YFV2_API int yfv2_op_upsample2_fwd(const float* x, float* y, int planes, int H, int W, void* stream);
@@ -459,13 +470,25 @@ YFV2_API int yfv2_op_upsample2_bwd(const float* dy, float* dx, int planes, int H
  *   dpreds[6]: d(loss)/d(preds) (e.g. from yfv2_compute_loss).  grads_flat: ONE buffer of yfv2_trainer_grad_floats() floats holding
  *     every parameter's gradient at yfv2_trainer_param_offset(i) in parameter order (the bucket a data-parallel step all-reduces);
  *     accumulate != 0 adds to it (gradient accumulation over sub-batches, train.py:122-124), 0 overwrites.
- * yfv2_train_backward must follow the yfv2_train_forward of the same batch on the same workspace (and stream order). */
+ * yfv2_train_backward must follow the yfv2_train_forward of the same batch on the same workspace (and stream order).
+ *
+ * Fine-tuning mode (yfv2_trainer_set_mode; default: every parameter trainable, every BatchNorm layer in train mode):
+ *   trainable[YFV2_NUM_PARAMS] (NULL: all 1): 0 for a parameter with requires_grad=False.  As autograd: it receives no gradient,
+ *     and an op's backward runs only if its output depends on a trainable parameter (the image does not), writing d(input) only
+ *     for an input that does; the backward below the lowest trainable layer is not run at all.
+ *   bn_eval[YFV2_NUM_BN] (NULL: all 0): 1 for a BatchNorm module in .eval() (e.g. after model.backbone.eval()): it normalises with
+ *     the running statistics and leaves them alone, as bn_eval above; its gamma / beta may still be trainable.
+ *   The mode takes effect at the next yfv2_train_forward.  yfv2_train_backward refuses, before any launch, a mode changed since
+ *   that forward and a mode with no trainable parameter (torch: "element 0 of tensors does not require grad").
+ *   yfv2_trainer_grad_floats / yfv2_trainer_param_offset report the current mode's flat layout: the trainable parameters only,
+ *   in parameter order (train_ddp.FlatGradBucket's layout); offset -1 for a frozen parameter. */
 typedef struct yfv2_trainer yfv2_trainer;
 YFV2_API int yfv2_trainer_create(yfv2_trainer** out, int device, int N, int H, int W, int A, int C);
 YFV2_API void yfv2_trainer_destroy(yfv2_trainer* t);
 YFV2_API int yfv2_trainer_workspace_bytes(const yfv2_trainer* t, size_t* bytes);
 YFV2_API int yfv2_trainer_grad_floats(const yfv2_trainer* t, long long* n);
 YFV2_API int yfv2_trainer_param_offset(const yfv2_trainer* t, int index, long long* offset, long long* numel);
+YFV2_API int yfv2_trainer_set_mode(yfv2_trainer* t, const unsigned char* trainable, const unsigned char* bn_eval);
 YFV2_API int yfv2_train_forward(yfv2_trainer* t, const float* x, const float* const* params, float* const* bn_running,
                                 float* const preds[6], void* workspace, void* stream);
 YFV2_API int yfv2_train_backward(yfv2_trainer* t, const float* x, const float* const* params, float* const preds[6],
@@ -519,6 +542,15 @@ typedef struct yfv2_trainer_tensor {
 YFV2_API int yfv2_trainer_debug_ops(const yfv2_trainer* t, yfv2_trainer_op* ops_host, int cap, int* n);
 YFV2_API int yfv2_trainer_debug_tensors(const yfv2_trainer* t, yfv2_trainer_tensor* tens_host, int cap, int* n);
 YFV2_API int yfv2_trainer_debug_layout(const yfv2_trainer* t, long long* layout_host);
+/* Host only, for the current mode: the ops whose backward runs, in the order it runs them (op = index into yfv2_trainer_debug_ops),
+ * and which outputs each writes: da / db the gradient of input a / b, dw, dbias, dgamma, dbeta the parameter gradients; bn_eval 1
+ * for a BatchNorm run by the eval-mode kernels.  (A train-mode BatchNorm with da = 0 still computes a dx nobody reads, into its
+ * input's own gradient slot.)  Writes min(cap, count) records, the count in *n. */
+typedef struct yfv2_trainer_bwd_op {
+    int op;
+    int da, db, dw, dbias, dgamma, dbeta, bn_eval;
+} yfv2_trainer_bwd_op;
+YFV2_API int yfv2_trainer_debug_backward(const yfv2_trainer* t, yfv2_trainer_bwd_op* ops_host, int cap, int* n);
 
 /* ---- test hook: the kernel launches of a whole forward, as the forward itself chooses them ----------------------------------
  * Host only: nothing is launched and workspace is not dereferenced; its address decides the kernels that need 16-byte-aligned

@@ -701,9 +701,54 @@ bn_bwd_apply_kernel(const float* __restrict__ x, const float* __restrict__ y, co
         }
     }
     if (pl < C && blockIdx.y == 0 && threadIdx.x == 0) {      // planes 0..C-1 are image 0's channels: one writer per channel
-        dgamma[c] = (float)sums[2 * c + 1];
-        dbeta[c] = (float)sums[2 * c];
+        if (dgamma) dgamma[c] = (float)sums[2 * c + 1];
+        if (dbeta) dbeta[c] = (float)sums[2 * c];
     }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// BatchNorm (eval mode inside a train-mode network: nn.BatchNorm2d.eval(), the frozen-statistics fine-tuning recipe)
+// ---------------------------------------------------------------------------------------------------------------------
+// mean = running_mean, invstd = (running_var + eps)^-1/2: what F.batch_norm(training=False) normalises with.  The forward then
+// runs bn_apply_kernel and the backward reads the same two vectors, so both see one rounding of invstd.
+__global__ void bn_eval_stats_kernel(const float* __restrict__ running_mean, const float* __restrict__ running_var,
+                                     float* __restrict__ mean, float* __restrict__ invstd, int C) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    mean[c] = running_mean[c];
+    invstd[c] = 1.f / sqrtf(running_var[c] + kBnEps);
+}
+
+// dx = g * gamma * invstd (g: dy masked by y > 0 under a fused ReLU); no batch-mean terms, the statistics are constants.
+// grid (N*C planes, chunks of 1024 pixels), four pixels per thread as bn_apply_kernel
+__global__ void __launch_bounds__(256)
+bn_eval_bwd_apply_kernel(const float* __restrict__ y, const float* __restrict__ dy, const float* __restrict__ invstd,
+                         const float* __restrict__ gamma, float* __restrict__ dx, int C, int HW, int relu) {
+    const long long pl = blockIdx.x;
+    const int c = (int)(pl % C);
+    const float s = __ldg(gamma + c) * __ldg(invstd + c);
+    const long long base = pl * HW;
+    const int p0 = blockIdx.y * 1024 + threadIdx.x * 4;
+    auto f = [&](float d, float yv) { return (relu && yv <= 0.f ? 0.f : d) * s; };      // threshold_backward: a NaN y passes dy
+    if ((HW & 3) == 0 && ((reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0) {
+        if (p0 < HW) {
+            const float4 d = __ldg(reinterpret_cast<const float4*>(dy + base + p0));
+            const float4 v = relu ? __ldg(reinterpret_cast<const float4*>(y + base + p0)) : make_float4(1.f, 1.f, 1.f, 1.f);
+            *reinterpret_cast<float4*>(dx + base + p0) = make_float4(f(d.x, v.x), f(d.y, v.y), f(d.z, v.z), f(d.w, v.w));
+        }
+    } else {
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+            if (p0 + q < HW) dx[base + p0 + q] = f(__ldg(dy + base + p0 + q), relu ? __ldg(y + base + p0 + q) : 1.f);
+    }
+}
+
+// dgamma = sum(g * xhat), dbeta = sum(g) from bn_bwd_reduce_kernel's fp64 sums; either pointer may be null
+__global__ void bn_affine_grads_kernel(const double* __restrict__ sums, float* __restrict__ dgamma, float* __restrict__ dbeta, int C) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    if (dgamma) dgamma[c] = (float)sums[2 * c + 1];
+    if (dbeta) dbeta[c] = (float)sums[2 * c];
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -758,6 +803,13 @@ __global__ void upsample2_bwd_kernel(const float* __restrict__ dy, float* __rest
 }
 
 int grid_for(long long total) { long long b = (total + 255) / 256; return (int)(b < 1 ? 1 : (b > 148 * 32 ? 148 * 32 : b)); }
+// image slices of the per-channel reductions: about 16 pixels per thread, at most 64 slices and one image per slice
+int bn_slices(int N, int HW) {
+    const long long per = (long long)N * HW;
+    int slices = (int)((per + 256 * 16 - 1) / (256 * 16));
+    slices = slices < 1 ? 1 : (slices > 64 ? 64 : slices);
+    return slices > N ? N : slices;
+}
 
 }  // namespace
 }  // namespace yfv2
@@ -910,7 +962,7 @@ extern "C" YFV2_API int yfv2_op_bn_train_fwd(const float* x, const float* gamma,
 extern "C" YFV2_API int yfv2_op_bn_train_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean,
                                              const float* save_invstd, float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW,
                                              int relu, void* stream) {
-    ARGCHK(x && y && dy && gamma && save_mean && save_invstd && dx && dgamma && dbeta && scratch, "bn_train_bwd: bad arguments");
+    ARGCHK(x && y && dy && gamma && save_mean && save_invstd && dx && scratch, "bn_train_bwd: bad arguments");      // dgamma / dbeta: NULL skips
     cudaStream_t s = (cudaStream_t)stream;
     YFV2_CUDA(cudaMemsetAsync(scratch, 0, (size_t)2 * C * sizeof(double), s));
     const long long per = (long long)N * HW;
@@ -922,6 +974,42 @@ extern "C" YFV2_API int yfv2_op_bn_train_bwd(const float* x, const float* y, con
     bn_bwd_apply_kernel<<<dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)), 256, 0, s>>>(x, y, dy, save_mean, save_invstd, gamma, scratch, dx,
                                                                                                dgamma, dbeta, C, HW, (double)per, relu);
     YFV2_LAUNCH_CHECK();
+    return YFV2_OK;
+}
+
+// Eval-mode BatchNorm: y = [ReLU]((x - running_mean) * (running_var + eps)^-1/2 * gamma + beta).  The running statistics are read,
+// never written; save_mean / save_invstd receive what the forward normalised with (they feed yfv2_op_bn_eval_bwd).
+extern "C" YFV2_API int yfv2_op_bn_eval_fwd(const float* x, const float* gamma, const float* beta, const float* running_mean,
+                                            const float* running_var, float* y, float* save_mean, float* save_invstd, int N, int C, int HW,
+                                            int relu, void* stream) {
+    ARGCHK(x && gamma && beta && running_mean && running_var && y && save_mean && save_invstd && N > 0 && C > 0 && HW > 0,
+           "bn_eval_fwd: bad arguments");
+    cudaStream_t s = (cudaStream_t)stream;
+    bn_eval_stats_kernel<<<(C + 127) / 128, 128, 0, s>>>(running_mean, running_var, save_mean, save_invstd, C);
+    YFV2_LAUNCH_CHECK();
+    bn_apply_kernel<<<dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)), 256, 0, s>>>(x, save_mean, save_invstd, gamma, beta, y, C, HW, relu);
+    YFV2_LAUNCH_CHECK();
+    return YFV2_OK;
+}
+// dx = g * gamma * invstd, dgamma = sum(g * xhat), dbeta = sum(g) (g: dy masked by y > 0 under ReLU).  Each of dx, dgamma, dbeta
+// may be NULL (skipped), not all three; scratch (2*C doubles) is needed only with dgamma or dbeta.
+extern "C" YFV2_API int yfv2_op_bn_eval_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean,
+                                            const float* save_invstd, float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW,
+                                            int relu, void* stream) {
+    ARGCHK(x && y && dy && gamma && save_mean && save_invstd && N > 0 && C > 0 && HW > 0 && (dx || dgamma || dbeta) &&
+           (scratch || !(dgamma || dbeta)), "bn_eval_bwd: bad arguments");
+    cudaStream_t s = (cudaStream_t)stream;
+    if (dgamma || dbeta) {
+        YFV2_CUDA(cudaMemsetAsync(scratch, 0, (size_t)2 * C * sizeof(double), s));
+        bn_bwd_reduce_kernel<<<dim3(C, bn_slices(N, HW)), 256, 0, s>>>(x, y, dy, save_mean, save_invstd, scratch, N, C, HW, relu);
+        YFV2_LAUNCH_CHECK();
+        bn_affine_grads_kernel<<<(C + 127) / 128, 128, 0, s>>>(scratch, dgamma, dbeta, C);
+        YFV2_LAUNCH_CHECK();
+    }
+    if (dx) {
+        bn_eval_bwd_apply_kernel<<<dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)), 256, 0, s>>>(y, dy, save_invstd, gamma, dx, C, HW, relu);
+        YFV2_LAUNCH_CHECK();
+    }
     return YFV2_OK;
 }
 

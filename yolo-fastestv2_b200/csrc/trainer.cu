@@ -16,6 +16,14 @@
 //     scratch tensor; the shared output convolutions (used at both pyramid levels) accumulate their weight gradients the same way.
 // The arithmetic is the training operators of k_train.cu (yfv2_op_*).  Gradients of all 225 parameters leave in ONE flat buffer in
 // parameter order (the bucket train_ddp.py all-reduces), either assigned or accumulated.
+//
+// Fine-tuning mode (yfv2_trainer_set_mode): what autograd does for parameters with requires_grad=False and BatchNorm modules in
+// .eval() inside a train-mode model.  The static program stays; the mode only selects, per op, the kernels and outputs:
+//   * rg(tensor): the tensor depends on a trainable parameter.  rg(image) = false, rg(y) = rg(a) | rg(b) | (the op owns a trainable
+//     parameter).  An op's backward runs iff rg(y); it writes d(a) iff rg(a) and a parameter gradient iff that parameter is trainable.
+//     Every consumer of an rg tensor has an rg output, so the first-consumer-assigns rule above holds unchanged;
+//   * an eval-mode BatchNorm normalises with the running statistics, leaves them alone and has no batch-mean terms in its backward;
+//   * the flat buffer holds the trainable parameters only, in parameter order (train_ddp.FlatGradBucket's layout).
 #include <algorithm>
 #include <cstdlib>
 #include <new>
@@ -47,6 +55,9 @@ struct Op {
 
 struct CB { int w, g, b, bn; };      // conv weight + its BatchNorm (gamma, beta, layer index)
 
+// what one op's backward does under the current mode (yfv2_trainer_debug_backward)
+struct BwdOp { bool run, da, db, dw, dbias, dgamma, dbeta, bn_eval; };
+
 }  // namespace
 }  // namespace yfv2
 
@@ -61,6 +72,12 @@ struct yfv2_trainer {
     long long gflat_off = 0, scratch_off = 0, pscratch_off = 0, wscratch_off = 0, pscratch_floats = 0;
     int x_ten = -1;
     int out_ten[6];
+    // fine-tuning mode: the current one, and the one the last forward ran under (a backward must see the same)
+    std::vector<unsigned char> trainable, bn_eval, fwd_trainable, fwd_bn_eval;
+    std::vector<yfv2::BwdOp> bwd;        // per op, from the current mode
+    std::vector<long long> coff;         // offset of every parameter's gradient in the caller's flat buffer; -1: frozen
+    long long ctotal = 0;
+    unsigned long long mode_hash = 0;
     // CUDA-graph replay of the two static programs (~1000 launches per step otherwise: the step is host-bound at 8 GPUs): a
     // program is captured on a private stream the first time a set of pointers is seen and replayed while they stay the same
     struct GraphSlot { cudaGraphExec_t exec = nullptr; unsigned long long key = 0; };
@@ -244,6 +261,31 @@ void build(yfv2_trainer& t) {
     t.wscratch_off = b.alloc(kWScratchFloats);
 }
 
+// The per-op backward plan and the flat layout of the current mode (host only)
+void apply_mode(yfv2_trainer& t) {
+    std::vector<char> rg(t.tens.size(), 0);
+    t.bwd.assign(t.ops.size(), BwdOp{});
+    auto tr = [&](int p) { return p >= 0 && t.trainable[p] != 0; };
+    for (size_t i = 0; i < t.ops.size(); ++i) {
+        const Op& o = t.ops[i];
+        BwdOp& b = t.bwd[i];
+        const bool ra = rg[o.a] != 0, rb = o.b >= 0 && rg[o.b] != 0;
+        b.dw = tr(o.pw); b.dbias = tr(o.pbias); b.dgamma = tr(o.pg); b.dbeta = tr(o.pb);
+        b.run = ra || rb || b.dw || b.dbias || b.dgamma || b.dbeta;
+        b.da = b.run && ra; b.db = b.run && rb;
+        b.bn_eval = o.kind == K_BN && t.bn_eval[o.bn] != 0;
+        rg[o.y] = b.run ? 1 : 0;
+    }
+    t.coff.assign(t.poff.size(), -1);
+    t.ctotal = 0;
+    for (size_t i = 0; i < t.poff.size(); ++i)
+        if (t.trainable[i]) { t.coff[i] = t.ctotal; t.ctotal += t.pnumel[i]; }
+    unsigned long long h = 1469598103934665603ull;                  // FNV-1a over both masks
+    for (unsigned char v : t.trainable) h = (h ^ v) * 1099511628211ull;
+    for (unsigned char v : t.bn_eval) h = (h ^ (unsigned)(v + 2)) * 1099511628211ull;
+    t.mode_hash = h;
+}
+
 // dst[n][doff + c*dstep][p] (+)= src[n][soff + c*sstep][p],  c < count
 __global__ void chan_copy_kernel(const float* __restrict__ src, int Cs, int soff, int sstep, float* __restrict__ dst, int Cd, int doff, int dstep,
                                  int count, int HW, long long total, int accumulate) {
@@ -296,6 +338,9 @@ int yfv2_op_stem_wgrad(const float*, const float*, float*, int, int, int, int, v
 int yfv2_op_bn_train_fwd(const float*, const float*, const float*, float*, float*, float*, float*, float*, double*, int, int, int, int, void*);
 int yfv2_op_bn_train_bwd(const float*, const float*, const float*, const float*, const float*, const float*, float*, float*, float*, double*,
                          int, int, int, int, void*);
+int yfv2_op_bn_eval_fwd(const float*, const float*, const float*, const float*, const float*, float*, float*, float*, int, int, int, int, void*);
+int yfv2_op_bn_eval_bwd(const float*, const float*, const float*, const float*, const float*, const float*, float*, float*, float*, double*,
+                        int, int, int, int, void*);
 int yfv2_op_maxpool_fwd(const float*, float*, int*, int, int, int, void*);
 int yfv2_op_maxpool_bwd(const float*, const int*, float*, int, int, int, void*);
 int yfv2_op_upsample2_fwd(const float*, float*, int, int, int, void*);
@@ -320,6 +365,10 @@ extern "C" int yfv2_trainer_create(yfv2_trainer** out, int device, int N, int H,
         delete t;
         return YFV2_EINVAL;
     }
+    t->trainable.assign(YFV2_NUM_PARAMS, 1);
+    t->bn_eval.assign(YFV2_NUM_BN, 0);
+    t->fwd_trainable = t->trainable; t->fwd_bn_eval = t->bn_eval;
+    apply_mode(*t);
     *out = t;
     return YFV2_OK;
 }
@@ -337,12 +386,38 @@ extern "C" int yfv2_trainer_workspace_bytes(const yfv2_trainer* t, size_t* bytes
 }
 extern "C" int yfv2_trainer_grad_floats(const yfv2_trainer* t, long long* n) {
     if (!t || !n) { set_error("trainer_grad_floats: null argument"); return YFV2_EINVAL; }
-    *n = t->ptotal;
+    *n = t->ctotal;
     return YFV2_OK;
 }
 extern "C" int yfv2_trainer_param_offset(const yfv2_trainer* t, int index, long long* offset, long long* numel) {
     if (!t || index < 0 || index >= (int)t->poff.size() || !offset || !numel) { set_error("trainer_param_offset: bad argument"); return YFV2_EINVAL; }
-    *offset = t->poff[index]; *numel = t->pnumel[index];
+    *offset = t->coff[index]; *numel = t->pnumel[index];
+    return YFV2_OK;
+}
+extern "C" int yfv2_trainer_set_mode(yfv2_trainer* t, const unsigned char* trainable, const unsigned char* bn_eval) {
+    if (!t) { set_error("trainer_set_mode: null trainer"); return YFV2_EINVAL; }
+    for (int i = 0; trainable && i < YFV2_NUM_PARAMS; ++i)
+        if (trainable[i] > 1) { set_error("trainer_set_mode: trainable[%d] = %d is not 0 or 1", i, trainable[i]); return YFV2_EINVAL; }
+    for (int i = 0; bn_eval && i < YFV2_NUM_BN; ++i)
+        if (bn_eval[i] > 1) { set_error("trainer_set_mode: bn_eval[%d] = %d is not 0 or 1", i, bn_eval[i]); return YFV2_EINVAL; }
+    for (int i = 0; i < YFV2_NUM_PARAMS; ++i) t->trainable[i] = trainable ? trainable[i] : 1;
+    for (int i = 0; i < YFV2_NUM_BN; ++i) t->bn_eval[i] = bn_eval ? bn_eval[i] : 0;
+    apply_mode(*t);
+    return YFV2_OK;
+}
+extern "C" int yfv2_trainer_debug_backward(const yfv2_trainer* t, yfv2_trainer_bwd_op* ops_host, int cap, int* n) {
+    if (!t || !n || cap < 0 || (cap > 0 && !ops_host)) { set_error("trainer_debug_backward: bad argument"); return YFV2_EINVAL; }
+    int k = 0;
+    for (int oi = (int)t->ops.size() - 1; oi >= 0; --oi) {      // backward order
+        const BwdOp& b = t->bwd[oi];
+        if (!b.run) continue;
+        if (k < cap) {
+            yfv2_trainer_bwd_op& d = ops_host[k];
+            d.op = oi; d.da = b.da; d.db = b.db; d.dw = b.dw; d.dbias = b.dbias; d.dgamma = b.dgamma; d.dbeta = b.dbeta; d.bn_eval = b.bn_eval;
+        }
+        ++k;
+    }
+    *n = k;
     return YFV2_OK;
 }
 
@@ -404,8 +479,12 @@ static int run_forward(yfv2_trainer* t, const float* x, const float* const* para
         case K_BN: {
             double* scr = reinterpret_cast<double*>(P.ws + o.aux);
             float* mean = P.ws + o.aux + 4LL * A.C;
-            TRYT(yfv2_op_bn_train_fwd(a, params[o.pg], params[o.pb], bn_running[2 * o.bn], bn_running[2 * o.bn + 1], y, mean, mean + A.C, scr,
-                                      N, A.C, A.H * A.W, o.relu, s));
+            if (t->bn_eval[o.bn])
+                TRYT(yfv2_op_bn_eval_fwd(a, params[o.pg], params[o.pb], bn_running[2 * o.bn], bn_running[2 * o.bn + 1], y, mean, mean + A.C,
+                                         N, A.C, A.H * A.W, o.relu, s));
+            else
+                TRYT(yfv2_op_bn_train_fwd(a, params[o.pg], params[o.pb], bn_running[2 * o.bn], bn_running[2 * o.bn + 1], y, mean, mean + A.C, scr,
+                                          N, A.C, A.H * A.W, o.relu, s));
         } break;
         case K_POOL: TRYT(yfv2_op_maxpool_fwd(a, y, reinterpret_cast<int*>(P.ws + o.aux), N * A.C, A.H, A.W, s)); break;
         case K_PW: TRYT(yfv2_op_conv1x1_fwd(a, params[o.pw], o.pbias >= 0 ? params[o.pbias] : nullptr, y, N, A.C, o.M, A.H * A.W, s)); break;
@@ -444,18 +523,20 @@ static int run_backward(yfv2_trainer* t, const float* x, const float* const* par
     };
     for (int oi = (int)t->ops.size() - 1; oi >= 0; --oi) {
         const Op& o = t->ops[oi];
+        const BwdOp& bo = t->bwd[oi];
+        if (!bo.run) continue;                      // no trainable parameter upstream of its output
         const Ten& A = t->tens[o.a];
         const Ten& Y = t->tens[o.y];
         const float* a = P.act(*t, o.a);
         const float* dy = P.grad(*t, o.y);
         // gradient of input a: assigned by the consumer that runs first in the backward (the last one in the forward), accumulated
-        // through the scratch tensor by the others; inputs that need no gradient (the image) get none
-        const bool need_da = A.ext == -1;
+        // through the scratch tensor by the others; inputs that need no gradient (the image, frozen bottoms of the network) get none
+        const bool need_da = bo.da;
         const bool acc_a = need_da && !A.partial && A.last_use != oi;
         float* da = !need_da ? nullptr : (acc_a ? scratch : P.gradw(*t, o.a));
         const long long an = (long long)N * A.C * A.H * A.W;
         switch (o.kind) {
-        case K_STEM: {
+        case K_STEM: {                              // runs only for a trainable stem weight (the image needs no gradient)
             bool via; float* dw = ptarget(o.pw, &via);
             TRYT(yfv2_op_stem_wgrad(a, dy, dw, N, Y.C, A.H, A.W, s));
             TRYT(pcommit(o.pw, via));
@@ -463,56 +544,77 @@ static int run_backward(yfv2_trainer* t, const float* x, const float* const* par
         case K_BN: {
             double* scr = reinterpret_cast<double*>(P.ws + o.aux);
             const float* mean = P.ws + o.aux + 4LL * A.C;
-            bool vg, vb; float* dg = ptarget(o.pg, &vg);
             // gamma and beta of one layer are never shared, so both go straight to their slots
-            float* db = G + t->poff[o.pb]; vb = false;
-            TRYT(yfv2_op_bn_train_bwd(a, P.act(*t, o.y), dy, params[o.pg], mean, mean + A.C, da, dg, db, scr, N, A.C, A.H * A.W, o.relu, s));
-            TRYT(pcommit(o.pg, vg)); TRYT(pcommit(o.pb, vb));
+            float* dg = bo.dgamma ? G + t->poff[o.pg] : nullptr;
+            float* db = bo.dbeta ? G + t->poff[o.pb] : nullptr;
+            if (bo.bn_eval) {
+                TRYT(yfv2_op_bn_eval_bwd(a, P.act(*t, o.y), dy, params[o.pg], mean, mean + A.C, da, dg, db, scr, N, A.C, A.H * A.W, o.relu, s));
+            } else {
+                // the batch-statistics backward needs the sums for its gamma / beta anyway; without rg(a) its dx goes to a's own
+                // gradient slot, which nothing reads (a's producer does not run)
+                TRYT(yfv2_op_bn_train_bwd(a, P.act(*t, o.y), dy, params[o.pg], mean, mean + A.C, da ? da : P.gradw(*t, o.a), dg, db, scr,
+                                          N, A.C, A.H * A.W, o.relu, s));
+            }
+            if (dg) pwritten[o.pg] = 1;
+            if (db) pwritten[o.pb] = 1;
         } break;
         case K_POOL: TRYT(yfv2_op_maxpool_bwd(dy, reinterpret_cast<const int*>(P.ws + o.aux), da, N * A.C, A.H, A.W, s)); break;
         case K_PW: {
-            bool vw, vb = false; float* dw = ptarget(o.pw, &vw);
+            bool vw = false, vb = false;
+            float* dw = bo.dw ? ptarget(o.pw, &vw) : nullptr;
             float* db = nullptr;
-            if (o.pbias >= 0) db = vw ? pscratch + t->pnumel[o.pw] : G + t->poff[o.pbias];      // bias rides behind the weight in the scratch
+            if (bo.dbias) { vb = pwritten[o.pbias] != 0; db = vb ? pscratch + t->pnumel[o.pw] : G + t->poff[o.pbias]; }  // bias rides behind the weight in the scratch
             TRYT(conv1x1_bwd_impl(a, params[o.pw], dy, da, dw, db, N, A.C, o.M, A.H * A.W, P.ws + t->wscratch_off, (size_t)kWScratchFloats, s));
-            if (o.pbias >= 0 && vw) { TRYT(axpy(pscratch + t->pnumel[o.pw], G + t->poff[o.pbias], t->pnumel[o.pbias], 1, s)); }
-            TRYT(pcommit(o.pw, vw));
-            if (o.pbias >= 0) pwritten[o.pbias] = 1;
-            (void)vb;
+            if (vb) { TRYT(axpy(pscratch + t->pnumel[o.pw], G + t->poff[o.pbias], t->pnumel[o.pbias], 1, s)); }
+            if (dw) TRYT(pcommit(o.pw, vw));
+            if (db) pwritten[o.pbias] = 1;
         } break;
         case K_DW: {
-            bool vw; float* dw = ptarget(o.pw, &vw);
+            bool vw = false; float* dw = bo.dw ? ptarget(o.pw, &vw) : nullptr;
             TRYT(yfv2_op_dwconv_bwd(a, params[o.pw], dy, da, dw, N, A.C, A.H, A.W, o.ks, o.stride, s));
-            TRYT(pcommit(o.pw, vw));
+            if (dw) TRYT(pcommit(o.pw, vw));
         } break;
         case K_UP: TRYT(yfv2_op_upsample2_bwd(dy, da, N * A.C, A.H, A.W, s)); break;
         case K_ODD: TRYT(chan_copy(dy, Y.C, 0, 1, P.gradw(*t, o.a), A.C, 1, 2, Y.C, N, A.H * A.W, 0, s)); break;          // odd half of d(a)
         case K_CATE: {
             const Ten& B = t->tens[o.b];
-            TRYT(chan_copy(dy, Y.C, 0, 1, P.gradw(*t, o.a), A.C, 0, 2, A.C / 2, N, A.H * A.W, 0, s));                       // even half of d(a)
-            TRYT(chan_copy(dy, Y.C, A.C / 2, 1, P.gradw(*t, o.b), B.C, 0, 1, B.C, N, A.H * A.W, 0, s));
+            if (bo.da) TRYT(chan_copy(dy, Y.C, 0, 1, P.gradw(*t, o.a), A.C, 0, 2, A.C / 2, N, A.H * A.W, 0, s));              // even half of d(a)
+            if (bo.db) TRYT(chan_copy(dy, Y.C, A.C / 2, 1, P.gradw(*t, o.b), B.C, 0, 1, B.C, N, A.H * A.W, 0, s));
         } break;
         case K_CAT2: {
             const Ten& B = t->tens[o.b];
             const bool acc_b = B.last_use != oi;
-            TRYT(chan_copy(dy, Y.C, 0, 1, P.gradw(*t, o.a), A.C, 0, 1, A.C, N, Y.H * Y.W, acc_a ? 1 : 0, s));
-            TRYT(chan_copy(dy, Y.C, A.C, 1, P.gradw(*t, o.b), B.C, 0, 1, B.C, N, Y.H * Y.W, acc_b ? 1 : 0, s));
+            if (bo.da) TRYT(chan_copy(dy, Y.C, 0, 1, P.gradw(*t, o.a), A.C, 0, 1, A.C, N, Y.H * Y.W, acc_a ? 1 : 0, s));
+            if (bo.db) TRYT(chan_copy(dy, Y.C, A.C, 1, P.gradw(*t, o.b), B.C, 0, 1, B.C, N, Y.H * Y.W, acc_b ? 1 : 0, s));
         } break;
         default: set_error("train_backward: unknown op"); return YFV2_EINVAL;
         }
         if (acc_a && o.kind != K_CAT2 && o.kind != K_ODD && o.kind != K_CATE) { TRYT(axpy(scratch, P.gradw(*t, o.a), an, 1, s)); }
     }
     for (size_t i = 0; i < pwritten.size(); ++i)
-        if (!pwritten[i]) { set_error("train_backward: parameter %d received no gradient (internal)", (int)i); return YFV2_EINVAL; }
-    TRYT(axpy(G, grads_flat, t->ptotal, accumulate ? 1 : 0, s));
+        if ((pwritten[i] != 0) != (t->trainable[i] != 0)) {
+            set_error("train_backward: parameter %d %s a gradient (internal)", (int)i, pwritten[i] ? "frozen but received" : "received no");
+            return YFV2_EINVAL;
+        }
+    // the trainable parameters' slots, packed in parameter order: one copy per run of consecutive trainable parameters (all
+    // trainable: one copy of the whole slot)
+    for (size_t i = 0; i < t->poff.size();) {
+        if (!t->trainable[i]) { ++i; continue; }
+        size_t j = i;
+        long long n = 0;
+        while (j < t->poff.size() && t->trainable[j]) n += t->pnumel[j++];
+        TRYT(axpy(G + t->poff[i], grads_flat + t->coff[i], n, accumulate ? 1 : 0, s));
+        i = j;
+    }
     return YFV2_OK;
 }
 
 namespace {
-unsigned long long mix(unsigned long long h, const void* p) {
-    h ^= (unsigned long long)reinterpret_cast<uintptr_t>(p) + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2);
+unsigned long long mix(unsigned long long h, unsigned long long v) {
+    h ^= v + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2);
     return h;
 }
+unsigned long long mix(unsigned long long h, const void* p) { return mix(h, (unsigned long long)reinterpret_cast<uintptr_t>(p)); }
 // Replays `slot` if it was captured for `key`; otherwise captures body() on the trainer's private stream, instantiates and replays.
 template <class Body>
 int replay_or_capture(yfv2_trainer* t, yfv2_trainer::GraphSlot& slot, unsigned long long key, cudaStream_t s, Body&& body) {
@@ -543,12 +645,18 @@ extern "C" int yfv2_train_forward(yfv2_trainer* t, const float* x, const float* 
     for (int i = 0; i < 2 * YFV2_NUM_BN; ++i) if (!bn_running[i]) { set_error("train_forward: null BN buffer %d", i); return YFV2_EINVAL; }
     cudaStream_t s = (cudaStream_t)stream;
     static const bool no_graph = getenv("YFV2_TRAIN_NOGRAPH") != nullptr;
-    if (no_graph || !t->use_graphs) return run_forward(t, x, params, bn_running, preds, workspace, s);
-    unsigned long long key = mix(mix(0x1234ull, x), workspace);
-    for (int i = 0; i < YFV2_NUM_PARAMS; ++i) key = mix(key, params[i]);
-    for (int i = 0; i < 2 * YFV2_NUM_BN; ++i) key = mix(key, bn_running[i]);
-    for (int i = 0; i < 6; ++i) key = mix(key, preds[i]);
-    return replay_or_capture(t, t->g_fwd, key, s, [&](cudaStream_t cs) { return run_forward(t, x, params, bn_running, preds, workspace, cs); });
+    int rc;
+    if (no_graph || !t->use_graphs) {
+        rc = run_forward(t, x, params, bn_running, preds, workspace, s);
+    } else {
+        unsigned long long key = mix(mix(mix(0x1234ull, t->mode_hash), x), workspace);
+        for (int i = 0; i < YFV2_NUM_PARAMS; ++i) key = mix(key, params[i]);
+        for (int i = 0; i < 2 * YFV2_NUM_BN; ++i) key = mix(key, bn_running[i]);
+        for (int i = 0; i < 6; ++i) key = mix(key, preds[i]);
+        rc = replay_or_capture(t, t->g_fwd, key, s, [&](cudaStream_t cs) { return run_forward(t, x, params, bn_running, preds, workspace, cs); });
+    }
+    if (rc == YFV2_OK) { t->fwd_trainable = t->trainable; t->fwd_bn_eval = t->bn_eval; }
+    return rc;
 }
 
 extern "C" int yfv2_train_backward(yfv2_trainer* t, const float* x, const float* const* params, float* const preds[6],
@@ -556,10 +664,15 @@ extern "C" int yfv2_train_backward(yfv2_trainer* t, const float* x, const float*
     if (!t || !x || !params || !preds || !dpreds || !grads_flat || !workspace) { set_error("train_backward: null argument"); return YFV2_EINVAL; }
     for (int i = 0; i < 6; ++i) if (!preds[i] || !dpreds[i]) { set_error("train_backward: null head tensor %d", i); return YFV2_EINVAL; }
     for (int i = 0; i < YFV2_NUM_PARAMS; ++i) if (!params[i]) { set_error("train_backward: null parameter %d", i); return YFV2_EINVAL; }
+    if (t->ctotal == 0) { set_error("train_backward: no parameter is trainable (element 0 of tensors does not require grad)"); return YFV2_EINVAL; }
+    if (t->trainable != t->fwd_trainable || t->bn_eval != t->fwd_bn_eval) {
+        set_error("train_backward: the mode changed after the forward (yfv2_trainer_set_mode applies from the next yfv2_train_forward)");
+        return YFV2_EINVAL;
+    }
     cudaStream_t s = (cudaStream_t)stream;
     static const bool no_graph = getenv("YFV2_TRAIN_NOGRAPH") != nullptr;
     if (no_graph || !t->use_graphs) return run_backward(t, x, params, preds, dpreds, grads_flat, accumulate, workspace, s);
-    unsigned long long key = mix(mix(mix(0x4321ull, x), workspace), grads_flat);
+    unsigned long long key = mix(mix(mix(mix(0x4321ull, t->mode_hash), x), workspace), grads_flat);
     for (int i = 0; i < YFV2_NUM_PARAMS; ++i) key = mix(key, params[i]);
     for (int i = 0; i < 6; ++i) key = mix(mix(key, preds[i]), dpreds[i]);
     return replay_or_capture(t, t->g_bwd[accumulate ? 1 : 0], key, s,

@@ -59,6 +59,14 @@ class Detector(nn.Module):
             self.__dict__["_train_buf_cache"] = c
         return c[0], c[1]
 
+    def _bn_modules(self):
+        """The 73 BatchNorm modules in module order (the trainer's BatchNorm layer order); cached like _train_buffers."""
+        c = self.__dict__.get("_bn_mod_cache")
+        if c is None:
+            c = [m for m in self.modules() if isinstance(m, nn.BatchNorm2d)]
+            self.__dict__["_bn_mod_cache"] = c
+        return c
+
     def invalidate_packed(self):
         """Forces the next eval forward to re-fold BN and re-pack the weights.  Needed after edits that do not bump
         `tensor._version` (`p.data.add_()`, raw-pointer updates); `forward()` in train mode and `load_state_dict` call it."""
@@ -76,7 +84,7 @@ class Detector(nn.Module):
         new = cls.__new__(cls)
         memo[id(self)] = new
         for k, v in self.__dict__.items():
-            if k == "_train_buf_cache":
+            if k in ("_train_buf_cache", "_bn_mod_cache"):
                 continue
             new.__dict__[k] = {} if k in ("_plans", "_trainers") else copy.deepcopy(v, memo)
         return new
@@ -86,6 +94,7 @@ class Detector(nn.Module):
         st["_plans"] = {}
         st["_trainers"] = {}
         st.pop("_train_buf_cache", None)
+        st.pop("_bn_mod_cache", None)
         return st
 
     def _trainer_for(self, x):
@@ -127,7 +136,9 @@ class Detector(nn.Module):
             x = x.float() if x.dtype != torch.float32 else x
             yfv2_engine.check_bn_batch(x.shape[0], x.shape[2], x.shape[3])
             # default: the native trainer (csrc/trainer.cu), one C-ABI call for the forward and one for the backward;
-            # YFV2_TRAIN_PYOPS=1 keeps the op-by-op autograd composition (the path the operator tests pin)
+            # YFV2_TRAIN_PYOPS=1 keeps the op-by-op autograd composition (the path the operator tests pin).  Both follow, per
+            # call, each parameter's requires_grad and each BatchNorm module's own .training (model.backbone.eval() freezes
+            # the backbone's statistics as in PyTorch); self.training only chooses training over the inference plan
             if os.environ.get("YFV2_TRAIN_PYOPS") or x.shape[2] % 32 or x.shape[3] % 32:
                 return train_ops.forward_train(self, x)
             return train_ops.forward_train_native(self, x)

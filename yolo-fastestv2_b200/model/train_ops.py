@@ -32,8 +32,8 @@ class Conv1x1(torch.autograd.Function):
         N, K, H, W = x.shape
         M = w.shape[0]
         dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
-        dw = torch.empty_like(w)
-        db = torch.empty(M, dtype=torch.float32, device=x.device) if ctx.has_bias else None
+        dw = torch.empty_like(w) if ctx.needs_input_grad[1] else None
+        db = torch.empty(M, dtype=torch.float32, device=x.device) if ctx.has_bias and ctx.needs_input_grad[2] else None
         eng.op("conv1x1_bwd", [x, w, dy, dx, dw, db, N, K, M, H * W], x.device)
         return dx, dw, db
 
@@ -58,7 +58,7 @@ class DwConv(torch.autograd.Function):
         N, C, H, W = x.shape
         ks = w.shape[-1]
         dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
-        dw = torch.empty_like(w)
+        dw = torch.empty_like(w) if ctx.needs_input_grad[1] else None
         eng.op("dwconv_bwd", [x, w, dy, dx, dw, N, C, H, W, ks, ctx.stride], x.device)
         return dx, dw, None
 
@@ -107,11 +107,38 @@ class BnTrain(torch.autograd.Function):
     def backward(ctx, dy):
         x, y, gamma, mean, invstd = ctx.saved_tensors
         N, C, H, W = x.shape
-        dx = torch.empty_like(x)
-        dgamma = torch.empty_like(gamma)
-        dbeta = torch.empty_like(gamma)
+        dx = torch.empty_like(x)                             # (needed for the sums even when x needs no gradient)
+        dgamma = torch.empty_like(gamma) if ctx.needs_input_grad[1] else None
+        dbeta = torch.empty_like(gamma) if ctx.needs_input_grad[2] else None
         scratch = torch.empty(2 * C, dtype=torch.float64, device=x.device)
         eng.op("bn_train_bwd", [x, y, _c(dy), gamma, mean, invstd, dx, dgamma, dbeta, scratch, N, C, H * W, ctx.relu], x.device)
+        return (dx if ctx.needs_input_grad[0] else None), dgamma, dbeta, None, None, None
+
+
+class BnEval(torch.autograd.Function):
+    """y = [ReLU](BN_eval(x)): a BatchNorm module in .eval() inside a train-mode network (running statistics, not updated)."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, running_mean, running_var, relu):
+        x = _c(x)
+        N, C, H, W = x.shape
+        y = torch.empty_like(x)
+        mean = torch.empty(C, dtype=torch.float32, device=x.device)
+        invstd = torch.empty(C, dtype=torch.float32, device=x.device)
+        eng.op("bn_eval_fwd", [x, gamma, beta, running_mean, running_var, y, mean, invstd, N, C, H * W, int(relu)], x.device)
+        ctx.save_for_backward(x, y, gamma, mean, invstd)
+        ctx.relu = int(relu)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, y, gamma, mean, invstd = ctx.saved_tensors
+        N, C, H, W = x.shape
+        dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
+        dgamma = torch.empty_like(gamma) if ctx.needs_input_grad[1] else None
+        dbeta = torch.empty_like(gamma) if ctx.needs_input_grad[2] else None
+        scratch = torch.empty(2 * C, dtype=torch.float64, device=x.device) if dgamma is not None or dbeta is not None else None
+        eng.op("bn_eval_bwd", [x, y, _c(dy), gamma, mean, invstd, dx, dgamma, dbeta, scratch, N, C, H * W, ctx.relu], x.device)
         return dx, dgamma, dbeta, None, None, None
 
 
@@ -157,6 +184,8 @@ class Upsample2x(torch.autograd.Function):
 
 # ---- network composition (same wiring as the eval engine, module parameters as weights) ---------------------------------
 def _bn(x, bn, relu):
+    if not bn.training:                                      # e.g. model.backbone.eval() inside a train-mode model
+        return BnEval.apply(x, bn.weight, bn.bias, bn.running_mean, bn.running_var, relu)
     y = BnTrain.apply(x, bn.weight, bn.bias, bn.running_mean, bn.running_var, relu)
     bn.num_batches_tracked += 1
     return y
@@ -195,9 +224,11 @@ def _head(block, x):
 # ---- the whole network as ONE autograd node over the native trainer (csrc/trainer.cu) ------------------------------------------
 class NetTrainFn(torch.autograd.Function):
     """preds = net(x) in train mode.  forward: yfv2_train_forward (saves activations in the trainer's workspace); backward:
-    yfv2_train_backward -> every parameter gradient in one flat buffer.  When the parameters' .grad already are the consecutive
-    views of one flat buffer in parameter order (train_ddp.FlatGradBucket), the gradients are ACCUMULATED straight into it and
-    autograd is told there is nothing more to add; otherwise they are returned as views of a fresh flat buffer."""
+    yfv2_train_backward -> every trainable parameter's gradient in one flat buffer.  When the trainable parameters' .grad already
+    are the consecutive views of one flat buffer in parameter order (train_ddp.FlatGradBucket), the gradients are ACCUMULATED
+    straight into it and autograd is told there is nothing more to add; otherwise they are returned as views of a fresh flat
+    buffer.  Frozen parameters (requires_grad=False) get None, and BatchNorm modules in .eval() run on their running statistics:
+    the trainer's mode follows both on every call."""
 
     @staticmethod
     def forward(ctx, x, model, *params):
@@ -205,9 +236,14 @@ class NetTrainFn(torch.autograd.Function):
             raise NotImplementedError("gradient with respect to the input image is not implemented (train.py never asks for it)")
         tr = model._trainer_for(x)
         bn, nbt = model._train_buffers()
+        bn_eval = [not m.training for m in model._bn_modules()]
+        tr.set_mode([p.requires_grad for p in params], bn_eval)
         plist = [p.detach() for p in params]
         preds = tr.forward(x, plist, bn)
-        torch._foreach_add_(nbt, 1)
+        if any(bn_eval):                                 # an eval-mode layer does not count the batch (nn.BatchNorm2d.forward)
+            nbt = [t for t, e in zip(nbt, bn_eval) if not e]
+        if nbt:
+            torch._foreach_add_(nbt, 1)
         ctx.tr, ctx.gen, ctx.plist, ctx.params = tr, tr.generation, plist, params
         return tuple(preds)
 
@@ -217,31 +253,29 @@ class NetTrainFn(torch.autograd.Function):
         if tr.generation != ctx.gen:
             raise RuntimeError("yfv2: the native trainer keeps ONE batch's activations per input shape; call backward() before the next "
                                "train-mode forward of that shape (or set YFV2_TRAIN_PYOPS=1 for the op-by-op autograd path)")
-        params = ctx.params
+        # the trainable parameters, each with its slot of the flat buffer (frozen ones have offset -1)
+        live = [(p, off, num) for p, (off, num) in zip(ctx.params, tr.param_offsets) if off >= 0]
         # fast path: .grad tensors are the slices of one flat bucket, in order
         base = None
-        if all(p.grad is not None and p.grad.is_contiguous() and p.grad.dtype == torch.float32 for p in params):
-            base = params[0].grad.data_ptr()
-            for p, (off, num) in zip(params, tr.param_offsets):
+        if live and all(p.grad is not None and p.grad.is_contiguous() and p.grad.dtype == torch.float32 for p, _, _ in live):
+            base = live[0][0].grad.data_ptr()
+            for p, off, num in live:
                 if p.grad.data_ptr() != base + 4 * off or p.grad.numel() != num:
                     base = None
                     break
         if base is not None:
-            g0 = params[0].grad
+            g0 = live[0][0].grad
             flat = torch.as_strided(g0, (tr.grad_floats,), (1,), g0.storage_offset()) if g0.untyped_storage().nbytes() >= 4 * (g0.storage_offset() + tr.grad_floats) else None
             if flat is not None:
                 tr.backward(ctx.plist, dpreds, flat, accumulate=True)
-                return (None, None) + tuple(None for _ in params)
+                return (None, None) + tuple(None for _ in ctx.params)
         flat = tr.backward(ctx.plist, dpreds, None, accumulate=False).clone()      # (autograd may keep what it is handed as .grad)
-        return (None, None) + tuple(flat[off:off + num].view_as(p) for p, (off, num) in zip(params, tr.param_offsets))
+        return (None, None) + tuple(flat[off:off + num].view_as(p) if off >= 0 else None for p, (off, num) in zip(ctx.params, tr.param_offsets))
 
 
 def forward_train_native(model, x):
     """Train-mode Detector.forward through the native trainer: one autograd node for the whole network."""
-    params = list(model.parameters())
-    if not all(p.requires_grad for p in params):
-        raise NotImplementedError("the native trainer differentiates all 225 parameters; frozen parameters need YFV2_TRAIN_PYOPS=1")
-    return NetTrainFn.apply(x.contiguous(), model, *params)
+    return NetTrainFn.apply(x.contiguous(), model, *model.parameters())
 
 
 def forward_train(model, x):

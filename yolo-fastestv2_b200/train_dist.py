@@ -19,6 +19,12 @@ reference's SGD.  BatchNorm statistics stay per rank (the reference has no SyncB
 workers read the files and parse the JPEG headers, and each batch is decoded and resized into the network input on the GPU, the
 same bytes as TensorDataset(imgaug=False) (DESIGN.md §13).
 
+`--freeze PREFIXES` fine-tunes with the parameters whose `named_parameters()` name starts with one of the comma-separated prefixes
+frozen (requires_grad=False: no gradient, no optimizer update, and the native trainer does not run the backward below the lowest
+trainable layer); `--freeze-bn` also puts the BatchNorm layers whose weight and bias are both frozen in eval mode (running
+statistics used and left alone); `--unfreeze-epoch E` makes everything trainable and every BatchNorm layer train-mode again from
+epoch E.  Without them every parameter trains, as in train.py.
+
 `--synthetic N` replaces the dataset by N seeded synthetic images with SURVEY 8(d) config[2] box statistics (no dataset and
 no reference checkout needed: used by the GPU tests and the 8-GPU measurement)."""
 import argparse
@@ -81,7 +87,16 @@ def main(argv=None):
     ap.add_argument("--device-aug-blur", action="store_true", help="with --device-aug: add motion_blur (utils/datasets.py:18-37)")
     ap.add_argument("--device-decode", action="store_true", help="read the train and validation images with utils.device_data: JPEG "
                                                                  "decode and resize to the network input on the GPU (needs --device-aug)")
+    ap.add_argument("--freeze", type=str, default="", help="comma-separated named_parameters() prefixes to freeze, e.g. "
+                                                           "'backbone' or 'backbone,fpn.conv1x1_2' (fine-tuning from pre_weights)")
+    ap.add_argument("--freeze-bn", action="store_true", help="with --freeze: BatchNorm layers whose weight and bias are both frozen run "
+                                                             "in eval mode (running statistics, not updated)")
+    ap.add_argument("--unfreeze-epoch", type=int, default=None, help="with --freeze: train everything, every BatchNorm layer in "
+                                                                      "train mode, from this epoch on")
     opt = ap.parse_args(argv)
+    freeze = [f for f in opt.freeze.split(",") if f]
+    if (opt.freeze_bn or opt.unfreeze_epoch is not None) and not freeze:
+        ap.error("--freeze-bn and --unfreeze-epoch need --freeze")
     if opt.device_decode and not opt.device_aug:
         ap.error("--device-decode needs --device-aug: the device loader does not run contrast_and_brightness, which "
                  "TensorDataset(imgaug=True) applies to training images")
@@ -147,6 +162,21 @@ def main(argv=None):
         for t in list(net.parameters()) + list(net.buffers()):
             dist.broadcast(t.data, src=0)
 
+    frozen_bn = []
+    if freeze:
+        names = [n for n, _ in net.named_parameters()]
+        unmatched = [f for f in freeze if not any(n.startswith(f) for n in names)]
+        if unmatched:
+            raise SystemExit("train_dist.py: --freeze prefix %s matches no parameter name" % ", ".join(repr(f) for f in unmatched))
+        for n, p in net.named_parameters():
+            p.requires_grad_(not any(n.startswith(f) for f in freeze))
+        if opt.freeze_bn:
+            frozen_bn = [m for m in net.modules() if isinstance(m, torch.nn.BatchNorm2d)
+                         and not m.weight.requires_grad and not m.bias.requires_grad]
+        if rank == 0:
+            print("fine-tuning: %d of %d parameters frozen, %d BatchNorm layers in eval mode" % (
+                sum(not p.requires_grad for p in net.parameters()), len(names), len(frozen_bn)))
+
     bucket = train_ddp.FlatGradBucket(net.parameters())
     optimizer = train_ddp.make_optimizer(net, cfg["learning_rate"])               # train.py:81-85
     scheduler = torch.optim.lr_scheduler.MultiStepLR(optimizer, milestones=[int(s) for s in cfg["steps"]], gamma=0.1)
@@ -155,7 +185,17 @@ def main(argv=None):
     batch_num, t0, seen = 0, time.time(), 0
     bucket.zero()
     for epoch in range(epochs):
+        if freeze and epoch == opt.unfreeze_epoch:
+            for p in net.parameters():
+                p.requires_grad_(True)
+            frozen_bn = []
+            bucket = train_ddp.FlatGradBucket(net.parameters())       # (the optimizer already holds every parameter)
+            bucket.zero()
+            if rank == 0:
+                print("fine-tuning: everything trainable from epoch %d" % epoch)
         net.train()
+        for m in frozen_bn:                                       # (after net.train(): rank 0's evaluation left the model in eval)
+            m.eval()
         sampler.set_epoch(epoch)
         for imgs, targets in train_dataloader:
             imgs = imgs.to(device, non_blocking=True)

@@ -54,6 +54,11 @@ class TrainerOp(ctypes.Structure):
                [("aux", ctypes.c_longlong)]
 
 
+class TrainerBwdOp(ctypes.Structure):
+    """yfv2_trainer_bwd_op: one op whose backward runs under the trainer's current mode, and what it writes (test hook)."""
+    _fields_ = [(f, ctypes.c_int) for f in ("op", "da", "db", "dw", "dbias", "dgamma", "dbeta", "bn_eval")]
+
+
 class TrainerTensor(ctypes.Structure):
     """yfv2_trainer_tensor: where the trainer keeps one tensor and its gradient (test hook)."""
     _fields_ = [("off", ctypes.c_longlong), ("goff", ctypes.c_longlong), ("C", ctypes.c_int), ("H", ctypes.c_int), ("W", ctypes.c_int),
@@ -81,6 +86,34 @@ def trainer_program(handle):
     for o in ops:
         o["kind"] = TRAINER_OP_KINDS[o["kind"]]
     return ops, [as_dict(t) for t in tens], dict(zip(TRAINER_LAYOUT, lay))
+
+
+def trainer_backward_plan(handle):
+    """The ops whose backward runs under a yfv2_trainer handle's current mode, in backward order, as dicts (host only; test hook)."""
+    L, n = lib(), ctypes.c_int()
+    _check(L.yfv2_trainer_debug_backward(handle, None, 0, ctypes.byref(n)), "trainer_debug_backward")
+    recs = (TrainerBwdOp * n.value)()
+    _check(L.yfv2_trainer_debug_backward(handle, recs, n.value, ctypes.byref(n)), "trainer_debug_backward")
+    return [{f: getattr(r, f) for f, _ in r._fields_} for r in recs]
+
+
+def trainer_mode(trainable=None, bn_eval=None):
+    """(trainable, bn_eval) as tuples of bools, None for the default (all trainable / all train mode); a flag list of the wrong
+    length raises (225 parameters, 73 BatchNorm layers)."""
+    trainable = None if trainable is None else tuple(bool(v) for v in trainable)
+    bn_eval = None if bn_eval is None else tuple(bool(v) for v in bn_eval)
+    if trainable is not None and len(trainable) != 225:
+        raise Yfv2Error("trainer mode: %d trainable flags, expected 225 (one per parameter)" % len(trainable))
+    if bn_eval is not None and len(bn_eval) != 73:
+        raise Yfv2Error("trainer mode: %d bn_eval flags, expected 73 (one per BatchNorm layer)" % len(bn_eval))
+    return (None if trainable is None or all(trainable) else trainable,
+            None if bn_eval is None or not any(bn_eval) else bn_eval)
+
+
+def trainer_set_mode(handle, trainable, bn_eval):
+    """yfv2_trainer_set_mode on a handle (host only); arguments as trainer_mode returns them."""
+    arr = lambda v: None if v is None else (ctypes.c_ubyte * len(v))(*v)
+    _check(lib().yfv2_trainer_set_mode(handle, arr(trainable), arr(bn_eval)), "trainer_set_mode")
 
 
 class LaunchRecord(ctypes.Structure):
@@ -215,6 +248,8 @@ PROTOTYPES = {
     "yfv2_op_stem_wgrad": (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int] * 4 + [ctypes.c_void_p]),
     "yfv2_op_bn_train_fwd": (ctypes.c_int, [ctypes.c_void_p] * 9 + [ctypes.c_int] * 4 + [ctypes.c_void_p]),
     "yfv2_op_bn_train_bwd": (ctypes.c_int, [ctypes.c_void_p] * 10 + [ctypes.c_int] * 4 + [ctypes.c_void_p]),
+    "yfv2_op_bn_eval_fwd": (ctypes.c_int, [ctypes.c_void_p] * 8 + [ctypes.c_int] * 4 + [ctypes.c_void_p]),
+    "yfv2_op_bn_eval_bwd": (ctypes.c_int, [ctypes.c_void_p] * 10 + [ctypes.c_int] * 4 + [ctypes.c_void_p]),
     "yfv2_op_maxpool_fwd": (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int] * 3 + [ctypes.c_void_p]),
     "yfv2_op_maxpool_bwd": (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int] * 3 + [ctypes.c_void_p]),
     "yfv2_op_upsample2_fwd": (ctypes.c_int, [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3 + [ctypes.c_void_p]),
@@ -224,6 +259,8 @@ PROTOTYPES = {
     "yfv2_trainer_workspace_bytes": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_size_t)]),
     "yfv2_trainer_grad_floats": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_longlong)]),
     "yfv2_trainer_param_offset": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_longlong), ctypes.POINTER(ctypes.c_longlong)]),
+    "yfv2_trainer_set_mode": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "yfv2_trainer_debug_backward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
     "yfv2_train_forward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, _c_void_pp, _c_void_pp, _c_void_pp, ctypes.c_void_p, ctypes.c_void_p]),
     "yfv2_train_backward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, _c_void_pp, _c_void_pp, _c_void_pp, ctypes.c_void_p, ctypes.c_int,
                                            ctypes.c_void_p, ctypes.c_void_p]),
@@ -319,6 +356,18 @@ class Trainer:
         nb = ctypes.c_size_t()
         _check(L.yfv2_trainer_workspace_bytes(self._h, ctypes.byref(nb)), "trainer_workspace_bytes")
         self.workspace = torch.empty(nb.value, dtype=torch.uint8, device=self.device)
+        self.mode = (None, None)              # (trainable, bn_eval) tuples of bools; None: the default (all trainable, all train)
+        self._read_layout()
+        self.generation = 0                  # bumped by every forward: a backward must see the generation of its own forward
+        # persistent buffers: the C side replays its two programs as CUDA graphs while every pointer stays the same
+        self.x_static = torch.empty((N, 3, H, W), dtype=torch.float32, device=self.device)
+        self.preds_static = self.alloc_preds()
+        self.dpreds_static = [torch.empty_like(p) for p in self.preds_static]
+        self.flat_static = torch.empty(self.grad_floats, dtype=torch.float32, device=self.device)
+
+    def _read_layout(self):
+        """grad_floats and param_offsets ((offset, numel) per parameter, offset -1 when frozen) of the current mode."""
+        L = lib()
         n = ctypes.c_longlong()
         _check(L.yfv2_trainer_grad_floats(self._h, ctypes.byref(n)), "trainer_grad_floats")
         self.grad_floats = n.value
@@ -327,12 +376,22 @@ class Trainer:
         for i in range(225):
             _check(L.yfv2_trainer_param_offset(self._h, i, ctypes.byref(off), ctypes.byref(num)), "trainer_param_offset")
             self.param_offsets.append((off.value, num.value))
-        self.generation = 0                  # bumped by every forward: a backward must see the generation of its own forward
-        # persistent buffers: the C side replays its two programs as CUDA graphs while every pointer stays the same
-        self.x_static = torch.empty((N, 3, H, W), dtype=torch.float32, device=self.device)
-        self.preds_static = self.alloc_preds()
-        self.dpreds_static = [torch.empty_like(p) for p in self.preds_static]
-        self.flat_static = torch.empty(self.grad_floats, dtype=torch.float32, device=self.device)
+
+    def set_mode(self, trainable=None, bn_eval=None):
+        """Fine-tuning mode from the next forward(): trainable = 225 flags (p.requires_grad in model.parameters() order), bn_eval =
+        73 flags (BatchNorm module not .training, in module order); None: all trainable / all train mode.  Cheap when unchanged."""
+        mode = trainer_mode(trainable, bn_eval)
+        if mode == self.mode:
+            return
+        trainer_set_mode(self._h, *mode)
+        self.mode = mode
+        self._read_layout()
+        if self.flat_static.numel() != self.grad_floats:
+            self.flat_static = torch.empty(self.grad_floats, dtype=torch.float32, device=self.device)
+
+    def backward_plan(self):
+        """trainer_backward_plan of the current mode (host only)."""
+        return trainer_backward_plan(self._h)
 
     def __del__(self):
         try:
