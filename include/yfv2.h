@@ -160,6 +160,78 @@ YFV2_API int yfv2_merge_regions(const float* dets, const int* counts, const yfv2
                                 int H, int W, double thr, int metric, int max_det, double* out, int* out_counts, int* kept_src,
                                 void* stream);
 
+/* ---- multi-object tracking across video frames: ByteTrack's association and lifecycle, S streams in one device state ---------
+ * No reference counterpart (the reference detects on single images).  The tracker keeps S streams (cameras) of at most K tracks
+ * each in one caller-owned device buffer of yfv2_track_state_bytes(S, K) bytes; yfv2_track_reset clears chosen streams (no
+ * tracks, frame 0, next id 1) and must run on every stream before its first update.  One yfv2_track_update call gives B distinct
+ * streams one frame each, in ONE launch with one CTA per stream; it allocates nothing and never synchronises.  Class-agnostic: a
+ * track takes the class of its latest detection.  Bit-exact to tests/track_oracle.py.
+ *
+ * Arithmetic: IEEE fp64, one rounding per operation (no FMA, no sqrt); min(a, b) = a < b ? a : b, max(a, b) = a > b ? a : b.
+ * Detections: dets [B, M, 6] float64 rows (x1, y1, x2, y2, conf, cls) in frame pixels (what yfv2_merge_regions writes), counts [B]
+ * (the first min(max(counts[b], 0), M) rows are read).  A row is used when all six values are finite, x2 > x1, y2 > y1 and
+ * conf > low_thresh; it is "high" if conf > high_thresh, else "low".  Its measurement z = (cx, cy, a, h): w = x2 - x1,
+ * h = y2 - y1, cx = x1 + w/2, cy = y1 + h/2, a = w / h.
+ * Kalman filter, constant velocity on (cx, cy, a, h), DeepSORT's noise model in four decoupled 2x2 blocks: coordinate k keeps
+ * position variance p, cross term x, velocity variance v; sp = 1/20, sv = 1/160; products left to right, squares as s * s.
+ *   initiate: mean = (z, 0, 0, 0, 0); std_pos = ((2*sp)*h, (2*sp)*h, 1e-2, (2*sp)*h); std_vel = ((10*sv)*h, (10*sv)*h, 1e-5,
+ *             (10*sv)*h); p = std_pos^2, x = 0, v = std_vel^2.
+ *   predict (every live track; a lost one first sets mean[7] = 0): h = mean[3] before the step; q_pos = (sp*h, sp*h, 1e-2,
+ *             sp*h)^2, q_vel = (sv*h, sv*h, 1e-5, sv*h)^2; mean[k] += mean[k+4]; t = x + v; p = ((p + x) + t) + q_pos; x = t;
+ *             v = v + q_vel.
+ *   update:  h = predicted mean[3]; r = (sp*h, sp*h, 1e-1, sp*h)^2; s = p + r; k0 = p / s; k1 = x / s; y = z[k] - mean[k];
+ *             mean[k] += k0*y; mean[k+4] += k1*y; p = p - k0*p; x' = x - k0*x; v = v - k1*x (the old x).
+ *   box:      h = mean[3]; w = mean[2]*h; x1 = mean[0] - w/2; y1 = mean[1] - h/2; x2 = x1 + w; y2 = y1 + h.
+ *   IoU(a, b), no +1: inter = max(0, min(a.x2, b.x2) - max(a.x1, b.x1)) * max(0, min(a.y2, b.y2) - max(a.y1, b.y1));
+ *             IoU = inter / ((area_a + area_b) - inter), area = (x2 - x1) * (y2 - y1); a is the track (the tracked one in
+ *             step 9).
+ * One association stage: rows = tracks in ascending id, columns = detections in row order, cost c = 1 - IoU or, "fused",
+ * 1 - IoU*conf; a pair is allowed iff c < thr.  (1) Only tracks and detections with an allowed pair are kept, in order; the
+ * smaller side plays the solver's rows (the tracks on equal sizes).  (2) C[i][j] = c - thr if allowed, else 0.  (3) Crouse's
+ * shortest augmenting path (scipy's linear_sum_assignment), rows in order; per row: SR = SC = {}, i = row, minVal = 0, shortest
+ * = +inf; until an unassigned column is reached: SR += i; for j not in SC: r = ((minVal + C[i][j]) - u[i]) - v[j], if r <
+ * shortest[j]: shortest[j] = r, path[j] = i; j* = the lowest j not in SC with the least shortest[j]; minVal = shortest[j*];
+ * SC += j*; i = row4col[j*].  Then u[row] += minVal; u[i] += minVal - shortest[col4row[i]] for the other i in SR; v[j] -= minVal
+ * - shortest[j] for j in SC; augment along path.  (4) Assigned pairs that are not allowed stay unmatched.
+ * One update of stream s: (1) frame += 1, predict every live track.  (2) stage 1, fused, thr = match_thresh: confirmed tracks
+ * (tracked or lost) x high detections.  (3) stage 2, thr 0.5: confirmed tracked tracks unmatched by stage 1 x low detections.
+ * (4) confirmed tracked tracks still unmatched become lost.  (5) stage 3, fused, thr 0.7: tentative tracks x high detections
+ * still unmatched; unmatched tentative tracks are removed.  (6) matched tracks: Kalman update, state tracked, confirmed, score,
+ * cls and det_row of the detection, end_frame = frame (a lost track found again keeps its id).  (7) births, in row order: every
+ * unmatched high detection with conf >= new_thresh starts a track with id next_id++, start_frame = end_frame = frame, confirmed
+ * iff frame == 1; with K live tracks it is not created, spends no id and counts in dropped[b].  (8) lost tracks with frame -
+ * end_frame > max_age are removed.  (9) of every pair (p tracked, tentative or not; q lost) with IoU(box p, box q) > 0.85, judged
+ * on the state before any of these removals, q is removed if age(p) > age(q), else p (age = frame - start_frame).  (10) out
+ * [B, K, 8] float64: the confirmed tracked tracks in ascending id, (x1, y1, x2, y2, score, cls, id, det_row) with the box of the
+ * updated mean; out_counts [B]; rows past the count are zeros.
+ * Checked before any launch (YFV2_EINVAL, naming the argument): non-null pointers; 1 <= K <= YFV2_TRACK_MAX_CAPACITY;
+ * 1 <= M <= YFV2_TRACK_MAX_ROWS; 1 <= B <= min(S, YFV2_TRACK_MAX_BATCH); streams_host[b] in [0, S), each at most once; thresholds finite with 0 <= low <
+ * high <= new <= 1 and 0 < match <= 1; max_age >= 0. */
+#define YFV2_TRACK_MAX_CAPACITY 1024
+#define YFV2_TRACK_MAX_ROWS     2048
+#define YFV2_TRACK_MAX_BATCH    4096   /* streams per call: their indices travel in the launch's parameters */
+#define YFV2_TRACK_TRACKED 1
+#define YFV2_TRACK_LOST    2
+typedef struct yfv2_track_params {
+    double high_thresh, low_thresh, new_thresh, match_thresh;   /* ByteTrack's 0.5, 0.1, 0.6, 0.8 */
+    int max_age;                                                /* frames a lost track survives (30) */
+} yfv2_track_params;
+typedef struct yfv2_track {
+    double mean[8];        /* cx, cy, a, h, then their velocities */
+    double cov[12];        /* coordinate k (cx, cy, a, h): p, x, v at [3k], [3k+1], [3k+2] */
+    double score, cls;     /* of the latest detection */
+    int id, state;         /* YFV2_TRACK_TRACKED | YFV2_TRACK_LOST */
+    int confirmed, start_frame, end_frame, det_row;
+} yfv2_track;
+YFV2_API int yfv2_track_state_bytes(int S, int K, size_t* bytes);
+YFV2_API int yfv2_track_reset(void* state, int S, int K, const int* streams_host, int B, void* stream);
+YFV2_API int yfv2_track_update(void* state, int S, int K, const int* streams_host, int B, const double* dets, const int* counts,
+                               int M, const yfv2_track_params* params, double* out, int* out_counts, int* dropped, void* stream);
+/* test hook: stream s's frame, next id and live tracks in ascending id (n_host of them, at most K) copied to the host; synchronises
+ * `stream` */
+YFV2_API int yfv2_track_debug_read(const void* state, int S, int K, int s, int* frame_host, int* next_id_host, yfv2_track* tracks_host,
+                                   int* n_host, void* stream);
+
 /* ---- get_batch_statistics (utils/utils.py:184-230): true-positive flags of NMS output rows ----------------
  * dets [N,max_det,6] / counts [N] as yfv2_nms writes them; targets [nt,6] rows (image, class, x1, y1, x2, y2) in
  * pixels (what evaluation() builds at utils/utils.py:372-375), nt <= 8192.  tp [N,max_det] receives 1.0 for a true

@@ -154,6 +154,23 @@ class Region(ctypes.Structure):
     _fields_ = [("frame", ctypes.c_int), ("x0", ctypes.c_int), ("y0", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int)]
 
 
+class TrackParams(ctypes.Structure):
+    """yfv2_track_params: the tracker's thresholds and the frames a lost track survives."""
+    _fields_ = [("high_thresh", ctypes.c_double), ("low_thresh", ctypes.c_double), ("new_thresh", ctypes.c_double),
+                ("match_thresh", ctypes.c_double), ("max_age", ctypes.c_int)]
+
+
+class TrackRecord(ctypes.Structure):
+    """yfv2_track: one track's state as yfv2_track_debug_read copies it."""
+    _fields_ = [("mean", ctypes.c_double * 8), ("cov", ctypes.c_double * 12), ("score", ctypes.c_double), ("cls", ctypes.c_double),
+                ("id", ctypes.c_int), ("state", ctypes.c_int), ("confirmed", ctypes.c_int), ("start_frame", ctypes.c_int),
+                ("end_frame", ctypes.c_int), ("det_row", ctypes.c_int)]
+
+
+TRACK_TRACKED, TRACK_LOST = 1, 2                     # yfv2_track.state
+TRACK_MAX_CAPACITY, TRACK_MAX_ROWS, TRACK_MAX_BATCH = 1024, 2048, 4096
+
+
 class AugParams(ctypes.Structure):
     """yfv2_aug_params: one image's contrast (alpha, beta) and random_resize size (rw, rh)."""
     _fields_ = [("alpha", ctypes.c_float), ("beta", ctypes.c_float), ("rw", ctypes.c_int), ("rh", ctypes.c_int)]
@@ -210,6 +227,15 @@ PROTOTYPES = {
     "yfv2_merge_regions": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Region), ctypes.c_int, ctypes.c_int,
                                           ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_int, ctypes.c_int,
                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "yfv2_track_state_bytes": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_size_t)]),
+    "yfv2_track_reset": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.c_int,
+                                        ctypes.c_void_p]),
+    "yfv2_track_update": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.c_int,
+                                         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(TrackParams), ctypes.c_void_p,
+                                         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "yfv2_track_debug_read": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_int),
+                                             ctypes.POINTER(ctypes.c_int), ctypes.POINTER(TrackRecord), ctypes.POINTER(ctypes.c_int),
+                                             ctypes.c_void_p]),
     "yfv2_batch_statistics": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                              ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]),
     "yfv2_aug_contrast_brightness": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_longlong, ctypes.c_void_p]),
@@ -671,6 +697,76 @@ def merge_regions(dets, counts, regions, F, W, H, thr, metric, max_det):
                                         ctypes.c_void_p(out_counts.data_ptr()), ctypes.c_void_p(kept.data_ptr()), _stream(dev)),
                "merge_regions")
     return out, out_counts, kept
+
+
+class Tracker:
+    """A multi-stream tracker (yfv2_track_*, include/yfv2.h): ByteTrack's association in three stages and its track lifecycle with
+    a constant-velocity Kalman filter, for `streams` streams (cameras) of at most `capacity` tracks each.  It owns the device state
+    tensor; every stream starts reset (no tracks, frame 0, next id 1).  Class-agnostic: a track takes the class of its latest
+    detection."""
+
+    def __init__(self, device, streams, capacity, high_thresh=0.5, low_thresh=0.1, new_thresh=0.6, match_thresh=0.8, max_age=30):
+        self.device = torch.device(device)
+        self.S, self.K = int(streams), int(capacity)
+        self.params = TrackParams(float(high_thresh), float(low_thresh), float(new_thresh), float(match_thresh), int(max_age))
+        nb = ctypes.c_size_t()
+        _check(lib().yfv2_track_state_bytes(self.S, self.K, ctypes.byref(nb)), "Tracker")
+        self.state = torch.zeros((nb.value,), dtype=torch.uint8, device=self.device)
+        self.reset()
+
+    @property
+    def low_thresh(self):
+        return self.params.low_thresh
+
+    def _streams(self, streams, B):
+        idx = list(range(B)) if streams is None else [int(s) for s in streams]
+        return idx, (ctypes.c_int * max(len(idx), 1))(*idx)
+
+    def reset(self, streams=None):
+        """Clears the given streams (all by default): no tracks, frame 0, next id 1."""
+        idx, arr = self._streams(streams, self.S)
+        with torch.cuda.device(self.device):
+            _check(lib().yfv2_track_reset(ctypes.c_void_p(self.state.data_ptr()), self.S, self.K, arr, len(idx), _stream(self.device)),
+                   "Tracker.reset")
+
+    def update(self, dets, counts, streams=None):
+        """One frame for each of B distinct streams (streams: B stream indices; None: 0..B-1), in one launch without a host
+        synchronisation.  dets: CUDA float64 [B, M, 6] rows (x1, y1, x2, y2, conf, cls) in frame pixels, counts int32 [B] (what
+        merge_regions returns).  Returns CUDA tensors (out float64 [B, capacity, 8]: the confirmed tracked tracks in ascending id,
+        (x1, y1, x2, y2, score, cls, track_id, det_row), zeros past the count; counts int32 [B]; dropped int32 [B]: births refused
+        for want of capacity)."""
+        _require_cuda(dets, "dets")
+        _require_cuda(counts, "counts")
+        if dets.dim() != 3 or dets.shape[2] != 6 or dets.dtype != torch.float64:
+            raise Yfv2Error("Tracker.update: dets must be float64 [B, M, 6], got %s %s" % (dets.dtype, tuple(dets.shape)))
+        B, M = dets.shape[0], dets.shape[1]
+        if counts.dtype != torch.int32 or tuple(counts.shape) != (B,):
+            raise Yfv2Error("Tracker.update: counts must be int32 [%d], got %s %s" % (B, counts.dtype, tuple(counts.shape)))
+        idx, arr = self._streams(streams, B)
+        if len(idx) != B:
+            raise Yfv2Error("Tracker.update: %d streams for %d row blocks" % (len(idx), B))
+        dets, counts = dets.contiguous(), counts.contiguous()
+        out = torch.empty((B, self.K, 8), dtype=torch.float64, device=self.device)
+        out_counts = torch.empty((B,), dtype=torch.int32, device=self.device)
+        dropped = torch.empty((B,), dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            _check(lib().yfv2_track_update(ctypes.c_void_p(self.state.data_ptr()), self.S, self.K, arr, B, ctypes.c_void_p(dets.data_ptr()),
+                                           ctypes.c_void_p(counts.data_ptr()), M, ctypes.byref(self.params),
+                                           ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(out_counts.data_ptr()),
+                                           ctypes.c_void_p(dropped.data_ptr()), _stream(self.device)), "Tracker.update")
+        return out, out_counts, dropped
+
+    def tracks(self, stream):
+        """Stream `stream`'s state on the host (test hook; synchronises): {"frame", "next_id", "tracks"}, the live tracks in
+        ascending id as dicts (id, cls, state, confirmed, start_frame, end_frame, score, det_row, mean [8], cov [12])."""
+        recs = (TrackRecord * self.K)()
+        frame, next_id, n = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        with torch.cuda.device(self.device):
+            _check(lib().yfv2_track_debug_read(ctypes.c_void_p(self.state.data_ptr()), self.S, self.K, int(stream), ctypes.byref(frame),
+                                               ctypes.byref(next_id), recs, ctypes.byref(n), _stream(self.device)), "Tracker.tracks")
+        keys = ("id", "cls", "state", "confirmed", "start_frame", "end_frame", "score", "det_row")
+        tracks = [dict({k: getattr(r, k) for k in keys}, mean=list(r.mean), cov=list(r.cov)) for r in recs[:n.value]]
+        return {"frame": frame.value, "next_id": next_id.value, "tracks": tracks}
 
 
 def batch_statistics(out, counts, targets, iou_threshold):
