@@ -443,6 +443,54 @@ YFV2_API int yfv2_jpeg_decode_resize(const void* meta_host, const void* meta_dev
                                      size_t files_bytes, int H, int W, uint8_t* dst, int* errors, void* workspace,
                                      size_t workspace_bytes, void* stream);
 
+/* ---- frames and regions -> JPEG files: cv2.imencode('.jpg', img, params) on the device ----------------------------------------
+ * Output i is, byte for byte, cv2.imencode('.jpg', img_i, params_i)[1] of OpenCV 4.13 (libjpeg-turbo 3.1): baseline, the Annex K
+ * Huffman tables, islow FDCT, jccolor's fixed-point RGB -> YCbCr, jcsample's downsampling, JFIF APP0.  img_i is the BGR image
+ * cv2.cvtColor(frame, COLOR_<LAYOUT>2BGR) gives the frame (yfv2_resize_*'s conversions), or for YFV2_JPEG_SRC_GRAY the grey
+ * frame itself (a one-component JPEG, as cv2 writes a 2-D array), cropped to [y0, y0 + h) x [x0, x0 + w) AFTER the conversion.
+ * params_i: cv2's (IMWRITE_*, value) pairs, nparams ints (host): IMWRITE_JPEG_QUALITY (1; default 95; clamped to 0..100 as cv2
+ * does, 0 encodes as 1), IMWRITE_JPEG_RST_INTERVAL (4; MCUs per restart interval, clamped to 0..65535 as cv2 does),
+ * IMWRITE_JPEG_SAMPLING_FACTOR (7; 0x221111 4:2:0 default, 0x211111 4:2:2, 0x111111 4:4:4; 0x121111 and 0x411111:
+ * YFV2_EUNSUPPORTED; other values YFV2_EINVAL).  IMWRITE_JPEG_PROGRESSIVE (2) and _OPTIMIZE (3) other than 0 and
+ * IMWRITE_JPEG_LUMA_QUALITY (5) / _CHROMA_QUALITY (6) >= 0 change cv2's output and are refused (YFV2_EUNSUPPORTED); ids of other
+ * formats are ignored, as cv2 ignores them.  Regions larger than 32768 on a side: YFV2_EUNSUPPORTED.
+ *
+ * yfv2_jpeg_encode_plan (host only, no device needed; frame pointers are recorded, never read): checks every output and its frame
+ * descriptor, names the first refused output (yfv2_last_error), and reports meta_bytes (the blob: headers, geometry, quantiser
+ * tables), workspace_bytes and arena_bytes.  out_offsets[N + 1] (may be NULL) receives where each output starts in the arena.
+ * Each output's arena slot is its worst case: headers + 2 * (blocks * 209 + segments) + 2 * segments + 2 bytes (every block at
+ * the longest codes the tables have, every byte stuffed).  With meta_host NULL only the sizes are computed.
+ * yfv2_jpeg_encode: meta_dev a device copy of the blob, meta_host the blob itself (checked before any launch).  Writes output i at
+ * arena + out_offsets[i] and its length into lengths[i] (device int64).  phases: YFV2_JPEG_ENC_ALL, or the stages to run in this
+ * call, in order, for timing them separately (transform: coefficients; scan: bit counts and offsets; pack: the bits of every
+ * segment; stuff: byte stuffing, markers and the final bytes).  Nothing is allocated and nothing synchronises. */
+#define YFV2_JPEG_SRC_BGR     0   /* f.bgr */
+#define YFV2_JPEG_SRC_STRIDED 1   /* f.strided: RGB, BGRA / RGBA, planar RGB (and grey replicated to BGR) */
+#define YFV2_JPEG_SRC_GRAY    2   /* f.strided, the byte at b: a one-component JPEG */
+#define YFV2_JPEG_SRC_YUV420  3   /* f.yuv420 */
+#define YFV2_JPEG_SRC_YUV422  4   /* f.yuv422 */
+#define YFV2_JPEG_ENC_TRANSFORM 1
+#define YFV2_JPEG_ENC_SCAN      2
+#define YFV2_JPEG_ENC_PACK      4
+#define YFV2_JPEG_ENC_STUFF     8
+#define YFV2_JPEG_ENC_ALL      15
+typedef struct yfv2_jpeg_enc_src {
+    int kind;                /* YFV2_JPEG_SRC_* */
+    int x0, y0, w, h;        /* the region of the converted frame, inside it, w, h >= 1 */
+    union {
+        yfv2_frame bgr;
+        yfv2_strided_frame strided;
+        yfv2_yuv420_frame yuv420;
+        yfv2_yuv422_frame yuv422;
+    } f;                     /* the frame, in device memory */
+    const int* params;       /* host: nparams ints, cv2.imencode's (IMWRITE_*, value) pairs; may be NULL with nparams 0 */
+    int nparams;
+} yfv2_jpeg_enc_src;
+YFV2_API int yfv2_jpeg_encode_plan(const yfv2_jpeg_enc_src* srcs, int N, void* meta_host, size_t meta_cap, size_t* meta_bytes,
+                                   size_t* workspace_bytes, long long* out_offsets, size_t* arena_bytes);
+YFV2_API int yfv2_jpeg_encode(const void* meta_host, const void* meta_dev, size_t meta_bytes, void* workspace, size_t workspace_bytes,
+                              uint8_t* arena, size_t arena_bytes, long long* lengths, int phases, void* stream);
+
 /* ---- anchor k-means (genanchors.py:17-102): R runs of the reference's kmeans over one box set, iteration by iteration ---------
  * boxes: device [N][2] fp64 (w, h) as genanchors reads them from the label files.  State of run r, all device and caller-owned:
  * centroids [R][k][2] fp64 (before the first step: the initial picks, boxes[init[r][j]]), assignments [R][N] int32 (before the

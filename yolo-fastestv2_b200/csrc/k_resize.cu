@@ -34,101 +34,6 @@ namespace {
 constexpr int kResizeBx = 64, kResizeBy = 4;
 constexpr int kResizeMaxSide = 32768;
 
-// Packed HWC BGR: pixel (r, c) is the three bytes at data + r * pitch + 3c.  StridedSource states this layout too, but is 2.5 %
-// slower on it (DESIGN.md §7), so BGR keeps its own fetch.
-struct BgrSource {
-    using Desc = yfv2_frame;
-    static constexpr int kChunk = 128;   // frames per launch: their 24-byte descriptors travel as kernel parameters (3 KB)
-    static constexpr int kMinBlocks = 0;
-    const uint8_t* row;
-    __device__ __forceinline__ BgrSource(const yfv2_frame& f, int r) : row(f.data + (long long)r * f.pitch) {}
-    // B, G, R of pixels (r, c0) and (r, c1)
-    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            p0[c] = __ldg(row + 3 * c0 + c);
-            p1[c] = __ldg(row + 3 * c1 + c);
-        }
-    }
-};
-
-// Strided: channel k of pixel (r, c) at ch_k + r * pitch + c * step (B, G, R).  Packed BGR / RGB / BGRA / RGBA, grey and planar
-// RGB differ only in the descriptor's values, so nothing here branches on the layout.
-struct StridedSource {
-    using Desc = yfv2_strided_frame;
-    static constexpr int kChunk = 80;    // 48-byte descriptors: 3.75 KB of kernel parameters, under the 4 KB launch limit
-    static constexpr int kMinBlocks = 8;
-    const uint8_t* ch[3];
-    int step;
-    __device__ __forceinline__ StridedSource(const yfv2_strided_frame& f, int r) : step(f.step) {
-        const long long off = (long long)r * f.pitch;
-        ch[0] = f.b + off; ch[1] = f.g + off; ch[2] = f.r + off;
-    }
-    // B, G, R of pixels (r, c0) and (r, c1)
-    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
-        const int k0 = c0 * step, k1 = c1 * step;     // step * w < 2^31, checked on the host
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            p0[c] = __ldg(ch[c] + k0);
-            p1[c] = __ldg(ch[c] + k1);
-        }
-    }
-};
-
-// cv2.cvtColor's YUV -> BGR of one pixel, 4:2:0 and 4:2:2 alike (OpenCV ITUR_BT_601: 20-bit fixed point, limited range)
-__device__ __forceinline__ void yuv_to_bgr(int y, int uu, int vv, int (&bgr)[3]) {
-    const int yy = max(0, y - 16) * 1220542 + (1 << 19);
-    bgr[0] = sat_u8((yy + 2116026 * uu) >> 20);
-    bgr[1] = sat_u8((yy - 852492 * vv - 409993 * uu) >> 20);
-    bgr[2] = sat_u8((yy + 1673527 * vv) >> 20);
-}
-
-// YUV 4:2:0: luma Y[r][c] at y + r * y_pitch + c; the chroma of pixel (r, c) at u / v + (r >> 1) * uv_pitch + (c >> 1) * uv_step.
-// The descriptor states every layout, so nothing here branches on it.
-struct Yuv420Source {
-    using Desc = yfv2_yuv420_frame;
-    static constexpr int kChunk = 64;    // 56-byte descriptors: 3.5 KB of kernel parameters, under the 4 KB launch limit
-    static constexpr int kMinBlocks = 0;
-    const uint8_t* luma;
-    const uint8_t* u;
-    const uint8_t* v;
-    int step;
-    __device__ __forceinline__ Yuv420Source(const yfv2_yuv420_frame& f, int r)
-        : luma(f.y + (long long)r * f.y_pitch), u(f.u + (long long)(r >> 1) * f.uv_pitch), v(f.v + (long long)(r >> 1) * f.uv_pitch),
-          step(f.uv_step) {}
-    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
-        const int k0 = (c0 >> 1) * step, k1 = (c1 >> 1) * step;
-        const int u0 = __ldg(u + k0) - 128, v0 = __ldg(v + k0) - 128;
-        int u1 = u0, v1 = v0;
-        if (k1 != k0) { u1 = __ldg(u + k1) - 128; v1 = __ldg(v + k1) - 128; }   // c0, c1 in different chroma columns
-        yuv_to_bgr(__ldg(luma + c0), u0, v0, p0);
-        yuv_to_bgr(__ldg(luma + c1), u1, v1, p1);
-    }
-};
-
-// Packed YUV 4:2:2: luma of (r, c) at y + r * pitch + 2c; U and V of the macropixel (r, 2j), (r, 2j + 1) at u / v + r * pitch + 4j.
-// YUYV, UYVY and YVYU differ only in the three pointers.
-struct Yuv422Source {
-    using Desc = yfv2_yuv422_frame;
-    static constexpr int kChunk = 96;    // 40-byte descriptors: 3.75 KB of kernel parameters
-    static constexpr int kMinBlocks = 8;
-    const uint8_t* luma;
-    const uint8_t* u;
-    const uint8_t* v;
-    __device__ __forceinline__ Yuv422Source(const yfv2_yuv422_frame& f, int r) {
-        const long long off = (long long)r * f.pitch;
-        luma = f.y + off; u = f.u + off; v = f.v + off;
-    }
-    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
-        const int k0 = (c0 >> 1) * 4, k1 = (c1 >> 1) * 4;
-        const int u0 = __ldg(u + k0) - 128, v0 = __ldg(v + k0) - 128;
-        int u1 = u0, v1 = v0;
-        if (k1 != k0) { u1 = __ldg(u + k1) - 128; v1 = __ldg(v + k1) - 128; }   // c0, c1 in different macropixels
-        yuv_to_bgr(__ldg(luma + 2 * c0), u0, v0, p0);
-        yuv_to_bgr(__ldg(luma + 2 * c1), u1, v1, p1);
-    }
-};
-
 template <class Src>
 struct ResizeChunk {
     typename Src::Desc src[Src::kChunk];

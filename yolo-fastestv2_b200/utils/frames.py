@@ -189,3 +189,54 @@ def detect_tiled(model, frames, cfg, cols, rows, overlap=0.2, full_frame=True, *
         h, w = frame_size(f, lay)
         regions.append(tile_regions(w, h, cols, rows, overlap, full_frame, lay))
     return detect_regions(model, frames, cfg, regions, **kw)
+
+
+def _jpeg_path(p):
+    if not str(p).lower().endswith((".jpg", ".jpeg", ".jpe")):
+        raise yfv2_engine.Yfv2Error("write_images: %s: only JPEG files (.jpg, .jpeg, .jpe) are written on the device" % (p,))
+
+
+def write_images(paths, frames, layout="bgr", quality=95, sampling="420", restart_interval=0, device=None):
+    """cv2.imwrite(path, cv2.cvtColor(frame, COLOR_<LAYOUT>2BGR)) of every frame, the file byte for byte cv2's (OpenCV 4.13), with
+    the encode on the device (yfv2_engine.encode_jpeg, one call); other extensions are refused before anything is encoded."""
+    paths = list(paths)
+    for p in paths:
+        _jpeg_path(p)
+    files = yfv2_engine.encode_jpeg(frames, quality, sampling, restart_interval, layout, device=device)
+    if len(files) != len(paths):
+        raise yfv2_engine.Yfv2Error("write_images: %d paths for %d frames" % (len(paths), len(files)))
+    for p, b in zip(paths, files):
+        with open(p, "wb") as f:
+            f.write(b)
+
+
+def detection_regions(rows, h, w):
+    """(x0, y0, w, h) of the crop of each row: test.py's integer corners (int_corners), clipped to the h x w frame, at least one
+    pixel: img[y1:y2, x1:x2] with x1, y1 in the frame and x2 > x1, y2 > y1."""
+    out = []
+    for x1, y1, x2, y2 in int_corners(rows).tolist():
+        x1, y1 = min(max(x1, 0), w - 1), min(max(y1, 0), h - 1)
+        x2, y2 = min(max(x2, x1 + 1), w), min(max(y2, y1 + 1), h)
+        out.append((x1, y1, x2 - x1, y2 - y1))
+    return out
+
+
+def encode_detections(frames, rows, layout="bgr", quality=95, sampling="420", device=None):
+    """A JPEG of the crop of every detection row, in one encode call: rows[i] are frame i's rows in source pixels (as detect_frames,
+    detect_files, detect_regions and track_frames return them; only the first four columns are read).  Returns one list of bytes
+    per frame, each cv2.imencode('.jpg', cv2.cvtColor(frame, ...)[y1:y2, x1:x2]) of a row (detection_regions)."""
+    frames = list(frames)
+    layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
+    regions, counts = [], []
+    for i, (f, lay, r) in enumerate(zip(frames, layouts, rows)):
+        h, w = frame_size(f, lay)
+        r = torch.as_tensor(r)
+        rs = detection_regions(r.reshape(-1, r.shape[-1]) if r.numel() else r.reshape(0, 4), h, w)
+        regions += [(i,) + reg for reg in rs]
+        counts.append(len(rs))
+    files = yfv2_engine.encode_jpeg(frames, quality, sampling, 0, layouts, regions, device) if regions else []
+    out, k = [], 0
+    for n in counts:
+        out.append(files[k:k + n])
+        k += n
+    return out

@@ -48,6 +48,16 @@ class Yuv422Frame(ctypes.Structure):
                 ("w", ctypes.c_int), ("h", ctypes.c_int)]
 
 
+class _EncFrame(ctypes.Union):
+    _fields_ = [("bgr", Frame), ("strided", StridedFrame), ("yuv420", Yuv420Frame), ("yuv422", Yuv422Frame)]
+
+
+class JpegEncSrc(ctypes.Structure):
+    """yfv2_jpeg_enc_src: one output of yfv2_jpeg_encode: a frame, its region and cv2.imencode's params."""
+    _fields_ = [("kind", ctypes.c_int), ("x0", ctypes.c_int), ("y0", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int),
+                ("f", _EncFrame), ("params", ctypes.POINTER(ctypes.c_int)), ("nparams", ctypes.c_int)]
+
+
 class TrainerOp(ctypes.Structure):
     """yfv2_trainer_op: one op of the native trainer's program (test hook)."""
     _fields_ = [(f, ctypes.c_int) for f in ("kind", "a", "b", "y", "pw", "pg", "pb", "pbias", "bn", "relu", "ks", "stride", "M")] + \
@@ -247,6 +257,11 @@ PROTOTYPES = {
                                            ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
     "yfv2_debug_bgr2hsv": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_void_p]),
     "yfv2_debug_hsv2bgr": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_int, ctypes.c_void_p]),
+    "yfv2_jpeg_encode_plan": (ctypes.c_int, [ctypes.POINTER(JpegEncSrc), ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
+                                             ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t),
+                                             ctypes.POINTER(ctypes.c_longlong), ctypes.POINTER(ctypes.c_size_t)]),
+    "yfv2_jpeg_encode": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t,
+                                        ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]),
     "yfv2_resize_bgr_u8": (ctypes.c_int, [ctypes.POINTER(Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                           ctypes.c_void_p]),
     "yfv2_resize_yuv420_u8": (ctypes.c_int, [ctypes.POINTER(Yuv420Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
@@ -1424,6 +1439,157 @@ def resize_frames(frames, W, H, layout, device=None, out=None):
             _resize_layout_run(checked[i:j], layouts[i:j], W, H, device, out[i:j])
         i = j
     return out
+
+
+# cv2's IMWRITE_* ids and IMWRITE_JPEG_SAMPLING_FACTOR_* values (yfv2_jpeg_encode_plan reads the same pairs)
+IMWRITE_JPEG_QUALITY, IMWRITE_JPEG_PROGRESSIVE, IMWRITE_JPEG_OPTIMIZE, IMWRITE_JPEG_RST_INTERVAL = 1, 2, 3, 4
+IMWRITE_JPEG_LUMA_QUALITY, IMWRITE_JPEG_CHROMA_QUALITY, IMWRITE_JPEG_SAMPLING_FACTOR = 5, 6, 7
+JPEG_SAMPLING = {"420": 0x221111, "422": 0x211111, "444": 0x111111, "440": 0x121111, "411": 0x411111}
+_ENC_KIND = {"bgr": 0, "strided": 1, "gray": 2, "yuv420": 3, "yuv422": 4}
+
+
+def _enc_frame(f, lay, device, d, keep):
+    """Fills d (a JpegEncSrc) with the descriptor of checked frame f in layout `lay`, its pixels on `device`; returns (h, w)."""
+    kind = "gray" if lay == "gray" else _KIND[lay]
+    d.kind = _ENC_KIND[kind]
+    if kind == "bgr":
+        f = _frame_on_device(f, device)
+        d.f.bgr.data, d.f.bgr.w, d.f.bgr.h, d.f.bgr.pitch = f.data_ptr(), f.shape[1], f.shape[0], f.stride(0)
+        keep.append(f)
+        return f.shape[0], f.shape[1]
+    if kind == "yuv420":
+        y, u, v = [p.to(device) for p in _yuv420_planes(f, lay, 0)]
+        y, u, v = [p if p.stride(1) == 1 else p.contiguous() for p in (y, u, v)]
+        e = d.f.yuv420
+        if lay in ("nv12", "nv21"):
+            e.u, e.v, e.uv_pitch, e.uv_step = u.data_ptr() + (lay == "nv21"), u.data_ptr() + (lay == "nv12"), u.stride(0), 2
+        else:
+            if u.stride(0) != v.stride(0):
+                u, v = u.contiguous(), v.contiguous()
+            e.u, e.v, e.uv_pitch, e.uv_step = u.data_ptr(), v.data_ptr(), u.stride(0), 1
+        e.y, e.y_pitch, e.h, e.w = y.data_ptr(), y.stride(0), y.shape[0], y.shape[1]
+        keep += [y, u, v]
+        return e.h, e.w
+    f = f.to(device)
+    if lay == "rgb_chw":
+        if f.stride(2) != 1 or f.stride(1) < f.shape[2]:
+            f = f.contiguous()
+        p, s = f.data_ptr(), f.stride(0)
+        e = d.f.strided
+        e.b, e.g, e.r, e.pitch, e.step, e.h, e.w = p + 2 * s, p + s, p, f.stride(1), 1, f.shape[1], f.shape[2]
+        keep.append(f)
+        return e.h, e.w
+    step = 1 if lay == "gray" else _CHANNELS[lay]
+    if f.stride(1) != step or (lay != "gray" and f.stride(2) != 1) or f.stride(0) < step * f.shape[1]:
+        f = f.contiguous()
+    p = f.data_ptr()
+    if kind == "yuv422":
+        e = d.f.yuv422
+        oy, ou, ov = _YUV422_OFFSETS[lay]
+        e.y, e.u, e.v = p + oy, p + ou, p + ov
+    else:
+        e = d.f.strided
+        ob, og, or_ = _BGR_OFFSETS[lay]
+        e.b, e.g, e.r, e.step = p + ob, p + og, p + or_, step
+    e.pitch, e.h, e.w = f.stride(0), f.shape[0], f.shape[1]
+    keep.append(f)
+    return e.h, e.w
+
+
+def _per_output(v, n, what):
+    v = list(v) if isinstance(v, (list, tuple)) else [v] * n
+    if len(v) != n:
+        raise Yfv2Error("encode_jpeg: %d values of %s for %d outputs" % (len(v), what, n))
+    return v
+
+
+def encode_jpeg(frames, quality=95, sampling="420", restart_interval=0, layout="bgr", regions=None, device=None, params=None,
+                device_out=False):
+    """cv2.imencode('.jpg', img, params)[1] of every output, byte for byte (OpenCV 4.13), encoded on the device in one call
+    (yfv2_jpeg_encode).  img is cv2.cvtColor(frame, COLOR_<LAYOUT>2BGR) for any layout of resize_frames (one name, or one per
+    frame); "gray" frames give one-component JPEGs, as cv2 does for a 2-D array.  regions: None (one output per frame, the whole
+    frame), or a list of (frame index, x0, y0, w, h), one output each, cropped from the converted frame (several may share a
+    frame).  quality (any int, clamped to 0..100 as cv2 does), sampling ("420", "422", "444") and restart_interval (MCUs, 0: none)
+    are one value or one per output; params: extra cv2 (IMWRITE_*, value) pairs for every output, or a list of them per output.
+    Everything is checked before anything is launched; a refusal raises Yfv2Error naming the output.  Returns a list of bytes, or
+    with device_out=True (arena, offsets, lengths): the uint8 CUDA arena, output i at offsets[i] (host int64 numpy) and
+    lengths[i] bytes long (CUDA int64), with no copy to the host."""
+    import numpy as np
+    frames = list(frames)
+    layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
+    if not frames:
+        raise Yfv2Error("encode_jpeg: no frames")
+    if len(layouts) != len(frames):
+        raise Yfv2Error("encode_jpeg: %d layouts for %d frames" % (len(layouts), len(frames)))
+    for lay in layouts:
+        if not isinstance(lay, str) or lay not in LAYOUTS:
+            raise Yfv2Error("encode_jpeg: layout must be one of %s, got %r" % (", ".join(LAYOUTS), lay))
+    checked = [_check_frame(f, lay, i) for i, (f, lay) in enumerate(zip(frames, layouts))]
+    if regions is None:
+        regions = [(i, 0, 0, None, None) for i in range(len(frames))]
+    regions = [tuple(r) for r in regions]
+    n = len(regions)
+    if n == 0:
+        raise Yfv2Error("encode_jpeg: no regions")
+    for k, r in enumerate(regions):
+        if len(r) != 5 or not 0 <= int(r[0]) < len(frames):
+            raise Yfv2Error("encode_jpeg: region %d must be (frame index in [0, %d), x0, y0, w, h), got %r" % (k, len(frames), r))
+    qs, ss, rs = _per_output(quality, n, "quality"), _per_output(sampling, n, "sampling"), _per_output(restart_interval, n, "restart")
+    extra = params if params and isinstance(params[0], (list, tuple)) else [params or []] * n
+    if len(extra) != n:
+        raise Yfv2Error("encode_jpeg: %d params lists for %d outputs" % (len(extra), n))
+    plist = []
+    for k in range(n):
+        if ss[k] not in JPEG_SAMPLING:
+            raise Yfv2Error("encode_jpeg: output %d: sampling must be one of %s, got %r" % (k, ", ".join(JPEG_SAMPLING), ss[k]))
+        plist.append([IMWRITE_JPEG_QUALITY, int(qs[k]), IMWRITE_JPEG_SAMPLING_FACTOR, JPEG_SAMPLING[ss[k]],
+                      IMWRITE_JPEG_RST_INTERVAL, int(rs[k])] + [int(x) for x in extra[k]])
+    if device is None:
+        cuda = [t.device for f in checked for t in (f if isinstance(f, (tuple, list)) else (f,))
+                if isinstance(t, torch.Tensor) and t.is_cuda]
+        device = cuda[0] if cuda else torch.device("cuda", torch.cuda.current_device())
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise Yfv2Error("encode_jpeg: runs on CUDA devices only (no CPU fallback)")
+    srcs = (JpegEncSrc * n)()
+    keep, cparams, frame_desc = [], [], {}
+    for k, (d, r) in enumerate(zip(srcs, regions)):
+        i = int(r[0])
+        if i not in frame_desc:
+            frame_desc[i] = JpegEncSrc()
+            frame_desc[i].hw = _enc_frame(checked[i], layouts[i], device, frame_desc[i], keep)
+        src = frame_desc[i]
+        d.kind, d.f = src.kind, src.f
+        fh, fw = src.hw
+        d.x0, d.y0 = int(r[1]), int(r[2])
+        d.w = fw if r[3] is None else int(r[3])
+        d.h = fh if r[4] is None else int(r[4])
+        pa = (ctypes.c_int * len(plist[k]))(*plist[k])
+        cparams.append(pa)
+        d.params, d.nparams = ctypes.cast(pa, ctypes.POINTER(ctypes.c_int)), len(plist[k])
+    L = lib()
+    meta_b, ws_b, arena_b = ctypes.c_size_t(), ctypes.c_size_t(), ctypes.c_size_t()
+    offsets = np.zeros(n + 1, np.int64)
+    off_p = offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong))
+    _check(L.yfv2_jpeg_encode_plan(srcs, n, None, 0, ctypes.byref(meta_b), ctypes.byref(ws_b), off_p, ctypes.byref(arena_b)),
+           "jpeg_encode_plan")
+    meta = torch.empty(meta_b.value, dtype=torch.uint8, pin_memory=True)
+    _check(L.yfv2_jpeg_encode_plan(srcs, n, ctypes.c_void_p(meta.data_ptr()), meta_b.value, ctypes.byref(meta_b),
+                                   ctypes.byref(ws_b), off_p, ctypes.byref(arena_b)), "jpeg_encode_plan")
+    with torch.cuda.device(device):
+        meta_dev = meta.to(device, non_blocking=True)
+        ws = torch.empty(ws_b.value, dtype=torch.uint8, device=device)
+        arena = torch.empty(arena_b.value, dtype=torch.uint8, device=device)
+        lengths = torch.empty(n, dtype=torch.int64, device=device)
+        _check(L.yfv2_jpeg_encode(ctypes.c_void_p(meta.data_ptr()), ctypes.c_void_p(meta_dev.data_ptr()), meta_b.value,
+                                  ctypes.c_void_p(ws.data_ptr()), ws_b.value, ctypes.c_void_p(arena.data_ptr()), arena_b.value,
+                                  ctypes.c_void_p(lengths.data_ptr()), 15, _stream(device)), "jpeg_encode")
+        if device_out:
+            torch.cuda.current_stream(device).synchronize()   # the host blob and the frames' copies stay alive until it ran
+            return arena, offsets[:n], lengths
+        lens = lengths.cpu().numpy()
+        # only the bytes written come back: each output's slot is its worst case, usually far larger than the file
+        return [arena[int(offsets[k]):int(offsets[k]) + int(lens[k])].cpu().numpy().tobytes() for k in range(n)]
 
 
 def crop_frame(frame, layout, x0, y0, w, h):
