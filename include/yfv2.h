@@ -233,10 +233,14 @@ YFV2_API int yfv2_track_debug_read(const void* state, int S, int K, int s, int* 
                                    int* n_host, void* stream);
 
 /* ---- get_batch_statistics (utils/utils.py:184-230): true-positive flags of NMS output rows ----------------
- * dets [N,max_det,6] / counts [N] as yfv2_nms writes them; targets [nt,6] rows (image, class, x1, y1, x2, y2) in
- * pixels (what evaluation() builds at utils/utils.py:372-375), nt <= 8192.  tp [N,max_det] receives 1.0 for a true
+ * dets [N,max_det,6] / counts [N] as yfv2_nms writes them (a count above max_det is taken as max_det); targets [nt,6]
+ * rows (image, class, x1, y1, x2, y2) in pixels (what evaluation() builds at utils/utils.py:372-375), in any order and
+ * any number (an image claims at most max_det of its annotations, and that claim list is all the state kept per image).
+ * max_det <= YFV2_EVAL_MAX_DET, else YFV2_EUNSUPPORTED before the launch.  tp [N,max_det] receives 1.0 for a true
  * positive, 0.0 otherwise (rows past counts[n] are 0).  Same greedy order and the same fp32 IoU (+1 convention) as the
- * reference: bit-identical flags. */
+ * reference, and its torch max(0) choice of annotation (first maximum; a NaN IoU counts as the maximum and then fails the
+ * threshold): bit-identical flags. */
+#define YFV2_EVAL_MAX_DET 8192
 YFV2_API int yfv2_batch_statistics(const float* dets, const int* counts, int N, int max_det, const float* targets, int nt,
                                    float iou_threshold, float* tp, void* stream);
 
@@ -520,8 +524,12 @@ YFV2_API int yfv2_anchor_kmeans_step(const double* boxes, int N, int k, int R, i
 YFV2_API int yfv2_anchor_avg_iou(const double* boxes, int N, int k, int R, const double* centroids, double* avg_iou, void* stream);
 
 /* ---- whole inference step with HOST buffers (the evaluation() inner loop, utils/utils.py:367-383) ----
- * x_host: pinned uint8 [N,3,H,W]; out_host: pinned [N,max_det,6]; counts_host: pinned [N].
- * Copies in, runs forward_u8 + decode_nms, copies out, all on `stream`; returns without synchronising. */
+ * x_host: pinned uint8 [N,3,H,W]; out_host: pinned [N,max_det,6]; counts_host: pinned [N]; anchors_host: 4 * A doubles as
+ * for yfv2_decode; workspace: at least yfv2_detect_workspace_bytes(plan, max_det) device bytes (more than
+ * yfv2_plan_workspace_bytes: the input copy, the head tensors and the detections live behind the forward's workspace).
+ * Copies in, runs forward_u8 + decode_nms, copies out, all on `stream`; returns without synchronising.  Every argument
+ * yfv2_decode_nms would refuse (max_det outside 1..4096, more than YFV2_NMS_MAX_CAND candidates per image, NMS state over
+ * the shared memory) is refused with its error before anything is enqueued.  Rows past counts_host[n] are unspecified. */
 YFV2_API int yfv2_detect_u8_host(yfv2_plan* plan, const uint8_t* x_host, const void* packed,
                         const double* anchors_host, float conf_thres, double iou_thres, int max_det,
                         float* out_host, int* counts_host, void* workspace, void* stream);

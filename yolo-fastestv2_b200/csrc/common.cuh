@@ -194,6 +194,12 @@ int fpn_launch(const Launch& L, const Planes& c3, const ChanTab& t3, const Plane
 int heads_launch(const Launch& L, int half, const Planes& sIn, const Planes& tcls, const Planes& treg, const float* const wdw[2],
                  const float* const wpw[2], float* reg, float* obj, float* cls, int A, int C, int N, cudaStream_t s);
 
+// Every host-side check of yfv2_decode_nms (k_post.cu): geometry, NMS arguments and the kernel's shared memory; set_error + its
+// code on a refusal.  Callers that enqueue work before the fused decode+NMS (yfv2_detect_u8_host) run it first.
+int decode_nms_check(const float* const preds[6], int N, int H, int W, int A, int C, const double* anchors_host, float conf_thres,
+                     double iou_thres, const int* class_filter, int n_filter, int max_det, float max_wh, float* out, int* counts,
+                     int* kept_idx);
+
 // conv1x1 backward with an optional scratch for per-block partial weight gradients (k_train.cu; the C-ABI operator passes none)
 int conv1x1_bwd_impl(const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias, int N, int K, int M, int HW,
                      float* wscratch, size_t wscratch_floats, cudaStream_t s);

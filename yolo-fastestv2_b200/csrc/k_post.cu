@@ -1262,7 +1262,44 @@ int fill_nms(NmsParams& p, int M, float conf_thres, double iou_thres, const int*
     p.list_min_det = lists_always ? 0 : kNmsListMinDet;
     return YFV2_OK;
 }
+
+// The fused decode+NMS launch: kernel variant and dynamic shared memory, from checked geometry and parameters
+struct DecodeNmsLaunch {
+    PostGeom g;
+    NmsParams p;
+    void (*kern)(PostGeom, NmsParams);
+    size_t bytes;
+};
+
+int decode_nms_prepare(DecodeNmsLaunch& d, const float* const preds[6], int N, int H, int W, int A, int C, const double* anchors_host,
+                       float conf_thres, double iou_thres, const int* class_filter, int n_filter, int max_det, float max_wh, float* out,
+                       int* counts, int* kept_idx) {
+    int rc = fill_geom(d.g, preds, N, H, W, A, C, anchors_host);
+    if (rc) return rc;
+    rc = fill_nms(d.p, d.g.M, conf_thres, iou_thres, class_filter, n_filter, max_det, max_wh, out, counts, kept_idx);
+    if (rc) return rc;
+    d.p.C = C;
+    d.p.prof = g_nms_prof;
+    static const bool warp_cells = getenv("YFV2_NMS_WARP_PER_CELL") != nullptr;
+    const int fast = (C > kCT || warp_cells) ? 0 : (C == kCT && A == 3) ? 2 : 1;
+    static void (*const kernels[2][3])(PostGeom, NmsParams) = {
+        {decode_nms_kernel<false, 0>, decode_nms_kernel<false, 1>, decode_nms_kernel<false, 2>},
+        {decode_nms_kernel<true, 0>, decode_nms_kernel<true, 1>, decode_nms_kernel<true, 2>}};
+    d.kern = kernels[d.p.prof != nullptr][fast];
+    // the warp-per-cell path stages 5A+C logits of 32 cells behind the NMS state
+    d.bytes = nms_smem_bytes(d.p.M, d.p.MCp, d.p.max_det) + (fast ? 0 : (size_t)(5 * A + C) * kSStride * sizeof(float));
+    if (d.bytes > kSmemCap) { set_error("decode_nms: %zu bytes of shared memory needed", d.bytes); return YFV2_EUNSUPPORTED; }
+    return YFV2_OK;
+}
 }  // namespace
+
+int decode_nms_check(const float* const preds[6], int N, int H, int W, int A, int C, const double* anchors_host, float conf_thres,
+                     double iou_thres, const int* class_filter, int n_filter, int max_det, float max_wh, float* out, int* counts,
+                     int* kept_idx) {
+    DecodeNmsLaunch d;
+    return decode_nms_prepare(d, preds, N, H, W, A, C, anchors_host, conf_thres, iou_thres, class_filter, n_filter, max_det, max_wh,
+                              out, counts, kept_idx);
+}
 }  // namespace yfv2
 
 using namespace yfv2;
@@ -1319,32 +1356,19 @@ extern "C" int yfv2_decode_nms(const float* const preds[6], int N, int H, int W,
                                float conf_thres, double iou_thres, const int* class_filter, int n_filter, int max_det,
                                float max_wh, float* out, int* counts, int* kept_idx, void* workspace, void* stream) {
     (void)workspace;
-    PostGeom g;
-    int rc = fill_geom(g, preds, N, H, W, A, C, anchors_host);
+    DecodeNmsLaunch d;
+    const int rc = decode_nms_prepare(d, preds, N, H, W, A, C, anchors_host, conf_thres, iou_thres, class_filter, n_filter, max_det,
+                                      max_wh, out, counts, kept_idx);
     if (rc) return rc;
-    NmsParams p;
-    rc = fill_nms(p, g.M, conf_thres, iou_thres, class_filter, n_filter, max_det, max_wh, out, counts, kept_idx);
-    if (rc) return rc;
-    p.C = C;
-    p.prof = g_nms_prof;
-    static const bool warp_cells = getenv("YFV2_NMS_WARP_PER_CELL") != nullptr;
-    const int fast = (C > kCT || warp_cells) ? 0 : (C == kCT && A == 3) ? 2 : 1;
-    static void (*const kernels[2][3])(PostGeom, NmsParams) = {
-        {decode_nms_kernel<false, 0>, decode_nms_kernel<false, 1>, decode_nms_kernel<false, 2>},
-        {decode_nms_kernel<true, 0>, decode_nms_kernel<true, 1>, decode_nms_kernel<true, 2>}};
-    void (*const kern)(PostGeom, NmsParams) = kernels[p.prof != nullptr][fast];
-    // the warp-per-cell path stages 5A+C logits of 32 cells behind the NMS state
-    const size_t bytes = nms_smem_bytes(p.M, p.MCp, p.max_det) + (fast ? 0 : (size_t)(5 * A + C) * kSStride * sizeof(float));
-    if (bytes > kSmemCap) { set_error("decode_nms: %zu bytes of shared memory needed", bytes); return YFV2_EUNSUPPORTED; }
-    YFV2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    YFV2_CUDA(cudaFuncSetAttribute(d.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d.bytes));
     {   // nothing is read before pdl_wait(), so overlapping the predecessor's tail is always safe
         cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3((unsigned)N); cfg.blockDim = dim3(NT); cfg.dynamicSmemBytes = bytes; cfg.stream = (cudaStream_t)stream;
+        cfg.gridDim = dim3((unsigned)N); cfg.blockDim = dim3(NT); cfg.dynamicSmemBytes = d.bytes; cfg.stream = (cudaStream_t)stream;
         cudaLaunchAttribute at[1];
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = at; cfg.numAttrs = pdl_allowed() ? 1 : 0;
-        YFV2_CUDA(cudaLaunchKernelEx(&cfg, kern, g, p));
+        YFV2_CUDA(cudaLaunchKernelEx(&cfg, d.kern, d.g, d.p));
     }
     YFV2_LAUNCH_CHECK();
     return YFV2_OK;

@@ -637,6 +637,9 @@ extern "C" int yfv2_detect_u8_host(yfv2_plan* p, const uint8_t* x_host, const vo
     for (int i = 0; i < 6; ++i) preds[i] = (float*)(ws + L.off_pred[i]);
     float* out_dev = (float*)(ws + L.off_out);
     int* counts_dev = (int*)(ws + L.off_counts);
+    // a request the fused decode+NMS refuses is refused here, before the copy and the forward are enqueued
+    TRY(decode_nms_check(preds, p->N, p->H, p->W, p->A, p->C, anchors_host, conf_thres, iou_thres, nullptr, 0, max_det, 4096.0f,
+                         out_dev, counts_dev, nullptr));
     YFV2_CUDA(cudaMemcpyAsync(x_dev, x_host, (size_t)p->N * 3 * p->H * p->W, cudaMemcpyHostToDevice, s));
     struct PdlOff { PdlOff() { g_pdl_call = false; } ~PdlOff() { g_pdl_call = true; } } pdl_off_guard;
     TRY(forward_impl(p, x_dev, 1, packed, preds, ws, 0, -1, s));

@@ -599,7 +599,22 @@ class Plan:
         return out
 
     def detect_u8_host(self, x_host, anchors, conf_thres, iou_thres, out_host, counts_host, max_det=MAX_DET):
-        """Whole step from pinned host uint8 images to pinned host detections (asynchronous)."""
+        """Whole step from pinned host uint8 images to pinned host detections (asynchronous).  x_host: uint8 [N,3,H,W], out_host:
+        float32 [N,max_det,6], counts_host: int32 [N], contiguous CPU tensors (pinned, so that the copies overlap); anchors: the
+        4*A doubles of anchors_array.  The plan must have been built with detect_max_det >= max_det."""
+        for t, name, dtype, shape in ((x_host, "x_host", torch.uint8, (self.N, 3, self.H, self.W)),
+                                      (out_host, "out_host", torch.float32, (self.N, max_det, 6)),
+                                      (counts_host, "counts_host", torch.int32, (self.N,))):
+            if (not isinstance(t, torch.Tensor) or t.device.type != "cpu" or t.dtype != dtype or tuple(t.shape) != shape
+                    or not t.is_contiguous()):
+                got = "%s %s on %s" % (t.dtype, tuple(t.shape), t.device) if isinstance(t, torch.Tensor) else type(t).__name__
+                raise Yfv2Error("detect_u8_host: %s must be a contiguous host tensor %s %s, got %s" % (name, dtype, shape, got))
+        if not isinstance(anchors, ctypes.Array) or anchors._type_ is not ctypes.c_double or len(anchors) < 4 * self.A:
+            raise Yfv2Error("detect_u8_host: anchors must be %d doubles (anchors_array)" % (4 * self.A))
+        need = lib().yfv2_detect_workspace_bytes(self._h, max_det)
+        if max_det > 0 and self.workspace.numel() < need:
+            raise Yfv2Error("detect_u8_host: max_det=%d needs a %d-byte workspace, the plan has %d (build it with detect_max_det >= %d)"
+                            % (max_det, need, self.workspace.numel(), max_det))
         with torch.cuda.device(self.device):
             _check(lib().yfv2_detect_u8_host(self._h, ctypes.c_void_p(x_host.data_ptr()), ctypes.c_void_p(self.packed.data_ptr()),
                                              anchors, ctypes.c_float(conf_thres), ctypes.c_double(iou_thres), max_det,
