@@ -12,16 +12,18 @@
 // LDS.128, i.e. 2592 FFMA against ~190 shared-memory instructions (93 % FFMA in the main loop).
 //
 // A work item is (image, band of TRo pooled rows, tile of TWo <= 44 pooled columns):
-//   0. fp32: the input patch arrives by one TMA bulk copy per (channel, row), issued after the previous item's conv, while it
-//      pools.  uint8: the raw bytes of the next item arrive by 16-byte cp.async (zero-filled outside the image) in the half of
-//      Hs that is free during the conv, issued before the conv; after it they are converted into Xin through a 256-entry
+//   0. fp32: the input patch arrives in Xin by one TMA bulk copy per (channel, row), issued after the previous item's conv.
+//      uint8: the raw bytes arrive by 16-byte cp.async (zero-filled outside the image) in one of two byte patches, issued
+//      while the previous item convolves from the other; each conv thread converts the bytes it reads through a 256-entry
 //      table of v / 255.0f (one correctly rounded division per byte value, so no per-pixel division).  A base that is not
-//      16-byte aligned (or, for uint8, W not a multiple of 16): scalar loads after the conv;
+//      16-byte aligned (or, for uint8, W not a multiple of 16): scalar loads at the same points;
 //   1. conv + BN (scale folded into the weights, shift = accumulator init) for the CR = 2 TRo + 1 conv rows the pool
 //      windows touch; positions outside the conv output become -inf (PyTorch pads max_pool2d with -inf);
-//   2. horizontal 3-max in registers (the one column a thread lacks comes from its right neighbour through shared
-//      memory), vertical 3-max + ReLU from shared memory -> framed output planes.  ReLU commutes with max, so it runs
-//      once per pooled value instead of once per conv value.
+//   2. horizontal 3-max in registers (the one column a thread lacks comes from the next lane by a shuffle, or from the next
+//      warp through shared memory) -> Hs;
+//   3. vertical 3-max + ReLU from Hs -> framed output planes, while the next item convolves.  ReLU commutes with max, so it
+//      runs once per pooled value instead of once per conv value.
+// Two barriers per item: B0 (patch staged, Hs complete) and B1 (patch and Hs read, Eb written).
 #include "common.cuh"
 #include "tc.cuh"
 
@@ -32,6 +34,10 @@ using namespace tc;
 
 constexpr int ST_THREADS = 256;
 constexpr int kStemW = 27 * 24 + 24;              // folded weights [27][24] | shift[24]
+constexpr int kStemE = (ST_THREADS / 32) * 24;    // one conv column per warp, passed to the warp before
+// copies of the byte -> float table: lane l reads copy l % 16, so two lanes of a warp share a bank only when they are 16 apart
+// and their bytes differ with the same parity (at most 2 wavefronts per table read, 1.5 on random bytes)
+constexpr int kLutCopies = 16;
 
 struct StemFArgs {
     const void* x;
@@ -56,23 +62,22 @@ stem_kernel(const __grid_constant__ StemFArgs p) {
     __shared__ __align__(8) uint64_t xbar;
     const int TRo = p.TRo, TWo = p.TWo, S = p.S;
     const int CR = 2 * TRo + 1, IR = 4 * TRo + 3, Wst = 4 * TWo + 12;     // staged column 0 <-> input column 4*ox0 - 4
-    const int HSW = 2 * S;
+    const int HSW = 2 * S, Wb = stem_byte_row(TWo);
     float* sW = smem;                                  // folded weights + shift
-    float* lut = sW + kStemW;                          // [256] byte v -> v / 255.0f
-    float* Xin = lut + 256;                            // [3][IR][Wst]
-    float* Hs = Xin + 3 * IR * Wst;                    // [24][CR][HSW] horizontal maxima; its head doubles as
-    float* E = Hs;                                     // [24][CR][S]   first conv column of every strip
-    // [3][IR][Wb] raw uint8 patch of the next item, in the half of Hs that is free from B0 until B2 (E is the other half)
-    const int Wb = stem_byte_row(TWo);
-    uint8_t* Xb = reinterpret_cast<uint8_t*>(Hs + 24 * CR * S);
-    const int tid = threadIdx.x;
+    float* Eb = sW + kStemW;                           // [8 warps][24] first conv column of each warp's lane 0
+    float* Hs = Eb + kStemE;                           // [24][CR][HSW] horizontal maxima of the last convolved item
+    float* Xin = Hs + 24 * CR * HSW;                   // fp32: [3][IR][Wst] input patch
+    float* lut = Xin;                                  // uint8: [256][kLutCopies] byte v -> v / 255.0f, one copy per bank pair
+    uint8_t* Xb = reinterpret_cast<uint8_t*>(lut + 256 * kLutCopies);   // uint8: two [3][IR][Wb] raw patches
+    const int xbytes = 3 * IR * Wb;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     {   // BN scale folded into the weights (one rounding per weight), shift kept as the accumulator's start value
         const float* scale = p.wpack + 27 * 24;
         for (int i = tid; i < 27 * 24; i += ST_THREADS) sW[i] = __fmul_rn(__ldg(p.wpack + i), __ldg(scale + (i % 24)));
         if (tid < 24) sW[27 * 24 + tid] = __ldg(scale + 24 + tid);
         // the `/255.0` of utils/utils.py:368 as a table: the same correctly rounded quotient without a division per pixel
         if (U8)
-            for (int v = tid; v < 256; v += ST_THREADS) lut[v] = __fdiv_rn((float)v, 255.0f);
+            for (int i = tid; i < 256 * kLutCopies; i += ST_THREADS) lut[i] = __fdiv_rn((float)(i / kLutCopies), 255.0f);
     }
     if (tid == 0) { mbar_init(&xbar, 1); fence_mbar_init(); }
     __syncthreads();
@@ -80,25 +85,50 @@ stem_kernel(const __grid_constant__ StemFArgs p) {
     const int H = p.H, W = p.W, HC = H / 2, WC = W / 2, HO = H / 4, WO = W / 4;
     const int items = p.N * p.tilesX * p.tilesY;
 
-    auto stage = [&](int item) {
+    // the input patch of `item`: uint8 into the raw patch xb, fp32 into Xin
+    auto stage = [&](int item, uint8_t* xb) {
         const int n = item / (p.tilesX * p.tilesY);
         const int rem = item - n * (p.tilesX * p.tilesY);
         const int ty = rem / p.tilesX, tx = rem - ty * p.tilesX;
         const int iy0 = 4 * (ty * TRo) - 3, ic0 = 4 * (tx * TWo) - 4;
-        const int c_lo = max(ic0, 0), c_hi = min(ic0 + Wst, W);
-        if (!p.vec) {
+        if (U8) {
+            // rows of Wb bytes that start at input column a0 = ic0 & ~15, so staged column j is byte (ic0 - a0) + j of its row
+            const uint8_t* x8 = reinterpret_cast<const uint8_t*>(p.x);
+            const int a0 = ic0 & ~15;
+            if (p.vec) {
+                // 16 bytes per cp.async, a row per 16 threads, every copy in flight at once.  The base and W are multiples of
+                // 16, so a chunk lies wholly inside or wholly outside the image; outside ones are zero-filled (byte 0 -> 0.f)
+                const int j = tid & 15;
+                if (j < Wb / 16) {
+                    int c = 0, r = tid >> 4;
+                    for (int cr = r; cr < 3 * IR; cr += ST_THREADS / 16, r += ST_THREADS / 16) {
+                        while (r >= IR) { r -= IR; ++c; }
+                        const int iy = iy0 + r, ix = a0 + 16 * j;
+                        const bool in = iy >= 0 && iy < H && ix >= 0 && ix < W;
+                        cp_async16_zfill(xb + cr * Wb + 16 * j, in ? x8 + (((size_t)n * 3 + c) * H + iy) * W + ix : x8, in ? 16u : 0u);
+                    }
+                }
+            } else {
+                for (int i = tid; i < 3 * IR * Wst; i += ST_THREADS) {
+                    const int cr = i / Wst, j = i - cr * Wst;
+                    const int c = cr / IR, r = cr - c * IR;
+                    const int iy = iy0 + r, ix = ic0 + j;
+                    uint8_t v = 0;
+                    if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = __ldg(x8 + (((size_t)n * 3 + c) * H + iy) * W + ix);
+                    xb[cr * Wb + (ic0 - a0) + j] = v;
+                }
+            }
+        } else if (!p.vec) {
             for (int i = tid; i < 3 * IR * Wst; i += ST_THREADS) {
                 const int cr = i / Wst, j = i - cr * Wst;
                 const int c = cr / IR, r = cr - c * IR;
                 const int iy = iy0 + r, ix = ic0 + j;
                 float v = 0.f;
-                if (iy >= 0 && iy < H && ix >= 0 && ix < W) {
-                    const size_t idx = (((size_t)n * 3 + c) * H + iy) * W + ix;
-                    v = U8 ? lut[__ldg(reinterpret_cast<const uint8_t*>(p.x) + idx)] : __ldg(reinterpret_cast<const float*>(p.x) + idx);
-                }
+                if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = __ldg(reinterpret_cast<const float*>(p.x) + (((size_t)n * 3 + c) * H + iy) * W + ix);
                 Xin[i] = v;
             }
-        } else if (!U8) {
+        } else {
+            const int c_lo = max(ic0, 0), c_hi = min(ic0 + Wst, W);
             const int r_lo = max(iy0, 0), r_hi = min(iy0 + IR, H);
             if (tid == 0) mbar_expect_tx(&xbar, (uint32_t)(3 * (r_hi - r_lo) * (c_hi - c_lo) * sizeof(float)));
             for (int i = tid; i < 3 * IR; i += ST_THREADS) {
@@ -114,59 +144,50 @@ stem_kernel(const __grid_constant__ StemFArgs p) {
                     for (int j = 0; j < Wst; ++j) dst[j] = 0.f;
                 }
             }
-        } else {
-            // raw bytes -> Xb rows of Wb bytes that start at input column ic0 & ~15, 16 per cp.async: every copy in flight at
-            // once.  The base and W are multiples of 16, so a chunk lies wholly inside or wholly outside the image; outside
-            // ones are zero-filled (byte 0 converts to 0.f)
-            const uint8_t* x8 = reinterpret_cast<const uint8_t*>(p.x);
-            const int a0 = ic0 & ~15, q16 = Wb / 16;
-            for (int i = tid; i < 3 * IR * q16; i += ST_THREADS) {
-                const int cr = i / q16, j = i - cr * q16;
-                const int c = cr / IR, r = cr - c * IR;
-                const int iy = iy0 + r, ix = a0 + 16 * j;
-                const bool in = iy >= 0 && iy < H && ix >= 0 && ix < W;
-                cp_async16_zfill(Xb + 16 * i, in ? x8 + (((size_t)n * 3 + c) * H + iy) * W + ix : x8, in ? 16u : 0u);
-            }
         }
     };
-    // uint8 with aligned base: Xb (complete, after a barrier) -> Xin, 4 pixels per step
-    auto convert = [&](int item) {
-        const int tx = item % p.tilesX;
-        const int off = (4 * (tx * TWo) - 4) & 15;           // ic0 - (ic0 & ~15)
-        const int q4 = Wst / 4;
-        for (int i = tid; i < 3 * IR * q4; i += ST_THREADS) {
-            const int cr = i / q4, j4 = i - cr * q4;
-            const uint32_t b = *reinterpret_cast<const uint32_t*>(Xb + cr * Wb + off + 4 * j4);
-            *reinterpret_cast<float4*>(Xin + 4 * i) = make_float4(lut[b & 255u], lut[(b >> 8) & 255u], lut[(b >> 16) & 255u], lut[b >> 24]);
-        }
-    };
-    const bool async_u8 = U8 && p.vec;
 
     const int r = tid / S, s = tid - r * S;                  // conv row of the band / strip of 4 conv columns
     const int p_oyl = tid / TWo, p_pc = tid - p_oyl * TWo;   // pooled pixel this thread writes in step 3
-    uint32_t xpar = 0;
-    if (blockIdx.x < items) {
-        stage(blockIdx.x);
-        if (async_u8) {
-            cp_async_wait_all();
-            __syncthreads();
-            convert(blockIdx.x);
-        }
-    }
-    for (int item = blockIdx.x; item < items; item += gridDim.x) {
+    // ---- 3. vertical 3-max + ReLU of `item` from Hs -> output planes: thread <-> pooled pixel, loop over the channels ------
+    auto pool = [&](int item) {
         const int n = item / (p.tilesX * p.tilesY);
         const int rem = item - n * (p.tilesX * p.tilesY);
         const int ty = rem / p.tilesX, tx = rem - ty * p.tilesX;
         const int oy0 = ty * TRo, ox0 = tx * TWo;
-        const int rows = min(TRo, HO - oy0), cols = min(TWo, WO - ox0);
+        if (p_oyl < min(TRo, HO - oy0) && p_pc < min(TWo, WO - ox0)) {
+            const float* hb = Hs + (2 * p_oyl) * HSW + p_pc;
+            float* op = plane_ptr(p.out, n, 0) + p.out.org + (oy0 + p_oyl) * p.out.Ws + ox0 + p_pc;
+            const int hstep = CR * HSW;
+            const size_t ostep = (size_t)p.out.sC;
+#pragma unroll 4
+            for (int ch = 0; ch < 24; ++ch) {
+                *op = fmaxf(max3(hb[0], hb[HSW], hb[2 * HSW]), 0.f);
+                hb += hstep;
+                op += ostep;
+            }
+        }
+    };
+    const float* lt = lut + (lane & (kLutCopies - 1));       // this lane's copy of the table
+    uint32_t xpar = 0;
+    if (blockIdx.x < items) stage(blockIdx.x, Xb);
+    int buf = 0;
+    for (int item = blockIdx.x; item < items; item += gridDim.x, buf ^= 1) {
+        const int n = item / (p.tilesX * p.tilesY);
+        const int rem = item - n * (p.tilesX * p.tilesY);
+        const int ty = rem / p.tilesX, tx = rem - ty * p.tilesX;
+        const int oy0 = ty * TRo, ox0 = tx * TWo;
+        const int rows = min(TRo, HO - oy0);
         const bool active = r < 2 * rows + 1;
-        if (!U8 && p.vec) { mbar_wait(&xbar, xpar); xpar ^= 1u; }
-        __syncthreads();                                      // B0: edge zero-fill / converted uint8 visible; Hs free again
+        if (U8 && p.vec) cp_async_wait_all();                // this thread's bytes of the item have landed
+        __syncthreads();                                      // B0: the item's patch is staged; Hs holds the previous item
         const bool more = item + gridDim.x < items;
-        if (async_u8 && more) stage(item + gridDim.x);        // the next item's bytes arrive while this one convolves
+        if (U8 && more) stage(item + gridDim.x, Xb + (buf ^ 1) * xbytes);   // arrives while this item convolves
+        if (item != blockIdx.x) pool(item - gridDim.x);
+        if (!U8 && p.vec) { mbar_wait(&xbar, xpar); xpar ^= 1u; }
 
         // ---- 1. conv: acc[j][ch], j = position 4s+j of conv row r (tile-local) ----------------------------------------
-        float h0[24], h1[24];
+        float h0[24], h1[24], e0[24];
         if (active) {
             // accumulators as channel pairs, read from shared memory as float4 / float2 weight vectors
             float2 acc2[4][12];
@@ -176,18 +197,35 @@ stem_kernel(const __grid_constant__ StemFArgs p) {
 #pragma unroll
                 for (int j = 0; j < 4; ++j) acc2[j][m] = sh;
             }
-            const float* xb = Xin + (2 * r) * Wst + 8 * s;   // staged col of (position j, tap kx) = 8s + 2j + kx + 1
+            // staged col of (position j, tap kx) = 8s + 2j + kx + 1
+            const float* xf = Xin + (2 * r) * Wst + 8 * s;
+            const uint8_t* x8 = Xb + buf * xbytes + (2 * r) * Wb + ((4 * ox0 - 4) & 15) + 8 * s;
 #pragma unroll
             for (int c = 0; c < 3; ++c) {
 #pragma unroll
                 for (int ky = 0; ky < 3; ++ky) {
-                    float x[12];
-                    const float4* xr = reinterpret_cast<const float4*>(xb + (c * IR + ky) * Wst);
-#pragma unroll
-                    for (int t = 0; t < 3; ++t) { const float4 v = xr[t]; x[4 * t] = v.x; x[4 * t + 1] = v.y; x[4 * t + 2] = v.z; x[4 * t + 3] = v.w; }
+                    float x[9];                               // staged cols 8s + 1 .. 8s + 9
+                    if constexpr (U8) {
+                        // bytes 1 .. 9 of three aligned words, each converted by the lane's copy of the table
+                        const uint32_t* xw = reinterpret_cast<const uint32_t*>(x8 + (c * IR + ky) * Wb);
+                        const uint32_t b0 = xw[0], b1 = xw[1], b2 = xw[2];
+                        x[0] = lt[((b0 >> 8) & 255u) * kLutCopies];
+                        x[1] = lt[((b0 >> 16) & 255u) * kLutCopies];
+                        x[2] = lt[(b0 >> 24) * kLutCopies];
+                        x[3] = lt[(b1 & 255u) * kLutCopies];
+                        x[4] = lt[((b1 >> 8) & 255u) * kLutCopies];
+                        x[5] = lt[((b1 >> 16) & 255u) * kLutCopies];
+                        x[6] = lt[(b1 >> 24) * kLutCopies];
+                        x[7] = lt[(b2 & 255u) * kLutCopies];
+                        x[8] = lt[((b2 >> 8) & 255u) * kLutCopies];
+                    } else {
+                        const float4* xr = reinterpret_cast<const float4*>(xf + (c * IR + ky) * Wst);
+                        const float4 v0 = xr[0], v1 = xr[1], v2 = xr[2];
+                        x[0] = v0.y; x[1] = v0.z; x[2] = v0.w; x[3] = v1.x; x[4] = v1.y; x[5] = v1.z; x[6] = v1.w; x[7] = v2.x; x[8] = v2.y;
+                    }
                     float2 xx[9];
 #pragma unroll
-                    for (int t = 0; t < 9; ++t) xx[t] = make_float2(x[t + 1], x[t + 1]);
+                    for (int t = 0; t < 9; ++t) xx[t] = make_float2(x[t], x[t]);
 #pragma unroll
                     for (int kx = 0; kx < 3; ++kx) {
                         const float4* wr = reinterpret_cast<const float4*>(sW + ((c * 3 + ky) * 3 + kx) * 24);
@@ -225,53 +263,47 @@ stem_kernel(const __grid_constant__ StemFArgs p) {
             // horizontal 3-max, part 1: pooled column 2s <- positions 0,1,2; 2s+1 <- positions 2,3 (+ the neighbour's 0 below)
 #pragma unroll
             for (int ch = 0; ch < 24; ++ch) {
-                E[(ch * CR + r) * S + s] = acc[0][ch];
+                e0[ch] = acc[0][ch];
                 h0[ch] = max3(acc[0][ch], acc[1][ch], acc[2][ch]);
                 h1[ch] = fmaxf(acc[2][ch], acc[3][ch]);
             }
         }
-        if (async_u8 && more) cp_async_wait_all();          // this thread's bytes of the next item have landed
-        __syncthreads();                                      // B1: every read of Xin is done, E and Xb are visible
-        if (async_u8 && more) {
-            convert(item + gridDim.x);
-        } else if (more) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of Xin before the async-proxy refill
-            stage(item + gridDim.x);                          // overlaps the pooling below
-        }
-        if (active && s + 1 < S) {
+        // ---- 2. part 2: strip s + 1 (thread tid + 1) is the next lane, or lane 0 of the next warp through Eb ----------------
+        const bool right = active && s + 1 < S;
 #pragma unroll
-            for (int ch = 0; ch < 24; ++ch) h1[ch] = fmaxf(h1[ch], E[(ch * CR + r) * S + s + 1]);
+        for (int ch = 0; ch < 24; ++ch) {
+            const float nb = __shfl_down_sync(0xffffffffu, e0[ch], 1);
+            if (right && lane != 31) h1[ch] = fmaxf(h1[ch], nb);
         }
-        __syncthreads();                                      // B2: E has been read, Hs may overwrite it
+        if (active && lane == 0) {
+#pragma unroll
+            for (int ch = 0; ch < 24; ++ch) Eb[warp * 24 + ch] = e0[ch];
+        }
+        __syncthreads();                                      // B1: every read of the patch and of Hs is done, Eb is visible
+        if (!U8 && more) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of Xin before the async-proxy refill
+            stage(item + gridDim.x, nullptr);                 // lands while this item's maxima are written and pooled
+        }
+        if (right && lane == 31) {
+#pragma unroll
+            for (int ch = 0; ch < 24; ++ch) h1[ch] = fmaxf(h1[ch], Eb[(warp + 1) * 24 + ch]);
+        }
         if (active) {
 #pragma unroll
             for (int ch = 0; ch < 24; ++ch)
                 *reinterpret_cast<float2*>(Hs + (ch * CR + r) * HSW + 2 * s) = make_float2(h0[ch], h1[ch]);
         }
-        __syncthreads();                                      // B3
-        // ---- 3. vertical 3-max + ReLU -> output planes: thread <-> pooled pixel of the tile, loop over the channels --------
-        if (p_oyl < rows && p_pc < cols) {
-            const float* hb = Hs + (2 * p_oyl) * HSW + p_pc;
-            float* op = plane_ptr(p.out, n, 0) + p.out.org + (oy0 + p_oyl) * p.out.Ws + ox0 + p_pc;
-            const int hstep = CR * HSW;
-            const size_t ostep = (size_t)p.out.sC;
-#pragma unroll 4
-            for (int ch = 0; ch < 24; ++ch) {
-                *op = fmaxf(max3(hb[0], hb[HSW], hb[2 * HSW]), 0.f);
-                hb += hstep;
-                op += ostep;
-            }
-        }
+    }
+    if (blockIdx.x < items) {                                 // the CTA's last item
+        __syncthreads();
+        pool(blockIdx.x + (items - 1 - (int)blockIdx.x) / (int)gridDim.x * gridDim.x);
     }
 }
 
-__host__ size_t stem_smem_bytes(int TRo, int TWo, int S) {
+__host__ size_t stem_smem_bytes(int TRo, int TWo, int S, bool u8) {
     const int CR = 2 * TRo + 1, IR = 4 * TRo + 3, Wst = 4 * TWo + 12;
-    return (size_t)(kStemW + 256 + 3 * IR * Wst + 24 * CR * 2 * S + 4) * sizeof(float);
-}
-// the uint8 patch fits the half of Hs that E leaves free
-__host__ bool stem_bytes_fit(int TRo, int TWo, int S) {
-    return 3 * (4 * TRo + 3) * stem_byte_row(TWo) <= 24 * (2 * TRo + 1) * S * (int)sizeof(float);
+    const size_t head = (size_t)(kStemW + kStemE + 24 * CR * 2 * S) * sizeof(float);
+    return head + (u8 ? 256 * kLutCopies * sizeof(float) + 2 * (size_t)(3 * IR * stem_byte_row(TWo)) : 3 * (size_t)(IR * Wst) * sizeof(float));
 }
 }  // namespace
 
@@ -296,12 +328,12 @@ int describe_stem(int N, int H, int W, int is_u8, int sms, Launch& L) {
     // as many conv rows as the 256 threads cover, within ~half an SM's shared memory (two CTAs per SM)
     k.TRo = (ST_THREADS / k.S - 1) / 2;
     if (k.TRo > HO) k.TRo = HO;
-    while (k.TRo > 1 && stem_smem_bytes(k.TRo, k.TWo, k.S) > 112 * 1024) --k.TRo;
+    while (k.TRo > 1 && stem_smem_bytes(k.TRo, k.TWo, k.S, is_u8) > 112 * 1024) --k.TRo;
     if (k.TRo < 1) k.TRo = 1;
-    const size_t bytes = stem_smem_bytes(k.TRo, k.TWo, k.S);
+    const size_t bytes = stem_smem_bytes(k.TRo, k.TWo, k.S, is_u8);
     if ((2 * k.TRo + 1) * k.S > ST_THREADS || k.TRo * k.TWo > ST_THREADS || bytes > kSmemCap - 1024) { set_error("stem: unsupported geometry %dx%d", H, W); return YFV2_EUNSUPPORTED; }
-    // asynchronous staging needs 16-byte aligned rows (uint8: and room for the bytes); other inputs take the scalar loads
-    k.vec = !is_u8 || (W % 16 == 0 && stem_bytes_fit(k.TRo, k.TWo, k.S));
+    // asynchronous staging needs 16-byte aligned rows; other inputs take the scalar loads
+    k.vec = !is_u8 || W % 16 == 0;
     k.tilesY = (HO + k.TRo - 1) / k.TRo;
     L.kernel = is_u8 ? KernelId::stem_u8 : KernelId::stem_f32;
     L.smem = bytes;
