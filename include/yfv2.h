@@ -107,7 +107,28 @@ YFV2_API int yfv2_export_heads(const float* const preds[6], int N, int H, int W,
  * inputWidth); anchors_host: 2*A*2 floats (the sample's `bias`, :34-37); scale_w/h: source image size / network input size
  * (:189-190).  Outputs per image, descending score: boxes [N,max_out,4] int32 (x1,y1,x2,y2), scores [N,max_out], cates
  * [N,max_out] int32, counts [N] = number kept (rows past min(count, max_out): zeros / cate -1; the sample has no cap, so pass
- * max_out = A*(H/16*W/16 + H/32*W/32) to never truncate).  Equal scores keep push order (the sample's std::sort leaves it open). */
+ * max_out = A*(H/16*W/16 + H/32*W/32) to never truncate).
+ *   Categories: the first strict maximum of cls*obj above 0, so among equal products the smaller class wins and NaN products
+ *   are skipped; a cell with none has score -1, cate -1 and is a candidate iff -1 > thresh (those suppress each other as a
+ *   class of their own).
+ *   Ties: equal scores keep push order (level, row, column, anchor).  The sample's std::sort leaves that order open; libstdc++'s
+ *   gives push order too while at most 16 candidates pass (insertion sort, stable).
+ *   Corners: each (c -/+ w/2)*scale in double becomes an int by yfv2_ncnn_corner below: truncation toward zero, and INT_MIN
+ *   for NaN or a truncated value outside the int range (what the sample's `int = double` compiles to on x86-64, cvttsd2si).
+ *   Box widths and intersections of such corners are int differences that wrap.
+ *   Limits: A <= 8, 1 <= C <= 32767, H and W multiples of 32, max_out >= 1 (else YFV2_EINVAL); the M = A*(H/16*W/16 +
+ *   H/32*W/32) candidate slots of one image are sorted and suppressed in one CTA's shared memory (about 20 bytes per slot
+ *   plus 8 per slot of M rounded up to a power of two, at most 227 KiB: A=3 up to 672x672, A=1 up to 1184x1184, A=8 up to
+ *   416x416), a larger M is YFV2_EUNSUPPORTED before anything is launched.  out3 must hold N*(H/32)*(W/32)*(5A+C) floats. */
+#ifdef __CUDACC__
+#define YFV2_HOST_DEVICE __host__ __device__
+#else
+#define YFV2_HOST_DEVICE
+#endif
+#include <limits.h>
+static inline YFV2_HOST_DEVICE int yfv2_ncnn_corner(double v) {
+    return (v > -2147483649.0 && v < 2147483648.0) ? (int)v : INT_MIN;
+}
 YFV2_API int yfv2_ncnn_post(const float* out2, const float* out3, int N, int H, int W, int A, int C, const float* anchors_host,
                             float thresh, float nms_thresh, float scale_w, float scale_h, int max_out, int* boxes, float* scores,
                             int* cates, int* counts, void* stream);

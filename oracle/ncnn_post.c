@@ -10,12 +10,16 @@
  * Pinned: tests/golden/ncnn_post.npz holds outputs of the reference's own C++ (compiled in place by `make ref`, stub ncnn /
  * OpenCV headers in oracle/ncnn_shim/) and tests/test_ncnn_post_cpu.py checks this restatement against them bit for bit.
  * One stated difference: the reference orders candidates with std::sort, whose order among EQUAL scores is unspecified; here
- * ties keep push order (level, row, column, anchor).  The golden generator asserts that no two candidates tie.
+ * ties keep push order (level, row, column, anchor), which libstdc++'s sort also gives while at most 16 candidates pass.
+ * Box corners go through yfv2_ncnn_corner (include/yfv2.h), the sample's `int = double` as compiled for x86-64 (INT_MIN for NaN
+ * and out-of-range values), so this restatement gives the same corners on every host; int differences of corners wrap.
  *
- * Build with -ffp-contract=off.
+ * Build with -ffp-contract=off -fwrapv.
  */
 #include <math.h>
 #include <stdlib.h>
+
+#include "yfv2.h"
 
 typedef struct { int x1, y1, x2, y2, cate; float score; int order; } tbox;
 
@@ -72,10 +76,10 @@ int oracle_ncnn_post(const float *out2, int h2, int w2, const float *out3, int h
                         float bw = (float)((tw * tw) * (double)anchors[(i * A * 2) + b * 2 + 0]);          /* pow(x, 2) is exact here */
                         float bh = (float)((th * th) * (double)anchors[(i * A * 2) + b * 2 + 1]);
                         tbox t;
-                        t.x1 = (int)(((double)bcx - 0.5 * (double)bw) * (double)scale_w);                  /* :170-173: double -> int truncates */
-                        t.y1 = (int)(((double)bcy - 0.5 * (double)bh) * (double)scale_h);
-                        t.x2 = (int)(((double)bcx + 0.5 * (double)bw) * (double)scale_w);
-                        t.y2 = (int)(((double)bcy + 0.5 * (double)bh) * (double)scale_h);
+                        t.x1 = yfv2_ncnn_corner(((double)bcx - 0.5 * (double)bw) * (double)scale_w);       /* :170-173: double -> int */
+                        t.y1 = yfv2_ncnn_corner(((double)bcy - 0.5 * (double)bh) * (double)scale_h);
+                        t.x2 = yfv2_ncnn_corner(((double)bcx + 0.5 * (double)bw) * (double)scale_w);
+                        t.y2 = yfv2_ncnn_corner(((double)bcy + 0.5 * (double)bh) * (double)scale_h);
                         t.score = score; t.cate = category; t.order = n;
                         tmp[n++] = t;
                     }

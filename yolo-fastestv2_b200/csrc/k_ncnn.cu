@@ -4,6 +4,7 @@
 //   getCategory        <- reference sample/ncnn/src/yolo-fastestv2.cpp:113-131  first strict maximum of cls*obj above 0
 //   predHandle         <- :134-183  ((v*2 - 0.5) + cell) * stride and (v*2)^2 * anchor in DOUBLE, rounded to float, box corners
 //                         (c -/+ 0.5 w) * scale in double, TRUNCATED to int (TargetBox has int coordinates, include/yolo-fastestv2.h:16-19)
+//                         by yfv2_ncnn_corner (include/yfv2.h): INT_MIN for NaN and out-of-range values, as x86-64's cvttsd2si
 //   intersection_area  <- :58-71    on the int corners
 //   nmsHandle          <- :78-110   descending score, greedy, a box is dropped iff IoU > thr with an earlier kept box OF ITS CLASS
 //
@@ -147,11 +148,11 @@ ncnn_post_kernel(const NcnnArgs p) {
                     const float bw = (float)__dmul_rn(__dmul_rn(tw, tw), (double)p.anchors[lv][b][0]);      // pow(x, 2) == x*x exactly
                     const float bh = (float)__dmul_rn(__dmul_rn(th, th), (double)p.anchors[lv][b][1]);
                     const double hx = __dmul_rn(0.5, (double)bw), hy = __dmul_rn(0.5, (double)bh);
-                    int4 bb;                                                                                  // :170-173, double -> int truncates
-                    bb.x = __double2int_rz(__dmul_rn(__dsub_rn((double)bcx, hx), (double)p.scale_w));
-                    bb.y = __double2int_rz(__dmul_rn(__dsub_rn((double)bcy, hy), (double)p.scale_h));
-                    bb.z = __double2int_rz(__dmul_rn(__dadd_rn((double)bcx, hx), (double)p.scale_w));
-                    bb.w = __double2int_rz(__dmul_rn(__dadd_rn((double)bcy, hy), (double)p.scale_h));
+                    int4 bb;                                          // :170-173, double -> int: truncates, INT_MIN for NaN / out of range
+                    bb.x = yfv2_ncnn_corner(__dmul_rn(__dsub_rn((double)bcx, hx), (double)p.scale_w));
+                    bb.y = yfv2_ncnn_corner(__dmul_rn(__dsub_rn((double)bcy, hy), (double)p.scale_h));
+                    bb.z = yfv2_ncnn_corner(__dmul_rn(__dadd_rn((double)bcx, hx), (double)p.scale_w));
+                    bb.w = yfv2_ncnn_corner(__dmul_rn(__dadd_rn((double)bcy, hy), (double)p.scale_h));
                     const unsigned int slot = atomicAdd(&s.misc[0], 1u);
                     s.box[slot] = bb;
                     s.area[slot] = __fmul_rn((float)(bb.z - bb.x), (float)(bb.w - bb.y));                     // TargetBox::area()

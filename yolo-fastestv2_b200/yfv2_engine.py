@@ -622,15 +622,43 @@ class Plan:
                                              ctypes.c_void_p(self.workspace.data_ptr()), _stream(self.device)), "detect_u8_host")
 
 
+def _expect_shapes(what, tensors, names, shapes):
+    """Raises Yfv2Error naming the first tensor that is not a CUDA tensor on tensors[0]'s device with the expected shape.  The
+    kernels take every extent from a few of these tensors and read the others blindly, so a mismatch would be an out-of-bounds
+    device read."""
+    dev = tensors[0].device if isinstance(tensors[0], torch.Tensor) else None
+    for t, name, want in zip(tensors, names, shapes):
+        _require_cuda(t, "%s: %s" % (what, name))
+        if t.device != dev:
+            raise Yfv2Error("%s: %s is on %s, expected %s like %s" % (what, name, t.device, dev, names[0]))
+        if tuple(t.shape) != tuple(want):
+            raise Yfv2Error("%s: %s has shape %s, expected %s" % (what, name, tuple(t.shape), tuple(want)))
+
+
+def head_geometry(what, preds):
+    """(N, h, w, A, C) of the six head tensors (reg, obj, cls of the stride-16 level, then of the stride-32 level), checked
+    against each other: preds[0] gives N, h, w, preds[1] A and preds[2] C; every tensor must match them, and the stride-32 maps
+    are (h/2, w/2) of an input whose sides are multiples of 32."""
+    if len(preds) != 6:
+        raise Yfv2Error("%s: expected preds to be the 6-tuple (reg,obj,cls) x 2 levels, got %d tensors" % (what, len(preds)))
+    for i, p in enumerate(preds):
+        _require_cuda(p, "%s: preds[%d]" % (what, i))
+        if p.dim() != 4:
+            raise Yfv2Error("%s: preds[%d] has shape %s, expected [N, channels, rows, columns]" % (what, i, tuple(p.shape)))
+    N, _, h, w = preds[0].shape
+    A, C = preds[1].shape[1], preds[2].shape[1]
+    if h % 2 or w % 2 or h == 0 or w == 0:
+        raise Yfv2Error("%s: preds[0] has shape %s: %dx%d maps are not those of an input whose sides are multiples of 32"
+                        % (what, tuple(preds[0].shape), h, w))
+    want = [(N, 4 * A, h, w), (N, A, h, w), (N, C, h, w), (N, 4 * A, h // 2, w // 2), (N, A, h // 2, w // 2), (N, C, h // 2, w // 2)]
+    _expect_shapes(what, preds, ["preds[%d]" % i for i in range(6)], want)
+    return N, h, w, A, C
+
+
 def decode(preds, cfg):
     """handel_preds on the device: returns [N, M, 5+C] fp32 CUDA tensor."""
-    for p in preds:
-        _require_cuda(p, "preds")
+    N, h, w, A, C = head_geometry("decode", preds)
     preds = [p.detach().contiguous().float() for p in preds]
-    N, A4, h, w = preds[0].shape
-    A, C = preds[1].shape[1], preds[2].shape[1]
-    if len(preds) != 6 or A4 != 4 * A:
-        raise Yfv2Error("decode: expected the 6-tuple (reg,obj,cls) x 2 levels")
     H, W = h * 16, w * 16
     if cfg is not None and (int(cfg["height"]) != H or int(cfg["width"]) != W):
         raise Yfv2Error("decode: head tensors are %dx%d/16 but cfg says %sx%s" % (H, W, cfg["height"], cfg["width"]))
@@ -672,11 +700,8 @@ def nms(dets, conf_thres=0.3, iou_thres=0.45, classes=None, max_det=MAX_DET, wan
 
 def decode_nms(preds, cfg, conf_thres=0.3, iou_thres=0.45, classes=None, max_det=MAX_DET, want_idx=False, max_wh=MAX_WH):
     """Fused handel_preds + non_max_suppression on the device (no [N,M,5+C] tensor)."""
-    for p in preds:
-        _require_cuda(p, "preds")
+    N, h, w, A, C = head_geometry("decode_nms", preds)
     preds = [p.detach().contiguous().float() for p in preds]
-    N, _, h, w = preds[0].shape
-    A, C = preds[1].shape[1], preds[2].shape[1]
     H, W = h * 16, w * 16
     dev = preds[0].device
     out = torch.empty((N, max_det, 6), dtype=torch.float32, device=dev)
@@ -1737,12 +1762,11 @@ def op(name, tensors_and_ints, device):
 
 def export_heads(preds):
     """Detector(..., export_onnx=True) output: two channel-last [N,h,w,5A+C] tensors (sigmoid / sigmoid / softmax)."""
+    N, h, w, A, C = head_geometry("export_heads", preds)
     preds = [p.detach().contiguous().float() for p in preds]
-    N, _, h, w = preds[0].shape
-    A, C = preds[1].shape[1], preds[2].shape[1]
     dev = preds[0].device
     o2 = torch.empty((N, h, w, 5 * A + C), dtype=torch.float32, device=dev)
-    o3 = torch.empty((N, preds[3].shape[2], preds[3].shape[3], 5 * A + C), dtype=torch.float32, device=dev)
+    o3 = torch.empty((N, h // 2, w // 2, 5 * A + C), dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
         _check(lib().yfv2_export_heads(_ptr_array(preds), N, h * 16, w * 16, A, C, ctypes.c_void_p(o2.data_ptr()),
                                        ctypes.c_void_p(o3.data_ptr()), _stream(dev)), "export_heads")
@@ -1757,15 +1781,19 @@ def ncnn_post(out2, out3, anchor_num, thresh=0.3, nms_thresh=0.25, src_size=None
     sample/ncnn/src/yolo-fastestv2.cpp:78-183) on the export_onnx tensors `out2` [N,h,w,5A+C], `out3` (export_heads above).
     src_size = (cols, rows) of the source image (default: the network input size, scale 1).  Returns a list of N tuples
     (boxes int32 [n,4], scores float32 [n], cates int32 [n]) on the CPU, descending score, like the sample's dstBoxes."""
-    if not (out2.is_cuda and out3.is_cuda):
-        raise RuntimeError("yfv2: ncnn_post needs CUDA tensors (there is no CPU fallback)")
-    out2 = out2.detach().contiguous().float(); out3 = out3.detach().contiguous().float()
+    _require_cuda(out2, "ncnn_post: out2")
+    if out2.dim() != 4 or out2.shape[1] % 2 or out2.shape[2] % 2 or out2.shape[1] == 0 or out2.shape[2] == 0:
+        raise Yfv2Error("ncnn_post: out2 has shape %s, expected [N, H/16, W/16, 5A+C] with H, W multiples of 32" % (tuple(out2.shape),))
     N, h, w, ch = out2.shape
+    _expect_shapes("ncnn_post", [out2, out3], ["out2", "out3"], [(N, h, w, ch), (N, h // 2, w // 2, ch)])
+    out2 = out2.detach().contiguous().float(); out3 = out3.detach().contiguous().float()
     A = int(anchor_num)
     C = ch - 5 * A
     H, W = h * 16, w * 16
-    M = A * (h * w + out3.shape[1] * out3.shape[2])
+    M = A * (h * w + (h // 2) * (w // 2))
     max_out = M if max_out is None else int(max_out)
+    if max_out < 1:
+        raise Yfv2Error("ncnn_post: max_out=%d, expected at least 1" % max_out)
     sw, sh = (W, H) if src_size is None else src_size
     import numpy as np
     scale_w = float(np.float32(sw) / np.float32(W)); scale_h = float(np.float32(sh) / np.float32(H))        # :189-190, float division
