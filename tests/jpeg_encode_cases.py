@@ -89,3 +89,19 @@ def cases():
 
 ROUNDTRIP = ["restart_3_420", "restart_1_422_352", "restart_1000_444", "restart_3_grey", "photo_000139_q75_422_r5",
              "size_37x53", "quality_100_420", "layout_nv12"]
+
+
+def plan_error(kind, member, frames):
+    """yfv2_jpeg_encode_plan of one whole-frame output per descriptor of `frames` (a ctypes array of the union member `member`),
+    each wrapped as a yfv2_jpeg_enc_src of `kind`: (return code, yfv2_last_error()).  The plan reads no pixels."""
+    import ctypes
+    import yfv2_engine as eng
+    srcs = (eng.JpegEncSrc * len(frames))()
+    for s, f in zip(srcs, frames):
+        s.kind = kind
+        setattr(s.f, member, f)
+        s.w, s.h = f.w, f.h
+    L = eng.lib()
+    mb, wb, ab = ctypes.c_size_t(), ctypes.c_size_t(), ctypes.c_size_t()
+    rc = L.yfv2_jpeg_encode_plan(srcs, len(frames), None, 0, ctypes.byref(mb), ctypes.byref(wb), None, ctypes.byref(ab))
+    return rc, L.yfv2_last_error()

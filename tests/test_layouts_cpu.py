@@ -1,6 +1,7 @@
 """RGB, BGRA / RGBA, grey, planar RGB and packed YUV 4:2:2 frames, CPU side: the numpy restatement (tests/layout_oracle.py over
 oracle/resize.py) against outputs of the real cv2.cvtColor + cv2.resize (tests/golden/layout_cases.npz), the descriptor checks
-of yfv2_resize_strided_u8 and yfv2_resize_yuv422_u8 before any launch, and the refusals of resize_frames and detect_frames."""
+of yfv2_resize_strided_u8 and yfv2_resize_yuv422_u8 (and of the JPEG encoder's plan on the same descriptors) before any launch, and
+the refusals of resize_frames, encode_jpeg, crop_frame and detect_frames."""
 import ctypes
 import hashlib
 import os
@@ -10,6 +11,7 @@ import pytest
 import torch
 
 import yfv2  # noqa: F401
+import jpeg_encode_cases as jc
 import layout_cases as lc
 import layout_oracle as lo
 
@@ -102,13 +104,19 @@ def call_faults(make, good, fields, frame_faults):
     return calls
 
 
-def check_refusals(fn, name, calls):
+def check_refusals(fn, name, calls, kind, member):
+    """Each call refused by the entry fn, naming it; each frame fault also refused by yfv2_jpeg_encode_plan with its descriptors
+    wrapped as `kind` (union member `member`), naming the output."""
+    assert jc.plan_error(kind, member, calls[1][0])[0] == 0                  # the good descriptor
     for i, args in enumerate(calls):
         assert fn(*args, None) == -1, i
         err = __import__("yfv2_engine").lib().yfv2_last_error()
         assert name in err, (i, err)
         if i >= 8:
-            assert (b"frame 130" if i == len(calls) - 1 else b"frame 1") in err, (i, err)
+            at = 130 if i == len(calls) - 1 else 1
+            assert b"frame %d" % at in err, (i, err)
+            rc, err = jc.plan_error(kind, member, args[0])
+            assert rc == -1 and b"jpeg_encode_plan: output %d: frame" % at in err, (i, err)
 
 
 def test_strided_abi_rejects_bad_descriptors_before_any_launch():
@@ -118,8 +126,16 @@ def test_strided_abi_rejects_bad_descriptors_before_any_launch():
     faults = [dict(b=None), dict(g=None), dict(r=None), dict(w=0), dict(h=0), dict(w=-1), dict(h=-3),
               dict(step=0), dict(step=-3), dict(pitch=640 * 3 - 1), dict(step=4, pitch=640 * 4 - 1),
               dict(step=1 << 22, pitch=1 << 40)]                # step * w past 2^31
-    check_refusals(eng.lib().yfv2_resize_strided_u8, b"resize_strided_u8",
-                   call_faults(strided, good, ("b", "g", "r", "pitch", "step", "w", "h"), faults))
+    fields = ("b", "g", "r", "pitch", "step", "w", "h")
+    check_refusals(eng.lib().yfv2_resize_strided_u8, b"resize_strided_u8", call_faults(strided, good, fields, faults),
+                   eng.JPEG_SRC_STRIDED, "strided")
+    # a grey output reads the byte at b only: the same faults are refused but for a null g or r
+    for f in faults:
+        d = dict(zip(fields, good))
+        d.update(f)
+        rc, err = jc.plan_error(eng.JPEG_SRC_GRAY, "strided", strided(good, tuple(d.values())))
+        assert rc == (0 if set(f) <= {"g", "r"} else -1), (f, err)
+        assert rc == 0 or b"output 1" in err, (f, err)
 
 
 def test_yuv422_abi_rejects_bad_descriptors_before_any_launch():
@@ -129,7 +145,7 @@ def test_yuv422_abi_rejects_bad_descriptors_before_any_launch():
     faults = [dict(y=None), dict(u=None), dict(v=None), dict(w=0), dict(h=0), dict(w=-2), dict(h=-1), dict(w=639),
               dict(pitch=640 * 2 - 1), dict(pitch=640)]
     check_refusals(eng.lib().yfv2_resize_yuv422_u8, b"resize_yuv422_u8",
-                   call_faults(yuv422, good, ("y", "u", "v", "pitch", "w", "h"), faults))
+                   call_faults(yuv422, good, ("y", "u", "v", "pitch", "w", "h"), faults), eng.JPEG_SRC_YUV422, "yuv422")
 
 
 def test_resize_frames_refuses_bad_frames_before_anything_runs():
@@ -150,9 +166,17 @@ def test_resize_frames_refuses_bad_frames_before_anything_runs():
         ([rgb, np.zeros((72, 64), np.uint8), yuyv, rgb, chw, yuyv[:, :63]], ["bgr", "nv12", "yuyv", "rgb", "rgb_chw", "yuyv"],
          "frame 5"),
     ]
+    # the same refusals from every entry that takes frames, each naming the function called
+    entries = {"resize_frames": lambda frames, layout: eng.resize_frames(frames, 352, 352, layout, device="cuda:0"),
+               "encode_jpeg": lambda frames, layout: eng.encode_jpeg(frames, layout=layout, device="cuda:0"),
+               "crop_frame": lambda frames, layout: eng.crop_frame(frames[0], layout, 0, 0, 2, 2)}
     for frames, layout, msg in cases:
-        with pytest.raises(eng.Yfv2Error, match=msg):
-            eng.resize_frames(frames, 352, 352, layout, device="cuda:0")
+        for name, call in entries.items():
+            if name == "crop_frame" and (len(frames) != 1 or not isinstance(layout, str)):
+                continue
+            with pytest.raises(eng.Yfv2Error, match=msg) as e:
+                call(frames, layout)
+            assert str(e.value).startswith(name + ": "), (layout, str(e.value))
     with pytest.raises(eng.Yfv2Error, match="CUDA"):
         eng.resize_frames([rgb], 352, 352, "rgb", device="cpu")
 

@@ -1,6 +1,6 @@
 """Raw-frame resize, CPU side: the numpy restatement (oracle/resize.py) against outputs of the real cv2.resize
-(tests/golden/resize_cases.npz, frames_modelzoo.npz), argument checks of yfv2_resize_bgr_u8 before any launch, and the
-host scale-back of detect_frames against test.py's own arithmetic."""
+(tests/golden/resize_cases.npz, frames_modelzoo.npz), argument checks of yfv2_resize_bgr_u8 (and of the JPEG encoder's plan on
+the same frames) before any launch, and the host scale-back of detect_frames against test.py's own arithmetic."""
 import ctypes
 import hashlib
 import os
@@ -10,6 +10,7 @@ import pytest
 import torch
 
 import yfv2  # noqa: F401
+import jpeg_encode_cases as jc
 import resize_cases as rc
 from oracle import resize as ore
 
@@ -67,10 +68,15 @@ def test_abi_rejects_bad_arguments_before_any_launch():
         (frames(ok, (fake, 640, 480, 1919)), 2, 352, 352, dst),          # pitch < 3 * w
         (frames(*([ok] * 200 + [(fake, 640, 480, -1)])), 201, 352, 352, dst),   # a bad frame in the second launch's chunk
     ]
+    assert jc.plan_error(eng.JPEG_SRC_BGR, "bgr", frames(ok))[0] == 0
     for i, args in enumerate(bad_calls):
         assert L.yfv2_resize_bgr_u8(*args, None) == -1, i
         assert b"resize_bgr_u8" in L.yfv2_last_error(), (i, L.yfv2_last_error())
-    assert b"frame 200" in L.yfv2_last_error()
+        if i >= 7:
+            at = 200 if i == len(bad_calls) - 1 else 1
+            assert b"frame %d" % at in L.yfv2_last_error(), (i, L.yfv2_last_error())
+            code, err = jc.plan_error(eng.JPEG_SRC_BGR, "bgr", args[0])     # the JPEG encoder's plan refuses them too
+            assert code == -1 and b"jpeg_encode_plan: output %d: frame" % at in err, (i, err)
 
 
 def test_python_entry_points_refuse_bad_frames():

@@ -1,6 +1,7 @@
 """YUV 4:2:0 frames, CPU side: the numpy restatement (tests/yuv_oracle.py over oracle/resize.py) against outputs of the real
 cv2.cvtColor + cv2.resize (tests/golden/yuv_cases.npz, including every (y, u, v) triple), the descriptor checks of
-yfv2_resize_yuv420_u8 before any launch, and the refusals of the Python wrapper."""
+yfv2_resize_yuv420_u8 (and of the JPEG encoder's plan on the same frames) before any launch, and the refusals of the Python
+entries that take 4:2:0 frames."""
 import ctypes
 import hashlib
 import os
@@ -9,6 +10,7 @@ import numpy as np
 import pytest
 
 import yfv2  # noqa: F401
+import jpeg_encode_cases as jc
 import yuv_cases as yc
 import yuv_oracle as yo
 
@@ -108,11 +110,15 @@ def test_abi_rejects_bad_descriptors_before_any_launch():
         bad_calls.append((yuv_descs(nv12, f), 2, 352, 352, dst))
     # a bad frame in the second launch's chunk (64 descriptors per launch)
     bad_calls.append((yuv_descs(*([nv12, i420] * 40 + [bad(h=7)])), 81, 352, 352, dst))
+    assert jc.plan_error(eng.JPEG_SRC_YUV420, "yuv420", yuv_descs(nv12, i420))[0] == 0
     for i, args in enumerate(bad_calls):
         assert L.yfv2_resize_yuv420_u8(*args, None) == -1, i
         assert b"resize_yuv420_u8" in L.yfv2_last_error(), (i, L.yfv2_last_error())
         if i >= 8:
-            assert (b"frame 80" if i == len(bad_calls) - 1 else b"frame 1") in L.yfv2_last_error(), (i, L.yfv2_last_error())
+            at = 80 if i == len(bad_calls) - 1 else 1
+            assert b"frame %d" % at in L.yfv2_last_error(), (i, L.yfv2_last_error())
+            rc, err = jc.plan_error(eng.JPEG_SRC_YUV420, "yuv420", args[0])     # the JPEG encoder's plan refuses them too
+            assert rc == -1 and b"jpeg_encode_plan: output %d: frame" % at in err, (i, err)
 
 
 def test_python_wrapper_refuses_bad_frames_before_copying():
@@ -136,9 +142,17 @@ def test_python_wrapper_refuses_bad_frames_before_copying():
         ([(np.zeros((480, 640), np.uint8), np.zeros((240, 320), np.uint8), np.zeros((240, 321), np.uint8))], "i420", "chroma"),
         ([(np.zeros((480, 640), np.uint8), np.zeros((240, 640), np.int16))], "nv12", "uint8"),
     ]
+    # the bad frames refused by every entry that takes them, each naming the function called
+    entries = {"resize_yuv420": lambda frames, layout: eng.resize_yuv420(frames, 352, 352, layout, device="cuda:0"),
+               "encode_jpeg": lambda frames, layout: eng.encode_jpeg(frames, layout=layout, device="cuda:0"),
+               "crop_frame": lambda frames, layout: eng.crop_frame(frames[0], layout, 0, 0, 2, 2)}
     for frames, layout, msg in cases:
-        with pytest.raises(eng.Yfv2Error, match=msg):
-            eng.resize_yuv420(frames, 352, 352, layout, device="cuda:0")
+        for name, call in entries.items():
+            if name != "resize_yuv420" and (msg == "layout" or name == "crop_frame" and len(frames) != 1):
+                continue
+            with pytest.raises(eng.Yfv2Error, match=msg) as e:
+                call(frames, layout)
+            assert str(e.value).startswith(name + ": "), (layout, str(e.value))
     with pytest.raises(eng.Yfv2Error, match="CUDA"):
         eng.resize_yuv420([nv12], 352, 352, "nv12", device="cpu")
 

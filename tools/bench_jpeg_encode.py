@@ -41,15 +41,16 @@ class Call:
         descs = {}
         regions = regions or [(i, 0, 0, None, None) for i in range(len(frames))]
         params = (ctypes.c_int * 6)(1, 95, 7, 0x221111, 4, 0)
-        for d, r in zip(srcs, regions):
+        for k, r in enumerate(regions):
             i = r[0]
             if i not in descs:
-                descs[i] = eng.JpegEncSrc()
-                descs[i].hw = eng._enc_frame(frames[i], layout, torch.device("cuda"), descs[i], self.keep)
-            d.kind, d.f = descs[i].kind, descs[i].f
+                f = eng._check_frame(frames[i], layout, i, "bench_jpeg_encode")
+                descs[i] = eng._describe(f, layout, torch.device("cuda"), self.keep)
+            srcs[k] = descs[i]
+            d = srcs[k]
             d.x0, d.y0 = r[1], r[2]
-            d.w = descs[i].hw[1] if r[3] is None else r[3]
-            d.h = descs[i].hw[0] if r[4] is None else r[4]
+            if r[3] is not None:
+                d.w, d.h = r[3], r[4]
             d.params, d.nparams = ctypes.cast(params, ctypes.POINTER(ctypes.c_int)), 6
         self.params = params
         L = eng.lib()

@@ -16,7 +16,6 @@
 //   stuff      each unit counts the output bytes it owns (staging bytes whose first bit is its, 0xFF counted twice, plus the header,
 //              RSTn or EOI it writes), a scan of the counts places them, and each unit writes its bytes with 0xFF 0x00 stuffing.
 #include <algorithm>
-#include <climits>
 #include <cstring>
 #include <vector>
 
@@ -233,41 +232,15 @@ int parse_params(int i, const int* p, int np, Params& o) {
     return YFV2_OK;
 }
 
-// The frame's size and a reason when its descriptor is unusable (the resize entries' checks)
+// The frame's size and a reason when its descriptor is unusable (the resize entries' checks, frame_fault)
 const char* check_frame(const yfv2_jpeg_enc_src& s, int& fw, int& fh) {
+    const auto fault = [&](const auto& f, const char* why) { fw = f.w; fh = f.h; return why; };
     switch (s.kind) {
-        case YFV2_JPEG_SRC_BGR: {
-            const yfv2_frame& f = s.f.bgr;
-            fw = f.w; fh = f.h;
-            if (!f.data) return "null data";
-            if (f.w <= 0 || f.h <= 0 || f.pitch < 3LL * f.w) return "need w, h > 0 and pitch >= 3*w";
-            return nullptr;
-        }
-        case YFV2_JPEG_SRC_STRIDED: case YFV2_JPEG_SRC_GRAY: {
-            const yfv2_strided_frame& f = s.f.strided;
-            fw = f.w; fh = f.h;
-            if (!f.b || (s.kind == YFV2_JPEG_SRC_STRIDED && (!f.g || !f.r))) return "null channel pointer";
-            if (f.w <= 0 || f.h <= 0 || f.step < 1) return "need w, h > 0 and step >= 1";
-            if ((long long)f.step * f.w > INT_MAX || f.pitch < (long long)f.step * f.w) return "need step*w < 2^31 and pitch >= step*w";
-            return nullptr;
-        }
-        case YFV2_JPEG_SRC_YUV420: {
-            const yfv2_yuv420_frame& f = s.f.yuv420;
-            fw = f.w; fh = f.h;
-            if (!f.y || !f.u || !f.v) return "null plane";
-            if (f.w <= 0 || f.h <= 0 || (f.w & 1) || (f.h & 1)) return "w and h must be even and > 0";
-            if (f.y_pitch < f.w || (f.uv_step != 1 && f.uv_step != 2) ||
-                f.uv_pitch < (f.uv_step == 2 ? (long long)f.w : (long long)(f.w / 2)))
-                return "need y_pitch >= w, uv_step 1 or 2, uv_pitch >= w / 2 * uv_step";
-            return nullptr;
-        }
-        case YFV2_JPEG_SRC_YUV422: {
-            const yfv2_yuv422_frame& f = s.f.yuv422;
-            fw = f.w; fh = f.h;
-            if (!f.y || !f.u || !f.v) return "null plane pointer";
-            if (f.w <= 0 || f.h <= 0 || (f.w & 1) || f.pitch < 2LL * f.w) return "need w even and > 0, h > 0, pitch >= 2*w";
-            return nullptr;
-        }
+        case YFV2_JPEG_SRC_BGR: return fault(s.f.bgr, frame_fault(s.f.bgr));
+        case YFV2_JPEG_SRC_STRIDED: case YFV2_JPEG_SRC_GRAY:
+            return fault(s.f.strided, frame_fault(s.f.strided, s.kind == YFV2_JPEG_SRC_GRAY));
+        case YFV2_JPEG_SRC_YUV420: return fault(s.f.yuv420, frame_fault(s.f.yuv420));
+        case YFV2_JPEG_SRC_YUV422: return fault(s.f.yuv422, frame_fault(s.f.yuv422));
         default: fw = fh = 0; return "unknown kind";
     }
 }

@@ -23,8 +23,6 @@
 // aug_resize_kernel (yfv2_aug_batch, k_aug.cu) runs random_resize as the second resize over a fetch that computes the pixels of
 // the first from the planar source where they are read (DESIGN.md §9).
 // The per-pixel arithmetic is in resize.cuh, shared with the fused JPEG decode + resize (k_jpeg.cu).
-#include <climits>
-
 #include "aug.cuh"
 #include "resize.cuh"
 
@@ -189,89 +187,40 @@ aug_resize_kernel(const __grid_constant__ Chunk a) {
     for (int c = 0; c < 3; ++c) out[c * plane] = (uint8_t)v[c];
 }
 
-// The checks every entry makes on its call before it looks at the frames.
-bool bad_call(const char* fn, const void* frames, int N, int H, int W, const uint8_t* dst) {
-    if (!frames || !dst || N <= 0) { set_error("%s: null frames / dst or N <= 0", fn); return true; }
+// Every resize entry: the call's checks, each frame's (frame_fault), then the launches; a refusal names the entry and the frame.
+template <class Src>
+int resize_entry(const char* fn, const typename Src::Desc* frames, int N, int H, int W, uint8_t* dst, void* stream) {
+    if (!frames || !dst || N <= 0) { set_error("%s: null frames / dst or N <= 0", fn); return YFV2_EINVAL; }
     if (H <= 0 || W <= 0 || H > kResizeMaxSide || W > kResizeMaxSide) {
         set_error("%s: target %dx%d outside 1..%d", fn, W, H, kResizeMaxSide);
-        return true;
+        return YFV2_EINVAL;
     }
-    return false;
+    for (int n = 0; n < N; ++n) {
+        if (const char* why = frame_fault(frames[n])) {
+            set_error("%s: frame %d: %s (%dx%d)", fn, n, why, frames[n].w, frames[n].h);
+            return YFV2_EINVAL;
+        }
+    }
+    return launch_resize<Src>(frames, N, H, W, dst, stream);
 }
 
 }  // namespace
 }  // namespace yfv2
 
 extern "C" int yfv2_resize_bgr_u8(const yfv2_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
-    using namespace yfv2;
-    if (bad_call("resize_bgr_u8", frames, N, H, W, dst)) return YFV2_EINVAL;
-    for (int n = 0; n < N; ++n) {
-        const yfv2_frame& f = frames[n];
-        if (!f.data || f.w <= 0 || f.h <= 0 || f.pitch < 3LL * f.w) {
-            set_error("resize_bgr_u8: frame %d: data %p, %dx%d, pitch %lld (need data, w, h > 0, pitch >= 3*w)", n, (const void*)f.data,
-                      f.w, f.h, f.pitch);
-            return YFV2_EINVAL;
-        }
-    }
-    return launch_resize<BgrSource>(frames, N, H, W, dst, stream);
+    return yfv2::resize_entry<yfv2::BgrSource>("resize_bgr_u8", frames, N, H, W, dst, stream);
 }
 
 extern "C" int yfv2_resize_yuv420_u8(const yfv2_yuv420_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
-    using namespace yfv2;
-    if (bad_call("resize_yuv420_u8", frames, N, H, W, dst)) return YFV2_EINVAL;
-    for (int n = 0; n < N; ++n) {
-        const yfv2_yuv420_frame& f = frames[n];
-        const char* why = nullptr;
-        if (!f.y || !f.u || !f.v) why = "null plane";
-        else if (f.w <= 0 || f.h <= 0 || (f.w & 1) || (f.h & 1)) why = "w and h must be even and > 0";
-        else if (f.y_pitch < f.w) why = "y_pitch < w";
-        else if (f.uv_step != 1 && f.uv_step != 2) why = "uv_step must be 1 (planar) or 2 (interleaved)";
-        else if (f.uv_pitch < (f.uv_step == 2 ? (long long)f.w : (long long)(f.w / 2))) why = "uv_pitch < w / 2 * uv_step";
-        if (why) {
-            set_error("resize_yuv420_u8: frame %d: %s (y %p, u %p, v %p, %dx%d, y_pitch %lld, uv_pitch %lld, uv_step %d)", n, why,
-                      (const void*)f.y, (const void*)f.u, (const void*)f.v, f.w, f.h, f.y_pitch, f.uv_pitch, f.uv_step);
-            return YFV2_EINVAL;
-        }
-    }
-    return launch_resize<Yuv420Source>(frames, N, H, W, dst, stream);
+    return yfv2::resize_entry<yfv2::Yuv420Source>("resize_yuv420_u8", frames, N, H, W, dst, stream);
 }
 
 extern "C" int yfv2_resize_strided_u8(const yfv2_strided_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
-    using namespace yfv2;
-    if (bad_call("resize_strided_u8", frames, N, H, W, dst)) return YFV2_EINVAL;
-    for (int n = 0; n < N; ++n) {
-        const yfv2_strided_frame& f = frames[n];
-        const char* why = nullptr;
-        if (!f.b || !f.g || !f.r) why = "null channel pointer";
-        else if (f.w <= 0 || f.h <= 0) why = "w and h must be > 0";
-        else if (f.step < 1) why = "step must be >= 1";
-        else if ((long long)f.step * f.w > INT_MAX) why = "step * w must be < 2^31";
-        else if (f.pitch < (long long)f.step * f.w) why = "pitch < step * w";
-        if (why) {
-            set_error("resize_strided_u8: frame %d: %s (b %p, g %p, r %p, %dx%d, pitch %lld, step %d)", n, why, (const void*)f.b,
-                      (const void*)f.g, (const void*)f.r, f.w, f.h, f.pitch, f.step);
-            return YFV2_EINVAL;
-        }
-    }
-    return launch_resize<StridedSource>(frames, N, H, W, dst, stream);
+    return yfv2::resize_entry<yfv2::StridedSource>("resize_strided_u8", frames, N, H, W, dst, stream);
 }
 
 extern "C" int yfv2_resize_yuv422_u8(const yfv2_yuv422_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
-    using namespace yfv2;
-    if (bad_call("resize_yuv422_u8", frames, N, H, W, dst)) return YFV2_EINVAL;
-    for (int n = 0; n < N; ++n) {
-        const yfv2_yuv422_frame& f = frames[n];
-        const char* why = nullptr;
-        if (!f.y || !f.u || !f.v) why = "null plane pointer";
-        else if (f.w <= 0 || f.h <= 0 || (f.w & 1)) why = "w must be even and > 0, h > 0";
-        else if (f.pitch < 2LL * f.w) why = "pitch < 2 * w";
-        if (why) {
-            set_error("resize_yuv422_u8: frame %d: %s (y %p, u %p, v %p, %dx%d, pitch %lld)", n, why, (const void*)f.y,
-                      (const void*)f.u, (const void*)f.v, f.w, f.h, f.pitch);
-            return YFV2_EINVAL;
-        }
-    }
-    return launch_resize<Yuv422Source>(frames, N, H, W, dst, stream);
+    return yfv2::resize_entry<yfv2::Yuv422Source>("resize_yuv422_u8", frames, N, H, W, dst, stream);
 }
 
 namespace yfv2 {

@@ -1,12 +1,46 @@
 // cv2.resize(INTER_LINEAR)'s per-pixel arithmetic (k_resize.cu states it): the coefficients of one target index and one output
 // pixel computed over any source type with a fetch(c0, c1, p0, p1) of two pixels of a row.  k_resize.cu's kernels and k_jpeg.cu's
 // fused decode + resize (JpegSource) share it.  The frame fetches (BGR, strided, YUV 4:2:0, packed YUV 4:2:2: cv2.cvtColor's BGR
-// bytes of any layout) are here too, shared by k_resize.cu and the JPEG encoder (k_jpeg_enc.cu).
+// bytes of any layout) are here too, shared by k_resize.cu and the JPEG encoder (k_jpeg_enc.cu), with the host checks of their
+// descriptors.
 #pragma once
+#include <climits>
 #include <stdint.h>
 
 namespace yfv2 {
 namespace {
+
+// Host checks of one frame descriptor: nullptr, or why it is refused.  The resize entries and yfv2_jpeg_encode_plan accept exactly
+// the descriptors these accept.
+inline const char* frame_fault(const yfv2_frame& f) {
+    if (!f.data) return "null data";
+    if (f.w <= 0 || f.h <= 0) return "w and h must be > 0";
+    if (f.pitch < 3LL * f.w) return "pitch < 3 * w";
+    return nullptr;
+}
+// grey (YFV2_JPEG_SRC_GRAY) reads the byte at b only
+inline const char* frame_fault(const yfv2_strided_frame& f, bool grey = false) {
+    if (!f.b || (!grey && (!f.g || !f.r))) return "null channel pointer";
+    if (f.w <= 0 || f.h <= 0) return "w and h must be > 0";
+    if (f.step < 1) return "step must be >= 1";
+    if ((long long)f.step * f.w > INT_MAX) return "step * w must be < 2^31";
+    if (f.pitch < (long long)f.step * f.w) return "pitch < step * w";
+    return nullptr;
+}
+inline const char* frame_fault(const yfv2_yuv420_frame& f) {
+    if (!f.y || !f.u || !f.v) return "null plane";
+    if (f.w <= 0 || f.h <= 0 || (f.w & 1) || (f.h & 1)) return "w and h must be even and > 0";
+    if (f.y_pitch < f.w) return "y_pitch < w";
+    if (f.uv_step != 1 && f.uv_step != 2) return "uv_step must be 1 (planar) or 2 (interleaved)";
+    if (f.uv_pitch < (f.uv_step == 2 ? (long long)f.w : (long long)(f.w / 2))) return "uv_pitch < w / 2 * uv_step";
+    return nullptr;
+}
+inline const char* frame_fault(const yfv2_yuv422_frame& f) {
+    if (!f.y || !f.u || !f.v) return "null plane pointer";
+    if (f.w <= 0 || f.h <= 0 || (f.w & 1)) return "w must be even and > 0, h > 0";
+    if (f.pitch < 2LL * f.w) return "pitch < 2 * w";
+    return nullptr;
+}
 
 __device__ __forceinline__ int sat_u8(int v) { return min(max(v, 0), 255); }
 

@@ -58,6 +58,9 @@ class JpegEncSrc(ctypes.Structure):
                 ("f", _EncFrame), ("params", ctypes.POINTER(ctypes.c_int)), ("nparams", ctypes.c_int)]
 
 
+JPEG_SRC_BGR, JPEG_SRC_STRIDED, JPEG_SRC_GRAY, JPEG_SRC_YUV420, JPEG_SRC_YUV422 = range(5)   # JpegEncSrc.kind (YFV2_JPEG_SRC_*)
+
+
 class TrainerOp(ctypes.Structure):
     """yfv2_trainer_op: one op of the native trainer's program (test hook)."""
     _fields_ = [(f, ctypes.c_int) for f in ("kind", "a", "b", "y", "pw", "pg", "pb", "pbias", "bn", "relu", "ks", "stride", "M")] + \
@@ -984,45 +987,11 @@ def debug_hsv2bgr(pixels):
     return _hsv_debug(lib().yfv2_debug_hsv2bgr, "debug_hsv2bgr", pixels, pixels.shape[-2] if pixels.dim() >= 2 else 1)
 
 
-def _frame_on_device(f, device):
-    """A packed HWC BGR uint8 frame as a CUDA tensor on `device` whose pixels are 3 bytes apart (rows may be further apart)."""
-    if not isinstance(f, torch.Tensor):
-        import numpy as np
-        f = torch.from_numpy(np.ascontiguousarray(f))
-    if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
-        raise Yfv2Error("resize_bgr: frames must be uint8 [h, w, 3] (BGR, as cv2.imread returns), got %s %s"
-                        % (f.dtype, tuple(f.shape)))
-    f = f.to(device)
-    if f.stride(2) != 1 or f.stride(1) != 3:
-        f = f.contiguous()
-    return f
-
-
 def resize_bgr(frames, W, H, device=None, out=None):
     """cv2.resize(frame, (W, H), interpolation=cv2.INTER_LINEAR) of every frame, transposed to the [N, 3, H, W] uint8 batch the
     network takes (test.py:34-37), bit for bit, in one kernel.  frames: HWC uint8 BGR numpy arrays or CUDA tensors, any sizes
     (host arrays are copied to `device` first; a CUDA tensor that is a row crop of a larger frame is read in place)."""
-    frames = list(frames)
-    if not frames:
-        raise Yfv2Error("resize_bgr: no frames")
-    if device is None:
-        cuda = [f.device for f in frames if isinstance(f, torch.Tensor) and f.is_cuda]
-        device = cuda[0] if cuda else torch.device("cuda", torch.cuda.current_device())
-    device = torch.device(device)
-    if device.type != "cuda":
-        raise Yfv2Error("resize_bgr: runs on CUDA devices only (no CPU fallback)")
-    dev_frames = [_frame_on_device(f, device) for f in frames]
-    descs = (Frame * len(dev_frames))()
-    for d, f in zip(descs, dev_frames):
-        d.data, d.w, d.h, d.pitch = f.data_ptr(), f.shape[1], f.shape[0], f.stride(0)
-    N = len(dev_frames)
-    if out is None:
-        out = torch.empty((N, 3, H, W), dtype=torch.uint8, device=device)
-    elif tuple(out.shape) != (N, 3, H, W) or out.dtype != torch.uint8 or not out.is_contiguous() or out.device != device:
-        raise Yfv2Error("resize_bgr: out must be a contiguous uint8 tensor of shape %s on %s" % ((N, 3, H, W), device))
-    with torch.cuda.device(device):
-        _check(lib().yfv2_resize_bgr_u8(descs, N, H, W, ctypes.c_void_p(out.data_ptr()), _stream(device)), "resize_bgr_u8")
-    return out
+    return _resize("resize_bgr", frames, "bgr", ("bgr",), W, H, device, out)
 
 
 def _jpeg_name(names, i):
@@ -1095,11 +1064,7 @@ class JpegBatch:
     elsewhere (another process, say), used instead of parsing `files` (which may then be None)."""
 
     def __init__(self, files, device=None, names=None, progressive=False, parsed=None):
-        device = torch.device(device if device is not None else torch.device("cuda", torch.cuda.current_device()))
-        if device.type != "cuda":
-            raise Yfv2Error("decode_jpeg: runs on CUDA devices only (no CPU fallback)")
-        if device.index is None:
-            device = torch.device("cuda", torch.cuda.current_device())
+        device = _device("decode_jpeg", (), device)
         self.device, self.names = device, names
         if parsed is None:
             parsed = parse_jpeg(files, names, blob=True, pin=True, progressive=progressive)
@@ -1127,11 +1092,9 @@ class JpegBatch:
 
     def decode_resize(self, out, W, H):
         """Every file as cv2.resize(cv2.imread(f), (W, H), INTER_LINEAR) transposed to CHW, into out (a contiguous CUDA uint8
-        [N, 3, H, W] tensor on the batch's device), on the current stream without synchronising; the flags as decode() sets them."""
-        N = len(self.infos)
-        if (not isinstance(out, torch.Tensor) or tuple(out.shape) != (N, 3, H, W) or out.dtype != torch.uint8 or not out.is_contiguous()
-                or out.device != self.device):
-            raise Yfv2Error("decode_resize_jpeg: out must be a contiguous uint8 tensor of shape %s on %s" % ((N, 3, H, W), self.device))
+        [N, 3, H, W] tensor on the batch's device; None: a new one), returned, on the current stream without synchronising; the
+        flags as decode() sets them."""
+        out = _out("decode_resize_jpeg", out, len(self.infos), H, W, self.device)
         p = lambda t: ctypes.c_void_p(t.data_ptr())     # noqa: E731
         with torch.cuda.device(self.device):
             _check(lib().yfv2_jpeg_decode_resize(p(self.blob), p(self.meta), self.blob.numel(), p(self.files), self.files_bytes, int(H),
@@ -1178,10 +1141,7 @@ def decode_resize_jpeg(files, W, H, device=None, names=None, progressive=False, 
     the network takes, in one call (yfv2_jpeg_decode_resize): bit-identical to resize_bgr(decode_jpeg(files), W, H), without the
     full-size frames.  Refuses and raises as decode_jpeg does; out: a contiguous CUDA uint8 [N, 3, H, W] tensor to write into."""
     b = JpegBatch(files, device, names, progressive)
-    N = len(b.infos)
-    if out is None:
-        out = torch.empty((N, 3, H, W), dtype=torch.uint8, device=b.device)
-    b.decode_resize(out, W, H)
+    out = b.decode_resize(out, W, H)
     b.check()
     return out
 
@@ -1231,46 +1191,43 @@ def kmeans_anchors(dims, k, init_idx, max_iter=1000, device=None):
 YUV420_LAYOUTS = ("nv12", "nv21", "i420", "yv12")
 
 
-def _uint8_plane(p, what):
+def _uint8_plane(p, what, fn):
     """p as a uint8 2-D torch tensor; a host numpy array is wrapped, not copied."""
     if not isinstance(p, torch.Tensor):
-        import numpy as np
         p = np.asarray(p)
         if p.dtype != np.uint8 or p.ndim != 2:
-            raise Yfv2Error("resize_yuv420: %s must be a uint8 2-D array, got %s %s" % (what, p.dtype, p.shape))
+            raise Yfv2Error("%s: %s must be a uint8 2-D array, got %s %s" % (fn, what, p.dtype, p.shape))
         p = torch.from_numpy(p if min(p.strides, default=0) >= 0 else np.ascontiguousarray(p))
     elif p.dtype != torch.uint8 or p.dim() != 2:
-        raise Yfv2Error("resize_yuv420: %s must be a uint8 2-D tensor, got %s %s" % (what, p.dtype, tuple(p.shape)))
+        raise Yfv2Error("%s: %s must be a uint8 2-D tensor, got %s %s" % (fn, what, p.dtype, tuple(p.shape)))
     return p
 
 
-def _yuv420_planes(f, layout, i):
-    """Frame i as (y, u, v) uint8 2-D planes (u and v are the same [h/2, w] UV or VU plane for NV12 / NV21), checked, not
-    copied.  A single buffer is cv2's [h*3/2, w] layout: the luma rows, then the chroma (interleaved rows for NV12 / NV21; for
-    I420 / YV12 the two w/2-wide planes back to back, read from a contiguous buffer)."""
+def _yuv420_planes(f, layout, i, fn):
+    """Frame i as uint8 2-D planes, checked, not copied: (y, uv) for NV12 / NV21, (y, u, v) for I420 / YV12.  A single buffer is
+    cv2's [h*3/2, w] layout: the luma rows, then the chroma (interleaved rows for NV12 / NV21; for I420 / YV12 the two w/2-wide
+    planes back to back, read from a contiguous buffer)."""
     interleaved = layout in ("nv12", "nv21")
     if isinstance(f, (tuple, list)):
-        planes = [_uint8_plane(p, "frame %d plane %d" % (i, k)) for k, p in enumerate(f)]
+        planes = tuple(_uint8_plane(p, "frame %d plane %d" % (i, k), fn) for k, p in enumerate(f))
         if len(planes) != (2 if interleaved else 3):
-            raise Yfv2Error("resize_yuv420: frame %d: %s takes %s, got %d planes"
-                            % (i, layout, "(y, uv)" if interleaved else "(y, u, v)", len(planes)))
+            raise Yfv2Error("%s: frame %d: %s takes %s, got %d planes"
+                            % (fn, i, layout, "(y, uv)" if interleaved else "(y, u, v)", len(planes)))
         y = planes[0]
         h, w = y.shape
         chroma = [(h // 2, w)] if interleaved else [(h // 2, w // 2)] * 2
         for k, (p, want) in enumerate(zip(planes[1:], chroma)):
             if tuple(p.shape) != want or h % 2 or w % 2:
-                raise Yfv2Error("resize_yuv420: frame %d: y %s needs even sizes and chroma planes of %s, plane %d is %s"
-                                % (i, tuple(y.shape), want, k + 1, tuple(p.shape)))
-        u, v = (planes[1], planes[1]) if interleaved else (planes[1], planes[2])
-        return y, u, v
-    buf = _uint8_plane(f, "frame %d" % i)
+                raise Yfv2Error("%s: frame %d: y %s needs even sizes and chroma planes of %s, plane %d is %s"
+                                % (fn, i, tuple(y.shape), want, k + 1, tuple(p.shape)))
+        return planes
+    buf = _uint8_plane(f, "frame %d" % i, fn)
     rows, w = buf.shape
     h = rows // 3 * 2
     if rows % 3 or h <= 0 or w <= 0 or w % 2:
-        raise Yfv2Error("resize_yuv420: frame %d: a single buffer is [h*3/2, w] with h, w even and > 0, got %s"
-                        % (i, tuple(buf.shape)))
+        raise Yfv2Error("%s: frame %d: a single buffer is [h*3/2, w] with h, w even and > 0, got %s" % (fn, i, tuple(buf.shape)))
     if interleaved:
-        return buf[:h], buf[h:], buf[h:]
+        return buf[:h], buf[h:]
     buf = buf.contiguous()
     flat, q = buf.reshape(-1), (h // 2) * (w // 2)
     first, second = (flat[h * w:h * w + q].view(h // 2, w // 2), flat[h * w + q:h * w + 2 * q].view(h // 2, w // 2))
@@ -1284,65 +1241,25 @@ def resize_yuv420(frames, W, H, layout, device=None, out=None):
     single uint8 buffer [h*3/2, w], or its planes: (y [h, w], uv [h/2, w]) for NV12 / NV21, (y, u [h/2, w/2], v [h/2, w/2]) for
     I420 / YV12; numpy arrays or CUDA tensors, any even sizes.  Planes may be views into larger surfaces (rows further apart than
     w): CUDA views are read in place, host arrays are copied to `device` (1.5 bytes per pixel)."""
-    frames = list(frames)
-    layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
-    for lay in layouts if layouts else [layout]:
-        if lay not in YUV420_LAYOUTS:
-            raise Yfv2Error("resize_yuv420: layout must be one of %s, got %r" % (", ".join(YUV420_LAYOUTS), lay))
-    if not frames:
-        raise Yfv2Error("resize_yuv420: no frames")
-    if len(layouts) != len(frames):
-        raise Yfv2Error("resize_yuv420: %d layouts for %d frames" % (len(layouts), len(frames)))
-    planes = [_yuv420_planes(f, lay, i) for i, (f, lay) in enumerate(zip(frames, layouts))]
-    if device is None:
-        cuda = [p.device for ps in planes for p in ps if p.is_cuda]
-        device = cuda[0] if cuda else torch.device("cuda", torch.cuda.current_device())
-    device = torch.device(device)
-    if device.type != "cuda":
-        raise Yfv2Error("resize_yuv420: runs on CUDA devices only (no CPU fallback)")
-    N = len(frames)
-    if out is None:
-        out = torch.empty((N, 3, H, W), dtype=torch.uint8, device=device)
-    elif tuple(out.shape) != (N, 3, H, W) or out.dtype != torch.uint8 or not out.is_contiguous() or out.device != device:
-        raise Yfv2Error("resize_yuv420: out must be a contiguous uint8 tensor of shape %s on %s" % ((N, 3, H, W), device))
-
-    def on_device(p):
-        p = p.to(device)
-        return p if p.stride(1) == 1 else p.contiguous()
-
-    descs = (Yuv420Frame * N)()
-    keep = []          # device copies stay referenced until the launch is queued: a freed block could take the next frame's copy
-    for d, (y, u, v), lay in zip(descs, planes, layouts):
-        if lay in ("nv12", "nv21"):
-            y, uv = on_device(y), on_device(u)
-            keep += [y, uv]
-            d.u = uv.data_ptr() + (lay == "nv21")
-            d.v = uv.data_ptr() + (lay == "nv12")
-            d.uv_pitch, d.uv_step = uv.stride(0), 2
-        else:
-            y, u, v = on_device(y), on_device(u), on_device(v)
-            if u.stride(0) != v.stride(0):                 # one chroma pitch per descriptor
-                u, v = u.contiguous(), v.contiguous()
-            keep += [y, u, v]
-            d.u, d.v, d.uv_pitch, d.uv_step = u.data_ptr(), v.data_ptr(), u.stride(0), 1
-        d.y, d.y_pitch, d.h, d.w = y.data_ptr(), y.stride(0), y.shape[0], y.shape[1]
-    with torch.cuda.device(device):
-        _check(lib().yfv2_resize_yuv420_u8(descs, N, H, W, ctypes.c_void_p(out.data_ptr()), _stream(device)), "resize_yuv420_u8")
-    return out
+    return _resize("resize_yuv420", frames, layout, YUV420_LAYOUTS, W, H, device, out)
 
 
-# Layouts yfv2_resize_strided_u8 takes: the byte offsets of B, G, R within a pixel of each packed one, and the number of bytes
-# per pixel of each packed one.  "rgb_chw" ([3, h, w], R plane first) is built from its channel stride instead.
+# Layouts yfv2_resize_strided_u8 takes: the byte offsets of B, G, R within a pixel of each packed one.  "rgb_chw" ([3, h, w], R
+# plane first) is built from its channel stride instead.
 STRIDED_LAYOUTS = ("rgb", "bgra", "rgba", "gray", "rgb_chw")
 _BGR_OFFSETS = {"rgb": (2, 1, 0), "bgra": (0, 1, 2), "rgba": (2, 1, 0), "gray": (0, 0, 0)}
 # packed YUV 4:2:2 (yfv2_resize_yuv422_u8): the byte offsets of the first Y, of U and of V within a 4-byte macropixel
 YUV422_LAYOUTS = ("yuyv", "uyvy", "yvyu")
 _YUV422_OFFSETS = {"yuyv": (0, 1, 3), "uyvy": (1, 0, 2), "yvyu": (0, 3, 1)}
-_CHANNELS = {"rgb": 3, "bgra": 4, "rgba": 4, "yuyv": 2, "uyvy": 2, "yvyu": 2}
+# bytes per pixel of each packed layout
+_CHANNELS = {"bgr": 3, "rgb": 3, "bgra": 4, "rgba": 4, "gray": 1, "yuyv": 2, "uyvy": 2, "yvyu": 2}
 LAYOUTS = ("bgr",) + YUV420_LAYOUTS + STRIDED_LAYOUTS + YUV422_LAYOUTS
-# the entry point (descriptor kind) of each layout
-_KIND = dict([("bgr", "bgr")] + [(k, "yuv420") for k in YUV420_LAYOUTS] + [(k, "strided") for k in STRIDED_LAYOUTS]
-             + [(k, "yuv422") for k in YUV422_LAYOUTS])
+# the descriptor kind (yfv2_jpeg_enc_src.kind) of each layout, and the union member of yfv2_jpeg_enc_src.f each kind fills: the
+# resize entry yfv2_resize_<member>_u8 takes an array of it
+_KIND = dict([("bgr", JPEG_SRC_BGR), ("gray", JPEG_SRC_GRAY)] + [(k, JPEG_SRC_YUV420) for k in YUV420_LAYOUTS]
+             + [(k, JPEG_SRC_STRIDED) for k in STRIDED_LAYOUTS if k != "gray"] + [(k, JPEG_SRC_YUV422) for k in YUV422_LAYOUTS])
+_MEMBER = ("bgr", "strided", "strided", "yuv420", "yuv422")
+_DESC = dict(_EncFrame._fields_)
 
 
 def frame_size(frame, layout):
@@ -1354,14 +1271,13 @@ def frame_size(frame, layout):
     return tuple(frame.shape[1:3]) if layout == "rgb_chw" else tuple(frame.shape[:2])
 
 
-def _layout_frame(f, layout, i):
+def _layout_frame(f, layout, i, fn):
     """Frame i of a strided or 4:2:2 layout as a uint8 tensor of the layout's shape, checked, not copied."""
     shape = ("[3, h, w]" if layout == "rgb_chw" else "[h, w]" if layout == "gray" else "[h, w, %d]" % _CHANNELS[layout])
     if not isinstance(f, torch.Tensor):
-        import numpy as np
         f = np.asarray(f)
         if f.dtype != np.uint8:
-            raise Yfv2Error("resize_frames: frame %d (%s) must be uint8 %s, got %s %s" % (i, layout, shape, f.dtype, f.shape))
+            raise Yfv2Error("%s: frame %d (%s) must be uint8 %s, got %s %s" % (fn, i, layout, shape, f.dtype, f.shape))
         f = torch.from_numpy(f if min(f.strides, default=0) >= 0 else np.ascontiguousarray(f))
     ok = f.dtype == torch.uint8 and f.dim() == (2 if layout == "gray" else 3) and f.numel() > 0
     if ok and layout == "rgb_chw":
@@ -1369,64 +1285,147 @@ def _layout_frame(f, layout, i):
     elif ok and layout != "gray":
         ok = f.shape[2] == _CHANNELS[layout]
     if not ok:
-        raise Yfv2Error("resize_frames: frame %d (%s) must be uint8 %s with h, w > 0, got %s %s"
-                        % (i, layout, shape, f.dtype, tuple(f.shape)))
+        raise Yfv2Error("%s: frame %d (%s) must be uint8 %s with h, w > 0, got %s %s"
+                        % (fn, i, layout, shape, f.dtype, tuple(f.shape)))
     if layout in YUV422_LAYOUTS and f.shape[1] % 2:
-        raise Yfv2Error("resize_frames: frame %d (%s): 4:2:2 needs an even width (two pixels per macropixel), got w = %d"
-                        % (i, layout, f.shape[1]))
+        raise Yfv2Error("%s: frame %d (%s): 4:2:2 needs an even width (two pixels per macropixel), got w = %d"
+                        % (fn, i, layout, f.shape[1]))
     return f
 
 
-def _check_frame(f, layout, i):
-    """Checks frame i against its layout without launching anything; returns what the layout's resize takes."""
+def _check_frame(f, layout, i, fn):
+    """Checks frame i against its layout without copying or launching anything; returns what _describe takes: the BGR array or
+    tensor, the planes of a 4:2:0 frame, a uint8 tensor of the layout's shape for the others.  A refusal names fn, the public
+    function called."""
     kind = _KIND[layout]
-    if kind == "bgr":
+    if kind == JPEG_SRC_BGR:
         if isinstance(f, torch.Tensor):
             ok = f.dtype == torch.uint8
         else:
-            import numpy as np
             f = np.asarray(f)
             ok = f.dtype == np.uint8
         if not ok or f.ndim != 3 or f.shape[2] != 3:
-            raise Yfv2Error("resize_frames: frame %d (bgr) must be uint8 [h, w, 3], got %s %s" % (i, f.dtype, tuple(f.shape)))
+            raise Yfv2Error("%s: frame %d (bgr) must be uint8 [h, w, 3], got %s %s" % (fn, i, f.dtype, tuple(f.shape)))
         return f
-    if kind == "yuv420":
-        _yuv420_planes(f, layout, i)
-        return f
-    return _layout_frame(f, layout, i)
+    if kind == JPEG_SRC_YUV420:
+        return _yuv420_planes(f, layout, i, fn)
+    return _layout_frame(f, layout, i, fn)
 
 
-def _resize_layout_run(frames, layouts, W, H, device, out):
-    """One yfv2_resize_strided_u8 or yfv2_resize_yuv422_u8 call for checked frames of one descriptor kind."""
-    N = len(frames)
-    strided = _KIND[layouts[0]] == "strided"
-    descs = ((StridedFrame if strided else Yuv422Frame) * N)()
-    keep = []          # device copies stay referenced until the launch is queued: a freed block could take the next frame's copy
-    for d, f, lay in zip(descs, frames, layouts):
-        f = f.to(device)
-        if lay == "rgb_chw":                                 # any channel and row stride, unit column stride
-            if f.stride(2) != 1 or f.stride(1) < f.shape[2]:
-                f = f.contiguous()
-            p, s = f.data_ptr(), f.stride(0)
-            d.b, d.g, d.r, d.pitch, d.step = p + 2 * s, p + s, p, f.stride(1), 1
-            d.h, d.w = f.shape[1], f.shape[2]
+def _checked_frames(fn, frames, layout, allowed=LAYOUTS):
+    """The frames as a list, each checked (_check_frame), and one layout name per frame from `layout` (one name, or one per frame),
+    each among `allowed`."""
+    frames = list(frames)
+    layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
+    for lay in layouts if layouts else [layout]:
+        if not isinstance(lay, str) or lay not in allowed:
+            raise Yfv2Error("%s: layout must be one of %s, got %r" % (fn, ", ".join(allowed), lay))
+    if not frames:
+        raise Yfv2Error("%s: no frames" % fn)
+    if len(layouts) != len(frames):
+        raise Yfv2Error("%s: %d layouts for %d frames" % (fn, len(layouts), len(frames)))
+    return [_check_frame(f, lay, i, fn) for i, (f, lay) in enumerate(zip(frames, layouts))], layouts
+
+
+def _device(fn, frames, device):
+    """The CUDA device a call runs on, with its index: `device`, else that of the first CUDA tensor among the checked frames (or
+    their planes), else the current one."""
+    if device is None:
+        device = next((t.device for f in frames for t in (f if isinstance(f, tuple) else (f,))
+                       if isinstance(t, torch.Tensor) and t.is_cuda), None)
+    device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    if device.type != "cuda":
+        raise Yfv2Error("%s: runs on CUDA devices only (no CPU fallback)" % fn)
+    return device if device.index is not None else torch.device("cuda", torch.cuda.current_device())
+
+
+def _out(fn, out, N, H, W, device):
+    """out checked to be a contiguous uint8 [N, 3, H, W] tensor on device, or a new one when None."""
+    if out is None:
+        return torch.empty((N, 3, H, W), dtype=torch.uint8, device=device)
+    if (not isinstance(out, torch.Tensor) or tuple(out.shape) != (N, 3, H, W) or out.dtype != torch.uint8 or not out.is_contiguous()
+            or out.device != device):
+        raise Yfv2Error("%s: out must be a contiguous uint8 tensor of shape %s on %s" % (fn, (N, 3, H, W), device))
+    return out
+
+
+def _describe(f, layout, device, keep):
+    """The descriptor of frame f (as _check_frame returned it) with its pixels on `device`: a JpegEncSrc of the layout's kind, its
+    union member filled and the whole frame as its region.  The only code that places frames: host frames are copied to
+    `device`; a CUDA frame is read in place when its strides fit the descriptor, else a contiguous copy of it is.  The device
+    tensors read go to keep, which must hold them until the launch is queued: a freed block could take the next frame's copy."""
+    kind = _KIND[layout]
+    s = JpegEncSrc(kind)
+    if kind == JPEG_SRC_YUV420:
+        planes = [p.to(device) for p in f]
+        planes = [p if p.stride(1) == 1 else p.contiguous() for p in planes]
+        y, u, e = planes[0], planes[1], s.f.yuv420
+        if len(planes) == 2:                                  # NV12 / NV21: one interleaved chroma plane, U first for NV12
+            e.u, e.v, e.uv_pitch, e.uv_step = u.data_ptr() + (layout == "nv21"), u.data_ptr() + (layout == "nv12"), u.stride(0), 2
         else:
-            step = 1 if lay == "gray" else _CHANNELS[lay]
-            if f.stride(1) != step or (lay != "gray" and f.stride(2) != 1) or f.stride(0) < step * f.shape[1]:
-                f = f.contiguous()
-            p = f.data_ptr()
-            if strided:
-                ob, og, or_ = _BGR_OFFSETS[lay]
-                d.b, d.g, d.r, d.step = p + ob, p + og, p + or_, step
-            else:
-                oy, ou, ov = _YUV422_OFFSETS[lay]
-                d.y, d.u, d.v = p + oy, p + ou, p + ov
-            d.pitch, d.h, d.w = f.stride(0), f.shape[0], f.shape[1]
-        keep.append(f)
-    fn, what = ((lib().yfv2_resize_strided_u8, "resize_strided_u8") if strided else
-                (lib().yfv2_resize_yuv422_u8, "resize_yuv422_u8"))
-    with torch.cuda.device(device):
-        _check(fn(descs, N, H, W, ctypes.c_void_p(out.data_ptr()), _stream(device)), what)
+            v = planes[2]
+            if u.stride(0) != v.stride(0):                    # one chroma pitch per descriptor
+                planes[1:] = u, v = u.contiguous(), v.contiguous()
+            e.u, e.v, e.uv_pitch, e.uv_step = u.data_ptr(), v.data_ptr(), u.stride(0), 1
+        e.y, e.y_pitch = y.data_ptr(), y.stride(0)
+        e.h, e.w = s.h, s.w = y.shape
+        keep += planes
+        return s
+    if not isinstance(f, torch.Tensor):                       # a host BGR array: the other layouts' checks return tensors
+        f = torch.from_numpy(np.ascontiguousarray(f))
+    f = f.to(device)
+    st = f.stride()
+    if layout == "rgb_chw":                                   # any channel and row stride, unit column stride
+        _, h, w = f.shape
+        if st[2] != 1 or st[1] < w:
+            f = f.contiguous()
+            st = f.stride()
+        p = f.data_ptr()
+        e = s.f.strided
+        e.b, e.g, e.r, e.pitch, e.step = p + 2 * st[0], p + st[0], p, st[1], 1
+    else:                                                     # packed: pixels `step` bytes apart, rows at least w pixels apart
+        (h, w), step = f.shape[:2], _CHANNELS[layout]
+        if st[1] != step or (layout != "gray" and st[2] != 1) or st[0] < step * w:
+            f = f.contiguous()
+            st = f.stride()
+        p = f.data_ptr()
+        if kind == JPEG_SRC_BGR:
+            e = s.f.bgr
+            e.data = p
+        elif kind == JPEG_SRC_YUV422:
+            e = s.f.yuv422
+            e.y, e.u, e.v = (p + o for o in _YUV422_OFFSETS[layout])
+        else:
+            e = s.f.strided
+            e.b, e.g, e.r = (p + o for o in _BGR_OFFSETS[layout])
+            e.step = step
+        e.pitch = st[0]
+    e.h, e.w = s.h, s.w = h, w
+    keep.append(f)
+    return s
+
+
+def _resize(fn, frames, layout, allowed, W, H, device, out):
+    """resize_bgr, resize_yuv420 and resize_frames: every frame checked, then one yfv2_resize_<member>_u8 call for each run of
+    consecutive frames that fill the same descriptor, each into its slice of out."""
+    checked, layouts = _checked_frames(fn, frames, layout, allowed)
+    device = _device(fn, checked, device)
+    N = len(checked)
+    out = _out(fn, out, N, H, W, device)
+    i = 0
+    while i < N:
+        member, j = _MEMBER[_KIND[layouts[i]]], i + 1
+        while j < N and _MEMBER[_KIND[layouts[j]]] == member:
+            j += 1
+        keep, desc = [], _DESC[member]
+        lo, hi = JpegEncSrc.f.offset, JpegEncSrc.f.offset + ctypes.sizeof(desc)     # the member's bytes in a JpegEncSrc
+        srcs = [bytes(_describe(checked[k], layouts[k], device, keep)) for k in range(i, j)]
+        descs = (desc * (j - i)).from_buffer_copy(b"".join(src[lo:hi] for src in srcs))
+        entry = getattr(lib(), "yfv2_resize_%s_u8" % member)
+        with torch.cuda.device(device):
+            _check(entry(descs, j - i, H, W, ctypes.c_void_p(out[i].data_ptr()), _stream(device)), "resize_%s_u8" % member)
+        i = j
+    return out
 
 
 def resize_frames(frames, W, H, layout, device=None, out=None):
@@ -1444,96 +1443,13 @@ def resize_frames(frames, W, H, layout, device=None, out=None):
     "rgb_chw" any channel and row stride with unit column stride), host arrays are copied to `device`.  Consecutive frames of
     one descriptor kind go to one call (yfv2_resize_bgr_u8 / _yuv420_u8 / _strided_u8 / _yuv422_u8), each into its slice of
     `out`.  Every frame is checked before anything is copied or launched."""
-    frames = list(frames)
-    layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
-    for lay in layouts if layouts else [layout]:
-        if not isinstance(lay, str) or lay not in LAYOUTS:
-            raise Yfv2Error("resize_frames: layout must be one of %s, got %r" % (", ".join(LAYOUTS), lay))
-    if not frames:
-        raise Yfv2Error("resize_frames: no frames")
-    if len(layouts) != len(frames):
-        raise Yfv2Error("resize_frames: %d layouts for %d frames" % (len(layouts), len(frames)))
-    checked = [_check_frame(f, lay, i) for i, (f, lay) in enumerate(zip(frames, layouts))]
-    if device is None:
-        cuda = [t.device for f in checked for t in (f if isinstance(f, (tuple, list)) else (f,))
-                if isinstance(t, torch.Tensor) and t.is_cuda]
-        device = cuda[0] if cuda else torch.device("cuda", torch.cuda.current_device())
-    device = torch.device(device)
-    if device.type != "cuda":
-        raise Yfv2Error("resize_frames: runs on CUDA devices only (no CPU fallback)")
-    N = len(frames)
-    if out is None:
-        out = torch.empty((N, 3, H, W), dtype=torch.uint8, device=device)
-    elif tuple(out.shape) != (N, 3, H, W) or out.dtype != torch.uint8 or not out.is_contiguous() or out.device != device:
-        raise Yfv2Error("resize_frames: out must be a contiguous uint8 tensor of shape %s on %s" % ((N, 3, H, W), device))
-    i = 0
-    while i < N:
-        kind, j = _KIND[layouts[i]], i + 1
-        while j < N and _KIND[layouts[j]] == kind:
-            j += 1
-        if kind == "bgr":
-            resize_bgr(checked[i:j], W, H, device, out[i:j])
-        elif kind == "yuv420":
-            resize_yuv420(checked[i:j], W, H, layouts[i:j], device, out[i:j])
-        else:
-            _resize_layout_run(checked[i:j], layouts[i:j], W, H, device, out[i:j])
-        i = j
-    return out
+    return _resize("resize_frames", frames, layout, LAYOUTS, W, H, device, out)
 
 
 # cv2's IMWRITE_* ids and IMWRITE_JPEG_SAMPLING_FACTOR_* values (yfv2_jpeg_encode_plan reads the same pairs)
 IMWRITE_JPEG_QUALITY, IMWRITE_JPEG_PROGRESSIVE, IMWRITE_JPEG_OPTIMIZE, IMWRITE_JPEG_RST_INTERVAL = 1, 2, 3, 4
 IMWRITE_JPEG_LUMA_QUALITY, IMWRITE_JPEG_CHROMA_QUALITY, IMWRITE_JPEG_SAMPLING_FACTOR = 5, 6, 7
 JPEG_SAMPLING = {"420": 0x221111, "422": 0x211111, "444": 0x111111, "440": 0x121111, "411": 0x411111}
-_ENC_KIND = {"bgr": 0, "strided": 1, "gray": 2, "yuv420": 3, "yuv422": 4}
-
-
-def _enc_frame(f, lay, device, d, keep):
-    """Fills d (a JpegEncSrc) with the descriptor of checked frame f in layout `lay`, its pixels on `device`; returns (h, w)."""
-    kind = "gray" if lay == "gray" else _KIND[lay]
-    d.kind = _ENC_KIND[kind]
-    if kind == "bgr":
-        f = _frame_on_device(f, device)
-        d.f.bgr.data, d.f.bgr.w, d.f.bgr.h, d.f.bgr.pitch = f.data_ptr(), f.shape[1], f.shape[0], f.stride(0)
-        keep.append(f)
-        return f.shape[0], f.shape[1]
-    if kind == "yuv420":
-        y, u, v = [p.to(device) for p in _yuv420_planes(f, lay, 0)]
-        y, u, v = [p if p.stride(1) == 1 else p.contiguous() for p in (y, u, v)]
-        e = d.f.yuv420
-        if lay in ("nv12", "nv21"):
-            e.u, e.v, e.uv_pitch, e.uv_step = u.data_ptr() + (lay == "nv21"), u.data_ptr() + (lay == "nv12"), u.stride(0), 2
-        else:
-            if u.stride(0) != v.stride(0):
-                u, v = u.contiguous(), v.contiguous()
-            e.u, e.v, e.uv_pitch, e.uv_step = u.data_ptr(), v.data_ptr(), u.stride(0), 1
-        e.y, e.y_pitch, e.h, e.w = y.data_ptr(), y.stride(0), y.shape[0], y.shape[1]
-        keep += [y, u, v]
-        return e.h, e.w
-    f = f.to(device)
-    if lay == "rgb_chw":
-        if f.stride(2) != 1 or f.stride(1) < f.shape[2]:
-            f = f.contiguous()
-        p, s = f.data_ptr(), f.stride(0)
-        e = d.f.strided
-        e.b, e.g, e.r, e.pitch, e.step, e.h, e.w = p + 2 * s, p + s, p, f.stride(1), 1, f.shape[1], f.shape[2]
-        keep.append(f)
-        return e.h, e.w
-    step = 1 if lay == "gray" else _CHANNELS[lay]
-    if f.stride(1) != step or (lay != "gray" and f.stride(2) != 1) or f.stride(0) < step * f.shape[1]:
-        f = f.contiguous()
-    p = f.data_ptr()
-    if kind == "yuv422":
-        e = d.f.yuv422
-        oy, ou, ov = _YUV422_OFFSETS[lay]
-        e.y, e.u, e.v = p + oy, p + ou, p + ov
-    else:
-        e = d.f.strided
-        ob, og, or_ = _BGR_OFFSETS[lay]
-        e.b, e.g, e.r, e.step = p + ob, p + og, p + or_, step
-    e.pitch, e.h, e.w = f.stride(0), f.shape[0], f.shape[1]
-    keep.append(f)
-    return e.h, e.w
 
 
 def _per_output(v, n, what):
@@ -1554,26 +1470,16 @@ def encode_jpeg(frames, quality=95, sampling="420", restart_interval=0, layout="
     Everything is checked before anything is launched; a refusal raises Yfv2Error naming the output.  Returns a list of bytes, or
     with device_out=True (arena, offsets, lengths): the uint8 CUDA arena, output i at offsets[i] (host int64 numpy) and
     lengths[i] bytes long (CUDA int64), with no copy to the host."""
-    import numpy as np
-    frames = list(frames)
-    layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
-    if not frames:
-        raise Yfv2Error("encode_jpeg: no frames")
-    if len(layouts) != len(frames):
-        raise Yfv2Error("encode_jpeg: %d layouts for %d frames" % (len(layouts), len(frames)))
-    for lay in layouts:
-        if not isinstance(lay, str) or lay not in LAYOUTS:
-            raise Yfv2Error("encode_jpeg: layout must be one of %s, got %r" % (", ".join(LAYOUTS), lay))
-    checked = [_check_frame(f, lay, i) for i, (f, lay) in enumerate(zip(frames, layouts))]
+    checked, layouts = _checked_frames("encode_jpeg", frames, layout)
     if regions is None:
-        regions = [(i, 0, 0, None, None) for i in range(len(frames))]
+        regions = [(i, 0, 0, None, None) for i in range(len(checked))]
     regions = [tuple(r) for r in regions]
     n = len(regions)
     if n == 0:
         raise Yfv2Error("encode_jpeg: no regions")
     for k, r in enumerate(regions):
-        if len(r) != 5 or not 0 <= int(r[0]) < len(frames):
-            raise Yfv2Error("encode_jpeg: region %d must be (frame index in [0, %d), x0, y0, w, h), got %r" % (k, len(frames), r))
+        if len(r) != 5 or not 0 <= int(r[0]) < len(checked):
+            raise Yfv2Error("encode_jpeg: region %d must be (frame index in [0, %d), x0, y0, w, h), got %r" % (k, len(checked), r))
     qs, ss, rs = _per_output(quality, n, "quality"), _per_output(sampling, n, "sampling"), _per_output(restart_interval, n, "restart")
     extra = params if params and isinstance(params[0], (list, tuple)) else [params or []] * n
     if len(extra) != n:
@@ -1584,26 +1490,17 @@ def encode_jpeg(frames, quality=95, sampling="420", restart_interval=0, layout="
             raise Yfv2Error("encode_jpeg: output %d: sampling must be one of %s, got %r" % (k, ", ".join(JPEG_SAMPLING), ss[k]))
         plist.append([IMWRITE_JPEG_QUALITY, int(qs[k]), IMWRITE_JPEG_SAMPLING_FACTOR, JPEG_SAMPLING[ss[k]],
                       IMWRITE_JPEG_RST_INTERVAL, int(rs[k])] + [int(x) for x in extra[k]])
-    if device is None:
-        cuda = [t.device for f in checked for t in (f if isinstance(f, (tuple, list)) else (f,))
-                if isinstance(t, torch.Tensor) and t.is_cuda]
-        device = cuda[0] if cuda else torch.device("cuda", torch.cuda.current_device())
-    device = torch.device(device)
-    if device.type != "cuda":
-        raise Yfv2Error("encode_jpeg: runs on CUDA devices only (no CPU fallback)")
+    device = _device("encode_jpeg", checked, device)
     srcs = (JpegEncSrc * n)()
-    keep, cparams, frame_desc = [], [], {}
-    for k, (d, r) in enumerate(zip(srcs, regions)):
+    keep, cparams, frame_src = [], [], {}
+    for k, r in enumerate(regions):
         i = int(r[0])
-        if i not in frame_desc:
-            frame_desc[i] = JpegEncSrc()
-            frame_desc[i].hw = _enc_frame(checked[i], layouts[i], device, frame_desc[i], keep)
-        src = frame_desc[i]
-        d.kind, d.f = src.kind, src.f
-        fh, fw = src.hw
+        if i not in frame_src:
+            frame_src[i] = _describe(checked[i], layouts[i], device, keep)
+        srcs[k] = frame_src[i]
+        d = srcs[k]
         d.x0, d.y0 = int(r[1]), int(r[2])
-        d.w = fw if r[3] is None else int(r[3])
-        d.h = fh if r[4] is None else int(r[4])
+        d.w, d.h = d.w if r[3] is None else int(r[3]), d.h if r[4] is None else int(r[4])
         pa = (ctypes.c_int * len(plist[k]))(*plist[k])
         cparams.append(pa)
         d.params, d.nparams = ctypes.cast(pa, ctypes.POINTER(ctypes.c_int)), len(plist[k])
@@ -1640,7 +1537,7 @@ def crop_frame(frame, layout, x0, y0, w, h):
     that the 2x2 chroma blocks of the crop are those of the frame.  Packed 4:2:2 needs even x0 and w (whole macropixels)."""
     if layout not in LAYOUTS:
         raise Yfv2Error("crop_frame: layout must be one of %s, got %r" % (", ".join(LAYOUTS), layout))
-    f = _check_frame(frame, layout, 0)
+    f = _check_frame(frame, layout, 0, "crop_frame")
     fh, fw = frame_size(f, layout)
     x0, y0, w, h = int(x0), int(y0), int(w), int(h)
     if w < 1 or h < 1 or x0 < 0 or y0 < 0 or x0 + w > fw or y0 + h > fh:
@@ -1651,12 +1548,11 @@ def crop_frame(frame, layout, x0, y0, w, h):
     if layout in YUV422_LAYOUTS and (x0 | w) & 1:
         raise Yfv2Error("crop_frame: %s crops need even x0 and w (two pixels per macropixel), got x0 %d, w %d" % (layout, x0, w))
     if layout in YUV420_LAYOUTS:
-        y, u, v = _yuv420_planes(f, layout, 0)
         cy = slice(y0 // 2, (y0 + h) // 2)
-        if layout in ("nv12", "nv21"):
-            return y[y0:y0 + h, x0:x0 + w], u[cy, x0:x0 + w]
+        if len(f) == 2:                                       # (y, uv)
+            return f[0][y0:y0 + h, x0:x0 + w], f[1][cy, x0:x0 + w]
         cx = slice(x0 // 2, (x0 + w) // 2)
-        return y[y0:y0 + h, x0:x0 + w], u[cy, cx], v[cy, cx]
+        return f[0][y0:y0 + h, x0:x0 + w], f[1][cy, cx], f[2][cy, cx]
     if layout == "rgb_chw":
         return f[:, y0:y0 + h, x0:x0 + w]
     return f[y0:y0 + h, x0:x0 + w]
