@@ -71,10 +71,10 @@ def candidates(x, conf_thres):
     return box, conf, j, rows
 
 
-def by_class(x, conf_thres, iou_thres, max_det, max_wh, lists_always=False):
+def by_class(x, conf_thres, iou_thres, max_det, max_wh):
     """sort_and_suppress's choice of the per-class kept lists for one image, restated: the lists fit, every candidate box lies
     inside (-max_wh/2, max_wh/2), the threshold's rounding boundary is positive, max_wh > 0, at most 256 classes, a cap of at least
-    kNmsListMinDet (any cap with YFV2_NMS_LISTS set) and no class holding more than half of the candidates."""
+    kNmsListMinDet and no class holding more than half of the candidates."""
     C = x.shape[1] - 5
     box, _, cls, _ = candidates(x, conf_thres)
     lim = f32(0.5) * f32(max_wh)
@@ -82,7 +82,7 @@ def by_class(x, conf_thres, iou_thres, max_det, max_wh, lists_always=False):
     hist = np.bincount(cls, minlength=1)
     no_majority = not np.any(2 * hist > len(cls))
     return (lists_fit(x.shape[0], max_det) and inside and iou_mid(iou_thres)[0] > 0.0 and max_wh > 0 and C <= LIST_CLASSES
-            and max_det >= (0 if lists_always else LIST_MIN_DET) and no_majority)
+            and max_det >= LIST_MIN_DET and no_majority)
 
 
 def sort_size(cnt):
@@ -310,11 +310,11 @@ def zone_heights(thr, n, seed):
     return hits_a[pick], hits_b[pick], sup
 
 
-def zone_image(thr, n, seed, layout, m=160, C=80):
-    """One image with n zone pairs (zone_heights) side by side in class 0, and 64 - n small far-apart class-1 boxes that are all
-    kept.  layout "adjacent": each pair is consecutive in score order (one chunk); "split": all first boxes, then the class-1
-    boxes, then the second boxes (chunk 1 meets its partners among the 64 kept boxes of chunk 0).  Returns (rows [m, 5+C],
-    suppressed [n])."""
+def zone_image(thr, n, seed, layout, m=160, C=80, fill_classes=1):
+    """One image with n zone pairs (zone_heights) side by side in class 0, and 64 - n small far-apart boxes that are all kept,
+    dealt in turn to classes 1 .. fill_classes.  layout "adjacent": each pair is consecutive in score order (one chunk); "split":
+    all first boxes, then the filler boxes, then the second boxes (chunk 1 meets its partners among the 64 kept boxes of chunk 0).
+    Returns (rows [m, 5+C], suppressed [n])."""
     ha, hb, sup = zone_heights(thr, n, seed)
     x = np.arange(n, dtype=np.float64) * 2
     a = np.stack((x, np.zeros(n), x + 1, ha), 1)
@@ -330,5 +330,5 @@ def zone_image(thr, n, seed, layout, m=160, C=80):
         ca, cb, cf = f32(0.9) - f32(0.001) * p, f32(0.3) - f32(0.001) * p, f32(0.6) - f32(0.001) * np.arange(nf)
     d = np.zeros((m, 5 + C), f32)
     d[:2 * n + nf] = np.concatenate((rows_from_boxes(a, ca, np.zeros(n, int), C), rows_from_boxes(b, cb, np.zeros(n, int), C),
-                                     rows_from_boxes(fil, cf, np.ones(nf, int), C)), 0)
+                                     rows_from_boxes(fil, cf, 1 + np.arange(nf) % fill_classes, C)), 0)
     return d[np.random.RandomState(seed + 1).permutation(m)], sup

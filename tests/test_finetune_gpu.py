@@ -5,7 +5,7 @@
   beta gradients writes the same dx bit for bit.
 * The native trainer under a mode (tests/test_finetune_cpu.py pins which ops and outputs its backward runs): the same head tensors
   and running statistics bit for bit as the unfrozen run when only requires_grad changes, trainable gradients to the fan-out
-  order of tests/test_trainer_gpu.py against the unfrozen run and the op-by-op autograd path (YFV2_TRAIN_PYOPS=1), with eval-mode
+  order of tests/test_trainer_gpu.py against the unfrozen run and the op-by-op autograd path (model/train_ops.py), with eval-mode
   BatchNorm as close to the fp64 oracle as the reference's own fp32 path; frozen .grad stays None and eval-mode statistics and
   num_batches_tracked stay untouched.
 * FlatGradBucket with frozen parameters, mode switches on one model, nothing trainable, and train_dist.py --freeze."""
@@ -176,11 +176,10 @@ def assert_grads(got, want, trainable, shape="small"):
 
 
 def run_pyops(monkeypatch, sd, x, t, cfg, trainable, bn_eval):
-    monkeypatch.setenv("YFV2_TRAIN_PYOPS", "1")
-    try:
+    from model import train_ops
+    with monkeypatch.context() as mp:
+        mp.setattr(train_ops, "forward_train_native", train_ops.forward_train)
         return step(make_model(sd, trainable, bn_eval), x, t, cfg)
-    finally:
-        monkeypatch.delenv("YFV2_TRAIN_PYOPS")
 
 
 @pytest.mark.parametrize("shape", list(SHAPES))

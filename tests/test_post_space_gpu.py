@@ -1,13 +1,10 @@
 """Device NMS and fused decode + NMS across the code paths k_post.cu picks from its arguments: caps (max_det 1 .. the largest that
 fits in shared memory), both suppression policies (dense scan / per-class kept lists), every sort size, the exact IoU fallback,
-thresholds outside (0, 1), degenerate boxes, score ties at chunk and cap boundaries, every candidate-generation path of the
-fused kernel, and the runtime switches of INTEGRATION.md §5.  Every case is bit-exact against oracle.post (rows and kept
+thresholds outside (0, 1), degenerate boxes, score ties at chunk and cap boundaries, and every candidate-generation path of the
+fused kernel (thread-per-cell up to 80 classes, warp-per-cell above).  Every case is bit-exact against oracle.post (rows and kept
 indices) on the same input tensor; fused cases are also bit-identical to yfv2_decode followed by yfv2_nms.
 tests/post_space.py restates the host-side choices, and the tests assert that each input lands on the side it was built for."""
 import ctypes
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -20,7 +17,6 @@ import yfv2_engine as eng
 from oracle import post as opost
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def check_nms(d, ct, it, max_det=300, max_wh=4096.0):
@@ -92,30 +88,22 @@ def policy_inputs():
 CAPS = [1, 63, 64, 65, 300, 513, 1000, 4096]
 
 
-def run_caps_and_policy(lists_always=False, names=None, caps=None, max_whs=(4096.0, 1024.0, 0.0), it=0.45):
-    """Every (input, cap, max_wh) bit-exact against the oracle; caps that do not fit in shared memory are replaced by the largest
-    that does.  Returns the number of cases on the per-class list path."""
-    n_lists = 0
-    for name, (d, meant) in policy_inputs().items():
-        if names is not None and name not in names:
-            continue
-        M = d.shape[1]
-        for md in sorted(set(min(c, ps.largest_cap(M)) for c in (caps or CAPS + [ps.largest_cap(M)]))):
-            for wh in max_whs:
-                lists = ps.by_class(d[0], 0.001, it, md, wh, lists_always)
-                if not lists_always:
-                    assert lists == meant(md, wh), (name, md, wh)                  # the input is on the side it was built for
-                n_lists += lists
-                counts = check_nms(d, 0.001, it, md, wh)
-                assert int(counts[0]) > 0
-    return n_lists
-
-
 def test_caps_and_suppression_policies():
+    """Every (input, cap, max_wh) bit-exact against the oracle; caps that do not fit in shared memory are replaced by the largest
+    that does."""
     assert ps.largest_cap(6000) == 2774 and ps.largest_cap(8192) == 801 and ps.largest_cap(1815) == 4096
     assert ps.lists_fit(6000, 2774) and not ps.lists_fit(1815, ps.LIST_MIN_DET) and not ps.lists_fit(2048, ps.LIST_MIN_DET)
-    n = run_caps_and_policy()
-    assert n >= 12
+    n_lists = 0
+    for name, (d, meant) in policy_inputs().items():
+        M = d.shape[1]
+        for md in sorted(set(min(c, ps.largest_cap(M)) for c in CAPS + [ps.largest_cap(M)])):
+            for wh in (4096.0, 1024.0, 0.0):
+                lists = ps.by_class(d[0], 0.001, 0.45, md, wh)
+                assert lists == meant(md, wh), (name, md, wh)                      # the input is on the side it was built for
+                n_lists += lists
+                counts = check_nms(d, 0.001, 0.45, md, wh)
+                assert int(counts[0]) > 0
+    assert n_lists >= 12
 
 
 def test_caps_reached_inside_a_chunk():
@@ -141,17 +129,13 @@ def test_largest_cap_that_fits_and_the_next_is_refused():
 NMS_CNTS = [1, 63, 64, 65, 128, 255, 256, 257, 512, 1024, 1025, 2048, 2049, 4096, 8192]
 
 
-def run_nms_sort_sizes(cnts=NMS_CNTS):
-    for k, cnt in enumerate(cnts):
+def test_nms_sort_sizes():
+    assert sorted(set(ps.sort_size(c) for c in NMS_CNTS)) == [64, 128, 256, 512, 1024, 2048, 4096, 8192]
+    for k, cnt in enumerate(NMS_CNTS):
         M = min(ps.MAX_CAND, cnt + 37 * (k + 1))
         d = ps.random_dets(120 + k, 1, M, side=640.0, size=40.0, n_pass=cnt)
         assert len(ps.candidates(d[0], 0.001)[0]) == cnt
         check_nms(d, 0.001, 0.45, min(4096, ps.largest_cap(M)))
-
-
-def test_nms_sort_sizes():
-    assert sorted(set(ps.sort_size(c) for c in NMS_CNTS)) == [64, 128, 256, 512, 1024, 2048, 4096, 8192]
-    run_nms_sort_sizes()
 
 
 def fused_sort_case(seed, cnt, H, W, A, C):
@@ -181,16 +165,17 @@ def profiled_candidates(preds, cfg, ct, it, max_det):
 
 FUSED_CNTS = [(64, 640, 640, 3, 80), (65, 640, 640, 3, 80), (256, 640, 640, 3, 80), (257, 640, 640, 3, 80),
               (1024, 640, 640, 3, 80), (2048, 640, 640, 3, 80), (2049, 640, 640, 3, 80), (4096, 640, 640, 3, 80),
-              (2048, 384, 544, 8, 20), (8160, 384, 544, 8, 20)]
+              (2048, 384, 544, 8, 20), (8160, 384, 544, 8, 20),
+              (2049, 640, 640, 3, 96), (4096, 640, 640, 3, 96), (2048, 384, 512, 8, 96), (7680, 384, 512, 8, 96)]
 
 
-def run_fused_sort_sizes(cases=FUSED_CNTS, warp_cells=False):
-    for k, (cnt, H, W, A, C) in enumerate(cases):
+def test_fused_sort_sizes():
+    for k, (cnt, H, W, A, C) in enumerate(FUSED_CNTS):
         hs = to_dev(fused_sort_case(130 + k, cnt, H, W, A, C))
         cfg = cfg_for(A, C, H, W)
         M = (H * W // 256 + H * W // 1024) * A
-        # the warp-per-cell path stages the logits of 32 cells behind the NMS state
-        md = min(4096, ps.largest_cap(M, (5 * A + C) * 33 * 4 if warp_cells or C > 80 else 0))
+        # the warp-per-cell path (more than 80 classes) stages the logits of 32 cells behind the NMS state
+        md = min(4096, ps.largest_cap(M, (5 * A + C) * 33 * 4 if C > 80 else 0))
         dh, counts = check_fused(hs, cfg, 0.001, 0.45, md)
         assert len(ps.candidates(dh[0], 0.001)[0]) == cnt
         pc, (p_out, p_counts, p_idx) = profiled_candidates(hs, cfg, 0.001, 0.45, md)
@@ -199,48 +184,44 @@ def run_fused_sort_sizes(cases=FUSED_CNTS, warp_cells=False):
         assert torch.equal(p_out, f_out) and torch.equal(p_counts, f_counts) and torch.equal(p_idx, f_idx)
 
 
-def test_fused_sort_sizes():
-    run_fused_sort_sizes()
-
-
 # ---------------------------------------------------------------------------------------------------------------------------
 # rounding edges
 
-def run_near_midpoint_pairs(thrs=(0.3, 0.4, 0.45, 0.5), caps=(300,)):
-    outcomes = set()
-    for k, thr in enumerate(thrs):
-        a, b, above, rel = ps.near_mid_pairs(thr, 20, 140 + k, min_side=400)
-        assert rel.max() < 1e-6 and above.sum() == 20 and (~above).sum() == 20
-        for layout in ("adjacent", "split"):
-            d = np.stack([ps.pair_image(a[:40], b[:40], layout)])
-            for md in caps:
-                check_nms(d, 0.001, thr, md)
-        rows, _ = opost.nms(torch.from_numpy(ps.pair_image(a, b, "adjacent")[None]), 0.001, thr, return_indices=True)
-        outcomes.add((thr, rows[0].shape[0] < 80))
-        outcomes.add((thr, rows[0].shape[0] > 40))
-    return outcomes
+# rows per image at which the per-class kept lists fit from a cap of LIST_MIN_DET on (the rows past the candidates are zero)
+LIST_ROWS = 640
 
 
 def test_iou_within_1e6_of_the_rounding_boundary():
     """Integer-corner pairs whose IoU lies within 1e-6 of the boundary, on both sides: the fp32 pre-test must hand them to the
-    exact fp64 test, inside one chunk and against the kept list."""
-    outcomes = run_near_midpoint_pairs()
+    exact fp64 test, inside one chunk and against the kept list, under the dense scan (cap 300) and the per-class lists."""
+    outcomes = set()
+    for k, thr in enumerate((0.3, 0.4, 0.45, 0.5)):
+        a, b, above, rel = ps.near_mid_pairs(thr, 20, 140 + k, min_side=400)
+        assert rel.max() < 1e-6 and above.sum() == 20 and (~above).sum() == 20
+        for layout in ("adjacent", "split"):
+            d = np.stack([ps.pair_image(a[:40], b[:40], layout)])
+            assert not ps.by_class(d[0], 0.001, thr, 300, 4096.0)
+            check_nms(d, 0.001, thr, 300)
+            d = np.concatenate((d, np.zeros((1, LIST_ROWS - d.shape[1], d.shape[2]), d.dtype)), 1)
+            assert ps.by_class(d[0], 0.001, thr, ps.LIST_MIN_DET, 4096.0)
+            check_nms(d, 0.001, thr, ps.LIST_MIN_DET)
+        rows, _ = opost.nms(torch.from_numpy(ps.pair_image(a, b, "adjacent")[None]), 0.001, thr, return_indices=True)
+        outcomes.add((thr, rows[0].shape[0] < 80))
+        outcomes.add((thr, rows[0].shape[0] > 40))
     assert all(v for _, v in outcomes)                                       # each threshold suppresses some pairs, keeps others
 
 
-def run_zone_pairs(thrs=(0.3, 0.35, 0.4)):
-    for k, thr in enumerate(thrs):
-        for layout in ("adjacent", "split"):
-            d, sup = ps.zone_image(thr, 16, 150 + k, layout)
-            counts = check_nms(d[None], 0.001, thr, 300)
-            assert int(counts[0]) == 64 + int((~sup).sum())
-
-
 def test_iou_between_the_boundary_and_its_fp32_rounding():
-    """Pairs an fp32 estimate of the boundary alone gets wrong; the 1e-6 guard band of iou_fast must route them to iou_gt."""
-    for thr in (0.3, 0.35, 0.4):
+    """Pairs an fp32 estimate of the boundary alone gets wrong; the 1e-6 guard band of iou_fast must route them to iou_gt, under
+    the dense scan (cap 300, one class holds the fillers) and the per-class lists (fillers over two classes: no majority)."""
+    for k, thr in enumerate((0.3, 0.35, 0.4)):
         assert len(ps.zone_heights(thr, 16, 0)[0]) == 16
-    run_zone_pairs()
+        for layout in ("adjacent", "split"):
+            for m, md, fill, lists in ((160, 300, 1, False), (LIST_ROWS, ps.LIST_MIN_DET, 2, True)):
+                d, sup = ps.zone_image(thr, 16, 150 + k, layout, m=m, fill_classes=fill)
+                assert ps.by_class(d, 0.001, thr, md, 4096.0) == lists
+                counts = check_nms(d[None], 0.001, thr, md)
+                assert int(counts[0]) == 64 + int((~sup).sum())
 
 
 def test_iou_exactly_at_the_threshold():
@@ -284,7 +265,9 @@ def test_score_ties_at_a_chunk_boundary_and_at_the_cap():
 # ---------------------------------------------------------------------------------------------------------------------------
 # fused candidate generation
 
-FUSED_SHAPES = [(3, 80), (2, 80), (8, 20), (1, 1), (3, 81), (3, 256)]
+FUSED_SHAPES = [(3, 80), (2, 80), (8, 20), (1, 1), (3, 81), (3, 256), (2, 96), (8, 96)]
+# the rounding-edge inputs: every candidate-generation path, and the warp-per-cell one (more than 80 classes) at 2, 3 and 8 anchors
+EDGE_SHAPES = ((3, 80), (2, 80), (8, 20), (3, 81), (2, 96), (8, 96), (3, 256))
 
 
 def tie_heads(seed, n, H, W, A, C):
@@ -322,59 +305,34 @@ def subnormal_heads(seed, n, H, W, A, C):
     return hs
 
 
-def run_fused_shapes(shapes=FUSED_SHAPES, H=352, W=352):
-    for k, (A, C) in enumerate(shapes):
-        cfg = cfg_for(A, C, H, W)
-        hs = to_dev(heads(190 + k, 2, H, W, A, C))
+def test_fused_shapes():
+    for k, (A, C) in enumerate(FUSED_SHAPES):
+        cfg = cfg_for(A, C, 352, 352)
+        hs = to_dev(heads(190 + k, 2, 352, 352, A, C))
         for ct, it in ((0.001, 0.45), (0.3, 0.5)):
             for md in (300, 1000):
                 check_fused(hs, cfg, ct, it, md)
 
 
-def test_fused_shapes():
-    run_fused_shapes()
-
-
-def run_fused_ties(shapes=((3, 80), (2, 80), (8, 20), (3, 81))):
-    for k, (A, C) in enumerate(shapes):
+def test_fused_class_ties():
+    for k, (A, C) in enumerate(EDGE_SHAPES):
         cfg = cfg_for(A, C, 224, 224)
         check_fused(to_dev(tie_heads(200 + k, 2, 224, 224, A, C)), cfg, 0.001, 0.45)
 
 
-def test_fused_class_ties():
-    run_fused_ties()
-
-
-def run_fused_subnormal(shapes=((3, 80), (2, 80), (8, 20), (3, 81))):
-    for k, (A, C) in enumerate(shapes):
+def test_fused_subnormal_confidences():
+    """conf = p * obj below FLT_MIN carries fewer than 24 bits: a class far more than 1e-5 below the maximum can round to the
+    same product, and the reference then reports the first such class.  At the cap of 1000 the NMS takes the per-class lists
+    wherever they fit (2 and 8 anchors at 352x352)."""
+    n_lists = 0
+    for k, (A, C) in enumerate(EDGE_SHAPES):
         cfg = cfg_for(A, C, 352, 352)
         dh, counts = check_fused(to_dev(subnormal_heads(210 + k, 2, 352, 352, A, C)), cfg, 0.0, 0.45, 1000)
         assert int(counts.min()) > 0
         conf = ps.candidates(dh[0], 0.0)[1]
         assert len(conf) and conf.max() < np.finfo(np.float32).tiny
-
-
-def test_fused_subnormal_confidences():
-    """conf = p * obj below FLT_MIN carries fewer than 24 bits: a class far more than 1e-5 below the maximum can round to the
-    same product, and the reference then reports the first such class."""
-    run_fused_subnormal()
-
-
-# ---------------------------------------------------------------------------------------------------------------------------
-# runtime switches: read once per process, so each runs in a child
-
-SWITCH_RUNS = {
-    "YFV2_NMS_WARP_PER_CELL": "T.run_fused_shapes([(3, 80), (2, 80), (8, 20)]); T.run_fused_ties(); T.run_fused_subnormal(); "
-                              "T.run_fused_sort_sizes(T.FUSED_CNTS[6:], warp_cells=True)",
-    "YFV2_NMS_LISTS": "assert T.run_caps_and_policy(True, ['m1815', 'm2048', 'm6000_640'], [64, 65, 300, 338]) >= 4; "
-                      "T.run_near_midpoint_pairs(caps=(64, 300)); T.run_zone_pairs(); T.run_fused_subnormal([(3, 80), (8, 20)])",
-}
-
-
-@pytest.mark.parametrize("switch", list(SWITCH_RUNS))
-def test_runtime_switch(switch):
-    code = "import sys; sys.path[:0] = [%r, %r]; import test_post_space_gpu as T; %s; print('ok')" % (
-        ROOT, os.path.join(ROOT, "tests"), SWITCH_RUNS[switch])
-    env = dict(os.environ, **{switch: "1"})
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, cwd=ROOT, timeout=600)
-    assert r.returncode == 0 and r.stdout.strip().endswith("ok"), r.stderr[-3000:]
+        for x in dh:
+            lists = ps.by_class(x, 0.0, 0.45, 1000, 4096.0)
+            assert lists == ps.lists_fit(x.shape[0], 1000), (A, C)
+            n_lists += lists
+    assert n_lists == 8

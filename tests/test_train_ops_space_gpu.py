@@ -3,12 +3,7 @@ and the elementwise bound of tests/test_train_fp64_gpu.py.  This covers the cell
 (tests/train_dispatch.py): base pointers only 4-byte aligned, HW%4 != 0, K = 24 with M = 48 / 72, the generic stem, 5x5 at
 stride 2, H or W = 1, maps smaller than the stencil, N > 16, HW > 1024, 64 BatchNorm slices, a large mean over a small spread;
 and the special values where the kernels must do what torch does: NaN and +-inf through BatchNorm + ReLU and max-pool, exact ties
-and all-equal windows, and the refusal of a BatchNorm over one value per channel.  YFV2_TRAIN_GEMM_OLD and YFV2_TRAIN_WGRAD_TILED
-are read once into a static, so each runs the conv1x1 cases again in a child process."""
-import os
-import subprocess
-import sys
-
+and all-equal windows, and the refusal of a BatchNorm over one value per channel."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -277,7 +272,8 @@ def test_one_value_per_channel_is_refused_like_torch(pyops, monkeypatch):
     import model.detector as det
     import synth
     if pyops:
-        monkeypatch.setenv("YFV2_TRAIN_PYOPS", "1")
+        from model import train_ops
+        monkeypatch.setattr(train_ops, "forward_train_native", train_ops.forward_train)
     m = det.Detector(80, 3, True)
     m.load_state_dict(synth.make_state_dict(5), strict=True)
     m = m.cuda().train()
@@ -289,17 +285,3 @@ def test_one_value_per_channel_is_refused_like_torch(pyops, monkeypatch):
     with pytest.raises(ValueError, match="Expected more than 1 value per channel when training"):
         F.batch_norm(torch.ones(1, 96, 1, 1, device="cuda"), None, None, training=True)
     m(synth.make_images(6, 1, 32, 64).cuda())                                          # two values per channel: accepted
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("var", ["YFV2_TRAIN_GEMM_OLD", "YFV2_TRAIN_WGRAD_TILED"])
-def test_conv1x1_switches_in_a_child_process(var):
-    """The conv1x1 cases again with a kernel switch set (read once into a static, hence a fresh process)."""
-    if os.environ.get(var):
-        pytest.skip("already inside the child run")
-    here = os.path.dirname(os.path.abspath(__file__))
-    env = dict(os.environ, **{var: "1"})
-    r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", "-m", "gpu", "-k", "test_conv1x1 and not switches",
-                        os.path.join(here, "test_train_ops_space_gpu.py")], capture_output=True, text=True, env=env, cwd=os.path.dirname(here))
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
-    assert "%d passed" % len(PW) in r.stdout, r.stdout[-2000:]

@@ -1,5 +1,5 @@
 """The native trainer (csrc/trainer.cu: yfv2_train_forward / yfv2_train_backward, one C-ABI call each) against the op-by-op
-autograd composition of the same kernels (model/train_ops.py, YFV2_TRAIN_PYOPS=1), which tests/test_train_gpu.py and
+autograd composition of the same kernels (model/train_ops.py), which tests/test_train_gpu.py and
 tests/test_train_ops_gpu.py pin to the reference: same head tensors and running statistics bit for bit, parameter gradients to
 fp32 summation order; gradient accumulation, the flat-bucket fast path and the one-batch-in-flight guard."""
 import numpy as np
@@ -32,10 +32,11 @@ def test_native_equals_op_by_op_autograd(monkeypatch):
     x = synth.make_images(72, 4, 96, 128).cuda()
     targets = synth.make_targets(73, 4).cuda()
     cfg = synth.coco_cfg(128, 96)
-    monkeypatch.setenv("YFV2_TRAIN_PYOPS", "1")
-    ma = make_model(sd)
-    pa, la = run(ma, x, targets, cfg)
-    monkeypatch.delenv("YFV2_TRAIN_PYOPS")
+    from model import train_ops
+    with monkeypatch.context() as mp:
+        mp.setattr(train_ops, "forward_train_native", train_ops.forward_train)
+        ma = make_model(sd)
+        pa, la = run(ma, x, targets, cfg)
     mb = make_model(sd)
     pb, lb = run(mb, x, targets, cfg)
     for a, b in zip(pa, pb):

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
-"""A/B helper: dumps the six head tensors and every block tap for a few seeded inputs to an .npz, so two builds /
-environment settings (e.g. YFV2_NO_PDL=1 vs default) can be compared bit for bit with --cmp."""
+"""A/B helper: dumps the six head tensors and every block tap for a few seeded inputs to an .npz, so two builds can be
+compared bit for bit (e.g. `ab_dump.py old.npz` in a build of the parent commit, `ab_dump.py new.npz` in a build of the
+change, then `ab_dump.py --cmp old.npz new.npz`)."""
 import os
 import sys
 

@@ -208,7 +208,6 @@ struct NmsParams {
     double iou_thres;
     double iou_mid;    // fl32(q) > iou_thres  <=>  q > iou_mid (or >= when iou_tie_up), see iou_gt()
     float iou_mid_f;   // (float)iou_mid: a 1e-6-wide fp32 pre-test decides almost every pair without the fp64 product
-    int list_min_det;    // per-class kept lists only for max_det >= this (YFV2_NMS_LISTS=1: always, for the tests of that path)
     float iou_fast_mid;  // iou_fast(): iou_mid_f, or NaN when iou_mid <= 0 (every pair then takes the exact path)
     float iou_zero;      // iou_fast(): 0 (an empty intersection is below a positive threshold), or NaN when iou_mid <= 0
     int iou_tie_up;
@@ -490,7 +489,7 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
     // (since the dense scan went branch-free it is the faster one while the kept list is short -- configs[4] sets, cap 300: 2.9 / 2.5 ms
     // per 10 000 images against 3.4 / 2.9 with the lists -- so the lists are only used for caps above kNmsListMinDet)
     bool by_class = s.lists_fit && s.misc->outside == 0u && p.iou_mid > 0.0 && p.max_wh > 0.f && p.C <= kNmsListClasses &&
-                    p.max_det >= p.list_min_det;
+                    p.max_det >= kNmsListMinDet;
     if (by_class) {
         for (int i = threadIdx.x; i < kNmsListClasses; i += NT) s.chist[i] = 0u;
         if (threadIdx.x == 0) s.misc->majority = 0u;
@@ -1258,8 +1257,6 @@ int fill_nms(NmsParams& p, int M, float conf_thres, double iou_thres, const int*
     while (p.MCp < M) p.MCp <<= 1;
     p.C = 1 << 30;                                           // callers that know the class count set it
     p.prof = nullptr;
-    static const bool lists_always = getenv("YFV2_NMS_LISTS") != nullptr;
-    p.list_min_det = lists_always ? 0 : kNmsListMinDet;
     return YFV2_OK;
 }
 
@@ -1280,8 +1277,7 @@ int decode_nms_prepare(DecodeNmsLaunch& d, const float* const preds[6], int N, i
     if (rc) return rc;
     d.p.C = C;
     d.p.prof = g_nms_prof;
-    static const bool warp_cells = getenv("YFV2_NMS_WARP_PER_CELL") != nullptr;
-    const int fast = (C > kCT || warp_cells) ? 0 : (C == kCT && A == 3) ? 2 : 1;
+    const int fast = C > kCT ? 0 : (C == kCT && A == 3) ? 2 : 1;
     static void (*const kernels[2][3])(PostGeom, NmsParams) = {
         {decode_nms_kernel<false, 0>, decode_nms_kernel<false, 1>, decode_nms_kernel<false, 2>},
         {decode_nms_kernel<true, 0>, decode_nms_kernel<true, 1>, decode_nms_kernel<true, 2>}};

@@ -4,83 +4,19 @@
 // the arithmetic is ours.  Round-1 goal here is correctness against the reference's autograd (tests/test_train_gpu.py);
 // these are straightforward FFMA kernels, not yet the fused tensor-core path of the inference engine.
 //
-//   conv1x1   fwd / dgrad / wgrad (+bias)      one generic strided batched GEMM (64x64x16 tiles, 4x4 micro-tiles)
+//   conv1x1   fwd / dgrad / wgrad (+bias)      batched GEMM over pixels (BM x 128 tiles); wgrad by pixel-sliced partial sums
 //   dwconv    fwd / dgrad / wgrad              3x3 or 5x5, stride 1 or 2, pad k/2      (shufflenetv2.py:25,36; fpn.py:12,19)
 //   stem conv fwd / wgrad                      dense 3x3 s2 p1, 3->24                   (shufflenetv2.py:75)
 //   batchnorm train fwd / bwd (+ReLU)          batch statistics, running-stat update    (nn.BatchNorm2d, momentum .1, eps 1e-5)
 //   maxpool 3x3 s2 p1 fwd / bwd, nearest 2x upsample fwd / bwd                           (shufflenetv2.py:80; fpn.py:57)
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace yfv2 {
 namespace {
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Generic batched GEMM with arbitrary strides:  C[b](i,j) (+)= sum_k A[b](i,k) * B[b](k,j)
-// ---------------------------------------------------------------------------------------------------------------------
-struct GemmArgs {
-    const float* A; const float* B; float* C;
-    int M, N, K, batch;
-    long long sAi, sAk, sAb, sBk, sBj, sBb, sCi, sCj, sCb;
-    const float* bias;      // per-row (i) bias added once (only when !atomic), may be null
-    int atomic;             // atomicAdd into C (reduction over the batch dimension with sCb == 0)
-};
-
-__global__ void __launch_bounds__(256)
-gemm_kernel(GemmArgs g) {
-    __shared__ float As[16][64 + 4];
-    __shared__ float Bs[16][64 + 4];
-    const int b = blockIdx.z;
-    const int i0 = blockIdx.y * 64, j0 = blockIdx.x * 64;
-    const float* A = g.A + b * g.sAb;
-    const float* B = g.B + b * g.sBb;
-    float* C = g.C + b * g.sCb;
-    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-    float acc[4][4];
-#pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) acc[a][c] = 0.f;
-    for (int k0 = 0; k0 < g.K; k0 += 16) {
-        for (int t = threadIdx.x; t < 16 * 64; t += 256) {
-            const int kk = t >> 6, ii = t & 63;
-            const int k = k0 + kk;
-            As[kk][ii] = (k < g.K && i0 + ii < g.M) ? A[(long long)(i0 + ii) * g.sAi + (long long)k * g.sAk] : 0.f;
-            Bs[kk][ii] = (k < g.K && j0 + ii < g.N) ? B[(long long)k * g.sBk + (long long)(j0 + ii) * g.sBj] : 0.f;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < 16; ++kk) {
-            float a[4], bb[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) { a[q] = As[kk][ty * 4 + q]; bb[q] = Bs[kk][tx * 4 + q]; }
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-#pragma unroll
-                for (int r = 0; r < 4; ++r) acc[q][r] = fmaf(a[q], bb[r], acc[q][r]);
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        const int i = i0 + ty * 4 + q;
-        if (i >= g.M) continue;
-        const float bv = (g.bias && !g.atomic) ? g.bias[i] : 0.f;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const int j = j0 + tx * 4 + r;
-            if (j >= g.N) continue;
-            float* dst = C + (long long)i * g.sCi + (long long)j * g.sCj;
-            if (g.atomic) atomicAdd(dst, acc[q][r]);
-            else *dst = acc[q][r] + bv;
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
 // conv1x1 forward / dgrad: C[b](i, j) = sum_k A(i, k) B[b](k, j) with j = pixel (contiguous in B and C), A the weight matrix
-// (shared by the batch; k- or i-contiguous).  torch.profiler on the round-1 generic kernel above: 153 launches, 7.8 ms of a
+// (shared by the batch; k- or i-contiguous).  torch.profiler on the round-1 generic GEMM it replaced: 153 launches, 7.8 ms of a
 // 22.6 ms batch-64 step (4.5 TFLOP/s): scalar loads with 64-bit index math per element, 4x4 micro-tiles, and a 64-row tile
 // for 24-row outputs.  Here: BM x 128 tiles (BM = 32 for the 24-channel layers, 64 otherwise), 16-deep k slabs, float4 loads of the
 // pixel-contiguous operand, TM x 4 micro-tiles (TM = BM / 8), next slab prefetched into registers while the current one is
@@ -336,13 +272,6 @@ wgrad_rows_kernel(const float* __restrict__ dy, const float* __restrict__ x, flo
                 if (partial) dst[(long long)(m0 + q) * KK + k] = v; else atomicAdd(dst + (long long)(m0 + q) * KK + k, v);
             }
         }
-}
-
-int run_gemm(const GemmArgs& g, cudaStream_t s) {
-    dim3 grid((g.N + 63) / 64, (g.M + 63) / 64, g.batch);
-    gemm_kernel<<<grid, 256, 0, s>>>(g);
-    YFV2_LAUNCH_CHECK();
-    return YFV2_OK;
 }
 
 // per-row sums of dy [N,M,HW] -> dbias[M]
@@ -821,11 +750,6 @@ using namespace yfv2;
 // y[n][m][p] = sum_k w[m][k] x[n][k][p] (+ bias[m])
 extern "C" YFV2_API int yfv2_op_conv1x1_fwd(const float* x, const float* w, const float* bias, float* y, int N, int K, int M, int HW, void* stream) {
     ARGCHK(x && w && y && N > 0 && K > 0 && M > 0 && HW > 0, "conv1x1_fwd: bad arguments");
-    static const bool old_gemm = getenv("YFV2_TRAIN_GEMM_OLD") != nullptr;      // round-1 generic kernel, kept for A/B runs
-    if (old_gemm) {
-        GemmArgs g{w, x, y, M, HW, K, N, K, 1, 0, HW, 1, (long long)K * HW, HW, 1, (long long)M * HW, bias, 0};
-        return run_gemm(g, (cudaStream_t)stream);
-    }
     Gemm2Args g{w, x, y, M, HW, K, N, K, 1, HW, (long long)K * HW, HW, (long long)M * HW, bias};
     return run_gemm2(g, (cudaStream_t)stream);
 }
@@ -836,26 +760,13 @@ namespace yfv2 {
 int conv1x1_bwd_impl(const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias, int N, int K, int M, int HW,
                      float* wscratch, size_t wscratch_floats, cudaStream_t s) {
     if (!(x && w && dy && N > 0 && K > 0 && M > 0 && HW > 0)) { set_error("conv1x1_bwd: bad arguments"); return YFV2_EINVAL; }
-    static const bool old_gemm = getenv("YFV2_TRAIN_GEMM_OLD") != nullptr;
-    static const bool tiled_only = getenv("YFV2_TRAIN_WGRAD_TILED") != nullptr;
     if (dx) {
-        int rc;
-        if (old_gemm) {
-            GemmArgs g{w, dy, dx, K, HW, M, N, 1, K, 0, HW, 1, (long long)M * HW, HW, 1, (long long)K * HW, nullptr, 0};
-            rc = run_gemm(g, s);
-        } else {
-            Gemm2Args g{w, dy, dx, K, HW, M, N, 1, K, HW, (long long)M * HW, HW, (long long)K * HW, nullptr};      // A(i=k, kk=m) = w[m][k]
-            rc = run_gemm2(g, s);
-        }
+        Gemm2Args g{w, dy, dx, K, HW, M, N, 1, K, HW, (long long)M * HW, HW, (long long)K * HW, nullptr};      // A(i=k, kk=m) = w[m][k]
+        const int rc = run_gemm2(g, s);
         if (rc) return rc;
     }
     if (dw) {
-        if (old_gemm) {
-            YFV2_CUDA(cudaMemsetAsync(dw, 0, (size_t)M * K * sizeof(float), s));
-            GemmArgs g{dy, x, dw, M, K, HW, N, HW, 1, (long long)M * HW, 1, HW, (long long)K * HW, K, 1, 0, nullptr, 1};
-            int rc = run_gemm(g, s);
-            if (rc) return rc;
-        } else if (K == 24 && M % 24 == 0 && !tiled_only) {      // (K = 48: 50 loads per 96 FMAs per lane measured 250 us per layer; the tiled kernel wins)
+        if (K == 24 && M % 24 == 0) {      // (K = 48: 50 loads per 96 FMAs per lane measured 250 us per layer; the tiled kernel wins)
             // pixel slices sized so that the grid has about two waves whatever the map size
             int pchunk = 2048;
             while (pchunk > 256 && (long long)N * (M / 24) * ((HW + pchunk - 1) / pchunk) < 2LL * sm_count()) pchunk >>= 1;

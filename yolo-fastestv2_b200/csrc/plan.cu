@@ -33,10 +33,9 @@ void set_error(const char* fmt, ...) {
 static thread_local bool g_pdl_next = false;
 static thread_local bool g_pdl_call = true;      // false inside yfv2_detect_u8_host: with copies and a second stream in flight the
                                                  // early-resident dependents cost more than the hidden prologues save (measured)
-static const bool g_pdl_off = getenv("YFV2_NO_PDL") != nullptr;
-bool pdl_take() { const bool r = g_pdl_next && g_pdl_call && !g_pdl_off; g_pdl_next = true; return r; }
+bool pdl_take() { const bool r = g_pdl_next && g_pdl_call; g_pdl_next = true; return r; }
 void pdl_reset() { g_pdl_next = false; }
-bool pdl_allowed() { return g_pdl_call && !g_pdl_off; }
+bool pdl_allowed() { return g_pdl_call; }
 
 int sm_count() {
     static thread_local int n = 0;

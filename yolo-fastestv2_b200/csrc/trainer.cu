@@ -83,7 +83,6 @@ struct yfv2_trainer {
     struct GraphSlot { cudaGraphExec_t exec = nullptr; unsigned long long key = 0; };
     GraphSlot g_fwd, g_bwd[2];
     cudaStream_t cap_stream = nullptr;
-    bool use_graphs = true;
 };
 
 namespace yfv2 {
@@ -644,17 +643,11 @@ extern "C" int yfv2_train_forward(yfv2_trainer* t, const float* x, const float* 
     for (int i = 0; i < YFV2_NUM_PARAMS; ++i) if (!params[i]) { set_error("train_forward: null parameter %d", i); return YFV2_EINVAL; }
     for (int i = 0; i < 2 * YFV2_NUM_BN; ++i) if (!bn_running[i]) { set_error("train_forward: null BN buffer %d", i); return YFV2_EINVAL; }
     cudaStream_t s = (cudaStream_t)stream;
-    static const bool no_graph = getenv("YFV2_TRAIN_NOGRAPH") != nullptr;
-    int rc;
-    if (no_graph || !t->use_graphs) {
-        rc = run_forward(t, x, params, bn_running, preds, workspace, s);
-    } else {
-        unsigned long long key = mix(mix(mix(0x1234ull, t->mode_hash), x), workspace);
-        for (int i = 0; i < YFV2_NUM_PARAMS; ++i) key = mix(key, params[i]);
-        for (int i = 0; i < 2 * YFV2_NUM_BN; ++i) key = mix(key, bn_running[i]);
-        for (int i = 0; i < 6; ++i) key = mix(key, preds[i]);
-        rc = replay_or_capture(t, t->g_fwd, key, s, [&](cudaStream_t cs) { return run_forward(t, x, params, bn_running, preds, workspace, cs); });
-    }
+    unsigned long long key = mix(mix(mix(0x1234ull, t->mode_hash), x), workspace);
+    for (int i = 0; i < YFV2_NUM_PARAMS; ++i) key = mix(key, params[i]);
+    for (int i = 0; i < 2 * YFV2_NUM_BN; ++i) key = mix(key, bn_running[i]);
+    for (int i = 0; i < 6; ++i) key = mix(key, preds[i]);
+    const int rc = replay_or_capture(t, t->g_fwd, key, s, [&](cudaStream_t cs) { return run_forward(t, x, params, bn_running, preds, workspace, cs); });
     if (rc == YFV2_OK) { t->fwd_trainable = t->trainable; t->fwd_bn_eval = t->bn_eval; }
     return rc;
 }
@@ -670,8 +663,6 @@ extern "C" int yfv2_train_backward(yfv2_trainer* t, const float* x, const float*
         return YFV2_EINVAL;
     }
     cudaStream_t s = (cudaStream_t)stream;
-    static const bool no_graph = getenv("YFV2_TRAIN_NOGRAPH") != nullptr;
-    if (no_graph || !t->use_graphs) return run_backward(t, x, params, preds, dpreds, grads_flat, accumulate, workspace, s);
     unsigned long long key = mix(mix(mix(mix(0x4321ull, t->mode_hash), x), workspace), grads_flat);
     for (int i = 0; i < YFV2_NUM_PARAMS; ++i) key = mix(key, params[i]);
     for (int i = 0; i < 6; ++i) key = mix(mix(key, preds[i]), dpreds[i]);

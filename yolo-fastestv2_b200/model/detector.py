@@ -135,11 +135,11 @@ class Detector(nn.Module):
             self.invalidate_packed()                      # the BN running statistics are updated through raw pointers
             x = x.float() if x.dtype != torch.float32 else x
             yfv2_engine.check_bn_batch(x.shape[0], x.shape[2], x.shape[3])
-            # default: the native trainer (csrc/trainer.cu), one C-ABI call for the forward and one for the backward;
-            # YFV2_TRAIN_PYOPS=1 keeps the op-by-op autograd composition (the path the operator tests pin).  Both follow, per
-            # call, each parameter's requires_grad and each BatchNorm module's own .training (model.backbone.eval() freezes
-            # the backbone's statistics as in PyTorch); self.training only chooses training over the inference plan
-            if os.environ.get("YFV2_TRAIN_PYOPS") or x.shape[2] % 32 or x.shape[3] % 32:
+            # the native trainer (csrc/trainer.cu), one C-ABI call for the forward and one for the backward; H or W not a
+            # multiple of 32 takes the op-by-op autograd composition.  Both follow, per call, each parameter's requires_grad
+            # and each BatchNorm module's own .training (model.backbone.eval() freezes the backbone's statistics as in
+            # PyTorch); self.training only chooses training over the inference plan
+            if x.shape[2] % 32 or x.shape[3] % 32:
                 return train_ops.forward_train(self, x)
             return train_ops.forward_train_native(self, x)
         if x.dim() != 4 or x.shape[1] != 3:

@@ -252,7 +252,7 @@ class NetTrainFn(torch.autograd.Function):
         tr = ctx.tr
         if tr.generation != ctx.gen:
             raise RuntimeError("yfv2: the native trainer keeps ONE batch's activations per input shape; call backward() before the next "
-                               "train-mode forward of that shape (or set YFV2_TRAIN_PYOPS=1 for the op-by-op autograd path)")
+                               "train-mode forward of that shape")
         # the trainable parameters, each with its slot of the flat buffer (frozen ones have offset -1)
         live = [(p, off, num) for p, (off, num) in zip(ctx.params, tr.param_offsets) if off >= 0]
         # fast path: .grad tensors are the slices of one flat bucket, in order
