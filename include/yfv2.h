@@ -724,6 +724,54 @@ typedef struct yfv2_launch {
 YFV2_API int yfv2_plan_debug_launches(const yfv2_plan* plan, const void* workspace, int is_u8, int sms, yfv2_launch* out, int cap,
                                       int* n);
 
+/* ---- test hooks: the kernel launches of the training operators and of a native training step, as the calls choose them -------
+ * Host only: nothing is launched and no address is dereferenced; the addresses only decide float4 access (16-byte alignment).
+ * sms: the GPU's multiprocessors (0: this device's count, 132 without a device).  Write min(cap, count) records and return the
+ * count in *n (cap 0 with a NULL array queries it); an argument the call would refuse is refused with the same code and message.
+ *   yfv2_op_debug_launches: one yfv2_op_* call.  op: YFV2_OP_*; ptrs / ints: that call's pointer and integer arguments in signature
+ *     order (the stream omitted), all of them: the arrays are read as long as that call's signature.
+ *   yfv2_trainer_debug_launches: one training step under the trainer's current mode, the records yfv2_train_forward then
+ *     yfv2_train_backward (accumulate = 0) capture into their CUDA graphs.  workspace: its address decides the alignment of the
+ *     workspace tensors (NULL: a 16-byte-aligned workspace); the image, parameters, BatchNorm buffers, head tensors and flat gradient
+ *     buffer are taken as 16-byte aligned.
+ * A record:
+ *   kernel:  the demangled name after yfv2::(anonymous namespace)::, without spaces ("gemm2_kernel<32>", "wgrad_rows_kernel<24,3>"),
+ *            or "memset" (cudaMemsetAsync of `bytes` to 0)
+ *   op, bwd: trainer: index into yfv2_trainer_debug_ops of the op the launch belongs to (-1: the copies into grads_flat) and 1 in
+ *            the backward; op calls: -1, 0
+ *   grid, block, smem: launch geometry (smem: dynamic shared memory, bytes)
+ *   bm: gemm2_kernel's tile height; vec_b, vec_c: gemm2_kernel's float4 access of B (the pixel-contiguous input) and C (the output);
+ *   vec: float4 access of bn_stats_kernel, bn_apply_kernel and bn_eval_bwd_apply_kernel
+ *   pchunk, chunks, partial: the 1x1 weight gradient's pixels per block slice, slices per image, and 1 for per-block partial sums
+ *            (summed by wgrad_reduce_kernel) where 0 adds into the zeroed gradient with atomics
+ *   slices: image slices (grid[1]) of bn_stats_kernel / bn_bwd_reduce_kernel; accumulate: chan_copy_kernel / axpy_kernel add to
+ *            their destination */
+#define YFV2_OP_CONV1X1_FWD   0
+#define YFV2_OP_CONV1X1_BWD   1
+#define YFV2_OP_DWCONV_FWD    2
+#define YFV2_OP_DWCONV_BWD    3
+#define YFV2_OP_STEM_FWD      4
+#define YFV2_OP_STEM_WGRAD    5
+#define YFV2_OP_BN_TRAIN_FWD  6
+#define YFV2_OP_BN_TRAIN_BWD  7
+#define YFV2_OP_BN_EVAL_FWD   8
+#define YFV2_OP_BN_EVAL_BWD   9
+#define YFV2_OP_MAXPOOL_FWD   10
+#define YFV2_OP_MAXPOOL_BWD   11
+#define YFV2_OP_UPSAMPLE2_FWD 12
+#define YFV2_OP_UPSAMPLE2_BWD 13
+typedef struct yfv2_train_launch {
+    char kernel[32];
+    int op, bwd;
+    int grid[3], block;
+    long long smem, bytes;
+    int bm, vec_b, vec_c, vec;
+    int pchunk, chunks, partial;
+    int slices, accumulate;
+} yfv2_train_launch;
+YFV2_API int yfv2_op_debug_launches(int op, const void* const* ptrs, const int* ints, int sms, yfv2_train_launch* out, int cap, int* n);
+YFV2_API int yfv2_trainer_debug_launches(const yfv2_trainer* t, const void* workspace, int sms, yfv2_train_launch* out, int cap, int* n);
+
 /* ---- test hook: one pointwise contraction on the tensor-core engine (3xTF32), out[n][p] = sum_k w[n][k]*x[k][p] ----
  * x: [K][P], w: [N][K], out: [N][P], pack_ws: unused (kept for ABI stability), may be NULL. */
 YFV2_API int yfv2_debug_pw_tc(const float* x, const float* w, float* out, float* pack_ws, int K, int N, int P,

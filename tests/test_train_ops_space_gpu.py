@@ -40,18 +40,31 @@ UP = [(2, 3, 5, 7), (1, 2, 1, 1)]
 
 
 def case_cells(sms):
+    """The cells the op calls of this suite reach, from the library's records of those calls (yfv2_op_debug_launches) at the
+    addresses buf() / empty() give: a 256-byte-aligned allocation, `off` floats into it."""
+    at = lambda off: (1 << 20) + 4 * off
+    a0 = at(0)
     out = set()
     for n, k, m, h, w, bias, off in PW:
-        out |= td.pw_cells(n, k, m, h * w, sms, bias, 0, off == 0, off == 0)
+        p = at(off)
+        out |= td.op_cells("conv1x1_fwd", [p, p, p if bias else None, p], [n, k, m, h * w], sms)
+        out |= td.op_cells("conv1x1_bwd", [p, p, p, p, p, p if bias else None], [n, k, m, h * w], sms)
     for n, c, h, w, ks, s in DW:
-        out |= td.dw_cells(n, c, h, w, ks, s)
+        out |= td.op_cells("dwconv_fwd", [a0] * 3, [n, c, h, w, ks, s], sms)
+        out |= td.op_cells("dwconv_bwd", [a0] * 5, [n, c, h, w, ks, s], sms)
     for n, c, h, w, relu, _, _, off in BN:
-        out |= td.bn_cells(n, c, h * w, relu, off == 0)
+        p = at(off)
+        out |= td.op_cells("bn_train_fwd", [p, a0, a0, a0, a0, p, a0, a0, a0], [n, c, h * w, int(relu)], sms)
+        out |= td.op_cells("bn_train_bwd", [p, p, p, a0, a0, a0, p, a0, a0, a0], [n, c, h * w, int(relu)], sms)
     for n, m, h, w in STEM:
-        out |= td.stem_cells(n, m, h, w)
+        out |= td.op_cells("stem_fwd", [a0] * 3, [n, m, h, w], sms)
+        out |= td.op_cells("stem_wgrad", [a0] * 3, [n, m, h, w], sms)
     for n, c, h, w in POOL:
-        out |= td.pool_cells(h, w)
-    out.add(("upsample", "2x"))
+        out |= td.op_cells("maxpool_fwd", [a0] * 3, [n * c, h, w], sms)
+        out |= td.op_cells("maxpool_bwd", [a0] * 3, [n * c, h, w], sms)
+    for n, c, h, w in UP:
+        out |= td.op_cells("upsample2_fwd", [a0] * 2, [n * c, h, w], sms)
+        out |= td.op_cells("upsample2_bwd", [a0] * 2, [n * c, h, w], sms)
     return out
 
 

@@ -1,104 +1,102 @@
-"""Python model of the host choices of the training kernels (csrc/k_train.cu) and of the native trainer's program
-(csrc/trainer.cu).
+"""Which kernel variants (cells) the training operators (csrc/k_train.cu) and the native trainer's step (csrc/trainer.cu) reach,
+read from the library's own launch records (yfv2_op_debug_launches / yfv2_trainer_debug_launches), and an independent statement of
+the trainer's program.
 
-Every rule below restates the C++ source named beside it.  A *cell* is one (operator, variant) pair, e.g. ("wgrad", "rows /
-partial / multi-chunk") or ("bn_stats", "float4"); pw_cells() / dw_cells() / bn_cells() / stem_cells() / pool_cells() give the
-cells one yfv2_op_* call reaches, trainer_cells() the cells a training step of the native trainer at (N, H, W, A, C) reaches.  `find_case()` searches trainer shapes for one that reaches
-a given cell.  tests/test_train_dispatch_cpu.py pins `program()` against the trainer's own op list (yfv2_trainer_debug_ops) and
-checks that the case lists of tests/test_train_fp64_gpu.py and tests/test_train_ops_space_gpu.py reach every cell."""
+A *cell* is one (site, variant) pair, e.g. ("wgrad", "rows / partial / multi-chunk") or ("bn_stats", "float4"): the dispatch cells
+come from the records (kernel, tile height, float4 choices, pixel chunks, partial sums, BatchNorm slices, grids), the input-shape
+cells (maps smaller than the stencil, odd inputs, ReLU, bias, ...) from the op's shapes.  op_cells() gives the cells of one
+yfv2_op_* call, trainer_cells() those of one training step of a library trainer at (N, H, W, A, C); `find_case()` searches
+trainer shapes for one that reaches a given cell.  tests/test_train_dispatch_cpu.py pins `program()` against the trainer's own op
+list (yfv2_trainer_debug_ops) and checks that the case lists of tests/test_train_fp64_gpu.py and tests/test_train_ops_space_gpu.py
+reach every cell."""
+import ctypes
 import functools
 
-K_WSCRATCH_FLOATS = 4 << 20          # trainer.cu kWScratchFloats: per-block weight-gradient partials of one layer
 STAGE_REPEATS = (4, 8, 4)            # trainer.cu kStageRepeats
 STAGE_OUT = (48, 96, 192)            # trainer.cu kStageOut
 
 
-# ---- k_train.cu host rules --------------------------------------------------------------------------------------------------
-def gemm2(M, N, sB, sC, b_aligned=True, c_aligned=True):
-    """run_gemm2 / gemm2_kernel: the tile height and the float4 conditions of B and C.  sB = (sBk, sBb), sC = (sCi, sCb)."""
-    bm = 32 if M <= 32 else 64                                                       # run_gemm2: g.M <= 32
-    vec_b = N % 4 == 0 and all(s % 4 == 0 for s in sB) and b_aligned                 # gemm2_kernel vecB (B 16-byte aligned)
-    vec_c = N % 4 == 0 and all(s % 4 == 0 for s in sC) and c_aligned                 # gemm2_kernel vecC
-    return bm, vec_b, vec_c
-
-
-def gemm2_variant(vec, hw):
-    return "float4" if vec else "scalar: HW%4" if hw % 4 else "scalar: unaligned"
-
-
-def wgrad(N, K, M, HW, sms, scratch_floats=0, tiled_only=False):
-    """conv1x1_bwd_impl's weight-gradient choice: (kernel, pchunk, chunks, partial, row groups)."""
-    if K == 24 and M % 24 == 0 and not tiled_only:                                   # wgrad_rows_kernel<24, 3>
-        pchunk = 2048
-        while pchunk > 256 and N * (M // 24) * -(-HW // pchunk) < 2 * sms:
-            pchunk >>= 1
-        kern, groups = "rows", M // 24
-    else:
-        bt = 32 if M <= 32 and K <= 32 else 64                                       # wgrad1x1_kernel<BT>
-        tiles = -(-M // bt) * -(-K // bt)
-        pchunk = 1024
-        while pchunk > 64 and tiles * N * -(-HW // pchunk) < 4 * sms:
-            pchunk >>= 1
-        kern, groups = "tiled%d" % bt, 1
-    chunks = -(-HW // pchunk)
-    partial = scratch_floats > 0 and N * chunks * M * K <= scratch_floats           # else memset + fp32 atomics
-    return kern, pchunk, chunks, partial, groups
-
-
-def bn_slices(N, HW):                                                                # yfv2_op_bn_train_fwd / _bwd
-    s = -(-(N * HW) // (256 * 16))
-    s = min(max(s, 1), 64)
-    return min(s, N)
-
-
+# ---- cells of launch records --------------------------------------------------------------------------------------------------
 def bucket_slices(s):
     return "1" if s == 1 else "64 (cap)" if s == 64 else "2..63"
 
 
-# ---- cells of one op call -----------------------------------------------------------------------------------------------------
-def pw_cells(N, K, M, HW, sms, bias=False, scratch_floats=0, x_aligned=True, y_aligned=True, dx=True, tiled_only=False):
-    """yfv2_op_conv1x1_fwd + conv1x1_bwd_impl: x [N,K,HW] -> y [N,M,HW]."""
+def shape_cells(kind, s):
+    """The input-shape cells of one op: kind as yfv2_trainer_op.kind, s = dict(N, C, H, W) of its input (+ M, ks, stride, relu,
+    bias where the op has them)."""
     out = set()
-    bm, vb, vc = gemm2(M, HW, (HW, K * HW), (HW, M * HW), x_aligned, y_aligned)      # forward: B = x, C = y
-    out |= {("gemm2", "BM=%d" % bm), ("gemm2 B", gemm2_variant(vb, HW)), ("gemm2 C", gemm2_variant(vc, HW))}
-    if dx:
-        bm, vb, vc = gemm2(K, HW, (HW, M * HW), (HW, K * HW), y_aligned, x_aligned)  # dgrad: B = dy, C = dx
-        out |= {("gemm2", "BM=%d" % bm), ("gemm2 B", gemm2_variant(vb, HW)), ("gemm2 C", gemm2_variant(vc, HW))}
-    kern, _, chunks, partial, groups = wgrad(N, K, M, HW, sms, scratch_floats, tiled_only)
-    out.add(("wgrad", "%s / %s / %s" % (kern, "partial" if partial else "atomic", "multi-chunk" if chunks > 1 else "one chunk")))
-    if kern == "rows" and groups > 1:
-        out.add(("wgrad", "rows / blockIdx.y > 0"))
-    if bias:
+    if kind == "pw" and s["bias"]:
         out.add(("conv1x1", "bias"))
+    elif kind == "dw":
+        ks, st = s["ks"], s["stride"]
+        out.add(("dw", "%dx%d s%d" % (ks, ks, st)))
+        if s["H"] < ks or s["W"] < ks:
+            out.add(("dw", "map smaller than the stencil"))
+        if st == 2 and (s["H"] % 2 or s["W"] % 2):
+            out.add(("dw", "s2 odd input"))
+    elif kind == "bn":
+        out.add(("bn", "relu" if s["relu"] else "no relu"))
+        if s["N"] * s["H"] * s["W"] == 2:
+            out.add(("bn", "2 values per channel"))
+    elif kind == "stem":
+        out.add(("stem_wgrad", "M%4=0" if s["M"] % 4 == 0 else "M%4!=0"))
+    elif kind == "pool":
+        out.add(("maxpool", "odd input" if s["H"] % 2 or s["W"] % 2 else "even input"))
     return out
 
 
-def dw_cells(N, C, H, W, ks, stride):
-    out = {("dw", "%dx%d s%d" % (ks, ks, stride))}
-    if H < ks or W < ks:
-        out.add(("dw", "map smaller than the stencil"))
-    if stride == 2 and (H % 2 or W % 2):
-        out.add(("dw", "s2 odd input"))
-    out.add(("dw_wgrad", "batch loop (N > 16)" if N > 16 else "grid.y = N"))
+def record_cells(r, s):
+    """The dispatch cells of one launch record r (a dict of yfv2_engine's TrainLaunchRecord) of an op whose input is s."""
+    k = r["kernel"]
+    hw = s["H"] * s["W"]
+    vec = lambda v: "float4" if v else "scalar"
+    if k.startswith("gemm2_kernel"):
+        why = "scalar: HW%4" if hw % 4 else "scalar: unaligned"
+        return {("gemm2", "BM=%d" % r["bm"]), ("gemm2 B", "float4" if r["vec_b"] else why), ("gemm2 C", "float4" if r["vec_c"] else why)}
+    if k.startswith(("wgrad_rows_kernel", "wgrad1x1_kernel")):
+        kern = "rows" if k.startswith("wgrad_rows") else "tiled" + k[k.index("<") + 1:-1]
+        out = {("wgrad", "%s / %s / %s" % (kern, "partial" if r["partial"] else "atomic", "multi-chunk" if r["chunks"] > 1 else "one chunk"))}
+        if kern == "rows" and r["grid"][1] > 1:
+            out.add(("wgrad", "rows / blockIdx.y > 0"))
+        return out
+    if k.startswith("dw_wgrad_kernel"):
+        return {("dw_wgrad", "batch loop (N > 16)" if r["grid"][1] < s["N"] else "grid.y = N")}
+    if k == "bn_stats_kernel":
+        return {("bn_stats", vec(r["vec"])), ("bn slices", bucket_slices(r["slices"]))}
+    if k == "bn_apply_kernel":
+        return {("bn_apply", vec(r["vec"])), ("bn y-grid", ">1" if r["grid"][1] > 1 else "1")}
+    if k.startswith("stem_fwd"):
+        return {("stem_fwd", "stem_fwd_kernel<24>" if k == "stem_fwd_kernel<24>" else "generic")}
+    if k == "upsample2_fwd_kernel":
+        return {("upsample", "2x")}
+    if k == "chan_copy_kernel":
+        return {("chan_copy", "accumulate" if r["accumulate"] else "assign")}
+    return set()
+
+
+def op_cells(name, ptrs, ints, sms):
+    """The cells one yfv2_op_<name> call reaches (ptrs: integer addresses or None, ints: its integer arguments)."""
+    import yfv2_engine
+    if name.startswith("conv1x1"):
+        n, k, m, hw = ints
+        s = dict(N=n, C=k, H=hw, W=1, M=m, bias=ptrs[2 if name == "conv1x1_fwd" else 5] is not None)
+        kind = "pw"
+    elif name.startswith("dwconv"):
+        s = dict(zip(("N", "C", "H", "W", "ks", "stride"), ints))
+        kind = "dw"
+    elif name.startswith("stem"):
+        s = dict(zip(("N", "M", "H", "W"), ints))
+        kind = "stem"
+    elif name.startswith("bn"):
+        s = dict(zip(("N", "C", "H", "relu"), ints), W=1)
+        kind = "bn"
+    else:
+        s = dict(zip(("N", "H", "W"), ints))
+        kind = "pool" if name.startswith("maxpool") else "up"
+    out = shape_cells(kind, s)
+    for r in yfv2_engine.op_launches(name, ptrs, ints, sms):
+        out |= record_cells(r, s)
     return out
-
-
-def bn_cells(N, C, HW, relu, aligned=True):
-    vec = HW % 4 == 0 and aligned
-    out = {("bn_stats", "float4" if vec else "scalar"), ("bn_apply", "float4" if vec else "scalar"),
-           ("bn slices", bucket_slices(bn_slices(N, HW))), ("bn y-grid", ">1" if HW > 1024 else "1"),
-           ("bn", "relu" if relu else "no relu")}
-    if N * HW == 2:
-        out.add(("bn", "2 values per channel"))
-    return out
-
-
-def stem_cells(N, M, H, W):
-    return {("stem_fwd", "stem_fwd_kernel<24>" if M == 24 else "generic"), ("stem_wgrad", "M%4=0" if M % 4 == 0 else "M%4!=0")}
-
-
-def pool_cells(H, W):
-    return {("maxpool", "odd input" if H % 2 or W % 2 else "even input")}
 
 
 # ---- the trainer's program (trainer.cu build()) -------------------------------------------------------------------------------
@@ -222,35 +220,34 @@ def pscratch_floats(pnumel, A, C):
 
 
 def trainer_cells(N, H, W, A=3, C=80, sms=132):
-    """The cells one training step (forward + backward) of the native trainer reaches."""
-    ops, tens, pnumel = program(N, H, W, A, C)
-    cons = consumers(ops, len(tens))
+    """The cells one training step (forward + backward) of a library trainer at (N, H, W, A, C) reaches, from its launch records."""
+    import yfv2_engine
+    lib = yfv2_engine.lib()
+    t = ctypes.c_void_p()
+    yfv2_engine._check(lib.yfv2_trainer_create(ctypes.byref(t), 0, N, H, W, A, C), "trainer_create")
+    try:
+        ops, tens, layout = yfv2_engine.trainer_program(t)
+        recs = yfv2_engine.trainer_launches(t, sms=sms)
+    finally:
+        lib.yfv2_trainer_destroy(t)
+    shapes = []
+    for o in ops:
+        x = tens[o["a"]]
+        shapes.append(dict(N=N, C=x["C"], H=x["H"], W=x["W"], M=tens[o["y"]]["C"], ks=o["ks"], stride=o["stride"], relu=o["relu"],
+                           bias=o["pbias"] >= 0))
     out = set()
-    for i, o in enumerate(ops):
-        c, h, w, _ = tens[o["a"]]
-        k = o["kind"]
-        if k == "stem":
-            out |= stem_cells(N, tens[o["y"]][0], h, w)
-        elif k == "bn":
-            out |= bn_cells(N, c, h * w, o["relu"])
-        elif k == "pool":
-            out |= pool_cells(h, w)
-        elif k == "pw":
-            out |= pw_cells(N, c, o["M"], h * w, sms, o["pbias"] >= 0, K_WSCRATCH_FLOATS)
-        elif k == "dw":
-            out |= dw_cells(N, c, h, w, o["ks"], o["stride"])
-        elif k == "up":
-            out.add(("upsample", "2x"))
-        elif k in ("odd", "cate"):
-            out.add(("chan_copy", "assign"))
-        elif k == "cat2":
-            acc = any(cons[t][-1] != i for t in (o["a"], o["b"]))                  # run_backward: not the tensor's last use
-            out.add(("chan_copy", "accumulate" if acc else "assign"))
-    for t, cs in enumerate(cons):
+    for o, s in zip(ops, shapes):
+        out |= shape_cells(o["kind"], s)
+    for r in recs:
+        if r["op"] >= 0:
+            out |= record_cells(r, shapes[r["op"]])
+    # the trainer's accumulation structure: a tensor read by several ops (not an odd / cate pair) sums their gradients through the
+    # scratch tensor; the shared output convolutions' second use goes through the parameter scratch
+    for t_, cs in enumerate(consumers(ops, len(tens))):
         if len(cs) > 1 and not any(ops[j]["kind"] in ("odd", "cate") for j in cs):
             out.add(("fan-in", "scratch + axpy"))
     out.add(("pscratch", "shared output conv"))
-    if pscratch_floats(pnumel, A, C) > max(pnumel):
+    if layout["pscratch_floats"] > max(program(N, H, W, A, C)[2]):
         out.add(("pscratch", "weight + bias above every parameter"))
     return out
 

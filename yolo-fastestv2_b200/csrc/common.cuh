@@ -15,6 +15,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <vector>
+
 #include "../../include/yfv2.h"
 
 namespace yfv2 {
@@ -200,8 +202,72 @@ int decode_nms_check(const float* const preds[6], int N, int H, int W, int A, in
                      double iou_thres, const int* class_filter, int n_filter, int max_det, float max_wh, float* out, int* counts,
                      int* kept_idx);
 
-// conv1x1 backward with an optional scratch for per-block partial weight gradients (k_train.cu; the C-ABI operator passes none)
-int conv1x1_bwd_impl(const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias, int N, int K, int M, int HW,
-                     float* wscratch, size_t wscratch_floats, cudaStream_t s);
+// ---- the training operators' launches: described on the host (k_train.cu describe_*), then launched ----------------------------
+// Every kernel a yfv2_op_* call or the native trainer launches, and the memsets they make.
+enum class TrainKernel {
+    memset, gemm2_32, gemm2_64, wgrad_rows, wgrad_tiled32, wgrad_tiled64, wgrad_reduce, bias_grad,
+    dw_fwd3, dw_fwd5, dw_dgrad3, dw_dgrad5, dw_wgrad3, dw_wgrad5, stem_fwd24, stem_fwd_generic, stem_wgrad,
+    bn_stats, bn_finalize, bn_apply, bn_bwd_reduce, bn_bwd_apply, bn_eval_stats, bn_eval_bwd_apply, bn_affine_grads,
+    maxpool_fwd, maxpool_bwd, upsample2_fwd, upsample2_bwd, chan_copy, axpy,
+};
+
+constexpr size_t kTrainLaunchPtrs = 10, kTrainLaunchInts = 10;      // most pointer / integer arguments of a training kernel
+
+// One kernel launch (or memset) of a training operator: the kernel and its geometry, the facts its variant was chosen by, and its
+// arguments in the kernel's signature order, pointers in p and integers in n (a memset: p[0] and bytes).
+struct TrainLaunch {
+    TrainKernel kernel = TrainKernel::memset;
+    dim3 grid;
+    int block = 256;
+    size_t smem = 0;                         // dynamic shared memory, bytes
+    int op = -1;                             // native trainer: the op of its program the launch belongs to (-1: none)
+    bool bwd = false;                        //   and whether it runs in the backward
+    int bm = 0;                              // gemm2: tile height
+    bool vec_b = false, vec_c = false;       // gemm2: float4 access of B / C
+    bool vec = false;                        // bn_stats / bn_apply / bn_eval_bwd_apply: float4 access
+    int pchunk = 0, chunks = 0;              // wgrad: pixels per block slice, slices per image
+    bool partial = false;                    // wgrad: per-block partial sums summed by wgrad_reduce_kernel, else atomics into zeroed dw
+    int slices = 0;                          // BatchNorm per-channel reductions: image slices (grid.y)
+    int accumulate = 0;                      // chan_copy / axpy: add to the destination
+    size_t bytes = 0;                        // memset
+    const void* p[kTrainLaunchPtrs] = {};
+    long long n[kTrainLaunchInts] = {};
+    double d = 0.0;
+    float f = 0.f;
+};
+using TrainLaunches = std::vector<TrainLaunch>;
+
+// One describe function per operator (k_train.cu): appends the records of one call; the addresses are never dereferenced, they only
+// decide alignment.  An argument the operator refuses is set_error + its code, with nothing appended.
+int describe_conv1x1_fwd(const float* x, const float* w, const float* bias, float* y, int N, int K, int M, int HW, TrainLaunches& L);
+int describe_conv1x1_bwd(const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias, int N, int K, int M, int HW,
+                         float* wscratch, size_t wscratch_floats, int sms, TrainLaunches& L);
+int describe_dwconv_fwd(const float* x, const float* w, float* y, int N, int C, int H, int W, int ks, int stride, TrainLaunches& L);
+int describe_dwconv_bwd(const float* x, const float* w, const float* dy, float* dx, float* dw, int N, int C, int H, int W, int ks, int stride,
+                        TrainLaunches& L);
+int describe_stem_fwd(const float* x, const float* w, float* y, int N, int M, int H, int W, TrainLaunches& L);
+int describe_stem_wgrad(const float* x, const float* dy, float* dw, int N, int M, int H, int W, TrainLaunches& L);
+int describe_bn_train_fwd(const float* x, const float* gamma, const float* beta, float* running_mean, float* running_var, float* y,
+                          float* save_mean, float* save_invstd, double* scratch, int N, int C, int HW, int relu, TrainLaunches& L);
+int describe_bn_train_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean, const float* save_invstd,
+                          float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW, int relu, TrainLaunches& L);
+int describe_bn_eval_fwd(const float* x, const float* gamma, const float* beta, const float* running_mean, const float* running_var, float* y,
+                         float* save_mean, float* save_invstd, int N, int C, int HW, int relu, TrainLaunches& L);
+int describe_bn_eval_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean, const float* save_invstd,
+                         float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW, int relu, TrainLaunches& L);
+int describe_maxpool_fwd(const float* x, float* y, int* idx, int planes, int H, int W, TrainLaunches& L);
+int describe_maxpool_bwd(const float* dy, const int* idx, float* dx, int planes, int H, int W, TrainLaunches& L);
+int describe_upsample2_fwd(const float* x, float* y, int planes, int H, int W, TrainLaunches& L);
+int describe_upsample2_bwd(const float* dy, float* dx, int planes, int H, int W, TrainLaunches& L);
+// the native trainer's channel copies and gradient sums: dst[n][doff + c*dstep][p] (+)= src[n][soff + c*sstep][p], dst[i] (+)= src[i]
+void describe_chan_copy(const float* src, int Cs, int soff, int sstep, float* dst, int Cd, int doff, int dstep, int count, int N, int HW,
+                        int accumulate, int sms, TrainLaunches& L);
+void describe_axpy(const float* src, float* dst, long long n, int accumulate, int sms, TrainLaunches& L);
+
+// The one launch path of the training operators: the record's kernel or memset, then its check
+int launch(const TrainLaunch& L, cudaStream_t s);
+int launch_all(const TrainLaunches& L, cudaStream_t s);
+// The records as the test hooks return them: min(cap, count) written, the count in *n
+int debug_records(const TrainLaunches& L, yfv2_train_launch* out, int cap, int* n);
 
 }  // namespace yfv2

@@ -9,6 +9,12 @@
 //   stem conv fwd / wgrad                      dense 3x3 s2 p1, 3->24                   (shufflenetv2.py:75)
 //   batchnorm train fwd / bwd (+ReLU)          batch statistics, running-stat update    (nn.BatchNorm2d, momentum .1, eps 1e-5)
 //   maxpool 3x3 s2 p1 fwd / bwd, nearest 2x upsample fwd / bwd                           (shufflenetv2.py:80; fpn.py:57)
+//
+// Every launch is chosen in one place: a describe_* function per operator turns a call into TrainLaunch records (common.cuh: kernel,
+// grid, memsets and the variant facts), launch() runs a record.  The yfv2_op_* entries, the native trainer (trainer.cu) and the test
+// hooks yfv2_op_debug_launches / yfv2_trainer_debug_launches all go through these functions.
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace yfv2 {
@@ -30,6 +36,16 @@ struct Gemm2Args {
     const float* bias;               // per-row bias or null
 };
 
+// The float4 conditions, written once for the kernels and for the describe_* records.  Expression macros, not functions: as a
+// __host__ __device__ function (inline, __forceinline__, __noinline__, constexpr or template alike) the same condition changes
+// the SASS of gemm2_kernel and the BatchNorm kernels under nvcc 12.9.
+// A gemm2_kernel operand (vecB / vecC): the row length and both strides multiples of 4 floats, the base 16-byte aligned
+#define YFV2_GEMM2_VEC(N, s1, s2, p) \
+    ((((N) & 3) == 0) && (((s1) & 3) == 0) && (((s2) & 3) == 0) && ((reinterpret_cast<uintptr_t>(p) & 15) == 0))
+// bn_stats_kernel, bn_apply_kernel, bn_eval_bwd_apply_kernel: planes of a multiple of 4 pixels, every operand 16-byte aligned
+// (addrs: their addresses or-ed together)
+#define YFV2_BN_VEC(HW, addrs) (((HW) & 3) == 0 && ((addrs) & 15) == 0)
+
 template <int BM>
 __global__ void __launch_bounds__(256)
 gemm2_kernel(Gemm2Args g) {
@@ -41,8 +57,8 @@ gemm2_kernel(Gemm2Args g) {
     const float* B = g.B + (long long)b * g.sBb;
     float* C = g.C + (long long)b * g.sCb;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;          // thread -> rows [ty*TM, +TM), cols [tx*4, +4)
-    const bool vecB = ((g.N & 3) == 0) && ((g.sBk & 3) == 0) && ((g.sBb & 3) == 0) && ((reinterpret_cast<uintptr_t>(g.B) & 15) == 0);
-    const bool vecC = ((g.N & 3) == 0) && ((g.sCi & 3) == 0) && ((g.sCb & 3) == 0) && ((reinterpret_cast<uintptr_t>(g.C) & 15) == 0);
+    const bool vecB = YFV2_GEMM2_VEC(g.N, g.sBk, g.sBb, g.B);
+    const bool vecC = YFV2_GEMM2_VEC(g.N, g.sCi, g.sCb, g.C);
     // loader roles: A slab = BM x 16 floats (BM*16/256 per thread), B slab = 16 x 128 floats (8 per thread: two float4)
     constexpr int APT = BM * BK / 256;
     float ra[APT];
@@ -118,18 +134,6 @@ gemm2_kernel(Gemm2Args g) {
             for (int r = 0; r < 4; ++r) if (j + r < g.N) dst[r] = acc[q][r] + bv;
         }
     }
-}
-
-int run_gemm2(const Gemm2Args& g, cudaStream_t s) {
-    if (g.M <= 32) {
-        dim3 grid((g.N + 127) / 128, (g.M + 31) / 32, g.batch);
-        gemm2_kernel<32><<<grid, 256, 0, s>>>(g);
-    } else {
-        dim3 grid((g.N + 127) / 128, (g.M + 63) / 64, g.batch);
-        gemm2_kernel<64><<<grid, 256, 0, s>>>(g);
-    }
-    YFV2_LAUNCH_CHECK();
-    return YFV2_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -517,7 +521,7 @@ __global__ void __launch_bounds__(256)
 bn_stats_kernel(const float* __restrict__ x, double* __restrict__ stats, int N, int C, int HW) {
     const int c = blockIdx.x;
     double s1 = 0.0, s2 = 0.0;
-    const bool vec = (HW & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+    const bool vec = YFV2_BN_VEC(HW, reinterpret_cast<uintptr_t>(x));
     for (int n = blockIdx.y; n < N; n += gridDim.y) {
         const float* xp = x + ((long long)n * C + c) * HW;
         if (vec) {
@@ -570,7 +574,7 @@ bn_apply_kernel(const float* __restrict__ x, const float* __restrict__ mean, con
     const int p0 = blockIdx.y * 1024 + threadIdx.x * 4;
     // ReLU as torch's threshold (r <= 0 ? 0 : r): a NaN passes through, where fmaxf(NaN, 0) would return 0
     auto f = [&](float v) { float r = (v - mu) * is * ga + be; return relu ? (r <= 0.f ? 0.f : r) : r; };      // same association as before
-    if ((HW & 3) == 0 && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0) {
+    if (YFV2_BN_VEC(HW, reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y))) {
         if (p0 < HW) {
             const float4 v = __ldg(reinterpret_cast<const float4*>(xp + p0));
             *reinterpret_cast<float4*>(yp + p0) = make_float4(f(v.x), f(v.y), f(v.z), f(v.w));
@@ -659,7 +663,7 @@ bn_eval_bwd_apply_kernel(const float* __restrict__ y, const float* __restrict__ 
     const long long base = pl * HW;
     const int p0 = blockIdx.y * 1024 + threadIdx.x * 4;
     auto f = [&](float d, float yv) { return (relu && yv <= 0.f ? 0.f : d) * s; };      // threshold_backward: a NaN y passes dy
-    if ((HW & 3) == 0 && ((reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0) {
+    if (YFV2_BN_VEC(HW, reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx))) {
         if (p0 < HW) {
             const float4 d = __ldg(reinterpret_cast<const float4*>(dy + base + p0));
             const float4 v = relu ? __ldg(reinterpret_cast<const float4*>(y + base + p0)) : make_float4(1.f, 1.f, 1.f, 1.f);
@@ -731,7 +735,41 @@ __global__ void upsample2_bwd_kernel(const float* __restrict__ dy, float* __rest
     }
 }
 
-int grid_for(long long total) { long long b = (total + 255) / 256; return (int)(b < 1 ? 1 : (b > 148 * 32 ? 148 * 32 : b)); }
+// ---------------------------------------------------------------------------------------------------------------------
+// the native trainer's channel copies (shuffle / split / concat and their backward) and gradient sums
+// ---------------------------------------------------------------------------------------------------------------------
+// dst[n][doff + c*dstep][p] (+)= src[n][soff + c*sstep][p],  c < count
+__global__ void chan_copy_kernel(const float* __restrict__ src, int Cs, int soff, int sstep, float* __restrict__ dst, int Cd, int doff, int dstep,
+                                 int count, int HW, long long total, int accumulate) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int p = (int)(i % HW);
+        const long long r = i / HW;
+        const int c = (int)(r % count);
+        const long long n = r / count;
+        const float v = src[(n * Cs + soff + (long long)c * sstep) * HW + p];
+        float* d = dst + (n * Cd + doff + (long long)c * dstep) * HW + p;
+        *d = accumulate ? *d + v : v;
+    }
+}
+__global__ void axpy_kernel(const float* __restrict__ src, float* __restrict__ dst, long long n, int accumulate) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        dst[i] = accumulate ? dst[i] + src[i] : src[i];
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// host: every launch is first described as a TrainLaunch record (describe_*), then run by launch()
+// ---------------------------------------------------------------------------------------------------------------------
+using TK = TrainKernel;
+
+// Grid of the grid-stride elementwise kernels: one thread per element in 256-thread blocks, at most `cap` blocks.  The operators
+// cap at kOpGridCap, 32 blocks per SM of a 148-SM B200 (the GPU these kernels were first written for; retuning it for the H100
+// changes the grids of large elementwise ops and wants its own measurement); the native trainer's copies cap at 16 per SM.
+constexpr long long kOpGridCap = 148 * 32;
+int elem_grid(long long total, long long cap) { const long long b = (total + 255) / 256; return (int)(b < 1 ? 1 : (b > cap ? cap : b)); }
+
+// GEMM tile height: 32 rows for the 24-channel layers (a 64-row tile would idle 5/8 of its rows), 64 otherwise
+int gemm2_bm(int M) { return M <= 32 ? 32 : 64; }
+
 // image slices of the per-channel reductions: about 16 pixels per thread, at most 64 slices and one image per slice
 int bn_slices(int N, int HW) {
     const long long per = (long long)N * HW;
@@ -740,215 +778,419 @@ int bn_slices(int N, int HW) {
     return slices > N ? N : slices;
 }
 
-}  // namespace
-}  // namespace yfv2
+// a kernel record with its pointer and integer arguments in signature order (launch() reads them back by position)
+template <size_t NP, size_t NN>
+TrainLaunch& add(TrainLaunches& L, TK k, dim3 grid, const void* const (&p)[NP], const long long (&n)[NN], int block = 256) {
+    static_assert(NP <= kTrainLaunchPtrs && NN <= kTrainLaunchInts, "a kernel with more arguments than a TrainLaunch holds");
+    L.emplace_back();
+    TrainLaunch& r = L.back();
+    r.kernel = k; r.grid = grid; r.block = block;
+    std::copy(p, p + NP, r.p);
+    std::copy(n, n + NN, r.n);
+    return r;
+}
+void add_memset(TrainLaunches& L, void* p, size_t bytes) {
+    L.emplace_back();
+    L.back().kernel = TK::memset; L.back().p[0] = p; L.back().bytes = bytes;
+}
 
-using namespace yfv2;
+void describe_gemm2(const Gemm2Args& g, TrainLaunches& L) {
+    const int bm = gemm2_bm(g.M);
+    TrainLaunch& r = add(L, bm == 32 ? TK::gemm2_32 : TK::gemm2_64, dim3((g.N + 127) / 128, (g.M + bm - 1) / bm, g.batch),
+                         {g.A, g.B, g.C, g.bias}, {g.M, g.N, g.K, g.batch, g.sAi, g.sAk, g.sBk, g.sBb, g.sCi, g.sCb});
+    r.bm = bm;
+    r.vec_b = YFV2_GEMM2_VEC(g.N, g.sBk, g.sBb, g.B);
+    r.vec_c = YFV2_GEMM2_VEC(g.N, g.sCi, g.sCb, g.C);
+}
+
+const char* kernel_name(TK k) {
+    switch (k) {
+    case TK::memset: return "memset";
+    case TK::gemm2_32: return "gemm2_kernel<32>";
+    case TK::gemm2_64: return "gemm2_kernel<64>";
+    case TK::wgrad_rows: return "wgrad_rows_kernel<24,3>";
+    case TK::wgrad_tiled32: return "wgrad1x1_kernel<32>";
+    case TK::wgrad_tiled64: return "wgrad1x1_kernel<64>";
+    case TK::wgrad_reduce: return "wgrad_reduce_kernel";
+    case TK::bias_grad: return "bias_grad_kernel";
+    case TK::dw_fwd3: return "dw_fwd_kernel<3>";
+    case TK::dw_fwd5: return "dw_fwd_kernel<5>";
+    case TK::dw_dgrad3: return "dw_dgrad_kernel<3>";
+    case TK::dw_dgrad5: return "dw_dgrad_kernel<5>";
+    case TK::dw_wgrad3: return "dw_wgrad_kernel<3>";
+    case TK::dw_wgrad5: return "dw_wgrad_kernel<5>";
+    case TK::stem_fwd24: return "stem_fwd_kernel<24>";
+    case TK::stem_fwd_generic: return "stem_fwd_generic_kernel";
+    case TK::stem_wgrad: return "stem_wgrad_kernel";
+    case TK::bn_stats: return "bn_stats_kernel";
+    case TK::bn_finalize: return "bn_finalize_kernel";
+    case TK::bn_apply: return "bn_apply_kernel";
+    case TK::bn_bwd_reduce: return "bn_bwd_reduce_kernel";
+    case TK::bn_bwd_apply: return "bn_bwd_apply_kernel";
+    case TK::bn_eval_stats: return "bn_eval_stats_kernel";
+    case TK::bn_eval_bwd_apply: return "bn_eval_bwd_apply_kernel";
+    case TK::bn_affine_grads: return "bn_affine_grads_kernel";
+    case TK::maxpool_fwd: return "maxpool_fwd_kernel";
+    case TK::maxpool_bwd: return "maxpool_bwd_kernel";
+    case TK::upsample2_fwd: return "upsample2_fwd_kernel";
+    case TK::upsample2_bwd: return "upsample2_bwd_kernel";
+    case TK::chan_copy: return "chan_copy_kernel";
+    case TK::axpy: return "axpy_kernel";
+    }
+    return "?";
+}
+
+}  // namespace
 
 #define ARGCHK(cond, msg) do { if (!(cond)) { set_error("%s", msg); return YFV2_EINVAL; } } while (0)
 
 // y[n][m][p] = sum_k w[m][k] x[n][k][p] (+ bias[m])
-extern "C" YFV2_API int yfv2_op_conv1x1_fwd(const float* x, const float* w, const float* bias, float* y, int N, int K, int M, int HW, void* stream) {
+int describe_conv1x1_fwd(const float* x, const float* w, const float* bias, float* y, int N, int K, int M, int HW, TrainLaunches& L) {
     ARGCHK(x && w && y && N > 0 && K > 0 && M > 0 && HW > 0, "conv1x1_fwd: bad arguments");
-    Gemm2Args g{w, x, y, M, HW, K, N, K, 1, HW, (long long)K * HW, HW, (long long)M * HW, bias};
-    return run_gemm2(g, (cudaStream_t)stream);
+    describe_gemm2(Gemm2Args{w, x, y, M, HW, K, N, K, 1, HW, (long long)K * HW, HW, (long long)M * HW, bias}, L);
+    return YFV2_OK;
 }
 // dx[n][k][p] = sum_m w[m][k] dy[n][m][p];  dw[m][k] = sum_{n,p} dy[n][m][p] x[n][k][p];  dbias[m] = sum dy
 // wscratch (optional, wscratch_floats long): per-block partial weight gradients, summed by a second kernel instead of fp32 atomics
 // into dw (torch.profiler: ~150 k same-address-line atomics per 24x24 layer cost 160 us where the arithmetic needs 20).
-namespace yfv2 {
-int conv1x1_bwd_impl(const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias, int N, int K, int M, int HW,
-                     float* wscratch, size_t wscratch_floats, cudaStream_t s) {
-    if (!(x && w && dy && N > 0 && K > 0 && M > 0 && HW > 0)) { set_error("conv1x1_bwd: bad arguments"); return YFV2_EINVAL; }
-    if (dx) {
-        Gemm2Args g{w, dy, dx, K, HW, M, N, 1, K, HW, (long long)M * HW, HW, (long long)K * HW, nullptr};      // A(i=k, kk=m) = w[m][k]
-        const int rc = run_gemm2(g, s);
-        if (rc) return rc;
-    }
+int describe_conv1x1_bwd(const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias, int N, int K, int M, int HW,
+                         float* wscratch, size_t wscratch_floats, int sms, TrainLaunches& L) {
+    ARGCHK(x && w && dy && N > 0 && K > 0 && M > 0 && HW > 0, "conv1x1_bwd: bad arguments");
+    if (dx) describe_gemm2(Gemm2Args{w, dy, dx, K, HW, M, N, 1, K, HW, (long long)M * HW, HW, (long long)K * HW, nullptr}, L);  // A(i=k, kk=m) = w[m][k]
     if (dw) {
-        if (K == 24 && M % 24 == 0) {      // (K = 48: 50 loads per 96 FMAs per lane measured 250 us per layer; the tiled kernel wins)
-            // pixel slices sized so that the grid has about two waves whatever the map size
-            int pchunk = 2048;
-            while (pchunk > 256 && (long long)N * (M / 24) * ((HW + pchunk - 1) / pchunk) < 2LL * sm_count()) pchunk >>= 1;
-            const int chunks = (HW + pchunk - 1) / pchunk;
-            const dim3 grid((unsigned)(N * chunks), (unsigned)(M / 24));
-            float* part = (wscratch && (size_t)N * chunks * M * K <= wscratch_floats) ? wscratch : nullptr;
-            if (!part) YFV2_CUDA(cudaMemsetAsync(dw, 0, (size_t)M * K * sizeof(float), s));
-            wgrad_rows_kernel<24, 3><<<grid, 256, 0, s>>>(dy, x, dw, N, M, HW, pchunk, part);
-            YFV2_LAUNCH_CHECK();
-            if (part) { wgrad_reduce_kernel<<<(M * K + 63) / 64, 256, 0, s>>>(part, N * chunks, M * K, dw); YFV2_LAUNCH_CHECK(); }
-        } else {
-            const int BT = (M <= 32 && K <= 32) ? 32 : 64;
-            const int tiles = ((M + BT - 1) / BT) * ((K + BT - 1) / BT);
-            int pchunk = 1024;
-            while (pchunk > 64 && (long long)tiles * N * ((HW + pchunk - 1) / pchunk) < 4LL * sm_count()) pchunk >>= 1;
-            const int chunks = (HW + pchunk - 1) / pchunk;
-            const dim3 grid((K + BT - 1) / BT, (M + BT - 1) / BT, N * chunks);
-            float* part = (wscratch && (size_t)N * chunks * M * K <= wscratch_floats) ? wscratch : nullptr;
-            if (!part) YFV2_CUDA(cudaMemsetAsync(dw, 0, (size_t)M * K * sizeof(float), s));
-            if (BT == 32) wgrad1x1_kernel<32><<<grid, 256, 0, s>>>(dy, x, dw, N, M, K, HW, pchunk, part);
-            else wgrad1x1_kernel<64><<<grid, 256, 0, s>>>(dy, x, dw, N, M, K, HW, pchunk, part);
-            YFV2_LAUNCH_CHECK();
-            if (part) { wgrad_reduce_kernel<<<(M * K + 63) / 64, 256, 0, s>>>(part, N * chunks, M * K, dw); YFV2_LAUNCH_CHECK(); }
-        }
+        // the register-only kernel for the narrowest layers (K = 48: 50 loads per 96 FMAs per lane measured 250 us per layer; the
+        // tiled kernel wins), else BT x BT tiles; pixel slices sized so that the grid has about two (rows) or four (tiled) waves
+        // whatever the map size
+        const bool rows = K == 24 && M % 24 == 0;
+        const int BT = (M <= 32 && K <= 32) ? 32 : 64;
+        const long long units = rows ? (long long)N * (M / 24) : (long long)(((M + BT - 1) / BT) * ((K + BT - 1) / BT)) * N;
+        int pchunk = rows ? 2048 : 1024;
+        while (pchunk > (rows ? 256 : 64) && units * ((HW + pchunk - 1) / pchunk) < (rows ? 2LL : 4LL) * sms) pchunk >>= 1;
+        const int chunks = (HW + pchunk - 1) / pchunk;
+        float* part = (wscratch && (size_t)N * chunks * M * K <= wscratch_floats) ? wscratch : nullptr;
+        if (!part) add_memset(L, dw, (size_t)M * K * sizeof(float));
+        TrainLaunch& r = rows ? add(L, TK::wgrad_rows, dim3((unsigned)(N * chunks), (unsigned)(M / 24)), {dy, x, dw, part}, {N, M, HW, pchunk})
+                              : add(L, BT == 32 ? TK::wgrad_tiled32 : TK::wgrad_tiled64, dim3((K + BT - 1) / BT, (M + BT - 1) / BT, N * chunks),
+                                    {dy, x, dw, part}, {N, M, K, HW, pchunk});
+        r.pchunk = pchunk; r.chunks = chunks; r.partial = part != nullptr;
+        if (part) add(L, TK::wgrad_reduce, dim3((M * K + 63) / 64), {part, dw}, {N * chunks, M * K});
     }
-    if (dbias) {
-        bias_grad_kernel<<<M, 256, 0, s>>>(dy, dbias, N, M, HW);
-        YFV2_LAUNCH_CHECK();
-    }
+    if (dbias) add(L, TK::bias_grad, dim3(M), {dy, dbias}, {N, M, HW});
     return YFV2_OK;
 }
-}  // namespace yfv2
-extern "C" YFV2_API int yfv2_op_conv1x1_bwd(const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias, int N, int K, int M,
-                                            int HW, void* stream) {
-    return yfv2::conv1x1_bwd_impl(x, w, dy, dx, dw, dbias, N, K, M, HW, nullptr, 0, (cudaStream_t)stream);
-}
 
-extern "C" YFV2_API int yfv2_op_dwconv_fwd(const float* x, const float* w, float* y, int N, int C, int H, int W, int ks, int stride, void* stream) {
+int describe_dwconv_fwd(const float* x, const float* w, float* y, int N, int C, int H, int W, int ks, int stride, TrainLaunches& L) {
     ARGCHK(x && w && y && (ks == 3 || ks == 5) && (stride == 1 || stride == 2), "dwconv_fwd: bad arguments");
     const int Ho = (H + 2 * (ks / 2) - ks) / stride + 1, Wo = (W + 2 * (ks / 2) - ks) / stride + 1;
-    const long long total = (long long)N * C * Ho * Wo;
-    if (ks == 3) dw_fwd_kernel<3><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(x, w, y, N, C, H, W, Ho, Wo, stride);
-    else dw_fwd_kernel<5><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(x, w, y, N, C, H, W, Ho, Wo, stride);
-    YFV2_LAUNCH_CHECK();
+    add(L, ks == 3 ? TK::dw_fwd3 : TK::dw_fwd5, dim3(elem_grid((long long)N * C * Ho * Wo, kOpGridCap)), {x, w, y}, {N, C, H, W, Ho, Wo, stride});
     return YFV2_OK;
 }
-extern "C" YFV2_API int yfv2_op_dwconv_bwd(const float* x, const float* w, const float* dy, float* dx, float* dw, int N, int C, int H, int W, int ks,
-                                           int stride, void* stream) {
+int describe_dwconv_bwd(const float* x, const float* w, const float* dy, float* dx, float* dw, int N, int C, int H, int W, int ks, int stride,
+                        TrainLaunches& L) {
     ARGCHK(x && w && dy && (ks == 3 || ks == 5) && (stride == 1 || stride == 2), "dwconv_bwd: bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
     const int Ho = (H + 2 * (ks / 2) - ks) / stride + 1, Wo = (W + 2 * (ks / 2) - ks) / stride + 1;
-    if (dx) {
-        const long long total = (long long)N * C * H * W;
-        if (ks == 3) dw_dgrad_kernel<3><<<grid_for(total), 256, 0, s>>>(dy, w, dx, N, C, H, W, Ho, Wo, stride);
-        else dw_dgrad_kernel<5><<<grid_for(total), 256, 0, s>>>(dy, w, dx, N, C, H, W, Ho, Wo, stride);
-        YFV2_LAUNCH_CHECK();
-    }
+    if (dx)
+        add(L, ks == 3 ? TK::dw_dgrad3 : TK::dw_dgrad5, dim3(elem_grid((long long)N * C * H * W, kOpGridCap)), {dy, w, dx},
+            {N, C, H, W, Ho, Wo, stride});
     if (dw) {
-        YFV2_CUDA(cudaMemsetAsync(dw, 0, (size_t)C * ks * ks * sizeof(float), s));
-        dim3 grid(C, N < 16 ? N : 16);
-        if (ks == 3) dw_wgrad_kernel<3><<<grid, 256, 0, s>>>(x, dy, dw, N, C, H, W, Ho, Wo, stride);
-        else dw_wgrad_kernel<5><<<grid, 256, 0, s>>>(x, dy, dw, N, C, H, W, Ho, Wo, stride);
-        YFV2_LAUNCH_CHECK();
+        add_memset(L, dw, (size_t)C * ks * ks * sizeof(float));
+        add(L, ks == 3 ? TK::dw_wgrad3 : TK::dw_wgrad5, dim3(C, N < 16 ? N : 16), {x, dy, dw}, {N, C, H, W, Ho, Wo, stride});
     }
     return YFV2_OK;
 }
 
-extern "C" YFV2_API int yfv2_op_stem_fwd(const float* x, const float* w, float* y, int N, int M, int H, int W, void* stream) {
+int describe_stem_fwd(const float* x, const float* w, float* y, int N, int M, int H, int W, TrainLaunches& L) {
     ARGCHK(x && w && y && H % 2 == 0 && W % 2 == 0, "stem_fwd: bad arguments");
-    if (M == 24) stem_fwd_kernel<24><<<grid_for((long long)N * (H / 2) * (W / 2)), 256, 0, (cudaStream_t)stream>>>(x, w, y, N, H, W);
-    else stem_fwd_generic_kernel<<<grid_for((long long)N * M * (H / 2) * (W / 2)), 256, 0, (cudaStream_t)stream>>>(x, w, y, N, M, H, W);
-    YFV2_LAUNCH_CHECK();
+    if (M == 24) add(L, TK::stem_fwd24, dim3(elem_grid((long long)N * (H / 2) * (W / 2), kOpGridCap)), {x, w, y}, {N, H, W});
+    else add(L, TK::stem_fwd_generic, dim3(elem_grid((long long)N * M * (H / 2) * (W / 2), kOpGridCap)), {x, w, y}, {N, M, H, W});
     return YFV2_OK;
 }
-extern "C" YFV2_API int yfv2_op_stem_wgrad(const float* x, const float* dy, float* dw, int N, int M, int H, int W, void* stream) {
+int describe_stem_wgrad(const float* x, const float* dy, float* dw, int N, int M, int H, int W, TrainLaunches& L) {
     ARGCHK(x && dy && dw, "stem_wgrad: bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
-    YFV2_CUDA(cudaMemsetAsync(dw, 0, (size_t)M * 27 * sizeof(float), s));
-    stem_wgrad_kernel<<<dim3((M + 3) / 4, 128), 256, 0, s>>>(x, dy, dw, N, M, H, W);
-    YFV2_LAUNCH_CHECK();
+    add_memset(L, dw, (size_t)M * 27 * sizeof(float));
+    add(L, TK::stem_wgrad, dim3((M + 3) / 4, 128), {x, dy, dw}, {N, M, H, W});
     return YFV2_OK;
 }
 
 // scratch: 2*C doubles.  save_mean / save_invstd: [C] each.  running_* may be null (no update).
-extern "C" YFV2_API int yfv2_op_bn_train_fwd(const float* x, const float* gamma, const float* beta, float* running_mean, float* running_var, float* y,
-                                             float* save_mean, float* save_invstd, double* scratch, int N, int C, int HW, int relu, void* stream) {
+int describe_bn_train_fwd(const float* x, const float* gamma, const float* beta, float* running_mean, float* running_var, float* y,
+                          float* save_mean, float* save_invstd, double* scratch, int N, int C, int HW, int relu, TrainLaunches& L) {
     ARGCHK(x && gamma && beta && y && save_mean && save_invstd && scratch && N > 0 && C > 0 && HW > 0, "bn_train_fwd: bad arguments");
     // F.batch_norm in training mode refuses one value per channel (its variance is undefined)
     ARGCHK((long long)N * HW > 1, "bn_train_fwd: expected more than 1 value per channel when training");
-    cudaStream_t s = (cudaStream_t)stream;
-    YFV2_CUDA(cudaMemsetAsync(scratch, 0, (size_t)2 * C * sizeof(double), s));
-    const long long per = (long long)N * HW;
-    int slices = (int)((per + 256 * 16 - 1) / (256 * 16));
-    slices = slices < 1 ? 1 : (slices > 64 ? 64 : slices);
-    if (slices > N) slices = N;
-    bn_stats_kernel<<<dim3(C, slices), 256, 0, s>>>(x, scratch, N, C, HW);
-    YFV2_LAUNCH_CHECK();
-    bn_finalize_kernel<<<(C + 127) / 128, 128, 0, s>>>(scratch, save_mean, save_invstd, running_mean, running_var, C, (double)per, 0.1f);
-    YFV2_LAUNCH_CHECK();
-    bn_apply_kernel<<<dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)), 256, 0, s>>>(x, save_mean, save_invstd, gamma, beta, y, C, HW, relu);
-    YFV2_LAUNCH_CHECK();
+    add_memset(L, scratch, (size_t)2 * C * sizeof(double));
+    TrainLaunch& r = add(L, TK::bn_stats, dim3(C, bn_slices(N, HW)), {x, scratch}, {N, C, HW});
+    r.slices = (int)r.grid.y; r.vec = YFV2_BN_VEC(HW, reinterpret_cast<uintptr_t>(x));
+    TrainLaunch& f = add(L, TK::bn_finalize, dim3((C + 127) / 128), {scratch, save_mean, save_invstd, running_mean, running_var}, {C}, 128);
+    f.d = (double)((long long)N * HW); f.f = 0.1f;
+    TrainLaunch& a = add(L, TK::bn_apply, dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)), {x, save_mean, save_invstd, gamma, beta, y},
+                         {C, HW, relu});
+    a.vec = YFV2_BN_VEC(HW, reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y));
     return YFV2_OK;
 }
-extern "C" YFV2_API int yfv2_op_bn_train_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean,
-                                             const float* save_invstd, float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW,
-                                             int relu, void* stream) {
+int describe_bn_train_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean, const float* save_invstd,
+                          float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW, int relu, TrainLaunches& L) {
     ARGCHK(x && y && dy && gamma && save_mean && save_invstd && dx && scratch, "bn_train_bwd: bad arguments");      // dgamma / dbeta: NULL skips
-    cudaStream_t s = (cudaStream_t)stream;
-    YFV2_CUDA(cudaMemsetAsync(scratch, 0, (size_t)2 * C * sizeof(double), s));
-    const long long per = (long long)N * HW;
-    int slices = (int)((per + 256 * 16 - 1) / (256 * 16));
-    slices = slices < 1 ? 1 : (slices > 64 ? 64 : slices);
-    if (slices > N) slices = N;
-    bn_bwd_reduce_kernel<<<dim3(C, slices), 256, 0, s>>>(x, y, dy, save_mean, save_invstd, scratch, N, C, HW, relu);
-    YFV2_LAUNCH_CHECK();
-    bn_bwd_apply_kernel<<<dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)), 256, 0, s>>>(x, y, dy, save_mean, save_invstd, gamma, scratch, dx,
-                                                                                               dgamma, dbeta, C, HW, (double)per, relu);
-    YFV2_LAUNCH_CHECK();
+    add_memset(L, scratch, (size_t)2 * C * sizeof(double));
+    TrainLaunch& r = add(L, TK::bn_bwd_reduce, dim3(C, bn_slices(N, HW)), {x, y, dy, save_mean, save_invstd, scratch}, {N, C, HW, relu});
+    r.slices = (int)r.grid.y;
+    add(L, TK::bn_bwd_apply, dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)),
+        {x, y, dy, save_mean, save_invstd, gamma, scratch, dx, dgamma, dbeta}, {C, HW, relu}).d = (double)((long long)N * HW);
     return YFV2_OK;
 }
 
 // Eval-mode BatchNorm: y = [ReLU]((x - running_mean) * (running_var + eps)^-1/2 * gamma + beta).  The running statistics are read,
 // never written; save_mean / save_invstd receive what the forward normalised with (they feed yfv2_op_bn_eval_bwd).
-extern "C" YFV2_API int yfv2_op_bn_eval_fwd(const float* x, const float* gamma, const float* beta, const float* running_mean,
-                                            const float* running_var, float* y, float* save_mean, float* save_invstd, int N, int C, int HW,
-                                            int relu, void* stream) {
+int describe_bn_eval_fwd(const float* x, const float* gamma, const float* beta, const float* running_mean, const float* running_var, float* y,
+                         float* save_mean, float* save_invstd, int N, int C, int HW, int relu, TrainLaunches& L) {
     ARGCHK(x && gamma && beta && running_mean && running_var && y && save_mean && save_invstd && N > 0 && C > 0 && HW > 0,
            "bn_eval_fwd: bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
-    bn_eval_stats_kernel<<<(C + 127) / 128, 128, 0, s>>>(running_mean, running_var, save_mean, save_invstd, C);
-    YFV2_LAUNCH_CHECK();
-    bn_apply_kernel<<<dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)), 256, 0, s>>>(x, save_mean, save_invstd, gamma, beta, y, C, HW, relu);
-    YFV2_LAUNCH_CHECK();
+    add(L, TK::bn_eval_stats, dim3((C + 127) / 128), {running_mean, running_var, save_mean, save_invstd}, {C}, 128);
+    add(L, TK::bn_apply, dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)), {x, save_mean, save_invstd, gamma, beta, y}, {C, HW, relu})
+        .vec = YFV2_BN_VEC(HW, reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y));
     return YFV2_OK;
 }
 // dx = g * gamma * invstd, dgamma = sum(g * xhat), dbeta = sum(g) (g: dy masked by y > 0 under ReLU).  Each of dx, dgamma, dbeta
 // may be NULL (skipped), not all three; scratch (2*C doubles) is needed only with dgamma or dbeta.
-extern "C" YFV2_API int yfv2_op_bn_eval_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean,
-                                            const float* save_invstd, float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW,
-                                            int relu, void* stream) {
+int describe_bn_eval_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean, const float* save_invstd,
+                         float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW, int relu, TrainLaunches& L) {
     ARGCHK(x && y && dy && gamma && save_mean && save_invstd && N > 0 && C > 0 && HW > 0 && (dx || dgamma || dbeta) &&
            (scratch || !(dgamma || dbeta)), "bn_eval_bwd: bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
     if (dgamma || dbeta) {
-        YFV2_CUDA(cudaMemsetAsync(scratch, 0, (size_t)2 * C * sizeof(double), s));
-        bn_bwd_reduce_kernel<<<dim3(C, bn_slices(N, HW)), 256, 0, s>>>(x, y, dy, save_mean, save_invstd, scratch, N, C, HW, relu);
-        YFV2_LAUNCH_CHECK();
-        bn_affine_grads_kernel<<<(C + 127) / 128, 128, 0, s>>>(scratch, dgamma, dbeta, C);
-        YFV2_LAUNCH_CHECK();
+        add_memset(L, scratch, (size_t)2 * C * sizeof(double));
+        TrainLaunch& r = add(L, TK::bn_bwd_reduce, dim3(C, bn_slices(N, HW)), {x, y, dy, save_mean, save_invstd, scratch}, {N, C, HW, relu});
+        r.slices = (int)r.grid.y;
+        add(L, TK::bn_affine_grads, dim3((C + 127) / 128), {scratch, dgamma, dbeta}, {C}, 128);
     }
-    if (dx) {
-        bn_eval_bwd_apply_kernel<<<dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)), 256, 0, s>>>(y, dy, save_invstd, gamma, dx, C, HW, relu);
-        YFV2_LAUNCH_CHECK();
+    if (dx)
+        add(L, TK::bn_eval_bwd_apply, dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)), {y, dy, save_invstd, gamma, dx}, {C, HW, relu})
+            .vec = YFV2_BN_VEC(HW, reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx));
+    return YFV2_OK;
+}
+
+int describe_maxpool_fwd(const float* x, float* y, int* idx, int planes, int H, int W, TrainLaunches& L) {
+    ARGCHK(x && y && idx, "maxpool_fwd: bad arguments");
+    const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+    add(L, TK::maxpool_fwd, dim3(elem_grid((long long)planes * Ho * Wo, kOpGridCap)), {x, y, idx}, {planes, H, W});
+    return YFV2_OK;
+}
+int describe_maxpool_bwd(const float* dy, const int* idx, float* dx, int planes, int H, int W, TrainLaunches& L) {
+    ARGCHK(dy && idx && dx, "maxpool_bwd: bad arguments");
+    add_memset(L, dx, (size_t)planes * H * W * sizeof(float));
+    const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+    add(L, TK::maxpool_bwd, dim3(elem_grid((long long)planes * Ho * Wo, kOpGridCap)), {dy, idx, dx}, {planes, H, W});
+    return YFV2_OK;
+}
+int describe_upsample2_fwd(const float* x, float* y, int planes, int H, int W, TrainLaunches& L) {
+    ARGCHK(x && y, "upsample2_fwd: bad arguments");
+    add(L, TK::upsample2_fwd, dim3(elem_grid((long long)planes * 4 * H * W, kOpGridCap)), {x, y}, {planes, H, W});
+    return YFV2_OK;
+}
+int describe_upsample2_bwd(const float* dy, float* dx, int planes, int H, int W, TrainLaunches& L) {
+    ARGCHK(dy && dx, "upsample2_bwd: bad arguments");
+    add(L, TK::upsample2_bwd, dim3(elem_grid((long long)planes * H * W, kOpGridCap)), {dy, dx}, {planes, H, W});
+    return YFV2_OK;
+}
+
+void describe_chan_copy(const float* src, int Cs, int soff, int sstep, float* dst, int Cd, int doff, int dstep, int count, int N, int HW,
+                        int accumulate, int sms, TrainLaunches& L) {
+    const long long total = (long long)N * count * HW;
+    add(L, TK::chan_copy, dim3(elem_grid(total, 16LL * sms)), {src, dst}, {Cs, soff, sstep, Cd, doff, dstep, count, HW, total, accumulate})
+        .accumulate = accumulate;
+}
+void describe_axpy(const float* src, float* dst, long long n, int accumulate, int sms, TrainLaunches& L) {
+    add(L, TK::axpy, dim3(elem_grid(n, 16LL * sms)), {src, dst}, {n, accumulate}).accumulate = accumulate;
+}
+
+// The one launch path: the record's kernel with its grid and arguments, or its memset; then the launch check.  The argument order
+// of each kernel is written twice, in its describe_* call of add() and in its case below: a kernel that gains or reorders an
+// argument changes both.
+int launch(const TrainLaunch& L, cudaStream_t s) {
+    if (L.kernel == TK::memset) {
+        YFV2_CUDA(cudaMemsetAsync(const_cast<void*>(L.p[0]), 0, L.bytes, s));
+        return YFV2_OK;
+    }
+    auto F = [&](int i) { return (float*)L.p[i]; };
+    auto D = [&](int i) { return (double*)L.p[i]; };
+    auto I = [&](int i) { return (int)L.n[i]; };
+    const long long* n = L.n;
+    const dim3 g = L.grid;
+    const int b = L.block;
+    const size_t sm = L.smem;
+    switch (L.kernel) {
+    case TK::memset: break;
+    case TK::gemm2_32:
+    case TK::gemm2_64: {
+        const Gemm2Args a{F(0), F(1), F(2), I(0), I(1), I(2), I(3), n[4], n[5], n[6], n[7], n[8], n[9], F(3)};
+        if (L.kernel == TK::gemm2_32) gemm2_kernel<32><<<g, b, sm, s>>>(a);
+        else gemm2_kernel<64><<<g, b, sm, s>>>(a);
+    } break;
+    case TK::wgrad_rows: wgrad_rows_kernel<24, 3><<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2), I(3), F(3)); break;
+    case TK::wgrad_tiled32: wgrad1x1_kernel<32><<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2), I(3), I(4), F(3)); break;
+    case TK::wgrad_tiled64: wgrad1x1_kernel<64><<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2), I(3), I(4), F(3)); break;
+    case TK::wgrad_reduce: wgrad_reduce_kernel<<<g, b, sm, s>>>(F(0), I(0), I(1), F(1)); break;
+    case TK::bias_grad: bias_grad_kernel<<<g, b, sm, s>>>(F(0), F(1), I(0), I(1), I(2)); break;
+    case TK::dw_fwd3: dw_fwd_kernel<3><<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2), I(3), I(4), I(5), I(6)); break;
+    case TK::dw_fwd5: dw_fwd_kernel<5><<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2), I(3), I(4), I(5), I(6)); break;
+    case TK::dw_dgrad3: dw_dgrad_kernel<3><<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2), I(3), I(4), I(5), I(6)); break;
+    case TK::dw_dgrad5: dw_dgrad_kernel<5><<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2), I(3), I(4), I(5), I(6)); break;
+    case TK::dw_wgrad3: dw_wgrad_kernel<3><<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2), I(3), I(4), I(5), I(6)); break;
+    case TK::dw_wgrad5: dw_wgrad_kernel<5><<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2), I(3), I(4), I(5), I(6)); break;
+    case TK::stem_fwd24: stem_fwd_kernel<24><<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2)); break;
+    case TK::stem_fwd_generic: stem_fwd_generic_kernel<<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2), I(3)); break;
+    case TK::stem_wgrad: stem_wgrad_kernel<<<g, b, sm, s>>>(F(0), F(1), F(2), I(0), I(1), I(2), I(3)); break;
+    case TK::bn_stats: bn_stats_kernel<<<g, b, sm, s>>>(F(0), D(1), I(0), I(1), I(2)); break;
+    case TK::bn_finalize: bn_finalize_kernel<<<g, b, sm, s>>>(D(0), F(1), F(2), F(3), F(4), I(0), L.d, L.f); break;
+    case TK::bn_apply: bn_apply_kernel<<<g, b, sm, s>>>(F(0), F(1), F(2), F(3), F(4), F(5), I(0), I(1), I(2)); break;
+    case TK::bn_bwd_reduce: bn_bwd_reduce_kernel<<<g, b, sm, s>>>(F(0), F(1), F(2), F(3), F(4), D(5), I(0), I(1), I(2), I(3)); break;
+    case TK::bn_bwd_apply:
+        bn_bwd_apply_kernel<<<g, b, sm, s>>>(F(0), F(1), F(2), F(3), F(4), F(5), D(6), F(7), F(8), F(9), I(0), I(1), L.d, I(2));
+        break;
+    case TK::bn_eval_stats: bn_eval_stats_kernel<<<g, b, sm, s>>>(F(0), F(1), F(2), F(3), I(0)); break;
+    case TK::bn_eval_bwd_apply: bn_eval_bwd_apply_kernel<<<g, b, sm, s>>>(F(0), F(1), F(2), F(3), F(4), I(0), I(1), I(2)); break;
+    case TK::bn_affine_grads: bn_affine_grads_kernel<<<g, b, sm, s>>>(D(0), F(1), F(2), I(0)); break;
+    case TK::maxpool_fwd: maxpool_fwd_kernel<<<g, b, sm, s>>>(F(0), F(1), (int*)L.p[2], n[0], I(1), I(2)); break;
+    case TK::maxpool_bwd: maxpool_bwd_kernel<<<g, b, sm, s>>>(F(0), (const int*)L.p[1], F(2), n[0], I(1), I(2)); break;
+    case TK::upsample2_fwd: upsample2_fwd_kernel<<<g, b, sm, s>>>(F(0), F(1), n[0], I(1), I(2)); break;
+    case TK::upsample2_bwd: upsample2_bwd_kernel<<<g, b, sm, s>>>(F(0), F(1), n[0], I(1), I(2)); break;
+    case TK::chan_copy: chan_copy_kernel<<<g, b, sm, s>>>(F(0), I(0), I(1), I(2), F(1), I(3), I(4), I(5), I(6), I(7), n[8], I(9)); break;
+    case TK::axpy: axpy_kernel<<<g, b, sm, s>>>(F(0), F(1), n[0], I(1)); break;
+    }
+    YFV2_LAUNCH_CHECK();
+    return YFV2_OK;
+}
+
+int launch_all(const TrainLaunches& L, cudaStream_t s) {
+    for (const TrainLaunch& r : L) {
+        const int rc = launch(r, s);
+        if (rc) return rc;
     }
     return YFV2_OK;
 }
 
-extern "C" YFV2_API int yfv2_op_maxpool_fwd(const float* x, float* y, int* idx, int planes, int H, int W, void* stream) {
-    ARGCHK(x && y && idx, "maxpool_fwd: bad arguments");
-    const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
-    maxpool_fwd_kernel<<<grid_for((long long)planes * Ho * Wo), 256, 0, (cudaStream_t)stream>>>(x, y, idx, planes, H, W);
-    YFV2_LAUNCH_CHECK();
+int debug_records(const TrainLaunches& L, yfv2_train_launch* out, int cap, int* n) {
+    *n = (int)L.size();
+    for (int i = 0; i < cap && i < *n; ++i) {
+        const TrainLaunch& r = L[i];
+        yfv2_train_launch& d = out[i];
+        snprintf(d.kernel, sizeof(d.kernel), "%s", kernel_name(r.kernel));
+        d.op = r.op; d.bwd = r.bwd;
+        d.grid[0] = (int)r.grid.x; d.grid[1] = (int)r.grid.y; d.grid[2] = (int)r.grid.z; d.block = r.block;
+        d.smem = (long long)r.smem; d.bytes = (long long)r.bytes;
+        d.bm = r.bm; d.vec_b = r.vec_b; d.vec_c = r.vec_c; d.vec = r.vec;
+        d.pchunk = r.pchunk; d.chunks = r.chunks; d.partial = r.partial; d.slices = r.slices; d.accumulate = r.accumulate;
+    }
     return YFV2_OK;
+}
+
+}  // namespace yfv2
+
+using namespace yfv2;
+
+namespace {
+// a yfv2_op_* call: its records, then each launched in order
+template <class Describe>
+int run(void* stream, Describe&& describe) {
+    TrainLaunches L;
+    const int rc = describe(L);
+    return rc ? rc : launch_all(L, (cudaStream_t)stream);
+}
+}  // namespace
+
+extern "C" YFV2_API int yfv2_op_conv1x1_fwd(const float* x, const float* w, const float* bias, float* y, int N, int K, int M, int HW, void* stream) {
+    return run(stream, [&](TrainLaunches& L) { return describe_conv1x1_fwd(x, w, bias, y, N, K, M, HW, L); });
+}
+extern "C" YFV2_API int yfv2_op_conv1x1_bwd(const float* x, const float* w, const float* dy, float* dx, float* dw, float* dbias, int N, int K, int M,
+                                            int HW, void* stream) {
+    return run(stream, [&](TrainLaunches& L) { return describe_conv1x1_bwd(x, w, dy, dx, dw, dbias, N, K, M, HW, nullptr, 0, sm_count(), L); });
+}
+extern "C" YFV2_API int yfv2_op_dwconv_fwd(const float* x, const float* w, float* y, int N, int C, int H, int W, int ks, int stride, void* stream) {
+    return run(stream, [&](TrainLaunches& L) { return describe_dwconv_fwd(x, w, y, N, C, H, W, ks, stride, L); });
+}
+extern "C" YFV2_API int yfv2_op_dwconv_bwd(const float* x, const float* w, const float* dy, float* dx, float* dw, int N, int C, int H, int W, int ks,
+                                           int stride, void* stream) {
+    return run(stream, [&](TrainLaunches& L) { return describe_dwconv_bwd(x, w, dy, dx, dw, N, C, H, W, ks, stride, L); });
+}
+extern "C" YFV2_API int yfv2_op_stem_fwd(const float* x, const float* w, float* y, int N, int M, int H, int W, void* stream) {
+    return run(stream, [&](TrainLaunches& L) { return describe_stem_fwd(x, w, y, N, M, H, W, L); });
+}
+extern "C" YFV2_API int yfv2_op_stem_wgrad(const float* x, const float* dy, float* dw, int N, int M, int H, int W, void* stream) {
+    return run(stream, [&](TrainLaunches& L) { return describe_stem_wgrad(x, dy, dw, N, M, H, W, L); });
+}
+extern "C" YFV2_API int yfv2_op_bn_train_fwd(const float* x, const float* gamma, const float* beta, float* running_mean, float* running_var, float* y,
+                                             float* save_mean, float* save_invstd, double* scratch, int N, int C, int HW, int relu, void* stream) {
+    return run(stream, [&](TrainLaunches& L) {
+        return describe_bn_train_fwd(x, gamma, beta, running_mean, running_var, y, save_mean, save_invstd, scratch, N, C, HW, relu, L);
+    });
+}
+extern "C" YFV2_API int yfv2_op_bn_train_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean,
+                                             const float* save_invstd, float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW,
+                                             int relu, void* stream) {
+    return run(stream, [&](TrainLaunches& L) {
+        return describe_bn_train_bwd(x, y, dy, gamma, save_mean, save_invstd, dx, dgamma, dbeta, scratch, N, C, HW, relu, L);
+    });
+}
+extern "C" YFV2_API int yfv2_op_bn_eval_fwd(const float* x, const float* gamma, const float* beta, const float* running_mean,
+                                            const float* running_var, float* y, float* save_mean, float* save_invstd, int N, int C, int HW,
+                                            int relu, void* stream) {
+    return run(stream, [&](TrainLaunches& L) {
+        return describe_bn_eval_fwd(x, gamma, beta, running_mean, running_var, y, save_mean, save_invstd, N, C, HW, relu, L);
+    });
+}
+extern "C" YFV2_API int yfv2_op_bn_eval_bwd(const float* x, const float* y, const float* dy, const float* gamma, const float* save_mean,
+                                            const float* save_invstd, float* dx, float* dgamma, float* dbeta, double* scratch, int N, int C, int HW,
+                                            int relu, void* stream) {
+    return run(stream, [&](TrainLaunches& L) {
+        return describe_bn_eval_bwd(x, y, dy, gamma, save_mean, save_invstd, dx, dgamma, dbeta, scratch, N, C, HW, relu, L);
+    });
+}
+extern "C" YFV2_API int yfv2_op_maxpool_fwd(const float* x, float* y, int* idx, int planes, int H, int W, void* stream) {
+    return run(stream, [&](TrainLaunches& L) { return describe_maxpool_fwd(x, y, idx, planes, H, W, L); });
 }
 extern "C" YFV2_API int yfv2_op_maxpool_bwd(const float* dy, const int* idx, float* dx, int planes, int H, int W, void* stream) {
-    ARGCHK(dy && idx && dx, "maxpool_bwd: bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
-    YFV2_CUDA(cudaMemsetAsync(dx, 0, (size_t)planes * H * W * sizeof(float), s));
-    const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
-    maxpool_bwd_kernel<<<grid_for((long long)planes * Ho * Wo), 256, 0, s>>>(dy, idx, dx, planes, H, W);
-    YFV2_LAUNCH_CHECK();
-    return YFV2_OK;
+    return run(stream, [&](TrainLaunches& L) { return describe_maxpool_bwd(dy, idx, dx, planes, H, W, L); });
 }
 extern "C" YFV2_API int yfv2_op_upsample2_fwd(const float* x, float* y, int planes, int H, int W, void* stream) {
-    ARGCHK(x && y, "upsample2_fwd: bad arguments");
-    upsample2_fwd_kernel<<<grid_for((long long)planes * 4 * H * W), 256, 0, (cudaStream_t)stream>>>(x, y, planes, H, W);
-    YFV2_LAUNCH_CHECK();
-    return YFV2_OK;
+    return run(stream, [&](TrainLaunches& L) { return describe_upsample2_fwd(x, y, planes, H, W, L); });
 }
 extern "C" YFV2_API int yfv2_op_upsample2_bwd(const float* dy, float* dx, int planes, int H, int W, void* stream) {
-    ARGCHK(dy && dx, "upsample2_bwd: bad arguments");
-    upsample2_bwd_kernel<<<grid_for((long long)planes * H * W), 256, 0, (cudaStream_t)stream>>>(dy, dx, planes, H, W);
-    YFV2_LAUNCH_CHECK();
-    return YFV2_OK;
+    return run(stream, [&](TrainLaunches& L) { return describe_upsample2_bwd(dy, dx, planes, H, W, L); });
+}
+
+// ---- test hook: the records of one yfv2_op_* call ---------------------------------------------------------------------------
+extern "C" YFV2_API int yfv2_op_debug_launches(int op, const void* const* ptrs, const int* ints, int sms, yfv2_train_launch* out, int cap,
+                                               int* n) {
+    if (!ptrs || !ints || !n || sms < 0 || cap < 0 || (cap > 0 && !out)) { set_error("op_debug_launches: bad argument"); return YFV2_EINVAL; }
+    auto F = [&](int i) { return (float*)ptrs[i]; };
+    auto D = [&](int i) { return (double*)ptrs[i]; };
+    const int* a = ints;
+    TrainLaunches L;
+    int rc;
+    switch (op) {
+    case YFV2_OP_CONV1X1_FWD: rc = describe_conv1x1_fwd(F(0), F(1), F(2), F(3), a[0], a[1], a[2], a[3], L); break;
+    case YFV2_OP_CONV1X1_BWD:
+        rc = describe_conv1x1_bwd(F(0), F(1), F(2), F(3), F(4), F(5), a[0], a[1], a[2], a[3], nullptr, 0, sms ? sms : sm_count(), L);
+        break;
+    case YFV2_OP_DWCONV_FWD: rc = describe_dwconv_fwd(F(0), F(1), F(2), a[0], a[1], a[2], a[3], a[4], a[5], L); break;
+    case YFV2_OP_DWCONV_BWD: rc = describe_dwconv_bwd(F(0), F(1), F(2), F(3), F(4), a[0], a[1], a[2], a[3], a[4], a[5], L); break;
+    case YFV2_OP_STEM_FWD: rc = describe_stem_fwd(F(0), F(1), F(2), a[0], a[1], a[2], a[3], L); break;
+    case YFV2_OP_STEM_WGRAD: rc = describe_stem_wgrad(F(0), F(1), F(2), a[0], a[1], a[2], a[3], L); break;
+    case YFV2_OP_BN_TRAIN_FWD:
+        rc = describe_bn_train_fwd(F(0), F(1), F(2), F(3), F(4), F(5), F(6), F(7), D(8), a[0], a[1], a[2], a[3], L);
+        break;
+    case YFV2_OP_BN_TRAIN_BWD:
+        rc = describe_bn_train_bwd(F(0), F(1), F(2), F(3), F(4), F(5), F(6), F(7), F(8), D(9), a[0], a[1], a[2], a[3], L);
+        break;
+    case YFV2_OP_BN_EVAL_FWD: rc = describe_bn_eval_fwd(F(0), F(1), F(2), F(3), F(4), F(5), F(6), F(7), a[0], a[1], a[2], a[3], L); break;
+    case YFV2_OP_BN_EVAL_BWD:
+        rc = describe_bn_eval_bwd(F(0), F(1), F(2), F(3), F(4), F(5), F(6), F(7), F(8), D(9), a[0], a[1], a[2], a[3], L);
+        break;
+    case YFV2_OP_MAXPOOL_FWD: rc = describe_maxpool_fwd(F(0), F(1), (int*)ptrs[2], a[0], a[1], a[2], L); break;
+    case YFV2_OP_MAXPOOL_BWD: rc = describe_maxpool_bwd(F(0), (const int*)ptrs[1], F(2), a[0], a[1], a[2], L); break;
+    case YFV2_OP_UPSAMPLE2_FWD: rc = describe_upsample2_fwd(F(0), F(1), a[0], a[1], a[2], L); break;
+    case YFV2_OP_UPSAMPLE2_BWD: rc = describe_upsample2_bwd(F(0), F(1), a[0], a[1], a[2], L); break;
+    default: set_error("op_debug_launches: unknown op %d", op); return YFV2_EINVAL;
+    }
+    if (rc) return rc;
+    return debug_records(L, out, cap, n);
 }

@@ -14,8 +14,8 @@
 //   * a tensor with several consumers (the input of a stride-2 block, C2, C3, S2, S3, the head features feeding obj and cls) gets
 //     the gradient of the consumer that runs first in the backward by assignment and the others by accumulation through a
 //     scratch tensor; the shared output convolutions (used at both pyramid levels) accumulate their weight gradients the same way.
-// The arithmetic is the training operators of k_train.cu (yfv2_op_*).  Gradients of all 225 parameters leave in ONE flat buffer in
-// parameter order (the bucket train_ddp.py all-reduces), either assigned or accumulated.
+// The arithmetic is the training operators of k_train.cu: the step is the list of their describe_* records.  Gradients of all 225
+// parameters leave in ONE flat buffer in parameter order (the bucket train_ddp.py all-reduces), either assigned or accumulated.
 //
 // Fine-tuning mode (yfv2_trainer_set_mode): what autograd does for parameters with requires_grad=False and BatchNorm modules in
 // .eval() inside a train-mode model.  The static program stays; the mode only selects, per op, the kernels and outputs:
@@ -251,7 +251,7 @@ void build(yfv2_trainer& t) {
     long long biggest = 0, pbig = 0;
     for (const Ten& x_ : t.tens) if (x_.ext == -1) biggest = std::max(biggest, (long long)t.N * x_.C * x_.H * x_.W);
     for (long long n : t.pnumel) pbig = std::max(pbig, n);
-    // the second use of a shared output convolution puts its bias gradient right behind the weight's (run_backward)
+    // the second use of a shared output convolution puts its bias gradient right behind the weight's (describe_backward)
     for (int w : {w_reg, w_obj, w_cls}) pbig = std::max(pbig, t.pnumel[w] + t.pnumel[w + 1]);
     t.scratch_off = b.alloc(biggest);
     t.pscratch_off = b.alloc(pbig);
@@ -285,66 +285,12 @@ void apply_mode(yfv2_trainer& t) {
     t.mode_hash = h;
 }
 
-// dst[n][doff + c*dstep][p] (+)= src[n][soff + c*sstep][p],  c < count
-__global__ void chan_copy_kernel(const float* __restrict__ src, int Cs, int soff, int sstep, float* __restrict__ dst, int Cd, int doff, int dstep,
-                                 int count, int HW, long long total, int accumulate) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int p = (int)(i % HW);
-        const long long r = i / HW;
-        const int c = (int)(r % count);
-        const long long n = r / count;
-        const float v = src[(n * Cs + soff + (long long)c * sstep) * HW + p];
-        float* d = dst + (n * Cd + doff + (long long)c * dstep) * HW + p;
-        *d = accumulate ? *d + v : v;
-    }
-}
-__global__ void axpy_kernel(const float* __restrict__ src, float* __restrict__ dst, long long n, int accumulate) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        dst[i] = accumulate ? dst[i] + src[i] : src[i];
-}
-int grid_for(long long total) {
-    long long g = (total + 255) / 256;
-    const long long cap = (long long)sm_count() * 16;
-    return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-int chan_copy(const float* src, int Cs, int soff, int sstep, float* dst, int Cd, int doff, int dstep, int count, int N, int HW, int acc,
-              cudaStream_t s) {
-    const long long total = (long long)N * count * HW;
-    chan_copy_kernel<<<grid_for(total), 256, 0, s>>>(src, Cs, soff, sstep, dst, Cd, doff, dstep, count, HW, total, acc);
-    YFV2_LAUNCH_CHECK();
-    return YFV2_OK;
-}
-int axpy(const float* src, float* dst, long long n, int acc, cudaStream_t s) {
-    axpy_kernel<<<grid_for(n), 256, 0, s>>>(src, dst, n, acc);
-    YFV2_LAUNCH_CHECK();
-    return YFV2_OK;
-}
-
 #define TRYT(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
 
 }  // namespace
 }  // namespace yfv2
 
 using namespace yfv2;
-
-extern "C" {
-int yfv2_op_conv1x1_fwd(const float*, const float*, const float*, float*, int, int, int, int, void*);
-int yfv2_op_conv1x1_bwd(const float*, const float*, const float*, float*, float*, float*, int, int, int, int, void*);
-int yfv2_op_dwconv_fwd(const float*, const float*, float*, int, int, int, int, int, int, void*);
-int yfv2_op_dwconv_bwd(const float*, const float*, const float*, float*, float*, int, int, int, int, int, int, void*);
-int yfv2_op_stem_fwd(const float*, const float*, float*, int, int, int, int, void*);
-int yfv2_op_stem_wgrad(const float*, const float*, float*, int, int, int, int, void*);
-int yfv2_op_bn_train_fwd(const float*, const float*, const float*, float*, float*, float*, float*, float*, double*, int, int, int, int, void*);
-int yfv2_op_bn_train_bwd(const float*, const float*, const float*, const float*, const float*, const float*, float*, float*, float*, double*,
-                         int, int, int, int, void*);
-int yfv2_op_bn_eval_fwd(const float*, const float*, const float*, const float*, const float*, float*, float*, float*, int, int, int, int, void*);
-int yfv2_op_bn_eval_bwd(const float*, const float*, const float*, const float*, const float*, const float*, float*, float*, float*, double*,
-                        int, int, int, int, void*);
-int yfv2_op_maxpool_fwd(const float*, float*, int*, int, int, int, void*);
-int yfv2_op_maxpool_bwd(const float*, const int*, float*, int, int, int, void*);
-int yfv2_op_upsample2_fwd(const float*, float*, int, int, int, void*);
-int yfv2_op_upsample2_bwd(const float*, float*, int, int, int, void*);
-}
 
 extern "C" int yfv2_trainer_create(yfv2_trainer** out, int device, int N, int H, int W, int A, int C) {
     if (!out || N <= 0 || H <= 0 || W <= 0 || H % 32 || W % 32 || A <= 0 || C <= 0) {
@@ -464,50 +410,55 @@ struct Ptrs {
 };
 }  // namespace
 
-static int run_forward(yfv2_trainer* t, const float* x, const float* const* params, float* const* bn_running,
-                       float* const preds[6], void* workspace, cudaStream_t s) {
+// The records of the train-mode forward, in launch order: what yfv2_train_forward captures and yfv2_trainer_debug_launches returns
+static int describe_forward(const yfv2_trainer* t, const float* x, const float* const* params, float* const* bn_running,
+                            float* const preds[6], void* workspace, int sms, TrainLaunches& L) {
     Ptrs P{(float*)workspace, x, preds, nullptr};
     const int N = t->N;
-    for (const Op& o : t->ops) {
+    for (int oi = 0; oi < (int)t->ops.size(); ++oi) {
+        const Op& o = t->ops[oi];
+        const size_t first = L.size();
         const Ten& A = t->tens[o.a];
         const Ten& Y = t->tens[o.y];
         const float* a = P.act(*t, o.a);
         float* y = P.actw(*t, o.y);
         switch (o.kind) {
-        case K_STEM: TRYT(yfv2_op_stem_fwd(a, params[o.pw], y, N, Y.C, A.H, A.W, s)); break;
+        case K_STEM: TRYT(describe_stem_fwd(a, params[o.pw], y, N, Y.C, A.H, A.W, L)); break;
         case K_BN: {
             double* scr = reinterpret_cast<double*>(P.ws + o.aux);
             float* mean = P.ws + o.aux + 4LL * A.C;
             if (t->bn_eval[o.bn])
-                TRYT(yfv2_op_bn_eval_fwd(a, params[o.pg], params[o.pb], bn_running[2 * o.bn], bn_running[2 * o.bn + 1], y, mean, mean + A.C,
-                                         N, A.C, A.H * A.W, o.relu, s));
+                TRYT(describe_bn_eval_fwd(a, params[o.pg], params[o.pb], bn_running[2 * o.bn], bn_running[2 * o.bn + 1], y, mean, mean + A.C,
+                                          N, A.C, A.H * A.W, o.relu, L));
             else
-                TRYT(yfv2_op_bn_train_fwd(a, params[o.pg], params[o.pb], bn_running[2 * o.bn], bn_running[2 * o.bn + 1], y, mean, mean + A.C, scr,
-                                          N, A.C, A.H * A.W, o.relu, s));
+                TRYT(describe_bn_train_fwd(a, params[o.pg], params[o.pb], bn_running[2 * o.bn], bn_running[2 * o.bn + 1], y, mean, mean + A.C,
+                                           scr, N, A.C, A.H * A.W, o.relu, L));
         } break;
-        case K_POOL: TRYT(yfv2_op_maxpool_fwd(a, y, reinterpret_cast<int*>(P.ws + o.aux), N * A.C, A.H, A.W, s)); break;
-        case K_PW: TRYT(yfv2_op_conv1x1_fwd(a, params[o.pw], o.pbias >= 0 ? params[o.pbias] : nullptr, y, N, A.C, o.M, A.H * A.W, s)); break;
-        case K_DW: TRYT(yfv2_op_dwconv_fwd(a, params[o.pw], y, N, A.C, A.H, A.W, o.ks, o.stride, s)); break;
-        case K_UP: TRYT(yfv2_op_upsample2_fwd(a, y, N * A.C, A.H, A.W, s)); break;
-        case K_ODD: TRYT(chan_copy(a, A.C, 1, 2, y, Y.C, 0, 1, Y.C, N, A.H * A.W, 0, s)); break;
+        case K_POOL: TRYT(describe_maxpool_fwd(a, y, reinterpret_cast<int*>(P.ws + o.aux), N * A.C, A.H, A.W, L)); break;
+        case K_PW: TRYT(describe_conv1x1_fwd(a, params[o.pw], o.pbias >= 0 ? params[o.pbias] : nullptr, y, N, A.C, o.M, A.H * A.W, L)); break;
+        case K_DW: TRYT(describe_dwconv_fwd(a, params[o.pw], y, N, A.C, A.H, A.W, o.ks, o.stride, L)); break;
+        case K_UP: TRYT(describe_upsample2_fwd(a, y, N * A.C, A.H, A.W, L)); break;
+        case K_ODD: describe_chan_copy(a, A.C, 1, 2, y, Y.C, 0, 1, Y.C, N, A.H * A.W, 0, sms, L); break;
         case K_CATE: {
             const Ten& B = t->tens[o.b];
-            TRYT(chan_copy(a, A.C, 0, 2, y, Y.C, 0, 1, A.C / 2, N, A.H * A.W, 0, s));
-            TRYT(chan_copy(P.act(*t, o.b), B.C, 0, 1, y, Y.C, A.C / 2, 1, B.C, N, A.H * A.W, 0, s));
+            describe_chan_copy(a, A.C, 0, 2, y, Y.C, 0, 1, A.C / 2, N, A.H * A.W, 0, sms, L);
+            describe_chan_copy(P.act(*t, o.b), B.C, 0, 1, y, Y.C, A.C / 2, 1, B.C, N, A.H * A.W, 0, sms, L);
         } break;
         case K_CAT2: {
             const Ten& B = t->tens[o.b];
-            TRYT(chan_copy(a, A.C, 0, 1, y, Y.C, 0, 1, A.C, N, Y.H * Y.W, 0, s));
-            TRYT(chan_copy(P.act(*t, o.b), B.C, 0, 1, y, Y.C, A.C, 1, B.C, N, Y.H * Y.W, 0, s));
+            describe_chan_copy(a, A.C, 0, 1, y, Y.C, 0, 1, A.C, N, Y.H * Y.W, 0, sms, L);
+            describe_chan_copy(P.act(*t, o.b), B.C, 0, 1, y, Y.C, A.C, 1, B.C, N, Y.H * Y.W, 0, sms, L);
         } break;
         default: set_error("train_forward: unknown op"); return YFV2_EINVAL;
         }
+        for (size_t j = first; j < L.size(); ++j) L[j].op = oi;
     }
     return YFV2_OK;
 }
 
-static int run_backward(yfv2_trainer* t, const float* x, const float* const* params, float* const preds[6],
-                        const float* const dpreds[6], float* grads_flat, int accumulate, void* workspace, cudaStream_t s) {
+// The records of the backward under the current mode, in launch order: what yfv2_train_backward captures
+static int describe_backward(const yfv2_trainer* t, const float* x, const float* const* params, float* const preds[6],
+                             const float* const dpreds[6], float* grads_flat, int accumulate, void* workspace, int sms, TrainLaunches& L) {
     Ptrs P{(float*)workspace, x, preds, dpreds};
     const int N = t->N;
     float* G = P.ws + t->gflat_off;                 // parameter gradients of this step, assigned
@@ -516,14 +467,15 @@ static int run_backward(yfv2_trainer* t, const float* x, const float* const* par
     std::vector<char> pwritten(t->poff.size(), 0);
     // parameter gradient target: the flat slot on first use, the parameter scratch (then added) for a shared layer's second use
     auto ptarget = [&](int idx, bool* via) { *via = pwritten[idx] != 0; return *via ? pscratch : G + t->poff[idx]; };
-    auto pcommit = [&](int idx, bool via) -> int {
+    auto pcommit = [&](int idx, bool via) {
         pwritten[idx] = 1;
-        return via ? axpy(pscratch, G + t->poff[idx], t->pnumel[idx], 1, s) : YFV2_OK;
+        if (via) describe_axpy(pscratch, G + t->poff[idx], t->pnumel[idx], 1, sms, L);
     };
     for (int oi = (int)t->ops.size() - 1; oi >= 0; --oi) {
         const Op& o = t->ops[oi];
         const BwdOp& bo = t->bwd[oi];
         if (!bo.run) continue;                      // no trainable parameter upstream of its output
+        const size_t first = L.size();
         const Ten& A = t->tens[o.a];
         const Ten& Y = t->tens[o.y];
         const float* a = P.act(*t, o.a);
@@ -537,8 +489,8 @@ static int run_backward(yfv2_trainer* t, const float* x, const float* const* par
         switch (o.kind) {
         case K_STEM: {                              // runs only for a trainable stem weight (the image needs no gradient)
             bool via; float* dw = ptarget(o.pw, &via);
-            TRYT(yfv2_op_stem_wgrad(a, dy, dw, N, Y.C, A.H, A.W, s));
-            TRYT(pcommit(o.pw, via));
+            TRYT(describe_stem_wgrad(a, dy, dw, N, Y.C, A.H, A.W, L));
+            pcommit(o.pw, via);
         } break;
         case K_BN: {
             double* scr = reinterpret_cast<double*>(P.ws + o.aux);
@@ -547,48 +499,50 @@ static int run_backward(yfv2_trainer* t, const float* x, const float* const* par
             float* dg = bo.dgamma ? G + t->poff[o.pg] : nullptr;
             float* db = bo.dbeta ? G + t->poff[o.pb] : nullptr;
             if (bo.bn_eval) {
-                TRYT(yfv2_op_bn_eval_bwd(a, P.act(*t, o.y), dy, params[o.pg], mean, mean + A.C, da, dg, db, scr, N, A.C, A.H * A.W, o.relu, s));
+                TRYT(describe_bn_eval_bwd(a, P.act(*t, o.y), dy, params[o.pg], mean, mean + A.C, da, dg, db, scr, N, A.C, A.H * A.W, o.relu, L));
             } else {
                 // the batch-statistics backward needs the sums for its gamma / beta anyway; without rg(a) its dx goes to a's own
                 // gradient slot, which nothing reads (a's producer does not run)
-                TRYT(yfv2_op_bn_train_bwd(a, P.act(*t, o.y), dy, params[o.pg], mean, mean + A.C, da ? da : P.gradw(*t, o.a), dg, db, scr,
-                                          N, A.C, A.H * A.W, o.relu, s));
+                TRYT(describe_bn_train_bwd(a, P.act(*t, o.y), dy, params[o.pg], mean, mean + A.C, da ? da : P.gradw(*t, o.a), dg, db, scr,
+                                           N, A.C, A.H * A.W, o.relu, L));
             }
             if (dg) pwritten[o.pg] = 1;
             if (db) pwritten[o.pb] = 1;
         } break;
-        case K_POOL: TRYT(yfv2_op_maxpool_bwd(dy, reinterpret_cast<const int*>(P.ws + o.aux), da, N * A.C, A.H, A.W, s)); break;
+        case K_POOL: TRYT(describe_maxpool_bwd(dy, reinterpret_cast<const int*>(P.ws + o.aux), da, N * A.C, A.H, A.W, L)); break;
         case K_PW: {
             bool vw = false, vb = false;
             float* dw = bo.dw ? ptarget(o.pw, &vw) : nullptr;
             float* db = nullptr;
             if (bo.dbias) { vb = pwritten[o.pbias] != 0; db = vb ? pscratch + t->pnumel[o.pw] : G + t->poff[o.pbias]; }  // bias rides behind the weight in the scratch
-            TRYT(conv1x1_bwd_impl(a, params[o.pw], dy, da, dw, db, N, A.C, o.M, A.H * A.W, P.ws + t->wscratch_off, (size_t)kWScratchFloats, s));
-            if (vb) { TRYT(axpy(pscratch + t->pnumel[o.pw], G + t->poff[o.pbias], t->pnumel[o.pbias], 1, s)); }
-            if (dw) TRYT(pcommit(o.pw, vw));
+            TRYT(describe_conv1x1_bwd(a, params[o.pw], dy, da, dw, db, N, A.C, o.M, A.H * A.W, P.ws + t->wscratch_off, (size_t)kWScratchFloats,
+                                      sms, L));
+            if (vb) describe_axpy(pscratch + t->pnumel[o.pw], G + t->poff[o.pbias], t->pnumel[o.pbias], 1, sms, L);
+            if (dw) pcommit(o.pw, vw);
             if (db) pwritten[o.pbias] = 1;
         } break;
         case K_DW: {
             bool vw = false; float* dw = bo.dw ? ptarget(o.pw, &vw) : nullptr;
-            TRYT(yfv2_op_dwconv_bwd(a, params[o.pw], dy, da, dw, N, A.C, A.H, A.W, o.ks, o.stride, s));
-            if (dw) TRYT(pcommit(o.pw, vw));
+            TRYT(describe_dwconv_bwd(a, params[o.pw], dy, da, dw, N, A.C, A.H, A.W, o.ks, o.stride, L));
+            if (dw) pcommit(o.pw, vw);
         } break;
-        case K_UP: TRYT(yfv2_op_upsample2_bwd(dy, da, N * A.C, A.H, A.W, s)); break;
-        case K_ODD: TRYT(chan_copy(dy, Y.C, 0, 1, P.gradw(*t, o.a), A.C, 1, 2, Y.C, N, A.H * A.W, 0, s)); break;          // odd half of d(a)
+        case K_UP: TRYT(describe_upsample2_bwd(dy, da, N * A.C, A.H, A.W, L)); break;
+        case K_ODD: describe_chan_copy(dy, Y.C, 0, 1, P.gradw(*t, o.a), A.C, 1, 2, Y.C, N, A.H * A.W, 0, sms, L); break;          // odd half of d(a)
         case K_CATE: {
             const Ten& B = t->tens[o.b];
-            if (bo.da) TRYT(chan_copy(dy, Y.C, 0, 1, P.gradw(*t, o.a), A.C, 0, 2, A.C / 2, N, A.H * A.W, 0, s));              // even half of d(a)
-            if (bo.db) TRYT(chan_copy(dy, Y.C, A.C / 2, 1, P.gradw(*t, o.b), B.C, 0, 1, B.C, N, A.H * A.W, 0, s));
+            if (bo.da) describe_chan_copy(dy, Y.C, 0, 1, P.gradw(*t, o.a), A.C, 0, 2, A.C / 2, N, A.H * A.W, 0, sms, L);              // even half of d(a)
+            if (bo.db) describe_chan_copy(dy, Y.C, A.C / 2, 1, P.gradw(*t, o.b), B.C, 0, 1, B.C, N, A.H * A.W, 0, sms, L);
         } break;
         case K_CAT2: {
             const Ten& B = t->tens[o.b];
             const bool acc_b = B.last_use != oi;
-            if (bo.da) TRYT(chan_copy(dy, Y.C, 0, 1, P.gradw(*t, o.a), A.C, 0, 1, A.C, N, Y.H * Y.W, acc_a ? 1 : 0, s));
-            if (bo.db) TRYT(chan_copy(dy, Y.C, A.C, 1, P.gradw(*t, o.b), B.C, 0, 1, B.C, N, Y.H * Y.W, acc_b ? 1 : 0, s));
+            if (bo.da) describe_chan_copy(dy, Y.C, 0, 1, P.gradw(*t, o.a), A.C, 0, 1, A.C, N, Y.H * Y.W, acc_a ? 1 : 0, sms, L);
+            if (bo.db) describe_chan_copy(dy, Y.C, A.C, 1, P.gradw(*t, o.b), B.C, 0, 1, B.C, N, Y.H * Y.W, acc_b ? 1 : 0, sms, L);
         } break;
         default: set_error("train_backward: unknown op"); return YFV2_EINVAL;
         }
-        if (acc_a && o.kind != K_CAT2 && o.kind != K_ODD && o.kind != K_CATE) { TRYT(axpy(scratch, P.gradw(*t, o.a), an, 1, s)); }
+        if (acc_a && o.kind != K_CAT2 && o.kind != K_ODD && o.kind != K_CATE) describe_axpy(scratch, P.gradw(*t, o.a), an, 1, sms, L);
+        for (size_t j = first; j < L.size(); ++j) { L[j].op = oi; L[j].bwd = true; }
     }
     for (size_t i = 0; i < pwritten.size(); ++i)
         if ((pwritten[i] != 0) != (t->trainable[i] != 0)) {
@@ -602,13 +556,19 @@ static int run_backward(yfv2_trainer* t, const float* x, const float* const* par
         size_t j = i;
         long long n = 0;
         while (j < t->poff.size() && t->trainable[j]) n += t->pnumel[j++];
-        TRYT(axpy(G + t->poff[i], grads_flat + t->coff[i], n, accumulate ? 1 : 0, s));
+        describe_axpy(G + t->poff[i], grads_flat + t->coff[i], n, accumulate ? 1 : 0, sms, L);
+        L.back().bwd = true;
         i = j;
     }
     return YFV2_OK;
 }
 
 namespace {
+// yfv2_train_backward's refusal of a mode with no trainable parameter (torch: nothing requires grad), shared with its test hook
+int check_trainable(const yfv2_trainer* t) {
+    if (t->ctotal == 0) { set_error("train_backward: no parameter is trainable (element 0 of tensors does not require grad)"); return YFV2_EINVAL; }
+    return YFV2_OK;
+}
 unsigned long long mix(unsigned long long h, unsigned long long v) {
     h ^= v + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2);
     return h;
@@ -647,7 +607,11 @@ extern "C" int yfv2_train_forward(yfv2_trainer* t, const float* x, const float* 
     for (int i = 0; i < YFV2_NUM_PARAMS; ++i) key = mix(key, params[i]);
     for (int i = 0; i < 2 * YFV2_NUM_BN; ++i) key = mix(key, bn_running[i]);
     for (int i = 0; i < 6; ++i) key = mix(key, preds[i]);
-    const int rc = replay_or_capture(t, t->g_fwd, key, s, [&](cudaStream_t cs) { return run_forward(t, x, params, bn_running, preds, workspace, cs); });
+    const int rc = replay_or_capture(t, t->g_fwd, key, s, [&](cudaStream_t cs) {
+        TrainLaunches L;
+        TRYT(describe_forward(t, x, params, bn_running, preds, workspace, sm_count(), L));
+        return launch_all(L, cs);
+    });
     if (rc == YFV2_OK) { t->fwd_trainable = t->trainable; t->fwd_bn_eval = t->bn_eval; }
     return rc;
 }
@@ -657,7 +621,7 @@ extern "C" int yfv2_train_backward(yfv2_trainer* t, const float* x, const float*
     if (!t || !x || !params || !preds || !dpreds || !grads_flat || !workspace) { set_error("train_backward: null argument"); return YFV2_EINVAL; }
     for (int i = 0; i < 6; ++i) if (!preds[i] || !dpreds[i]) { set_error("train_backward: null head tensor %d", i); return YFV2_EINVAL; }
     for (int i = 0; i < YFV2_NUM_PARAMS; ++i) if (!params[i]) { set_error("train_backward: null parameter %d", i); return YFV2_EINVAL; }
-    if (t->ctotal == 0) { set_error("train_backward: no parameter is trainable (element 0 of tensors does not require grad)"); return YFV2_EINVAL; }
+    TRYT(check_trainable(t));
     if (t->trainable != t->fwd_trainable || t->bn_eval != t->fwd_bn_eval) {
         set_error("train_backward: the mode changed after the forward (yfv2_trainer_set_mode applies from the next yfv2_train_forward)");
         return YFV2_EINVAL;
@@ -666,6 +630,27 @@ extern "C" int yfv2_train_backward(yfv2_trainer* t, const float* x, const float*
     unsigned long long key = mix(mix(mix(mix(0x4321ull, t->mode_hash), x), workspace), grads_flat);
     for (int i = 0; i < YFV2_NUM_PARAMS; ++i) key = mix(key, params[i]);
     for (int i = 0; i < 6; ++i) key = mix(mix(key, preds[i]), dpreds[i]);
-    return replay_or_capture(t, t->g_bwd[accumulate ? 1 : 0], key, s,
-                             [&](cudaStream_t cs) { return run_backward(t, x, params, preds, dpreds, grads_flat, accumulate, workspace, cs); });
+    return replay_or_capture(t, t->g_bwd[accumulate ? 1 : 0], key, s, [&](cudaStream_t cs) {
+        TrainLaunches L;
+        TRYT(describe_backward(t, x, params, preds, dpreds, grads_flat, accumulate, workspace, sm_count(), L));
+        return launch_all(L, cs);
+    });
+}
+
+// ---- test hook: the records of one training step ------------------------------------------------------------------------------
+extern "C" int yfv2_trainer_debug_launches(const yfv2_trainer* t, const void* workspace, int sms, yfv2_train_launch* out, int cap, int* n) {
+    if (!t || !n || sms < 0 || cap < 0 || (cap > 0 && !out)) { set_error("trainer_debug_launches: bad argument"); return YFV2_EINVAL; }
+    TRYT(check_trainable(t));
+    // the caller's tensors: any 16-byte-aligned addresses (never dereferenced); NULL workspace: a 16-byte-aligned one
+    float* const fake = reinterpret_cast<float*>((uintptr_t)256);
+    void* ws = workspace ? const_cast<void*>(workspace) : fake;
+    const std::vector<const float*> params(YFV2_NUM_PARAMS, fake);
+    const std::vector<float*> bn_running(2 * YFV2_NUM_BN, fake);
+    float* const preds[6] = {fake, fake, fake, fake, fake, fake};
+    const float* const dpreds[6] = {fake, fake, fake, fake, fake, fake};
+    if (!sms) sms = sm_count();
+    TrainLaunches L;
+    TRYT(describe_forward(t, fake, params.data(), bn_running.data(), preds, ws, sms, L));
+    TRYT(describe_backward(t, fake, params.data(), preds, dpreds, fake, 0, ws, sms, L));
+    return debug_records(L, out, cap, n);
 }

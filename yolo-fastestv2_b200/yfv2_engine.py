@@ -151,6 +151,52 @@ def plan_launches(handle, workspace=None, is_u8=False, sms=0):
     return out
 
 
+class TrainLaunchRecord(ctypes.Structure):
+    """yfv2_train_launch: one kernel launch or memset of a training operator or a native training step (test hook)."""
+    _fields_ = [("kernel", ctypes.c_char * 32), ("op", ctypes.c_int), ("bwd", ctypes.c_int), ("grid", ctypes.c_int * 3), ("block", ctypes.c_int),
+                ("smem", ctypes.c_longlong), ("bytes", ctypes.c_longlong)] + \
+               [(f, ctypes.c_int) for f in ("bm", "vec_b", "vec_c", "vec", "pchunk", "chunks", "partial", "slices", "accumulate")]
+
+
+TRAIN_OPS = ("conv1x1_fwd", "conv1x1_bwd", "dwconv_fwd", "dwconv_bwd", "stem_fwd", "stem_wgrad", "bn_train_fwd", "bn_train_bwd",
+             "bn_eval_fwd", "bn_eval_bwd", "maxpool_fwd", "maxpool_bwd", "upsample2_fwd", "upsample2_bwd")     # YFV2_OP_*
+
+
+def _train_launches(call, what):
+    n = ctypes.c_int()
+    _check(call(None, 0, ctypes.byref(n)), what)
+    recs = (TrainLaunchRecord * n.value)()
+    _check(call(recs, n.value, ctypes.byref(n)), what)
+    names = [f for f, _ in TrainLaunchRecord._fields_]
+    out = []
+    for r in recs:
+        d = {f: getattr(r, f) for f in names}
+        d["kernel"], d["grid"], d["bwd"] = r.kernel.decode(), tuple(r.grid), bool(r.bwd)
+        out.append(d)
+    return out
+
+
+def trainer_launches(handle, workspace=None, sms=0):
+    """The kernel launches and memsets of one training step of a yfv2_trainer handle under its current mode (forward, then backward
+    with accumulate = 0), in order, as dicts (yfv2_trainer_debug_launches; host only).  workspace None: a 16-byte-aligned workspace;
+    sms 0: this device's SM count."""
+    L, ws = lib(), ctypes.c_void_p(workspace)
+    return _train_launches(lambda out, cap, n: L.yfv2_trainer_debug_launches(handle, ws, sms, out, cap, n), "trainer_debug_launches")
+
+
+def op_launches(name, ptrs, ints, sms=0):
+    """The kernel launches and memsets of one yfv2_op_<name> call, in order, as dicts (yfv2_op_debug_launches; host only).  ptrs: the
+    call's pointer arguments as integer addresses (None: NULL), ints: its integer arguments, both in signature order."""
+    args = PROTOTYPES["yfv2_op_" + name][1][:-1]                         # the call's arguments without the stream
+    want = (sum(a is ctypes.c_void_p for a in args), sum(a is ctypes.c_int for a in args))
+    if (len(ptrs), len(ints)) != want:
+        raise Yfv2Error("op_launches: yfv2_op_%s takes %d pointers and %d integers, got %d and %d" % ((name,) + want + (len(ptrs), len(ints))))
+    L = lib()
+    p = (ctypes.c_void_p * len(ptrs))(*ptrs)
+    i = (ctypes.c_int * len(ints))(*ints)
+    return _train_launches(lambda out, cap, n: L.yfv2_op_debug_launches(TRAIN_OPS.index(name), p, i, sms, out, cap, n), "op_debug_launches")
+
+
 def check_bn_batch(N, H, W):
     """F.batch_norm in training mode refuses a layer with one value per channel; the deepest BatchNorm layers of the network run
     at stride 32 (stem 3x3 s2, max-pool 3x3 s2 p1 and three stride-2 blocks: each (h - 1) // 2 + 1), the first of them on the
@@ -320,6 +366,10 @@ PROTOTYPES = {
     "yfv2_debug_gather": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
                                          ctypes.POINTER(ctypes.c_int), ctypes.c_void_p]),
     "yfv2_debug_nms_profile": (ctypes.c_int, [ctypes.c_void_p]),
+    "yfv2_op_debug_launches": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                              ctypes.POINTER(ctypes.c_int)]),
+    "yfv2_trainer_debug_launches": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                                   ctypes.POINTER(ctypes.c_int)]),
     "yfv2_plan_debug_launches": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                 ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
     "yfv2_jpeg_parse": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
