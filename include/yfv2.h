@@ -401,6 +401,31 @@ typedef struct yfv2_yuv422_frame {
 } yfv2_yuv422_frame;
 YFV2_API int yfv2_resize_yuv422_u8(const yfv2_yuv422_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
 
+/* ---- raw Bayer frames -> network input: cv2.cvtColor(COLOR_Bayer??2BGR / _EA) + cv2.resize INTER_LINEAR ----------------------
+ * What machine-vision (GigE Vision, USB3 Vision) and CSI sensors deliver: one byte per pixel through a 2x2 colour filter array.
+ * red_x, red_y are the column and row parity of the red sites; cv2's codes (its sensor-order aliases, COLOR_BayerRGGB2BGR ==
+ * COLOR_BayerBG2BGR and so on, are the same codes):
+ *   COLOR_BayerBG2BGR (raw rows R G / G B): 0, 0      COLOR_BayerGB2BGR (G R / B G): 1, 0
+ *   COLOR_BayerRG2BGR (B G / G R):          1, 1      COLOR_BayerGR2BGR (G B / R G): 0, 1
+ * edge_aware 0 is the bilinear demosaic (COLOR_Bayer??2BGR), 1 the edge-aware one (COLOR_Bayer??2BGR_EA), which differs only in
+ * G at the R and B sites: (L + R + 1) >> 1 when |L - R| <= |U - D|, else (U + D + 1) >> 1.  The whole demosaic, its borders (the
+ * interior pixel at the clamped coordinate) and frames under 3 pixels on a side (all zeros) are stated in DESIGN.md §17 and
+ * tests/bayer_oracle.py.
+ * The demosaic of a pixel reads its neighbours and the frame's edges, so a crop of the raw bytes does not convert to the crop of
+ * the converted frame.  A descriptor therefore names the WHOLE frame (data, pitch, fw, fh) and the window of its conversion that
+ * it stands for: the source image is cv2.cvtColor(raw, code)[y0:y0+h, x0:x0+w], any offsets, odd ones included.
+ * Needs data non-null, fw, fh >= 1, pitch >= fw, the window non-empty and inside the frame, red_x, red_y and edge_aware 0 or 1.
+ * frames, dst, H, W: as yfv2_resize_strided_u8 (64 descriptors per launch). */
+typedef struct yfv2_bayer_frame {
+    const uint8_t* data;   /* device pointer to raw pixel (0,0) of the WHOLE frame */
+    long long pitch;       /* bytes from one raw row to the next, >= fw */
+    int fw, fh;            /* the whole frame: the demosaic's borders are its edges */
+    int x0, y0, w, h;      /* the window of the converted frame this descriptor stands for */
+    int red_x, red_y;      /* column / row parity of the red sites */
+    int edge_aware;        /* 0: COLOR_Bayer??2BGR, 1: COLOR_Bayer??2BGR_EA */
+} yfv2_bayer_frame;
+YFV2_API int yfv2_resize_bayer_u8(const yfv2_bayer_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
+
 /* ---- JPEG files -> packed HWC BGR frames: cv2.imread(path) (test.py:34; utils/datasets.py:106) on the device -----------------
  * The bytes OpenCV 4.13 (libjpeg-turbo 3.1) returns for IMREAD_COLOR: ISLOW IDCT, fancy upsampling, jdcolor's YCbCr -> BGR, grey
  * replicated to B = G = R, and the EXIF orientation applied.  Supported: baseline sequential Huffman-coded DCT (SOF0, SOF1) with
@@ -494,6 +519,7 @@ YFV2_API int yfv2_jpeg_decode_resize(const void* meta_host, const void* meta_dev
 #define YFV2_JPEG_SRC_GRAY    2   /* f.strided, the byte at b: a one-component JPEG */
 #define YFV2_JPEG_SRC_YUV420  3   /* f.yuv420 */
 #define YFV2_JPEG_SRC_YUV422  4   /* f.yuv422 */
+#define YFV2_JPEG_SRC_BAYER   5   /* f.bayer: the region lies in its window, (x0, y0) relative to the window */
 #define YFV2_JPEG_ENC_TRANSFORM 1
 #define YFV2_JPEG_ENC_SCAN      2
 #define YFV2_JPEG_ENC_PACK      4
@@ -507,6 +533,7 @@ typedef struct yfv2_jpeg_enc_src {
         yfv2_strided_frame strided;
         yfv2_yuv420_frame yuv420;
         yfv2_yuv422_frame yuv422;
+        yfv2_bayer_frame bayer;
     } f;                     /* the frame, in device memory */
     const int* params;       /* host: nparams ints, cv2.imencode's (IMWRITE_*, value) pairs; may be NULL with nparams 0 */
     int nparams;

@@ -15,11 +15,12 @@ batch: frames that start on the host are bound by that copy (about 6.2 MB per fr
 
 --layout nv12 | i420 feeds the steps YUV 4:2:0 frames of the same size (cv2's single [h*3/2, w] buffer) through
 yfv2_resize_yuv420_u8 instead; --layout rgb | bgra | rgba | gray | rgb_chw feeds contiguous frames of that layout through
-yfv2_resize_strided_u8, and --layout yuyv | uyvy | yvyu packed 4:2:2 frames through yfv2_resize_yuv422_u8.  Each run then also
-times the BGR resize of the same frame size (bgr_resize_us), alternated launch by launch with the layout's resize, each after an
-L2 flush; the touched bytes count the sectors of the rows (and planes) the layout's resize reads; `h2d_ms_per_batch` is the pinned
-copy of a batch in that layout next to `h2d_bgr_ms_per_batch`; and the parity check runs tests/layout_oracle.py on frames 0 and
-N-1."""
+yfv2_resize_strided_u8, --layout yuyv | uyvy | yvyu packed 4:2:2 frames through yfv2_resize_yuv422_u8, and --layout
+bayer_bg | bayer_gb | bayer_rg | bayer_gr (and their _ea edge-aware variants) raw [h, w] Bayer frames through
+yfv2_resize_bayer_u8.  Each run then also times the BGR resize of the same frame size (bgr_resize_us), alternated launch
+by launch with the layout's resize, each after an L2 flush; the touched bytes count the sectors of the rows (and planes) the
+layout's resize reads; `h2d_ms_per_batch` is the pinned copy of a batch in that layout next to `h2d_bgr_ms_per_batch`; and the
+parity check runs tests/layout_oracle.py (for Bayer tests/bayer_oracle.py) on frames 0 and N-1."""
 import argparse
 import ctypes
 import json
@@ -87,6 +88,33 @@ def touched_bytes_layout(h, w, H, W, layout):
     return 32 * len(np.unique(np.concatenate([a.reshape(-1) for a in addr]) // 32)) + 3 * H * W
 
 
+def touched_bytes_bayer(h, w, H, W):
+    """The same count for one contiguous raw Bayer frame: the sectors of the 3 x 4 raw windows (rows R - 1 .. R + 1, columns
+    C0 - 1 .. C1 + 1 around the clamped interior pixels) the kernel reads for each output pixel, plus the bytes it writes."""
+    from oracle import resize as ore
+    sx, _, _ = ore.coeffs(w, W, True)
+    sy, _, _ = ore.coeffs(h, H, False)
+    if h < 3 or w < 3:
+        return 3 * H * W
+    cols = np.clip(np.unique(np.concatenate([sx, np.minimum(sx + 1, w - 1)])), 1, w - 2)
+    rows = np.clip(np.unique(np.clip(np.concatenate([sy, sy + 1]), 0, h - 1)), 1, h - 2)
+    cols = np.unique((cols[:, None] + np.arange(-1, 2)[None, :]).reshape(-1))
+    rows = np.unique((rows[:, None] + np.arange(-1, 2)[None, :]).reshape(-1))
+    return 32 * len(np.unique((rows[:, None] * w + cols[None, :]).reshape(-1) // 32)) + 3 * H * W
+
+
+def bayer_descs(fb, layout):
+    """Descriptors of a [N, h, w] batch of contiguous raw Bayer frames, each converted whole."""
+    import yfv2_engine as eng
+    N, h, w = fb.shape
+    red_x, red_y = eng._BAYER_RED[layout[6:8]]
+    d = (eng.BayerFrame * N)()
+    for i in range(N):
+        d[i].data, d[i].pitch, d[i].fw, d[i].fh, d[i].x0, d[i].y0, d[i].w, d[i].h = fb[i].data_ptr(), w, w, h, 0, 0, w, h
+        d[i].red_x, d[i].red_y, d[i].edge_aware = red_x, red_y, layout.endswith("_ea")
+    return d
+
+
 def layout_descs(fb, layout):
     """Descriptors of a [N, ...] batch of contiguous frames of a strided or packed 4:2:2 layout, and the entry that takes them."""
     import yfv2_engine as eng
@@ -147,7 +175,9 @@ def main():
     ap.add_argument("--frame", default="1920x1080", help="source frame WxH")
     ap.add_argument("--runs", type=int, default=2, help="measurement runs, alternated within one process")
     ap.add_argument("--layout", default="bgr", choices=("bgr", "nv12", "i420", "rgb", "bgra", "rgba", "gray", "rgb_chw", "yuyv",
-                                                        "uyvy", "yvyu"), help="source frame format")
+                                                        "uyvy", "yvyu", "bayer_bg", "bayer_gb", "bayer_rg", "bayer_gr",
+                                                        "bayer_bg_ea", "bayer_gb_ea", "bayer_rg_ea", "bayer_gr_ea"),
+                    help="source frame format")
     args = ap.parse_args()
     import yfv2  # noqa: F401
     import yfv2_engine as eng
@@ -175,14 +205,19 @@ def main():
         descs.append(d)
     other = args.layout != "bgr"
     yuv420 = args.layout in ("nv12", "i420")
+    bayer = args.layout in eng.BAYER_LAYOUTS
     if other:
+        import bayer_oracle as bo
         import layout_cases as lc
         import layout_oracle as lo
-        shape = (fh * 3 // 2, fw) if yuv420 else lc.frame_shape(args.layout, fh, fw)
+        shape = (fh * 3 // 2, fw) if yuv420 else (fh, fw) if bayer else lc.frame_shape(args.layout, fh, fw)
         yframes = [torch.randint(0, 256, (N,) + shape, generator=g, dtype=torch.uint8, device=dev) for _ in range(2)]
         if yuv420:
             ydescs = [yuv420_descs(fb, args.layout) for fb in yframes]
             yentry = L.yfv2_resize_yuv420_u8
+        elif bayer:
+            ydescs = [bayer_descs(fb, args.layout) for fb in yframes]
+            yentry = L.yfv2_resize_bayer_u8
         else:
             ydescs = [layout_descs(fb, args.layout)[0] for fb in yframes]
             yentry = layout_descs(yframes[0][:1], args.layout)[1]
@@ -226,7 +261,8 @@ def main():
     last = (yframes if other else frames)[(it[0] - 1) % 2]
     for i in (0, N - 1):
         src = last[i].cpu().numpy()
-        want = lo.resize_planar(src, args.layout, S, S) if other else ore.resize_bgr_planar(src, S, S)
+        want = (bo.resize_planar(src, args.layout, S, S) if bayer else lo.resize_planar(src, args.layout, S, S) if other
+                else ore.resize_bgr_planar(src, S, S))
         if not np.array_equal(x[i].cpu().numpy(), want):
             raise AssertionError("bench_frames parity: resized frame %d differs from the oracle" % i)
 
@@ -234,6 +270,7 @@ def main():
     per_frame = touched_bytes(fh, fw, S, S, frames[0][0].stride(0))
     if other:
         per_frame_bgr, per_frame = per_frame, (touched_bytes_yuv420(fh, fw, S, S, args.layout) if yuv420 else
+                                               touched_bytes_bayer(fh, fw, S, S) if bayer else
                                                touched_bytes_layout(fh, fw, S, S, args.layout))
     peak, peak_src = bench.measured_peak()
     sampler = bench.ClockSampler(0)
@@ -295,7 +332,8 @@ def main():
                      "timing": line["timing"] + "; bgr_resize_us: the BGR resize of the same frame size, alternated with it",
                      "h2d_note": "one pinned host->device copy of %d %s frames (%.1f MB); h2d_bgr_ms_per_batch: the same frames as BGR "
                                  "(%.1f MB)" % (N, args.layout.upper(), N * frame_bytes / 1e6, N * fh * fw * 3 / 1e6),
-                     "parity": "resized frames 0 and %d equal the oracle (tests/layout_oracle.py) byte for byte" % (N - 1)})
+                     "parity": "resized frames 0 and %d equal the oracle (tests/%s) byte for byte"
+                               % (N - 1, "bayer_oracle.py" if bayer else "layout_oracle.py")})
     print(json.dumps(line), flush=True)
 
 

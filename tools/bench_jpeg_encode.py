@@ -1,7 +1,8 @@
 """Device time of the JPEG encode (yfv2_jpeg_encode) per call, split by stage, against cv2.imencode in host threads.
   python tools/bench_jpeg_encode.py [--n 256] [--reps 20] [--out FILE]
-Cases: N full-HD BGR frames and N full-HD NV12 frames at quality 95, 4:2:0 (smooth seeded content, so the files are photo-sized),
-and N detection crops of assorted sizes from those frames.  Each stage is timed with CUDA events over `reps` calls, the stages
+Cases: N full-HD BGR frames, N full-HD NV12 frames and N full-HD raw Bayer frames (RGGB, "bayer_bg", bilinear and edge-aware: the
+mosaic of the BGR frames) at quality 95, 4:2:0 (smooth seeded content, so the files are photo-sized), and N detection crops of
+assorted sizes from the BGR frames.  Each stage is timed with CUDA events over `reps` calls, the stages
 alternated within every repetition; medians are printed with the card's name, power limit and SM clock limit."""
 import argparse
 import json
@@ -130,6 +131,16 @@ def main():
     c = Call([yuv[i % 4] for i in range(a.n)], "nv12")
     res["nv12_1080p_ms"] = time_call(c, a.reps)
     del c
+    raw = []
+    for f in bgr[:4]:                                  # RGGB: R at (even, even), B at (odd, odd), G elsewhere
+        m = f[..., 1].copy()
+        m[0::2, 0::2], m[1::2, 1::2] = f[0::2, 0::2, 2], f[1::2, 1::2, 0]
+        raw.append(torch.from_numpy(m).cuda())
+    for layout in ("bayer_bg", "bayer_bg_ea"):
+        c = Call([raw[i % 4] for i in range(a.n)], layout)
+        res[layout + "_1080p_ms"] = time_call(c, a.reps)
+        res[layout + "_1080p_bytes_per_file"] = float(c.lengths.float().mean())
+        del c
     rng = np.random.RandomState(1)
     regions = []
     for k in range(a.n):

@@ -43,6 +43,7 @@ struct alignas(16) EncImage {
         yfv2_strided_frame strided;
         yfv2_yuv420_frame yuv420;
         yfv2_yuv422_frame yuv422;
+        yfv2_bayer_frame bayer;
     } f;
 };
 
@@ -241,6 +242,7 @@ const char* check_frame(const yfv2_jpeg_enc_src& s, int& fw, int& fh) {
             return fault(s.f.strided, frame_fault(s.f.strided, s.kind == YFV2_JPEG_SRC_GRAY));
         case YFV2_JPEG_SRC_YUV420: return fault(s.f.yuv420, frame_fault(s.f.yuv420));
         case YFV2_JPEG_SRC_YUV422: return fault(s.f.yuv422, frame_fault(s.f.yuv422));
+        case YFV2_JPEG_SRC_BAYER: return fault(s.f.bayer, frame_fault(s.f.bayer));
         default: fw = fh = 0; return "unknown kind";
     }
 }
@@ -273,6 +275,7 @@ __device__ __forceinline__ int enc_sample(const EncImage& im, int c, int i, int 
         case YFV2_JPEG_SRC_BGR: return comp_sample(FramePx<BgrSource>{im.f.bgr, im.x0, im.y0}, im.g, c, i, j);
         case YFV2_JPEG_SRC_YUV420: return comp_sample(FramePx<Yuv420Source>{im.f.yuv420, im.x0, im.y0}, im.g, c, i, j);
         case YFV2_JPEG_SRC_YUV422: return comp_sample(FramePx<Yuv422Source>{im.f.yuv422, im.x0, im.y0}, im.g, c, i, j);
+        case YFV2_JPEG_SRC_BAYER: return comp_sample(FramePx<BayerSource>{im.f.bayer, im.x0, im.y0}, im.g, c, i, j);
         default: return comp_sample(FramePx<StridedSource>{im.f.strided, im.x0, im.y0}, im.g, c, i, j);
     }
 }

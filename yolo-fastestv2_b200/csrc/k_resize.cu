@@ -9,7 +9,9 @@
 //   fixed point, limited range, chroma not interpolated; (U, V) is the sample of the pixel's 2x2 block for 4:2:0, of its
 //   two-pixel macropixel for 4:2:2):
 //     uu = U - 128, vv = V - 128, y = max(0, Y[r][c] - 16) * 1220542 + (1 << 19)
-//     B = sat_u8((y + 2116026 uu) >> 20), G = sat_u8((y - 852492 vv - 409993 uu) >> 20), R = sat_u8((y + 1673527 vv) >> 20).
+//     B = sat_u8((y + 2116026 uu) >> 20), G = sat_u8((y - 852492 vv - 409993 uu) >> 20), R = sat_u8((y + 1673527 vv) >> 20);
+//   raw Bayer frames (yfv2_resize_bayer_u8), each source pixel demosaiced as cv2.cvtColor(COLOR_Bayer??2BGR / _EA) does, in
+//   integers on the 3x3 raw neighbourhood of its clamped frame coordinate (resize.cuh's BayerSource, tests/bayer_oracle.py).
 // The resize is bit-identical to OpenCV's x86 8-bit path, all integer after the coefficients:
 //   coefficients per axis: f = fl32((d + 0.5) * (n / m) - 0.5) (product and difference rounded in double), s = floor(f),
 //     f = fl32(f - s); weights rint(fl32(1 - f) * 2048), rint(f * 2048).  Along x, s < 0 -> (0, 0) then s >= w - 1 -> (w - 1, 0);
@@ -221,6 +223,10 @@ extern "C" int yfv2_resize_strided_u8(const yfv2_strided_frame* frames, int N, i
 
 extern "C" int yfv2_resize_yuv422_u8(const yfv2_yuv422_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
     return yfv2::resize_entry<yfv2::Yuv422Source>("resize_yuv422_u8", frames, N, H, W, dst, stream);
+}
+
+extern "C" int yfv2_resize_bayer_u8(const yfv2_bayer_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
+    return yfv2::resize_entry<yfv2::BayerSource>("resize_bayer_u8", frames, N, H, W, dst, stream);
 }
 
 namespace yfv2 {

@@ -1,8 +1,8 @@
 // cv2.resize(INTER_LINEAR)'s per-pixel arithmetic (k_resize.cu states it): the coefficients of one target index and one output
 // pixel computed over any source type with a fetch(c0, c1, p0, p1) of two pixels of a row.  k_resize.cu's kernels and k_jpeg.cu's
-// fused decode + resize (JpegSource) share it.  The frame fetches (BGR, strided, YUV 4:2:0, packed YUV 4:2:2: cv2.cvtColor's BGR
-// bytes of any layout) are here too, shared by k_resize.cu and the JPEG encoder (k_jpeg_enc.cu), with the host checks of their
-// descriptors.
+// fused decode + resize (JpegSource) share it.  The frame fetches (BGR, strided, YUV 4:2:0, packed YUV 4:2:2, raw Bayer:
+// cv2.cvtColor's BGR bytes of any layout) are here too, shared by k_resize.cu and the JPEG encoder (k_jpeg_enc.cu), with the host
+// checks of their descriptors.
 #pragma once
 #include <climits>
 #include <stdint.h>
@@ -39,6 +39,16 @@ inline const char* frame_fault(const yfv2_yuv422_frame& f) {
     if (!f.y || !f.u || !f.v) return "null plane pointer";
     if (f.w <= 0 || f.h <= 0 || (f.w & 1)) return "w must be even and > 0, h > 0";
     if (f.pitch < 2LL * f.w) return "pitch < 2 * w";
+    return nullptr;
+}
+inline const char* frame_fault(const yfv2_bayer_frame& f) {
+    if (!f.data) return "null data";
+    if (f.fw < 1 || f.fh < 1) return "fw and fh must be >= 1";
+    if (f.pitch < f.fw) return "pitch < fw";
+    if (f.w < 1 || f.h < 1 || f.x0 < 0 || f.y0 < 0 || (long long)f.x0 + f.w > f.fw || (long long)f.y0 + f.h > f.fh)
+        return "window empty or outside the frame";
+    if ((f.red_x | f.red_y) & ~1) return "red_x and red_y must be 0 or 1";
+    if (f.edge_aware & ~1) return "edge_aware must be 0 or 1";
     return nullptr;
 }
 
@@ -136,6 +146,65 @@ struct Yuv422Source {
         if (k1 != k0) { u1 = __ldg(u + k1) - 128; v1 = __ldg(v + k1) - 128; }   // c0, c1 in different macropixels
         yuv_to_bgr(__ldg(luma + 2 * c0), u0, v0, p0);
         yuv_to_bgr(__ldg(luma + 2 * c1), u1, v1, p1);
+    }
+};
+
+// cv2.cvtColor's COLOR_Bayer??2BGR (_EA) of one interior pixel from its 3x3 raw neighbourhood (row-major: up, centre, down),
+// into B, G, R.  red_row / red_col: the pixel's row / column holds red sites; both or neither: an R or B site, else a G site.
+__device__ __forceinline__ void demosaic(int ul, int u, int ur, int l, int c, int r, int dl, int d, int dr, bool red_row,
+                                         bool red_col, bool ea, int (&p)[3]) {
+    const int hor = (l + r + 1) >> 1, ver = (u + d + 1) >> 1;
+    if (red_row == red_col) {
+        const int diag = (ul + ur + dl + dr + 2) >> 2;
+        p[1] = ea ? (abs(l - r) <= abs(u - d) ? hor : ver) : (u + d + l + r + 2) >> 2;
+        p[0] = red_row ? diag : c;
+        p[2] = red_row ? c : diag;
+    } else {
+        p[1] = c;
+        p[0] = red_row ? ver : hor;
+        p[2] = red_row ? hor : ver;
+    }
+}
+
+// Raw Bayer: the window (x0, y0, w, h) of cv2.cvtColor(raw, COLOR_Bayer??2BGR / _EA) of the whole fw x fh frame.  Pixel (r, c) of
+// the window is demosaiced where it is read, at the frame's interior pixel (clamp(y0 + r, 1, fh - 2), clamp(x0 + c, 1, fw - 2));
+// frames under 3 pixels on a side are zeros.  The pattern (red_x, red_y) and the method are descriptor values, so nothing here
+// branches on the layout.  The two columns of a fetch are adjacent or equal after the clamp, so they share one 3 x 4 raw window.
+struct BayerSource {
+    using Desc = yfv2_bayer_frame;
+    static constexpr int kChunk = 64;    // 56-byte descriptors: 3.5 KB of kernel parameters, under the 4 KB launch limit
+    static constexpr int kMinBlocks = 0;
+    const yfv2_bayer_frame& f;           // the rest is read from the descriptor where it is used: no registers held across fetches
+    const uint8_t* mid;                  // the clamped row
+    bool red_row;
+    __device__ __forceinline__ BayerSource(const yfv2_bayer_frame& f_, int r) : f(f_) {
+        const int R = min(max(f.y0 + r, 1), f.fh - 2);
+        mid = f.data + (long long)R * f.pitch;
+        red_row = ((R ^ f.red_y) & 1) == 0;
+    }
+    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
+        if (f.fw < 3 || f.fh < 3) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) p0[c] = p1[c] = 0;
+            return;
+        }
+        const int C0 = min(max(f.x0 + c0, 1), f.fw - 2), C1 = min(max(f.x0 + c1, 1), f.fw - 2);
+        const bool d = C1 != C0;                                  // C1 == C0 + 1
+        const bool ea = f.edge_aware;
+        int a[3][4];                                              // raw columns C0 - 1 .. C0 + 1, C1 + 1 of rows R - 1 .. R + 1
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            const uint8_t* row = mid + (k - 1) * f.pitch + C0;
+            a[k][0] = __ldg(row - 1); a[k][1] = __ldg(row); a[k][2] = __ldg(row + 1); a[k][3] = __ldg(row + d + 1);
+        }
+        const bool red_col0 = ((C0 ^ f.red_x) & 1) == 0;
+        demosaic(a[0][0], a[0][1], a[0][2], a[1][0], a[1][1], a[1][2], a[2][0], a[2][1], a[2][2], red_row, red_col0, ea, p0);
+        int b[3][3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+#pragma unroll
+            for (int j = 0; j < 3; ++j) b[k][j] = d ? a[k][j + 1] : a[k][j];
+        demosaic(b[0][0], b[0][1], b[0][2], b[1][0], b[1][1], b[1][2], b[2][0], b[2][1], b[2][2], red_row, red_col0 != d, ea, p1);
     }
 };
 

@@ -3,9 +3,9 @@
 The reference resizes each frame on the host with cv2.resize (test.py:35), runs the network on the resized batch and scales the
 boxes back to the frame with scale_w = w / cfg["width"], scale_h = h / cfg["height"] (test.py:57-68).  Here the resize runs on
 the device (resize_bgr: yfv2_resize_bgr_u8, bit-identical to cv2's INTER_LINEAR bytes; resize_yuv420: yfv2_resize_yuv420_u8, the
-same after cv2.cvtColor(COLOR_YUV2BGR_*); resize_frames: every layout, RGB, BGRA / RGBA, grey, planar RGB and packed YUV 4:2:2
-included, the same after the cv2.cvtColor that brings it to BGR), followed by the uint8 forward and the fused decode + NMS; only
-the scale-back of at most 300 rows per frame stays on the host, in float64 like test.py's Python floats.
+same after cv2.cvtColor(COLOR_YUV2BGR_*); resize_frames: every layout, RGB, BGRA / RGBA, grey, planar RGB, packed YUV 4:2:2
+and raw Bayer included, the same after the cv2.cvtColor that brings it to BGR), followed by the uint8 forward and the fused
+decode + NMS; only the scale-back of at most 300 rows per frame stays on the host, in float64 like test.py's Python floats.
 
 detect_regions / detect_tiled look at each frame through several regions (tiles, zones): every region is cropped in place,
 stretched to the network input and detected on like a frame, and yfv2_merge_regions maps the rows of all regions back to frame
@@ -43,10 +43,11 @@ def _yuv420_size(f):
 def detect_frames(model, frames, cfg, conf_thres=0.3, iou_thres=0.4, layout="bgr"):
     """Raw frames -> detections in each frame's own pixels: a list of float64 CPU [n_i, 6] tensors (x1, y1, x2, y2, conf, cls),
     descending conf.  model: an eval-mode Detector on a CUDA device; cfg: the load_datafile dict (width, height, anchors).
-    layout: one of yfv2_engine.LAYOUTS, or a list with one per frame; the frames are what resize_frames takes for it ("bgr": HWC
-    uint8 numpy arrays or CUDA tensors of any sizes; "nv12" | "nv21" | "i420" | "yv12": cv2's single [h*3/2, w] buffer or a tuple
-    of planes; "rgb", "bgra" / "rgba", "gray", "rgb_chw" [3, h, w], "yuyv" / "uyvy" / "yvyu" [h, w, 2]), converted as
-    cv2.cvtColor(COLOR_<LAYOUT>2BGR) does.  The boxes come back in pixels of each frame's h x w (the luma plane for YUV)."""
+    layout: one of yfv2_engine.LAYOUTS or BAYER_LAYOUTS, or a list with one per frame; the frames are what resize_frames takes for
+    it ("bgr": HWC uint8 numpy arrays or CUDA tensors of any sizes; "nv12" | "nv21" | "i420" | "yv12": cv2's single [h*3/2, w]
+    buffer or a tuple of planes; "rgb", "bgra" / "rgba", "gray", "rgb_chw" [3, h, w], "yuyv" / "uyvy" / "yvyu" [h, w, 2]; the
+    Bayer layouts [h, w] raw frames or a BayerWindow of one), converted as cv2.cvtColor(COLOR_<LAYOUT>2BGR) does.  The boxes
+    come back in pixels of each frame's h x w (the luma plane for YUV, the window for a BayerWindow)."""
     frames = list(frames)
     layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
     x = resize_frames(frames, cfg["width"], cfg["height"], layouts, next(model.parameters()).device)
@@ -106,7 +107,8 @@ def tile_regions(w, h, cols, rows, overlap=0.2, full_frame=True, layout="bgr"):
     """A cols x rows grid of overlapping tiles of a w x h frame, as a list of (x0, y0, tw, th), row by row.
     tw = ceil(w / (cols - (cols - 1) * overlap)), at most w (th likewise), and tile k starts at floor(k * (w - tw) / (cols - 1)), so
     the last tile ends on the frame's edge and adjacent tiles overlap by at least overlap * tw - 2 pixels.  For the 4:2:0 layouts
-    origins are rounded down and sizes up to even numbers on both axes, for packed 4:2:2 along x only (what crop_frame needs).
+    origins are rounded down and sizes up to even numbers on both axes, for packed 4:2:2 along x only (what crop_frame needs);
+    Bayer windows are not rounded (crop_frame keeps the whole raw frame, so any offset converts as cv2 does).
     full_frame: the whole frame comes first, as one more region for objects larger than a tile (first, it wins ties of conf).
     Each tile is stretched to the network input like a whole frame."""
     cols, rows, w, h = int(cols), int(rows), int(w), int(h)
@@ -170,7 +172,9 @@ def detect_regions(model, frames, cfg, regions, conf_thres=0.3, iou_thres=0.4, l
 
 
 def _on_device(f, layout, dev):
-    """A frame (or tuple of planes) as CUDA tensors on `dev`: host arrays copied once, CUDA tensors as they are."""
+    """A frame (or tuple of planes, or BayerWindow) as CUDA tensors on `dev`: host arrays copied once, CUDA tensors as they are."""
+    if isinstance(f, yfv2_engine.BayerWindow):
+        return yfv2_engine.BayerWindow(_on_device(f.raw, layout, dev), f.x0, f.y0, f.w, f.h)
     if isinstance(f, (tuple, list)):
         return tuple(_on_device(p, layout, dev) for p in f)
     if not isinstance(f, torch.Tensor):

@@ -48,8 +48,16 @@ class Yuv422Frame(ctypes.Structure):
                 ("w", ctypes.c_int), ("h", ctypes.c_int)]
 
 
+class BayerFrame(ctypes.Structure):
+    """yfv2_bayer_frame: the window (x0, y0, w, h) of the demosaic of a whole raw Bayer frame in device memory."""
+    _fields_ = [("data", ctypes.c_void_p), ("pitch", ctypes.c_longlong), ("fw", ctypes.c_int), ("fh", ctypes.c_int),
+                ("x0", ctypes.c_int), ("y0", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int), ("red_x", ctypes.c_int),
+                ("red_y", ctypes.c_int), ("edge_aware", ctypes.c_int)]
+
+
 class _EncFrame(ctypes.Union):
-    _fields_ = [("bgr", Frame), ("strided", StridedFrame), ("yuv420", Yuv420Frame), ("yuv422", Yuv422Frame)]
+    _fields_ = [("bgr", Frame), ("strided", StridedFrame), ("yuv420", Yuv420Frame), ("yuv422", Yuv422Frame),
+                ("bayer", BayerFrame)]
 
 
 class JpegEncSrc(ctypes.Structure):
@@ -58,7 +66,8 @@ class JpegEncSrc(ctypes.Structure):
                 ("f", _EncFrame), ("params", ctypes.POINTER(ctypes.c_int)), ("nparams", ctypes.c_int)]
 
 
-JPEG_SRC_BGR, JPEG_SRC_STRIDED, JPEG_SRC_GRAY, JPEG_SRC_YUV420, JPEG_SRC_YUV422 = range(5)   # JpegEncSrc.kind (YFV2_JPEG_SRC_*)
+# JpegEncSrc.kind (YFV2_JPEG_SRC_*)
+JPEG_SRC_BGR, JPEG_SRC_STRIDED, JPEG_SRC_GRAY, JPEG_SRC_YUV420, JPEG_SRC_YUV422, JPEG_SRC_BAYER = range(6)
 
 
 class TrainerOp(ctypes.Structure):
@@ -319,6 +328,8 @@ PROTOTYPES = {
                                               ctypes.c_void_p, ctypes.c_void_p]),
     "yfv2_resize_yuv422_u8": (ctypes.c_int, [ctypes.POINTER(Yuv422Frame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                              ctypes.c_void_p]),
+    "yfv2_resize_bayer_u8": (ctypes.c_int, [ctypes.POINTER(BayerFrame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                            ctypes.c_void_p]),
     "yfv2_detect_u8_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                            ctypes.POINTER(ctypes.c_double), ctypes.c_float, ctypes.c_double, ctypes.c_int,
                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
@@ -1304,16 +1315,38 @@ _YUV422_OFFSETS = {"yuyv": (0, 1, 3), "uyvy": (1, 0, 2), "yvyu": (0, 3, 1)}
 # bytes per pixel of each packed layout
 _CHANNELS = {"bgr": 3, "rgb": 3, "bgra": 4, "rgba": 4, "gray": 1, "yuyv": 2, "uyvy": 2, "yvyu": 2}
 LAYOUTS = ("bgr",) + YUV420_LAYOUTS + STRIDED_LAYOUTS + YUV422_LAYOUTS
+# raw Bayer frames (yfv2_resize_bayer_u8): "bayer_<xy>" is cv2's COLOR_Bayer<XY>2BGR, "bayer_<xy>_ea" its edge-aware
+# COLOR_Bayer<XY>2BGR_EA; _BAYER_RED holds the column and row parity of the red sites of each pattern
+_BAYER_RED = {"bg": (0, 0), "gb": (1, 0), "rg": (1, 1), "gr": (0, 1)}
+BAYER_LAYOUTS = tuple("bayer_" + k for k in _BAYER_RED) + tuple("bayer_%s_ea" % k for k in _BAYER_RED)
+_FRAME_LAYOUTS = LAYOUTS + BAYER_LAYOUTS          # every layout resize_frames, encode_jpeg and crop_frame take
 # the descriptor kind (yfv2_jpeg_enc_src.kind) of each layout, and the union member of yfv2_jpeg_enc_src.f each kind fills: the
 # resize entry yfv2_resize_<member>_u8 takes an array of it
 _KIND = dict([("bgr", JPEG_SRC_BGR), ("gray", JPEG_SRC_GRAY)] + [(k, JPEG_SRC_YUV420) for k in YUV420_LAYOUTS]
-             + [(k, JPEG_SRC_STRIDED) for k in STRIDED_LAYOUTS if k != "gray"] + [(k, JPEG_SRC_YUV422) for k in YUV422_LAYOUTS])
-_MEMBER = ("bgr", "strided", "strided", "yuv420", "yuv422")
+             + [(k, JPEG_SRC_STRIDED) for k in STRIDED_LAYOUTS if k != "gray"] + [(k, JPEG_SRC_YUV422) for k in YUV422_LAYOUTS]
+             + [(k, JPEG_SRC_BAYER) for k in BAYER_LAYOUTS])
+_MEMBER = ("bgr", "strided", "strided", "yuv420", "yuv422", "bayer")
 _DESC = dict(_EncFrame._fields_)
 
 
+class BayerWindow:
+    """The w x h window at (x0, y0) of cv2.cvtColor(raw, COLOR_Bayer??2BGR) of a whole raw Bayer frame: what crop_frame returns for
+    the Bayer layouts, and what resize_frames, encode_jpeg, frame_size and crop_frame take for them besides whole frames.  raw is
+    the whole [fh, fw] uint8 frame (numpy or CUDA), never copied.  The demosaic of a pixel reads its neighbours and the frame's
+    edges, so the window cannot be a crop of the raw bytes."""
+    __slots__ = ("raw", "x0", "y0", "w", "h")
+
+    def __init__(self, raw, x0, y0, w, h):
+        self.raw, self.x0, self.y0, self.w, self.h = raw, int(x0), int(y0), int(w), int(h)
+
+    def __repr__(self):
+        return "BayerWindow(raw %s, x0 %d, y0 %d, %dx%d)" % (tuple(self.raw.shape), self.x0, self.y0, self.w, self.h)
+
+
 def frame_size(frame, layout):
-    """(h, w) in pixels of a frame in the given layout, as resize_frames takes it."""
+    """(h, w) in pixels of a frame in the given layout, as resize_frames takes it (of its window for a BayerWindow)."""
+    if isinstance(frame, BayerWindow):
+        return frame.h, frame.w
     if layout in YUV420_LAYOUTS:
         if isinstance(frame, (tuple, list)):
             return tuple(frame[0].shape[:2])
@@ -1343,11 +1376,29 @@ def _layout_frame(f, layout, i, fn):
     return f
 
 
+def _bayer_window(f, layout, i, fn):
+    """Frame i of a Bayer layout, a whole [fh, fw] uint8 frame or a BayerWindow, as a BayerWindow over a uint8 2-D tensor, checked,
+    not copied."""
+    win = f if isinstance(f, BayerWindow) else None
+    raw = _uint8_plane(win.raw if win else f, "frame %d (%s)" % (i, layout), fn)
+    fh, fw = raw.shape
+    if fh < 1 or fw < 1:
+        raise Yfv2Error("%s: frame %d (%s) must be uint8 [h, w] with h, w > 0, got %s" % (fn, i, layout, tuple(raw.shape)))
+    if win is None:
+        return BayerWindow(raw, 0, 0, fw, fh)
+    if win.w < 1 or win.h < 1 or win.x0 < 0 or win.y0 < 0 or win.x0 + win.w > fw or win.y0 + win.h > fh:
+        raise Yfv2Error("%s: frame %d (%s): window (x0 %d, y0 %d, %dx%d) is not inside the %dx%d frame"
+                        % (fn, i, layout, win.x0, win.y0, win.w, win.h, fw, fh))
+    return BayerWindow(raw, win.x0, win.y0, win.w, win.h)
+
+
 def _check_frame(f, layout, i, fn):
     """Checks frame i against its layout without copying or launching anything; returns what _describe takes: the BGR array or
-    tensor, the planes of a 4:2:0 frame, a uint8 tensor of the layout's shape for the others.  A refusal names fn, the public
-    function called."""
+    tensor, the planes of a 4:2:0 frame, a BayerWindow over a tensor for Bayer, a uint8 tensor of the layout's shape for the
+    others.  A refusal names fn, the public function called."""
     kind = _KIND[layout]
+    if kind == JPEG_SRC_BAYER:
+        return _bayer_window(f, layout, i, fn)
     if kind == JPEG_SRC_BGR:
         if isinstance(f, torch.Tensor):
             ok = f.dtype == torch.uint8
@@ -1362,7 +1413,7 @@ def _check_frame(f, layout, i, fn):
     return _layout_frame(f, layout, i, fn)
 
 
-def _checked_frames(fn, frames, layout, allowed=LAYOUTS):
+def _checked_frames(fn, frames, layout, allowed=_FRAME_LAYOUTS):
     """The frames as a list, each checked (_check_frame), and one layout name per frame from `layout` (one name, or one per frame),
     each among `allowed`."""
     frames = list(frames)
@@ -1381,7 +1432,8 @@ def _device(fn, frames, device):
     """The CUDA device a call runs on, with its index: `device`, else that of the first CUDA tensor among the checked frames (or
     their planes), else the current one."""
     if device is None:
-        device = next((t.device for f in frames for t in (f if isinstance(f, tuple) else (f,))
+        device = next((t.device for f in frames
+                       for t in (f if isinstance(f, tuple) else (f.raw,) if isinstance(f, BayerWindow) else (f,))
                        if isinstance(t, torch.Tensor) and t.is_cuda), None)
     device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     if device.type != "cuda":
@@ -1406,6 +1458,20 @@ def _describe(f, layout, device, keep):
     tensors read go to keep, which must hold them until the launch is queued: a freed block could take the next frame's copy."""
     kind = _KIND[layout]
     s = JpegEncSrc(kind)
+    if kind == JPEG_SRC_BAYER:                                # the whole raw frame, any row stride, unit column stride
+        raw = f.raw.to(device)
+        fh, fw = raw.shape
+        if (fw > 1 and raw.stride(1) != 1) or (fh > 1 and raw.stride(0) < fw):
+            raw = raw.contiguous()
+        e = s.f.bayer
+        # torch keeps any stride on a dimension of size 1 (contiguous() too); one row has no next row, so its pitch is fw
+        e.data, e.pitch, e.fh, e.fw = raw.data_ptr(), raw.stride(0) if fh > 1 else fw, fh, fw
+        e.x0, e.y0, e.w, e.h = f.x0, f.y0, f.w, f.h
+        e.red_x, e.red_y = _BAYER_RED[layout[6:8]]
+        e.edge_aware = layout.endswith("_ea")
+        s.w, s.h = f.w, f.h
+        keep.append(raw)
+        return s
     if kind == JPEG_SRC_YUV420:
         planes = [p.to(device) for p in f]
         planes = [p if p.stride(1) == 1 else p.contiguous() for p in planes]
@@ -1489,11 +1555,13 @@ def resize_frames(frames, W, H, layout, device=None, out=None):
       "gray"                            [h, w], COLOR_GRAY2BGR
       "rgb_chw"                         [3, h, w] planar RGB (torchvision's decode_jpeg): transpose + COLOR_RGB2BGR
       "yuyv" | "uyvy" | "yvyu"          [h, w, 2] packed 4:2:2 (w even), COLOR_YUV2BGR_<LAYOUT>
+      "bayer_bg" | "bayer_gb"           [h, w] raw Bayer (BAYER_LAYOUTS), COLOR_Bayer<XY>2BGR; "bayer_<xy>_ea": _EA, the
+        | "bayer_rg" | "bayer_gr"       edge-aware demosaic; or a BayerWindow of one (crop_frame)
     Frames are numpy arrays or CUDA tensors; CUDA views with larger row strides or crop offsets are read in place (for
     "rgb_chw" any channel and row stride with unit column stride), host arrays are copied to `device`.  Consecutive frames of
-    one descriptor kind go to one call (yfv2_resize_bgr_u8 / _yuv420_u8 / _strided_u8 / _yuv422_u8), each into its slice of
-    `out`.  Every frame is checked before anything is copied or launched."""
-    return _resize("resize_frames", frames, layout, LAYOUTS, W, H, device, out)
+    one descriptor kind go to one call (yfv2_resize_bgr_u8 / _yuv420_u8 / _strided_u8 / _yuv422_u8 / _bayer_u8), each into its
+    slice of `out`.  Every frame is checked before anything is copied or launched."""
+    return _resize("resize_frames", frames, layout, _FRAME_LAYOUTS, W, H, device, out)
 
 
 # cv2's IMWRITE_* ids and IMWRITE_JPEG_SAMPLING_FACTOR_* values (yfv2_jpeg_encode_plan reads the same pairs)
@@ -1515,10 +1583,10 @@ def encode_jpeg(frames, quality=95, sampling="420", restart_interval=0, layout="
     (yfv2_jpeg_encode).  img is cv2.cvtColor(frame, COLOR_<LAYOUT>2BGR) for any layout of resize_frames (one name, or one per
     frame); "gray" frames give one-component JPEGs, as cv2 does for a 2-D array.  regions: None (one output per frame, the whole
     frame), or a list of (frame index, x0, y0, w, h), one output each, cropped from the converted frame (several may share a
-    frame).  quality (any int, clamped to 0..100 as cv2 does), sampling ("420", "422", "444") and restart_interval (MCUs, 0: none)
-    are one value or one per output; params: extra cv2 (IMWRITE_*, value) pairs for every output, or a list of them per output.
-    Everything is checked before anything is launched; a refusal raises Yfv2Error naming the output.  Returns a list of bytes, or
-    with device_out=True (arena, offsets, lengths): the uint8 CUDA arena, output i at offsets[i] (host int64 numpy) and
+    frame; for a BayerWindow, from its window).  quality (any int, clamped to 0..100 as cv2 does), sampling ("420", "422",
+    "444") and restart_interval (MCUs, 0: none) are one value or one per output; params: extra cv2 (IMWRITE_*, value) pairs for
+    every output, or a list of them per output.  Everything is checked before anything is launched; a refusal raises Yfv2Error
+    naming the output.  Returns a list of bytes, or with device_out=True (arena, offsets, lengths): the uint8 CUDA arena, output i at offsets[i] (host int64 numpy) and
     lengths[i] bytes long (CUDA int64), with no copy to the host."""
     checked, layouts = _checked_frames("encode_jpeg", frames, layout)
     if regions is None:
@@ -1584,9 +1652,11 @@ def crop_frame(frame, layout, x0, y0, w, h):
     resize_frames of the crop gives the bytes of cv2.resize(cv2.cvtColor(frame, COLOR_<LAYOUT>2BGR)[y0:y0+h, x0:x0+w]).  HWC
     layouts and grey are sliced in place, "rgb_chw" as [3, h, w].  A 4:2:0 frame (a single [h*3/2, w] buffer or its planes)
     becomes a tuple of cropped planes, (y, uv) for NV12 / NV21 and (y, u, v) for I420 / YV12; x0, y0, w, h must then be even, so
-    that the 2x2 chroma blocks of the crop are those of the frame.  Packed 4:2:2 needs even x0 and w (whole macropixels)."""
-    if layout not in LAYOUTS:
-        raise Yfv2Error("crop_frame: layout must be one of %s, got %r" % (", ".join(LAYOUTS), layout))
+    that the 2x2 chroma blocks of the crop are those of the frame.  Packed 4:2:2 needs even x0 and w (whole macropixels).  A Bayer
+    frame, or a BayerWindow of one, becomes a BayerWindow of the whole raw frame (any offsets): the conversion of a pixel reads its
+    neighbours and the frame's edges, so the raw bytes are not cropped.  A crop of a crop is the crop of the frame."""
+    if layout not in _FRAME_LAYOUTS:
+        raise Yfv2Error("crop_frame: layout must be one of %s, got %r" % (", ".join(_FRAME_LAYOUTS), layout))
     f = _check_frame(frame, layout, 0, "crop_frame")
     fh, fw = frame_size(f, layout)
     x0, y0, w, h = int(x0), int(y0), int(w), int(h)
@@ -1603,6 +1673,8 @@ def crop_frame(frame, layout, x0, y0, w, h):
             return f[0][y0:y0 + h, x0:x0 + w], f[1][cy, x0:x0 + w]
         cx = slice(x0 // 2, (x0 + w) // 2)
         return f[0][y0:y0 + h, x0:x0 + w], f[1][cy, cx], f[2][cy, cx]
+    if layout in BAYER_LAYOUTS:
+        return BayerWindow(f.raw, f.x0 + x0, f.y0 + y0, w, h)
     if layout == "rgb_chw":
         return f[:, y0:y0 + h, x0:x0 + w]
     return f[y0:y0 + h, x0:x0 + w]
