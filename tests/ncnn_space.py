@@ -28,7 +28,7 @@ def pow2_at_least(m, lo=64):
 
 
 def smem_bytes(M):
-    """k_ncnn.cu smem_bytes(M, MCp): shared memory of one ncnn CTA for M candidate slots."""
+    """k_ncnn.cu ncnn_layout(s, nullptr, M, MCp): shared memory of one ncnn CTA for M candidate slots."""
     r16 = lambda b: (b + 15) & ~15  # noqa: E731
     b = pow2_at_least(M) * 8 + M * 16 + r16(M * 4) + r16(M * 2) * 2
     return b + CHUNK * 16 + CHUNK * 4 + r16(CHUNK * 2) + CHUNK * 8 + 32

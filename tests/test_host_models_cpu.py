@@ -4,7 +4,7 @@
    fold_head_kernel composes in fp64 into one [M x 72] matrix + bias.  Here the same composition is done with numpy on
    the oracle's tensors and pushed through the oracle: the folded head must reproduce the reference ordering
    (fpn.py DWConvblock tail + detector.py:17-19,35-41) to fp32 round-off.
-2. The NMS sort: k_post.cu's bitonic_sort_desc_reg keeps NT*E keys in registers and mixes in-thread compare-exchanges,
+2. The NMS sort: nms.cuh's bitonic_sort_desc_reg keeps NT*E keys in registers and mixes in-thread compare-exchanges,
    warp shuffles and a few shared-memory steps.  A numpy model of exactly those index / direction rules must sort, and
    every shuffle partner must sit in the same warp.
 """

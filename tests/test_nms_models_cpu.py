@@ -1,4 +1,4 @@
-"""CPU models of the reasoning behind three pieces of k_post.cu's suppression code (no GPU, no CUDA library calls).
+"""CPU models of the reasoning behind three pieces of the suppression code of k_post.cu and nms.cuh (no GPU, no CUDA library calls).
 
 1. iou_fast: a branch-free fp32 estimate decides an IoU test whenever it is not `amb`; the claim is that its answer then equals
    torchvision's `(double)(inter / (a + b - inter)) > thr` with fp32 arithmetic (utils/utils.py:286 -> torchvision.ops.nms).
@@ -97,7 +97,8 @@ def test_branch_free_iou_front_agrees_with_the_exact_test_whenever_it_decides():
 
 
 def _resolve_halves(alive, rows, room):
-    """sort_and_suppress (c): low 32 candidates first, a row's upper word applied to the upper live bits off the chain."""
+    """nms.cuh resolve_chunk (written out in sort_and_suppress (c)): low 32 candidates first, a row's upper word applied to the upper
+    live bits off the chain."""
     lo, hi = alive & 0xFFFFFFFF, alive >> 32
     klo = khi = 0
     while lo and room > 0:

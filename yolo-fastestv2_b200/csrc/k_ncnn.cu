@@ -10,22 +10,20 @@
 //
 // Input: the two [N,h,w,5A+C] tensors yfv2_export_heads writes (sigmoid reg | sigmoid obj | softmax cls, model/detector.py:33-44).
 // One CTA per image.  Candidates are scored a warp per cell (coalesced reads of the cell's 5A+C floats, shuffle arg-max with the
-// smaller class winning ties = the reference's strict '>' scan), keyed (score, push order) and sorted by a bitonic network in shared
-// memory, then suppressed in blocks of 64 sorted candidates: block vs everything kept so far, 64x64 pairs inside the block, a serial
-// resolve over bit masks.  Every floating-point step is the reference's operation with round-to-nearest intrinsics (no contraction).
+// smaller class winning ties = the reference's strict '>' scan), keyed (score, push order) and sorted by nms.cuh's bitonic networks,
+// then suppressed by its greedy_pass in blocks of 64 sorted candidates: block vs everything kept so far, 64x64 pairs inside the
+// block, an in-order resolve over bit masks.  Every floating-point step is the reference's operation with round-to-nearest
+// intrinsics (no contraction).
 // The reference sorts with std::sort (order among equal scores unspecified); ties here keep push order (level, row, column, anchor).
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
+#include "nms.cuh"
 
 namespace yfv2 {
 namespace {
-
-constexpr int NT = 256;
-constexpr int kMaxA = 8;
-constexpr int kChunk = 64;
 
 struct NcnnArgs {
     const float* out[2];
@@ -52,34 +50,19 @@ struct Smem {
     unsigned int* misc;         // [0] candidate count, [1..2] dead bits, [3..4] kept bits
 };
 
-__host__ __device__ inline size_t smem_bytes(int M, int MCp) {
-    size_t b = (size_t)MCp * 8 + (size_t)M * 16 + (((size_t)M * 4 + 15) & ~(size_t)15);
-    b += (((size_t)M * 2 + 15) & ~(size_t)15) * 2;
-    b += kChunk * 16 + kChunk * 4 + (((size_t)kChunk * 2 + 15) & ~(size_t)15) + kChunk * 8 + 32;
-    return b;
-}
-
-__device__ __forceinline__ Smem carve(unsigned char* p, int M, int MCp) {
-    Smem s;
-    s.keys = reinterpret_cast<unsigned long long*>(p); p += (size_t)MCp * 8;
-    s.box = reinterpret_cast<int4*>(p); p += (size_t)M * 16;
-    s.area = reinterpret_cast<float*>(p); p += (((size_t)M * 4 + 15) & ~(size_t)15);
-    s.cate = reinterpret_cast<short*>(p); p += (((size_t)M * 2 + 15) & ~(size_t)15);
-    s.picked = reinterpret_cast<unsigned short*>(p); p += (((size_t)M * 2 + 15) & ~(size_t)15);
-    s.chbox = reinterpret_cast<int4*>(p); p += kChunk * 16;
-    s.charea = reinterpret_cast<float*>(p); p += kChunk * 4;
-    s.chcate = reinterpret_cast<short*>(p); p += (((size_t)kChunk * 2 + 15) & ~(size_t)15);
-    s.cmask = reinterpret_cast<unsigned int*>(p); p += kChunk * 8;
-    s.misc = reinterpret_cast<unsigned int*>(p);
-    return s;
-}
-
-__device__ __forceinline__ unsigned int f2sortable(float f) {
-    const unsigned int u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float sortable2f(unsigned int s) {
-    return __uint_as_float((s & 0x80000000u) ? (s & 0x7fffffffu) : ~s);
+// The shared memory of one CTA, laid out from `base` (16-byte aligned).  Returns the end of the layout.
+__host__ __device__ __forceinline__ unsigned char* ncnn_layout(Smem& s, unsigned char* base, int M, int MCp) {
+    s.keys = take<unsigned long long>(base, MCp);
+    s.box = take<int4>(base, M);
+    s.area = take<float>(base, M);
+    s.cate = take<short>(base, M);
+    s.picked = take<unsigned short>(base, M);
+    s.chbox = take<int4>(base, kChunk);
+    s.charea = take<float>(base, kChunk);
+    s.chcate = take<short>(base, kChunk);
+    s.cmask = take<unsigned int>(base, 2 * kChunk);
+    s.misc = take<unsigned int>(base, 8);
+    return base;
 }
 
 // IoU of two int boxes exactly as nmsHandle computes it (:91-96): float(inter) / (area_a + area_b - float(inter)) > thr
@@ -91,26 +74,52 @@ __device__ __forceinline__ bool iou_gt(const int4& a, float aa, const int4& b, f
     return __fdiv_rn(ia, ua) > thr;
 }
 
-__device__ void bitonic_sort_desc(unsigned long long* keys, int n2) {
-    for (int k = 2; k <= n2; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = threadIdx.x; i < n2; i += NT) {
-                const int ixj = i ^ j;
-                if (ixj > i) {
-                    const unsigned long long a = keys[i], b = keys[ixj];
-                    const bool desc = (i & k) == 0;
-                    if (desc ? (a < b) : (a > b)) { keys[i] = b; keys[ixj] = a; }
-                }
-            }
-            __syncthreads();
+// nmsHandle's side of greedy_pass: a box suppresses only boxes of its category, and every kept box is recorded, the first max_out
+// of them in the outputs.
+struct NcnnPass {
+    const NcnnArgs& p;
+    const Smem& s;
+    int* oboxes;
+    float* oscores;
+    int* ocates;
+
+    __device__ __forceinline__ void stage(int j, unsigned long long key) const {
+        const unsigned int slot = (unsigned int)(key & 0xFFFFull);
+        s.chbox[j] = s.box[slot]; s.charea[j] = s.area[slot]; s.chcate[j] = s.cate[slot];
+    }
+    struct Cand {
+        int4 box;
+        float area;
+        short cate;
+    };
+    __device__ __forceinline__ Cand cand(int j) const { return {s.chbox[j], s.charea[j], s.chcate[j]}; }
+    __device__ __forceinline__ bool kept_other_source(int, const Cand&) const { return true; }
+    __device__ __forceinline__ bool kept_same_class(int i, const Cand& c) const { return s.cate[s.picked[i]] == c.cate; }
+    __device__ __forceinline__ bool kept_kills(int i, const Cand& c) const {
+        const unsigned int ks = s.picked[i];
+        return iou_gt(c.box, c.area, s.box[ks], s.area[ks], p.nms_thresh);
+    }
+    __device__ __forceinline__ bool other_source(const Cand&, int) const { return true; }
+    __device__ __forceinline__ bool same_class(const Cand& c, int j) const { return s.chcate[j] == c.cate; }
+    __device__ __forceinline__ bool kills(const Cand& c, int j) const {
+        return iou_gt(s.chbox[j], s.charea[j], c.box, c.area, p.nms_thresh);
+    }
+    __device__ __forceinline__ void append(int pos, int j, const unsigned long long& key) const {
+        s.picked[pos] = (unsigned short)(key & 0xFFFFull);
+        if (pos < p.max_out) {
+            const int4 b = s.chbox[j];
+            oboxes[4 * pos] = b.x; oboxes[4 * pos + 1] = b.y; oboxes[4 * pos + 2] = b.z; oboxes[4 * pos + 3] = b.w;
+            oscores[pos] = sortable2f((unsigned int)(key >> 32));
+            ocates[pos] = (int)s.chcate[j];
         }
     }
-}
+};
 
 __global__ void __launch_bounds__(NT)
 ncnn_post_kernel(const NcnnArgs p) {
     extern __shared__ __align__(16) unsigned char smraw[];
-    const Smem s = carve(smraw, p.M, p.MCp);
+    Smem s;
+    ncnn_layout(s, smraw, p.M, p.MCp);
     const int n = blockIdx.x, t = threadIdx.x;
     const int warp = t >> 5, lane = t & 31;
     if (t == 0) s.misc[0] = 0u;
@@ -166,88 +175,13 @@ ncnn_post_kernel(const NcnnArgs p) {
     }
     __syncthreads();
     const int cnt = (int)s.misc[0];
-    int n2 = 64;
-    while (n2 < cnt) n2 <<= 1;
-    for (int i = cnt + t; i < n2; i += NT) s.keys[i] = 0ull;
-    __syncthreads();
-    bitonic_sort_desc(s.keys, n2);                                           // nmsHandle :84
+    sort_keys_desc(s.keys, cnt);                                             // nmsHandle :84
 
-    // ---- greedy per-class suppression (:86-103), 64 sorted candidates at a time -------------------------------------
+    // ---- greedy per-class suppression (:86-103), 64 sorted candidates at a time; counts[n] reports every kept box ----------
     int* oboxes = p.boxes + (long long)n * p.max_out * 4;
     float* oscores = p.scores + (long long)n * p.max_out;
     int* ocates = p.cates + (long long)n * p.max_out;
-    int np = 0;
-    for (int c0 = 0; c0 < cnt; c0 += kChunk) {
-        const int cn = min(kChunk, cnt - c0);
-        if (t < kChunk) {
-            s.cmask[2 * t] = 0u; s.cmask[2 * t + 1] = 0u;
-            if (t < cn) {
-                const unsigned int slot = (unsigned int)(s.keys[c0 + t] & 0xFFFFull);
-                s.chbox[t] = s.box[slot]; s.charea[t] = s.area[slot]; s.chcate[t] = s.cate[slot];
-            }
-        }
-        if (t == 0) { s.misc[1] = 0u; s.misc[2] = 0u; }
-        __syncthreads();
-        {   // (a) against everything kept so far: four threads per candidate, every fourth kept box each
-            const int j = t & (kChunk - 1), q = t / kChunk;
-            if (j < cn) {
-                const int4 bj = s.chbox[j];
-                const float aj = s.charea[j];
-                const short cj = s.chcate[j];
-                bool dead = false;
-                for (int i = q; i < np && !dead; i += NT / kChunk) {
-                    const unsigned int ks = s.picked[i];
-                    dead = s.cate[ks] == cj && iou_gt(bj, aj, s.box[ks], s.area[ks], p.nms_thresh);
-                }
-                if (dead) atomicOr(&s.misc[1 + (j >> 5)], 1u << (j & 31));
-            }
-        }
-        __syncthreads();
-        {   // (b) pairs inside the block: thread -> earlier candidate i, 16 later candidates
-            const unsigned long long deadm = ((unsigned long long)s.misc[2] << 32) | s.misc[1];
-            const int i = t >> 2, jq = t & 3;
-            if (i < cn && !((deadm >> i) & 1ull)) {
-                const int4 bi = s.chbox[i];
-                const float ai = s.charea[i];
-                const short ci = s.chcate[i];
-                unsigned int bits = 0u;
-                for (int e = 0; e < 16; ++e) {
-                    const int j = jq * 16 + e;
-                    if (j > i && j < cn && !((deadm >> j) & 1ull) && s.chcate[j] == ci && iou_gt(s.chbox[j], s.charea[j], bi, ai, p.nms_thresh))
-                        bits |= 1u << e;
-                }
-                if (bits) atomicOr(&s.cmask[2 * i + (jq >> 1)], bits << ((jq & 1) * 16));
-            }
-        }
-        __syncthreads();
-        if (t == 0) {   // (c) serial resolve
-            unsigned long long alive = ~(((unsigned long long)s.misc[2] << 32) | s.misc[1]);
-            if (cn < 64) alive &= (1ull << cn) - 1ull;
-            unsigned long long kept = 0ull;
-            while (alive) {
-                const int i = __ffsll((long long)alive) - 1;
-                kept |= 1ull << i;
-                alive &= ~(((unsigned long long)s.cmask[2 * i + 1] << 32) | s.cmask[2 * i]);
-                alive &= ~(1ull << i);
-            }
-            s.misc[3] = (unsigned int)kept; s.misc[4] = (unsigned int)(kept >> 32);
-        }
-        __syncthreads();
-        const unsigned long long kept = ((unsigned long long)s.misc[4] << 32) | s.misc[3];
-        if (t < cn && ((kept >> t) & 1ull)) {   // (d) append
-            const int pos = np + __popcll(kept & ((1ull << t) - 1ull));
-            const unsigned long long key = s.keys[c0 + t];
-            s.picked[pos] = (unsigned short)(key & 0xFFFFull);
-            if (pos < p.max_out) {
-                const int4 b = s.chbox[t];
-                oboxes[4 * pos] = b.x; oboxes[4 * pos + 1] = b.y; oboxes[4 * pos + 2] = b.z; oboxes[4 * pos + 3] = b.w;
-                oscores[pos] = sortable2f((unsigned int)(key >> 32));
-                ocates[pos] = (int)s.chcate[t];
-            }
-        }
-        np += __popcll(kept);
-        __syncthreads();
-    }
+    const int np = greedy_pass(s.keys, cnt, cnt, s.cmask, s.misc + 1, NcnnPass{p, s, oboxes, oscores, ocates});
     if (t == 0) p.counts[n] = np;
     for (int i = min(np, p.max_out) + t; i < p.max_out; i += NT) {
         oboxes[4 * i] = 0; oboxes[4 * i + 1] = 0; oboxes[4 * i + 2] = 0; oboxes[4 * i + 3] = 0;
@@ -278,11 +212,11 @@ extern "C" int yfv2_ncnn_post(const float* out2, const float* out3, int N, int H
     }
     p.A = A; p.C = C; p.ch = 5 * A + C;
     p.M = A * (p.h[0] * p.w[0] + p.h[1] * p.w[1]);
-    p.MCp = 64;
-    while (p.MCp < p.M) p.MCp <<= 1;
+    p.MCp = pow2_at_least(p.M);
     p.thresh = thresh; p.nms_thresh = nms_thresh; p.scale_w = scale_w; p.scale_h = scale_h;
     p.max_out = max_out; p.boxes = boxes; p.scores = scores; p.cates = cates; p.counts = counts;
-    const size_t bytes = smem_bytes(p.M, p.MCp);
+    Smem s;
+    const size_t bytes = reinterpret_cast<size_t>(ncnn_layout(s, nullptr, p.M, p.MCp));
     if (p.M > 0xFFFF || bytes > kSmemCap) { set_error("ncnn_post: %d candidates per image need %zu bytes of shared memory", p.M, bytes); return YFV2_EUNSUPPORTED; }
     YFV2_CUDA(cudaFuncSetAttribute(ncnn_post_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     ncnn_post_kernel<<<N, NT, bytes, (cudaStream_t)stream>>>(p);

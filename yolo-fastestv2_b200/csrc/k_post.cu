@@ -21,16 +21,14 @@
 #include <new>
 
 #include "common.cuh"
+#include "nms.cuh"
 
 namespace yfv2 {
 namespace {
 
-constexpr int NT = 256;
-constexpr int kMaxA = 8;
 constexpr int kCPL = 8;              // classes per lane -> C <= 256
 constexpr int kChunkCells = 32;
 constexpr int kSStride = kChunkCells + 1;
-constexpr int kNmsChunk = 64;
 constexpr int kNmsListMinDet = 513;    // per-class kept lists pay off only for long kept lists (see sort_and_suppress)
 constexpr int kNmsListClasses = 256;   // per-class kept lists (heads + class histogram) for up to this many classes
 
@@ -251,14 +249,6 @@ struct NmsSmem {
     }* misc;
 };
 
-// n elements of T at `at`; the next buffer starts 16-byte aligned
-template <class T>
-__host__ __device__ __forceinline__ T* take(unsigned char*& at, size_t n) {
-    T* r = reinterpret_cast<T*>(at);
-    at += (n * sizeof(T) + 15) & ~(size_t)15;
-    return r;
-}
-
 // The shared memory of one NMS CTA, laid out from `base` (16-byte aligned).  Returns the end of the layout.
 __host__ __device__ __forceinline__ unsigned char* nms_layout(NmsSmem& s, unsigned char* base, int M, int MCp, int max_det) {
     s.keys = take<unsigned long long>(base, MCp);
@@ -266,11 +256,11 @@ __host__ __device__ __forceinline__ unsigned char* nms_layout(NmsSmem& s, unsign
     s.ccls = take<unsigned short>(base, M);
     s.kbox = take<float4>(base, max_det);
     s.karea = take<float>(base, max_det);
-    s.chbox = take<float4>(base, 2 * kNmsChunk);
-    s.charea = take<float>(base, 2 * kNmsChunk);
-    s.cmask = take<unsigned int>(base, 2 * kNmsChunk);
-    s.alist = take<unsigned char>(base, kNmsChunk);
-    s.chcls = take<unsigned short>(base, 2 * kNmsChunk);
+    s.chbox = take<float4>(base, 2 * kChunk);
+    s.charea = take<float>(base, 2 * kChunk);
+    s.cmask = take<unsigned int>(base, 2 * kChunk);
+    s.alist = take<unsigned char>(base, kChunk);
+    s.chcls = take<unsigned short>(base, 2 * kChunk);
     s.misc = take<NmsSmem::Misc>(base, 1);
     unsigned char* tail = reinterpret_cast<unsigned char*>(s.keys + M);
     s.kcn = reinterpret_cast<unsigned int*>(tail); tail += (size_t)max_det * 4;
@@ -283,14 +273,6 @@ __host__ __device__ __forceinline__ unsigned char* nms_layout(NmsSmem& s, unsign
 inline size_t nms_smem_bytes(int M, int MCp, int max_det) {
     NmsSmem s;
     return reinterpret_cast<size_t>(nms_layout(s, nullptr, M, MCp, max_det));
-}
-
-__device__ __forceinline__ unsigned int f2sortable(float f) {
-    const unsigned int u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float sortable2f(unsigned int s) {
-    return __uint_as_float((s & 0x80000000u) ? (s & 0x7fffffffu) : ~s);
 }
 
 __device__ __forceinline__ bool class_ok(const NmsParams& p, int cls) {
@@ -316,10 +298,10 @@ __device__ __forceinline__ void write_candidate(const NmsSmem& s, unsigned int s
                    ((unsigned long long)(0xFFFFu - (unsigned)row) << 16) | (unsigned long long)slot;
 }
 // Warp-aggregated slot allocation: one shared-memory atomic per warp call instead of one per candidate.  All 32 lanes call.
-__device__ __forceinline__ unsigned int alloc_slots(const NmsSmem& s, bool want) {
+__device__ __forceinline__ unsigned int alloc_slots(unsigned int* count, bool want) {
     const unsigned int bal = __ballot_sync(0xffffffffu, want);
     unsigned int base = 0;
-    if ((threadIdx.x & 31) == 0 && bal) base = atomicAdd(&s.misc->count, (unsigned int)__popc(bal));
+    if ((threadIdx.x & 31) == 0 && bal) base = atomicAdd(count, (unsigned int)__popc(bal));
     base = __shfl_sync(0xffffffffu, base, 0);
     return base + __popc(bal & ((1u << (threadIdx.x & 31)) - 1u));
 }
@@ -368,103 +350,6 @@ __device__ __forceinline__ void iou_fast(const float4& a, float aa, const float4
     amb = !(((above | below) & sane) | (inter == p.iou_zero));                    // iou_zero: 0, or NaN when the threshold is not positive
 }
 
-__device__ void bitonic_sort_desc(unsigned long long* keys, int n2) {
-    for (int k = 2; k <= n2; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = threadIdx.x; i < n2; i += NT) {
-                const int ixj = i ^ j;
-                if (ixj > i) {
-                    const unsigned long long a = keys[i], b = keys[ixj];
-                    const bool desc = (i & k) == 0;
-                    if (desc ? (a < b) : (a > b)) { keys[i] = b; keys[ixj] = a; }
-                }
-            }
-            __syncthreads();
-        }
-    }
-}
-
-// Same network with E = n2 / NT keys per thread held in registers (thread t owns elements [E t, E t + E)): strides below E
-// are compare-exchanges inside the thread, strides below 32 E are 64-bit warp shuffles, and only the log2(NT/32) largest
-// strides of the last merges (6 of the 66 steps for 2048 keys) go through shared memory and barriers.  The keys are
-// unique (or equal padding zeros), so every correct sorting network yields the same order as bitonic_sort_desc.
-// The stage loops are unrolled for E <= 4 and rolled for E = 8: unrolled, the 2048-key network is ~4000 SASS instructions that
-// every warp runs exactly once, and ncu found 58 % of the stall samples inside it on instruction fetch (decode + NMS 178.8 us
-// per launch unrolled, 161.1 rolled, on the bench workload).  Rolled, k and j are run-time values and the strides below E
-// dispatch to three instantiated bodies of sort_intra.
-template <int E, int J>
-__device__ __forceinline__ void sort_intra(unsigned long long (&v)[E], int k, int t) {
-#pragma unroll
-    for (int m = 0; m < E; ++m) {
-        if ((m & J) == 0) {
-            const int i = E * t + m;
-            const unsigned long long a = v[m], b = v[m | J];
-            const bool desc = (i & k) == 0;
-            if (desc ? (a < b) : (a > b)) { v[m] = b; v[m | J] = a; }
-        }
-    }
-}
-template <int E>
-__device__ void bitonic_sort_desc_reg(unsigned long long* keys) {
-    constexpr int n2 = NT * E;
-    const int t = threadIdx.x;
-    unsigned long long v[E];
-#pragma unroll
-    for (int m = 0; m < E; ++m) v[m] = keys[E * t + m];
-#pragma unroll (E == 8 ? 1 : 16)
-    for (int k = 2; k <= n2; k <<= 1) {
-#pragma unroll (E == 8 ? 1 : 16)
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            if (j >= E) {
-                unsigned long long o[E];
-                const int pj = j / E;                            // partner thread t ^ pj
-                if (j >= 32 * E) {
-                    __syncthreads();                             // every earlier read of `keys` is done
-#pragma unroll
-                    for (int m = 0; m < E; ++m) keys[m * NT + t] = v[m];          // transposed: conflict-free both ways
-                    __syncthreads();
-#pragma unroll
-                    for (int m = 0; m < E; ++m) o[m] = keys[m * NT + (t ^ pj)];
-                } else {
-#pragma unroll
-                    for (int m = 0; m < E; ++m) o[m] = __shfl_xor_sync(0xffffffffu, v[m], pj);
-                }
-                // element i = E t + m: bits of j and k at or above E only depend on t, so the direction is the same for all m
-                const int i0 = E * t;
-                const bool keep_max = ((i0 & k) == 0) == ((i0 & j) == 0);
-#pragma unroll
-                for (int m = 0; m < E; ++m) {
-                    const unsigned long long a = v[m], b = o[m];
-                    v[m] = keep_max ? (a > b ? a : b) : (a < b ? a : b);
-                }
-            } else {
-                if (E > 4 && j == 4) sort_intra<E, (E > 4 ? 4 : 1)>(v, k, t);
-                else if (E > 2 && j == 2) sort_intra<E, (E > 2 ? 2 : 1)>(v, k, t);
-                else sort_intra<E, 1>(v, k, t);
-            }
-        }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int m = 0; m < E; ++m) keys[E * t + m] = v[m];
-    __syncthreads();
-}
-
-// Sorts the first `cnt` keys descending: pads them with zeros to n2 = the power of two >= max(cnt, 64) (the buffer must hold n2)
-// and runs the register network for 256..2048 keys, the shared-memory one otherwise.  All threads of the CTA call this.
-// (sort_and_suppress spells the same dispatch out inline: calling this helper there changes its register allocation.)
-__device__ __forceinline__ void sort_keys_desc(unsigned long long* keys, int cnt) {
-    int n2 = 64;
-    while (n2 < cnt) n2 <<= 1;
-    for (int i = cnt + threadIdx.x; i < n2; i += NT) keys[i] = 0ull;
-    __syncthreads();
-    if (n2 == NT) bitonic_sort_desc_reg<1>(keys);
-    else if (n2 == 2 * NT) bitonic_sort_desc_reg<2>(keys);
-    else if (n2 == 4 * NT) bitonic_sort_desc_reg<4>(keys);
-    else if (n2 == 8 * NT) bitonic_sort_desc_reg<8>(keys);
-    else bitonic_sort_desc(keys, n2);
-}
-
 // Sort the pushed candidates and run the blocked greedy suppression.  All threads of the CTA call this.
 // PROF (debug builds of the kernels, yfv2_debug_nms_profile): thread 0 accumulates clock64 ticks per phase; `tstart` is the
 // kernel's first timestamp.  Phases: 0 candidate generation, 1 class histogram + sort, 2 staging of the first chunk, 3 chunk vs
@@ -500,8 +385,7 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
         __syncthreads();
         by_class = s.misc->majority == 0u;
     }
-    int n2 = 64;
-    while (n2 < cnt) n2 <<= 1;
+    const int n2 = pow2_at_least(cnt);
     for (int i = cnt + threadIdx.x; i < n2; i += NT) s.keys[i] = 0ull;
     __syncthreads();
     if (n2 == NT) bitonic_sort_desc_reg<1>(s.keys);
@@ -532,23 +416,23 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
             const float4 b = s.cbox[slot];
             const float off = __fmul_rn((float)s.ccls[slot], p.max_wh);            // utils/utils.py:283
             const float4 ob = make_float4(__fadd_rn(b.x, off), __fadd_rn(b.y, off), __fadd_rn(b.z, off), __fadd_rn(b.w, off));
-            s.chbox[buf * kNmsChunk + j] = ob;
-            s.charea[buf * kNmsChunk + j] = __fmul_rn(__fsub_rn(ob.z, ob.x), __fsub_rn(ob.w, ob.y));
-            if (by_class) s.chcls[buf * kNmsChunk + j] = s.ccls[slot];
+            s.chbox[buf * kChunk + j] = ob;
+            s.charea[buf * kChunk + j] = __fmul_rn(__fsub_rn(ob.z, ob.x), __fsub_rn(ob.w, ob.y));
+            if (by_class) s.chcls[buf * kChunk + j] = s.ccls[slot];
         }
     };
-    if (t < kNmsChunk) stage(0, 0, t);
+    if (t < kChunk) stage(0, 0, t);
     if (t == 0) { s.misc->dead[0] = 0u; s.misc->dead[1] = 0u; }
     __syncthreads();
     tick(2);
-    for (int c0 = 0, it = 0; c0 < cnt && nk < p.max_det; c0 += kNmsChunk, ++it) {
-        const int cn = min(kNmsChunk, cnt - c0);
-        const float4* chbox = s.chbox + (it & 1) * kNmsChunk;
-        const float* charea = s.charea + (it & 1) * kNmsChunk;
-        const unsigned short* chcls = s.chcls + (it & 1) * kNmsChunk;
+    for (int c0 = 0, it = 0; c0 < cnt && nk < p.max_det; c0 += kChunk, ++it) {
+        const int cn = min(kChunk, cnt - c0);
+        const float4* chbox = s.chbox + (it & 1) * kChunk;
+        const float* charea = s.charea + (it & 1) * kChunk;
+        const unsigned short* chcls = s.chcls + (it & 1) * kChunk;
         ++nchunks;
         {   // (a) chunk candidates against everything kept so far
-            const int j = t & (kNmsChunk - 1), q = t / kNmsChunk;
+            const int j = t & (kChunk - 1), q = t / kChunk;
             if (j < cn && by_class) {
                 // walk the kept boxes of this candidate's class; the candidate's four threads test every fourth node
                 const float4 bj = chbox[j];
@@ -556,14 +440,14 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
                 bool dead = false;
                 int k = 0;
                 for (unsigned i = s.khead[chcls[j]]; i != 0xFFFFu && !dead; i = s.kcn[i] >> 16, ++k)
-                    if ((k & (NT / kNmsChunk - 1)) == q) dead = iou_gt(s.kbox[i], s.karea[i], bj, aj, p);
+                    if ((k & (NT / kChunk - 1)) == q) dead = iou_gt(s.kbox[i], s.karea[i], bj, aj, p);
                 if (dead) atomicOr(&s.misc->dead[j >> 5], 1u << (j & 31));
             } else if (j < cn) {
                 const float4 bj = chbox[j];
                 const float aj = charea[j];
                 // four kept boxes per trip: the loads and IoU fronts are independent, only the exit test is shared
                 bool dead = false;
-                constexpr int STEP = NT / kNmsChunk;
+                constexpr int STEP = NT / kChunk;
                 int i = q;
                 for (; i + 3 * STEP < nk && !dead; i += 4 * STEP) {
                     bool d[4], m[4];
@@ -588,11 +472,11 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
         unsigned long long alive = ~(((unsigned long long)s.misc->dead[1] << 32) | s.misc->dead[0]);
         if (cn < 64) alive &= (1ull << cn) - 1ull;
         const int na = __popcll(alive);
-        if (t < kNmsChunk) {
+        if (t < kChunk) {
             s.cmask[2 * t] = 0u; s.cmask[2 * t + 1] = 0u;
             if ((alive >> t) & 1ull) s.alist[__popcll(alive & ((1ull << t) - 1ull))] = (unsigned char)t;
-        } else if (t < 2 * kNmsChunk) {
-            stage(c0 + kNmsChunk, (it + 1) & 1, t - kNmsChunk);       // (nothing to do past the end)
+        } else if (t < 2 * kChunk) {
+            stage(c0 + kChunk, (it + 1) & 1, t - kChunk);       // (nothing to do past the end)
         }
         __syncthreads();
         if (t == 0) { s.misc->dead[0] = 0u; s.misc->dead[1] = 0u; }  // every thread has read the dead bits
@@ -633,9 +517,8 @@ __device__ void sort_and_suppress(const NmsSmem& s, const NmsParams& p, int n, l
         }
         __syncthreads();
         tick(4);
-        // (c) greedy resolve over the kill rows by warp 0: the lowest live candidate is kept and its row cleared from the live set.  Two
-        // 32-bit halves keep the dependent chain short (find-first-set, one shared load, one logic op per kept candidate); a row's
-        // upper half is applied to the upper live bits off the chain.
+        // (c) greedy resolve over the kill rows by warp 0: resolve_chunk written out (calling it here reorders two compares in the
+        // SASS of every NMS kernel)
         if (t < 32) {
             unsigned int lo = (unsigned int)alive, hi = (unsigned int)(alive >> 32), klo = 0u, khi = 0u;
             int room = p.max_det - nk;
@@ -882,7 +765,7 @@ __device__ __forceinline__ void thread_cell_candidates(const PostGeom& g, const 
                 }
             }
         }
-        const unsigned int slot = alloc_slots(s, want);
+        const unsigned int slot = alloc_slots(&s.misc->count, want);
         if (want) write_candidate(s, slot, box.x, box.y, box.z, box.w, conf, cls, row0 + cell * A + a, p.max_wh);
     }
 }
@@ -937,7 +820,7 @@ __device__ __forceinline__ void thread_cell_candidates_80x3(const PostGeom& g, c
     for (int a = 0; a < A; ++a) {
         float4 box = make_float4(0.f, 0.f, 0.f, 0.f);
         if (want[a]) box = decode_box(r[a][0], r[a][1], r[a][2], r[a][3], x, y, g.stride[lv], g.anc[lv][a][0], g.anc[lv][a][1]);
-        const unsigned int slot = alloc_slots(s, want[a]);
+        const unsigned int slot = alloc_slots(&s.misc->count, want[a]);
         if (want[a]) write_candidate(s, slot, box.x, box.y, box.z, box.w, conf[a], cls[a], row0 + cell * A + a, p.max_wh);
     }
 }
@@ -1000,7 +883,7 @@ decode_nms_kernel(PostGeom g, NmsParams p) {
                         warp_argmax(best, bi);
                         if (lane == a && best > p.conf_thres && class_ok(p, bi)) { my_want = true; my_conf = best; my_cls = bi; }
                     }
-                    const unsigned int slot = alloc_slots(s, my_want);
+                    const unsigned int slot = alloc_slots(&s.misc->count, my_want);
                     if (my_want)
                         write_candidate(s, slot, r.box.x, r.box.y, r.box.z, r.box.w, my_conf, my_cls, row0 + (cell0 + cl) * A + lane, p.max_wh);
                 }
@@ -1015,7 +898,6 @@ decode_nms_kernel(PostGeom g, NmsParams p) {
 // frame.  The region descriptors of a launch's frames travel in the kernel parameters; the rows are read from global memory and
 // mapped to frame pixels on the fly, and only the kept boxes are held in shared memory (fp64).
 constexpr int kMergeFrames = 128;              // frames per launch
-constexpr int kMergeChunk = 64;                // candidates per step of the blocked greedy pass
 
 struct MergeArgs {
     const float* dets;           // [T, max_det_in, 6]
@@ -1048,13 +930,13 @@ struct MergeSmem {
 __host__ __device__ __forceinline__ unsigned char* merge_layout(MergeSmem& s, unsigned char* base, int MCp, int KC) {
     s.keys = take<unsigned long long>(base, MCp);
     s.kbox = take<double4>(base, KC);
-    s.chbox = take<double4>(base, kMergeChunk);
+    s.chbox = take<double4>(base, kChunk);
     s.kcls = take<float>(base, KC);
-    s.chcls = take<float>(base, kMergeChunk);
-    s.cmask = take<unsigned int>(base, 2 * kMergeChunk);
+    s.chcls = take<float>(base, kChunk);
+    s.cmask = take<unsigned int>(base, 2 * kChunk);
     s.misc = take<unsigned int>(base, 8);
     s.kt = take<unsigned short>(base, KC);
-    s.cht = take<unsigned short>(base, kMergeChunk);
+    s.cht = take<unsigned short>(base, kChunk);
     return base;
 }
 
@@ -1079,6 +961,55 @@ __device__ __forceinline__ bool overlap_gt(const double4& a, const double4& b, d
     const double den = metric ? dmin(aa, ab) : __dsub_rn(__dadd_rn(aa, ab), inter);
     return __ddiv_rn(inter, den) > thr;
 }
+
+// The merge's side of greedy_pass: candidates staged from the rows in global memory, mapped to frame pixels; a box suppresses
+// only boxes of other regions and the same class.
+struct MergePass {
+    const MergeArgs& a;
+    const MergeSmem& s;
+    double* out;
+    int* ksrc;
+    long long tg0;                                               // global index of the frame's first region
+    int rb;                                                      // the frame's first region in a.reg
+
+    __device__ __forceinline__ void stage(int j, unsigned long long key) const {
+        const int mdi = a.max_det_in;
+        const unsigned int slot = 0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull);
+        const int tl = (int)slot / mdi, row = (int)slot - tl * mdi;
+        const float* r = a.dets + ((tg0 + tl) * mdi + row) * 6;
+        const int4 g = a.reg[rb + tl];
+        const double sx = __ddiv_rn((double)g.z, (double)a.W), sy = __ddiv_rn((double)g.w, (double)a.H);
+        const double x0 = (double)g.x, y0 = (double)g.y;
+        s.chbox[j] = make_double4(__dadd_rn(__dmul_rn((double)__ldg(r), sx), x0), __dadd_rn(__dmul_rn((double)__ldg(r + 1), sy), y0),
+                                  __dadd_rn(__dmul_rn((double)__ldg(r + 2), sx), x0), __dadd_rn(__dmul_rn((double)__ldg(r + 3), sy), y0));
+        s.chcls[j] = __ldg(r + 5);
+        s.cht[j] = (unsigned short)tl;
+    }
+    struct Cand {
+        double4 box;
+        float cls;
+        unsigned short t;
+    };
+    __device__ __forceinline__ Cand cand(int j) const { return {s.chbox[j], s.chcls[j], s.cht[j]}; }
+    __device__ __forceinline__ bool kept_other_source(int i, const Cand& c) const { return s.kt[i] != c.t; }
+    __device__ __forceinline__ bool kept_same_class(int i, const Cand& c) const { return s.kcls[i] == c.cls; }
+    __device__ __forceinline__ bool kept_kills(int i, const Cand& c) const { return overlap_gt(s.kbox[i], c.box, a.thr, a.metric); }
+    __device__ __forceinline__ bool other_source(const Cand& c, int j) const { return s.cht[j] != c.t; }
+    __device__ __forceinline__ bool same_class(const Cand& c, int j) const { return s.chcls[j] == c.cls; }
+    __device__ __forceinline__ bool kills(const Cand& c, int j) const { return overlap_gt(c.box, s.chbox[j], a.thr, a.metric); }
+    __device__ __forceinline__ void append(int pos, int j, const unsigned long long& key) const {
+        const double4 b = s.chbox[j];
+        s.kbox[pos] = b;
+        s.kcls[pos] = s.chcls[j];
+        s.kt[pos] = s.cht[j];
+        const unsigned int slot = 0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull);
+        double* o = out + pos * 6;
+        o[0] = b.x; o[1] = b.y; o[2] = b.z; o[3] = b.w;
+        o[4] = (double)__ldg(a.dets + (tg0 * a.max_det_in + slot) * 6 + 4);     // (the key holds conf + 0)
+        o[5] = (double)s.chcls[j];
+        if (ksrc) ksrc[pos] = (int)(tg0 * a.max_det_in + slot);
+    }
+};
 
 __global__ void __launch_bounds__(NT)
 merge_regions_kernel(const __grid_constant__ MergeArgs a) {
@@ -1109,10 +1040,7 @@ merge_regions_kernel(const __grid_constant__ MergeArgs a) {
                 }
             }
         }
-        const unsigned int bal = __ballot_sync(0xffffffffu, want);
-        unsigned int pos = 0;
-        if ((t & 31) == 0 && bal) pos = atomicAdd(&s.misc[0], (unsigned int)__popc(bal));
-        pos = __shfl_sync(0xffffffffu, pos, 0) + __popc(bal & ((1u << (t & 31)) - 1u));
+        const unsigned int pos = alloc_slots(&s.misc[0], want);
         if (want) s.keys[pos] = key;
     }
     __syncthreads();
@@ -1121,91 +1049,7 @@ merge_regions_kernel(const __grid_constant__ MergeArgs a) {
 
     double* out = a.out + (long long)f * a.max_det * 6;
     int* ksrc = a.kept_src ? a.kept_src + (long long)f * a.max_det : nullptr;
-    int nk = 0;
-    for (int c0 = 0; c0 < cnt && nk < a.max_det; c0 += kMergeChunk) {
-        const int cn = min(kMergeChunk, cnt - c0);
-        if (t < cn) {                                        // stage the chunk: rows mapped to frame pixels
-            const unsigned int slot = 0xFFFFFFFFu - (unsigned int)(s.keys[c0 + t] & 0xFFFFFFFFull);
-            const int tl = (int)slot / mdi, row = (int)slot - tl * mdi;
-            const float* r = a.dets + ((tg0 + tl) * mdi + row) * 6;
-            const int4 g = a.reg[rb + tl];
-            const double sx = __ddiv_rn((double)g.z, (double)a.W), sy = __ddiv_rn((double)g.w, (double)a.H);
-            const double x0 = (double)g.x, y0 = (double)g.y;
-            s.chbox[t] = make_double4(__dadd_rn(__dmul_rn((double)__ldg(r), sx), x0), __dadd_rn(__dmul_rn((double)__ldg(r + 1), sy), y0),
-                                      __dadd_rn(__dmul_rn((double)__ldg(r + 2), sx), x0), __dadd_rn(__dmul_rn((double)__ldg(r + 3), sy), y0));
-            s.chcls[t] = __ldg(r + 5);
-            s.cht[t] = (unsigned short)tl;
-        }
-        if (t < 2 * kMergeChunk) s.cmask[t] = 0u;
-        if (t == 0) { s.misc[1] = 0u; s.misc[2] = 0u; }
-        __syncthreads();
-        {   // (a) the chunk against every box kept so far, four threads per candidate
-            const int j = t & (kMergeChunk - 1), q = t / kMergeChunk;
-            if (j < cn) {
-                const double4 bj = s.chbox[j];
-                const float cj = s.chcls[j];
-                const unsigned short tj = s.cht[j];
-                bool dead = false;
-                for (int i = q; i < nk && !dead; i += NT / kMergeChunk)
-                    dead = s.kt[i] != tj && s.kcls[i] == cj && overlap_gt(s.kbox[i], bj, a.thr, a.metric);
-                if (dead) atomicOr(&s.misc[1 + (j >> 5)], 1u << (j & 31));
-            }
-        }
-        __syncthreads();
-        unsigned long long alive = ~(((unsigned long long)s.misc[2] << 32) | s.misc[1]);
-        if (cn < 64) alive &= (1ull << cn) - 1ull;
-        {   // (b) pairs inside the chunk among the survivors of (a): candidate i against 16 of the later ones per thread
-            const int i = t >> 2, jq = t & 3;
-            if ((alive >> i) & 1ull) {
-                const double4 bi = s.chbox[i];
-                const float ci = s.chcls[i];
-                const unsigned short ti = s.cht[i];
-                unsigned int bits = 0u;
-                for (int e = 0; e < 16; ++e) {
-                    const int j = jq * 16 + e;
-                    if (j > i && ((alive >> j) & 1ull) && s.cht[j] != ti && s.chcls[j] == ci && overlap_gt(bi, s.chbox[j], a.thr, a.metric))
-                        bits |= 1u << e;
-                }
-                if (bits) atomicOr(&s.cmask[2 * i + (jq >> 1)], bits << ((jq & 1) * 16));
-            }
-        }
-        __syncthreads();
-        if (t < 32) {                                        // (c) greedy resolve, as in sort_and_suppress
-            unsigned int lo = (unsigned int)alive, hi = (unsigned int)(alive >> 32), klo = 0u, khi = 0u;
-            int room = a.max_det - nk;
-            while (lo && room > 0) {
-                const int i = __ffs((int)lo) - 1;
-                klo |= 1u << i;
-                --room;
-                lo &= ~(1u << i) & ~s.cmask[2 * i];
-                hi &= ~s.cmask[2 * i + 1];
-            }
-            while (hi && room > 0) {
-                const int i = __ffs((int)hi) - 1;
-                khi |= 1u << i;
-                --room;
-                hi &= ~(1u << i) & ~s.cmask[2 * (i + 32) + 1];
-            }
-            if (t == 0) { s.misc[3] = klo; s.misc[4] = khi; }
-        }
-        __syncthreads();
-        const unsigned long long kept = ((unsigned long long)s.misc[4] << 32) | (unsigned long long)s.misc[3];
-        if (t < cn && ((kept >> t) & 1ull)) {                // (d) append
-            const int pos = nk + __popcll(kept & ((1ull << t) - 1ull));
-            const double4 b = s.chbox[t];
-            s.kbox[pos] = b;
-            s.kcls[pos] = s.chcls[t];
-            s.kt[pos] = s.cht[t];
-            const unsigned int slot = 0xFFFFFFFFu - (unsigned int)(s.keys[c0 + t] & 0xFFFFFFFFull);
-            double* o = out + pos * 6;
-            o[0] = b.x; o[1] = b.y; o[2] = b.z; o[3] = b.w;
-            o[4] = (double)__ldg(a.dets + (tg0 * mdi + slot) * 6 + 4);     // (the key holds conf + 0)
-            o[5] = (double)s.chcls[t];
-            if (ksrc) ksrc[pos] = (int)(tg0 * mdi + slot);
-        }
-        nk += __popcll(kept);
-        __syncthreads();
-    }
+    const int nk = greedy_pass(s.keys, cnt, a.max_det, s.cmask, s.misc + 1, MergePass{a, s, out, ksrc, tg0, rb});
     if (t == 0) a.out_counts[f] = nk;
     for (int i = nk * 6 + t; i < a.max_det * 6; i += NT) out[i] = 0.0;
     if (ksrc) for (int i = nk + t; i < a.max_det; i += NT) ksrc[i] = -1;
@@ -1253,8 +1097,7 @@ int fill_nms(NmsParams& p, int M, float conf_thres, double iou_thres, const int*
     }
     p.class_filter = n_filter > 0 ? class_filter : nullptr; p.n_filter = n_filter;
     p.max_det = max_det; p.max_wh = max_wh; p.out = out; p.counts = counts; p.kept_idx = kept_idx; p.M = M;
-    p.MCp = 64;
-    while (p.MCp < M) p.MCp <<= 1;
+    p.MCp = pow2_at_least(M);
     p.C = 1 << 30;                                           // callers that know the class count set it
     p.prof = nullptr;
     return YFV2_OK;
@@ -1432,8 +1275,7 @@ extern "C" int yfv2_merge_regions(const float* dets, const int* counts, const yf
         a.rbeg[nf] = nr;
         a.f0 = f0; a.t0 = t0;
         const int slots = most * max_det_in;
-        a.MCp = 64;
-        while (a.MCp < slots) a.MCp <<= 1;
+        a.MCp = pow2_at_least(slots);
         a.KC = std::max(1, std::min(max_det, slots));
         const size_t bytes = merge_smem_bytes(a.MCp, a.KC);
         if (bytes > kSmemCap) { set_error("merge_regions: %zu bytes of shared memory needed", bytes); return YFV2_EUNSUPPORTED; }
