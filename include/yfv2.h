@@ -426,6 +426,45 @@ typedef struct yfv2_bayer_frame {
 } yfv2_bayer_frame;
 YFV2_API int yfv2_resize_bayer_u8(const yfv2_bayer_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
 
+/* ---- lens-corrected views -> network input: cv2.remap(INTER_LINEAR) of any frame above, then cv2.resize INTER_LINEAR --------
+ * What a calibrated camera's frames go through before detection: map1, map2 = cv2.initUndistortRectifyMap(...) (or
+ * cv2.fisheye.*, or any maps), then img = cv2.remap(cv2.cvtColor(frame, code), map1, map2, cv2.INTER_LINEAR) with the default
+ * BORDER_CONSTANT 0.  The remapped image has the map's size (mw x mh); a descriptor stands for the window (x0, y0, w, h) of it,
+ * and yfv2_resize_remap_u8 gives the bytes of cv2.resize(img[y0:y0+h, x0:x0+w], (W, H), INTER_LINEAR), transposed to CHW.
+ * The map is cv2's fixed form (CV_16SC2 map1 + CV_16UC1 map2, what cv2.convertMaps(..., CV_16SC2) and
+ * initUndistortRectifyMap(..., CV_16SC2) give); it addresses the inner frame's converted pixels (for a Bayer descriptor, its
+ * window).  Remapped pixel (c, r), with (X, Y) = xy[r][c] and k = code[r][c] & 1023, i = k >> 5, j = k & 31, is per channel
+ *   sat_u8((w00 p(X, Y) + w01 p(X+1, Y) + w10 p(X, Y+1) + w11 p(X+1, Y+1) + 16384) >> 15),
+ *   w00 = 32 (32-i)(32-j), w01 = 32 (32-i) j, w10 = 32 i (32-j), w11 = 32 i j   (cv2's 2-D table; the four sum to 32768),
+ * a tap outside the inner frame contributing 0 (the inner frame is never read out of range).  DESIGN.md §18 states it.
+ * kind: YFV2_JPEG_SRC_BGR, _STRIDED (grey is a strided frame with b = g = r), _YUV420, _YUV422 or _BAYER, naming the member of f,
+ * which is checked as the matching resize entry checks it.  The map needs xy and code non-null, 1 <= mw, mh <= 32767,
+ * xy_pitch >= 4*mw and code_pitch >= 2*mw, xy 4-byte and code 2-byte aligned with pitches multiples of that; the window must be
+ * non-empty and inside the map.  frames, dst, H, W: as yfv2_resize_strided_u8; consecutive frames of one kind go to one launch. */
+typedef struct yfv2_remap_map {
+    const int16_t* xy;     /* device [mh][mw][2] (X, Y): cv2's CV_16SC2 map1 */
+    long long xy_pitch;    /* bytes from one map row of xy to the next */
+    const uint16_t* code;  /* device [mh][mw]: cv2's CV_16UC1 map2, the interpolation code in its low 10 bits */
+    long long code_pitch;  /* bytes from one map row of code to the next */
+    int mw, mh;            /* the map's size: the remapped image's */
+} yfv2_remap_map;
+typedef struct yfv2_remap_frame {
+    int kind;              /* YFV2_JPEG_SRC_* of the inner frame, not YFV2_JPEG_SRC_GRAY */
+    int x0, y0, w, h;      /* the window of the remapped image this descriptor stands for */
+    union {
+        yfv2_frame bgr;
+        yfv2_strided_frame strided;
+        yfv2_yuv420_frame yuv420;
+        yfv2_yuv422_frame yuv422;
+        yfv2_bayer_frame bayer;
+    } f;                   /* the inner frame, in device memory */
+    yfv2_remap_map map;
+} yfv2_remap_frame;
+YFV2_API int yfv2_resize_remap_u8(const yfv2_remap_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
+/* cv2.remap on the device: the window of frame n's remapped image written as packed HWC BGR to dst[n] (device, h*w*3 bytes, rows
+ * 3*w apart), with the per-pixel arithmetic of yfv2_resize_remap_u8.  dst: N HOST pointers.  Checked as yfv2_resize_remap_u8. */
+YFV2_API int yfv2_remap_u8(const yfv2_remap_frame* frames, int N, uint8_t* const* dst, void* stream);
+
 /* ---- JPEG files -> packed HWC BGR frames: cv2.imread(path) (test.py:34; utils/datasets.py:106) on the device -----------------
  * The bytes OpenCV 4.13 (libjpeg-turbo 3.1) returns for IMREAD_COLOR: ISLOW IDCT, fancy upsampling, jdcolor's YCbCr -> BGR, grey
  * replicated to B = G = R, and the EXIF orientation applied.  Supported: baseline sequential Huffman-coded DCT (SOF0, SOF1) with

@@ -167,6 +167,125 @@ def events_ms(fn, n, stream):
     return e0.elapsed_time(e1)
 
 
+def remap_main(args):
+    """--remap: lens-corrected views (yfv2_resize_remap_u8) of N fh x fw frames through one undistortion map of the frame's size
+    (tests/remap_cases.py's numpy model, fixed K and D), for BGR, NV12 and BAYER_BG frames.  Per layout and run, L2 flushed before
+    each launch and the three paths alternated: fused_us (the fused remap + resize launch), two_pass_us (yfv2_remap_u8 into BGR
+    frames, then yfv2_resize_bgr_u8: remap_frames + resize), plain_us (the layout's own resize of the same frames, no remap), and
+    step_ms (fused resize + forward + decode/NMS, CUDA events over K steps).  Parity: frames 0 and N-1 of both paths against
+    tests/remap_oracle.py."""
+    import yfv2  # noqa: F401
+    import yfv2_engine as eng
+    import remap_cases as rc
+    import remap_oracle as ro
+    fw, fh = (int(v) for v in args.frame.lower().split("x"))
+    N, S = args.batch, bench.SIDE
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    model, _ = bench.random_state_dict()
+    model = model.to(dev).eval()
+    c = bench.cfg()
+    L = eng.lib()
+    stream = torch.cuda.current_stream(dev)
+    sp = ctypes.c_void_p(stream.cuda_stream)
+    mx, my = rc.float_maps("undistort", fw, fh, fw, fh, 0)
+    maps = eng.RemapMaps(mx, my, dev)
+    fixed = ro.convert_maps(mx, my)
+    x = torch.empty((N, 3, S, S), dtype=torch.uint8, device=dev)
+    plan = model._plan_for(x)
+    preds = plan.alloc_preds()
+    anchors = eng.anchors_array(c)
+    out = torch.empty((N, eng.MAX_DET, 6), dtype=torch.float32, device=dev)
+    counts = torch.empty((N,), dtype=torch.int32, device=dev)
+    inter = torch.empty((N, fh, fw, 3), dtype=torch.uint8, device=dev)          # the two-pass path's remapped BGR frames
+    inter_descs = (eng.Frame * N)()
+    for i in range(N):
+        inter_descs[i].data, inter_descs[i].w, inter_descs[i].h, inter_descs[i].pitch = inter[i].data_ptr(), fw, fh, 3 * fw
+    inter_ptrs = (ctypes.c_void_p * N)(*[inter[i].data_ptr() for i in range(N)])
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)     # 256 MB > L2
+    g = torch.Generator(device=dev).manual_seed(3)
+
+    def ok(rc_):
+        if rc_:
+            raise RuntimeError(L.yfv2_last_error())
+
+    def detect():
+        plan.forward(x, preds)
+        ok(L.yfv2_decode_nms(eng._ptr_array(preds), N, S, S, bench.ANCHORS, bench.CLASSES, anchors, ctypes.c_float(bench.CONF),
+                             ctypes.c_double(bench.IOU), None, 0, eng.MAX_DET, ctypes.c_float(eng.MAX_WH),
+                             ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(counts.data_ptr()), None, None, sp))
+
+    results = {}
+    for layout in ("bgr", "nv12", "bayer_bg"):
+        shape = (fh, fw, 3) if layout == "bgr" else (fh * 3 // 2, fw) if layout == "nv12" else (fh, fw)
+        frames = torch.randint(0, 256, (N,) + shape, generator=g, dtype=torch.uint8, device=dev)
+        keep = []
+        plain = [eng._describe(eng._check_frame(frames[i], layout, i, "bench"), layout, dev, keep) for i in range(N)]
+        member = eng._MEMBER[eng._KIND[layout]]
+        desc = eng._DESC[member]
+        lo, hi = eng.JpegEncSrc.f.offset, eng.JpegEncSrc.f.offset + ctypes.sizeof(desc)
+        plain_descs = (desc * N).from_buffer_copy(b"".join(bytes(s)[lo:hi] for s in plain))
+        plain_entry = getattr(L, "yfv2_resize_%s_u8" % member)
+        views = [eng._check_frame(eng.RemapView(frames[i], maps), layout, i, "bench") for i in range(N)]
+        rdescs = (eng.RemapFrame * N)(*[eng._describe(v, layout, dev, keep) for v in views])
+
+        def fused():
+            ok(L.yfv2_resize_remap_u8(rdescs, N, S, S, ctypes.c_void_p(x.data_ptr()), sp))
+
+        def two_pass():
+            ok(L.yfv2_remap_u8(rdescs, N, inter_ptrs, sp))
+            ok(L.yfv2_resize_bgr_u8(inter_descs, N, S, S, ctypes.c_void_p(x.data_ptr()), sp))
+
+        def plain_resize():
+            ok(plain_entry(plain_descs, N, S, S, ctypes.c_void_p(x.data_ptr()), sp))
+
+        def step():
+            fused()
+            detect()
+
+        for _ in range(max(args.warmup, 3)):
+            step()
+            two_pass()
+            plain_resize()
+        torch.cuda.synchronize(dev)
+        fused()
+        got_fused = x[[0, N - 1]].cpu().numpy()
+        two_pass()
+        got_two = x[[0, N - 1]].cpu().numpy()
+        for k, i in enumerate((0, N - 1)):
+            img = ro.inner_bgr(frames[i].cpu().numpy(), layout)
+            want = ro.resize_planar(img, fixed[0], fixed[1], (0, 0, fw, fh), S, S)
+            if not (np.array_equal(got_fused[k], want) and np.array_equal(got_two[k], want)):
+                raise AssertionError("bench_frames --remap parity: %s frame %d differs from the oracle" % (layout, i))
+        runs = []
+        for _ in range(args.runs):
+            ms_step = events_ms(step, args.steps, stream)
+            tot = {"fused": 0.0, "two_pass": 0.0, "plain": 0.0}
+            reps = max(5, min(args.steps, 20))
+            for _ in range(reps):
+                for name, fn in (("fused", fused), ("two_pass", two_pass), ("plain", plain_resize)):
+                    flush.zero_()
+                    tot[name] += events_ms(fn, 1, stream)
+            runs.append({"fused_us": round(1e3 * tot["fused"] / reps, 1), "two_pass_us": round(1e3 * tot["two_pass"] / reps, 1),
+                         "plain_us": round(1e3 * tot["plain"] / reps, 1), "step_ms": round(ms_step / args.steps, 3)})
+        results[layout] = runs
+        del frames, keep, plain, views
+    power = None
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        power = pynvml.nvmlDeviceGetPowerManagementLimit(pynvml.nvmlDeviceGetHandleByIndex(0)) / 1000.0
+    except Exception:
+        pass
+    print(json.dumps({"metric": "remapped %dx%d frames -> %dx%d input, fused vs remap_frames + resize" % (fw, fh, S, S),
+                      "batch": N, "steps": args.steps, "runs": results, "device": torch.cuda.get_device_name(dev),
+                      "power_limit_w": power,
+                      "timing": "CUDA events; frames resident in HBM; L2 flushed before each launch; fused, two-pass and plain "
+                                "launches alternated; step_ms: fused resize + forward + decode/NMS",
+                      "parity": "frames 0 and %d of the fused and two-pass paths equal tests/remap_oracle.py byte for byte"
+                                % (N - 1)}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -178,7 +297,12 @@ def main():
                                                         "uyvy", "yvyu", "bayer_bg", "bayer_gb", "bayer_rg", "bayer_gr",
                                                         "bayer_bg_ea", "bayer_gb_ea", "bayer_rg_ea", "bayer_gr_ea"),
                     help="source frame format")
+    ap.add_argument("--remap", action="store_true", help="lens-corrected views of bgr, nv12 and bayer_bg frames (remap_main)")
     args = ap.parse_args()
+    if args.remap:
+        if not torch.cuda.is_available():
+            raise SystemExit("bench_frames.py: no CUDA device (the product path has no CPU fallback)")
+        return remap_main(args)
     import yfv2  # noqa: F401
     import yfv2_engine as eng
     from oracle import resize as ore

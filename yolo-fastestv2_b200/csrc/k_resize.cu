@@ -11,7 +11,10 @@
 //     uu = U - 128, vv = V - 128, y = max(0, Y[r][c] - 16) * 1220542 + (1 << 19)
 //     B = sat_u8((y + 2116026 uu) >> 20), G = sat_u8((y - 852492 vv - 409993 uu) >> 20), R = sat_u8((y + 1673527 vv) >> 20);
 //   raw Bayer frames (yfv2_resize_bayer_u8), each source pixel demosaiced as cv2.cvtColor(COLOR_Bayer??2BGR / _EA) does, in
-//   integers on the 3x3 raw neighbourhood of its clamped frame coordinate (resize.cuh's BayerSource, tests/bayer_oracle.py).
+//   integers on the 3x3 raw neighbourhood of its clamped frame coordinate (resize.cuh's BayerSource, tests/bayer_oracle.py);
+//   lens-corrected views of any of these (yfv2_resize_remap_u8): each source pixel is cv2.remap(INTER_LINEAR)'s pixel of the
+//   inner frame (resize.cuh's RemapSource over the inner fetch, remap_pixel), one instantiation per inner kind.
+// yfv2_remap_u8 writes the remapped windows alone (remap_kernel), with the same remap_pixel.
 // The resize is bit-identical to OpenCV's x86 8-bit path, all integer after the coefficients:
 //   coefficients per axis: f = fl32((d + 0.5) * (n / m) - 0.5) (product and difference rounded in double), s = floor(f),
 //     f = fl32(f - s); weights rint(fl32(1 - f) * 2048), rint(f * 2048).  Along x, s < 0 -> (0, 0) then s >= w - 1 -> (w - 1, 0);
@@ -206,8 +209,112 @@ int resize_entry(const char* fn, const typename Src::Desc* frames, int N, int H,
     return launch_resize<Src>(frames, N, H, W, dst, stream);
 }
 
+// cv2.remap alone: one thread per pixel of the window of frame blockIdx.z's remapped image, written as packed HWC BGR
+template <class Inner>
+struct RemapChunk {
+    RemapDesc<Inner> src[RemapSource<Inner>::kChunk];
+    uint8_t* dst[RemapSource<Inner>::kChunk];
+};
+
+template <class Inner>
+__global__ void __launch_bounds__(kResizeBx * kResizeBy)
+remap_kernel(const __grid_constant__ RemapChunk<Inner> a) {
+    const RemapDesc<Inner>& fr = a.src[blockIdx.z];
+    const int x = blockIdx.x * kResizeBx + threadIdx.x;
+    const int y = blockIdx.y * kResizeBy + threadIdx.y;
+    if (x >= fr.w || y >= fr.h) return;
+    int v[3];
+    remap_pixel<Inner>(fr.f, fr.m, fr.x0 + x, fr.y0 + y, v);
+    uint8_t* out = a.dst[blockIdx.z] + 3 * ((size_t)y * fr.w + x);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out[c] = (uint8_t)v[c];
+}
+
+// The inner frame of a checked remap descriptor, as Inner's descriptor
+template <class Inner> const typename Inner::Desc& inner_of(const yfv2_remap_frame& f);
+template <> const yfv2_frame& inner_of<BgrSource>(const yfv2_remap_frame& f) { return f.f.bgr; }
+template <> const yfv2_strided_frame& inner_of<StridedSource>(const yfv2_remap_frame& f) { return f.f.strided; }
+template <> const yfv2_yuv420_frame& inner_of<Yuv420Source>(const yfv2_remap_frame& f) { return f.f.yuv420; }
+template <> const yfv2_yuv422_frame& inner_of<Yuv422Source>(const yfv2_remap_frame& f) { return f.f.yuv422; }
+template <> const yfv2_bayer_frame& inner_of<BayerSource>(const yfv2_remap_frame& f) { return f.f.bayer; }
+
+// frames[0, n), all of Inner's kind, RemapSource<Inner>::kChunk per launch: with dst the fused resize into dst's H x W images,
+// else the remap alone into dst_each[i]
+template <class Inner>
+int launch_remap(const yfv2_remap_frame* frames, int n, int H, int W, uint8_t* dst, uint8_t* const* dst_each, cudaStream_t stream) {
+    constexpr int kChunk = RemapSource<Inner>::kChunk;
+    const dim3 block(kResizeBx, kResizeBy);
+    for (int n0 = 0; n0 < n; n0 += kChunk) {
+        const int cnt = n - n0 < kChunk ? n - n0 : kChunk;
+        RemapDesc<Inner> d[kChunk];
+        int mw = 1, mh = 1;
+        for (int i = 0; i < cnt; ++i) {
+            const yfv2_remap_frame& fr = frames[n0 + i];
+            d[i] = RemapDesc<Inner>{inner_of<Inner>(fr), fr.map, fr.x0, fr.y0, fr.w, fr.h};
+            mw = fr.w > mw ? fr.w : mw;
+            mh = fr.h > mh ? fr.h : mh;
+        }
+        if (dst) {
+            ResizeChunk<RemapSource<Inner>> a{};
+            for (int i = 0; i < cnt; ++i) a.src[i] = d[i];
+            a.dst = dst + (size_t)n0 * 3 * H * W;
+            a.H = H; a.W = W;
+            const dim3 grid((unsigned)((W + kResizeBx - 1) / kResizeBx), (unsigned)((H + kResizeBy - 1) / kResizeBy), (unsigned)cnt);
+            resize_kernel<RemapSource<Inner>><<<grid, block, 0, stream>>>(a);
+        } else {
+            RemapChunk<Inner> a{};
+            for (int i = 0; i < cnt; ++i) {
+                a.src[i] = d[i];
+                a.dst[i] = dst_each[n0 + i];
+            }
+            const dim3 grid((unsigned)((mw + kResizeBx - 1) / kResizeBx), (unsigned)((mh + kResizeBy - 1) / kResizeBy), (unsigned)cnt);
+            remap_kernel<Inner><<<grid, block, 0, stream>>>(a);
+        }
+        YFV2_LAUNCH_CHECK();
+    }
+    return YFV2_OK;
+}
+
+// Both remap entries: the call's checks, each frame's (frame_fault), then one launch_remap per run of consecutive frames of one
+// kind, so that no kernel branches on the kind.  dst (the fused resize, H x W) or dst_each (the remap alone) is non-null.
+int remap_entry(const char* fn, const yfv2_remap_frame* frames, int N, int H, int W, uint8_t* dst, uint8_t* const* dst_each,
+                void* stream) {
+    if (!frames || (!dst && !dst_each) || N <= 0) { set_error("%s: null frames / dst or N <= 0", fn); return YFV2_EINVAL; }
+    if (dst && (H <= 0 || W <= 0 || H > kResizeMaxSide || W > kResizeMaxSide)) {
+        set_error("%s: target %dx%d outside 1..%d", fn, W, H, kResizeMaxSide);
+        return YFV2_EINVAL;
+    }
+    for (int n = 0; n < N; ++n) {
+        if (const char* why = frame_fault(frames[n])) {
+            set_error("%s: frame %d: %s (window %dx%d of a %dx%d map)", fn, n, why, frames[n].w, frames[n].h, frames[n].map.mw,
+                      frames[n].map.mh);
+            return YFV2_EINVAL;
+        }
+        if (dst_each && !dst_each[n]) { set_error("%s: frame %d: null dst", fn, n); return YFV2_EINVAL; }
+    }
+    const cudaStream_t s = (cudaStream_t)stream;
+    for (int i = 0; i < N;) {
+        int j = i + 1;
+        while (j < N && frames[j].kind == frames[i].kind) ++j;
+        uint8_t* d = dst ? dst + (size_t)i * 3 * H * W : nullptr;
+        uint8_t* const* de = dst_each ? dst_each + i : nullptr;
+        int rc = YFV2_OK;
+        switch (frames[i].kind) {
+            case YFV2_JPEG_SRC_BGR: rc = launch_remap<BgrSource>(frames + i, j - i, H, W, d, de, s); break;
+            case YFV2_JPEG_SRC_STRIDED: rc = launch_remap<StridedSource>(frames + i, j - i, H, W, d, de, s); break;
+            case YFV2_JPEG_SRC_YUV420: rc = launch_remap<Yuv420Source>(frames + i, j - i, H, W, d, de, s); break;
+            case YFV2_JPEG_SRC_YUV422: rc = launch_remap<Yuv422Source>(frames + i, j - i, H, W, d, de, s); break;
+            default: rc = launch_remap<BayerSource>(frames + i, j - i, H, W, d, de, s); break;   // kinds checked above
+        }
+        if (rc != YFV2_OK) return rc;
+        i = j;
+    }
+    return YFV2_OK;
+}
+
 }  // namespace
 }  // namespace yfv2
+
 
 extern "C" int yfv2_resize_bgr_u8(const yfv2_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
     return yfv2::resize_entry<yfv2::BgrSource>("resize_bgr_u8", frames, N, H, W, dst, stream);
@@ -227,6 +334,14 @@ extern "C" int yfv2_resize_yuv422_u8(const yfv2_yuv422_frame* frames, int N, int
 
 extern "C" int yfv2_resize_bayer_u8(const yfv2_bayer_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
     return yfv2::resize_entry<yfv2::BayerSource>("resize_bayer_u8", frames, N, H, W, dst, stream);
+}
+
+extern "C" int yfv2_resize_remap_u8(const yfv2_remap_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
+    return yfv2::remap_entry("resize_remap_u8", frames, N, H, W, dst, nullptr, stream);
+}
+
+extern "C" int yfv2_remap_u8(const yfv2_remap_frame* frames, int N, uint8_t* const* dst, void* stream) {
+    return yfv2::remap_entry("remap_u8", frames, N, 0, 0, nullptr, dst, stream);
 }
 
 namespace yfv2 {

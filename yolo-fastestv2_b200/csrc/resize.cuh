@@ -51,6 +51,30 @@ inline const char* frame_fault(const yfv2_bayer_frame& f) {
     if (f.edge_aware & ~1) return "edge_aware must be 0 or 1";
     return nullptr;
 }
+inline const char* frame_fault(const yfv2_remap_map& m) {
+    if (!m.xy || !m.code) return "null map plane";
+    if (m.mw < 1 || m.mh < 1 || m.mw > 32767 || m.mh > 32767) return "map sides must be in 1..32767";
+    if (((uintptr_t)m.xy & 3) || (m.xy_pitch & 3) || m.xy_pitch < 4LL * m.mw) return "xy must be 4-byte aligned, xy_pitch >= 4 * mw";
+    if (((uintptr_t)m.code & 1) || (m.code_pitch & 1) || m.code_pitch < 2LL * m.mw)
+        return "code must be 2-byte aligned, code_pitch >= 2 * mw";
+    return nullptr;
+}
+inline const char* frame_fault(const yfv2_remap_frame& f) {
+    const char* why = "kind must be YFV2_JPEG_SRC_BGR, _STRIDED, _YUV420, _YUV422 or _BAYER";
+    switch (f.kind) {
+        case YFV2_JPEG_SRC_BGR: why = frame_fault(f.f.bgr); break;
+        case YFV2_JPEG_SRC_STRIDED: why = frame_fault(f.f.strided); break;
+        case YFV2_JPEG_SRC_YUV420: why = frame_fault(f.f.yuv420); break;
+        case YFV2_JPEG_SRC_YUV422: why = frame_fault(f.f.yuv422); break;
+        case YFV2_JPEG_SRC_BAYER: why = frame_fault(f.f.bayer); break;
+        default: break;
+    }
+    if (why) return why;
+    if ((why = frame_fault(f.map))) return why;
+    if (f.w < 1 || f.h < 1 || f.x0 < 0 || f.y0 < 0 || (long long)f.x0 + f.w > f.map.mw || (long long)f.y0 + f.h > f.map.mh)
+        return "window empty or outside the map";
+    return nullptr;
+}
 
 __device__ __forceinline__ int sat_u8(int v) { return min(max(v, 0), 255); }
 
@@ -205,6 +229,62 @@ struct BayerSource {
 #pragma unroll
             for (int j = 0; j < 3; ++j) b[k][j] = d ? a[k][j + 1] : a[k][j];
         demosaic(b[0][0], b[0][1], b[0][2], b[1][0], b[1][1], b[1][2], b[2][0], b[2][1], b[2][2], red_row, red_col0 != d, ea, p1);
+    }
+};
+
+// cv2.remap(INTER_LINEAR, BORDER_CONSTANT 0) of an Inner frame through fixed maps: pixel (mx, my) of the remapped image, B, G,
+// R in v.  cv2's weights for code (i, j) are rint(fl32(fl32(1 - i/32) * fl32(1 - j/32)) * 32768) and so on; every factor is a
+// multiple of 1/32, so each product is exact and the weights are the integers 32 (32 - i)(32 - j) ..., already summing to 32768
+// (initInterTab2D's correction never fires; tests/remap_oracle.py computes the table cv2's way and checks this).  A tap outside
+// the inner frame's w x h weighs 0, and its fetch reads the clamped coordinate, so Inner is never read out of range; the two
+// columns of a fetch stay equal or adjacent, as BayerSource needs.
+template <class Inner>
+__device__ __forceinline__ void remap_pixel(const typename Inner::Desc& f, const yfv2_remap_map& m, int mx, int my, int (&v)[3]) {
+    const int xy = __ldg((const int*)((const uint8_t*)m.xy + (long long)my * m.xy_pitch) + mx);    // 4-byte aligned: checked
+    const int X = (int)(int16_t)(xy & 0xffff), Y = xy >> 16;
+    const int k = __ldg((const uint16_t*)((const uint8_t*)m.code + (long long)my * m.code_pitch) + mx) & 1023;
+    const int i = k >> 5, j = k & 31;
+    const int w = f.w, h = f.h;
+    const bool x0in = (unsigned)X < (unsigned)w, x1in = (unsigned)(X + 1) < (unsigned)w;
+    const bool y0in = (unsigned)Y < (unsigned)h, y1in = (unsigned)(Y + 1) < (unsigned)h;
+    if (!((x0in || x1in) && (y0in || y1in))) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) v[c] = 0;
+        return;
+    }
+    const int ax0 = x0in ? 32 - j : 0, ax1 = x1in ? j : 0;
+    const int by0 = y0in ? 32 - i : 0, by1 = y1in ? i : 0;
+    const int cx0 = min(max(X, 0), w - 1), cx1 = min(max(X + 1, 0), w - 1);
+    const Inner row0(f, min(max(Y, 0), h - 1)), row1(f, min(max(Y + 1, 0), h - 1));
+    int p00[3], p01[3], p10[3], p11[3];          // [row][column] taps, B G R
+    row0.fetch(cx0, cx1, p00, p01);
+    row1.fetch(cx0, cx1, p10, p11);
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+        v[c] = sat_u8(((by0 * (p00[c] * ax0 + p01[c] * ax1) + by1 * (p10[c] * ax0 + p11[c] * ax1)) * 32 + 16384) >> 15);
+}
+
+// A remapped view's descriptor on the device: the inner frame, the map and the window (w, h: the resize's source size)
+template <class Inner>
+struct RemapDesc {
+    typename Inner::Desc f;
+    yfv2_remap_map m;
+    int x0, y0, w, h;
+};
+
+// Pixels of the window of cv2.remap(inner frame), each computed from the inner frame where it is read
+template <class Inner>
+struct RemapSource {
+    using Desc = RemapDesc<Inner>;
+    // frames per launch: each descriptor, plus yfv2_remap_u8's output pointer, under the 4 KB launch limit with the chunk's rest
+    static constexpr int kChunk = 4000 / (int)(sizeof(Desc) + sizeof(void*));
+    static constexpr int kMinBlocks = 0;
+    const Desc& f;
+    int my;
+    __device__ __forceinline__ RemapSource(const Desc& f_, int r) : f(f_), my(f_.y0 + r) {}
+    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
+        remap_pixel<Inner>(f.f, f.m, f.x0 + c0, my, p0);
+        remap_pixel<Inner>(f.f, f.m, f.x0 + c1, my, p1);
     }
 };
 

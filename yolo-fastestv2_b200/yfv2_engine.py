@@ -70,6 +70,18 @@ class JpegEncSrc(ctypes.Structure):
 JPEG_SRC_BGR, JPEG_SRC_STRIDED, JPEG_SRC_GRAY, JPEG_SRC_YUV420, JPEG_SRC_YUV422, JPEG_SRC_BAYER = range(6)
 
 
+class RemapMap(ctypes.Structure):
+    """yfv2_remap_map: cv2's fixed remap maps in device memory, xy (CV_16SC2) and code (CV_16UC1)."""
+    _fields_ = [("xy", ctypes.c_void_p), ("xy_pitch", ctypes.c_longlong), ("code", ctypes.c_void_p),
+                ("code_pitch", ctypes.c_longlong), ("mw", ctypes.c_int), ("mh", ctypes.c_int)]
+
+
+class RemapFrame(ctypes.Structure):
+    """yfv2_remap_frame: the window (x0, y0, w, h) of cv2.remap of an inner frame (kind: YFV2_JPEG_SRC_*, not GRAY)."""
+    _fields_ = [("kind", ctypes.c_int), ("x0", ctypes.c_int), ("y0", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int),
+                ("f", _EncFrame), ("map", RemapMap)]
+
+
 class TrainerOp(ctypes.Structure):
     """yfv2_trainer_op: one op of the native trainer's program (test hook)."""
     _fields_ = [(f, ctypes.c_int) for f in ("kind", "a", "b", "y", "pw", "pg", "pb", "pbias", "bn", "relu", "ks", "stride", "M")] + \
@@ -330,6 +342,9 @@ PROTOTYPES = {
                                              ctypes.c_void_p]),
     "yfv2_resize_bayer_u8": (ctypes.c_int, [ctypes.POINTER(BayerFrame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                             ctypes.c_void_p]),
+    "yfv2_resize_remap_u8": (ctypes.c_int, [ctypes.POINTER(RemapFrame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                            ctypes.c_void_p]),
+    "yfv2_remap_u8": (ctypes.c_int, [ctypes.POINTER(RemapFrame), ctypes.c_int, ctypes.POINTER(ctypes.c_void_p), ctypes.c_void_p]),
     "yfv2_detect_u8_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                            ctypes.POINTER(ctypes.c_double), ctypes.c_float, ctypes.c_double, ctypes.c_int,
                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
@@ -1326,7 +1341,7 @@ _KIND = dict([("bgr", JPEG_SRC_BGR), ("gray", JPEG_SRC_GRAY)] + [(k, JPEG_SRC_YU
              + [(k, JPEG_SRC_STRIDED) for k in STRIDED_LAYOUTS if k != "gray"] + [(k, JPEG_SRC_YUV422) for k in YUV422_LAYOUTS]
              + [(k, JPEG_SRC_BAYER) for k in BAYER_LAYOUTS])
 _MEMBER = ("bgr", "strided", "strided", "yuv420", "yuv422", "bayer")
-_DESC = dict(_EncFrame._fields_)
+_DESC = dict(_EncFrame._fields_ + [("remap", RemapFrame)])
 
 
 class BayerWindow:
@@ -1343,9 +1358,113 @@ class BayerWindow:
         return "BayerWindow(raw %s, x0 %d, y0 %d, %dx%d)" % (tuple(self.raw.shape), self.x0, self.y0, self.w, self.h)
 
 
+REMAP_MAX_SIDE = 32766          # cv2.remap asserts map sides below SHRT_MAX
+
+
+def convert_maps(mx, my):
+    """cv2.convertMaps(mx, my, cv2.CV_16SC2) of float32 maps (torch tensors of one shape, on any device): (xy int16 [h, w, 2],
+    code int16 [h, w] holding cv2's uint16 map2).  X = rint_half_even(fl32(x * 32)), or INT32_MIN for NaN, +-inf and |x * 32| >=
+    2^31 (x86's cvRound); x0 = saturate_int16(X >> 5), j = X & 31; the same for y; code = 32 i + j.  The non-finite and huge
+    entries are masked before any float -> int cast, whose result for them differs between the CPU and the device."""
+    def fixed(v):
+        v = v * 32.0                                          # fp32, exact unless it overflows to inf (masked)
+        ok = torch.isfinite(v) & (v.abs() < 2.0 ** 31)
+        r = torch.round(torch.where(ok, v, torch.zeros_like(v))).to(torch.int64)     # half to even, as cvRound
+        r = torch.where(ok, r, torch.full_like(r, -2 ** 31))
+        return (r >> 5).clamp(-32768, 32767), r & 31
+    x0, j = fixed(mx)
+    y0, i = fixed(my)
+    return torch.stack([x0, y0], -1).to(torch.int16), (32 * i + j).to(torch.int16)
+
+
+def _map_tensor(m, what):
+    """A map plane as a torch tensor (numpy wrapped, not copied; uint16 viewed as int16) and whether it was unsigned."""
+    if isinstance(m, torch.Tensor):
+        if m.dtype == torch.uint16:
+            return m.view(torch.int16), True
+        return m, False
+    m = np.asarray(m)
+    if m.dtype == np.uint16:
+        return torch.from_numpy(np.ascontiguousarray(m).view(np.int16)), True
+    if m.dtype not in (np.float32, np.int16):
+        raise Yfv2Error("RemapMaps: %s must be float32, int16 or uint16 (cv2's map types), got %s" % (what, m.dtype))
+    return torch.from_numpy(m if min(m.strides, default=0) >= 0 else np.ascontiguousarray(m)), False
+
+
+class RemapMaps:
+    """cv2.remap's maps, held on a CUDA device in cv2's fixed form: xy int16 [mh, mw, 2] (CV_16SC2 map1) and code int16 [mh, mw]
+    (CV_16UC1 map2's bits), both contiguous.  Takes what cv2.remap takes for INTER_LINEAR, as numpy arrays or torch tensors:
+      float maps   map1, map2 float32 [h, w] (x and y), or map1 float32 [h, w, 2] with map2 None: converted once exactly as
+                   cv2.convertMaps(map1, map2, CV_16SC2) (convert_maps), so the remap gives cv2.remap's bytes for them;
+      fixed maps   map1 int16 [h, w, 2] and map2 uint16 (or int16) [h, w], what cv2.convertMaps or
+                   cv2.initUndistortRectifyMap(..., CV_16SC2) return: taken as they are (only map2's low 10 bits are read).
+    A fixed map and the conversion of the float map it was made from may differ (initUndistortRectifyMap rounds in fp64), so
+    pass the form whose cv2.remap bytes you want.  h, w in 1..32766, as cv2 requires.  device: where the maps are held (default:
+    map1's CUDA device, else the current one)."""
+    __slots__ = ("xy", "code", "mw", "mh")
+
+    def __init__(self, map1, map2=None, device=None):
+        m1, u1 = _map_tensor(map1, "map1")
+        m2, u2 = (None, False) if map2 is None else _map_tensor(map2, "map2")
+        if m1.dtype == torch.float32:
+            if m2 is None:
+                if m1.dim() != 3 or m1.shape[2] != 2:
+                    raise Yfv2Error("RemapMaps: a single float map must be float32 [h, w, 2], got %s" % (tuple(m1.shape),))
+                mx, my = m1[..., 0], m1[..., 1]
+            else:
+                if m2.dtype != torch.float32 or m1.dim() != 2 or tuple(m2.shape) != tuple(m1.shape):
+                    raise Yfv2Error("RemapMaps: float maps must be two float32 [h, w] planes of one shape, got %s %s and %s %s"
+                                    % (m1.dtype, tuple(m1.shape), m2.dtype, tuple(m2.shape)))
+                mx, my = m1, m2
+            xy, code = convert_maps(mx, my)
+        elif m1.dtype == torch.int16 and not u1:
+            if m1.dim() != 3 or m1.shape[2] != 2:
+                raise Yfv2Error("RemapMaps: a fixed map1 must be int16 [h, w, 2], got %s" % (tuple(m1.shape),))
+            if m2 is None or m2.dtype != torch.int16 or tuple(m2.shape) != tuple(m1.shape[:2]):
+                raise Yfv2Error("RemapMaps: a fixed map1 needs map2 uint16 [h, w] (its interpolation codes), got %s"
+                                % ("None" if m2 is None else "%s %s" % ("uint16" if u2 else m2.dtype, tuple(m2.shape))))
+            xy, code = m1, m2
+        else:
+            raise Yfv2Error("RemapMaps: map1 must be float32 or int16 (cv2's map types), got %s" % ("uint16" if u1 else m1.dtype))
+        mh, mw = xy.shape[:2]
+        if not (1 <= mw <= REMAP_MAX_SIDE and 1 <= mh <= REMAP_MAX_SIDE):
+            raise Yfv2Error("RemapMaps: map sides must be in 1..%d, got %dx%d" % (REMAP_MAX_SIDE, mw, mh))
+        if device is None:
+            device = m1.device if m1.is_cuda else torch.device("cuda", torch.cuda.current_device())
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise Yfv2Error("RemapMaps: maps are held on a CUDA device (no CPU fallback), got %s" % device)
+        self.xy, self.code = xy.to(device).contiguous(), code.to(device).contiguous()
+        self.mw, self.mh = int(mw), int(mh)
+
+    def __repr__(self):
+        return "RemapMaps(%dx%d on %s)" % (self.mw, self.mh, self.xy.device)
+
+
+class RemapView:
+    """The w x h window at (x0, y0) of cv2.remap(cv2.cvtColor(frame, COLOR_<LAYOUT>2BGR), map1, map2, cv2.INTER_LINEAR) (constant 0
+    border): a lens-corrected view of a frame, read where it is used, never stored.  frame: any frame resize_frames takes for the
+    layout (a BayerWindow or a crop included: the maps address its converted pixels); maps: a RemapMaps.  The layout passed with
+    a view names its frame's layout.  The window defaults to the whole remapped image (the map's size).  resize_frames,
+    remap_frames, encode_jpeg, crop_frame, frame_size and the detection and tracking helpers take views; boxes come back in the
+    view's pixels."""
+    __slots__ = ("frame", "maps", "x0", "y0", "w", "h")
+
+    def __init__(self, frame, maps, x0=0, y0=0, w=None, h=None):
+        if not isinstance(maps, RemapMaps):
+            raise Yfv2Error("RemapView: maps must be a RemapMaps, got %s" % type(maps).__name__)
+        self.frame, self.maps, self.x0, self.y0 = frame, maps, int(x0), int(y0)
+        self.w = maps.mw - self.x0 if w is None else int(w)
+        self.h = maps.mh - self.y0 if h is None else int(h)
+
+    def __repr__(self):
+        return "RemapView(%r, %r, x0 %d, y0 %d, %dx%d)" % (type(self.frame).__name__, self.maps, self.x0, self.y0, self.w, self.h)
+
+
 def frame_size(frame, layout):
-    """(h, w) in pixels of a frame in the given layout, as resize_frames takes it (of its window for a BayerWindow)."""
-    if isinstance(frame, BayerWindow):
+    """(h, w) in pixels of a frame in the given layout, as resize_frames takes it (of its window for a BayerWindow or a
+    RemapView)."""
+    if isinstance(frame, (BayerWindow, RemapView)):
         return frame.h, frame.w
     if layout in YUV420_LAYOUTS:
         if isinstance(frame, (tuple, list)):
@@ -1395,7 +1514,15 @@ def _bayer_window(f, layout, i, fn):
 def _check_frame(f, layout, i, fn):
     """Checks frame i against its layout without copying or launching anything; returns what _describe takes: the BGR array or
     tensor, the planes of a 4:2:0 frame, a BayerWindow over a tensor for Bayer, a uint8 tensor of the layout's shape for the
-    others.  A refusal names fn, the public function called."""
+    others, a RemapView over the checked frame for a view.  A refusal names fn, the public function called."""
+    if isinstance(f, RemapView):
+        if isinstance(f.frame, RemapView):
+            raise Yfv2Error("%s: frame %d: a RemapView of a RemapView (compose the maps instead)" % (fn, i))
+        m = f.maps
+        if f.w < 1 or f.h < 1 or f.x0 < 0 or f.y0 < 0 or f.x0 + f.w > m.mw or f.y0 + f.h > m.mh:
+            raise Yfv2Error("%s: frame %d (%s view): window (x0 %d, y0 %d, %dx%d) is not inside the %dx%d map"
+                            % (fn, i, layout, f.x0, f.y0, f.w, f.h, m.mw, m.mh))
+        return RemapView(_check_frame(f.frame, layout, i, fn), m, f.x0, f.y0, f.w, f.h)
     kind = _KIND[layout]
     if kind == JPEG_SRC_BAYER:
         return _bayer_window(f, layout, i, fn)
@@ -1428,13 +1555,18 @@ def _checked_frames(fn, frames, layout, allowed=_FRAME_LAYOUTS):
     return [_check_frame(f, lay, i, fn) for i, (f, lay) in enumerate(zip(frames, layouts))], layouts
 
 
+def _tensors(f):
+    """The arrays or tensors a checked frame reads: its planes, a BayerWindow's raw frame, a RemapView's frame and then its maps."""
+    if isinstance(f, RemapView):
+        return _tensors(f.frame) + (f.maps.xy,)
+    return f if isinstance(f, tuple) else (f.raw,) if isinstance(f, BayerWindow) else (f,)
+
+
 def _device(fn, frames, device):
     """The CUDA device a call runs on, with its index: `device`, else that of the first CUDA tensor among the checked frames (or
-    their planes), else the current one."""
+    their planes, or a view's maps), else the current one."""
     if device is None:
-        device = next((t.device for f in frames
-                       for t in (f if isinstance(f, tuple) else (f.raw,) if isinstance(f, BayerWindow) else (f,))
-                       if isinstance(t, torch.Tensor) and t.is_cuda), None)
+        device = next((t.device for f in frames for t in _tensors(f) if isinstance(t, torch.Tensor) and t.is_cuda), None)
     device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     if device.type != "cuda":
         raise Yfv2Error("%s: runs on CUDA devices only (no CPU fallback)" % fn)
@@ -1455,7 +1587,17 @@ def _describe(f, layout, device, keep):
     """The descriptor of frame f (as _check_frame returned it) with its pixels on `device`: a JpegEncSrc of the layout's kind, its
     union member filled and the whole frame as its region.  The only code that places frames: host frames are copied to
     `device`; a CUDA frame is read in place when its strides fit the descriptor, else a contiguous copy of it is.  The device
-    tensors read go to keep, which must hold them until the launch is queued: a freed block could take the next frame's copy."""
+    tensors read go to keep, which must hold them until the launch is queued: a freed block could take the next frame's copy.
+    For a RemapView: a RemapFrame of its frame's descriptor (grey as strided), its maps on `device` and its window."""
+    if isinstance(f, RemapView):
+        s = _describe(f.frame, layout, device, keep)
+        r = RemapFrame(JPEG_SRC_STRIDED if s.kind == JPEG_SRC_GRAY else s.kind, f.x0, f.y0, f.w, f.h)
+        r.f = s.f
+        xy, code = f.maps.xy.to(device), f.maps.code.to(device)
+        r.map.xy, r.map.xy_pitch, r.map.code, r.map.code_pitch = xy.data_ptr(), 4 * f.maps.mw, code.data_ptr(), 2 * f.maps.mw
+        r.map.mw, r.map.mh = f.maps.mw, f.maps.mh
+        keep += [xy, code]
+        return r
     kind = _KIND[layout]
     s = JpegEncSrc(kind)
     if kind == JPEG_SRC_BAYER:                                # the whole raw frame, any row stride, unit column stride
@@ -1523,18 +1665,24 @@ def _describe(f, layout, device, keep):
 
 def _resize(fn, frames, layout, allowed, W, H, device, out):
     """resize_bgr, resize_yuv420 and resize_frames: every frame checked, then one yfv2_resize_<member>_u8 call for each run of
-    consecutive frames that fill the same descriptor, each into its slice of out."""
+    consecutive frames that fill the same descriptor (RemapViews of any kind: yfv2_resize_remap_u8), each into its slice of out."""
     checked, layouts = _checked_frames(fn, frames, layout, allowed)
     device = _device(fn, checked, device)
     N = len(checked)
     out = _out(fn, out, N, H, W, device)
+
+    def member_of(k):
+        return "remap" if isinstance(checked[k], RemapView) else _MEMBER[_KIND[layouts[k]]]
+
     i = 0
     while i < N:
-        member, j = _MEMBER[_KIND[layouts[i]]], i + 1
-        while j < N and _MEMBER[_KIND[layouts[j]]] == member:
+        member, j = member_of(i), i + 1
+        while j < N and member_of(j) == member:
             j += 1
         keep, desc = [], _DESC[member]
         lo, hi = JpegEncSrc.f.offset, JpegEncSrc.f.offset + ctypes.sizeof(desc)     # the member's bytes in a JpegEncSrc
+        if member == "remap":
+            lo, hi = 0, ctypes.sizeof(desc)
         srcs = [bytes(_describe(checked[k], layouts[k], device, keep)) for k in range(i, j)]
         descs = (desc * (j - i)).from_buffer_copy(b"".join(src[lo:hi] for src in srcs))
         entry = getattr(lib(), "yfv2_resize_%s_u8" % member)
@@ -1557,11 +1705,31 @@ def resize_frames(frames, W, H, layout, device=None, out=None):
       "yuyv" | "uyvy" | "yvyu"          [h, w, 2] packed 4:2:2 (w even), COLOR_YUV2BGR_<LAYOUT>
       "bayer_bg" | "bayer_gb"           [h, w] raw Bayer (BAYER_LAYOUTS), COLOR_Bayer<XY>2BGR; "bayer_<xy>_ea": _EA, the
         | "bayer_rg" | "bayer_gr"       edge-aware demosaic; or a BayerWindow of one (crop_frame)
+    and a RemapView of a frame of any of these layouts (layout: its frame's): cv2.remap(INTER_LINEAR) of the converted frame,
+    cropped to the view's window, computed where the resize reads it (yfv2_resize_remap_u8).
     Frames are numpy arrays or CUDA tensors; CUDA views with larger row strides or crop offsets are read in place (for
     "rgb_chw" any channel and row stride with unit column stride), host arrays are copied to `device`.  Consecutive frames of
-    one descriptor kind go to one call (yfv2_resize_bgr_u8 / _yuv420_u8 / _strided_u8 / _yuv422_u8 / _bayer_u8), each into its
-    slice of `out`.  Every frame is checked before anything is copied or launched."""
+    one descriptor kind go to one call (yfv2_resize_bgr_u8 / _yuv420_u8 / _strided_u8 / _yuv422_u8 / _bayer_u8 / _remap_u8), each
+    into its slice of `out`.  Every frame is checked before anything is copied or launched."""
     return _resize("resize_frames", frames, layout, _FRAME_LAYOUTS, W, H, device, out)
+
+
+def remap_frames(views, layout, device=None):
+    """cv2.remap(cv2.cvtColor(frame, COLOR_<LAYOUT>2BGR), map1, map2, cv2.INTER_LINEAR)[y0:y0+h, x0:x0+w] of every RemapView, bit
+    for bit, computed on the device (yfv2_remap_u8): a list of CUDA uint8 [h, w, 3] BGR tensors.  layout: the views' frames'
+    layout, one name or one per view.  Every view is checked before anything is copied or launched."""
+    checked, layouts = _checked_frames("remap_frames", views, layout)
+    for i, v in enumerate(checked):
+        if not isinstance(v, RemapView):
+            raise Yfv2Error("remap_frames: frame %d is a %s, not a RemapView" % (i, type(views[i]).__name__))
+    device = _device("remap_frames", checked, device)
+    outs = [torch.empty((v.h, v.w, 3), dtype=torch.uint8, device=device) for v in checked]
+    keep = []
+    descs = (RemapFrame * len(checked))(*[_describe(v, lay, device, keep) for v, lay in zip(checked, layouts)])
+    dst = (ctypes.c_void_p * len(outs))(*[o.data_ptr() for o in outs])
+    with torch.cuda.device(device):
+        _check(lib().yfv2_remap_u8(descs, len(checked), dst, _stream(device)), "remap_u8")
+    return outs
 
 
 # cv2's IMWRITE_* ids and IMWRITE_JPEG_SAMPLING_FACTOR_* values (yfv2_jpeg_encode_plan reads the same pairs)
@@ -1609,6 +1777,18 @@ def encode_jpeg(frames, quality=95, sampling="420", restart_interval=0, layout="
         plist.append([IMWRITE_JPEG_QUALITY, int(qs[k]), IMWRITE_JPEG_SAMPLING_FACTOR, JPEG_SAMPLING[ss[k]],
                       IMWRITE_JPEG_RST_INTERVAL, int(rs[k])] + [int(x) for x in extra[k]])
     device = _device("encode_jpeg", checked, device)
+    # each RemapView an output reads: remapped once (remap_frames) and encoded as the BGR frame it gives
+    views = sorted({int(r[0]) for r in regions if isinstance(checked[int(r[0])], RemapView)})
+    for k, r in enumerate(regions):
+        v = checked[int(r[0])]
+        if isinstance(v, RemapView) and None not in r[3:]:
+            x0, y0, w, h = (int(a) for a in r[1:])
+            if w < 1 or h < 1 or x0 < 0 or y0 < 0 or x0 + w > v.w or y0 + h > v.h:
+                raise Yfv2Error("encode_jpeg: output %d: region (x0 %d, y0 %d, %dx%d) is not inside the %dx%d view"
+                                % (k, x0, y0, w, h, v.w, v.h))
+    if views:
+        for i, t in zip(views, remap_frames([checked[i] for i in views], [layouts[i] for i in views], device)):
+            checked[i], layouts[i] = t, "bgr"
     srcs = (JpegEncSrc * n)()
     keep, cparams, frame_src = [], [], {}
     for k, r in enumerate(regions):
@@ -1654,7 +1834,8 @@ def crop_frame(frame, layout, x0, y0, w, h):
     becomes a tuple of cropped planes, (y, uv) for NV12 / NV21 and (y, u, v) for I420 / YV12; x0, y0, w, h must then be even, so
     that the 2x2 chroma blocks of the crop are those of the frame.  Packed 4:2:2 needs even x0 and w (whole macropixels).  A Bayer
     frame, or a BayerWindow of one, becomes a BayerWindow of the whole raw frame (any offsets): the conversion of a pixel reads its
-    neighbours and the frame's edges, so the raw bytes are not cropped.  A crop of a crop is the crop of the frame."""
+    neighbours and the frame's edges, so the raw bytes are not cropped.  A RemapView becomes the RemapView of the window of its
+    remapped image (any offsets, whatever its frame's layout).  A crop of a crop is the crop of the frame."""
     if layout not in _FRAME_LAYOUTS:
         raise Yfv2Error("crop_frame: layout must be one of %s, got %r" % (", ".join(_FRAME_LAYOUTS), layout))
     f = _check_frame(frame, layout, 0, "crop_frame")
@@ -1662,6 +1843,8 @@ def crop_frame(frame, layout, x0, y0, w, h):
     x0, y0, w, h = int(x0), int(y0), int(w), int(h)
     if w < 1 or h < 1 or x0 < 0 or y0 < 0 or x0 + w > fw or y0 + h > fh:
         raise Yfv2Error("crop_frame: window (x0 %d, y0 %d, %dx%d) is not inside the %dx%d frame" % (x0, y0, w, h, fw, fh))
+    if isinstance(f, RemapView):                              # a window of the remapped image: any offsets, any layout
+        return RemapView(f.frame, f.maps, f.x0 + x0, f.y0 + y0, w, h)
     if layout in YUV420_LAYOUTS and (x0 | y0 | w | h) & 1:
         raise Yfv2Error("crop_frame: %s crops need even x0, y0, w and h (2x2 chroma blocks), got (x0 %d, y0 %d, %dx%d)"
                         % (layout, x0, y0, w, h))
