@@ -848,6 +848,16 @@ YFV2_API int yfv2_debug_pw_tc(const float* x, const float* w, float* out, float*
  * chunk, [5] resolve + append, [6] unused, [7] tail; [8] chunks, [9] candidates, [10] kept.  dev_buf: N x 16 int64 on the device. */
 YFV2_API int yfv2_debug_nms_profile(long long* dev_buf);
 
+/* ---- test hook: choose launches as another GPU would dispatch them ------------------------------------------------------------
+ * sms > 0: every launch decision that depends on the SM count (band heights, forward and training grids, augmentation grid caps,
+ * and yfv2_plan_debug_launches / yfv2_*_debug_launches called with sms = 0) takes sms instead of this device's count.
+ * persistent_ctas > 0: a persistent forward launch runs exactly min(items, persistent_ctas) CTAs instead of the grid occupancy
+ * allows; no persistent kernel synchronises across its grid, so more CTAs than can be resident is still correct.
+ * 0 turns a setting off; a negative one is refused with YFV2_EINVAL.  Both hold for every thread of the process (the autograd
+ * engine runs the trainer's backward on a thread of its own).  The native trainer captures its CUDA graphs again when either
+ * changes. */
+YFV2_API int yfv2_debug_set_dispatch(int sms, int persistent_ctas);
+
 #ifdef __cplusplus
 }
 #endif

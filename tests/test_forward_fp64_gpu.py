@@ -77,14 +77,16 @@ def sm_count():
     return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
 
 
-def setup(name):
+def setup(name, case=None, seed=None):
+    """model, state dict, input and checked images of case `name` of CASES, or of `case` (a CASES value) seeded by `seed`"""
     import model.detector as det
-    n, h, w, a, c, imgs = CASES[name]
-    sd = synth.make_state_dict(SEED[name], classes=c, anchor_num=a)
+    n, h, w, a, c, imgs = case or CASES[name]
+    seed = SEED[name] if seed is None else seed
+    sd = synth.make_state_dict(seed, classes=c, anchor_num=a)
     m = det.Detector(c, a, True)
     m.load_state_dict(sd, strict=True)
     m = m.cuda().eval()
-    x = synth.make_images(SEED[name] + 1, n, h, w).cuda()
+    x = synth.make_images(seed + 1, n, h, w).cuda()
     imgs = list(range(n)) if imgs is None else list(imgs)
     return m, sd, x, imgs
 

@@ -141,14 +141,16 @@ def nerr(got, ref, mag):
 
 
 # ---- one training step, every op checked --------------------------------------------------------------------------------------
-def run_step(name):
+def run_step(name, m=None):
+    """one training step of case `name`; m: the model of an earlier run_step of the case, to step its trainer again"""
     import model.detector as det
     import utils.loss as ul
     n, h, w, a, c = CASES[name]
-    sd = synth.make_state_dict(SEED[name], classes=c, anchor_num=a)
-    m = det.Detector(c, a, True)
-    m.load_state_dict(sd, strict=True)
-    m = m.cuda().train()
+    if m is None:
+        sd = synth.make_state_dict(SEED[name], classes=c, anchor_num=a)
+        m = det.Detector(c, a, True)
+        m.load_state_dict(sd, strict=True)
+        m = m.cuda().train()
     x = synth.make_images(SEED[name] + 1, n, h, w).cuda()
     targets = synth.make_targets(SEED[name] + 2, n, classes=c).cuda()
     cfg = synth.coco_cfg(w, h, c)
@@ -184,9 +186,10 @@ def site_name(o, tens):
     return "%s %dx%dx%d%s" % (o["kind"], c, h, w, extra)
 
 
-def check_case(name, cpu_check=False):
+def check_case(name, cpu_check=False, step=None):
+    """step: what run_step(name) returned, to check that step instead of running one"""
     n, h, w, a, c = CASES[name]
-    m, tr, bn_before = run_step(name)
+    m, tr, bn_before = step or run_step(name)
     ops, tens, layout = tr.program()
     assert [o["kind"] for o in ops] == [o["kind"] for o in td.program(n, h, w, a, c)[0]]
     params = [p.detach() for p in m.parameters()]

@@ -110,7 +110,8 @@ __device__ __forceinline__ void cp_async_wait_all() {
     asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;\n" ::: "memory");
 }
 
-int sm_count();
+int sm_count();                  // the device's SM count, or the one yfv2_debug_set_dispatch set
+int persistent_cta_cap();        // yfv2_debug_set_dispatch: CTAs of a persistent launch (at most one per item), 0: by occupancy
 constexpr size_t kSmemCap = 227 * 1024;
 
 // ---- programmatic dependent launch (PDL) ------------------------------------------------------------------

@@ -1253,9 +1253,13 @@ int launch(const Launch& L, const void* args, cudaStream_t s) {
     YFV2_CUDA(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
     dim3 grid = L.grid;
     if (L.persistent) {
-        int per_sm = 0;
-        YFV2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.fn, kThreads, L.smem));
-        const long long cap = (long long)(per_sm > 0 ? per_sm : 1) * L.grid.x;
+        // no persistent kernel synchronises across its grid, so a cap above what can be resident is still correct
+        long long cap = persistent_cta_cap();
+        if (!cap) {
+            int per_sm = 0;
+            YFV2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.fn, kThreads, L.smem));
+            cap = (long long)(per_sm > 0 ? per_sm : 1) * L.grid.x;
+        }
         grid.x = (unsigned)(L.items < cap ? L.items : cap);
     }
     YFV2_CUDA(launch_k(k.fn, grid, kThreads, L.smem, s, pdl_take(), args));

@@ -7,6 +7,7 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <atomic>
 #include <new>
 #include <vector>
 
@@ -37,7 +38,13 @@ bool pdl_take() { const bool r = g_pdl_next && g_pdl_call; g_pdl_next = true; re
 void pdl_reset() { g_pdl_next = false; }
 bool pdl_allowed() { return g_pdl_call; }
 
+// yfv2_debug_set_dispatch: the SM count the dispatch assumes (0: the device's) and the CTAs of a persistent launch (0: sized by
+// occupancy).  Process-wide, not per thread: the autograd engine runs the trainer's backward on a thread of its own.
+static std::atomic<int> g_sim_sms{0}, g_sim_ctas{0};
+int persistent_cta_cap() { return g_sim_ctas.load(); }
+
 int sm_count() {
+    if (const int s = g_sim_sms.load()) return s;
     static thread_local int n = 0;
     if (!n) {
         int dev = 0;
@@ -245,6 +252,16 @@ size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 extern "C" int yfv2_abi_version(void) { return YFV2_ABI_VERSION; }
 extern "C" const char* yfv2_last_error(void) { return g_err; }
+
+extern "C" int yfv2_debug_set_dispatch(int sms, int persistent_ctas) {
+    if (sms < 0 || persistent_ctas < 0) {
+        set_error("debug_set_dispatch: negative setting (sms=%d persistent_ctas=%d); 0 turns a setting off", sms, persistent_ctas);
+        return YFV2_EINVAL;
+    }
+    g_sim_sms = sms;
+    g_sim_ctas = persistent_ctas;
+    return YFV2_OK;
+}
 
 extern "C" int yfv2_plan_create(yfv2_plan** out, int device, int N, int H, int W, int A, int C, int training) {
     if (!out || N <= 0 || H <= 0 || W <= 0 || H % 32 || W % 32 || A <= 0 || A > 8 || C <= 0 || C > 256) {

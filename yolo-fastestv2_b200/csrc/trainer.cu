@@ -574,6 +574,9 @@ unsigned long long mix(unsigned long long h, unsigned long long v) {
     return h;
 }
 unsigned long long mix(unsigned long long h, const void* p) { return mix(h, (unsigned long long)reinterpret_cast<uintptr_t>(p)); }
+// the SM count and persistent-CTA cap the launches were described for (yfv2_debug_set_dispatch changes both): a graph captured
+// under another dispatch is not replayed
+unsigned long long dispatch_key(unsigned long long h) { return mix(mix(h, (unsigned long long)sm_count()), (unsigned long long)persistent_cta_cap()); }
 // Replays `slot` if it was captured for `key`; otherwise captures body() on the trainer's private stream, instantiates and replays.
 template <class Body>
 int replay_or_capture(yfv2_trainer* t, yfv2_trainer::GraphSlot& slot, unsigned long long key, cudaStream_t s, Body&& body) {
@@ -603,7 +606,7 @@ extern "C" int yfv2_train_forward(yfv2_trainer* t, const float* x, const float* 
     for (int i = 0; i < YFV2_NUM_PARAMS; ++i) if (!params[i]) { set_error("train_forward: null parameter %d", i); return YFV2_EINVAL; }
     for (int i = 0; i < 2 * YFV2_NUM_BN; ++i) if (!bn_running[i]) { set_error("train_forward: null BN buffer %d", i); return YFV2_EINVAL; }
     cudaStream_t s = (cudaStream_t)stream;
-    unsigned long long key = mix(mix(mix(0x1234ull, t->mode_hash), x), workspace);
+    unsigned long long key = mix(mix(mix(dispatch_key(0x1234ull), t->mode_hash), x), workspace);
     for (int i = 0; i < YFV2_NUM_PARAMS; ++i) key = mix(key, params[i]);
     for (int i = 0; i < 2 * YFV2_NUM_BN; ++i) key = mix(key, bn_running[i]);
     for (int i = 0; i < 6; ++i) key = mix(key, preds[i]);
@@ -627,7 +630,7 @@ extern "C" int yfv2_train_backward(yfv2_trainer* t, const float* x, const float*
         return YFV2_EINVAL;
     }
     cudaStream_t s = (cudaStream_t)stream;
-    unsigned long long key = mix(mix(mix(mix(0x4321ull, t->mode_hash), x), workspace), grads_flat);
+    unsigned long long key = mix(mix(mix(mix(dispatch_key(0x4321ull), t->mode_hash), x), workspace), grads_flat);
     for (int i = 0; i < YFV2_NUM_PARAMS; ++i) key = mix(key, params[i]);
     for (int i = 0; i < 6; ++i) key = mix(mix(key, preds[i]), dpreds[i]);
     return replay_or_capture(t, t->g_bwd[accumulate ? 1 : 0], key, s, [&](cudaStream_t cs) {

@@ -6,6 +6,7 @@ There is NO CPU fallback: if the library is missing or the tensors are not on a 
 raise.
 """
 import collections
+import contextlib
 import ctypes
 import os
 import threading
@@ -218,6 +219,24 @@ def op_launches(name, ptrs, ints, sms=0):
     return _train_launches(lambda out, cap, n: L.yfv2_op_debug_launches(TRAIN_OPS.index(name), p, i, sms, out, cap, n), "op_debug_launches")
 
 
+_dispatch = [(0, 0)]         # the (sms, ctas) simulated_dispatch last set (the library's setting is process-wide)
+
+
+@contextlib.contextmanager
+def simulated_dispatch(sms=0, ctas=0):
+    """Within the block, launches are chosen as on a GPU of `sms` SMs, and a persistent forward launch runs exactly min(items, ctas)
+    CTAs (yfv2_debug_set_dispatch; 0 leaves a setting off).  The setting holds for every thread of the process, the autograd
+    engine's included.  The previous setting is restored on exit, also when the block raises."""
+    L, prev = lib(), _dispatch[0]
+    _check(L.yfv2_debug_set_dispatch(sms, ctas), "debug_set_dispatch")
+    _dispatch[0] = (sms, ctas)
+    try:
+        yield
+    finally:
+        _check(L.yfv2_debug_set_dispatch(*prev), "debug_set_dispatch")
+        _dispatch[0] = prev
+
+
 def check_bn_batch(N, H, W):
     """F.batch_norm in training mode refuses a layer with one value per channel; the deepest BatchNorm layers of the network run
     at stride 32 (stem 3x3 s2, max-pool 3x3 s2 p1 and three stride-2 blocks: each (h - 1) // 2 + 1), the first of them on the
@@ -392,6 +411,7 @@ PROTOTYPES = {
     "yfv2_debug_gather": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
                                          ctypes.POINTER(ctypes.c_int), ctypes.c_void_p]),
     "yfv2_debug_nms_profile": (ctypes.c_int, [ctypes.c_void_p]),
+    "yfv2_debug_set_dispatch": (ctypes.c_int, [ctypes.c_int, ctypes.c_int]),
     "yfv2_op_debug_launches": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                               ctypes.POINTER(ctypes.c_int)]),
     "yfv2_trainer_debug_launches": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
