@@ -211,8 +211,11 @@ YFV2_API int yfv2_merge_regions(const float* dets, const int* counts, const yfv2
  * smaller side plays the solver's rows (the tracks on equal sizes).  (2) C[i][j] = c - thr if allowed, else 0.  (3) Crouse's
  * shortest augmenting path (scipy's linear_sum_assignment), rows in order; per row: SR = SC = {}, i = row, minVal = 0, shortest
  * = +inf; until an unassigned column is reached: SR += i; for j not in SC: r = ((minVal + C[i][j]) - u[i]) - v[j], if r <
- * shortest[j]: shortest[j] = r, path[j] = i; j* = the lowest j not in SC with the least shortest[j]; minVal = shortest[j*];
- * SC += j*; i = row4col[j*].  Then u[row] += minVal; u[i] += minVal - shortest[col4row[i]] for the other i in SR; v[j] -= minVal
+ * shortest[j]: shortest[j] = r, path[j] = i; j* = the lowest j not in SC with the least shortest[j] (-inf included; a NaN r
+ * never enters shortest, as NaN < x is false); minVal = shortest[j*]; SC += j*; i = row4col[j*].  Some j* < +inf always exists:
+ * the first step of row `row` gives every unassigned column shortest[j] = C[row][j] (u[row] and such a column's v are still
+ * 0), C is never +inf, and unassigned columns stay out of SC until one ends the path; so with confidences near DBL_MAX the duals
+ * may overflow to +-inf or NaN, but the argmin is never empty and this rule fixes every step.  Then u[row] += minVal; u[i] += minVal - shortest[col4row[i]] for the other i in SR; v[j] -= minVal
  * - shortest[j] for j in SC; augment along path.  (4) Assigned pairs that are not allowed stay unmatched.
  * One update of stream s: (1) frame += 1, predict every live track.  (2) stage 1, fused, thr = match_thresh: confirmed tracks
  * (tracked or lost) x high detections.  (3) stage 2, thr 0.5: confirmed tracked tracks unmatched by stage 1 x low detections.

@@ -2,8 +2,15 @@
 three association stages, each solved by Crouse's shortest augmenting path, and its track lifecycle with a constant-velocity
 Kalman filter in four decoupled 2x2 blocks.  Every value is a Python float and every operation one IEEE fp64 operation with one
 rounding, in the order the contract writes it, so the kernel must match this bit for bit.  min / max are `a < b ? a : b` /
-`a > b ? a : b`; a division by zero gives what IEEE gives (Python would raise)."""
+`a > b ? a : b`; a division by zero gives what IEEE gives (Python would raise).
+
+The stage costs, the solver's sweeps and dual updates and the duplicate rule also exist as numpy float64 operations over whole
+rows (np.where for min / max, never np.minimum / np.maximum, and IEEE division): the same operations on the same values, fast
+enough for 1024 x 2048 stages with long augmenting paths.  Tracker uses those by default; Tracker(scalar=True) runs the
+element-by-element form, and the tests hold the two equal."""
 import math
+
+import numpy as np
 
 INF = math.inf
 SP, SV = 1 / 20, 1 / 160
@@ -95,9 +102,26 @@ def update(t, z):
         c[3 * k + 2] = v - k1 * x
 
 
-def crouse(C, nr, nc):
-    """Crouse's shortest augmenting path on the nr x nc (nr <= nc) matrix C, rows in order, the argmin's ties to the lowest
-    column.  Returns col4row."""
+NT = 128                  # threads per CTA of k_track.cu: solver column j belongs to thread j % NT, warp (j % NT) // 32
+
+
+def argmin(shortest, sc):
+    """The argmin of one path step, the kernel's rule: start from (+inf, no column) and take an unvisited column only when its
+    shortest is strictly smaller, so the lowest column wins ties.  shortest is never NaN (it is only ever set by r < shortest),
+    and the first step of a path sets every free column below +inf (see yfv2.h), so a step without a candidate is a broken
+    contract: it raises."""
+    best, bj = INF, -1
+    for j in range(len(shortest)):
+        if not sc[j] and shortest[j] < best:
+            best, bj = shortest[j], j
+    if bj < 0:
+        raise AssertionError("argmin: no unvisited column below +inf")
+    return best, bj
+
+
+def crouse_scalar(C, nr, nc):
+    """Crouse's shortest augmenting path on the nr x nc (nr <= nc) matrix C, rows in order, element by element.  Returns
+    col4row."""
     u, v = [0.0] * nr, [0.0] * nc
     col4row, row4col = [-1] * nr, [-1] * nc
     for cur in range(nr):
@@ -106,16 +130,13 @@ def crouse(C, nr, nc):
         while sink < 0:
             SR.append(i)
             Ci, ui = C[i], u[i]
-            best, bj = INF, -1
             for j in range(nc):
                 if SC[j]:
                     continue
                 r = ((min_val + Ci[j]) - ui) - v[j]
                 if r < shortest[j]:
                     shortest[j], path[j] = r, i
-                if bj < 0 or shortest[j] < best:
-                    best, bj = shortest[j], j
-            min_val = best
+            min_val, bj = argmin(shortest, SC)
             SC[bj] = True
             if row4col[bj] < 0:
                 sink = bj
@@ -138,7 +159,73 @@ def crouse(C, nr, nc):
     return col4row
 
 
-def assign(cost, thr):
+def tie_kinds(cols):
+    """Which owners a tie among solver columns `cols` spans: "thread" (two columns of one thread), "lane" (two threads of one
+    warp), "warp" (two warps)."""
+    own = np.asarray(cols) % NT
+    kinds = set()
+    if len(np.unique(own)) < len(own):
+        kinds.add("thread")
+    warps = own // 32
+    for w in np.unique(warps):
+        if len(np.unique(own[warps == w])) > 1:
+            kinds.add("lane")
+    if len(np.unique(warps)) > 1:
+        kinds.add("warp")
+    return kinds
+
+
+def crouse(C, log=None):
+    """crouse_scalar with each relaxation sweep and dual update as numpy float64 operations over the columns: the same IEEE
+    operations on the same values.  C: float64 [nr, nc], nr <= nc.  log (a dict): steps of each row's path, the length of each
+    augmenting path, the owner kinds of every tie the argmin met, and whether a dual left the finite numbers."""
+    nr, nc = C.shape
+    u, v = np.zeros(nr), np.zeros(nc)
+    col4row, row4col = np.full(nr, -1), np.full(nc, -1)
+    steps, plen, ties = [], [], set()
+    with np.errstate(all="ignore"):
+        for cur in range(nr):
+            shortest, path, SC, SR = np.full(nc, INF), np.full(nc, -1), np.zeros(nc, bool), []
+            i, min_val, sink = cur, 0.0, -1
+            while sink < 0:
+                SR.append(i)
+                r = ((min_val + C[i]) - u[i]) - v
+                better = (r < shortest) & ~SC
+                shortest[better] = r[better]
+                path[better] = i
+                cand = np.where(SC, INF, shortest)
+                min_val = float(cand.min())
+                if not min_val < INF:
+                    raise AssertionError("argmin: no unvisited column below +inf (row %d, step %d)" % (cur, len(SR)))
+                tied = np.flatnonzero(cand == min_val)
+                bj = int(tied[0])
+                if len(tied) > 1:
+                    ties |= tie_kinds(tied)
+                SC[bj] = True
+                if row4col[bj] < 0:
+                    sink = bj
+                else:
+                    i = int(row4col[bj])
+            u[cur] = u[cur] + min_val
+            sr = np.asarray(SR[1:], int)
+            u[sr] = u[sr] + (min_val - shortest[col4row[sr]])
+            v[SC] = v[SC] - (min_val - shortest[SC])
+            j, n = sink, 0
+            while True:
+                i = int(path[j])
+                row4col[j] = i
+                col4row[i], j = j, int(col4row[i])
+                n += 1
+                if i == cur:
+                    break
+            steps.append(len(SR))
+            plen.append(n)
+    if log is not None:
+        log.update(steps=steps, plen=plen, ties=ties, nonfinite=not (np.isfinite(u).all() and np.isfinite(v).all()))
+    return col4row.tolist()
+
+
+def assign_scalar(cost, thr):
     """One association stage on cost[t][d] (tracks in ascending id x detections in row order): the reduction, the smaller side
     as rows, C = c - thr for allowed pairs (c < thr) else 0, Crouse, and the allowed assigned pairs.  Returns [(t, d)]."""
     nt = len(cost)
@@ -161,7 +248,7 @@ def assign(cost, thr):
             a, b = pair(i, j)
             row.append(cost[a][b] - thr if ok[a][b] else 0.0)
         C.append(row)
-    col4row = crouse(C, len(rows), len(cols))
+    col4row = crouse_scalar(C, len(rows), len(cols))
     out = []
     for i, j in enumerate(col4row):
         a, b = pair(i, j)
@@ -170,8 +257,64 @@ def assign(cost, thr):
     return out
 
 
-def stage_costs(tracks, dets, fused):
+def assign(cost, thr, log=None):
+    """assign_scalar on a float64 [nt, nd] array (or nested lists).  log (a dict) gets the sizes before and after the reduction,
+    the orientation tr (detections as rows) and what crouse logs."""
+    cost = np.asarray(cost, np.float64)
+    if cost.ndim != 2 or cost.size == 0:
+        return []
+    ok = cost < thr
+    rt, rd = np.flatnonzero(ok.any(1)), np.flatnonzero(ok.any(0))
+    if log is not None:
+        log.update(nt=cost.shape[0], nd=cost.shape[1], ntr=len(rt), ndr=len(rd))
+    if not len(rt):
+        return []
+    tr = len(rt) > len(rd)
+    sub, oks = cost[np.ix_(rt, rd)], ok[np.ix_(rt, rd)]
+    with np.errstate(all="ignore"):
+        C = np.where(oks, sub - thr, 0.0)
+    if tr:
+        C = np.ascontiguousarray(C.T)
+    if log is not None:
+        log.update(tr=bool(tr), nrow=C.shape[0], ncol=C.shape[1])
+    col4row = crouse(C, log)
+    out = []
+    for i, j in enumerate(col4row):
+        a, b = (rt[j], rd[i]) if tr else (rt[i], rd[j])
+        if ok[a, b]:
+            out.append((int(a), int(b)))
+    return out
+
+
+def iou_matrix(A, B):
+    """iou of every box of A [n, 4] (the tracks) with every box of B [m, 4], elementwise numpy with mn / mx as np.where and the
+    division IEEE's (what div restates)."""
+    def vmn(x, y):
+        return np.where(x < y, x, y)
+
+    def vmx(x, y):
+        return np.where(x > y, x, y)
+
+    a, b = A[:, None, :], B[None, :, :]
+    with np.errstate(all="ignore"):
+        iw = vmx(0.0, vmn(a[..., 2], b[..., 2]) - vmx(a[..., 0], b[..., 0]))
+        ih = vmx(0.0, vmn(a[..., 3], b[..., 3]) - vmx(a[..., 1], b[..., 1]))
+        inter = iw * ih
+        aa = (a[..., 2] - a[..., 0]) * (a[..., 3] - a[..., 1])
+        ab = (b[..., 2] - b[..., 0]) * (b[..., 3] - b[..., 1])
+        return inter / ((aa + ab) - inter)
+
+
+def stage_costs_scalar(tracks, dets, fused):
     return [[1.0 - (iou(t["box"], d["box"]) * d["conf"] if fused else iou(t["box"], d["box"])) for d in dets] for t in tracks]
+
+
+def stage_costs(tracks, dets, fused):
+    if not tracks or not dets:
+        return np.zeros((len(tracks), len(dets)))
+    q = iou_matrix(np.array([t["box"] for t in tracks], np.float64), np.array([d["box"] for d in dets], np.float64))
+    with np.errstate(all="ignore"):
+        return 1.0 - (q * np.array([d["conf"] for d in dets], np.float64) if fused else q)
 
 
 def finite(v):
@@ -181,8 +324,13 @@ def finite(v):
 class Tracker:
     """S streams of at most K tracks, as the device state holds them."""
 
-    def __init__(self, S, K, **params):
+    def __init__(self, S, K, scalar=False, log=False, **params):
+        """scalar: the element-by-element stage costs, solver and duplicate rule instead of the numpy ones.  log: keep in
+        self.log one dict per association stage (what assign logs, with the stream, frame and stage) and per duplicate rule
+        (the number of pairs)."""
         self.S, self.K = S, K
+        self.scalar = scalar
+        self.log = [] if log else None
         self.p = dict(DEFAULTS, **params)
         self.streams = [None] * S
         self.reset()
@@ -199,6 +347,7 @@ class Tracker:
         for b, s in enumerate(streams):
             M = len(dets[b])
             n = min(max(int(counts[b]), 0), M)
+            self._where = dict(stream=s)
             o, d = self._step(self.streams[s], [tuple(float(v) for v in dets[b][j]) for j in range(n)])
             rows.append(o)
             dropped.append(d)
@@ -221,14 +370,21 @@ class Tracker:
         lo = [d for d in dets if not d["high"]]
         kind = {id(t): (2 if t["state"] == LOST else (1 if t["confirmed"] else 0)) for t in tracks}
 
-        def stage(ts, ds, fused, thr):
-            for a, b in assign(stage_costs(ts, ds, fused), thr):
+        def stage(k, ts, ds, fused, thr):
+            if self.scalar:
+                pairs = assign_scalar(stage_costs_scalar(ts, ds, fused), thr)
+            else:
+                lg = None if self.log is None else dict(self._where, frame=frame, stage=k, thr=thr)
+                pairs = assign(stage_costs(ts, ds, fused), thr, lg)
+                if lg is not None:
+                    self.log.append(lg)
+            for a, b in pairs:
                 ts[a]["match"] = ds[b]
                 ds[b]["match"] = ts[a]
 
-        stage([t for t in tracks if kind[id(t)] != 0], hi, True, p["match_thresh"])
-        stage([t for t in tracks if kind[id(t)] == 1 and t["match"] is None], lo, False, STAGE2_THR)
-        stage([t for t in tracks if kind[id(t)] == 0], [d for d in hi if d["match"] is None], True, STAGE3_THR)
+        stage(1, [t for t in tracks if kind[id(t)] != 0], hi, True, p["match_thresh"])
+        stage(2, [t for t in tracks if kind[id(t)] == 1 and t["match"] is None], lo, False, STAGE2_THR)
+        stage(3, [t for t in tracks if kind[id(t)] == 0], [d for d in hi if d["match"] is None], True, STAGE3_THR)
         live = []
         for t in tracks:
             d = t["match"]
@@ -253,10 +409,17 @@ class Tracker:
             if t["state"] == LOST and frame - t["end_frame"] > p["max_age"]:
                 gone.add(id(t))
         dup = set()
-        for a in (t for t in live if t["state"] == TRACKED):
-            for b in (t for t in live if t["state"] == LOST and id(t) not in gone):
-                if iou(a["box"], b["box"]) > DUP_IOU:
-                    dup.add(id(b) if frame - a["start_frame"] > frame - b["start_frame"] else id(a))
+        tk = [t for t in live if t["state"] == TRACKED]
+        lo = [t for t in live if t["state"] == LOST and id(t) not in gone]
+        if self.scalar:
+            over = [(a, b) for a in tk for b in lo if iou(a["box"], b["box"]) > DUP_IOU]
+        else:
+            if self.log is not None:
+                self.log.append(dict(self._where, frame=frame, stage="dup", pairs=len(tk) * len(lo)))
+            q = iou_matrix(np.array([t["box"] for t in tk], np.float64).reshape(-1, 4), np.array([t["box"] for t in lo], np.float64).reshape(-1, 4))
+            over = [(tk[x], lo[y]) for x, y in zip(*np.nonzero(q > DUP_IOU))]
+        for a, b in over:
+            dup.add(id(b) if frame - a["start_frame"] > frame - b["start_frame"] else id(a))
         st["tracks"] = [t for t in live if id(t) not in gone and id(t) not in dup]
         out = [t["box"] + (t["score"], t["cls"], float(t["id"]), float(t["det_row"]))
                for t in st["tracks"] if t["state"] == TRACKED and t["confirmed"]]

@@ -251,6 +251,15 @@ __device__ __forceinline__ double pair_cost(const TrackSmem& s, int tk, int dj, 
 // One association stage: tracks rows[0, nt) (ranks, ascending id) against detections cols[0, nd) (rows, ascending).  Matches are
 // recorded in s.tm (by rank) and s.dm (by detection row).  Columns of the solver are owned by thread j % NT: shortest, path, sc
 // and v of a column are touched only by its owner while a path grows, so each step of a path costs one barrier (the argmin).
+//
+// The argmin starts from (+inf, INT_MAX) and takes only a strictly smaller shortest[j], so it needs a column below +inf at every
+// step.  There always is one, whatever the duals do: when row cur starts, u[cur] is 0 (only rows already processed change their
+// u) and so is v[j] of every unassigned column (only columns in SC change their v, and they all end assigned), so the first
+// sweep sets shortest[j] = C(cur, j) for each of the ncol - cur >= 1 unassigned columns; C is c - thr < 0 or 0, never +inf
+// (c = -inf, from a confidence near DBL_MAX, gives -inf); and no unassigned column enters SC before the one that ends the path.
+// shortest[j] is never NaN (NaN < x is false).  So with huge confidences the duals may reach +-inf or NaN and change which
+// optimum is found, but bj is always a real column and the rule of yfv2.h fixes it; tests/track_oracle.py raises if a step ever
+// found none.
 __device__ void associate(TrackSmem& s, const short* rows, int nt, const short* cols, int nd, bool fused, double thr) {
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     if (nt == 0 || nd == 0) return;

@@ -877,11 +877,13 @@ class Tracker:
         return idx, (ctypes.c_int * max(len(idx), 1))(*idx)
 
     def reset(self, streams=None):
-        """Clears the given streams (all by default): no tracks, frame 0, next id 1."""
-        idx, arr = self._streams(streams, self.S)
-        with torch.cuda.device(self.device):
-            _check(lib().yfv2_track_reset(ctypes.c_void_p(self.state.data_ptr()), self.S, self.K, arr, len(idx), _stream(self.device)),
-                   "Tracker.reset")
+        """Clears the given streams (all by default, in calls of at most TRACK_MAX_BATCH streams): no tracks, frame 0, next id 1."""
+        calls = [range(b, min(b + TRACK_MAX_BATCH, self.S)) for b in range(0, self.S, TRACK_MAX_BATCH)] if streams is None else [streams]
+        for part in calls:
+            idx, arr = self._streams(part, self.S)
+            with torch.cuda.device(self.device):
+                _check(lib().yfv2_track_reset(ctypes.c_void_p(self.state.data_ptr()), self.S, self.K, arr, len(idx), _stream(self.device)),
+                       "Tracker.reset")
 
     def update(self, dets, counts, streams=None):
         """One frame for each of B distinct streams (streams: B stream indices; None: 0..B-1), in one launch without a host
