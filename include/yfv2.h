@@ -468,6 +468,51 @@ YFV2_API int yfv2_resize_remap_u8(const yfv2_remap_frame* frames, int N, int H, 
  * 3*w apart), with the per-pixel arithmetic of yfv2_resize_remap_u8.  dst: N HOST pointers.  Checked as yfv2_resize_remap_u8. */
 YFV2_API int yfv2_remap_u8(const yfv2_remap_frame* frames, int N, uint8_t* const* dst, void* stream);
 
+/* ---- rotated, de-skewed and bird's-eye views -> network input: cv2.warpAffine / cv2.warpPerspective (INTER_LINEAR) ------------
+ * What a rotated mount, a de-skew or a ground-plane rectification does before detection: img = cv2.warpAffine(cv2.cvtColor(frame,
+ * code), M, (dw, dh)) for a 2x3 M (perspective 0), cv2.warpPerspective(..., M, (dw, dh)) for a 3x3 M (perspective 1, whatever its
+ * last row), with the default BORDER_CONSTANT 0, and WARP_INVERSE_MAP when inverse is 1.  A descriptor stands for the window
+ * (x0, y0, w, h) of img; yfv2_resize_warp_u8 gives the bytes of cv2.resize(img[y0:y0+h, x0:x0+w], (W, H), INTER_LINEAR),
+ * transposed to CHW, and yfv2_warp_u8 the window itself.  No map is stored: each coordinate is computed where it is read.
+ * M is the matrix as given to cv2 (row-major, m[6..8] unused for affine).  Without inverse it is inverted once per call on the
+ * host, as cv2 does: affine by warpAffine's closed form (D = 1 / (m0 m4 - m1 m3); m0, m4 = m4 D, m0 D; m1 *= -D; m3 *= -D;
+ * m2, m5 = -m0 m2 - m1 m5, -m3 m2 - m4 m5 with the new values), perspective as cv2.invert(M, DECOMP_LU) for 3x3 (cofactors
+ * times 1 / det3).  With m the destination -> source matrix, all in fp64 in this order with no fused multiply-add, output pixel
+ * (x, y) reads the fixed-point source coordinate (X, Y) in 1/32 pixel:
+ *   affine       X = (cvRound((m1 y + m2) 1024) + 16 + cvRound((m0 x) 1024)) >> 5, Y the same with m3, m4, m5;
+ *   perspective  W = (m7 y + m8) + m6 x, W = W ? 32 / W : 0, X = cvRound(clamp(((m1 y + m2) + m0 x) W, INT_MIN, INT_MAX)),
+ *                Y the same with m3, m4, m5 (a W of exactly 0 samples source (0, 0) with code 0, as cv2 does);
+ * cvRound rounds half to even.  (sat_short(X >> 5), sat_short(Y >> 5)) and code (Y & 31) * 32 + (X & 31) are then sampled as
+ * yfv2_resize_remap_u8 samples a map entry.  DESIGN.md §19 states it; tests/warp_oracle.py restates it.
+ * Refused before any launch, besides the inner frame's checks (kind as in yfv2_remap_frame): a non-finite entry of M or of its
+ * inverse; a singular M that must be inverted (determinant 0); perspective or inverse not 0 or 1; dw, dh outside 1..32767; a
+ * window empty or outside the dw x dh output; and an affine view where |(m0 x) 1024|, |(m1 y + m2) 1024| or the same terms of
+ * Y reach 2^30 at any output x, y (cv2's int32 sums would overflow; the terms are linear, so the end points bound them).
+ * Each descriptor carries its own matrix: a batch of differently warped frames of one kind is one launch. */
+typedef struct yfv2_warp_frame {
+    int kind;              /* YFV2_JPEG_SRC_* of the inner frame, not YFV2_JPEG_SRC_GRAY */
+    int x0, y0, w, h;      /* the window of the warped image this descriptor stands for */
+    union {
+        yfv2_frame bgr;
+        yfv2_strided_frame strided;
+        yfv2_yuv420_frame yuv420;
+        yfv2_yuv422_frame yuv422;
+        yfv2_bayer_frame bayer;
+    } f;                   /* the inner frame, in device memory */
+    double m[9];           /* the matrix as given to cv2, row-major: 2x3 in m[0..5], or 3x3 */
+    int perspective;       /* 0: warpAffine, 1: warpPerspective */
+    int inverse;           /* 1: m is already destination -> source (cv2.WARP_INVERSE_MAP) */
+    int dw, dh;            /* dsize: the warped image's size */
+} yfv2_warp_frame;
+YFV2_API int yfv2_resize_warp_u8(const yfv2_warp_frame* frames, int N, int H, int W, uint8_t* dst, void* stream);
+/* The warp alone: the window of frame n's warped image written as packed HWC BGR to dst[n] (device, h*w*3 bytes, rows 3*w apart).
+ * dst: N HOST pointers.  Checked as yfv2_resize_warp_u8. */
+YFV2_API int yfv2_warp_u8(const yfv2_warp_frame* frames, int N, uint8_t* const* dst, void* stream);
+/* The destination -> source matrix a checked descriptor samples with (host only, nothing launched): m_out[9] gets M itself with
+ * inverse, else its inversion as above (affine: m_out[6..8] = 0, 0, 1).  Refuses what yfv2_resize_warp_u8 refuses of the
+ * descriptor, the inner frame excepted (it is not read). */
+YFV2_API int yfv2_warp_matrix(const yfv2_warp_frame* frame, double* m_out);
+
 /* ---- JPEG files -> packed HWC BGR frames: cv2.imread(path) (test.py:34; utils/datasets.py:106) on the device -----------------
  * The bytes OpenCV 4.13 (libjpeg-turbo 3.1) returns for IMREAD_COLOR: ISLOW IDCT, fancy upsampling, jdcolor's YCbCr -> BGR, grey
  * replicated to B = G = R, and the EXIF orientation applied.  Supported: baseline sequential Huffman-coded DCT (SOF0, SOF1) with

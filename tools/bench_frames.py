@@ -286,6 +286,110 @@ def remap_main(args):
                                 % (N - 1)}), flush=True)
 
 
+def warp_main(args):
+    """--warp: warped views (yfv2_resize_warp_u8) of N fh x fw frames, for BGR, NV12 and BAYER_BG frames, each frame with its own
+    matrix: a rotation of a few degrees (warpAffine) and a de-skew homography (warpPerspective), both dsize = the frame's.  Per
+    layout and run, L2 flushed before each launch and the paths alternated: affine_us and persp_us (the fused warp + resize
+    launch), two_pass_us (yfv2_warp_u8 of the perspective views into BGR frames, then yfv2_resize_bgr_u8: warp_frames + resize),
+    remap_us (yfv2_resize_remap_u8 through the oracle's fixed maps of the same perspective warp, one map shared by all frames:
+    RemapView with precomputed maps) and plain_us (the layout's own resize, no warp).  Parity: frames 0 and N-1 of the fused,
+    two-pass and remap paths against tests/warp_oracle.py."""
+    import yfv2  # noqa: F401
+    import yfv2_engine as eng
+    import remap_oracle as ro
+    import warp_cases as wc
+    import warp_oracle as wo
+    fw, fh = (int(v) for v in args.frame.lower().split("x"))
+    N, S = args.batch, bench.SIDE
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    L = eng.lib()
+    stream = torch.cuda.current_stream(dev)
+    sp = ctypes.c_void_p(stream.cuda_stream)
+    rs = np.random.RandomState(7)
+    affine = [wc.rotation(fw / 2, fh / 2, rs.uniform(-5, 5), rs.uniform(0.95, 1.05)) for _ in range(N)]
+    persp = [wc.quad_homography(fw, fh, rs.uniform(-0.06, 0.06, (4, 2))) for _ in range(N)]
+    shared = persp[0]
+    pm, pv = wo.dst_to_src(shared, False)
+    maps = eng.RemapMaps(*wo.warp_maps(pv, pm, 0, 0, fw, fh), dev)
+    x = torch.empty((N, 3, S, S), dtype=torch.uint8, device=dev)
+    inter = torch.empty((N, fh, fw, 3), dtype=torch.uint8, device=dev)          # the two-pass path's warped BGR frames
+    inter_descs = (eng.Frame * N)()
+    for i in range(N):
+        inter_descs[i].data, inter_descs[i].w, inter_descs[i].h, inter_descs[i].pitch = inter[i].data_ptr(), fw, fh, 3 * fw
+    inter_ptrs = (ctypes.c_void_p * N)(*[inter[i].data_ptr() for i in range(N)])
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)     # 256 MB > L2
+    g = torch.Generator(device=dev).manual_seed(3)
+
+    def ok(rc_):
+        if rc_:
+            raise RuntimeError(L.yfv2_last_error())
+
+    results = {}
+    for layout in ("bgr", "nv12", "bayer_bg"):
+        shape = (fh, fw, 3) if layout == "bgr" else (fh * 3 // 2, fw) if layout == "nv12" else (fh, fw)
+        frames = torch.randint(0, 256, (N,) + shape, generator=g, dtype=torch.uint8, device=dev)
+        keep = []
+        plain = [eng._describe(eng._check_frame(frames[i], layout, i, "bench"), layout, dev, keep) for i in range(N)]
+        member = eng._MEMBER[eng._KIND[layout]]
+        desc = eng._DESC[member]
+        lo, hi = eng.JpegEncSrc.f.offset, eng.JpegEncSrc.f.offset + ctypes.sizeof(desc)
+        plain_descs = (desc * N).from_buffer_copy(b"".join(bytes(s)[lo:hi] for s in plain))
+        plain_entry = getattr(L, "yfv2_resize_%s_u8" % member)
+
+        def descs(cls, items):
+            views = [eng._check_frame(cls(frames[i], *items[i]), layout, i, "bench") for i in range(N)]
+            return (eng._DESC["warp" if cls is eng.WarpView else "remap"] * N)(*[eng._describe(v, layout, dev, keep) for v in views])
+        a_descs = descs(eng.WarpView, [(M, (fw, fh)) for M in affine])
+        p_descs = descs(eng.WarpView, [(M, (fw, fh)) for M in persp])
+        r_descs = descs(eng.RemapView, [(maps,)] * N)
+        paths = {
+            "affine": lambda: ok(L.yfv2_resize_warp_u8(a_descs, N, S, S, ctypes.c_void_p(x.data_ptr()), sp)),
+            "persp": lambda: ok(L.yfv2_resize_warp_u8(p_descs, N, S, S, ctypes.c_void_p(x.data_ptr()), sp)),
+            "two_pass": lambda: (ok(L.yfv2_warp_u8(p_descs, N, inter_ptrs, sp)),
+                                 ok(L.yfv2_resize_bgr_u8(inter_descs, N, S, S, ctypes.c_void_p(x.data_ptr()), sp))),
+            "remap": lambda: ok(L.yfv2_resize_remap_u8(r_descs, N, S, S, ctypes.c_void_p(x.data_ptr()), sp)),
+            "plain": lambda: ok(plain_entry(plain_descs, N, S, S, ctypes.c_void_p(x.data_ptr()), sp)),
+        }
+        for _ in range(max(args.warmup, 3)):
+            for fn in paths.values():
+                fn()
+        torch.cuda.synchronize(dev)
+        for name, mats in (("affine", affine), ("persp", persp), ("two_pass", persp), ("remap", [shared] * N)):
+            paths[name]()
+            got = x[[0, N - 1]].cpu().numpy()
+            for k, i in enumerate((0, N - 1)):
+                img = ro.inner_bgr(frames[i].cpu().numpy(), layout)
+                want = wo.resize_planar(img, mats[i], (fw, fh), None, S, S)
+                if not np.array_equal(got[k], want):
+                    raise AssertionError("bench_frames --warp parity: %s %s frame %d differs from the oracle" % (layout, name, i))
+        runs = []
+        for _ in range(args.runs):
+            tot = dict.fromkeys(paths, 0.0)
+            reps = max(5, min(args.steps, 20))
+            for _ in range(reps):
+                for name, fn in paths.items():
+                    flush.zero_()
+                    tot[name] += events_ms(fn, 1, stream)
+            runs.append({name + "_us": round(1e3 * t / reps, 1) for name, t in tot.items()})
+        results[layout] = runs
+        del frames, keep, plain
+    power = None
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        power = pynvml.nvmlDeviceGetPowerManagementLimit(pynvml.nvmlDeviceGetHandleByIndex(0)) / 1000.0
+    except Exception:
+        pass
+    print(json.dumps({"metric": "warped %dx%d frames -> %dx%d input, fused vs warp_frames + resize vs remap maps" % (fw, fh, S, S),
+                      "batch": N, "steps": args.steps, "runs": results, "device": torch.cuda.get_device_name(dev),
+                      "power_limit_w": power,
+                      "timing": "CUDA events; frames resident in HBM; L2 flushed before each launch; paths alternated; a matrix "
+                                "per frame for affine and persp; remap: one shared map of the first perspective warp",
+                      "parity": "frames 0 and %d of the fused, two-pass and remap paths equal tests/warp_oracle.py byte for byte"
+                                % (N - 1)}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -298,7 +402,12 @@ def main():
                                                         "bayer_bg_ea", "bayer_gb_ea", "bayer_rg_ea", "bayer_gr_ea"),
                     help="source frame format")
     ap.add_argument("--remap", action="store_true", help="lens-corrected views of bgr, nv12 and bayer_bg frames (remap_main)")
+    ap.add_argument("--warp", action="store_true", help="warped views of bgr, nv12 and bayer_bg frames (warp_main)")
     args = ap.parse_args()
+    if args.warp:
+        if not torch.cuda.is_available():
+            raise SystemExit("bench_frames.py: no CUDA device (the product path has no CPU fallback)")
+        return warp_main(args)
     if args.remap:
         if not torch.cuda.is_available():
             raise SystemExit("bench_frames.py: no CUDA device (the product path has no CPU fallback)")

@@ -13,8 +13,11 @@
 //   raw Bayer frames (yfv2_resize_bayer_u8), each source pixel demosaiced as cv2.cvtColor(COLOR_Bayer??2BGR / _EA) does, in
 //   integers on the 3x3 raw neighbourhood of its clamped frame coordinate (resize.cuh's BayerSource, tests/bayer_oracle.py);
 //   lens-corrected views of any of these (yfv2_resize_remap_u8): each source pixel is cv2.remap(INTER_LINEAR)'s pixel of the
-//   inner frame (resize.cuh's RemapSource over the inner fetch, remap_pixel), one instantiation per inner kind.
-// yfv2_remap_u8 writes the remapped windows alone (remap_kernel), with the same remap_pixel.
+//   inner frame (resize.cuh's RemapSource over the inner fetch, remap_pixel), one instantiation per inner kind;
+//   rotated, de-skewed and bird's-eye views of any of these (yfv2_resize_warp_u8): each source pixel is cv2.warpAffine's or
+//   cv2.warpPerspective's pixel of the inner frame, its fixed-point coordinate computed from the descriptor's matrix where it is
+//   read (resize.cuh's WarpSource, warp_pixel), sampled by remap_pixel's own sample_fixed.
+// yfv2_remap_u8 and yfv2_warp_u8 write the views' windows alone (remap_kernel, warp_kernel), with the same per-pixel functions.
 // The resize is bit-identical to OpenCV's x86 8-bit path, all integer after the coefficients:
 //   coefficients per axis: f = fl32((d + 0.5) * (n / m) - 0.5) (product and difference rounded in double), s = floor(f),
 //     f = fl32(f - s); weights rint(fl32(1 - f) * 2048), rint(f * 2048).  Along x, s < 0 -> (0, 0) then s >= w - 1 -> (w - 1, 0);
@@ -209,16 +212,18 @@ int resize_entry(const char* fn, const typename Src::Desc* frames, int N, int H,
     return launch_resize<Src>(frames, N, H, W, dst, stream);
 }
 
-// cv2.remap alone: one thread per pixel of the window of frame blockIdx.z's remapped image, written as packed HWC BGR
-template <class Inner>
-struct RemapChunk {
-    RemapDesc<Inner> src[RemapSource<Inner>::kChunk];
-    uint8_t* dst[RemapSource<Inner>::kChunk];
+// A view alone (yfv2_remap_u8, yfv2_warp_u8): one thread per pixel of the window of frame blockIdx.z's view, written as packed
+// HWC BGR to its own dst
+template <class Src>
+struct ViewChunk {
+    typename Src::Desc src[Src::kChunk];
+    uint8_t* dst[Src::kChunk];
 };
 
+// cv2.remap alone
 template <class Inner>
 __global__ void __launch_bounds__(kResizeBx * kResizeBy)
-remap_kernel(const __grid_constant__ RemapChunk<Inner> a) {
+remap_kernel(const __grid_constant__ ViewChunk<RemapSource<Inner>> a) {
     const RemapDesc<Inner>& fr = a.src[blockIdx.z];
     const int x = blockIdx.x * kResizeBx + threadIdx.x;
     const int y = blockIdx.y * kResizeBy + threadIdx.y;
@@ -230,55 +235,103 @@ remap_kernel(const __grid_constant__ RemapChunk<Inner> a) {
     for (int c = 0; c < 3; ++c) out[c] = (uint8_t)v[c];
 }
 
-// The inner frame of a checked remap descriptor, as Inner's descriptor
-template <class Inner> const typename Inner::Desc& inner_of(const yfv2_remap_frame& f);
-template <> const yfv2_frame& inner_of<BgrSource>(const yfv2_remap_frame& f) { return f.f.bgr; }
-template <> const yfv2_strided_frame& inner_of<StridedSource>(const yfv2_remap_frame& f) { return f.f.strided; }
-template <> const yfv2_yuv420_frame& inner_of<Yuv420Source>(const yfv2_remap_frame& f) { return f.f.yuv420; }
-template <> const yfv2_yuv422_frame& inner_of<Yuv422Source>(const yfv2_remap_frame& f) { return f.f.yuv422; }
-template <> const yfv2_bayer_frame& inner_of<BayerSource>(const yfv2_remap_frame& f) { return f.f.bayer; }
-
-// frames[0, n), all of Inner's kind, RemapSource<Inner>::kChunk per launch: with dst the fused resize into dst's H x W images,
-// else the remap alone into dst_each[i]
+// cv2.warpAffine / cv2.warpPerspective alone
 template <class Inner>
-int launch_remap(const yfv2_remap_frame* frames, int n, int H, int W, uint8_t* dst, uint8_t* const* dst_each, cudaStream_t stream) {
-    constexpr int kChunk = RemapSource<Inner>::kChunk;
+__global__ void __launch_bounds__(kResizeBx * kResizeBy)
+warp_kernel(const __grid_constant__ ViewChunk<WarpSource<Inner>> a) {
+    const WarpDesc<Inner>& fr = a.src[blockIdx.z];
+    const int x = blockIdx.x * kResizeBx + threadIdx.x;
+    const int y = blockIdx.y * kResizeBy + threadIdx.y;
+    if (x >= fr.w || y >= fr.h) return;
+    int v[3];
+    warp_pixel<Inner>(fr, fr.x0 + x, fr.y0 + y, v);
+    uint8_t* out = a.dst[blockIdx.z] + 3 * ((size_t)y * fr.w + x);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out[c] = (uint8_t)v[c];
+}
+
+// The inner frame of a checked view descriptor (remap or warp), as Inner's descriptor
+template <class Inner> struct InnerOf;
+template <> struct InnerOf<BgrSource> { template <class F> static const yfv2_frame& get(const F& f) { return f.f.bgr; } };
+template <> struct InnerOf<StridedSource> { template <class F> static const yfv2_strided_frame& get(const F& f) { return f.f.strided; } };
+template <> struct InnerOf<Yuv420Source> { template <class F> static const yfv2_yuv420_frame& get(const F& f) { return f.f.yuv420; } };
+template <> struct InnerOf<Yuv422Source> { template <class F> static const yfv2_yuv422_frame& get(const F& f) { return f.f.yuv422; } };
+template <> struct InnerOf<BayerSource> { template <class F> static const yfv2_bayer_frame& get(const F& f) { return f.f.bayer; } };
+
+// What the two view entries differ in: the source of the fused resize, the device descriptor of a checked host one, the kernel of
+// the view alone, and how a refused descriptor is described
+template <class Frame> struct ViewOf;
+template <> struct ViewOf<yfv2_remap_frame> {
+    template <class Inner> using Src = RemapSource<Inner>;
+    template <class Inner> static RemapDesc<Inner> desc(const yfv2_remap_frame& fr) {
+        return RemapDesc<Inner>{InnerOf<Inner>::get(fr), fr.map, fr.x0, fr.y0, fr.w, fr.h};
+    }
+    template <class Inner> static void launch_alone(dim3 grid, dim3 block, cudaStream_t s, const ViewChunk<Src<Inner>>& a) {
+        remap_kernel<Inner><<<grid, block, 0, s>>>(a);
+    }
+    static void refuse(const char* fn, int n, const char* why, const yfv2_remap_frame& f) {
+        set_error("%s: frame %d: %s (window %dx%d of a %dx%d map)", fn, n, why, f.w, f.h, f.map.mw, f.map.mh);
+    }
+};
+template <> struct ViewOf<yfv2_warp_frame> {
+    template <class Inner> using Src = WarpSource<Inner>;
+    template <class Inner> static WarpDesc<Inner> desc(const yfv2_warp_frame& fr) {
+        WarpDesc<Inner> d{InnerOf<Inner>::get(fr), {}, fr.perspective, fr.x0, fr.y0, fr.w, fr.h};
+        warp_matrix_fault(fr, d.m);                             // checked: the destination -> source matrix
+        return d;
+    }
+    template <class Inner> static void launch_alone(dim3 grid, dim3 block, cudaStream_t s, const ViewChunk<Src<Inner>>& a) {
+        warp_kernel<Inner><<<grid, block, 0, s>>>(a);
+    }
+    static void refuse(const char* fn, int n, const char* why, const yfv2_warp_frame& f) {
+        set_error("%s: frame %d: %s (window (%d, %d) %dx%d of a %dx%d %s warp)", fn, n, why, f.x0, f.y0, f.w, f.h, f.dw, f.dh,
+                  f.perspective == 1 ? "perspective" : "affine");
+    }
+};
+
+// frames[0, n), all of Inner's kind, Src<Inner>::kChunk per launch: with dst the fused resize into dst's H x W images, else the
+// view alone into dst_each[i]
+template <class Frame, class Inner>
+int launch_view(const Frame* frames, int n, int H, int W, uint8_t* dst, uint8_t* const* dst_each, cudaStream_t stream) {
+    using V = ViewOf<Frame>;
+    using Src = typename V::template Src<Inner>;
+    constexpr int kChunk = Src::kChunk;
     const dim3 block(kResizeBx, kResizeBy);
     for (int n0 = 0; n0 < n; n0 += kChunk) {
         const int cnt = n - n0 < kChunk ? n - n0 : kChunk;
-        RemapDesc<Inner> d[kChunk];
+        typename Src::Desc d[kChunk];
         int mw = 1, mh = 1;
         for (int i = 0; i < cnt; ++i) {
-            const yfv2_remap_frame& fr = frames[n0 + i];
-            d[i] = RemapDesc<Inner>{inner_of<Inner>(fr), fr.map, fr.x0, fr.y0, fr.w, fr.h};
+            const Frame& fr = frames[n0 + i];
+            d[i] = V::template desc<Inner>(fr);
             mw = fr.w > mw ? fr.w : mw;
             mh = fr.h > mh ? fr.h : mh;
         }
         if (dst) {
-            ResizeChunk<RemapSource<Inner>> a{};
+            ResizeChunk<Src> a{};
             for (int i = 0; i < cnt; ++i) a.src[i] = d[i];
             a.dst = dst + (size_t)n0 * 3 * H * W;
             a.H = H; a.W = W;
             const dim3 grid((unsigned)((W + kResizeBx - 1) / kResizeBx), (unsigned)((H + kResizeBy - 1) / kResizeBy), (unsigned)cnt);
-            resize_kernel<RemapSource<Inner>><<<grid, block, 0, stream>>>(a);
+            resize_kernel<Src><<<grid, block, 0, stream>>>(a);
         } else {
-            RemapChunk<Inner> a{};
+            ViewChunk<Src> a{};
             for (int i = 0; i < cnt; ++i) {
                 a.src[i] = d[i];
                 a.dst[i] = dst_each[n0 + i];
             }
             const dim3 grid((unsigned)((mw + kResizeBx - 1) / kResizeBx), (unsigned)((mh + kResizeBy - 1) / kResizeBy), (unsigned)cnt);
-            remap_kernel<Inner><<<grid, block, 0, stream>>>(a);
+            V::template launch_alone<Inner>(grid, block, stream, a);
         }
         YFV2_LAUNCH_CHECK();
     }
     return YFV2_OK;
 }
 
-// Both remap entries: the call's checks, each frame's (frame_fault), then one launch_remap per run of consecutive frames of one
-// kind, so that no kernel branches on the kind.  dst (the fused resize, H x W) or dst_each (the remap alone) is non-null.
-int remap_entry(const char* fn, const yfv2_remap_frame* frames, int N, int H, int W, uint8_t* dst, uint8_t* const* dst_each,
-                void* stream) {
+// The remap and warp entries: the call's checks, each frame's (frame_fault), then one launch_view per run of consecutive frames
+// of one kind, so that no kernel branches on the kind.  dst (the fused resize, H x W) or dst_each (the view alone) is non-null.
+template <class Frame>
+int view_entry(const char* fn, const Frame* frames, int N, int H, int W, uint8_t* dst, uint8_t* const* dst_each, void* stream) {
     if (!frames || (!dst && !dst_each) || N <= 0) { set_error("%s: null frames / dst or N <= 0", fn); return YFV2_EINVAL; }
     if (dst && (H <= 0 || W <= 0 || H > kResizeMaxSide || W > kResizeMaxSide)) {
         set_error("%s: target %dx%d outside 1..%d", fn, W, H, kResizeMaxSide);
@@ -286,8 +339,7 @@ int remap_entry(const char* fn, const yfv2_remap_frame* frames, int N, int H, in
     }
     for (int n = 0; n < N; ++n) {
         if (const char* why = frame_fault(frames[n])) {
-            set_error("%s: frame %d: %s (window %dx%d of a %dx%d map)", fn, n, why, frames[n].w, frames[n].h, frames[n].map.mw,
-                      frames[n].map.mh);
+            ViewOf<Frame>::refuse(fn, n, why, frames[n]);
             return YFV2_EINVAL;
         }
         if (dst_each && !dst_each[n]) { set_error("%s: frame %d: null dst", fn, n); return YFV2_EINVAL; }
@@ -300,11 +352,11 @@ int remap_entry(const char* fn, const yfv2_remap_frame* frames, int N, int H, in
         uint8_t* const* de = dst_each ? dst_each + i : nullptr;
         int rc = YFV2_OK;
         switch (frames[i].kind) {
-            case YFV2_JPEG_SRC_BGR: rc = launch_remap<BgrSource>(frames + i, j - i, H, W, d, de, s); break;
-            case YFV2_JPEG_SRC_STRIDED: rc = launch_remap<StridedSource>(frames + i, j - i, H, W, d, de, s); break;
-            case YFV2_JPEG_SRC_YUV420: rc = launch_remap<Yuv420Source>(frames + i, j - i, H, W, d, de, s); break;
-            case YFV2_JPEG_SRC_YUV422: rc = launch_remap<Yuv422Source>(frames + i, j - i, H, W, d, de, s); break;
-            default: rc = launch_remap<BayerSource>(frames + i, j - i, H, W, d, de, s); break;   // kinds checked above
+            case YFV2_JPEG_SRC_BGR: rc = launch_view<Frame, BgrSource>(frames + i, j - i, H, W, d, de, s); break;
+            case YFV2_JPEG_SRC_STRIDED: rc = launch_view<Frame, StridedSource>(frames + i, j - i, H, W, d, de, s); break;
+            case YFV2_JPEG_SRC_YUV420: rc = launch_view<Frame, Yuv420Source>(frames + i, j - i, H, W, d, de, s); break;
+            case YFV2_JPEG_SRC_YUV422: rc = launch_view<Frame, Yuv422Source>(frames + i, j - i, H, W, d, de, s); break;
+            default: rc = launch_view<Frame, BayerSource>(frames + i, j - i, H, W, d, de, s); break;   // kinds checked above
         }
         if (rc != YFV2_OK) return rc;
         i = j;
@@ -337,11 +389,27 @@ extern "C" int yfv2_resize_bayer_u8(const yfv2_bayer_frame* frames, int N, int H
 }
 
 extern "C" int yfv2_resize_remap_u8(const yfv2_remap_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
-    return yfv2::remap_entry("resize_remap_u8", frames, N, H, W, dst, nullptr, stream);
+    return yfv2::view_entry("resize_remap_u8", frames, N, H, W, dst, nullptr, stream);
 }
 
 extern "C" int yfv2_remap_u8(const yfv2_remap_frame* frames, int N, uint8_t* const* dst, void* stream) {
-    return yfv2::remap_entry("remap_u8", frames, N, 0, 0, nullptr, dst, stream);
+    return yfv2::view_entry("remap_u8", frames, N, 0, 0, nullptr, dst, stream);
+}
+
+extern "C" int yfv2_resize_warp_u8(const yfv2_warp_frame* frames, int N, int H, int W, uint8_t* dst, void* stream) {
+    return yfv2::view_entry("resize_warp_u8", frames, N, H, W, dst, nullptr, stream);
+}
+
+extern "C" int yfv2_warp_u8(const yfv2_warp_frame* frames, int N, uint8_t* const* dst, void* stream) {
+    return yfv2::view_entry("warp_u8", frames, N, 0, 0, nullptr, dst, stream);
+}
+
+extern "C" int yfv2_warp_matrix(const yfv2_warp_frame* frame, double* m_out) {
+    if (!frame || !m_out) { yfv2::set_error("warp_matrix: null frame or m_out"); return YFV2_EINVAL; }
+    double m[9];
+    if (const char* why = yfv2::warp_matrix_fault(*frame, m)) { yfv2::set_error("warp_matrix: %s", why); return YFV2_EINVAL; }
+    for (int k = 0; k < 9; ++k) m_out[k] = m[k];
+    return YFV2_OK;
 }
 
 namespace yfv2 {

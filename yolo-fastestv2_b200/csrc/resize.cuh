@@ -5,6 +5,7 @@
 // checks of their descriptors.
 #pragma once
 #include <climits>
+#include <cmath>
 #include <stdint.h>
 
 namespace yfv2 {
@@ -73,6 +74,67 @@ inline const char* frame_fault(const yfv2_remap_frame& f) {
     if ((why = frame_fault(f.map))) return why;
     if (f.w < 1 || f.h < 1 || f.x0 < 0 || f.y0 < 0 || (long long)f.x0 + f.w > f.map.mw || (long long)f.y0 + f.h > f.map.mh)
         return "window empty or outside the map";
+    return nullptr;
+}
+
+// The destination -> source matrix of a warp descriptor in m (9 values), inverted as cv2 inverts it, or why the descriptor is
+// refused; its inner frame is not checked.  Host code: each line is one IEEE double operation (no x86-64 host compiler fuses
+// them without FMA enabled, and tests/test_warp_cpu.py pins the results to cv2's own bits).
+inline const char* warp_matrix_fault(const yfv2_warp_frame& f, double (&m)[9]) {
+    if (f.perspective & ~1) return "perspective must be 0 or 1";
+    if (f.inverse & ~1) return "inverse must be 0 or 1";
+    if (f.dw < 1 || f.dh < 1 || f.dw > 32767 || f.dh > 32767) return "dw and dh must be in 1..32767";
+    const int n = f.perspective ? 9 : 6;
+    for (int k = 0; k < n; ++k)
+        if (!std::isfinite(f.m[k])) return "matrix entries must be finite";
+    for (int k = 0; k < 9; ++k) m[k] = k < n ? f.m[k] : k == 8 ? 1.0 : 0.0;
+    if (!f.inverse && !f.perspective) {                       // warpAffine's inversion
+        double D = m[0] * m[4] - m[1] * m[3];
+        if (D == 0) return "singular matrix (determinant 0)";
+        D = 1. / D;
+        const double A11 = m[4] * D, A22 = m[0] * D;
+        m[0] = A11; m[1] *= -D;
+        m[3] *= -D; m[4] = A22;
+        const double b1 = -m[0] * m[2] - m[1] * m[5];
+        const double b2 = -m[3] * m[2] - m[4] * m[5];
+        m[2] = b1; m[5] = b2;
+    } else if (!f.inverse) {                                  // cv2.invert(M, DECOMP_LU) of a 3x3 matrix
+        const double* a = f.m;
+        double d = a[0] * (a[4] * a[8] - a[5] * a[7]) - a[1] * (a[3] * a[8] - a[5] * a[6]) + a[2] * (a[3] * a[7] - a[4] * a[6]);
+        if (d == 0) return "singular matrix (determinant 0)";
+        d = 1. / d;
+        m[0] = (a[4] * a[8] - a[5] * a[7]) * d; m[1] = (a[2] * a[7] - a[1] * a[8]) * d; m[2] = (a[1] * a[5] - a[2] * a[4]) * d;
+        m[3] = (a[5] * a[6] - a[3] * a[8]) * d; m[4] = (a[0] * a[8] - a[2] * a[6]) * d; m[5] = (a[2] * a[3] - a[0] * a[5]) * d;
+        m[6] = (a[3] * a[7] - a[4] * a[6]) * d; m[7] = (a[1] * a[6] - a[0] * a[7]) * d; m[8] = (a[0] * a[4] - a[1] * a[3]) * d;
+    }
+    for (int k = 0; k < 9; ++k)
+        if (!std::isfinite(m[k])) return "the inverse has non-finite entries";
+    if (!f.perspective) {                                     // every scaled term below 2^30: the int32 sums cannot overflow
+        const double lim = 1073741824.0;
+        for (int e = 0; e < 2; ++e) {
+            const double x = e ? f.dw - 1 : 0, y = e ? f.dh - 1 : 0;
+            if (std::fabs((m[0] * x) * 1024) >= lim || std::fabs((m[3] * x) * 1024) >= lim ||
+                std::fabs((m[1] * y + m[2]) * 1024) >= lim || std::fabs((m[4] * y + m[5]) * 1024) >= lim)
+                return "affine coordinates reach 2^30 / 1024 pixels (cv2's int32 sums would overflow)";
+        }
+    }
+    return nullptr;
+}
+inline const char* frame_fault(const yfv2_warp_frame& f) {
+    const char* why = "kind must be YFV2_JPEG_SRC_BGR, _STRIDED, _YUV420, _YUV422 or _BAYER";
+    switch (f.kind) {
+        case YFV2_JPEG_SRC_BGR: why = frame_fault(f.f.bgr); break;
+        case YFV2_JPEG_SRC_STRIDED: why = frame_fault(f.f.strided); break;
+        case YFV2_JPEG_SRC_YUV420: why = frame_fault(f.f.yuv420); break;
+        case YFV2_JPEG_SRC_YUV422: why = frame_fault(f.f.yuv422); break;
+        case YFV2_JPEG_SRC_BAYER: why = frame_fault(f.f.bayer); break;
+        default: break;
+    }
+    if (why) return why;
+    double m[9];
+    if ((why = warp_matrix_fault(f, m))) return why;
+    if (f.w < 1 || f.h < 1 || f.x0 < 0 || f.y0 < 0 || (long long)f.x0 + f.w > f.dw || (long long)f.y0 + f.h > f.dh)
+        return "window empty or outside the output";
     return nullptr;
 }
 
@@ -232,17 +294,15 @@ struct BayerSource {
     }
 };
 
-// cv2.remap(INTER_LINEAR, BORDER_CONSTANT 0) of an Inner frame through fixed maps: pixel (mx, my) of the remapped image, B, G,
-// R in v.  cv2's weights for code (i, j) are rint(fl32(fl32(1 - i/32) * fl32(1 - j/32)) * 32768) and so on; every factor is a
-// multiple of 1/32, so each product is exact and the weights are the integers 32 (32 - i)(32 - j) ..., already summing to 32768
-// (initInterTab2D's correction never fires; tests/remap_oracle.py computes the table cv2's way and checks this).  A tap outside
-// the inner frame's w x h weighs 0, and its fetch reads the clamped coordinate, so Inner is never read out of range; the two
-// columns of a fetch stay equal or adjacent, as BayerSource needs.
+// cv2.remap(INTER_LINEAR, BORDER_CONSTANT 0)'s sampling of an Inner frame at one fixed-point entry: integer source pixel (X, Y)
+// and interpolation code k (0..1023), B, G, R in v.  cv2's weights for code (i, j) are rint(fl32(fl32(1 - i/32) *
+// fl32(1 - j/32)) * 32768) and so on; every factor is a multiple of 1/32, so each product is exact and the weights are the
+// integers 32 (32 - i)(32 - j) ..., already summing to 32768 (initInterTab2D's correction never fires; tests/remap_oracle.py
+// computes the table cv2's way and checks this).  A tap outside the inner frame's w x h weighs 0, and its fetch reads the clamped
+// coordinate, so Inner is never read out of range; the two columns of a fetch stay equal or adjacent, as BayerSource needs.
+// remap_pixel (a map entry) and warp_pixel (a computed coordinate) share it.
 template <class Inner>
-__device__ __forceinline__ void remap_pixel(const typename Inner::Desc& f, const yfv2_remap_map& m, int mx, int my, int (&v)[3]) {
-    const int xy = __ldg((const int*)((const uint8_t*)m.xy + (long long)my * m.xy_pitch) + mx);    // 4-byte aligned: checked
-    const int X = (int)(int16_t)(xy & 0xffff), Y = xy >> 16;
-    const int k = __ldg((const uint16_t*)((const uint8_t*)m.code + (long long)my * m.code_pitch) + mx) & 1023;
+__device__ __forceinline__ void sample_fixed(const typename Inner::Desc& f, int X, int Y, int k, int (&v)[3]) {
     const int i = k >> 5, j = k & 31;
     const int w = f.w, h = f.h;
     const bool x0in = (unsigned)X < (unsigned)w, x1in = (unsigned)(X + 1) < (unsigned)w;
@@ -263,6 +323,72 @@ __device__ __forceinline__ void remap_pixel(const typename Inner::Desc& f, const
     for (int c = 0; c < 3; ++c)
         v[c] = sat_u8(((by0 * (p00[c] * ax0 + p01[c] * ax1) + by1 * (p10[c] * ax0 + p11[c] * ax1)) * 32 + 16384) >> 15);
 }
+
+// cv2.remap(INTER_LINEAR, BORDER_CONSTANT 0) of an Inner frame through fixed maps: pixel (mx, my) of the remapped image, B, G,
+// R in v
+template <class Inner>
+__device__ __forceinline__ void remap_pixel(const typename Inner::Desc& f, const yfv2_remap_map& m, int mx, int my, int (&v)[3]) {
+    const int xy = __ldg((const int*)((const uint8_t*)m.xy + (long long)my * m.xy_pitch) + mx);    // 4-byte aligned: checked
+    const int k = __ldg((const uint16_t*)((const uint8_t*)m.code + (long long)my * m.code_pitch) + mx) & 1023;
+    sample_fixed<Inner>(f, (int)(int16_t)(xy & 0xffff), xy >> 16, k, v);
+}
+
+// A warped view's descriptor on the device: the inner frame, the destination -> source matrix (inverted on the host), whether
+// it is a perspective one, and the window of the warped image (w, h: the resize's source size)
+template <class Inner>
+struct WarpDesc {
+    typename Inner::Desc f;
+    double m[9];
+    int perspective;
+    int x0, y0, w, h;
+};
+
+// cvRound of a perspective coordinate: std::max(INT_MIN, std::min(INT_MAX, v)) as cv2 writes it (a NaN becomes INT_MAX), then
+// half to even
+__device__ __forceinline__ int clamp_round(double v) {
+    v = v < 2147483647.0 ? v : 2147483647.0;
+    v = -2147483648.0 < v ? v : -2147483648.0;
+    return __double2int_rn(v);
+}
+
+// cv2.warpAffine / cv2.warpPerspective(INTER_LINEAR, BORDER_CONSTANT 0) of an Inner frame: pixel (x, y) of the warped image, B,
+// G, R in v.  The fixed-point coordinate is computed here in cv2's order of fp64 operations (yfv2.h states them), each rounded
+// on its own (__dmul_rn / __dadd_rn: no FMA contraction), then sampled as a remap map entry.
+template <class Inner>
+__device__ __forceinline__ void warp_pixel(const WarpDesc<Inner>& d, int x, int y, int (&v)[3]) {
+    const double* m = d.m;
+    const double dx = (double)x, dy = (double)y;
+    int X, Y;
+    if (!d.perspective) {                     // cvRound((m1 y + m2) 1024) + 16 + cvRound((m0 x) 1024), >> 5; |terms| < 2^30
+        X = (__double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[1], dy), m[2]), 1024.0)) + 16 +
+             __double2int_rn(__dmul_rn(__dmul_rn(m[0], dx), 1024.0))) >> 5;
+        Y = (__double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[4], dy), m[5]), 1024.0)) + 16 +
+             __double2int_rn(__dmul_rn(__dmul_rn(m[3], dx), 1024.0))) >> 5;
+    } else {
+        double W = __dadd_rn(__dadd_rn(__dmul_rn(m[7], dy), m[8]), __dmul_rn(m[6], dx));
+        W = W != 0.0 ? __ddiv_rn(32.0, W) : 0.0;
+        X = clamp_round(__dmul_rn(__dadd_rn(__dadd_rn(__dmul_rn(m[1], dy), m[2]), __dmul_rn(m[0], dx)), W));
+        Y = clamp_round(__dmul_rn(__dadd_rn(__dadd_rn(__dmul_rn(m[4], dy), m[5]), __dmul_rn(m[3], dx)), W));
+    }
+    const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767);
+    sample_fixed<Inner>(d.f, sx, sy, ((Y & 31) << 5) + (X & 31), v);
+}
+
+// Pixels of the window of cv2.warpAffine / cv2.warpPerspective(inner frame), each computed from the inner frame where it is read
+template <class Inner>
+struct WarpSource {
+    using Desc = WarpDesc<Inner>;
+    // frames per launch: each descriptor, plus yfv2_warp_u8's output pointer, under the 4 KB launch limit with the chunk's rest
+    static constexpr int kChunk = 4000 / (int)(sizeof(Desc) + sizeof(void*));
+    static constexpr int kMinBlocks = 0;
+    const Desc& f;
+    int y;
+    __device__ __forceinline__ WarpSource(const Desc& f_, int r) : f(f_), y(f_.y0 + r) {}
+    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
+        warp_pixel<Inner>(f, f.x0 + c0, y, p0);
+        warp_pixel<Inner>(f, f.x0 + c1, y, p1);
+    }
+};
 
 // A remapped view's descriptor on the device: the inner frame, the map and the window (w, h: the resize's source size)
 template <class Inner>

@@ -46,9 +46,10 @@ def detect_frames(model, frames, cfg, conf_thres=0.3, iou_thres=0.4, layout="bgr
     layout: one of yfv2_engine.LAYOUTS or BAYER_LAYOUTS, or a list with one per frame; the frames are what resize_frames takes for
     it ("bgr": HWC uint8 numpy arrays or CUDA tensors of any sizes; "nv12" | "nv21" | "i420" | "yv12": cv2's single [h*3/2, w]
     buffer or a tuple of planes; "rgb", "bgra" / "rgba", "gray", "rgb_chw" [3, h, w], "yuyv" / "uyvy" / "yvyu" [h, w, 2]; the
-    Bayer layouts [h, w] raw frames or a BayerWindow of one; or a yfv2_engine.RemapView of any of these, its lens-corrected view),
-    converted as cv2.cvtColor(COLOR_<LAYOUT>2BGR) does.  The boxes come back in pixels of each frame's h x w (the luma plane for
-    YUV, the window for a BayerWindow, the corrected view for a RemapView)."""
+    Bayer layouts [h, w] raw frames or a BayerWindow of one; or a yfv2_engine.RemapView of any of these, its lens-corrected view,
+    or a yfv2_engine.WarpView, its rotated, de-skewed or bird's-eye view), converted as cv2.cvtColor(COLOR_<LAYOUT>2BGR) does.  The
+    boxes come back in pixels of each frame's h x w (the luma plane for YUV, the window for a BayerWindow, the view's window for a
+    RemapView or WarpView)."""
     frames = list(frames)
     layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
     x = resize_frames(frames, cfg["width"], cfg["height"], layouts, next(model.parameters()).device)
@@ -173,10 +174,12 @@ def detect_regions(model, frames, cfg, regions, conf_thres=0.3, iou_thres=0.4, l
 
 
 def _on_device(f, layout, dev):
-    """A frame (or tuple of planes, BayerWindow or RemapView) as CUDA tensors on `dev`: host arrays copied once, CUDA tensors as
-    they are."""
+    """A frame (or tuple of planes, BayerWindow, RemapView or WarpView) as CUDA tensors on `dev`: host arrays copied once, CUDA
+    tensors as they are."""
     if isinstance(f, yfv2_engine.RemapView):
         return yfv2_engine.RemapView(_on_device(f.frame, layout, dev), f.maps, f.x0, f.y0, f.w, f.h)
+    if isinstance(f, yfv2_engine.WarpView):
+        return f.over(_on_device(f.frame, layout, dev), f.x0, f.y0, f.w, f.h)
     if isinstance(f, yfv2_engine.BayerWindow):
         return yfv2_engine.BayerWindow(_on_device(f.raw, layout, dev), f.x0, f.y0, f.w, f.h)
     if isinstance(f, (tuple, list)):
@@ -188,15 +191,16 @@ def _on_device(f, layout, dev):
 
 
 def detect_tiled(model, frames, cfg, cols, rows, overlap=0.2, full_frame=True, **kw):
-    """detect_regions over tile_regions(w, h, cols, rows, overlap, full_frame, layout) of each frame's size (for a RemapView, tiles
-    of the remapped image, not rounded whatever its frame's layout)."""
+    """detect_regions over tile_regions(w, h, cols, rows, overlap, full_frame, layout) of each frame's size (for a RemapView or
+    WarpView, tiles of the remapped or warped image, not rounded whatever its frame's layout)."""
     frames = list(frames)
     layout = kw.get("layout", "bgr")
     layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
     regions = []
     for f, lay in zip(frames, layouts):
         h, w = frame_size(f, lay)
-        regions.append(tile_regions(w, h, cols, rows, overlap, full_frame, "bgr" if isinstance(f, yfv2_engine.RemapView) else lay))
+        view = isinstance(f, (yfv2_engine.RemapView, yfv2_engine.WarpView))
+        regions.append(tile_regions(w, h, cols, rows, overlap, full_frame, "bgr" if view else lay))
     return detect_regions(model, frames, cfg, regions, **kw)
 
 

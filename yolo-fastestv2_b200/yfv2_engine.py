@@ -83,6 +83,13 @@ class RemapFrame(ctypes.Structure):
                 ("f", _EncFrame), ("map", RemapMap)]
 
 
+class WarpFrame(ctypes.Structure):
+    """yfv2_warp_frame: the window (x0, y0, w, h) of cv2.warpAffine / cv2.warpPerspective (dsize dw x dh) of an inner frame."""
+    _fields_ = [("kind", ctypes.c_int), ("x0", ctypes.c_int), ("y0", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int),
+                ("f", _EncFrame), ("m", ctypes.c_double * 9), ("perspective", ctypes.c_int), ("inverse", ctypes.c_int),
+                ("dw", ctypes.c_int), ("dh", ctypes.c_int)]
+
+
 class TrainerOp(ctypes.Structure):
     """yfv2_trainer_op: one op of the native trainer's program (test hook)."""
     _fields_ = [(f, ctypes.c_int) for f in ("kind", "a", "b", "y", "pw", "pg", "pb", "pbias", "bn", "relu", "ks", "stride", "M")] + \
@@ -364,6 +371,10 @@ PROTOTYPES = {
     "yfv2_resize_remap_u8": (ctypes.c_int, [ctypes.POINTER(RemapFrame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                             ctypes.c_void_p]),
     "yfv2_remap_u8": (ctypes.c_int, [ctypes.POINTER(RemapFrame), ctypes.c_int, ctypes.POINTER(ctypes.c_void_p), ctypes.c_void_p]),
+    "yfv2_resize_warp_u8": (ctypes.c_int, [ctypes.POINTER(WarpFrame), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                           ctypes.c_void_p]),
+    "yfv2_warp_u8": (ctypes.c_int, [ctypes.POINTER(WarpFrame), ctypes.c_int, ctypes.POINTER(ctypes.c_void_p), ctypes.c_void_p]),
+    "yfv2_warp_matrix": (ctypes.c_int, [ctypes.POINTER(WarpFrame), ctypes.POINTER(ctypes.c_double)]),
     "yfv2_detect_u8_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                            ctypes.POINTER(ctypes.c_double), ctypes.c_float, ctypes.c_double, ctypes.c_int,
                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
@@ -1363,7 +1374,7 @@ _KIND = dict([("bgr", JPEG_SRC_BGR), ("gray", JPEG_SRC_GRAY)] + [(k, JPEG_SRC_YU
              + [(k, JPEG_SRC_STRIDED) for k in STRIDED_LAYOUTS if k != "gray"] + [(k, JPEG_SRC_YUV422) for k in YUV422_LAYOUTS]
              + [(k, JPEG_SRC_BAYER) for k in BAYER_LAYOUTS])
 _MEMBER = ("bgr", "strided", "strided", "yuv420", "yuv422", "bayer")
-_DESC = dict(_EncFrame._fields_ + [("remap", RemapFrame)])
+_DESC = dict(_EncFrame._fields_ + [("remap", RemapFrame), ("warp", WarpFrame)])
 
 
 class BayerWindow:
@@ -1483,10 +1494,79 @@ class RemapView:
         return "RemapView(%r, %r, x0 %d, y0 %d, %dx%d)" % (type(self.frame).__name__, self.maps, self.x0, self.y0, self.w, self.h)
 
 
+WARP_MAX_SIDE = 32767
+
+
+def _warp_desc(m, perspective, inverse, dsize, x0=0, y0=0, w=1, h=1):
+    """A WarpFrame of the matrix, output size and window, its inner frame left empty."""
+    d = WarpFrame(0, x0, y0, w, h)
+    d.m[:] = list(m) + [0.0] * (9 - len(m))
+    d.perspective, d.inverse, (d.dw, d.dh) = int(perspective), int(inverse), dsize
+    return d
+
+
+def warp_matrix(M, inverse=False):
+    """The destination -> source matrix (float64 [3, 3]) cv2.warpAffine (M 2x3) or cv2.warpPerspective (M 3x3) samples with: M
+    itself with inverse (WARP_INVERSE_MAP), else M inverted on the host as cv2 inverts it, bit for bit (yfv2_warp_matrix).  Raises
+    Yfv2Error for what a WarpView of M refuses (a singular M, non-finite entries)."""
+    m, perspective = _warp_entries(M, "warp_matrix")
+    out = (ctypes.c_double * 9)()
+    d = _warp_desc(m, perspective, inverse, (1, 1))
+    if lib().yfv2_warp_matrix(ctypes.byref(d), out):
+        raise Yfv2Error(lib().yfv2_last_error().decode())
+    return np.array(list(out), np.float64).reshape(3, 3)
+
+
+def _warp_entries(M, fn):
+    """M (a 2x3 or 3x3 numpy array or nested list) as a tuple of its float64 values, and whether it is 3x3."""
+    try:
+        a = np.array(M, dtype=np.float64)
+    except (TypeError, ValueError):
+        raise Yfv2Error("%s: M must be a 2x3 or 3x3 matrix of numbers, got %r" % (fn, type(M).__name__))
+    if a.shape not in ((2, 3), (3, 3)):
+        raise Yfv2Error("%s: M must be 2x3 (warpAffine) or 3x3 (warpPerspective), got shape %s" % (fn, a.shape))
+    return tuple(float(v) for v in a.reshape(-1)), a.shape == (3, 3)
+
+
+class WarpView:
+    """The w x h window at (x0, y0) of cv2.warpAffine(img, M, dsize) (M 2x3) or cv2.warpPerspective(img, M, dsize) (M 3x3, whatever
+    its last row), img = cv2.cvtColor(frame, COLOR_<LAYOUT>2BGR), INTER_LINEAR with the constant 0 border, and cv2.WARP_INVERSE_MAP
+    when inverse: a rotated, de-skewed or bird's-eye view of a frame, computed where it is read, never stored.  frame: any frame
+    resize_frames takes for the layout (a BayerWindow or a crop included: M addresses its converted pixels); M: numpy or nested
+    lists, copied as float64 (later changes to the caller's array do not reach the view); dsize: (width, height), as cv2 takes it,
+    each in 1..32767.  The window defaults to the whole warped image.  The layout passed with a view names its frame's layout.
+    resize_frames, warp_frames, encode_jpeg, crop_frame, frame_size and the detection and tracking helpers take views; boxes come
+    back in the view's pixels."""
+    __slots__ = ("frame", "m", "perspective", "inverse", "dw", "dh", "x0", "y0", "w", "h")
+
+    def __init__(self, frame, M, dsize, x0=0, y0=0, w=None, h=None, inverse=False):
+        self.m, self.perspective = _warp_entries(M, "WarpView")
+        if len(dsize) != 2:
+            raise Yfv2Error("WarpView: dsize must be (width, height), got %r" % (dsize,))
+        self.frame, self.inverse = frame, bool(inverse)
+        self.dw, self.dh = int(dsize[0]), int(dsize[1])
+        self.x0, self.y0 = int(x0), int(y0)
+        self.w = self.dw - self.x0 if w is None else int(w)
+        self.h = self.dh - self.y0 if h is None else int(h)
+
+    def over(self, frame, x0, y0, w, h):
+        """The same warp of `frame` (checked or placed elsewhere), with the window (x0, y0, w, h)."""
+        v = object.__new__(WarpView)
+        for k in self.__slots__:
+            setattr(v, k, getattr(self, k))
+        v.frame, v.x0, v.y0, v.w, v.h = frame, x0, y0, w, h
+        return v
+
+    def __repr__(self):
+        return "WarpView(%r, %s, %dx%d output, x0 %d, y0 %d, %dx%d%s)" % (
+            type(self.frame).__name__, "perspective" if self.perspective else "affine", self.dw, self.dh, self.x0, self.y0,
+            self.w, self.h, ", inverse" if self.inverse else "")
+
+
 def frame_size(frame, layout):
-    """(h, w) in pixels of a frame in the given layout, as resize_frames takes it (of its window for a BayerWindow or a
-    RemapView)."""
-    if isinstance(frame, (BayerWindow, RemapView)):
+    """(h, w) in pixels of a frame in the given layout, as resize_frames takes it (of its window for a BayerWindow, a RemapView or
+    a WarpView)."""
+    if isinstance(frame, (BayerWindow, RemapView, WarpView)):
         return frame.h, frame.w
     if layout in YUV420_LAYOUTS:
         if isinstance(frame, (tuple, list)):
@@ -1536,10 +1616,21 @@ def _bayer_window(f, layout, i, fn):
 def _check_frame(f, layout, i, fn):
     """Checks frame i against its layout without copying or launching anything; returns what _describe takes: the BGR array or
     tensor, the planes of a 4:2:0 frame, a BayerWindow over a tensor for Bayer, a uint8 tensor of the layout's shape for the
-    others, a RemapView over the checked frame for a view.  A refusal names fn, the public function called."""
+    others, a RemapView or WarpView over the checked frame for a view.  A refusal names fn, the public function called."""
+    if isinstance(f, (RemapView, WarpView)) and isinstance(f.frame, (RemapView, WarpView)):
+        raise Yfv2Error("%s: frame %d: a %s of a %s (views do not nest: compose the maps or matrices instead)"
+                        % (fn, i, type(f).__name__, type(f.frame).__name__))
+    if isinstance(f, WarpView):
+        if not (1 <= f.dw <= WARP_MAX_SIDE and 1 <= f.dh <= WARP_MAX_SIDE):
+            raise Yfv2Error("%s: frame %d (%s view): dsize %dx%d outside 1..%d" % (fn, i, layout, f.dw, f.dh, WARP_MAX_SIDE))
+        if f.w < 1 or f.h < 1 or f.x0 < 0 or f.y0 < 0 or f.x0 + f.w > f.dw or f.y0 + f.h > f.dh:
+            raise Yfv2Error("%s: frame %d (%s view): window (x0 %d, y0 %d, %dx%d) is not inside the %dx%d output"
+                            % (fn, i, layout, f.x0, f.y0, f.w, f.h, f.dw, f.dh))
+        d = _warp_desc(f.m, f.perspective, f.inverse, (f.dw, f.dh))
+        if lib().yfv2_warp_matrix(ctypes.byref(d), (ctypes.c_double * 9)()):
+            raise Yfv2Error("%s: frame %d (%s view): %s" % (fn, i, layout, lib().yfv2_last_error().decode().split(": ", 1)[1]))
+        return f.over(_check_frame(f.frame, layout, i, fn), f.x0, f.y0, f.w, f.h)
     if isinstance(f, RemapView):
-        if isinstance(f.frame, RemapView):
-            raise Yfv2Error("%s: frame %d: a RemapView of a RemapView (compose the maps instead)" % (fn, i))
         m = f.maps
         if f.w < 1 or f.h < 1 or f.x0 < 0 or f.y0 < 0 or f.x0 + f.w > m.mw or f.y0 + f.h > m.mh:
             raise Yfv2Error("%s: frame %d (%s view): window (x0 %d, y0 %d, %dx%d) is not inside the %dx%d map"
@@ -1578,9 +1669,12 @@ def _checked_frames(fn, frames, layout, allowed=_FRAME_LAYOUTS):
 
 
 def _tensors(f):
-    """The arrays or tensors a checked frame reads: its planes, a BayerWindow's raw frame, a RemapView's frame and then its maps."""
+    """The arrays or tensors a checked frame reads: its planes, a BayerWindow's raw frame, a RemapView's frame and then its maps, a
+    WarpView's frame."""
     if isinstance(f, RemapView):
         return _tensors(f.frame) + (f.maps.xy,)
+    if isinstance(f, WarpView):
+        return _tensors(f.frame)
     return f if isinstance(f, tuple) else (f.raw,) if isinstance(f, BayerWindow) else (f,)
 
 
@@ -1610,7 +1704,13 @@ def _describe(f, layout, device, keep):
     union member filled and the whole frame as its region.  The only code that places frames: host frames are copied to
     `device`; a CUDA frame is read in place when its strides fit the descriptor, else a contiguous copy of it is.  The device
     tensors read go to keep, which must hold them until the launch is queued: a freed block could take the next frame's copy.
-    For a RemapView: a RemapFrame of its frame's descriptor (grey as strided), its maps on `device` and its window."""
+    For a RemapView: a RemapFrame of its frame's descriptor (grey as strided), its maps on `device` and its window; for a
+    WarpView, a WarpFrame of its frame's descriptor, its matrix, output size and window."""
+    if isinstance(f, WarpView):
+        s = _describe(f.frame, layout, device, keep)
+        r = _warp_desc(f.m, f.perspective, f.inverse, (f.dw, f.dh), f.x0, f.y0, f.w, f.h)
+        r.kind, r.f = JPEG_SRC_STRIDED if s.kind == JPEG_SRC_GRAY else s.kind, s.f
+        return r
     if isinstance(f, RemapView):
         s = _describe(f.frame, layout, device, keep)
         r = RemapFrame(JPEG_SRC_STRIDED if s.kind == JPEG_SRC_GRAY else s.kind, f.x0, f.y0, f.w, f.h)
@@ -1687,14 +1787,16 @@ def _describe(f, layout, device, keep):
 
 def _resize(fn, frames, layout, allowed, W, H, device, out):
     """resize_bgr, resize_yuv420 and resize_frames: every frame checked, then one yfv2_resize_<member>_u8 call for each run of
-    consecutive frames that fill the same descriptor (RemapViews of any kind: yfv2_resize_remap_u8), each into its slice of out."""
+    consecutive frames that fill the same descriptor (RemapViews of any kind: yfv2_resize_remap_u8; WarpViews:
+    yfv2_resize_warp_u8), each into its slice of out."""
     checked, layouts = _checked_frames(fn, frames, layout, allowed)
     device = _device(fn, checked, device)
     N = len(checked)
     out = _out(fn, out, N, H, W, device)
 
     def member_of(k):
-        return "remap" if isinstance(checked[k], RemapView) else _MEMBER[_KIND[layouts[k]]]
+        f = checked[k]
+        return "remap" if isinstance(f, RemapView) else "warp" if isinstance(f, WarpView) else _MEMBER[_KIND[layouts[k]]]
 
     i = 0
     while i < N:
@@ -1703,7 +1805,7 @@ def _resize(fn, frames, layout, allowed, W, H, device, out):
             j += 1
         keep, desc = [], _DESC[member]
         lo, hi = JpegEncSrc.f.offset, JpegEncSrc.f.offset + ctypes.sizeof(desc)     # the member's bytes in a JpegEncSrc
-        if member == "remap":
+        if member in ("remap", "warp"):
             lo, hi = 0, ctypes.sizeof(desc)
         srcs = [bytes(_describe(checked[k], layouts[k], device, keep)) for k in range(i, j)]
         descs = (desc * (j - i)).from_buffer_copy(b"".join(src[lo:hi] for src in srcs))
@@ -1728,10 +1830,12 @@ def resize_frames(frames, W, H, layout, device=None, out=None):
       "bayer_bg" | "bayer_gb"           [h, w] raw Bayer (BAYER_LAYOUTS), COLOR_Bayer<XY>2BGR; "bayer_<xy>_ea": _EA, the
         | "bayer_rg" | "bayer_gr"       edge-aware demosaic; or a BayerWindow of one (crop_frame)
     and a RemapView of a frame of any of these layouts (layout: its frame's): cv2.remap(INTER_LINEAR) of the converted frame,
-    cropped to the view's window, computed where the resize reads it (yfv2_resize_remap_u8).
+    cropped to the view's window, computed where the resize reads it (yfv2_resize_remap_u8); a WarpView likewise with
+    cv2.warpAffine / cv2.warpPerspective (yfv2_resize_warp_u8).
     Frames are numpy arrays or CUDA tensors; CUDA views with larger row strides or crop offsets are read in place (for
     "rgb_chw" any channel and row stride with unit column stride), host arrays are copied to `device`.  Consecutive frames of
-    one descriptor kind go to one call (yfv2_resize_bgr_u8 / _yuv420_u8 / _strided_u8 / _yuv422_u8 / _bayer_u8 / _remap_u8), each
+    one descriptor kind go to one call (yfv2_resize_bgr_u8 / _yuv420_u8 / _strided_u8 / _yuv422_u8 / _bayer_u8 / _remap_u8 /
+    _warp_u8), each
     into its slice of `out`.  Every frame is checked before anything is copied or launched."""
     return _resize("resize_frames", frames, layout, _FRAME_LAYOUTS, W, H, device, out)
 
@@ -1740,17 +1844,30 @@ def remap_frames(views, layout, device=None):
     """cv2.remap(cv2.cvtColor(frame, COLOR_<LAYOUT>2BGR), map1, map2, cv2.INTER_LINEAR)[y0:y0+h, x0:x0+w] of every RemapView, bit
     for bit, computed on the device (yfv2_remap_u8): a list of CUDA uint8 [h, w, 3] BGR tensors.  layout: the views' frames'
     layout, one name or one per view.  Every view is checked before anything is copied or launched."""
-    checked, layouts = _checked_frames("remap_frames", views, layout)
+    return _view_frames("remap_frames", RemapView, views, layout, device)
+
+
+def warp_frames(views, layout, device=None):
+    """cv2.warpAffine / cv2.warpPerspective(cv2.cvtColor(frame, COLOR_<LAYOUT>2BGR), M, dsize, INTER_LINEAR)[y0:y0+h, x0:x0+w] of
+    every WarpView, bit for bit, computed on the device (yfv2_warp_u8): a list of CUDA uint8 [h, w, 3] BGR tensors.  layout: the
+    views' frames' layout, one name or one per view.  Every view is checked before anything is copied or launched."""
+    return _view_frames("warp_frames", WarpView, views, layout, device)
+
+
+def _view_frames(fn, cls, views, layout, device):
+    """remap_frames and warp_frames: every view of class cls checked, then one yfv2_remap_u8 / yfv2_warp_u8 call."""
+    checked, layouts = _checked_frames(fn, views, layout)
     for i, v in enumerate(checked):
-        if not isinstance(v, RemapView):
-            raise Yfv2Error("remap_frames: frame %d is a %s, not a RemapView" % (i, type(views[i]).__name__))
-    device = _device("remap_frames", checked, device)
+        if not isinstance(v, cls):
+            raise Yfv2Error("%s: frame %d is a %s, not a %s" % (fn, i, type(views[i]).__name__, cls.__name__))
+    device = _device(fn, checked, device)
     outs = [torch.empty((v.h, v.w, 3), dtype=torch.uint8, device=device) for v in checked]
     keep = []
-    descs = (RemapFrame * len(checked))(*[_describe(v, lay, device, keep) for v, lay in zip(checked, layouts)])
+    member = "remap" if cls is RemapView else "warp"
+    descs = (_DESC[member] * len(checked))(*[_describe(v, lay, device, keep) for v, lay in zip(checked, layouts)])
     dst = (ctypes.c_void_p * len(outs))(*[o.data_ptr() for o in outs])
     with torch.cuda.device(device):
-        _check(lib().yfv2_remap_u8(descs, len(checked), dst, _stream(device)), "remap_u8")
+        _check(getattr(lib(), "yfv2_%s_u8" % member)(descs, len(checked), dst, _stream(device)), "%s_u8" % member)
     return outs
 
 
@@ -1799,18 +1916,20 @@ def encode_jpeg(frames, quality=95, sampling="420", restart_interval=0, layout="
         plist.append([IMWRITE_JPEG_QUALITY, int(qs[k]), IMWRITE_JPEG_SAMPLING_FACTOR, JPEG_SAMPLING[ss[k]],
                       IMWRITE_JPEG_RST_INTERVAL, int(rs[k])] + [int(x) for x in extra[k]])
     device = _device("encode_jpeg", checked, device)
-    # each RemapView an output reads: remapped once (remap_frames) and encoded as the BGR frame it gives
-    views = sorted({int(r[0]) for r in regions if isinstance(checked[int(r[0])], RemapView)})
+    # each RemapView or WarpView an output reads: computed once (remap_frames, warp_frames) and encoded as the BGR frame it gives
+    views = sorted({int(r[0]) for r in regions if isinstance(checked[int(r[0])], (RemapView, WarpView))})
     for k, r in enumerate(regions):
         v = checked[int(r[0])]
-        if isinstance(v, RemapView) and None not in r[3:]:
+        if isinstance(v, (RemapView, WarpView)) and None not in r[3:]:
             x0, y0, w, h = (int(a) for a in r[1:])
             if w < 1 or h < 1 or x0 < 0 or y0 < 0 or x0 + w > v.w or y0 + h > v.h:
                 raise Yfv2Error("encode_jpeg: output %d: region (x0 %d, y0 %d, %dx%d) is not inside the %dx%d view"
                                 % (k, x0, y0, w, h, v.w, v.h))
-    if views:
-        for i, t in zip(views, remap_frames([checked[i] for i in views], [layouts[i] for i in views], device)):
-            checked[i], layouts[i] = t, "bgr"
+    for cls, fn in ((RemapView, remap_frames), (WarpView, warp_frames)):
+        idx = [i for i in views if isinstance(checked[i], cls)]
+        if idx:
+            for i, t in zip(idx, fn([checked[i] for i in idx], [layouts[i] for i in idx], device)):
+                checked[i], layouts[i] = t, "bgr"
     srcs = (JpegEncSrc * n)()
     keep, cparams, frame_src = [], [], {}
     for k, r in enumerate(regions):
@@ -1856,8 +1975,9 @@ def crop_frame(frame, layout, x0, y0, w, h):
     becomes a tuple of cropped planes, (y, uv) for NV12 / NV21 and (y, u, v) for I420 / YV12; x0, y0, w, h must then be even, so
     that the 2x2 chroma blocks of the crop are those of the frame.  Packed 4:2:2 needs even x0 and w (whole macropixels).  A Bayer
     frame, or a BayerWindow of one, becomes a BayerWindow of the whole raw frame (any offsets): the conversion of a pixel reads its
-    neighbours and the frame's edges, so the raw bytes are not cropped.  A RemapView becomes the RemapView of the window of its
-    remapped image (any offsets, whatever its frame's layout).  A crop of a crop is the crop of the frame."""
+    neighbours and the frame's edges, so the raw bytes are not cropped.  A RemapView (WarpView) becomes the RemapView (WarpView)
+    of the window of its remapped (warped) image (any offsets, whatever its frame's layout).  A crop of a crop is the crop of the
+    frame."""
     if layout not in _FRAME_LAYOUTS:
         raise Yfv2Error("crop_frame: layout must be one of %s, got %r" % (", ".join(_FRAME_LAYOUTS), layout))
     f = _check_frame(frame, layout, 0, "crop_frame")
@@ -1867,6 +1987,8 @@ def crop_frame(frame, layout, x0, y0, w, h):
         raise Yfv2Error("crop_frame: window (x0 %d, y0 %d, %dx%d) is not inside the %dx%d frame" % (x0, y0, w, h, fw, fh))
     if isinstance(f, RemapView):                              # a window of the remapped image: any offsets, any layout
         return RemapView(f.frame, f.maps, f.x0 + x0, f.y0 + y0, w, h)
+    if isinstance(f, WarpView):                               # a window of the warped image: any offsets, any layout
+        return f.over(f.frame, f.x0 + x0, f.y0 + y0, w, h)
     if layout in YUV420_LAYOUTS and (x0 | y0 | w | h) & 1:
         raise Yfv2Error("crop_frame: %s crops need even x0, y0, w and h (2x2 chroma blocks), got (x0 %d, y0 %d, %dx%d)"
                         % (layout, x0, y0, w, h))
