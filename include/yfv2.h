@@ -320,6 +320,33 @@ YFV2_API int yfv2_aug_blur_workspace_bytes(int N, int H, int W, size_t* bytes);
 YFV2_API int yfv2_aug_batch_blur(const uint8_t* img, uint8_t* out, int N, int H, int W, const yfv2_aug_params* params,
                                  const uint8_t* luts, const yfv2_aug_blur* blur, int flags, void* workspace,
                                  size_t workspace_bytes, void* stream);
+/* ---- Geometric training augmentation: YOLOv5's load_mosaic, random_perspective and fliplr on the device -------------------------
+ * One pass over img [N,3,H,W] (planar B, G, R uint8) into out, before the photometric steps above.  Output image n, with
+ * p = params[n]:
+ *   canvas  without mosaic: image p.src[0], W x H.  With mosaic: load_mosaic's 2W x 2H canvas filled with 114, images
+ *           p.src[0..3] top-left, top-right, bottom-left, bottom-right around (xc, yc), clipped to the canvas as load_mosaic's
+ *           x1a .. y2b lines clip them: canvas pixel (r, c) is tile 2 (r >= yc) + (c >= xc) at local
+ *           (c - xc + W (c < xc), r - yc + H (r < yc)), and 114 where that falls outside the W x H tile.
+ *   warp    random_perspective's cv2.warpAffine(canvas, M[:2], (W, H), borderValue=(114, 114, 114)), or cv2.warpPerspective(canvas,
+ *           M, (W, H), borderValue=...) with perspective: INTER_LINEAR with the coordinate arithmetic of yfv2_resize_warp_u8 (M
+ *           inverted on the host as there, the fixed-point coordinate in cv2's fp64 order), sampled as yfv2_resize_remap_u8 samples,
+ *           except that a tap outside the canvas reads 114 instead of weighing 0 (a pixel with all four taps outside is 114).
+ *   flip    with flip, np.fliplr of the warped image: output pixel (x, y) is the warp's (W - 1 - x, y).
+ * params: HOST array [N].  Refused before anything is launched (YFV2_EINVAL): null pointers, N <= 0; H, W outside 1..32768; out
+ * overlapping img at all (a mosaic reads other images); perspective, mosaic or flip not 0 or 1; src[0] (and with mosaic src[1..3])
+ * outside [0, N); a canvas side of 32767 (SHRT_MAX) or more, so W, H <= 32766 without mosaic and <= 16383 with it (cv2.remap
+ * refuses such sources, and the fixed-point coordinate saturates at 32767); with mosaic an odd H or W, or xc outside [W/2, 2W - W/2], yc outside [H/2, 2H - H/2] (inclusive: YOLOv5's
+ * int(uniform(a, b)) can return b); and whatever yfv2_warp_matrix refuses of M with dsize (W, H) (a singular or non-finite M, an
+ * affine M whose scaled terms reach 2^30, sides over 32767). */
+typedef struct yfv2_aug_geom {
+    double m[9];      /* M as cv2.warpAffine (m[0..5]) / cv2.warpPerspective receives it: canvas -> output */
+    int perspective;  /* 0 warpAffine, 1 warpPerspective */
+    int mosaic;       /* 0: canvas = image src[0]; 1: 2W x 2H mosaic of src[0..3] around (xc, yc) */
+    int src[4];
+    int xc, yc;
+    int flip;         /* 0 or 1: np.fliplr of the warped image */
+} yfv2_aug_geom;
+YFV2_API int yfv2_aug_geometric(const uint8_t* img, uint8_t* out, int N, int H, int W, const yfv2_aug_geom* params, void* stream);
 /* Test hooks: n packed 3-byte pixels through the device's cv2.cvtColor COLOR_BGR2HSV / COLOR_HSV2BGR (any input bytes).  cv2's
  * 8-bit HSV2BGR rounds the last (row_w mod 32) pixels of each row differently from the others (OpenCV 4.13 x86: vector code
  * truncates, the scalar tail rounds), so the pixels are taken as rows of row_w. */

@@ -2,7 +2,7 @@
 """Training-batch augmentation on the device: img_aug (utils/datasets.py:63-68) with motion_blur, random_resize and augment_hsv
 enabled.
 
-  python tools/bench_aug.py [--batch 256 --size 352 --iters 50 --host-images 16]
+  python tools/bench_aug.py [--batch 256 --size 352 --iters 50 --host-images 16] [--geom]
 
 Times, on a uint8 [batch, 3, size, size] batch resident in HBM, each launch after an L2 flush (a 256 MB memset), with CUDA events
 around the launch alone:
@@ -12,6 +12,14 @@ around the launch alone:
                          degree 2, half 3; the reference blurs half of its images, see datasets.py:19);
   *_GBps                 the batch read once plus the batch written once, over the time (the elementwise modes' minimum traffic;
                          the resize modes read about (rw*rh)/(W*H) of each source image more than once, which this does not count).
+--geom adds yfv2_aug_geometric (YOLOv5's load_mosaic -> random_perspective with border 114 -> fliplr) to the same run:
+  geom_mosaic_affine_us / geom_mosaic_persp_us   every image a mosaic of four batch images, warped by cv2.warpAffine /
+                         cv2.warpPerspective matrices drawn with degrees 10, shear 5, scale 0.5, translate 0.1 (perspective
+                         5e-4), half of them flipped;
+  geom_flip_us           fliplr alone (identity M);
+  geom_draws_us / geom_labels_us / geom_host_us   the host side of one batch of 64 mosaics with 8 boxes per image, as the
+                         trainer runs it in its main process: utils.device_aug.draw_geometric, geometric_targets, and the two
+                         together, medians of 20 (host times, not device times).
 host_*_us: the reference's own contrast_and_brightness, motion_blur (blurred images only), random_resize and augment_hsv per
 image on one core
 (cv2.setNumThreads(1)), when the reference checkout is on PYTHONPATH; otherwise they are reported as not measured.
@@ -95,6 +103,7 @@ def main():
     ap.add_argument("--size", type=int, default=352)
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--host-images", type=int, default=16)
+    ap.add_argument("--geom", action="store_true", help="also time yfv2_aug_geometric and the host label step")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_aug.py: needs a CUDA device")
@@ -142,6 +151,20 @@ def main():
     assert torch.equal(eng.augment_batch(x, a, b, rw, rh, luts), (modes["all"](), out)[1])      # the timed call is the API's
     assert torch.equal(eng.augment_batch(x, blur=blur), (modes["blur"](), out)[1])
     assert torch.equal(eng.augment_batch(x, a, b, rw, rh, luts, blur=blur), (modes["blur_all"](), out)[1])
+    if args.geom:
+        import random
+        import utils.device_aug as da
+        draws = {
+            "geom_mosaic_affine": da.draw_geometric(N, S, S, random.Random(2), mosaic=1.0, degrees=10, shear=5),
+            "geom_mosaic_persp": da.draw_geometric(N, S, S, random.Random(3), mosaic=1.0, degrees=10, shear=5, perspective=0.0005),
+            "geom_flip": [dict(M=np.eye(3), perspective=False, mosaic=False, src=[i] * 4, flip=True) for i in range(N)],
+        }
+        for name, d in draws.items():
+            modes[name] = (lambda gd: lambda: eng._check(L.yfv2_aug_geometric(ctypes.c_void_p(x.data_ptr()),
+                                                                               ctypes.c_void_p(out.data_ptr()), N, S, S, gd,
+                                                                               stream), "aug_geometric"))(eng.geom_descriptors(d))
+            assert torch.equal(eng.augment_geometric(x, d), (modes[name](), out)[1])
+        assert torch.equal(out, torch.flip(x, [3]))
     res = {"gpu": gpu_info(), "batch": N, "size": S, "iters": args.iters}
     moved = 2 * x.numel()
     for name, fn in modes.items():
@@ -153,6 +176,24 @@ def main():
         res[name + "_us_range"] = [round(lo, 1), round(hi, 1)]
         res[name + "_GBps"] = round(moved / med / 1e3, 1)
     res["bytes_moved"] = moved
+    if args.geom:
+        import random
+        import utils.device_aug as da
+        rs = np.random.RandomState(4)
+        t = np.concatenate([np.column_stack([np.full(8, n), rs.randint(0, 80, 8), rs.uniform(0.1, 0.9, (8, 2)),
+                                             rs.uniform(0.05, 0.4, (8, 2))]) for n in range(64)]).astype(np.float32)
+        tt = torch.from_numpy(t)
+        ts = []
+        for i in range(21):
+            t0 = time.perf_counter()
+            d = da.draw_geometric(64, S, S, random.Random(5 + i), mosaic=1.0, degrees=10, shear=5)
+            t1 = time.perf_counter()
+            da.geometric_targets(tt, d, S, S)
+            ts.append((t1 - t0, time.perf_counter() - t1))
+        ts = np.array(ts[1:]) * 1e6
+        res["geom_draws_us"] = round(float(np.median(ts[:, 0])), 1)
+        res["geom_labels_us"] = round(float(np.median(ts[:, 1])), 1)
+        res["geom_host_us"] = round(float(np.median(ts.sum(1))), 1)
     ht = host_times(args.host_images, S)
     res.update({k: round(v, 1) for k, v in ht.items()} if ht else {"host": "reference checkout not on PYTHONPATH: not measured"})
     print(json.dumps(res))

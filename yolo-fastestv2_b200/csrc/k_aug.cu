@@ -8,9 +8,13 @@
 // aug_pixel_kernel runs it elementwise, with it k_resize.cu's aug_resize_kernel (aug.cuh holds the shared pixel arithmetic).
 // yfv2_aug_batch_blur adds motion_blur (:18-37) between contrast and the resize: blur_kernel filters each blurred image into the
 // workspace and reduces its byte range, then the same two kernels read it there through cv2.normalize's byte map.
+// yfv2_aug_geometric (geom_kernel) runs YOLOv5's geometric steps before all of these: load_mosaic's canvas, random_perspective's
+// warp with border 114 and fliplr, one output pixel per thread through resize.cuh's warp_pixel.
 #include <cmath>
+#include <vector>
 
 #include "aug.cuh"
+#include "resize.cuh"
 
 namespace yfv2 {
 namespace {
@@ -344,8 +348,194 @@ int aug_batch(const char* fn, int allowed, const uint8_t* img, uint8_t* out, int
     return YFV2_OK;
 }
 
+// ---- yfv2_aug_geometric: load_mosaic's canvas -> random_perspective's warp (border 114) -> fliplr ---------------------------------
+constexpr int kGeomBorder = 114;                    // load_mosaic's fill and random_perspective's borderValue
+constexpr int kGeomBx = 64, kGeomBy = 4;
+constexpr int kGeomMaxCanvas = 32767;               // SHRT_MAX: cv2.remap refuses sources this large, warp_pixel saturates there
+
+// load_mosaic's 2W x 2H canvas of four W x H planar images of the batch around (xc, yc)
+struct MosaicFrame {
+    const uint8_t* img;                             // image 0 of the batch, [N][3][th][tw]
+    int src[4];                                     // top-left, top-right, bottom-left, bottom-right
+    int xc, yc;
+    int w, h;                                       // the canvas, 2 tw x 2 th: sample_fixed's bounds
+    int tw, th;                                     // one tile (a batch image)
+};
+
+// Canvas pixel (r, c) is tile 2 (r >= yc) + (c >= xc) at local (c - xc + tw (c < xc), r - yc + th (r < yc)), and kGeomBorder
+// where that falls outside the tile.  The row's two tiles are found once per row.
+struct MosaicSource {
+    using Desc = MosaicFrame;
+    const uint8_t* left;                            // the row's left and right tiles at the local row
+    const uint8_t* right;
+    long long plane;
+    int xc, tw;
+    bool row_in;
+    __device__ __forceinline__ MosaicSource(const MosaicFrame& f, int r) : plane((long long)f.tw * f.th), xc(f.xc), tw(f.tw) {
+        const int below = r >= f.yc;
+        const int lr = r - f.yc + (below ? 0 : f.th);
+        row_in = (unsigned)lr < (unsigned)f.th;
+        const long long off = row_in ? (long long)lr * f.tw : 0;
+        left = f.img + 3 * plane * f.src[2 * below] + off;
+        right = f.img + 3 * plane * f.src[2 * below + 1] + off;
+    }
+    __device__ __forceinline__ void pixel(int c, int (&p)[3]) const {
+        const bool r = c >= xc;
+        const int lc = c - xc + (r ? 0 : tw);
+        const bool in = row_in && (unsigned)lc < (unsigned)tw;
+        const uint8_t* q = (r ? right : left) + (in ? lc : 0);
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) p[ch] = in ? __ldg(q + ch * plane) : kGeomBorder;
+    }
+    __device__ __forceinline__ void fetch(int c0, int c1, int (&p0)[3], int (&p1)[3]) const {
+        pixel(c0, p0);
+        pixel(c1, p1);
+    }
+};
+
+// Images of one canvas kind (MosaicSource, or StridedSource over one planar batch image): each warp descriptor (the canvas, M
+// inverted, the window (0, 0, W, H)), its output image and flip, under the 4 KB launch limit with the chunk's rest
+template <class Inner>
+struct GeomChunk {
+    static constexpr int kChunk = 3968 / (int)(sizeof(WarpDesc<Inner>) + sizeof(int) + 1);
+    WarpDesc<Inner> d[kChunk];
+    int n[kChunk];
+    uint8_t flip[kChunk];
+    uint8_t* out;                                   // image 0 of the batch
+    int H, W;
+};
+static_assert(sizeof(GeomChunk<MosaicSource>) <= 4000 && sizeof(GeomChunk<StridedSource>) <= 4000, "kernel parameters over 4 KB");
+
+// One thread per output pixel of image a.n[blockIdx.z]: the warp's pixel at the flipped column, written to the three planes
+template <class Inner>
+__global__ void __launch_bounds__(kGeomBx * kGeomBy)
+geom_kernel(const __grid_constant__ GeomChunk<Inner> a) {
+    const int x = blockIdx.x * kGeomBx + threadIdx.x;
+    const int y = blockIdx.y * kGeomBy + threadIdx.y;
+    if (x >= a.W || y >= a.H) return;
+    const int i = blockIdx.z;
+    int v[3];
+    warp_pixel<Inner, kGeomBorder>(a.d[i], a.flip[i] ? a.W - 1 - x : x, y, v);
+    const size_t plane = (size_t)a.H * a.W;
+    uint8_t* out = a.out + (size_t)a.n[i] * 3 * plane + (size_t)y * a.W + x;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out[c * plane] = (uint8_t)v[c];
+}
+
+// The canvas of a checked image: the mosaic, or the planar image src[0] as a strided frame
+inline void geom_canvas(MosaicFrame& f, const yfv2_aug_geom& p, const uint8_t* img, int H, int W) {
+    f = MosaicFrame{img, {p.src[0], p.src[1], p.src[2], p.src[3]}, p.xc, p.yc, 2 * W, 2 * H, W, H};
+}
+inline void geom_canvas(yfv2_strided_frame& f, const yfv2_aug_geom& p, const uint8_t* img, int H, int W) {
+    const size_t plane = (size_t)H * W;
+    const uint8_t* b = img + 3 * plane * p.src[0];
+    f = yfv2_strided_frame{b, b + plane, b + 2 * plane, W, 1, W, H};
+}
+
+// The matrix check of yfv2_warp_matrix (warp_matrix_fault) for M with dsize (W, H); m gets the output -> canvas matrix
+inline const char* geom_matrix_fault(const yfv2_aug_geom& p, int H, int W, double (&m)[9]) {
+    yfv2_warp_frame wf{};
+    for (int k = 0; k < 9; ++k) wf.m[k] = p.m[k];
+    wf.perspective = p.perspective;
+    wf.dw = W;
+    wf.dh = H;
+    return warp_matrix_fault(wf, m);
+}
+
+// The images idx[0, cnt), all of Inner's canvas kind, GeomChunk<Inner>::kChunk per launch
+template <class Inner>
+int launch_geom(const yfv2_aug_geom* params, const int* idx, int cnt, const uint8_t* img, uint8_t* out, int H, int W,
+                cudaStream_t stream) {
+    using Chunk = GeomChunk<Inner>;
+    for (int i0 = 0; i0 < cnt; i0 += Chunk::kChunk) {
+        const int k = cnt - i0 < Chunk::kChunk ? cnt - i0 : Chunk::kChunk;
+        Chunk a{};
+        for (int i = 0; i < k; ++i) {
+            const yfv2_aug_geom& p = params[idx[i0 + i]];
+            WarpDesc<Inner>& d = a.d[i];
+            geom_canvas(d.f, p, img, H, W);
+            geom_matrix_fault(p, H, W, d.m);                // checked
+            d.perspective = p.perspective;
+            d.x0 = 0; d.y0 = 0; d.w = W; d.h = H;
+            a.n[i] = idx[i0 + i];
+            a.flip[i] = (uint8_t)p.flip;
+        }
+        a.out = out;
+        a.H = H; a.W = W;
+        const dim3 grid((unsigned)((W + kGeomBx - 1) / kGeomBx), (unsigned)((H + kGeomBy - 1) / kGeomBy), (unsigned)k);
+        geom_kernel<Inner><<<grid, dim3(kGeomBx, kGeomBy), 0, stream>>>(a);
+        YFV2_LAUNCH_CHECK();
+    }
+    return YFV2_OK;
+}
+
+// yfv2_aug_geometric: every check, then one launch sequence for the mosaic images and one for the others
+int aug_geometric(const uint8_t* img, uint8_t* out, int N, int H, int W, const yfv2_aug_geom* params, void* stream) {
+    const char* fn = "aug_geometric";
+    if (!img || !out || !params || N <= 0) { set_error("%s: null img / out / params or N <= 0", fn); return YFV2_EINVAL; }
+    if (H <= 0 || W <= 0 || H > kAugMaxSide || W > kAugMaxSide) {
+        set_error("%s: image %dx%d outside 1..%d", fn, W, H, kAugMaxSide);
+        return YFV2_EINVAL;
+    }
+    const size_t bytes = (size_t)N * 3 * H * W;
+    if (overlaps(reinterpret_cast<uintptr_t>(img), bytes, reinterpret_cast<uintptr_t>(out), bytes)) {
+        set_error("%s: img and out overlap (a mosaic reads other images: use another buffer)", fn);
+        return YFV2_EINVAL;
+    }
+    for (int n = 0; n < N; ++n) {
+        const yfv2_aug_geom& p = params[n];
+        if ((p.perspective | p.mosaic | p.flip) & ~1) {
+            set_error("%s: image %d: perspective, mosaic and flip must be 0 or 1 (got %d, %d, %d)", fn, n, p.perspective, p.mosaic,
+                      p.flip);
+            return YFV2_EINVAL;
+        }
+        for (int t = 0; t < (p.mosaic ? 4 : 1); ++t) {
+            if (p.src[t] < 0 || p.src[t] >= N) {
+                set_error("%s: image %d: src[%d] = %d outside [0, %d)", fn, n, t, p.src[t], N);
+                return YFV2_EINVAL;
+            }
+        }
+        const int cw = p.mosaic ? 2 * W : W, ch = p.mosaic ? 2 * H : H;
+        if (cw >= kGeomMaxCanvas || ch >= kGeomMaxCanvas) {
+            set_error("%s: image %d: %s canvas %dx%d: its sides must be below %d (cv2.remap's limit; the fixed-point source "
+                      "coordinate saturates there)", fn, n, p.mosaic ? "mosaic" : "image", cw, ch, kGeomMaxCanvas);
+            return YFV2_EINVAL;
+        }
+        if (p.mosaic) {
+            if ((H | W) & 1) { set_error("%s: image %d: mosaic needs even H and W (got %dx%d)", fn, n, W, H); return YFV2_EINVAL; }
+            if (p.xc < W / 2 || p.xc > 2 * W - W / 2 || p.yc < H / 2 || p.yc > 2 * H - H / 2) {
+                set_error("%s: image %d: mosaic centre (%d, %d) outside [%d, %d] x [%d, %d]", fn, n, p.xc, p.yc, W / 2,
+                          2 * W - W / 2, H / 2, 2 * H - H / 2);
+                return YFV2_EINVAL;
+            }
+        }
+        double m[9];
+        if (const char* why = geom_matrix_fault(p, H, W, m)) {
+            set_error("%s: image %d: %s (%s M, dsize %dx%d)", fn, n, why, p.perspective ? "perspective" : "affine", W, H);
+            return YFV2_EINVAL;
+        }
+    }
+    std::vector<int> idx;
+    for (int mosaic = 0; mosaic < 2; ++mosaic) {
+        idx.clear();
+        for (int n = 0; n < N; ++n)
+            if (params[n].mosaic == mosaic) idx.push_back(n);
+        if (idx.empty()) continue;
+        const int cnt = (int)idx.size();
+        const int rc = mosaic ? launch_geom<MosaicSource>(params, idx.data(), cnt, img, out, H, W, (cudaStream_t)stream)
+                              : launch_geom<StridedSource>(params, idx.data(), cnt, img, out, H, W, (cudaStream_t)stream);
+        if (rc != YFV2_OK) return rc;
+    }
+    return YFV2_OK;
+}
+
 }  // namespace
 }  // namespace yfv2
+
+extern "C" int yfv2_aug_geometric(const uint8_t* img, uint8_t* out, int N, int H, int W, const yfv2_aug_geom* params,
+                                  void* stream) {
+    return yfv2::aug_geometric(img, out, N, H, W, params, stream);
+}
 
 extern "C" int yfv2_aug_contrast_brightness(const uint8_t* img, uint8_t* out, const float* alpha, const float* beta, int N,
                                             long long bytes_per_image, void* stream) {

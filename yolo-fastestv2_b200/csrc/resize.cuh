@@ -301,7 +301,9 @@ struct BayerSource {
 // computes the table cv2's way and checks this).  A tap outside the inner frame's w x h weighs 0, and its fetch reads the clamped
 // coordinate, so Inner is never read out of range; the two columns of a fetch stay equal or adjacent, as BayerSource needs.
 // remap_pixel (a map entry) and warp_pixel (a computed coordinate) share it.
-template <class Inner>
+// Border != 0 is BORDER_CONSTANT with that value instead (YOLOv5's borderValue 114): a tap outside weighs as it would inside and
+// reads Border, so a pixel with all four taps outside is Border.  Border 0, the default, is the rule above.
+template <class Inner, int Border = 0>
 __device__ __forceinline__ void sample_fixed(const typename Inner::Desc& f, int X, int Y, int k, int (&v)[3]) {
     const int i = k >> 5, j = k & 31;
     const int w = f.w, h = f.h;
@@ -309,16 +311,23 @@ __device__ __forceinline__ void sample_fixed(const typename Inner::Desc& f, int 
     const bool y0in = (unsigned)Y < (unsigned)h, y1in = (unsigned)(Y + 1) < (unsigned)h;
     if (!((x0in || x1in) && (y0in || y1in))) {
 #pragma unroll
-        for (int c = 0; c < 3; ++c) v[c] = 0;
+        for (int c = 0; c < 3; ++c) v[c] = Border;
         return;
     }
-    const int ax0 = x0in ? 32 - j : 0, ax1 = x1in ? j : 0;
-    const int by0 = y0in ? 32 - i : 0, by1 = y1in ? i : 0;
+    const int ax0 = x0in || Border ? 32 - j : 0, ax1 = x1in || Border ? j : 0;
+    const int by0 = y0in || Border ? 32 - i : 0, by1 = y1in || Border ? i : 0;
     const int cx0 = min(max(X, 0), w - 1), cx1 = min(max(X + 1, 0), w - 1);
     const Inner row0(f, min(max(Y, 0), h - 1)), row1(f, min(max(Y + 1, 0), h - 1));
     int p00[3], p01[3], p10[3], p11[3];          // [row][column] taps, B G R
     row0.fetch(cx0, cx1, p00, p01);
     row1.fetch(cx0, cx1, p10, p11);
+    if (Border) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            p00[c] = y0in && x0in ? p00[c] : Border; p01[c] = y0in && x1in ? p01[c] : Border;
+            p10[c] = y1in && x0in ? p10[c] : Border; p11[c] = y1in && x1in ? p11[c] : Border;
+        }
+    }
 #pragma unroll
     for (int c = 0; c < 3; ++c)
         v[c] = sat_u8(((by0 * (p00[c] * ax0 + p01[c] * ax1) + by1 * (p10[c] * ax0 + p11[c] * ax1)) * 32 + 16384) >> 15);
@@ -353,8 +362,8 @@ __device__ __forceinline__ int clamp_round(double v) {
 
 // cv2.warpAffine / cv2.warpPerspective(INTER_LINEAR, BORDER_CONSTANT 0) of an Inner frame: pixel (x, y) of the warped image, B,
 // G, R in v.  The fixed-point coordinate is computed here in cv2's order of fp64 operations (yfv2.h states them), each rounded
-// on its own (__dmul_rn / __dadd_rn: no FMA contraction), then sampled as a remap map entry.
-template <class Inner>
+// on its own (__dmul_rn / __dadd_rn: no FMA contraction), then sampled as a remap map entry (with Border: sample_fixed's).
+template <class Inner, int Border = 0>
 __device__ __forceinline__ void warp_pixel(const WarpDesc<Inner>& d, int x, int y, int (&v)[3]) {
     const double* m = d.m;
     const double dx = (double)x, dy = (double)y;
@@ -371,7 +380,7 @@ __device__ __forceinline__ void warp_pixel(const WarpDesc<Inner>& d, int x, int 
         Y = clamp_round(__dmul_rn(__dadd_rn(__dadd_rn(__dmul_rn(m[4], dy), m[5]), __dmul_rn(m[3], dx)), W));
     }
     const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767);
-    sample_fixed<Inner>(d.f, sx, sy, ((Y & 31) << 5) + (X & 31), v);
+    sample_fixed<Inner, Border>(d.f, sx, sy, ((Y & 31) << 5) + (X & 31), v);
 }
 
 // Pixels of the window of cv2.warpAffine / cv2.warpPerspective(inner frame), each computed from the inner frame where it is read

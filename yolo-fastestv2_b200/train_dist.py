@@ -25,6 +25,11 @@ trainable layer); `--freeze-bn` also puts the BatchNorm layers whose weight and 
 statistics used and left alone); `--unfreeze-epoch E` makes everything trainable and every BatchNorm layer train-mode again from
 epoch E.  Without them every parameter trains, as in train.py.
 
+`--device-aug-geom [k=v,...]` (with `--device-aug`) adds YOLOv5's geometric augmentation before img_aug: load_mosaic of four
+batch images, random_perspective and fliplr on the GPU into a second batch buffer, with the targets moved alongside on the host
+(utils.device_aug.geometric_batch, DESIGN.md §20).  The optional k=v list overrides YOLOv5's hyp.scratch-low values of mosaic,
+degrees, translate, scale, shear, perspective and fliplr.  Validation batches are not augmented.
+
 `--synthetic N` replaces the dataset by N seeded synthetic images with SURVEY 8(d) config[2] box statistics (no dataset and
 no reference checkout needed: used by the GPU tests and the 8-GPU measurement)."""
 import argparse
@@ -85,6 +90,9 @@ def main(argv=None):
     ap.add_argument("--device-aug-resize", action="store_true", help="with --device-aug: add random_resize (utils/datasets.py:54-61)")
     ap.add_argument("--device-aug-hsv", action="store_true", help="with --device-aug: add augment_hsv (utils/datasets.py:39-51)")
     ap.add_argument("--device-aug-blur", action="store_true", help="with --device-aug: add motion_blur (utils/datasets.py:18-37)")
+    ap.add_argument("--device-aug-geom", nargs="?", const="", default=None, metavar="K=V,...",
+                    help="with --device-aug: add YOLOv5's mosaic, random_perspective and fliplr before img_aug; optional "
+                         "comma-separated overrides of mosaic, degrees, translate, scale, shear, perspective, fliplr")
     ap.add_argument("--device-decode", action="store_true", help="read the train and validation images with utils.device_data: JPEG "
                                                                  "decode and resize to the network input on the GPU (needs --device-aug)")
     ap.add_argument("--freeze", type=str, default="", help="comma-separated named_parameters() prefixes to freeze, e.g. "
@@ -104,6 +112,20 @@ def main(argv=None):
         ap.error("--device-decode reads cfg['train'] and cfg['val']; it does not combine with --synthetic")
     if (opt.device_aug_resize or opt.device_aug_hsv or opt.device_aug_blur) and not opt.device_aug:
         ap.error("--device-aug-resize, --device-aug-hsv and --device-aug-blur need --device-aug")
+    geom_hyp = None
+    if opt.device_aug_geom is not None:
+        if not opt.device_aug:
+            ap.error("--device-aug-geom needs --device-aug")
+        import utils.device_aug
+        geom_hyp = {}
+        for kv in filter(None, opt.device_aug_geom.split(",")):
+            k, _, v = kv.partition("=")
+            if k not in utils.device_aug.GEOM_HYP or not v:
+                ap.error("--device-aug-geom: %r is not k=v with k one of %s" % (kv, ", ".join(utils.device_aug.GEOM_HYP)))
+            try:
+                geom_hyp[k] = float(v)
+            except ValueError:
+                ap.error("--device-aug-geom: %s=%r is not a number" % (k, v))
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -183,6 +205,7 @@ def main(argv=None):
 
     epochs = opt.epochs if opt.epochs is not None else cfg["epochs"]
     batch_num, t0, seen = 0, time.time(), 0
+    geom_buf = None                                                              # --device-aug-geom's output batch, allocated once
     bucket.zero()
     for epoch in range(epochs):
         if freeze and epoch == opt.unfreeze_epoch:
@@ -201,6 +224,10 @@ def main(argv=None):
             imgs = imgs.to(device, non_blocking=True)
             if opt.device_aug and imgs.dtype == torch.uint8:
                 import utils.device_aug
+                if geom_hyp is not None:                                          # mosaic, random_perspective, fliplr
+                    if geom_buf is None or geom_buf.shape != imgs.shape:
+                        geom_buf = torch.empty_like(imgs)
+                    imgs, targets = utils.device_aug.geometric_batch(imgs, targets, out=geom_buf, **geom_hyp)
                 imgs = utils.device_aug.img_aug_batch(imgs, out=imgs, random_resize=opt.device_aug_resize,   # datasets.py:63-68
                                                       augment_hsv=opt.device_aug_hsv,                  # on the device, in place
                                                       motion_blur=opt.device_aug_blur)

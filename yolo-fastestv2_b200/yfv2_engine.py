@@ -291,6 +291,12 @@ class AugBlur(ctypes.Structure):
     _fields_ = [("ksize", ctypes.c_int), ("taps", ctypes.c_float * 9)]
 
 
+class AugGeom(ctypes.Structure):
+    """yfv2_aug_geom: one image's mosaic canvas, random_perspective matrix (canvas -> output) and fliplr."""
+    _fields_ = [("m", ctypes.c_double * 9), ("perspective", ctypes.c_int), ("mosaic", ctypes.c_int), ("src", ctypes.c_int * 4),
+                ("xc", ctypes.c_int), ("yc", ctypes.c_int), ("flip", ctypes.c_int)]
+
+
 class JpegInfo(ctypes.Structure):
     """yfv2_jpeg_info: what yfv2_jpeg_parse found in one file."""
     _fields_ = [("status", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int), ("components", ctypes.c_int),
@@ -351,6 +357,8 @@ PROTOTYPES = {
     "yfv2_aug_batch_blur": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                            ctypes.POINTER(AugParams), ctypes.c_void_p, ctypes.POINTER(AugBlur), ctypes.c_int,
                                            ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "yfv2_aug_geometric": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                          ctypes.POINTER(AugGeom), ctypes.c_void_p]),
     "yfv2_debug_bgr2hsv": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_void_p]),
     "yfv2_debug_hsv2bgr": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_int, ctypes.c_void_p]),
     "yfv2_jpeg_encode_plan": (ctypes.c_int, [ctypes.POINTER(JpegEncSrc), ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
@@ -1073,6 +1081,42 @@ def augment_batch(imgs, alpha=None, beta=None, rw=None, rh=None, luts=None, out=
         ws = torch.empty(nb.value, dtype=torch.uint8, device=imgs.device)
         _check(lib().yfv2_aug_batch_blur(p(imgs), p(out), N, H, W, params, p(lut_dev), desc, flags | AUG_BLUR, p(ws), nb.value,
                                          _stream(imgs.device)), "aug_batch_blur")
+    return out
+
+
+def geom_descriptors(params):
+    """The yfv2_aug_geom array of augment_geometric's params (dicts with M, perspective, mosaic, src, xc, yc, flip)."""
+    desc = (AugGeom * len(params))()
+    for i, p in enumerate(params):
+        d = desc[i]
+        d.m[:] = [float(v) for v in np.asarray(p["M"], np.float64).reshape(-1)[:9]]
+        d.perspective, d.mosaic, d.flip = int(p["perspective"]), int(p["mosaic"]), int(p["flip"])
+        d.src[:] = [int(v) for v in p["src"]]
+        d.xc, d.yc = int(p.get("xc", 0)), int(p.get("yc", 0))
+    return desc
+
+
+def augment_geometric(imgs, params, out=None):
+    """YOLOv5's geometric augmentation on a CUDA uint8 [N, 3, H, W] planar BGR batch (yfv2_aug_geometric): per output image,
+    load_mosaic's canvas (or the image src[0] alone), cv2.warpAffine / cv2.warpPerspective of it by M with borderValue 114, then
+    np.fliplr.  params: N dicts (utils.device_aug.draw_geometric returns them) with M (3x3, canvas -> output, as cv2 receives it),
+    perspective, mosaic, src (4 batch indices; src[0] alone without mosaic), xc, yc and flip.  Returns a new tensor, or writes
+    `out`, which must not overlap `imgs`."""
+    _require_cuda(imgs, "imgs")
+    if imgs.dtype != torch.uint8 or imgs.dim() != 4 or imgs.shape[1] != 3:
+        raise TypeError("augment_geometric expects uint8 [N, 3, H, W] images")
+    imgs = imgs.contiguous()
+    N, _, H, W = imgs.shape
+    if len(params) != N:
+        raise ValueError("one geometric descriptor per image")
+    desc = geom_descriptors(params)
+    if out is None:
+        out = torch.empty_like(imgs)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != tuple(imgs.shape) or not out.is_contiguous() or out.device != imgs.device:
+        raise ValueError("out must be a contiguous uint8 tensor of the batch's shape on its device")
+    with torch.cuda.device(imgs.device):
+        _check(lib().yfv2_aug_geometric(ctypes.c_void_p(imgs.data_ptr()), ctypes.c_void_p(out.data_ptr()), N, H, W, desc,
+                                        _stream(imgs.device)), "aug_geometric")
     return out
 
 
