@@ -180,6 +180,25 @@ typedef struct yfv2_region {
 YFV2_API int yfv2_merge_regions(const float* dets, const int* counts, const yfv2_region* regions, int T, int max_det_in, int F,
                                 int H, int W, double thr, int metric, int max_det, double* out, int* out_counts, int* kept_src,
                                 void* stream);
+/* Greedy non-maximum merging (NMM): yfv2_merge_regions, but each kept row's box grows to the union of the boxes it absorbed, so an
+ * object cut by a tile's edge comes out whole even when the cut piece scored highest.  Same arguments plus `merged` (optional, may
+ * be NULL): [F, max_det] int.  Same limits, same checks before any launch, no workspace, no synchronisation.  Per frame, bit-exact
+ * to tests/region_nmm_oracle.py:
+ *   1. steps 1-5 above, unchanged: the kept rows, their order, conf, cls, kept_src and out_counts are those yfv2_merge_regions
+ *      writes for the same input; only the four box columns may differ.
+ *   2. absorb: every mapped row j that is not an output row (NaN conf rows are already gone), rows after the max_det cap
+ *      included, belongs to the FIRST output row i before j in the order that matches it by step 3's test (other region, same
+ *      cls, overlap(box_i, box_j) > thr on the mapped boxes).  A row suppressed before the last output row always has one (the
+ *      row that suppressed it); a row after the cap has none when no output row matches it.
+ *   3. fold: per output row i, B = box_i; for each absorbed row j in the order: if overlap(B, box_j) > thr (step 4, B in the kept
+ *      row's place of min / max) then B = (min(B.x1, j.x1), min(B.y1, j.y1), max(B.x2, j.x2), max(B.y2, j.y2)), B's value first
+ *      in step 4's min / max, and merged[f, i] += 1.  A NaN overlap does not fold.  conf and cls stay row i's; out gets B.
+ *   4. fp64, one rounding per operation, no FMA; no atomics whose order reaches the output.  merged is 0 past out_counts[f].
+ * Known differences from SAHI's GreedyNMMPostprocess: both tests are strict (SAHI uses >= to group, > to re-check), fp64 (SAHI
+ * float32), rows of one region never merge (its own NMS separated them), and there is no class-agnostic mode. */
+YFV2_API int yfv2_merge_regions_nmm(const float* dets, const int* counts, const yfv2_region* regions, int T, int max_det_in,
+                                    int F, int H, int W, double thr, int metric, int max_det, double* out, int* out_counts,
+                                    int* kept_src, int* merged, void* stream);
 
 /* ---- multi-object tracking across video frames: ByteTrack's association and lifecycle, S streams in one device state ---------
  * No reference counterpart (the reference detects on single images).  The tracker keeps S streams (cameras) of at most K tracks

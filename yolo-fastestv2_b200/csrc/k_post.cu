@@ -962,6 +962,20 @@ __device__ __forceinline__ bool overlap_gt(const double4& a, const double4& b, d
     return __ddiv_rn(inter, den) > thr;
 }
 
+// Row `slot` (t_local * max_det_in + row) of the frame whose first region is tg0 (rb in a.reg): its box mapped to frame pixels
+// (contract step 1), its region relative to the frame's first (tl) and its row in dets (r: r[4] conf, r[5] cls).
+__device__ __forceinline__ double4 map_row(const MergeArgs& a, long long tg0, int rb, unsigned int slot, int& tl, const float*& r) {
+    const int mdi = a.max_det_in;
+    tl = (int)slot / mdi;
+    const int row = (int)slot - tl * mdi;
+    r = a.dets + ((tg0 + tl) * mdi + row) * 6;
+    const int4 g = a.reg[rb + tl];
+    const double sx = __ddiv_rn((double)g.z, (double)a.W), sy = __ddiv_rn((double)g.w, (double)a.H);
+    const double x0 = (double)g.x, y0 = (double)g.y;
+    return make_double4(__dadd_rn(__dmul_rn((double)__ldg(r), sx), x0), __dadd_rn(__dmul_rn((double)__ldg(r + 1), sy), y0),
+                        __dadd_rn(__dmul_rn((double)__ldg(r + 2), sx), x0), __dadd_rn(__dmul_rn((double)__ldg(r + 3), sy), y0));
+}
+
 // The merge's side of greedy_pass: candidates staged from the rows in global memory, mapped to frame pixels; a box suppresses
 // only boxes of other regions and the same class.
 struct MergePass {
@@ -973,15 +987,10 @@ struct MergePass {
     int rb;                                                      // the frame's first region in a.reg
 
     __device__ __forceinline__ void stage(int j, unsigned long long key) const {
-        const int mdi = a.max_det_in;
         const unsigned int slot = 0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull);
-        const int tl = (int)slot / mdi, row = (int)slot - tl * mdi;
-        const float* r = a.dets + ((tg0 + tl) * mdi + row) * 6;
-        const int4 g = a.reg[rb + tl];
-        const double sx = __ddiv_rn((double)g.z, (double)a.W), sy = __ddiv_rn((double)g.w, (double)a.H);
-        const double x0 = (double)g.x, y0 = (double)g.y;
-        s.chbox[j] = make_double4(__dadd_rn(__dmul_rn((double)__ldg(r), sx), x0), __dadd_rn(__dmul_rn((double)__ldg(r + 1), sy), y0),
-                                  __dadd_rn(__dmul_rn((double)__ldg(r + 2), sx), x0), __dadd_rn(__dmul_rn((double)__ldg(r + 3), sy), y0));
+        int tl;
+        const float* r;
+        s.chbox[j] = map_row(a, tg0, rb, slot, tl, r);
         s.chcls[j] = __ldg(r + 5);
         s.cht[j] = (unsigned short)tl;
     }
@@ -1010,6 +1019,42 @@ struct MergePass {
         if (ksrc) ksrc[pos] = (int)(tg0 * a.max_det_in + slot);
     }
 };
+
+// Candidates of frame block fl into s.keys, sorted descending (contract step 2); returns their number.  All threads call this.
+// (merge_regions_kernel spells the same steps out inline: calling this helper there reschedules its SASS.)
+__device__ __forceinline__ int merge_candidates(const MergeArgs& a, const MergeSmem& s, int fl) {
+    const int t = threadIdx.x;
+    const int rb = a.rbeg[fl], nreg = a.rbeg[fl + 1] - rb;
+    const int mdi = a.max_det_in;
+    const long long tg0 = (long long)a.t0 + rb;
+    if (t == 0) s.misc[0] = 0u;
+    __syncthreads();
+    // candidates: rows below each region's count whose conf is not NaN, keyed by (conf, then lower t, then lower row first)
+    const int nslots = nreg * mdi;
+    for (int base = 0; base < nslots; base += NT) {
+        const int slot = base + t;
+        bool want = false;
+        unsigned long long key = 0ull;
+        if (slot < nslots) {
+            const int tl = slot / mdi, row = slot - tl * mdi;
+            const int cnt = min(max(__ldg(a.counts + tg0 + tl), 0), mdi);
+            if (row < cnt) {
+                const float conf = __ldg(a.dets + ((tg0 + tl) * mdi + row) * 6 + 4);
+                if (!isnan(conf)) {
+                    want = true;
+                    // + 0 turns -0 into +0, so that the two zeros tie like any equal confidences
+                    key = ((unsigned long long)f2sortable(__fadd_rn(conf, 0.0f)) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)slot);
+                }
+            }
+        }
+        const unsigned int pos = alloc_slots(&s.misc[0], want);
+        if (want) s.keys[pos] = key;
+    }
+    __syncthreads();
+    const int cnt = (int)s.misc[0];
+    sort_keys_desc(s.keys, cnt);
+    return cnt;
+}
 
 __global__ void __launch_bounds__(NT)
 merge_regions_kernel(const __grid_constant__ MergeArgs a) {
@@ -1053,6 +1098,102 @@ merge_regions_kernel(const __grid_constant__ MergeArgs a) {
     if (t == 0) a.out_counts[f] = nk;
     for (int i = nk * 6 + t; i < a.max_det * 6; i += NT) out[i] = 0.0;
     if (ksrc) for (int i = nk + t; i < a.max_det; i += NT) ksrc[i] = -1;
+}
+
+// Greedy non-maximum merging (yfv2_merge_regions_nmm): merge_regions_kernel's pass, which also marks the output rows by slot in
+// `kept` (one bit per candidate slot), then
+//   absorb: every other sorted row, after the cap too, scans the kept boxes in order and stops at the first one that would
+//           suppress it (step 3's test).  The first matching kept row comes before the row: a kept row before it that matches
+//           suppressed it, and a row after the last kept one comes after all of them.  Each absorbed row becomes the grouping key
+//           (0xFFFF - absorber) << 32 | (0xFFFF - sorted position) << 16 | slot, compacted to the front of the key buffer (a
+//           tile's writes land below the next tile's reads) and sorted descending: absorbers ascending, each group in order.
+//   fold:   the thread holding a group's first key grows the absorber's box B through the group, re-testing each row against B.
+// All sizes fit 16 bits: absorber < 4096, sorted position and slot < YFV2_NMS_MAX_CAND.  The bitmap is the only shared memory
+// added to merge_regions_kernel's (MCp / 8 bytes, 1 KB at the limit).
+struct MergeNmmPass : MergePass {
+    unsigned int* kept;
+    __device__ __forceinline__ void append(int pos, int j, const unsigned long long& key) const {
+        MergePass::append(pos, j, key);
+        const unsigned int slot = 0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull);
+        atomicOr(&kept[slot >> 5], 1u << (slot & 31));
+    }
+};
+
+inline size_t merge_nmm_smem_bytes(int MCp, int KC) { return merge_smem_bytes(MCp, KC) + (size_t)MCp / 8; }
+
+__global__ void __launch_bounds__(NT)
+merge_regions_nmm_kernel(const __grid_constant__ MergeArgs a, int* merged) {
+    extern __shared__ __align__(32) unsigned char smraw[];
+    MergeSmem s;
+    unsigned char* tail = merge_layout(s, smraw, a.MCp, a.KC);
+    unsigned int* kept = take<unsigned int>(tail, a.MCp / 32);
+    const int t = threadIdx.x, fl = blockIdx.x, f = a.f0 + fl;
+    const int rb = a.rbeg[fl];
+    const long long tg0 = (long long)a.t0 + rb;
+    double* out = a.out + (long long)f * a.max_det * 6;
+    int* ksrc = a.kept_src ? a.kept_src + (long long)f * a.max_det : nullptr;
+    for (int i = t; i < a.MCp / 32; i += NT) kept[i] = 0u;
+    const int cnt = merge_candidates(a, s, fl);
+    const int nk = greedy_pass(s.keys, cnt, a.max_det, s.cmask, s.misc + 1, MergeNmmPass{{a, s, out, ksrc, tg0, rb}, kept});
+    if (t == 0) a.out_counts[f] = nk;
+    for (int i = nk * 6 + t; i < a.max_det * 6; i += NT) out[i] = 0.0;
+    if (ksrc) for (int i = nk + t; i < a.max_det; i += NT) ksrc[i] = -1;
+    int* mrg = merged ? merged + (long long)f * a.max_det : nullptr;
+    if (mrg) for (int i = t; i < a.max_det; i += NT) mrg[i] = 0;   // ordered before the fold's writes by the barriers between
+
+    // absorb
+    if (t == 0) s.misc[0] = 0u;
+    __syncthreads();
+    for (int base = 0; base < cnt; base += NT) {
+        const int p = base + t;
+        bool want = false;
+        unsigned long long g = 0ull;
+        if (p < cnt) {
+            const unsigned int slot = 0xFFFFFFFFu - (unsigned int)(s.keys[p] & 0xFFFFFFFFull);
+            if (!((kept[slot >> 5] >> (slot & 31)) & 1u)) {
+                int tl;
+                const float* r;
+                const double4 box = map_row(a, tg0, rb, slot, tl, r);
+                const float cls = __ldg(r + 5);
+                for (int i = 0; i < nk; ++i) {
+                    if (s.kt[i] != tl && s.kcls[i] == cls && overlap_gt(s.kbox[i], box, a.thr, a.metric)) {
+                        want = true;
+                        g = ((unsigned long long)(0xFFFFu - (unsigned)i) << 32) | ((unsigned long long)(0xFFFFu - (unsigned)p) << 16) | slot;
+                        break;
+                    }
+                }
+            }
+        }
+        __syncthreads();                                         // the tile's keys are read
+        const unsigned int pos = alloc_slots(&s.misc[0], want);
+        if (want) s.keys[pos] = g;
+    }
+    __syncthreads();
+    const int ng = (int)s.misc[0];
+    sort_keys_desc(s.keys, ng);
+
+    // fold
+    for (int k = t; k < ng; k += NT) {
+        const unsigned int gi = (unsigned int)(s.keys[k] >> 32);
+        if (k > 0 && (unsigned int)(s.keys[k - 1] >> 32) == gi) continue;
+        const int i = (int)(0xFFFFu - gi);
+        double4 B = s.kbox[i];
+        int m = 0;
+        for (int q = k; q < ng; ++q) {
+            const unsigned long long key = s.keys[q];
+            if ((unsigned int)(key >> 32) != gi) break;
+            int tl;
+            const float* r;
+            const double4 b = map_row(a, tg0, rb, (unsigned int)(key & 0xFFFFu), tl, r);
+            if (overlap_gt(B, b, a.thr, a.metric)) {
+                B = make_double4(dmin(B.x, b.x), dmin(B.y, b.y), dmax(B.z, b.z), dmax(B.w, b.w));
+                ++m;
+            }
+        }
+        double* o = out + i * 6;
+        o[0] = B.x; o[1] = B.y; o[2] = B.z; o[3] = B.w;
+        if (mrg) mrg[i] = m;
+    }
 }
 
 long long* g_nms_prof = nullptr;       // yfv2_debug_nms_profile
@@ -1220,18 +1361,21 @@ extern "C" int yfv2_debug_nms_profile(long long* dev_buf) {
     return YFV2_OK;
 }
 
-extern "C" int yfv2_merge_regions(const float* dets, const int* counts, const yfv2_region* regions, int T, int max_det_in, int F,
-                                  int H, int W, double thr, int metric, int max_det, double* out, int* out_counts, int* kept_src,
-                                  void* stream) {
-    if (!dets || !counts || !regions || !out || !out_counts) { set_error("merge_regions: null dets / counts / regions / out / out_counts"); return YFV2_EINVAL; }
-    if (T < 1 || F < 1 || W < 1 || H < 1) { set_error("merge_regions: need T, F, W, H >= 1 (T=%d F=%d W=%d H=%d)", T, F, W, H); return YFV2_EINVAL; }
+namespace yfv2 {
+namespace {
+// yfv2_merge_regions (nmm false) and yfv2_merge_regions_nmm: the same checks, launches and layout; `who` names the call in errors.
+int merge_regions_run(const char* who, bool nmm, const float* dets, const int* counts, const yfv2_region* regions, int T,
+                      int max_det_in, int F, int H, int W, double thr, int metric, int max_det, double* out, int* out_counts,
+                      int* kept_src, int* merged, void* stream) {
+    if (!dets || !counts || !regions || !out || !out_counts) { set_error("%s: null dets / counts / regions / out / out_counts", who); return YFV2_EINVAL; }
+    if (T < 1 || F < 1 || W < 1 || H < 1) { set_error("%s: need T, F, W, H >= 1 (T=%d F=%d W=%d H=%d)", who, T, F, W, H); return YFV2_EINVAL; }
     if (max_det_in < 1 || max_det_in > 4096 || max_det < 1 || max_det > 4096) {
-        set_error("merge_regions: max_det_in=%d and max_det=%d must be in 1..4096", max_det_in, max_det);
+        set_error("%s: max_det_in=%d and max_det=%d must be in 1..4096", who, max_det_in, max_det);
         return YFV2_EINVAL;
     }
-    if (metric != 0 && metric != 1) { set_error("merge_regions: metric=%d (0: IoU, 1: IoS)", metric); return YFV2_EINVAL; }
-    if (thr != thr) { set_error("merge_regions: thr is NaN"); return YFV2_EINVAL; }
-    if ((long long)T * max_det_in > INT_MAX) { set_error("merge_regions: T * max_det_in = %lld rows exceeds 2^31 - 1", (long long)T * max_det_in); return YFV2_EINVAL; }
+    if (metric != 0 && metric != 1) { set_error("%s: metric=%d (0: IoU, 1: IoS)", who, metric); return YFV2_EINVAL; }
+    if (thr != thr) { set_error("%s: thr is NaN", who); return YFV2_EINVAL; }
+    if ((long long)T * max_det_in > INT_MAX) { set_error("%s: T * max_det_in = %lld rows exceeds 2^31 - 1", who, (long long)T * max_det_in); return YFV2_EINVAL; }
     int run = 0;                                                   // regions of the current frame
     for (int t = 0; t < T; ++t) {
         const yfv2_region& r = regions[t];
@@ -1241,19 +1385,19 @@ extern "C" int yfv2_merge_regions(const float* dets, const int* counts, const yf
         else if (r.frame < 0 || r.frame >= F) why = "frame outside [0, F)";
         else if (t && r.frame < regions[t - 1].frame) why = "frame index decreases (regions of a frame must be contiguous, frames ascending)";
         if (why) {
-            set_error("merge_regions: region %d: %s (frame %d of F=%d, x0 %d, y0 %d, %dx%d)", t, why, r.frame, F, r.x0, r.y0, r.w, r.h);
+            set_error("%s: region %d: %s (frame %d of F=%d, x0 %d, y0 %d, %dx%d)", who, t, why, r.frame, F, r.x0, r.y0, r.w, r.h);
             return YFV2_EINVAL;
         }
         run = (t && r.frame == regions[t - 1].frame) ? run + 1 : 1;
         if (run > YFV2_MERGE_MAX_REGIONS || (long long)run * max_det_in > YFV2_NMS_MAX_CAND) {
-            set_error("merge_regions: region %d: frame %d has %d regions x max_det_in %d: more than %d regions or %d candidates", t,
+            set_error("%s: region %d: frame %d has %d regions x max_det_in %d: more than %d regions or %d candidates", who, t,
                       r.frame, run, max_det_in, YFV2_MERGE_MAX_REGIONS, YFV2_NMS_MAX_CAND);
             return YFV2_EINVAL;
         }
     }
     // launches of whole frames: at most kMergeFrames frames and YFV2_MERGE_MAX_REGIONS regions each
     std::unique_ptr<MergeArgs> ap(new (std::nothrow) MergeArgs);  // 17 KB of kernel parameters: on the heap, not the stack
-    if (!ap) { set_error("merge_regions: host allocation failed"); return YFV2_ENOMEM; }
+    if (!ap) { set_error("%s: host allocation failed", who); return YFV2_ENOMEM; }
     MergeArgs& a = *ap;
     a.dets = dets; a.counts = counts; a.out = out; a.out_counts = out_counts; a.kept_src = kept_src;
     a.thr = thr; a.W = W; a.H = H; a.max_det_in = max_det_in; a.max_det = max_det; a.metric = metric;
@@ -1277,12 +1421,33 @@ extern "C" int yfv2_merge_regions(const float* dets, const int* counts, const yf
         const int slots = most * max_det_in;
         a.MCp = pow2_at_least(slots);
         a.KC = std::max(1, std::min(max_det, slots));
-        const size_t bytes = merge_smem_bytes(a.MCp, a.KC);
-        if (bytes > kSmemCap) { set_error("merge_regions: %zu bytes of shared memory needed", bytes); return YFV2_EUNSUPPORTED; }
-        YFV2_CUDA(cudaFuncSetAttribute(merge_regions_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-        merge_regions_kernel<<<nf, NT, bytes, (cudaStream_t)stream>>>(a);
+        const size_t bytes = nmm ? merge_nmm_smem_bytes(a.MCp, a.KC) : merge_smem_bytes(a.MCp, a.KC);
+        if (bytes > kSmemCap) { set_error("%s: %zu bytes of shared memory needed", who, bytes); return YFV2_EUNSUPPORTED; }
+        if (nmm) {
+            YFV2_CUDA(cudaFuncSetAttribute(merge_regions_nmm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+            merge_regions_nmm_kernel<<<nf, NT, bytes, (cudaStream_t)stream>>>(a, merged);
+        } else {
+            YFV2_CUDA(cudaFuncSetAttribute(merge_regions_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+            merge_regions_kernel<<<nf, NT, bytes, (cudaStream_t)stream>>>(a);
+        }
         YFV2_LAUNCH_CHECK();
         f0 += nf;
     }
     return YFV2_OK;
+}
+}  // namespace
+}  // namespace yfv2
+
+extern "C" int yfv2_merge_regions(const float* dets, const int* counts, const yfv2_region* regions, int T, int max_det_in, int F,
+                                  int H, int W, double thr, int metric, int max_det, double* out, int* out_counts, int* kept_src,
+                                  void* stream) {
+    return yfv2::merge_regions_run("merge_regions", false, dets, counts, regions, T, max_det_in, F, H, W, thr, metric, max_det, out,
+                                   out_counts, kept_src, nullptr, stream);
+}
+
+extern "C" int yfv2_merge_regions_nmm(const float* dets, const int* counts, const yfv2_region* regions, int T, int max_det_in,
+                                      int F, int H, int W, double thr, int metric, int max_det, double* out, int* out_counts,
+                                      int* kept_src, int* merged, void* stream) {
+    return yfv2::merge_regions_run("merge_regions_nmm", true, dets, counts, regions, T, max_det_in, F, H, W, thr, metric, max_det,
+                                   out, out_counts, kept_src, merged, stream);
 }

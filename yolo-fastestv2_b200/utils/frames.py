@@ -126,15 +126,17 @@ def tile_regions(w, h, cols, rows, overlap=0.2, full_frame=True, layout="bgr"):
 
 
 def detect_regions(model, frames, cfg, regions, conf_thres=0.3, iou_thres=0.4, layout="bgr", merge="ios", merge_thres=0.5,
-                   max_det=1000, batch=256):
+                   max_det=1000, batch=256, merge_mode="nms"):
     """Detections on regions of frames, merged per frame: a list of float64 CPU [n_i, 6] tensors (x1, y1, x2, y2, conf, cls) in
     pixels of each frame, descending conf, like detect_frames.  regions: one list of (x0, y0, w, h) per frame (may be empty).
     Each region is cropped in place (crop_frame), stretched to cfg's width x height by resize_frames, run through the uint8 forward
     and the fused decode + NMS (conf_thres, iou_thres, 300 rows per region), in chunks of at most `batch` region images.  The rows
     of all regions then go through one yfv2_merge_regions call: mapped to frame pixels, sorted by conf, and a row is dropped when a
     kept row of ANOTHER region and the same class overlaps it by more than merge_thres ("ios": intersection over the smaller box,
-    which removes the part of an object cut by a tile's edge; "iou"); at most max_det rows per frame.  Host frames are copied to
-    the device once; nothing is copied back before the merge.  With one whole-frame region per frame this is detect_frames."""
+    which removes the part of an object cut by a tile's edge; "iou"); at most max_det rows per frame.  merge_mode "nmm" keeps the
+    same rows but grows each kept box to the union of the rows it absorbed (greedy non-maximum merging, yfv2_merge_regions_nmm),
+    so an object cut by a tile's edge comes out whole even when the cut piece scored highest.  Host frames are copied to the
+    device once; nothing is copied back before the merge.  With one whole-frame region per frame this is detect_frames."""
     frames = list(frames)
     layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
     regions = [list(r) for r in regions]
@@ -142,6 +144,8 @@ def detect_regions(model, frames, cfg, regions, conf_thres=0.3, iou_thres=0.4, l
         raise yfv2_engine.Yfv2Error("detect_regions: %d frames, %d layouts, %d region lists" % (len(frames), len(layouts), len(regions)))
     if merge not in yfv2_engine.MERGE_METRICS:
         raise yfv2_engine.Yfv2Error("detect_regions: merge must be 'iou' or 'ios', got %r" % (merge,))
+    if merge_mode not in yfv2_engine.MERGE_MODES:
+        raise yfv2_engine.Yfv2Error("detect_regions: merge_mode must be 'nms' or 'nmm', got %r" % (merge_mode,))
     if int(batch) < 1:
         raise yfv2_engine.Yfv2Error("detect_regions: batch must be >= 1, got %r" % (batch,))
     dev = next(model.parameters()).device
@@ -168,7 +172,7 @@ def detect_regions(model, frames, cfg, regions, conf_thres=0.3, iou_thres=0.4, l
         out, cnt, _ = yfv2_engine.decode_nms(preds, cfg, conf_thres, iou_thres)
         dets[k:k + batch].copy_(out)
         counts[k:k + batch].copy_(cnt)
-    out, n, _ = yfv2_engine.merge_regions(dets, counts, descs, F, W, H, merge_thres, merge, max_det)
+    out, n, _ = yfv2_engine.merge_regions(dets, counts, descs, F, W, H, merge_thres, merge, max_det, mode=merge_mode)
     out, n = out.cpu(), n.cpu().tolist()
     return [out[i, :n[i]].clone() for i in range(F)]
 

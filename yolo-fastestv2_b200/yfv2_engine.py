@@ -339,6 +339,9 @@ PROTOTYPES = {
     "yfv2_merge_regions": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Region), ctypes.c_int, ctypes.c_int,
                                           ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_int, ctypes.c_int,
                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "yfv2_merge_regions_nmm": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Region), ctypes.c_int, ctypes.c_int,
+                                              ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_int, ctypes.c_int,
+                                              ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "yfv2_track_state_bytes": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_size_t)]),
     "yfv2_track_reset": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.c_int,
                                         ctypes.c_void_p]),
@@ -835,14 +838,22 @@ def decode_nms(preds, cfg, conf_thres=0.3, iou_thres=0.45, classes=None, max_det
 
 
 MERGE_METRICS = {"iou": 0, "ios": 1}
+MERGE_MODES = ("nms", "nmm")
 
 
-def merge_regions(dets, counts, regions, F, W, H, thr, metric, max_det):
+def merge_regions(dets, counts, regions, F, W, H, thr, metric, max_det, mode="nms", want_merged=False):
     """yfv2_merge_regions: the NMS rows of T region images -> one list per frame in frame pixels (a cross-region NMS, see
     include/yfv2.h).  dets: CUDA float32 [T, max_det_in, 6] and counts int32 [T], as decode_nms / nms return them for the region
     images; regions: T tuples (frame, x0, y0, w, h), the regions of one frame contiguous, frames ascending; F frames; W x H the
     network input the regions were stretched to; metric "iou" | "ios" (or 0 | 1).  Returns CUDA tensors (out float64
-    [F, max_det, 6], counts int32 [F], kept_src int32 [F, max_det]: t * max_det_in + row of each kept row, -1 past the count)."""
+    [F, max_det, 6], counts int32 [F], kept_src int32 [F, max_det]: t * max_det_in + row of each kept row, -1 past the count).
+    mode "nmm" runs yfv2_merge_regions_nmm instead: the same rows, counts and kept_src, with each kept box grown to the union of
+    the rows it absorbed (greedy non-maximum merging).  want_merged (nmm only) appends a fourth tensor, int32 [F, max_det]: how
+    many rows each kept box absorbed (0 past the count)."""
+    if mode not in MERGE_MODES:
+        raise Yfv2Error("merge_regions: mode must be 'nms' or 'nmm', got %r" % (mode,))
+    if want_merged and mode != "nmm":
+        raise Yfv2Error("merge_regions: want_merged needs mode='nmm'")
     _require_cuda(dets, "dets")
     _require_cuda(counts, "counts")
     if dets.dim() != 3 or dets.shape[2] != 6 or dets.dtype != torch.float32:
@@ -864,12 +875,17 @@ def merge_regions(dets, counts, regions, F, W, H, thr, metric, max_det):
     out = torch.empty((max(F, 0), max_det, 6), dtype=torch.float64, device=dev)
     out_counts = torch.empty((max(F, 0),), dtype=torch.int32, device=dev)
     kept = torch.empty((max(F, 0), max_det), dtype=torch.int32, device=dev)
+    merged = torch.empty((max(F, 0), max_det), dtype=torch.int32, device=dev) if want_merged else None
     with torch.cuda.device(dev):
-        _check(lib().yfv2_merge_regions(ctypes.c_void_p(dets.data_ptr()), ctypes.c_void_p(counts.data_ptr()), descs, T, max_det_in, F,
-                                        H, W, ctypes.c_double(thr), m, max_det, ctypes.c_void_p(out.data_ptr()),
-                                        ctypes.c_void_p(out_counts.data_ptr()), ctypes.c_void_p(kept.data_ptr()), _stream(dev)),
-               "merge_regions")
-    return out, out_counts, kept
+        args = (ctypes.c_void_p(dets.data_ptr()), ctypes.c_void_p(counts.data_ptr()), descs, T, max_det_in, F, H, W,
+                ctypes.c_double(thr), m, max_det, ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(out_counts.data_ptr()),
+                ctypes.c_void_p(kept.data_ptr()))
+        if mode == "nmm":
+            _check(lib().yfv2_merge_regions_nmm(*args, ctypes.c_void_p(merged.data_ptr()) if want_merged else None, _stream(dev)),
+                   "merge_regions_nmm")
+        else:
+            _check(lib().yfv2_merge_regions(*args, _stream(dev)), "merge_regions")
+    return (out, out_counts, kept, merged) if want_merged else (out, out_counts, kept)
 
 
 class Tracker:
