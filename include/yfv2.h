@@ -275,6 +275,65 @@ YFV2_API int yfv2_track_update(void* state, int S, int K, const int* streams_hos
 YFV2_API int yfv2_track_debug_read(const void* state, int S, int K, int s, int* frame_host, int* next_id_host, yfv2_track* tracks_host,
                                    int* n_host, void* stream);
 
+/* ---- line crossings and zone occupancy of tracked objects, S streams in one device state, read from the tracker's state ---------
+ * A counter keeps, for each of the tracker's S streams, that stream's geometry (at most L directed lines and Z zones of at most P
+ * vertices), one record per track slot and running totals, in one caller-owned device buffer of yfv2_count_state_bytes(S, K, L, Z,
+ * P) bytes, zeroed by the caller before first use (no geometry, no records, zero totals).  yfv2_count_set_geometry copies one
+ * stream's geometry from the host and clears that stream's records and totals; a stream without geometry counts nothing.
+ * yfv2_count_reset clears records and totals of chosen streams and keeps their geometry: the tracker restarts ids at 1 when one
+ * of its streams is reset, so reset the counter's stream with it.  One yfv2_count_update call reads the tracker state (S, K as
+ * given to the tracker) of B distinct streams in ONE launch with one CTA per stream; it allocates nothing and never synchronises.
+ * Bit-exact to tests/count_oracle.py.
+ *
+ * Arithmetic: IEEE fp64, one rounding per operation, no FMA.  Anchor of a track: (x1, y1, x2, y2) = the box yfv2_track_update
+ * writes to out for it; ax = (x1 + x2) / 2, ay = y2, in the pixels of the frame given to the tracker.
+ * A track APPEARS at an update when it is confirmed and tracked (exactly the rows of the tracker's out).  Its record is created
+ * at its first appearance and lives while the track is live in the tracker; ids are never reused, so a record keyed by slot and
+ * checked against the slot's id is one keyed by id.  A record keeps the anchor of its last appearance, per line the last nonzero
+ * side (0: none yet) and per zone whether that anchor was inside.
+ * Lines: a directed segment A -> B, A != B, fp64.  o(A, B, P) = (B.x - A.x)*(P.y - A.y) - (B.y - A.y)*(P.x - A.x); side(P) =
+ * sign(o(A, B, P)).  At an appearance with anchor Q, P the record's anchor, stored its side: a crossing is counted iff stored != 0,
+ * side(Q) = -stored and the closed segments PQ and AB meet: sign(o(A,B,P))*sign(o(A,B,Q)) <= 0 and sign(o(P,Q,A))*sign(o(P,Q,B))
+ * <= 0.  Its dir is side(Q).  Then stored = side(Q) if nonzero.  So a step onto the line and off it counts once, on the step
+ * off; a pass around an end of the segment counts nothing but flips the stored side; a track lost and found again on the other
+ * side counts when found.
+ * Zones: 3..P float32 vertices.  inside(Q) is cv2.pointPolygonTest(contour, (float)Q, false) >= 0 (the boundary is inside):
+ * the anchor rounded to float32; for each edge (v0 = the previous vertex, v): skipped when (v0.y <= y && v.y <= y) || (v0.y > y
+ * && v.y > y) || (v0.x < x && v.x < x), and then on the boundary iff y == v.y && (x == v.x || (y == v0.y && x between v0.x and
+ * v.x)); else dist = (double)(y - v0.y)*(v.x - v0.x) - (double)(x - v0.x)*(v.y - v0.y), the differences in float32: on the
+ * boundary iff dist == 0, and the edge counts iff (v.y < v0.y ? -dist : dist) > 0; inside iff on the boundary or the count is
+ * odd.  An entry / exit is an outside -> inside / inside -> outside change between two appearances of a track; a first
+ * appearance inside is no entry; a removed track makes no exit.  occupancy[b][z] = appearing tracks inside zone z (0 for z past
+ * the stream's zones).
+ * Events, per stream in ascending track id, then lines in order, then zones in order: events [B, E, 8] float64 (kind, index,
+ * dir, track id, cls, ax, ay, tracker frame), kind YFV2_COUNT_LINE (dir = side(Q)), YFV2_COUNT_ENTRY (dir +1) or YFV2_COUNT_EXIT
+ * (dir -1); the first E are written, rows past them are zeros; event_counts [B] = every event, possibly > E.  Totals count every
+ * event: per line, crossings with dir +1 and dir -1; per zone, entries and exits.  A second update without a tracker update in
+ * between emits nothing and changes nothing.
+ * Checked before any launch (YFV2_EINVAL, naming the argument): non-null pointers (events may be null when E = 0);
+ * 1 <= K <= YFV2_TRACK_MAX_CAPACITY; 0 <= L <= YFV2_COUNT_MAX_LINES, 0 <= Z <= YFV2_COUNT_MAX_ZONES, 3 <= P <=
+ * YFV2_COUNT_MAX_VERTICES; 1 <= B <= min(S, YFV2_TRACK_MAX_BATCH), streams in [0, S), each at most once; E >= 0; geometry: finite
+ * coordinates, A != B, nl <= L, nz <= Z, 3..P vertices per zone. */
+#define YFV2_COUNT_MAX_LINES    32
+#define YFV2_COUNT_MAX_ZONES    16
+#define YFV2_COUNT_MAX_VERTICES 64
+#define YFV2_COUNT_LINE  0
+#define YFV2_COUNT_ENTRY 1
+#define YFV2_COUNT_EXIT  2
+YFV2_API int yfv2_count_state_bytes(int S, int K, int L, int Z, int P, size_t* bytes);
+YFV2_API int yfv2_count_reset(void* count_state, int S, int K, int L, int Z, int P, const int* streams_host, int B, void* stream);
+/* stream s: lines_host [nl, 4] (ax, ay, bx, by), zones_host [nz, P, 2] float32 with nverts_host [nz] vertices used per zone */
+YFV2_API int yfv2_count_set_geometry(void* count_state, int S, int K, int L, int Z, int P, int s, const double* lines_host, int nl,
+                                     const float* zones_host, const int* nverts_host, int nz, void* stream);
+YFV2_API int yfv2_count_update(const void* track_state, void* count_state, int S, int K, int L, int Z, int P, const int* streams_host,
+                               int B, int E, double* events, int* event_counts, int* occupancy, void* stream);
+/* test hook, synchronises `stream`: stream s's line and zone counts (geom_host [2]), totals_host [2L + 2Z] (per line +1, -1, then
+ * per zone entries, exits) and the record of every slot: ids_host [K] (0: none), anchors_host [K, 2], sides_host [K, L],
+ * inside_host [K] (bit z: zone z) */
+YFV2_API int yfv2_count_debug_read(const void* count_state, int S, int K, int L, int Z, int P, int s, int* geom_host,
+                                   long long* totals_host, int* ids_host, double* anchors_host, signed char* sides_host,
+                                   unsigned int* inside_host, void* stream);
+
 /* ---- get_batch_statistics (utils/utils.py:184-230): true-positive flags of NMS output rows ----------------
  * dets [N,max_det,6] / counts [N] as yfv2_nms writes them (a count above max_det is taken as max_det); targets [nt,6]
  * rows (image, class, x1, y1, x2, y2) in pixels (what evaluation() builds at utils/utils.py:372-375), in any order and

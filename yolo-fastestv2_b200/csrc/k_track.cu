@@ -9,6 +9,9 @@
 // yfv2_track slots, all in global memory.  A CTA keeps in shared memory what its loops touch many times: the boxes of its tracks
 // and detections, the confidences, the solver's per-row / per-column arrays and the index lists of each stage; the Kalman state
 // of a track is read and written in global memory by the one thread that owns the track.
+//
+// Counting (yfv2_count_*) lives here too, because it reads this layout: one CTA per stream walks the tracker's `ord` and counts
+// line crossings and zone entries, exits and occupancy of the tracks' anchors (tests/count_oracle.py restates it).
 #include <float.h>
 #include <limits.h>
 #include <math.h>
@@ -522,6 +525,238 @@ int check_streams(const char* what, int S, int K, const int* streams, int B, std
     return YFV2_OK;
 }
 
+// ---- line and zone counting (yfv2_count_*): reads the tracker state above, one CTA per stream ---------------------------------
+// Counter state, per stream at s * stride:  int hdr[4] = {nl, nz, 0, 0};  long long totals[2L + 2Z];  double4 lines[L];
+// int nverts[Z];  float2 verts[Z][P];  then the records of the K slots: int id[K];  unsigned inside[K];  double2 anchor[K];
+// signed char side[K][L].
+constexpr int kMaxLines = YFV2_COUNT_MAX_LINES, kMaxZones = YFV2_COUNT_MAX_ZONES, kMaxVerts = YFV2_COUNT_MAX_VERTICES;
+
+struct CountLayout {
+    size_t totals, lines, nverts, verts, rid, rin, rpos, rside, stride;
+};
+
+__host__ __device__ inline size_t up16(size_t v) { return (v + 15) & ~(size_t)15; }
+
+inline CountLayout count_layout(int K, int L, int Z, int P) {
+    CountLayout c;
+    c.totals = 16;
+    c.lines = c.totals + up16((size_t)(2 * L + 2 * Z) * sizeof(long long));
+    c.nverts = c.lines + (size_t)L * sizeof(double4);
+    c.verts = c.nverts + up16((size_t)Z * sizeof(int));
+    c.rid = c.verts + up16((size_t)Z * P * sizeof(float2));
+    c.rin = c.rid + up16((size_t)K * sizeof(int));
+    c.rpos = c.rin + up16((size_t)K * sizeof(unsigned));
+    c.rside = c.rpos + (size_t)K * sizeof(double2);
+    c.stride = (c.rside + (size_t)K * L + 255) & ~(size_t)255;
+    return c;
+}
+
+struct CountArgs {
+    const unsigned char* track;
+    unsigned char* count;
+    size_t track_stride;
+    CountLayout lay;
+    int K, L, Z, P, E;
+    double* events;              // [B, E, 8]
+    int* event_counts;           // [B]
+    int* occupancy;              // [B, Z]
+    int streams[kTrackLaunch];
+};
+
+struct CountResetArgs {
+    unsigned char* count;
+    CountLayout lay;
+    int K, L, Z;
+    int streams[kTrackLaunch];
+};
+
+struct CountSmem {
+    double4 lines[kMaxLines];
+    float2 verts[kMaxZones * kMaxVerts];   // zone z's vertices from z * P on
+    int nverts[kMaxZones];
+    int occ[kMaxZones];
+    int tot[2 * kMaxLines + 2 * kMaxZones];   // this call's events: per line dir +1, dir -1; per zone entries, exits
+    int scratch[NW];
+};
+
+__device__ __forceinline__ double orient(double ax, double ay, double bx, double by, double px, double py) {
+    return __dsub_rn(__dmul_rn(__dsub_rn(bx, ax), __dsub_rn(py, ay)), __dmul_rn(__dsub_rn(by, ay), __dsub_rn(px, ax)));
+}
+
+__device__ __forceinline__ int sgn(double v) { return (v > 0.0) - (v < 0.0); }
+
+// cv2.pointPolygonTest(contour, (x, y), false) >= 0 for a float32 contour of n vertices: the differences in float32, the products
+// and their difference in fp64, as cv2 computes them
+__device__ bool in_polygon(const float2* v, int n, float x, float y) {
+    float2 b = v[n - 1];
+    int crossings = 0;
+    bool edge = false;
+    for (int i = 0; i < n; ++i) {
+        const float2 a = b;
+        b = v[i];
+        if ((a.y <= y && b.y <= y) || (a.y > y && b.y > y) || (a.x < x && b.x < x)) {
+            if (y == b.y && (x == b.x || (y == a.y && ((a.x <= x && x <= b.x) || (b.x <= x && x <= a.x))))) edge = true;
+            continue;
+        }
+        double dist = __dsub_rn(__dmul_rn((double)__fsub_rn(y, a.y), (double)__fsub_rn(b.x, a.x)),
+                                __dmul_rn((double)__fsub_rn(x, a.x), (double)__fsub_rn(b.y, a.y)));
+        if (dist == 0.0) edge = true;
+        if (b.y < a.y) dist = -dist;
+        crossings += dist > 0.0;
+    }
+    return edge || (crossings & 1);
+}
+
+// Exclusive prefix sum of v over the CTA; every thread calls it and gets the CTA's total.
+__device__ int block_scan(int v, int* scratch, int& total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int x = v;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, x, off);
+        if (lane >= off) x += y;
+    }
+    if (lane == 31) scratch[warp] = x;
+    __syncthreads();
+    int before = 0;
+    total = 0;
+#pragma unroll
+    for (int w = 0; w < NW; ++w) {
+        const int c = scratch[w];
+        before += w < warp ? c : 0;
+        total += c;
+    }
+    __syncthreads();
+    return before + x - v;
+}
+
+// One appearance of a track at anchor (qx, qy), in zones `qin`, against its record (fresh: none yet).  Without `write` the
+// events are only counted; with it they are written to ev from position pos on (those below E), and this call's totals and the
+// record's sides are updated.
+__device__ int appear(CountSmem& s, int nl, int nz, bool fresh, double px, double py, double qx, double qy, signed char* side,
+                      unsigned pin, unsigned qin, bool write, double* ev, int pos, int E, double id, double cls, double frame) {
+    int cnt = 0;
+    auto emit = [&](int kind, int index, int dir) {
+        if (write && pos + cnt < E) {
+            double* o = ev + (size_t)(pos + cnt) * 8;
+            o[0] = kind; o[1] = index; o[2] = dir; o[3] = id; o[4] = cls; o[5] = qx; o[6] = qy; o[7] = frame;
+        }
+        ++cnt;
+    };
+    for (int l = 0; l < nl; ++l) {
+        const double4 g = s.lines[l];
+        const int sq = sgn(orient(g.x, g.y, g.z, g.w, qx, qy));
+        const int stored = fresh ? 0 : side[l];
+        if (stored != 0 && sq == -stored && sgn(orient(g.x, g.y, g.z, g.w, px, py)) * sq <= 0 &&
+            sgn(orient(px, py, qx, qy, g.x, g.y)) * sgn(orient(px, py, qx, qy, g.z, g.w)) <= 0) {
+            if (write) atomicAdd(&s.tot[2 * l + (sq > 0 ? 0 : 1)], 1);
+            emit(YFV2_COUNT_LINE, l, sq);
+        }
+        if (write && (sq != 0 || fresh)) side[l] = (signed char)sq;
+    }
+    for (int z = 0; z < nz; ++z) {
+        const unsigned bit = 1u << z;
+        if (fresh || ((pin ^ qin) & bit) == 0) continue;
+        const bool entry = (qin & bit) != 0;
+        if (write) atomicAdd(&s.tot[2 * kMaxLines + 2 * z + (entry ? 0 : 1)], 1);
+        emit(entry ? YFV2_COUNT_ENTRY : YFV2_COUNT_EXIT, z, entry ? 1 : -1);
+    }
+    return cnt;
+}
+
+__global__ void __launch_bounds__(NT)
+count_update_kernel(const __grid_constant__ CountArgs a) {
+    __shared__ CountSmem s;
+    const int t = threadIdx.x, b = blockIdx.x, K = a.K, L = a.L, Z = a.Z, P = a.P, E = a.E;
+    const CountLayout& c = a.lay;
+    const unsigned char* tb = a.track + (size_t)a.streams[b] * a.track_stride;
+    const int* thdr = reinterpret_cast<const int*>(tb);
+    const int* gord = thdr + 4;
+    const yfv2_track* tracks = reinterpret_cast<const yfv2_track*>(tb + tracks_offset(K));
+    unsigned char* cb = a.count + (size_t)a.streams[b] * c.stride;
+    const int* chdr = reinterpret_cast<const int*>(cb);
+    long long* totals = reinterpret_cast<long long*>(cb + c.totals);
+    int* rid = reinterpret_cast<int*>(cb + c.rid);
+    unsigned* rin = reinterpret_cast<unsigned*>(cb + c.rin);
+    double2* rpos = reinterpret_cast<double2*>(cb + c.rpos);
+    signed char* rside = reinterpret_cast<signed char*>(cb + c.rside);
+    const int frame = thdr[0], n = thdr[2], nl = chdr[0], nz = chdr[1];
+
+    const double4* glines = reinterpret_cast<const double4*>(cb + c.lines);
+    const int* gnv = reinterpret_cast<const int*>(cb + c.nverts);
+    const float2* gverts = reinterpret_cast<const float2*>(cb + c.verts);
+    for (int l = t; l < nl; l += NT) s.lines[l] = glines[l];
+    for (int q = t; q < nz * P; q += NT) s.verts[q] = gverts[q];
+    for (int z = t; z < kMaxZones; z += NT) { s.nverts[z] = z < nz ? gnv[z] : 0; s.occ[z] = 0; }
+    for (int q = t; q < 2 * kMaxLines + 2 * kMaxZones; q += NT) s.tot[q] = 0;
+    __syncthreads();
+
+    // ranks of ord are in ascending id: one chunk of NT tracks at a time, the events of a chunk placed by a prefix sum
+    double* ev = a.events + (size_t)b * E * 8;
+    int base = 0;
+    for (int k0 = 0; k0 < n; k0 += NT) {
+        const int k = k0 + t;
+        const int slot = k < n ? gord[k] : 0;
+        const yfv2_track* tr = tracks + slot;
+        const bool app = k < n && tr->state == YFV2_TRACK_TRACKED && tr->confirmed;
+        int cnt = 0, pos = 0, chunk = 0;
+        bool fresh = true;
+        double qx = 0.0, qy = 0.0, px = 0.0, py = 0.0, id = 0.0, cls = 0.0;
+        unsigned pin = 0, qin = 0;
+        if (app) {
+            const double4 bx = track_box(tr->mean);
+            qx = __ddiv_rn(__dadd_rn(bx.x, bx.z), 2.0);
+            qy = bx.w;
+            const float fx = __double2float_rn(qx), fy = __double2float_rn(qy);
+            for (int z = 0; z < nz; ++z)
+                if (in_polygon(s.verts + z * P, s.nverts[z], fx, fy)) { qin |= 1u << z; atomicAdd(&s.occ[z], 1); }
+            fresh = rid[slot] != tr->id;
+            if (!fresh) { const double2 p = rpos[slot]; px = p.x; py = p.y; pin = rin[slot]; }
+            id = (double)tr->id;
+            cls = tr->cls;
+            cnt = appear(s, nl, nz, fresh, px, py, qx, qy, rside + (size_t)slot * L, pin, qin, false, ev, 0, E, id, cls, frame);
+        }
+        pos = base + block_scan(cnt, s.scratch, chunk);
+        if (app) {
+            appear(s, nl, nz, fresh, px, py, qx, qy, rside + (size_t)slot * L, pin, qin, true, ev, pos, E, id, cls, frame);
+            rid[slot] = tr->id;
+            rin[slot] = qin;
+            rpos[slot] = make_double2(qx, qy);
+        }
+        base += chunk;
+    }
+    __syncthreads();
+    for (int e = min(base, E) * 8 + t; e < E * 8; e += NT) ev[e] = 0.0;
+    for (int z = t; z < Z; z += NT) a.occupancy[(size_t)b * Z + z] = s.occ[z];
+    for (int l = t; l < nl; l += NT) { totals[2 * l] += s.tot[2 * l]; totals[2 * l + 1] += s.tot[2 * l + 1]; }
+    for (int z = t; z < nz; z += NT) {
+        totals[2 * L + 2 * z] += s.tot[2 * kMaxLines + 2 * z];
+        totals[2 * L + 2 * z + 1] += s.tot[2 * kMaxLines + 2 * z + 1];
+    }
+    if (t == 0) a.event_counts[b] = base;
+}
+
+__global__ void count_reset_kernel(const __grid_constant__ CountResetArgs a) {
+    unsigned char* cb = a.count + (size_t)a.streams[blockIdx.x] * a.lay.stride;
+    long long* totals = reinterpret_cast<long long*>(cb + a.lay.totals);
+    int* rid = reinterpret_cast<int*>(cb + a.lay.rid);
+    for (int q = threadIdx.x; q < 2 * a.L + 2 * a.Z; q += blockDim.x) totals[q] = 0;
+    for (int k = threadIdx.x; k < a.K; k += blockDim.x) rid[k] = 0;
+}
+
+int check_count_dims(const char* what, int S, int K, int L, int Z, int P) {
+    if (S < 1 || K < 1 || K > YFV2_TRACK_MAX_CAPACITY) {
+        set_error("%s: need S >= 1 and capacity K in 1..%d, as the tracker's (S=%d K=%d)", what, YFV2_TRACK_MAX_CAPACITY, S, K);
+        return YFV2_EINVAL;
+    }
+    if (L < 0 || L > kMaxLines || Z < 0 || Z > kMaxZones || P < 3 || P > kMaxVerts) {
+        set_error("%s: need L in 0..%d lines, Z in 0..%d zones and P in 3..%d vertices (L=%d Z=%d P=%d)", what, kMaxLines, kMaxZones,
+                  kMaxVerts, L, Z, P);
+        return YFV2_EINVAL;
+    }
+    return YFV2_OK;
+}
+
 }  // namespace
 }  // namespace yfv2
 
@@ -609,5 +844,125 @@ extern "C" int yfv2_track_debug_read(const void* state, int S, int K, int s, int
     *next_id_host = head[1];
     *n_host = n;
     for (int k = 0; k < n; ++k) tracks_host[k] = all[(size_t)head[4 + k]];
+    return YFV2_OK;
+}
+
+extern "C" int yfv2_count_state_bytes(int S, int K, int L, int Z, int P, size_t* bytes) {
+    if (!bytes) { set_error("count_state_bytes: null bytes"); return YFV2_EINVAL; }
+    if (int rc = check_count_dims("count_state_bytes", S, K, L, Z, P)) return rc;
+    *bytes = (size_t)S * count_layout(K, L, Z, P).stride;
+    return YFV2_OK;
+}
+
+extern "C" int yfv2_count_reset(void* count_state, int S, int K, int L, int Z, int P, const int* streams_host, int B, void* stream) {
+    if (!count_state || !streams_host) { set_error("count_reset: null count_state / streams_host"); return YFV2_EINVAL; }
+    if (int rc = check_count_dims("count_reset", S, K, L, Z, P)) return rc;
+    std::vector<unsigned char> seen;
+    if (int rc = check_streams("count_reset", S, K, streams_host, B, seen)) return rc;
+    std::unique_ptr<CountResetArgs> ap(new (std::nothrow) CountResetArgs);
+    if (!ap) { set_error("count_reset: host allocation failed"); return YFV2_ENOMEM; }
+    CountResetArgs& a = *ap;
+    a.count = static_cast<unsigned char*>(count_state);
+    a.lay = count_layout(K, L, Z, P);
+    a.K = K; a.L = L; a.Z = Z;
+    std::copy(streams_host, streams_host + B, a.streams);
+    count_reset_kernel<<<B, NT, 0, (cudaStream_t)stream>>>(a);
+    YFV2_LAUNCH_CHECK();
+    return YFV2_OK;
+}
+
+extern "C" int yfv2_count_set_geometry(void* count_state, int S, int K, int L, int Z, int P, int s, const double* lines_host, int nl,
+                                       const float* zones_host, const int* nverts_host, int nz, void* stream) {
+    if (!count_state) { set_error("count_set_geometry: null count_state"); return YFV2_EINVAL; }
+    if (int rc = check_count_dims("count_set_geometry", S, K, L, Z, P)) return rc;
+    if (s < 0 || s >= S) { set_error("count_set_geometry: stream %d outside [0, S=%d)", s, S); return YFV2_EINVAL; }
+    if (nl < 0 || nl > L) { set_error("count_set_geometry: %d lines: need 0..L=%d", nl, L); return YFV2_EINVAL; }
+    if (nz < 0 || nz > Z) { set_error("count_set_geometry: %d zones: need 0..Z=%d", nz, Z); return YFV2_EINVAL; }
+    if ((nl > 0 && !lines_host) || (nz > 0 && (!zones_host || !nverts_host))) {
+        set_error("count_set_geometry: null lines_host / zones_host / nverts_host");
+        return YFV2_EINVAL;
+    }
+    for (int l = 0; l < nl; ++l) {
+        const double* g = lines_host + 4 * (size_t)l;
+        if (!isfinite(g[0]) || !isfinite(g[1]) || !isfinite(g[2]) || !isfinite(g[3])) {
+            set_error("count_set_geometry: lines[%d] has a non-finite coordinate", l);
+            return YFV2_EINVAL;
+        }
+        if (g[0] == g[2] && g[1] == g[3]) { set_error("count_set_geometry: lines[%d] has A = B = (%g, %g)", l, g[0], g[1]); return YFV2_EINVAL; }
+    }
+    for (int z = 0; z < nz; ++z) {
+        const int nv = nverts_host[z];
+        if (nv < 3 || nv > P) { set_error("count_set_geometry: zones[%d] has %d vertices: need 3..P=%d", z, nv, P); return YFV2_EINVAL; }
+        for (int i = 0; i < 2 * nv; ++i)
+            if (!isfinite(zones_host[(size_t)z * P * 2 + i])) {
+                set_error("count_set_geometry: zones[%d] vertex %d has a non-finite coordinate", z, i / 2);
+                return YFV2_EINVAL;
+            }
+    }
+    // header, zeroed totals, lines and zones in one copy from the host; then the records cleared
+    const CountLayout c = count_layout(K, L, Z, P);
+    std::vector<unsigned char> head(c.rid, 0);
+    int* hdr = reinterpret_cast<int*>(head.data());
+    hdr[0] = nl;
+    hdr[1] = nz;
+    if (nl) std::copy(lines_host, lines_host + 4 * (size_t)nl, reinterpret_cast<double*>(head.data() + c.lines));
+    if (nz) {
+        std::copy(nverts_host, nverts_host + nz, reinterpret_cast<int*>(head.data() + c.nverts));
+        std::copy(zones_host, zones_host + (size_t)nz * P * 2, reinterpret_cast<float*>(head.data() + c.verts));
+    }
+    unsigned char* base = static_cast<unsigned char*>(count_state) + (size_t)s * c.stride;
+    cudaStream_t st = (cudaStream_t)stream;
+    YFV2_CUDA(cudaMemcpyAsync(base, head.data(), head.size(), cudaMemcpyHostToDevice, st));
+    YFV2_CUDA(cudaMemsetAsync(base + c.rid, 0, (size_t)K * sizeof(int), st));
+    return YFV2_OK;
+}
+
+extern "C" int yfv2_count_update(const void* track_state, void* count_state, int S, int K, int L, int Z, int P, const int* streams_host,
+                                 int B, int E, double* events, int* event_counts, int* occupancy, void* stream) {
+    if (!track_state || !count_state || !streams_host || !event_counts || (Z > 0 && !occupancy) || (E > 0 && !events)) {
+        set_error("count_update: null track_state / count_state / streams_host / events / event_counts / occupancy");
+        return YFV2_EINVAL;
+    }
+    if (int rc = check_count_dims("count_update", S, K, L, Z, P)) return rc;
+    std::vector<unsigned char> seen;
+    if (int rc = check_streams("count_update", S, K, streams_host, B, seen)) return rc;
+    if (E < 0) { set_error("count_update: E=%d events per stream: need E >= 0", E); return YFV2_EINVAL; }
+    std::unique_ptr<CountArgs> ap(new (std::nothrow) CountArgs);   // 16 KB of kernel parameters: on the heap, not the stack
+    if (!ap) { set_error("count_update: host allocation failed"); return YFV2_ENOMEM; }
+    CountArgs& a = *ap;
+    a.track = static_cast<const unsigned char*>(track_state);
+    a.count = static_cast<unsigned char*>(count_state);
+    a.track_stride = stream_stride(K);
+    a.lay = count_layout(K, L, Z, P);
+    a.K = K; a.L = L; a.Z = Z; a.P = P; a.E = E;
+    a.events = events; a.event_counts = event_counts; a.occupancy = occupancy;
+    std::copy(streams_host, streams_host + B, a.streams);
+    count_update_kernel<<<B, NT, 0, (cudaStream_t)stream>>>(a);
+    YFV2_LAUNCH_CHECK();
+    return YFV2_OK;
+}
+
+extern "C" int yfv2_count_debug_read(const void* count_state, int S, int K, int L, int Z, int P, int s, int* geom_host,
+                                     long long* totals_host, int* ids_host, double* anchors_host, signed char* sides_host,
+                                     unsigned int* inside_host, void* stream) {
+    if (!count_state || !geom_host || !totals_host || !ids_host || !anchors_host || (L > 0 && !sides_host) || !inside_host) {
+        set_error("count_debug_read: null pointer");
+        return YFV2_EINVAL;
+    }
+    if (int rc = check_count_dims("count_debug_read", S, K, L, Z, P)) return rc;
+    if (s < 0 || s >= S) { set_error("count_debug_read: stream %d outside [0, S=%d)", s, S); return YFV2_EINVAL; }
+    const CountLayout c = count_layout(K, L, Z, P);
+    std::vector<unsigned char> blk(c.stride);
+    cudaStream_t st = (cudaStream_t)stream;
+    YFV2_CUDA(cudaMemcpyAsync(blk.data(), static_cast<const unsigned char*>(count_state) + (size_t)s * c.stride, c.stride,
+                              cudaMemcpyDeviceToHost, st));
+    YFV2_CUDA(cudaStreamSynchronize(st));
+    const unsigned char* p = blk.data();
+    std::copy(p, p + 2 * sizeof(int), reinterpret_cast<unsigned char*>(geom_host));
+    std::copy(p + c.totals, p + c.totals + (size_t)(2 * L + 2 * Z) * sizeof(long long), reinterpret_cast<unsigned char*>(totals_host));
+    std::copy(p + c.rid, p + c.rid + (size_t)K * sizeof(int), reinterpret_cast<unsigned char*>(ids_host));
+    std::copy(p + c.rin, p + c.rin + (size_t)K * sizeof(unsigned), reinterpret_cast<unsigned char*>(inside_host));
+    std::copy(p + c.rpos, p + c.rpos + (size_t)K * 2 * sizeof(double), reinterpret_cast<unsigned char*>(anchors_host));
+    if (L > 0) std::copy(p + c.rside, p + c.rside + (size_t)K * L, reinterpret_cast<unsigned char*>(sides_host));
     return YFV2_OK;
 }

@@ -275,6 +275,8 @@ class TrackRecord(ctypes.Structure):
 
 TRACK_TRACKED, TRACK_LOST = 1, 2                     # yfv2_track.state
 TRACK_MAX_CAPACITY, TRACK_MAX_ROWS, TRACK_MAX_BATCH = 1024, 2048, 4096
+COUNT_MAX_LINES, COUNT_MAX_ZONES, COUNT_MAX_VERTICES = 32, 16, 64
+COUNT_LINE, COUNT_ENTRY, COUNT_EXIT = 0, 1, 2           # kind of a yfv2_count_update event
 
 
 class AugParams(ctypes.Structure):
@@ -351,6 +353,23 @@ PROTOTYPES = {
     "yfv2_track_debug_read": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_int),
                                              ctypes.POINTER(ctypes.c_int), ctypes.POINTER(TrackRecord), ctypes.POINTER(ctypes.c_int),
                                              ctypes.c_void_p]),
+    "yfv2_count_state_bytes": (ctypes.c_int, [ctypes.c_int] * 5 + [ctypes.POINTER(ctypes.c_size_t)]),
+    "yfv2_count_reset": (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 5 + [ctypes.POINTER(ctypes.c_int), ctypes.c_int,
+                                                                                 ctypes.c_void_p]),
+    "yfv2_count_set_geometry": (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 6 + [ctypes.POINTER(ctypes.c_double), ctypes.c_int,
+                                                                                        ctypes.POINTER(ctypes.c_float),
+                                                                                        ctypes.POINTER(ctypes.c_int), ctypes.c_int,
+                                                                                        ctypes.c_void_p]),
+    "yfv2_count_update": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 5 + [ctypes.POINTER(ctypes.c_int),
+                                                                                                   ctypes.c_int, ctypes.c_int,
+                                                                                                   ctypes.c_void_p, ctypes.c_void_p,
+                                                                                                   ctypes.c_void_p, ctypes.c_void_p]),
+    "yfv2_count_debug_read": (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 6 + [ctypes.POINTER(ctypes.c_int),
+                                                                                      ctypes.POINTER(ctypes.c_longlong),
+                                                                                      ctypes.POINTER(ctypes.c_int),
+                                                                                      ctypes.POINTER(ctypes.c_double),
+                                                                                      ctypes.POINTER(ctypes.c_byte),
+                                                                                      ctypes.POINTER(ctypes.c_uint), ctypes.c_void_p]),
     "yfv2_batch_statistics": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                              ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]),
     "yfv2_aug_contrast_brightness": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_longlong, ctypes.c_void_p]),
@@ -958,6 +977,122 @@ class Tracker:
         keys = ("id", "cls", "state", "confirmed", "start_frame", "end_frame", "score", "det_row")
         tracks = [dict({k: getattr(r, k) for k in keys}, mean=list(r.mean), cov=list(r.cov)) for r in recs[:n.value]]
         return {"frame": frame.value, "next_id": next_id.value, "tracks": tracks}
+
+
+class Counter:
+    """Line crossings and zone occupancy of a Tracker's tracks (yfv2_count_*, include/yfv2.h), for every stream of the tracker.
+    A track's anchor is the bottom centre of its box; a line is a directed segment (ax, ay, bx, by) and a crossing's dir is the
+    side of the line the anchor ends on (+1: left of A -> B in image coordinates, y down); a zone is a polygon of 3..max_vertices
+    vertices, rounded to float32, tested as cv2.pointPolygonTest tests it (the boundary is inside).  It owns the device state
+    tensor; `lines` / `zones` given here apply to every stream, set_geometry gives one stream its own.  After Tracker.reset of
+    some streams (their ids start again at 1), reset the same streams here."""
+
+    def __init__(self, tracker, lines=None, zones=None, max_lines=8, max_zones=8, max_vertices=32):
+        self.tracker = tracker
+        self.device = tracker.device
+        self.S, self.K = tracker.S, tracker.K
+        self.L, self.Z, self.P = int(max_lines), int(max_zones), int(max_vertices)
+        nb = ctypes.c_size_t()
+        _check(lib().yfv2_count_state_bytes(self.S, self.K, self.L, self.Z, self.P, ctypes.byref(nb)), "Counter")
+        geom = self._geometry(lines, zones, "Counter") if lines is not None or zones is not None else None
+        self.state = torch.zeros((nb.value,), dtype=torch.uint8, device=self.device)
+        if geom is not None:
+            for s in range(self.S):
+                self._set(s, geom, "Counter")
+
+    def _geometry(self, lines, zones, what):
+        ln = np.ascontiguousarray(np.asarray([] if lines is None else lines, np.float64).reshape(-1, 4))
+        if len(ln) > self.L:
+            raise Yfv2Error("%s: %d lines, max_lines=%d" % (what, len(ln), self.L))
+        zs = [np.asarray(z) for z in ([] if zones is None else zones)]
+        if len(zs) > self.Z:
+            raise Yfv2Error("%s: %d zones, max_zones=%d" % (what, len(zs), self.Z))
+        zf = np.zeros((max(len(zs), 1), self.P, 2), np.float32)
+        nv = np.zeros((max(len(zs), 1),), np.int32)
+        for z, v in enumerate(zs):
+            if v.ndim != 2 or v.shape[1] != 2 or not 3 <= v.shape[0] <= self.P:
+                raise Yfv2Error("%s: zones[%d] must be [n, 2] with n in 3..max_vertices=%d, got %s" % (what, z, self.P, tuple(v.shape)))
+            zf[z, :len(v)] = v.astype(np.float32)
+            nv[z] = len(v)
+        return ln, zf, nv, len(zs)
+
+    def _set(self, s, geom, what):
+        ln, zf, nv, nz = geom
+        with torch.cuda.device(self.device):
+            _check(lib().yfv2_count_set_geometry(ctypes.c_void_p(self.state.data_ptr()), self.S, self.K, self.L, self.Z, self.P, int(s),
+                                                 ln.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), len(ln),
+                                                 zf.ctypes.data_as(ctypes.POINTER(ctypes.c_float)),
+                                                 nv.ctypes.data_as(ctypes.POINTER(ctypes.c_int)), nz, _stream(self.device)), what)
+
+    def set_geometry(self, stream, lines=None, zones=None):
+        """Stream `stream`'s lines [n, 4] and zones (a list of [n, 2] polygons); clears its records and totals."""
+        if not 0 <= int(stream) < self.S:
+            raise Yfv2Error("Counter.set_geometry: stream %d outside [0, %d)" % (int(stream), self.S))
+        self._set(int(stream), self._geometry(lines, zones, "Counter.set_geometry"), "Counter.set_geometry")
+
+    def _streams(self, streams):
+        idx = list(range(self.S)) if streams is None else [int(s) for s in streams]
+        return idx, (ctypes.c_int * max(len(idx), 1))(*idx)
+
+    def reset(self, streams=None):
+        """Clears the records and totals of the given streams (all by default), keeping their geometry."""
+        calls = [range(b, min(b + TRACK_MAX_BATCH, self.S)) for b in range(0, self.S, TRACK_MAX_BATCH)] if streams is None else [streams]
+        for part in calls:
+            idx, arr = self._streams(part)
+            with torch.cuda.device(self.device):
+                _check(lib().yfv2_count_reset(ctypes.c_void_p(self.state.data_ptr()), self.S, self.K, self.L, self.Z, self.P, arr, len(idx),
+                                              _stream(self.device)), "Counter.reset")
+
+    def update(self, streams=None, max_events=64):
+        """Counts the tracker's current frame of the given streams (None: all, at most TRACK_MAX_BATCH) in one launch without a
+        host synchronisation.  Returns CUDA tensors (events float64 [B, max_events, 8]: (kind, index, dir, track_id, cls, x, y,
+        frame) in ascending track id, then line, then zone order, zeros past the count; event_counts int32 [B]: every event,
+        possibly more than max_events; occupancy int32 [B, max_zones])."""
+        if (self.tracker.S, self.tracker.K) != (self.S, self.K):
+            raise Yfv2Error("Counter.update: the tracker has S=%d K=%d, the counter S=%d K=%d" % (self.tracker.S, self.tracker.K, self.S, self.K))
+        E = int(max_events)
+        if E < 0:
+            raise Yfv2Error("Counter.update: max_events=%d must be >= 0" % E)
+        idx, arr = self._streams(streams)
+        B = len(idx)
+        events = torch.empty((B, E, 8), dtype=torch.float64, device=self.device)
+        counts = torch.empty((B,), dtype=torch.int32, device=self.device)
+        occupancy = torch.empty((B, self.Z), dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            _check(lib().yfv2_count_update(ctypes.c_void_p(self.tracker.state.data_ptr()), ctypes.c_void_p(self.state.data_ptr()), self.S,
+                                           self.K, self.L, self.Z, self.P, arr, B, E, ctypes.c_void_p(events.data_ptr() if E else None),
+                                           ctypes.c_void_p(counts.data_ptr()), ctypes.c_void_p(occupancy.data_ptr() if self.Z else None),
+                                           _stream(self.device)), "Counter.update")
+        return events, counts, occupancy
+
+    def _read(self, stream):
+        geom = (ctypes.c_int * 2)()
+        totals = np.zeros((2 * self.L + 2 * self.Z,), np.int64)
+        ids = np.zeros((self.K,), np.int32)
+        anchors = np.zeros((self.K, 2), np.float64)
+        sides = np.zeros((self.K, max(self.L, 1)), np.int8)
+        inside = np.zeros((self.K,), np.uint32)
+        with torch.cuda.device(self.device):
+            _check(lib().yfv2_count_debug_read(ctypes.c_void_p(self.state.data_ptr()), self.S, self.K, self.L, self.Z, self.P, int(stream),
+                                               geom, totals.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong)),
+                                               ids.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+                                               anchors.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
+                                               sides.ctypes.data_as(ctypes.POINTER(ctypes.c_byte)),
+                                               inside.ctypes.data_as(ctypes.POINTER(ctypes.c_uint)), _stream(self.device)), "Counter")
+        return geom[0], geom[1], totals, ids, anchors, sides, inside
+
+    def totals(self, stream):
+        """Stream `stream`'s running totals on the host (synchronises): {"lines": int64 [n_lines, 2] (crossings with dir +1, -1),
+        "zones": int64 [n_zones, 2] (entries, exits)}."""
+        nl, nz, totals = self._read(stream)[:3]
+        return {"lines": totals[:2 * nl].reshape(nl, 2), "zones": totals[2 * self.L:2 * self.L + 2 * nz].reshape(nz, 2)}
+
+    def records(self, stream):
+        """Test hook (synchronises): the record of every slot that holds one, {track id: (anchor (x, y), sides [n_lines], inside
+        bits)}; a slot's record outlives its track until the slot's next track appears."""
+        nl, nz, _, ids, anchors, sides, inside = self._read(stream)
+        return {int(i): ((float(anchors[k, 0]), float(anchors[k, 1])), sides[k, :nl].tolist(), int(inside[k]))
+                for k, i in enumerate(ids) if i != 0}
 
 
 def batch_statistics(out, counts, targets, iou_threshold):
